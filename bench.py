@@ -2,6 +2,7 @@
 """bench.py - audio samples/sec of the Harmonic(100)+FilteredNoise(65) decoder.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+                  [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N \
       --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
@@ -17,7 +18,10 @@ of the audio is timed separately and reported as `all_gather`.  configs[1]
 (B=32), configs[0] (Harmonic only, B=1) and configs[3] (forward + backward
 through SpectralLoss, B=128) ride along as extra keys timed on rank 0.
 
-One JSON line on stdout (rank 0).  See the task contract for the keys.
+One JSON line on stdout (rank 0).  --dump-outputs DIR also writes what the last
+timed step computed as DIR/<name>.npy (float32; a fixed seeded sample of batch
+rows when the whole output is larger than 60 MB).  Inputs are seeded, so two
+builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -39,7 +43,9 @@ N_HARM = 100
 N_BANDS = 65
 SAMPLE_RATE = 16000
 BATCH_PER_GPU = 256
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024          # H100 SXM
+HBM_DATASHEET_GBS = 3350.0           # H100 SXM data sheet, HBM3
+DUMP_BUDGET_BYTES = 60 * 1000 * 1000
 
 # Algorithmic bytes per batch item (BASELINE.md section 3 / SURVEY.md 8d), fp32.
 BYTES_HARMONIC = 4 * (2 * N_FRAMES + N_FRAMES * N_HARM) + 4 * N_SAMPLES  # 664000
@@ -52,8 +58,8 @@ def _measured_peaks():
   path = os.path.join(ROOT, 'MEASURED_PEAKS.json')
   if os.path.exists(path):
     with open(path) as f:
-      return float(json.load(f)['hbm_gbs']), 'measured'
-  return 6650.0, 'fallback'
+      return float(json.load(f)['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
+  return HBM_DATASHEET_GBS, 'H100 SXM data sheet'
 
 
 class ClockSampler:
@@ -71,6 +77,7 @@ class ClockSampler:
     self.index = index
     self.samples = []            # (t, sm_mhz, reasons bitmask)
     self.smax = None
+    self.power_limit_w = None
     self.stop_flag = False
     self.thread = None
     self.err = None
@@ -87,6 +94,7 @@ class ClockSampler:
       except Exception:  # pylint: disable=broad-except
         h = pynvml.nvmlDeviceGetHandleByIndex(self.index)
       self.smax = float(pynvml.nvmlDeviceGetMaxClockInfo(h, pynvml.NVML_CLOCK_SM))
+      self.power_limit_w = pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
       get_reasons = getattr(pynvml, 'nvmlDeviceGetCurrentClocksEventReasons',
                             None) or pynvml.nvmlDeviceGetCurrentClocksThrottleReasons
 
@@ -115,6 +123,7 @@ class ClockSampler:
       self.thread.join(timeout=2)
     if not self.samples:
       return {'sm_mhz': None, 'sm_max_mhz': self.smax, 'samples': 0,
+              'power_limit_w': self.power_limit_w,
               'reasons': ['nvml unavailable: %s' % self.err]}
     t0, t1 = self.t_timed
     window = 'timed region'
@@ -131,7 +140,7 @@ class ClockSampler:
     reasons = sorted(k for k, bit in self.REASONS.items() if mask & bit)
     return {'sm_mhz': statistics.median(r[1] for r in rows),
             'sm_max_mhz': self.smax, 'samples': len(rows), 'window': window,
-            'reasons': reasons}
+            'power_limit_w': self.power_limit_w, 'reasons': reasons}
 
 
 def make_host_inputs(batch, seed):
@@ -139,6 +148,24 @@ def make_host_inputs(batch, seed):
   inp = synth_inputs(batch, N_FRAMES, N_HARM, N_BANDS, N_SAMPLES, seed=seed)
   return {k: inp[k] for k in ['amps', 'harmonic_distribution', 'f0_hz',
                               'noise_magnitudes']}
+
+
+def dump_outputs(dump_dir, arrays):
+  """Writes each [B, ...] array of `arrays` (name -> float32 numpy) to
+  dump_dir/<name>.npy.  When together they exceed DUMP_BUDGET_BYTES, every array
+  keeps the same fixed seeded sample of batch rows (sorted)."""
+  os.makedirs(dump_dir, exist_ok=True)
+  batch = {len(a) for a in arrays.values() if a.ndim}
+  assert len(batch) <= 1, batch
+  row_bytes = sum(a[0].nbytes for a in arrays.values() if a.ndim)
+  rows = None
+  if batch and row_bytes * next(iter(batch)) > DUMP_BUDGET_BYTES:
+    b = next(iter(batch))
+    rows = np.sort(np.random.default_rng(0).choice(
+        b, size=DUMP_BUDGET_BYTES // row_bytes, replace=False))
+  for name, a in arrays.items():
+    np.save(os.path.join(dump_dir, name + '.npy'),
+            a if rows is None or not a.ndim else a[rows])
 
 
 # ----------------------------------------------------------------------------
@@ -370,12 +397,13 @@ def run_ours(args):
       graph_note = 'eager ProcessorGroup.__call__ (graph capture failed: %r)' % (e,)
       torch.cuda.synchronize()
 
+  last_audio = []
   if graphs:
     def step_resident(i):
       graphs[i % n_sets].replay()
   else:
     def step_resident(i):
-      group(dev_sets[i % n_sets])
+      last_audio[:] = [group(dev_sets[i % n_sets])]
 
   sampler = ClockSampler(local_rank)
   if rank == 0:
@@ -390,6 +418,9 @@ def run_ours(args):
     launches_timed = launches * args.steps // (args.steps + args.warmup)
   ms_per_step = ms_total / args.steps
   value = world * B * N_SAMPLES / (ms_per_step * 1e-3)
+  if args.dump_outputs and rank == 0:
+    last = graph_out[(args.warmup + args.steps - 1) % n_sets] if graphs else last_audio[0]
+    dump_outputs(args.dump_outputs, {'audio': last.float().cpu().numpy()})
 
   # -- e2e: host buffers in, host audio out, copies inside the timed region ---
   # The public host-buffer call: HostDecoder = ProcessorGroup over pinned host
@@ -415,8 +446,7 @@ def run_ours(args):
     if best_ms is None or ms < best_ms:
       best_c, best_ms = c, ms
   host_dec = decs[best_c]
-  e2e_steps = max(min(args.steps, 30), 10)
-  ms_e2e = timed(step_e2e_with(host_dec), e2e_steps, 3) / e2e_steps
+  ms_e2e = timed(step_e2e_with(host_dec), args.steps, 3) / args.steps
   e2e_value = world * B * N_SAMPLES / (ms_e2e * 1e-3)
 
   # link floor of the same round trip: the H2D bytes alone, pinned -> device,
@@ -597,16 +627,6 @@ def run_ours(args):
     return None
 
   peak, peak_src = _measured_peaks()
-  # DRAM traffic of the same kernels from one ncu --set full capture of this
-  # workload (profiles/*traffic*.json; null for any other batch size)
-  traffic = {}
-  for name in ('r02_traffic_b256.json', 'r01_traffic_b32.json'):
-    tpath = os.path.join(ROOT, 'profiles', name)
-    if os.path.exists(tpath):
-      with open(tpath) as f:
-        traffic = {k: v for k, v in json.load(f).items() if v.get('batch') == B}
-      if traffic:
-        break
   dom_is_harm = ms_harm >= ms_noise
   dom_ms = ms_harm if dom_is_harm else ms_noise
   dom_bytes = (BYTES_HARMONIC if dom_is_harm else BYTES_NOISE + 4 * N_SAMPLES) * B
@@ -615,11 +635,7 @@ def run_ours(args):
       'bound': 'hbm', 'kernel': 'harmonic_forward' if dom_is_harm else
                'filtered_noise_forward(accumulate)',
       'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
-      'frac': achieved / peak, 'peak_source': peak_src + ' (MEASURED_PEAKS.json hbm_gbs)',
-      'traffic': (traffic.get('harmonic_forward' if dom_is_harm else
-                              'filtered_noise_forward') or {}).get('traffic'),
-      'traffic_source': (traffic.get('harmonic_forward' if dom_is_harm else
-                                     'filtered_noise_forward') or {}).get('source'),
+      'frac': achieved / peak, 'peak_source': peak_src,
       'algorithmic_bytes_per_launch': dom_bytes,
       'kernel_ms': {'harmonic_forward': ms_harm,
                     'filtered_noise_forward': ms_noise,
@@ -637,15 +653,16 @@ def run_ours(args):
                      'of ddsp core/synths, validated against the unmodified '
                      'reference run on oracle/tf_shim; %.2f s)' % (items, B, dt)}
 
-  cfg_name = ('configs[4]: decoder batch %d sharded over %d B200 (%d per GPU)'
-              % (B * world, world, B)) if world > 1 else (
-                  'configs[2]: decoder batch %d on one B200' % B)
+  gpu_name = torch.cuda.get_device_name(dev)
+  cfg_name = ('configs[4]: decoder batch %d sharded over %d x %s (%d per GPU)'
+              % (B * world, world, gpu_name, B)) if world > 1 else (
+                  'configs[2]: decoder batch %d on one %s' % (B, gpu_name))
   line = {
       'metric': 'audio samples/sec (Harmonic+FilteredNoise decoder)',
       'value': value, 'unit': 'samples/s', 'n_gpus': world,
       'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': ms_per_step,
       'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
-      'dtype': 'f32', 'data': 'synthetic',
+      'dtype': 'f32', 'data': 'synthetic', 'gpu': gpu_name,
       'config': {
           'workload': cfg_name + ' - ae.gin Harmonic(100)+FilteredNoise(65)+Add via '
                       'ProcessorGroup (get_controls + get_signal), N=64000 @16kHz, '
@@ -750,6 +767,7 @@ def run_c4(args):
     import datetime
     dist.init_process_group('nccl', device_id=dev, timeout=datetime.timedelta(seconds=300))
   lib = _lib.load()
+  torch.manual_seed(4321 + rank)       # the targets: same inputs on every run
   B = C4_BATCH
   keys = ('amps', 'harmonic_distribution', 'f0_hz', 'noise_magnitudes')
   grad_keys = ('amps', 'harmonic_distribution', 'noise_magnitudes')
@@ -812,6 +830,11 @@ def run_c4(args):
   sampler.mark_timed(0)
   ms_step = timed(step, args.steps, args.warmup) / args.steps
   sampler.mark_timed(1)
+  if args.dump_outputs and rank == 0:
+    d = sets[(args.warmup + args.steps - 1) % len(sets)]
+    out = {'grad_' + k: d[k].grad.float().cpu().numpy() for k in grad_keys}
+    out['loss'] = last['loss'].detach().float().cpu().numpy()
+    dump_outputs(args.dump_outputs, out)
   launches = (lib.ddsp_b200_launch_count() - c0) * args.steps // (args.steps + args.warmup)
   value = world * B * N_SAMPLES / (ms_step * 1e-3)
 
@@ -858,8 +881,7 @@ def run_c4(args):
     loss_host.copy_(loss.detach(), non_blocking=True)
     torch.cuda.current_stream().synchronize()
 
-  e2e_steps = max(5, min(args.steps, 20))
-  ms_e2e = timed(step_e2e, e2e_steps, 3) / e2e_steps
+  ms_e2e = timed(step_e2e, args.steps, 3) / args.steps
 
   # dominant kernel of the step: the one-pass L1 magnitude / log-magnitude kernel
   # (18 launches per step, the largest share of the GPU time); timed alone on the
@@ -908,6 +930,7 @@ def run_c4(args):
       'value': value, 'unit': 'samples/s', 'n_gpus': world, 'steps': args.steps,
       'warmup': args.warmup, 'ms_per_step': ms_step, 'higher_is_better': True,
       'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
+      'gpu': torch.cuda.get_device_name(dev),
       'config': {'workload': 'configs[3]: ae.gin decoder forward + backward through '
                              'SpectralLoss (L1 mag + log-mag, FFT 2048..64), batch %d per '
                              'GPU, N=64000 @16kHz; gradients to amps, '
@@ -926,7 +949,7 @@ def run_c4(args):
       'roofline': {'bound': 'hbm', 'kernel': 'spectral_l1 (2048-point STFTs)',
                    'achieved': l1_bytes / (ms_l1 * 1e-3) / 1e9, 'peak': peak,
                    'unit': 'GB/s', 'frac': l1_bytes / (ms_l1 * 1e-3) / 1e9 / peak,
-                   'peak_source': peak_src + ' (MEASURED_PEAKS.json hbm_gbs)',
+                   'peak_source': peak_src,
                    'traffic': None, 'algorithmic_bytes_per_launch': l1_bytes,
                    'kernel_ms': {'spectral_l1': ms_l1}},
       'cpu_baseline': cpu,
@@ -961,7 +984,8 @@ def main():
 def _main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--gpus', type=int, default=1)
-  ap.add_argument('--steps', type=int, default=50)
+  ap.add_argument('--steps', type=int, default=None,
+                  help='timed steps (default 50; 10 with --config c4)')
   ap.add_argument('--warmup', type=int, default=10)
   ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
   ap.add_argument('--batch', type=int, default=BATCH_PER_GPU,
@@ -976,11 +1000,17 @@ def _main():
   ap.add_argument('--config', default='decoder', choices=['decoder', 'c4'],
                   help="'decoder' (default): configs[2] / configs[4]; 'c4': configs[3], "
                        'forward + backward through SpectralLoss, batch 128 per GPU')
+  ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                  help='write what the last timed step computed to DIR/<name>.npy')
   args = ap.parse_args()
   args.warmup = max(args.warmup, 3)
+  if args.steps is None:
+    args.steps = 10 if args.config == 'c4' else 50
+  if args.steps < 1:
+    ap.error('--steps must be >= 1')
+  if args.dump_outputs and args.impl == 'reference':
+    ap.error('--dump-outputs writes the outputs of the CUDA path (--impl ours)')
   if args.config == 'c4':
-    if args.steps == 50:
-      args.steps = 10
     return run_c4_reference(args) if args.impl == 'reference' else run_c4(args)
   if args.impl == 'reference':
     return run_reference(args)

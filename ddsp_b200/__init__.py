@@ -1,4 +1,4 @@
-"""ddsp_b200 - B200-native (sm_100a) Harmonic + FilteredNoise DDSP decoder.
+"""ddsp_b200 - H100-native (sm_90a) Harmonic + FilteredNoise DDSP decoder.
 
 Drop-in for the signal-generation layer of magenta/ddsp: `Processor`,
 `ProcessorGroup`, `Harmonic`, `FilteredNoise`, `Add` with the reference's API,

@@ -1,4 +1,4 @@
-"""Builds libddsp_b200.so in-tree with nvcc for sm_100a (B200) only."""
+"""Builds libddsp_b200.so in-tree with nvcc for sm_90a (H100) only."""
 import os
 import subprocess
 import sys
@@ -6,9 +6,11 @@ import sys
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, 'csrc')
 LIB_PATH = os.path.join(_HERE, 'libddsp_b200.so')
+# the nvcc command line that built LIB_PATH: other flags or another arch rebuild
+CMD_PATH = LIB_PATH + '.cmd'
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-O3', '-lineinfo', '-std=c++17',
     '-Xcompiler', '-fPIC', '-shared',
 ]
@@ -27,22 +29,40 @@ def _newest_mtime():
   return newest
 
 
+def _command(verbose=False):
+  nvcc = os.environ.get('NVCC', 'nvcc')
+  extra = os.environ.get('DDSP_B200_NVCC_EXTRA', '').split()   # e.g. -DDDSP_HV4_NW=4
+  return [nvcc] + NVCC_FLAGS + extra + (['-Xptxas', '-v'] if verbose else []) + [
+      '-o', LIB_PATH] + _sources()
+
+
+def _built_with():
+  try:
+    with open(CMD_PATH) as f:
+      return f.read()
+  except OSError:
+    return None
+
+
 def is_stale():
+  """True if the library is missing, older than its sources, or was built by
+  another nvcc command line (flags, arch, DDSP_B200_NVCC_EXTRA)."""
   return (not os.path.exists(LIB_PATH) or
-          os.path.getmtime(LIB_PATH) < _newest_mtime())
+          os.path.getmtime(LIB_PATH) < _newest_mtime() or
+          _built_with() != ' '.join(_command()))
 
 
 def build(force=False, verbose=False):
-  """Compiles the CUDA library if missing or older than its sources."""
+  """Compiles the CUDA library if missing, older than its sources or built with
+  another command line."""
   if not force and not is_stale():
     return LIB_PATH
-  nvcc = os.environ.get('NVCC', 'nvcc')
-  extra = os.environ.get('DDSP_B200_NVCC_EXTRA', '').split()   # e.g. -DDDSP_HV3_MIN_CTAS=5
-  cmd = [nvcc] + NVCC_FLAGS + extra + (['-Xptxas', '-v'] if verbose else []) + [
-      '-o', LIB_PATH] + _sources()
+  cmd = _command(verbose)
   proc = subprocess.run(cmd, capture_output=True, text=True)
   if proc.returncode != 0:
     raise RuntimeError('nvcc failed:\n%s\n%s' % (' '.join(cmd), proc.stderr))
+  with open(CMD_PATH, 'w') as f:
+    f.write(' '.join(_command()))
   if verbose:
     sys.stderr.write(proc.stderr)
   return LIB_PATH

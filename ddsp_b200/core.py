@@ -2,7 +2,7 @@
 
 Same names, argument meaning and error behaviour as the reference (file:line
 cited per function); the arithmetic happens in libddsp_b200.so (hand-written
-sm_100a kernels) through the ctypes C ABI in `_lib.py`.  torch is plumbing:
+sm_90a kernels) through the ctypes C ABI in `_lib.py`.  torch is plumbing:
 device memory and streams.  There is no CPU fallback.
 """
 from collections import abc
@@ -22,7 +22,7 @@ AMP_METHODS = {'window': _lib.AMP_WINDOW, 'linear': _lib.AMP_LINEAR}
 def _device():
   if not torch.cuda.is_available():
     raise RuntimeError(
-        'ddsp_b200 needs a CUDA device (B200, sm_100a); there is no CPU '
+        'ddsp_b200 needs a CUDA device (H100, sm_90a); there is no CPU '
         'fallback.')
   return torch.device('cuda', torch.cuda.current_device())
 

@@ -39,7 +39,7 @@ void set_error(const char* fmt, ...) {
 
 static inline int grid_for(int64_t n, int threads, int cap_per_sm = 8) {
   int64_t blocks = (n + threads - 1) / threads;
-  int64_t cap = (int64_t)kNumSMs * cap_per_sm;
+  int64_t cap = (int64_t)num_sms() * cap_per_sm;
   return (int)std::max<int64_t>(1, std::min(blocks, cap));
 }
 
@@ -151,7 +151,7 @@ int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
   p.Kp = (K + 3) & ~3;
   // frames per tile: ~2048 samples, enough CTAs to fill the chip, bounded smem
   int FT = std::max(1, 2048 / p.hop);
-  const int64_t want_ctas = 4ll * kNumSMs;
+  const int64_t want_ctas = 4ll * num_sms();
   int ft_fill = (int)std::max<int64_t>(1, ((int64_t)B * F + want_ctas - 1) / want_ctas);
   FT = std::min(FT, std::max(ft_fill, std::min(4, F)));
   FT = std::min(FT, F);
@@ -546,7 +546,7 @@ int ddsp_b200_decoder_forward_host(ddsp_b200_host_pipeline* handle,
   }
   hp->used = true;
   // Two host->device streams (harmonic_distribution on one; magnitudes and the
-  // small per-frame vectors on the other): a copy costs ~10 us of set-up however
+  // small per-frame vectors on the other): a copy has a fixed set-up cost however
   // small it is, and on one stream those set-ups do not overlap the previous
   // transfer - two streams keep the link busy while one of them sets up.  The
   // per-frame vectors go over once for the whole batch.
@@ -566,7 +566,7 @@ int ddsp_b200_decoder_forward_host(ddsp_b200_host_pipeline* handle,
   }
   // First queue EVERY host->device copy: the copy engines then never wait for
   // this thread to get through the launches and event calls of earlier chunks
-  // (~35 us of driver time per chunk, longer than a small chunk's transfer).
+  // (driver time per chunk can exceed a small chunk's transfer).
   for (int c = 0, b0 = 0; c < n_c; b0 += sizes[c], ++c) {
     const int nbi = sizes[c];
     const size_t o1 = (size_t)b0 * F;
@@ -783,7 +783,7 @@ int ddsp_b200_filtered_noise_backward(const float* grad_audio, const float* nois
   int rc = set_smem(noise_backward_kernel, smem, "filtered_noise_backward");
   if (rc) return rc;
   const int per_sm = smem <= 100 * 1024 ? 2 : 1;
-  const int grid = (int)std::min<long long>(n_tiles, (long long)kNumSMs * per_sm);
+  const int grid = (int)std::min<long long>(n_tiles, (long long)num_sms() * per_sm);
   noise_backward_kernel<<<grid, kNbThreads, smem, (cudaStream_t)stream>>>(p);
   DDSP_CHECK_LAUNCH("filtered_noise_backward");
   return 0;
@@ -898,7 +898,7 @@ int ddsp_b200_fft_convolve_lti(const float* audio, const float* impulse_response
                     st>>>(
       Z, H, W, g.n_in, g.P, g.n_out, ir_batch == 1 ? 0 : g.P * lc::M, j_first, n_blocks);
   DDSP_CHECK_LAUNCH("fft_convolve_lti(multiply-accumulate + inverse)");
-  const int cgrid = std::min((out_len + 255) / 256, 8 * kNumSMs);
+  const int cgrid = std::min((out_len + 255) / 256, 8 * num_sms());
   lc::lc_combine<<<dim3(cgrid, B), 256, 0, st>>>(W, out, g.n2, g.w_len, start, out_len,
                                                N + S - 1, accumulate, j_first * lc::L,
                                                (j_last + 1) * lc::L);
@@ -1132,7 +1132,7 @@ int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
                (long long)n_bins_total, n_bins, irfft_size);
   DDSP_REQUIRE((((uintptr_t)stft_target | (uintptr_t)stft_value | (uintptr_t)grad_value) & 15) == 0,
                DDSP_B200_E_INVALID, "spectral_l1: tensors must be 16-byte aligned");
-  const long long blocks = std::min<long long>((n_bins_total / 2 + 255) / 256 + 1, 8ll * kNumSMs);
+  const long long blocks = std::min<long long>((n_bins_total / 2 + 255) / 256 + 1, 8ll * num_sms());
   spectral_l1_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
       reinterpret_cast<const float2*>(stft_target), reinterpret_cast<const float2*>(stft_value),
       reinterpret_cast<float2*>(grad_value), sums, n_bins_total, mag_weight, logmag_weight,
@@ -1143,10 +1143,10 @@ int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
 
 #ifdef DDSP_NR_TIMING
 // measurement builds only (tools/noise_timing.py): the noise_ring phase counters of
-// the last launch, [148 CTAs][32 warps][8 phases] cycles
+// the last launch, [kMaxSMs CTAs][32 warps][8 phases] cycles (rows past the grid stay 0)
 int ddsp_b200_debug_noise_timing(unsigned* host_out) {
   cudaError_t e = cudaMemcpyFromSymbol(host_out, ddsp::nr_::g_nr_timing,
-                                       sizeof(unsigned) * kNumSMs * 32 * 8);
+                                       sizeof(unsigned) * kMaxSMs * 32 * 8);
   return e == cudaSuccess ? 0 : DDSP_B200_E_CUDA;
 }
 #endif

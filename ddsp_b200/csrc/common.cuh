@@ -1,6 +1,7 @@
-// Shared helpers for libddsp_b200 (sm_100a only).
+// Shared helpers for libddsp_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
+#include <atomic>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -31,7 +32,38 @@ void count_launch();
     }                                                                   \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+// Upper bound on the SM count, for per-SM debug arrays (H100 SXM has 132).
+constexpr int kMaxSMs = 256;
+
+// SM count of the current device (132 on H100 SXM, 114 on H100 PCIe), queried
+// once per device: persistent grids and grid caps are sized by it.
+inline int num_sms() {
+  static std::atomic<int> cache[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0) dev = 0;
+  std::atomic<int>* slot = dev < 64 ? &cache[dev] : nullptr;
+  int n = slot ? slot->load(std::memory_order_relaxed) : 0;
+  if (n > 0) return n;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+    n = 132;   // the error surfaces at the launch that follows
+  if (n > kMaxSMs) n = kMaxSMs;
+  if (slot) slot->store(n, std::memory_order_relaxed);
+  return n;
+}
+
+// ---- f32x2 arithmetic -------------------------------------------------------
+// Two float lanes computed as two scalar round-to-nearest operations (Hopper has
+// no packed f32x2 FMA).  The _rn intrinsics are never contracted or reassociated,
+// so every lane is rounded exactly as the packed instruction would round it.
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
+}
 
 // ---- fixed-point phase ------------------------------------------------------
 // Phase is kept in *turns* as a 64-bit fixed-point fraction (2^64 == 1 turn).

@@ -4,7 +4,7 @@
 // kernel instead of one sinpif per oscillator: 10 packed instructions per sample
 // pair and harmonic pair, plus a 16-value transposing warp reduction per 8
 // harmonics.  Tiling, frame records and the phase prefix are those of the third
-// forward generation (profiles/experiments/harmonic_v3.cuh.txt).  Every element of G0 / G1 is written (zeros above the live
+// forward generation.  Every element of G0 / G1 is written (zeros above the live
 // count), so the caller needs no memset.
 #pragma once
 #include "backward.cuh"
@@ -54,7 +54,7 @@ __device__ __forceinline__ void chain_seed(Chain& c, uint32_t p,
 }
 __device__ __forceinline__ void chain_step(Chain& c) {
   const float2 sg = make_float2(c.sigma, c.sigma);
-  c.Dd = ffma2(c.sna, c.S, __fmul2_rn(sg, c.Dd));
+  c.Dd = ffma2(c.sna, c.S, fmul2(sg, c.Dd));
   c.S = ffma2(sg, c.S, c.Dd);
 }
 
@@ -211,8 +211,8 @@ harmonic_backward2_kernel(HarmonicParams p, const float* __restrict__ grad,
             if (k1 > kbl) { wb0.x = 0.f; wb1.x = 0.f; }
             if (k2 > kbl) { wb0.y = 0.f; wb1.y = 0.f; }
           }
-          const float2 t0 = ffma2(wb0, cb.S, __fmul2_rn(wa0, ca.S));
-          const float2 t1 = ffma2(wb1, cb.S, __fmul2_rn(wa1, ca.S));
+          const float2 t0 = ffma2(wb0, cb.S, fmul2(wa0, ca.S));
+          const float2 t1 = ffma2(wb1, cb.S, fmul2(wa1, ca.S));
           val[2 * st] = t0.x; val[2 * st + 1] = t0.y;
           val[8 + 2 * st] = t1.x; val[8 + 2 * st + 1] = t1.y;
           chain_step(ca);
@@ -244,7 +244,7 @@ inline int launch_harmonic_backward2(HarmonicParams p, const float* grad, float*
                                      float* g1, cudaStream_t st) {
   using namespace hb2;
   int FW = 16;
-  const long long want_ctas = 8ll * kNumSMs;
+  const long long want_ctas = 8ll * num_sms();
   while (FW > 4 && (long long)p.B * ((p.F + FW * NW - 1) / (FW * NW)) < want_ctas) FW >>= 1;
   FW = std::max(1, std::min(FW, (p.F + NW - 1) / NW));
   const size_t smem = smem_layout(FW).total;

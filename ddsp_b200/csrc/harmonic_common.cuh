@@ -1,13 +1,12 @@
-// Shared pieces of the fused harmonic kernels (hop % 64 == 0): the packed f32x2
-// helpers, the 256-entry sin / cos table, the 64-bit fixed-point phase, the
+// Shared pieces of the fused harmonic kernels (hop % 64 == 0): the 256-entry
+// sin / cos table, the 64-bit fixed-point phase, the
 // per-sample oscillator state (two Reinsch chains over the harmonics, odd / even,
 // in one f32x2), the exact per-oscillator slow path for f0 < 1 Hz, and the
 // get_controls rows for wide harmonic distributions.  Used by harmonic_v4.cuh
 // (forward), harmonic_bwd2.cuh / backward.cuh (backward).
 //
 // Derivations (closed-form phase, Reinsch recurrence, per-row accumulators,
-// live-count Nyquist culling) are in DESIGN.md section 3.1; the first two kernel
-// generations that introduced them are kept under profiles/experiments/.
+// live-count Nyquist culling) are in DESIGN.md section 3.1.
 #pragma once
 #include <cmath>
 #include <cstdlib>
@@ -19,16 +18,6 @@ namespace ddsp {
 constexpr int kSinTabBits = 8;
 constexpr int kSinTab = 1 << kSinTabBits;  // 256-entry (sin, cos) table
 
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  return __ffma2_rn(a, b, c);
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-  return __fadd2_rn(a, b);
-}
-
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-  return __fmul2_rn(a, b);
-}
 __device__ __forceinline__ float2 bc2(float x) { return make_float2(x, x); }
 
 // Slow, exact per-oscillator evaluation of one sample (frames with f0 < 1 Hz,
@@ -130,8 +119,8 @@ __device__ __forceinline__ float osc_finish(const Osc& st, float w0, float w1) {
 }
 
 // Frame record and oscillator seed of the (odd, even)-chain layout: the backward
-// kernel (harmonic_bwd2.cuh) keeps the third forward generation's records
-// (profiles/experiments/harmonic_v3.cuh.txt); the forward kernel is harmonic_v4.cuh.
+// kernel (harmonic_bwd2.cuh) keeps the third forward generation's records; the
+// forward kernel is harmonic_v4.cuh.
 constexpr int kBwdWarps = 4;     // warps per CTA of the backward kernel
 struct __align__(16) FrameRec {
   unsigned long long P, A;       // P carries the +2^31 rounding offset

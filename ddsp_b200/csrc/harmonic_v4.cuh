@@ -2,22 +2,21 @@
 // The mathematics is that of the earlier generations (closed-form phase, Reinsch
 // chains over the harmonics with angle 2 phi, per-row accumulators, live-count
 // Nyquist culling, get_controls fused into the slab staging - DESIGN.md 3.1).
-// ncu on the third generation at B = 256 (profiles/r02_ncu_summary.txt): 425 warp
-// instructions per 64-sample frame, 106 of them the oscillator loop, which already
-// runs at the FMA pipe's packed rate (2 cycles per FFMA2) - everything else was
-// overhead at one issue slot each.  What changed:
+// In the third generation the oscillator loop was about a quarter of the warp
+// instructions per 64-sample frame; everything else was overhead at one issue
+// slot each.  What changed:
 //
 //   * the f32x2 lanes hold the SAME chain of the lane's TWO samples (r, r + 32),
 //     not the (odd, even) chains of one sample.  Harmonic amplitudes enter as
-//     broadcast scalar operands (FFMA2 R, R.F32, RR, RR); the seeds (table
-//     look-up, rotation, double-angle, Reinsch constants), the weights and the
-//     final combination are packed over the two samples: half the instructions,
-//     no cross-half sums, eight accumulator registers less;
-//   * the per-sample phase is two DFMAs on the otherwise idle FP64 pipe:
-//     y = P' + c1 A + c2 D with P' = P + 1.5 * 2^20, whose low mantissa word IS
-//     the 32-bit fixed-point phase (the frame phases P stay exact 64-bit
-//     fixed point; the in-frame offset is < 2^13 turns, so the rounding is
-//     <= 2^-32 turn).  Was 4 IMAD + 3 on the FMA / ALU pipes, twice per frame;
+//     broadcast scalar operands; the seeds (table look-up, rotation,
+//     double-angle, Reinsch constants), the weights and the final combination
+//     are f32x2 over the two samples: no cross-half sums, eight accumulator
+//     registers less;
+//   * the per-sample phase is 4 IMADs on the 64-bit fixed-point frame phase
+//     (hcm::phase32).  DDSP_HV4_PHASE_F64=1 builds the alternative, off by
+//     default: two DFMAs on the FP64 pipe, y = P' + c1 A + c2 D with
+//     P' = P + 1.5 * 2^20, whose low mantissa word IS the 32-bit fixed-point
+//     phase (the in-frame offset is < 2^13 turns, so the rounding is <= 2^-32 turn);
 //   * get_controls writes each row once: exp_sigmoid on the live prefix, zeros
 //     above it, and the row's 1 / sum goes into the frame amplitude (amp / sum),
 //     not into a second pass over the row;
@@ -83,10 +82,10 @@ __host__ __device__ inline Smem smem_layout(int FW, int Kp, int hop) {
 using hcm::phase32;
 
 __device__ __forceinline__ float2 bffma2(float x, float2 v, float2 acc) {
-  return __ffma2_rn(make_float2(x, x), v, acc);
+  return ffma2(make_float2(x, x), v, acc);
 }
 __device__ __forceinline__ float2 bfmul2(float x, float2 v) {
-  return __fmul2_rn(make_float2(x, x), v);
+  return fmul2(make_float2(x, x), v);
 }
 
 // Harmonic.get_controls for up to four rows (r0 .. r0+3 of this warp's block) in
@@ -158,35 +157,35 @@ __device__ __forceinline__ void osc_seed2(Osc2& st, uint32_t qa, uint32_t qb,
   constexpr uint32_t kLow = (1u << (32 - kSinTabBits)) - 1u;
   constexpr float kC = 1.4629180792671596e-9f;                    // 2 pi / 2^32
   constexpr float kOff = -(float)(1u << (31 - kSinTabBits)) * kC;
-  const float2 eps = __ffma2_rn(make_float2((float)(qa & kLow), (float)(qb & kLow)),
+  const float2 eps = ffma2(make_float2((float)(qa & kLow), (float)(qb & kLow)),
                                 make_float2(kC, kC), make_float2(kOff, kOff));
-  const float2 e2 = __fmul2_rn(eps, eps);
-  const float2 ce = __ffma2_rn(e2, make_float2(-0.5f, -0.5f), make_float2(1.f, 1.f));
-  const float2 se = __fmul2_rn(eps, __ffma2_rn(e2, make_float2(-0.16666667f, -0.16666667f),
+  const float2 e2 = fmul2(eps, eps);
+  const float2 ce = ffma2(e2, make_float2(-0.5f, -0.5f), make_float2(1.f, 1.f));
+  const float2 se = fmul2(eps, ffma2(e2, make_float2(-0.16666667f, -0.16666667f),
                                                make_float2(1.f, 1.f)));
   const float2 nse = make_float2(-se.x, -se.y);
-  const float2 s1 = __ffma2_rn(ty, se, __fmul2_rn(tx, ce));
-  const float2 c1 = __ffma2_rn(tx, nse, __fmul2_rn(ty, ce));
-  const float2 ss = __fmul2_rn(s1, s1), cc = __fmul2_rn(c1, c1);
-  const float2 s2 = __fmul2_rn(__fadd2_rn(s1, s1), c1);           // sin(2 phi)
+  const float2 s1 = ffma2(ty, se, fmul2(tx, ce));
+  const float2 c1 = ffma2(tx, nse, fmul2(ty, ce));
+  const float2 ss = fmul2(s1, s1), cc = fmul2(c1, c1);
+  const float2 s2 = fmul2(fadd2(s1, s1), c1);           // sin(2 phi)
   st.sg = make_float2(ss.x > cc.x ? -1.0f : 1.0f, ss.y > cc.y ? -1.0f : 1.0f);
-  st.na = __fmul2_rn(make_float2(fminf(ss.x, cc.x), fminf(ss.y, cc.y)),
+  st.na = fmul2(make_float2(fminf(ss.x, cc.x), fminf(ss.y, cc.y)),
                      make_float2(-4.0f, -4.0f));
   st.vo = s1;
   st.ve = s2;
-  st.dlo = __ffma2_rn(s1, st.sg, s1);                             // 2 s1, or 0 if shifted
+  st.dlo = ffma2(s1, st.sg, s1);                             // 2 s1, or 0 if shifted
   st.dle = s2;
 }
 
 __device__ __forceinline__ void osc_step(Osc2& st) {
-  st.dlo = __ffma2_rn(st.na, st.vo, st.dlo);
-  st.dle = __ffma2_rn(st.na, st.ve, st.dle);
-  st.vo = __fadd2_rn(st.vo, st.dlo);
-  st.ve = __fadd2_rn(st.ve, st.dle);
+  st.dlo = ffma2(st.na, st.vo, st.dlo);
+  st.dle = ffma2(st.na, st.ve, st.dle);
+  st.vo = fadd2(st.vo, st.dlo);
+  st.ve = fadd2(st.ve, st.dle);
 }
 
 // Four harmonics (k+1 .. k+4) of both samples: two chain steps.  Each of the
-// eight accumulators takes ONE FFMA2 per group (two back-to-back updates of one
+// eight accumulators takes ONE f32x2 FMA per group (two back-to-back updates of one
 // accumulator made ptxas rotate registers through MOVs at the loop edge).
 __device__ __forceinline__ void osc_group(Osc2& st, const float4& X0, const float4& X1) {
   st.s0e = bffma2(X0.x, st.vo, st.s0e);
@@ -305,7 +304,7 @@ __device__ __forceinline__ void frame_chunk(
   const uint32_t qb = phase32(PA.x, PA.y, D, lc.c1b, lc.c2b);
 #endif
   // (1 - w1) amp0, w1 amp1
-  const float2 w0 = __ffma2_rn(make_float2(-lc.w1.x, -lc.w1.y), make_float2(fa.z, fa.z),
+  const float2 w0 = ffma2(make_float2(-lc.w1.x, -lc.w1.y), make_float2(fa.z, fa.z),
                                make_float2(fa.z, fa.z));
   const float2 w1 = bfmul2(fa.w, lc.w1);
   float2 y;
@@ -363,9 +362,9 @@ __device__ __forceinline__ void frame_chunk(
         osc_group_masked(st, X0, X1, k, ka, kb);
       }
     }
-    const float2 t0 = __ffma2_rn(st.sg, __fadd2_rn(st.s0o, st.t0o), __fadd2_rn(st.s0e, st.t0e));
-    const float2 t1 = __ffma2_rn(st.sg, __fadd2_rn(st.s1o, st.t1o), __fadd2_rn(st.s1e, st.t1e));
-    y = __ffma2_rn(t1, w1, __fmul2_rn(t0, w0));
+    const float2 t0 = ffma2(st.sg, fadd2(st.s0o, st.t0o), fadd2(st.s0e, st.t0e));
+    const float2 t1 = ffma2(st.sg, fadd2(st.s1o, st.t1o), fadd2(st.s1e, st.t1e));
+    y = ffma2(t1, w1, fmul2(t0, w0));
   }
   if (accumulate) {
     y.x += out[0];
@@ -682,13 +681,13 @@ inline int launch_harmonic_v4(HarmonicParams p, cudaStream_t st) {
   using namespace hv4;
   p.Kp = (p.K + 3) & ~3;
   static const int env_fw = [] { const char* e = getenv("DDSP_B200_HARM_FW"); return e ? atoi(e) : 0; }();
-  // One warp per CTA and 11 frames per warp (12 rows = three get_controls passes):
-  // measured 295 us per B=256 decoder step against 301 for four warps x 8 frames
-  // and 306 for four warps x 16.  Small grids shrink the tile until every SM has one.
+  // One warp per CTA and 11 frames per warp (12 rows = three get_controls passes);
+  // DDSP_B200_HARM_FW overrides the frames per warp for A/B timing.  Small grids
+  // shrink the tile until every SM has one.
   int FW = (NW == 1) ? 11 : 8;
-  const long long want_ctas = 8ll * kNumSMs * (4 / NW);        // 32 warps per SM
+  const long long want_ctas = 8ll * num_sms() * (4 / NW);        // 32 warps per SM
   while (FW > 4 && (long long)p.B * ((p.F + FW * NW - 1) / (FW * NW)) < want_ctas) FW = (FW + 1) >> 1;
-  while (FW > 1 && (long long)p.B * ((p.F + FW * NW - 1) / (FW * NW)) < kNumSMs) FW = (FW + 1) >> 1;
+  while (FW > 1 && (long long)p.B * ((p.F + FW * NW - 1) / (FW * NW)) < num_sms()) FW = (FW + 1) >> 1;
   if (env_fw > 0) FW = std::min(32, env_fw);
   FW = std::max(1, std::min(FW, (p.F + NW - 1) / NW));
   while (FW > 1 && smem_layout(FW, p.Kp, p.hop).total > 64 * 1024) FW = (FW + 1) / 2;

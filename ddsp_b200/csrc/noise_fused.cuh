@@ -27,7 +27,7 @@
 //      accumulators; two register windows of 8 tap PAIRS slide over the lane's
 //      IR row (one window of even-aligned pairs for even input samples, one of
 //      odd-aligned pairs - from a copy of the row shifted by one tap - for odd
-//      ones), so two input samples cost 3 LDS.64 + 16 FFMA2 (= 32 lane-FMAs)
+//      ones), so two input samples cost 3 LDS.64 + 32 lane-FMAs
 //   E. overlap-add in shared memory (skewed layout, blocks that could collide
 //      are serialised by frame-group), F. crop + (+= harmonic) + coalesced store
 #pragma once
@@ -80,7 +80,7 @@ __host__ __device__ inline NfSmem nf_smem_layout(const NoiseFusedParams& p) {
 }
 
 __device__ __forceinline__ float2 nf_ffma2(float x, float2 w, float2 acc) {
-  return __ffma2_rn(make_float2(x, x), w, acc);
+  return ffma2(make_float2(x, x), w, acc);
 }
 
 // cp.async (LDGSTS) of one float: global -> shared without register staging.
@@ -502,7 +502,7 @@ inline int launch_noise_fused(const float* mags, const float* noise,
     return DDSP_B200_E_CUDA;
   }
   const int ctas_per_sm = smem <= 110 * 1024 ? 2 : 1;
-  const int grid = (int)std::min<long long>(n_tiles, (long long)kNumSMs * ctas_per_sm);
+  const int grid = (int)std::min<long long>(n_tiles, (long long)num_sms() * ctas_per_sm);
   noise_fused_kernel<<<grid, kNfThreads, smem, st>>>(p);
   DDSP_CHECK_LAUNCH("filtered_noise_forward(fused)");
   return 0;

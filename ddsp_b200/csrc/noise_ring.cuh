@@ -2,11 +2,9 @@
 // frame = 64 samples, 128-tap IR; ae.gin:60-68), third generation.  Same maths as
 // noise_fused.cuh (windowed zero-phase IR per frame by E/O cosine
 // sums, Philox noise, time-varying FIR == the reference's framed FFT convolution
-// + overlap-add + crop, core.py:1382-1473); the second generation
-// (profiles/experiments/noise_pipe.cuh.txt) was bound by
-// shared-memory bandwidth (67 % of LSU wavefronts at 47 % FMA-pipe utilisation,
-// profiles/r01_ncu_summary_v7.txt) and by consumer warps marching in lock step
-// through an overlap-add buffer.  What changed:
+// + overlap-add + crop, core.py:1382-1473); the second generation was bound by
+// shared-memory bandwidth and by consumer warps marching in lock step through an
+// overlap-add buffer.  What changed:
 //
 //   * GATHER FORM, NO OVERLAP-ADD.  out[64 q + n] = sum_i x_q[i] h_q[n + 62 - i]
 //     + sum_i x_{q+1}[i] h_{q+1}[n - 2 - i] + sum_i x_{q-1}[i] h_{q-1}[n + 126 - i]
@@ -22,21 +20,19 @@
 //   * TWO ACCUMULATOR SETS ON ONE TAP PAIR.  For an even input x[i] the tap pair
 //     (h[m], h[m+1]) feeds the output pair (n, n+1); for the odd input x[i+1] the
 //     SAME pair feeds (n+1, n+2).  Set A holds pairs (n, n+1), set B pairs
-//     (n+1, n+2): every MAC is an FFMA2 with a broadcast scalar input and ONE copy
-//     of the impulse response in shared memory.
+//     (n+1, n+2): every MAC is an f32x2 FMA with a broadcast scalar input and ONE
+//     copy of the impulse response in shared memory.
 //   * TAP-STATIONARY ORDER.  The 16 input pairs of a body sit in registers and the
 //     tap pairs stream through: a pair serves every (output, input) combination on
-//     its diagonal, so up to 32 consecutive FFMA2 share their packed multiplicand
-//     (the form tools/microbench3.cu measured at 2.02 cycles per instruction; the
-//     earlier sliding 16-pair tap window changed it every other instruction -
-//     profiles/experiments/noise_ring_r02_sliding_window.cuh.txt).
+//     its diagonal, so up to 32 consecutive f32x2 FMAs share their multiplicand
+//     (the earlier sliding 16-pair tap window changed it every other instruction).
 //   * TRIANGULAR TRIMMING at compile time: the rows of frames q+1 and q-1 cover
 //     complementary triangles of the (n, i) square; fully unrolled bodies skip the
 //     pairs whose taps are all out of range.
 //   * producers: two groups of 4 warps alternate tiles; a group takes its tile
 //     from raw magnitudes (TMA) through exp_sigmoid, the cosine sums (odd k, and the
 //     even k split once more by quarter-wave symmetry: 1601 MACs per frame instead
-//     of 4225; in registers as FFMA2, no exchange) and the windowed taps to the
+//     of 4225; in registers as f32x2, no exchange) and the windowed taps to the
 //     Philox rows, and asks for its ring slot only when the sums are done.
 #pragma once
 #include "noise_fused.cuh"
@@ -49,9 +45,8 @@ constexpr int NE = 33, NO = 32, SHIFT = 64;
 // A consumer warp owns a UNIT of 2 NW outputs of 32 frames: NW input pairs in
 // registers, NW + NW + 1 packed accumulators.  NW = 16 (two units per frame, ~150
 // registers, 9 KB FIR bodies) is the product; NW = 8 (four units, 96 registers,
-// twice the shared-memory loads per FFMA2) compiles (-DDDSP_NR_NW=8) and was measured
-// slower both times it was tried (357 vs 343 us per B=256 decoder step in round 1,
-// 170 vs 142 us for the kernel in round 2).
+// twice the shared-memory loads per FMA) compiles (-DDDSP_NR_NW=8) as an
+// alternative for A/B timing.
 #ifndef DDSP_NR_NW
 #define DDSP_NR_NW 16
 #endif
@@ -60,8 +55,7 @@ constexpr int UPT = FRAME / (2 * NW);              // units per 64-sample frame
 // Producer groups and ring slots.  The four consumer tile groups hold NTG + 1 = 5
 // slots between them; what is left decouples producers from consumers.  227 KB of
 // shared memory hold 7 slots next to three raw-magnitude staging buffers or 8 next
-// to two.  Measured (B = 256, kernel alone): 3 groups / 7 slots 142.2 us, 2 groups
-// / 8 slots 139.4 us (with the register split below), 2 groups / 7 slots 162 us.
+// to two; the default is 2 groups / 8 slots.
 #ifndef DDSP_NR_PROD_GROUPS
 #define DDSP_NR_PROD_GROUPS 2
 #endif
@@ -76,10 +70,10 @@ constexpr int RING = 32 * SLOTS;
 constexpr int THREADS = 32 * (CONS_WARPS + PROD_WARPS);
 // NW = 16 only: 512 threads launch with 128 registers each (the whole file); the
 // consumers (256 threads) grow to CONS_REGS out of what the producers (256 threads)
-// give back: CONS_REGS + PROD_REGS <= 256.  Measured (kernel alone, B = 256): 152 /
-// 104 138.3 us, 168 / 88 135.7 us, 136 / 120 141.1 us.  (Three groups: 640 threads at
-// 96, 144 / 64.  A split that leaves setmaxnreg.inc short of registers hangs the
-// CTA: 72 / 144 with three groups did.)
+// give back: CONS_REGS + PROD_REGS <= 256.  On sm_90a the producers spill a little
+// at 88 (fewer bytes at 96 or 104); the three splits time the same on H100
+// (DESIGN.md 3.2).  (Three groups: 640 threads at 96,
+// 144 / 64.  A split that leaves setmaxnreg.inc short of registers hangs the CTA.)
 #ifndef DDSP_NR_PROD_REGS
 #define DDSP_NR_PROD_REGS 88
 #endif
@@ -97,7 +91,7 @@ constexpr int NQ = FRAME / 4;
 // them back through ddsp_b200_debug_noise_timing); measurement builds only.
 #ifdef DDSP_NR_TIMING
 #define NR_TIMING_DECL unsigned tprev__ = (unsigned)clock()
-__device__ unsigned g_nr_timing[kNumSMs * 32 * 8];
+__device__ unsigned g_nr_timing[kMaxSMs * 32 * 8];
 #define NR_LAP(i)                                                                       \
   do {                                                                                  \
     const unsigned n__ = (unsigned)clock();                                             \
@@ -229,7 +223,7 @@ __device__ __forceinline__ Op block_op(int i, int u, const float* x_m1,
 
 // TAP-STATIONARY ORDER: the NW input pairs of a body sit in registers and the tap
 // pairs stream through - a pair P(d) at hp + 2 d serves every (c, k) with c - k = d,
-// so up to 2 NW consecutive FFMA2 share their packed multiplicand (the operand
+// so up to 2 NW consecutive f32x2 FMAs share their multiplicand (the operand
 // collector keeps it).  Bm1 (= B[-1]) takes x[2k - 1] through P(-k).
 __device__ __forceinline__ void consume_block(Acc& a, int u, const float* x_m1,
                                                  const float* h_m1, const float* x_0,
@@ -735,7 +729,7 @@ inline int launch_noise_ring(const float* mags, const float* noise, uint64_t see
   }
   // one persistent CTA per SM; tiny workloads get one CTA per 32-frame tile
   const int grid = (int)std::max<long long>(
-      1, std::min<long long>((long long)kNumSMs, (T + 31) / 32));
+      1, std::min<long long>((long long)num_sms(), (T + 31) / 32));
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(grid);
   cfg.blockDim = dim3(nr_::THREADS);

@@ -3,7 +3,7 @@
 The reference's `ProcessorGroup.__call__` is fed numpy arrays and hands back a
 tensor the caller reads on the host (processors_test.py:35-42, 80-87).  On a GPU
 that round trip is PCIe-bound: at the `ae.gin` shapes a batch item is 668 kB of
-network outputs in and 256 kB of audio out, against ~1 us of synthesis.
+network outputs in and 256 kB of audio out, against microseconds of synthesis.
 `HostDecoder` therefore cuts the batch into chunks and keeps three streams busy
 (host->device copies, the two decoder kernels, device->host copies) through
 `ddsp_b200_decoder_forward_host` (include/ddsp_b200.h), so a call costs about

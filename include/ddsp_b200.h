@@ -1,5 +1,5 @@
 /*
- * ddsp_b200.h - C ABI of libddsp_b200.so (hand-written sm_100a kernels for the
+ * ddsp_b200.h - C ABI of libddsp_b200.so (hand-written sm_90a kernels for the
  * DDSP Harmonic + FilteredNoise decoder signal path).
  *
  * The reference (magenta/ddsp v3.7.0) has no FFI: its operator API is the Python

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-  config.addinivalue_line('markers', 'gpu: needs a CUDA device (B200)')
+  config.addinivalue_line('markers', 'gpu: needs a CUDA device (H100)')
 
 
 def pytest_collection_modifyitems(config, items):

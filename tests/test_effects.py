@@ -72,30 +72,15 @@ def test_filtered_noise_reverb_composition_matches_reference(monkeypatch, traina
   are replaced by the oracle here (they have their own parity tests): what is under
   test is the composition - scale + bias, synthesis of the impulse response, tiling
   of the single learned response, dry-tap masking, 'same' convolution with zero
-  delay compensation, dry mix."""
-  from oracle import ref_on_shim
-  if not ref_on_shim.available():
-    pytest.skip('reference sources not present')
+  delay compensation, dry mix.  The reference's results, with its random draw pinned
+  to the same noise, are tests/golden/reverb_composition.npz (make_golden.py)."""
+  import os
   from ddsp_b200 import effects
-  ref = ref_on_shim.load()
-  tf = ref_on_shim.tf()
-  rng = np.random.default_rng(5)
-  B, N, L, F, NB, WS = 2, 3000, 1920, 40, 16, 257
-  audio = rng.standard_normal((B, N)).astype(np.float32)
-  mags = rng.standard_normal((1 if trainable else B, F, NB)).astype(np.float32)
-  noise = rng.uniform(-1, 1, (mags.shape[0], L)).astype(np.float32)
-
-  # ---- the reference, on the shim, with its random draw pinned ----
-  monkeypatch.setattr(tf.random, 'uniform',
-                      lambda shape, minval=0, maxval=1, **kw: tf.constant(noise))
-  r = ref.effects.FilteredNoiseReverb(trainable=trainable, reverb_length=L, window_size=WS,
-                                      n_frames=F, n_filter_banks=NB)
-  if trainable:
-    r.build(None)
-    r._magnitudes = tf.constant(mags[0])
-    want = ref_on_shim.to_numpy(r(audio))
-  else:
-    want = ref_on_shim.to_numpy(r(audio, mags))
+  from tests.golden import make_golden as mg
+  B, N, L, F, NB, WS = (mg.REVERB[k] for k in ('B', 'N', 'L', 'F', 'NB', 'WS'))
+  audio, mags, noise = mg.reverb_inputs(trainable)
+  want = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden',
+                              'reverb_composition.npz'))['out_trainable_%d' % trainable]
 
   # ---- ours, kernels swapped for the oracle ----
   def t32(x, device=None):

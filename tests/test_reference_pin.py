@@ -1,16 +1,14 @@
 """Pins the oracle to the reference itself (CPU, no GPU).
 
-tests/golden/*.npz hold outputs of the UNMODIFIED reference (/root/reference/ddsp
-run on oracle/tf_shim, see tests/golden/make_golden.py): "f32" = the reference's
-own float32 arithmetic, "wide" = the same reference code evaluated in float64.
-
-  * wherever the reference sources are present (the authoring container) the
-    fixtures are regenerated and must match bit for bit, and the reference's own
-    unit tests for the path must pass on the shim;
-  * everywhere (GPU box included) oracle/ddsp_oracle.py - the arbiter of the
-    `-m gpu` parity tests - must reproduce the fixtures: its float32 mode to the
-    reference's float32 result within a few ulp, its float64 mode to the wide
-    result to 1e-9.
+tests/golden/*.npz hold outputs of the UNMODIFIED reference (magenta/ddsp run on
+oracle/tf_shim, see tests/golden/make_golden.py): "f32" = the reference's own
+float32 arithmetic, "wide" = the same reference code evaluated in float64.
+oracle/ddsp_oracle.py - the arbiter of the `-m gpu` parity tests - must reproduce
+them: its float32 mode to the reference's float32 result within a few ulp, its
+float64 mode to the wide result to 1e-9.  Where the reference sources are checked
+out, `make_golden.py --check` regenerates the fixtures and compares them bit for
+bit, and `python -m oracle.run_reference_tests` runs the reference's own unit tests
+of the path on the shim.
 """
 import os
 
@@ -18,13 +16,9 @@ import numpy as np
 import pytest
 
 from oracle import ddsp_oracle as o
-from oracle import ref_on_shim
 from tests.util import rel_err, synth_inputs
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
-needs_reference = pytest.mark.skipif(
-    not ref_on_shim.available(),
-    reason='reference sources (/root/reference) are only in the authoring container')
 
 
 def gold(name):
@@ -37,27 +31,6 @@ def inputs_for(g, *shape, **kw):
   assert abs(checksum(inp) - float(g['input_checksum'])) <= 1e-6 * abs(float(g['input_checksum'])), \
       'synth_inputs no longer reproduces the inputs this fixture was made from'
   return inp
-
-
-# ---------------------------------------------------------------------------
-# fixtures <-> reference (authoring container only)
-# ---------------------------------------------------------------------------
-@needs_reference
-def test_fixtures_are_outputs_of_the_unmodified_reference():
-  from tests.golden import make_golden as mg
-  for name, fn in mg.FIXTURES.items():
-    mg.compare(name, fn(), gold(name), atol=0.0)
-
-
-@needs_reference
-def test_reference_own_unit_tests_pass_on_the_shim():
-  """ddsp/core_test.py, synths_test.py, processors_test.py - the reference's own
-  tests of this path - run unmodified against oracle/tf_shim."""
-  import io
-  from oracle import run_reference_tests
-  res = run_reference_tests.run(stream=io.StringIO())
-  assert res.testsRun >= 96
-  assert res.wasSuccessful(), (res.failures[:2], res.errors[:2])
 
 
 # ---------------------------------------------------------------------------

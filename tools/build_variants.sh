@@ -4,7 +4,7 @@ cd "$(dirname "$0")/.."
 mkdir -p tools/variants
 while [ $# -gt 1 ]; do
   name=$1; flags=$2; shift 2
-  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -shared $flags \
+  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -shared $flags \
     -o tools/variants/lib_$name.so ddsp_b200/csrc/capi.cu &
 done
 wait

@@ -26,16 +26,19 @@ for i in range(4):
                                             0, 1, None, 0, st)
   assert rc == 0, lib.ddsp_b200_last_error()
 torch.cuda.synchronize()
-buf = np.zeros((148, 32, 8), np.uint32)
+MAX_SMS = 256   # kMaxSMs in ddsp_b200/csrc/common.cuh
+buf = np.zeros((MAX_SMS, 32, 8), np.uint32)
 assert lib.ddsp_b200_debug_noise_timing(buf.ctypes.data) == 0
 t = buf.astype(np.float64)
+t = t[t.sum(axis=(1, 2)) > 0]                    # the CTAs of the grid
+N_SMS = len(t)
 n_warps = int((t.sum(axis=(0, 2)) > 0).sum())
 cons, prod = t[:, :8], t[:, 8:n_warps]
 cn = ['wait full', 'FIR', 'release + store', 'loop / skip']
 pn = ['wait raw (TMA)', 'exp_sigmoid + bar', 'wait empty', 'cosine sums', 'bar + prefetch',
       'taps epilogue', 'Philox rows + arrive', 'iterate']
-print('%s: B=%d, %d warps per CTA; cycles per warp, mean over 148 CTAs (min .. max of the per-CTA means)' %
-      (os.path.basename(path), B, n_warps))
+print('%s: B=%d, %d warps per CTA; cycles per warp, mean over %d CTAs (min .. max of the per-CTA means)' %
+      (os.path.basename(path), B, n_warps, N_SMS))
 tot = cons.sum(axis=2).mean()
 print('consumers: %.0f cycles in the tile loop' % tot)
 for i, nm in enumerate(cn):

@@ -24,6 +24,7 @@ def main(tag):
                        check=True).stdout
   funcs = re.split(r'\n\s*Function : ', txt)
   out_dir = os.path.join(ROOT, 'profiles')
+  os.makedirs(out_dir, exist_ok=True)
   for short, pat in KERNELS.items():
     body = next((f for f in funcs if pat in f.split('\n', 1)[0]), None)
     if body is None:
@@ -57,7 +58,7 @@ def main(tag):
     path = os.path.join(out_dir, '%s_sass_%s.txt' % (tag, short))
     with open(path, 'w') as f:
       f.write('%s\n%d SASS instructions (cuobjdump -sass of ddsp_b200/libddsp_b200.so, '
-              'sm_100a)\n\nopcode histogram (top 24):\n' % (name, len(lines)))
+              'sm_90a)\n\nopcode histogram (top 24):\n' % (name, len(lines)))
       for op, n in ops.most_common(24):
         f.write('  %-12s %5d\n' % (op, n))
       marks = {k: ops.get(k, 0) for k in ('FFMA2', 'FADD2', 'FMUL2', 'UBLKCP', 'SYNCS',
