@@ -220,6 +220,12 @@ struct NoiseBwdParams {
 };
 constexpr int kEoStride = 36;       // 33 columns k = 0..32, padded to float4s
 
+// Offset in floats of the cosine table: behind the tables and rows, rounded up to a
+// float4.
+__host__ __device__ inline size_t noise_bwd_eo_offset(const NoiseBwdParams& p) {
+  return ((size_t)p.g.S0 + p.S + 32 * (size_t)(p.xS + p.gS + p.hS) + 3) & ~(size_t)3;
+}
+
 __global__ void __launch_bounds__(kNbThreads)
 noise_backward_kernel(NoiseBwdParams p) {
   extern __shared__ __align__(16) float sm[];
@@ -228,7 +234,9 @@ noise_backward_kernel(NoiseBwdParams p) {
   float* sX = sWin + p.S;                        // [32][xS]
   float* sG = sX + 32 * p.xS;                    // [32][gS]   gy rows
   float* sH = sG + 32 * p.gS;                    // [32][hS]   dh rows, then dh0
-  float* sEo = sH + 32 * p.hS;                   // [nh][kEoStride] cos(2 pi k n / S0), k <= 32
+  // [nh][kEoStride] cos(2 pi k n / S0), k <= 32, read as float4: 16-byte aligned even
+  // when S is odd (padded windows)
+  float* sEo = sm + noise_bwd_eo_offset(p);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nb = p.nb, S = p.S, S0 = p.g.S0, frame = p.frame;
   for (int i = tid; i < S0; i += kNbThreads) sCos[i] = cospif(2.0f * (float)i / (float)S0);

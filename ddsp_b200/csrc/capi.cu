@@ -776,7 +776,7 @@ int ddsp_b200_filtered_noise_backward(const float* grad_audio, const float* nois
                "filtered_noise_backward: too many tiles");
   p.n_tiles = (int)n_tiles;
   p.eo_tab = (nb == 65 && p.g.S0 == 128 && p.nh == 65) ? 1 : 0;
-  const size_t smem = sizeof(float) * ((size_t)p.g.S0 + p.S + 32 * (size_t)(p.xS + p.gS + p.hS) +
+  const size_t smem = sizeof(float) * (noise_bwd_eo_offset(p) +
                                        (p.eo_tab ? (size_t)p.nh * kEoStride : 0));
   DDSP_REQUIRE(smem <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
                "filtered_noise_backward: shape needs %zu B of shared memory", smem);

@@ -1,0 +1,224 @@
+"""Differentiable float64 torch restatements of core.harmonic_synthesis and
+core.frequency_filter, the references the backward kernels are checked against
+(float64 autograd through them is "what TF autodiff gives the reference").
+
+Both follow oracle/ddsp_oracle.py op by op, so that tests/test_grad_ref.py can pin
+them to the oracle at <= 1e-12 on the CPU, and both run on whatever device their
+inputs live on.
+
+* `harmonic`: any integer hop, amp_resample_method 'window' or 'linear', any
+  sample rate.  The audio-rate Nyquist mask is an input: `nyquist_mask` takes that
+  yes / no decision in float32 (f0 * k, then the lerp), as the reference's float32
+  arithmetic and `oracle.harmonic_synthesis(mask_in_float32=True)` do.  Deciding it
+  in float64 would flip whole oscillators on samples whose frequency lies within
+  an ulp of Nyquist.
+* `impulse_response` / `frequency_filter`: any number of bins and any window size
+  (symmetric Hann for odd windows, the padded / centred layout and its slicing,
+  the `(S - 1) // 2 - 1` crop), and ragged frames (`frame = ceil(N / F)`, the last
+  frame zero padded).
+"""
+import math
+
+import torch
+
+TWO_PI = 2.0 * math.pi
+
+
+def _frame_index(n_frames, n_samples, device):
+  """Bilinear-resize index math (align_corners=False) for an integer hop: lower /
+  upper frame and the float64 lerp weight of every sample."""
+  if n_samples % n_frames:
+    raise ValueError('n_samples (%d) must be a multiple of n_frames (%d)'
+                     % (n_samples, n_frames))
+  hop = n_samples // n_frames
+  t = torch.arange(n_samples, device=device)
+  lo, r = t // hop, t % hop
+  hi = torch.clamp(lo + (r > 0).long(), max=n_frames - 1)
+  return hop, lo, hi, r, r.to(torch.float64) / hop
+
+
+def nyquist_mask(f0_hz, n_harmonics, n_samples, sample_rate):
+  """[B, N, K] bool, True where harmonic k is silenced at sample t: the float32
+  decision f_k(t) >= sr / 2 with f_k = f0 * k and the lerp each rounded to float32
+  (core.py:869-891 evaluated as the reference does; oracle `mask_in_float32`)."""
+  f0 = f0_hz.to(torch.float32)
+  b, f, _ = f0.shape
+  ratios = torch.arange(1, n_harmonics + 1, dtype=torch.float32, device=f0.device)
+  hf = f0 * ratios
+  _, lo, hi, _, frac = _frame_index(f, n_samples, f0.device)
+  top, bottom = hf[:, lo], hf[:, hi]
+  fe = top + (bottom - top) * frac.to(torch.float32)[None, :, None]
+  return fe >= torch.tensor(sample_rate / 2.0, dtype=torch.float32)
+
+
+def harmonic(f0_hz, amplitudes, harmonic_distribution, n_samples, sample_rate=16000,
+             amp_resample_method='window', mask=None):
+  """core.harmonic_synthesis (core.py:1048-1111) in float64 torch ops, without
+  harmonic_shifts.  `mask` is a `nyquist_mask` (computed here when None)."""
+  f0 = f0_hz.to(torch.float64)
+  amp = amplitudes.to(torch.float64)
+  hd = harmonic_distribution.to(torch.float64)
+  b, f, k = hd.shape
+  dev = hd.device
+  if mask is None:
+    mask = nyquist_mask(f0_hz, k, n_samples, sample_rate)
+  hop, lo, hi, r, frac = _frame_index(f, n_samples, dev)
+  hf = f0 * torch.arange(1, k + 1, dtype=torch.float64, device=dev)
+  ha = amp * hd
+  frac = frac[None, :, None]
+  fe = hf[:, lo] + (hf[:, hi] - hf[:, lo]) * frac
+  if amp_resample_method == 'window':
+    # upsample_with_windows (core.py:645-714): Hann(2 hop) overlap-add on the frames
+    # plus a copy of the last one; sample r of frame i sees window taps hop + r and r
+    nxt = torch.clamp(lo + 1, max=f - 1)
+    rr = r.to(torch.float64)[None, :, None]
+    w_prev = 0.5 - 0.5 * torch.cos(TWO_PI * (hop + rr) / (2 * hop))
+    w_next = 0.5 - 0.5 * torch.cos(TWO_PI * rr / (2 * hop))
+    ae = ha[:, lo] * w_prev + ha[:, nxt] * w_next
+  elif amp_resample_method == 'linear':
+    ae = ha[:, lo] + (ha[:, hi] - ha[:, lo]) * frac
+  else:
+    raise ValueError(amp_resample_method)
+  ae = torch.where(mask, torch.zeros_like(ae), ae)
+  phase = torch.cumsum(fe * TWO_PI / float(sample_rate), dim=1)
+  return (ae * torch.sin(phase)).sum(-1)
+
+
+def hann_window(n, dtype=torch.float64, device=None):
+  """tf.signal.hann_window(n): periodic for even n, symmetric for odd n, [1] for
+  n = 1 (oracle.hann_window)."""
+  if n == 1:
+    return torch.ones(1, dtype=dtype, device=device)
+  k = torch.arange(n, dtype=torch.float64, device=device)
+  d = n if n % 2 == 0 else n - 1
+  return (0.5 - 0.5 * torch.cos(TWO_PI * k / d)).to(dtype)
+
+
+def impulse_response(magnitudes, window_size=0):
+  """core.frequency_impulse_response (core.py:1534-1565) with
+  apply_window_to_impulse_response (core.py:1477-1531): [..., nb] -> [..., S]."""
+  mags = magnitudes.to(torch.float64)
+  ir = torch.fft.irfft(mags.to(torch.complex128))
+  s = ir.shape[-1]
+  if window_size <= 0 or window_size > s:
+    window_size = s
+  win = hann_window(window_size, device=ir.device)
+  padding = s - window_size
+  if padding > 0:
+    half = (window_size + 1) // 2
+    win = torch.cat([win[half:], win.new_zeros(padding), win[:half]])
+  else:
+    win = torch.fft.fftshift(win)
+  ir = win * ir
+  if padding > 0:
+    first_half_start = (s - (half - 1)) + 1
+    second_half_end = half + 1
+    return torch.cat([ir[..., first_half_start:], ir[..., :second_half_end]], dim=-1)
+  return torch.fft.fftshift(ir, dim=-1)
+
+
+def fft_convolve(audio, ir):
+  """core.fft_convolve(padding='same', delay_compensation=-1) (core.py:1382-1473)
+  of [B, N] audio with [B, F, S] impulse responses: frames of ceil(N / F) samples,
+  the last one zero padded, FFT size the next power of two of S + frame - 1."""
+  audio = audio.to(torch.float64)
+  b, n = audio.shape
+  _, f, s = ir.shape
+  frame = -(-n // f)
+  if -(-n // frame) != f:
+    raise ValueError('%d frames do not tile %d samples' % (f, n))
+  frames = torch.nn.functional.pad(audio, (0, f * frame - n)).reshape(b, f, frame)
+  nfft = 1 << (s + frame - 2).bit_length()
+  y = torch.fft.irfft(torch.fft.rfft(frames, nfft) * torch.fft.rfft(ir, nfft), nfft)
+  # overlap-add: split every frame's output into blocks of `frame` samples and add
+  # block j of frame i at output block i + j
+  m = -(-nfft // frame)
+  y = torch.nn.functional.pad(y, (0, m * frame - nfft)).reshape(b, f, m, frame)
+  out = sum(torch.nn.functional.pad(y[:, :, j], (0, 0, j, m - 1 - j)) for j in range(m))
+  total = (f - 1) * frame + nfft
+  out = out.reshape(b, (f + m - 1) * frame)[:, :total]
+  # crop_and_compensate_delay, sliced as the reference slices (a window of one or
+  # two taps gives start = -1)
+  start = (s - 1) // 2 - 1
+  end = total - n - start
+  return out[:, start:-end]
+
+
+def frequency_filter(audio, magnitudes, window_size=0):
+  """core.frequency_filter (core.py:1628-1655), padding='same'."""
+  return fft_convolve(audio, impulse_response(magnitudes, window_size))
+
+
+# Harmonic backward cases: (B, F, K, hop, sample_rate, amp method, f0 regime).  Every
+# hop (64: harmonic_backward2_kernel; 128 / 192 / 256: harmonic_backward_kernel), K,
+# F, method, rate and regime at least once; K = 7 / 9 / 100 / 260 reach the uniform
+# loop of the hop-64 kernel with K % 8 != 0.
+HARMONIC_CASES = [
+    (2, 33, 100, 64, 16000, 'window', 'jump'),
+    (2, 33, 100, 64, 16000, 'linear', 'glide'),
+    (1, 257, 7, 64, 44100, 'window', 'unvoiced'),
+    (2, 33, 260, 64, 16000, 'linear', 'subhertz'),
+    (2, 2, 9, 128, 16000, 'window', 'cross1hz'),
+    (1, 257, 1, 128, 44100, 'linear', 'nyquist'),
+    (1, 33, 100, 128, 44100, 'window', 'glide'),
+    (1, 1, 8, 192, 44100, 'linear', 'cross1hz'),
+    (2, 33, 7, 192, 16000, 'window', 'unvoiced'),
+    (2, 33, 260, 256, 16000, 'window', 'nyquist'),
+    (1, 33, 100, 256, 16000, 'linear', 'jump'),
+]
+
+# Filtered-noise backward cases: (B, F, nb, window_size, frame, ragged).  `ragged`
+# drops 7 samples from the last frame (N = F * frame - 7).  Padded windows odd and
+# even, windows clamped to the IR, even nb, frames other than 64, F not a multiple
+# of 32.
+NOISE_CASES = [
+    (2, 32, 65, 0, 64, False),
+    (1, 33, 65, 64, 64, False),
+    (2, 31, 65, 65, 64, False),
+    (1, 100, 65, 31, 16, False),
+    (2, 1, 64, 0, 48, False),
+    (1, 33, 33, 257, 100, True),
+    (2, 100, 16, 257, 48, False),
+    (1, 31, 129, 0, 64, False),
+    (2, 32, 129, 101, 64, False),
+]
+
+
+def low_f0_regime(regime, B, F, sample_rate, seed):
+  """[B, F, 1] float32 f0 tracks for the edges of the harmonic kernels:
+    'unvoiced'  - runs of f0 = 0 between voiced frames;
+    'subhertz'  - runs of 0 < f0 < 1 Hz;
+    'cross1hz'  - frames alternating across 1 Hz (0.3 .. 3 Hz);
+    'jump'      - f0 = 0 next to 1500 .. 2000 Hz: in those frames the per-oscillator
+                  mask of the exact (f0 < 1 Hz) branch silences upper harmonics;
+    'glide'     - fast glides whose live harmonic count changes inside most frames;
+    'nyquist'   - runs of frames at or above sr / 2 (no live harmonic at all).
+  Voiced frames elsewhere sit at 80 .. 600 Hz."""
+  g = torch.Generator().manual_seed(seed)
+  base = 80.0 + 520.0 * torch.rand(B, F, 1, generator=g, dtype=torch.float64)
+  i = torch.arange(F, dtype=torch.float64)[None, :, None]
+  run = ((torch.arange(F) // 3) % 2 == 1)[None, :, None]
+  if regime == 'unvoiced':
+    f0 = torch.where(run, torch.zeros_like(base), base)
+  elif regime == 'subhertz':
+    sub = 0.05 + 0.9 * torch.rand(B, F, 1, generator=g, dtype=torch.float64)
+    f0 = torch.where(run, sub, base)
+  elif regime == 'cross1hz':
+    f0 = torch.where(((torch.arange(F) % 2) == 0)[None, :, None],
+                     0.3 + 0.6 * torch.rand(B, F, 1, generator=g, dtype=torch.float64),
+                     1.2 + 1.8 * torch.rand(B, F, 1, generator=g, dtype=torch.float64))
+  elif regime == 'jump':
+    hi = 1500.0 + 500.0 * torch.rand(B, F, 1, generator=g, dtype=torch.float64)
+    f0 = torch.where(((torch.arange(F) % 2) == 0)[None, :, None], torch.zeros_like(hi), hi)
+  elif regime == 'glide':
+    # +-40 % per frame around 500 Hz: with K harmonics the live count changes inside
+    # almost every frame once K * f0 reaches sr / 2
+    f0 = 500.0 * (1.0 + 0.4 * torch.sin(2.1 * i + 6.0 * torch.rand(B, 1, 1, generator=g,
+                                                                     dtype=torch.float64)))
+  elif regime == 'nyquist':
+    f0 = torch.where(run, (0.5 + 0.2 * torch.rand(B, F, 1, generator=g,
+                                                   dtype=torch.float64)) * sample_rate,
+                     base)
+  else:
+    raise ValueError(regime)
+  return f0.to(torch.float32)

@@ -1,55 +1,26 @@
 """Backward kernels vs float64 torch autograd of an op-by-op restatement."""
-import math
-
 import numpy as np
 import pytest
 import torch
 
 from ddsp_b200 import autograd as ag
 from ddsp_b200 import losses
+from tests import grad_ref
 from tests.util import synth_inputs
 
 pytestmark = pytest.mark.gpu
 
 
 def ref_harmonic(f0, amp, hd, n_samples, sr=16000.0, linear_amp=False):
-  """core.harmonic_synthesis (core.py:1048-1111) in float64 torch ops."""
-  b, f, k = hd.shape
-  hop = n_samples // f
-  ratios = torch.arange(1, k + 1, dtype=torch.float64, device=f0.device)
-  hf = f0 * ratios
-  ha = amp * hd
-  t = torch.arange(n_samples, device=f0.device)
-  i, r = t // hop, (t % hop).to(torch.float64)
-  i1 = torch.clamp(i + 1, max=f - 1)
-  frac = (r / hop)[None, :, None]
-  fe = hf[:, i] + (hf[:, i1] - hf[:, i]) * frac
-  w1 = (0.5 - 0.5 * torch.cos(math.pi * r / hop))[None, :, None]
-  if linear_amp:
-    w1 = frac
-  ae = ha[:, i] * (1 - w1) + ha[:, i1] * w1
-  ae = torch.where(fe >= sr / 2, torch.zeros_like(ae), ae)
-  phase = torch.cumsum(fe * (2 * math.pi / sr), dim=1)
-  return (ae * torch.sin(phase)).sum(-1)
+  """core.harmonic_synthesis in float64 torch ops (tests/grad_ref.py)."""
+  return grad_ref.harmonic(f0, amp, hd, n_samples, sr,
+                           'linear' if linear_amp else 'window')
 
 
 def ref_noise(mags, noise, n_samples):
-  """core.frequency_filter (core.py:1628-1655), window_size=0, float64."""
-  b, f, nb = mags.shape
-  ir = torch.fft.irfft(mags.to(torch.complex128))
-  s = ir.shape[-1]
-  win = torch.hann_window(s, periodic=True, dtype=torch.float64, device=mags.device)
-  ir = torch.fft.fftshift(torch.fft.fftshift(win) * ir, dim=-1)
-  frame = n_samples // f
-  frames = noise.reshape(b, f, frame)
-  nfft = 1 << (s + frame - 2).bit_length()
-  y = torch.fft.irfft(torch.fft.rfft(frames, nfft) * torch.fft.rfft(ir, nfft), nfft)
-  total = (f - 1) * frame + nfft
-  out = torch.zeros(b, total, dtype=torch.float64, device=mags.device)
-  for j in range(f):
-    out[:, j * frame:j * frame + nfft] += y[:, j]
-  start = (s - 1) // 2 - 1
-  return out[:, start:start + n_samples]
+  """core.frequency_filter, window_size=0, in float64 torch ops (tests/grad_ref.py)."""
+  assert noise.shape[-1] == n_samples
+  return grad_ref.frequency_filter(noise, mags, 0)
 
 
 @pytest.mark.parametrize('B,F,K', [(2, 20, 12), (1, 33, 100), (2, 8, 5)])

@@ -389,7 +389,7 @@ def test_noise_ring_stress_random_shapes_against_the_generic_path():
   (every segment geometry: items shorter than a tile, CTA ranges cut mid-item, ring
   wrap-around), back to back on one stream, each result compared (a) bit for bit
   with a repeat of the same launch and (b) with the generic, unspecialised path -
-  separate impulse-response and FIR kernels, no ring, no warp roles - to 2e-6 of
+  separate impulse-response and FIR kernels, no ring, no warp roles - to 2e-5 of
   the peak.  A stale tap row or a half-written noise row would be an O(1) error."""
   from ddsp_b200 import _lib
   lib = _lib.load()
