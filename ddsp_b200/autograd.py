@@ -154,7 +154,11 @@ class FftConvolveLtiFn(torch.autograd.Function):
     dL/dx[m]  = (g * reverse(h)) [m + S - 1 - start]
     dL/dh[s]  = (g * reverse(x)) [s + N - 1 - start]     (summed over the batch when
                                                           the IR is shared)
-  - three calls of the same partitioned overlap-save kernels."""
+  - three calls of the same partitioned overlap-save kernels.  The crop ends at
+  start + out_len, so audio samples and taps at or beyond it reach no output: their
+  gradients are zero and only the taps / samples below it are convolved (an
+  impulse response longer than the audio asks for a d IR crop past the end of
+  g * reverse(x) otherwise)."""
 
   @staticmethod
   def forward(ctx, audio, ir, start, out_len):
@@ -171,21 +175,26 @@ class FftConvolveLtiFn(torch.autograd.Function):
     b, n = audio.shape
     ir_batch, s = ir.shape
     g = g.contiguous().to(torch.float32)
+    end = start + out_len
     d_audio = d_ir = None
     if ctx.needs_input_grad[0]:
+      live = min(n, end)
       off = s - 1 - start
       if off >= 0:
-        d_audio = core.fft_convolve_lti(g, ir, off, n, reverse_ir=True)
+        d_audio = core.fft_convolve_lti(g, ir, off, live, reverse_ir=True)
       else:      # crop starts beyond the IR length: shift through a padded gradient
         gp = torch.nn.functional.pad(g, (-off, 0))
-        d_audio = core.fft_convolve_lti(gp, ir, 0, n, reverse_ir=True)
+        d_audio = core.fft_convolve_lti(gp, ir, 0, live, reverse_ir=True)
+      d_audio = torch.nn.functional.pad(d_audio, (0, n - live))
     if ctx.needs_input_grad[1]:
+      live = min(s, end)
       off = n - 1 - start
       if off >= 0:
-        d_ir = core.fft_convolve_lti(g, audio, off, s, reverse_ir=True)
+        d_ir = core.fft_convolve_lti(g, audio, off, live, reverse_ir=True)
       else:
         gp = torch.nn.functional.pad(g, (-off, 0))
-        d_ir = core.fft_convolve_lti(gp, audio, 0, s, reverse_ir=True)
+        d_ir = core.fft_convolve_lti(gp, audio, 0, live, reverse_ir=True)
+      d_ir = torch.nn.functional.pad(d_ir, (0, s - live))
       if ir_batch == 1 and b > 1:
         d_ir = d_ir.sum(0, keepdim=True)
     return d_audio, d_ir, None, None

@@ -16,6 +16,10 @@ inputs live on.
   (symmetric Hann for odd windows, the padded / centred layout and its slicing,
   the `(S - 1) // 2 - 1` crop), and ragged frames (`frame = ceil(N / F)`, the last
   frame zero padded).
+* `convolve_lti`: the long-impulse-response convolution (`FftConvolveLtiFn`,
+  `Reverb`) at any crop.
+* `spectral_loss`: the multi-scale 'L1' spectrogram loss (`SpectralLossFn`) at any
+  FFT sizes and weights; `stft_frames` is its framing (`FrameWindowFn`).
 """
 import math
 
@@ -149,6 +153,67 @@ def frequency_filter(audio, magnitudes, window_size=0):
   return fft_convolve(audio, impulse_response(magnitudes, window_size))
 
 
+def convolve_lti(audio, ir, start, out_len):
+  """Full linear convolution of audio [B, N] with one impulse response per item
+  [1 or B, S] (batch 1 broadcast), cropped to [start, start + out_len): rfft / irfft
+  at length N + S - 1, and zeros past it, as in the reference's zero-padded FFT
+  buffer.  This is core.fft_convolve on a 2-D impulse response, and what
+  `ddsp_b200_fft_convolve_lti` computes."""
+  audio = audio.to(torch.float64)
+  ir = ir.to(torch.float64)
+  n, s = audio.shape[-1], ir.shape[-1]
+  m = n + s - 1
+  y = torch.fft.irfft(torch.fft.rfft(audio, m) * torch.fft.rfft(ir, m), m)
+  y = torch.nn.functional.pad(y, (0, max(0, start + out_len - m)))
+  return y[:, start:start + out_len]
+
+
+def stft_frames(audio, frame_size):
+  """spectral_ops.stft's framing (spectral_ops.py:34-47): tf.signal.stft with
+  pad_end=True and the periodic Hann window, step frame_size / 4, frames of
+  [B, ceil(N / step), frame_size] before the rfft."""
+  audio = audio.to(torch.float64)
+  step = frame_size // 4
+  n = audio.shape[-1]
+  n_frames = -(-n // step)
+  pad = (n_frames - 1) * step + frame_size - n
+  frames = torch.nn.functional.pad(audio, (0, pad)).unfold(-1, frame_size, step)
+  return frames * hann_window(frame_size, device=audio.device)
+
+
+def safe_log(x, eps=1e-5):
+  """core.safe_log (core.py:213-216): log(eps) where x <= 0, with no gradient
+  there."""
+  return torch.log(torch.where(x <= 0.0, torch.full_like(x, eps), x))
+
+
+def spectral_loss(target, value, fft_sizes=(2048, 1024, 512, 256, 128, 64),
+                  mag_weight=1.0, logmag_weight=0.0, spectra=None):
+  """SpectralLoss.call with loss_type='L1' (losses.py:194-243): per FFT size, the
+  mean over batch, frames and bins of |mag_t - mag_v| and of |safe_log mag_t -
+  safe_log mag_v|; a weight of 0 drops its term.
+
+  `spectra`: optional (target STFT, value STFT) per FFT size, e.g. the float32 ones
+  a kernel saw.  The loss and its derivatives are then evaluated AT those spectra,
+  while d STFT / d value stays the float64 framing and rfft.  The log-magnitude
+  gradient is sign / |X| per bin, so with float32 spectra the float32 rounding of
+  the smallest magnitudes and of near-zero differences would otherwise dominate an
+  elementwise comparison of d value."""
+  loss = 0.0
+  for i, size in enumerate(fft_sizes):
+    xt = torch.fft.rfft(stft_frames(target, size), dim=-1)
+    xv = torch.fft.rfft(stft_frames(value, size), dim=-1)
+    if spectra is not None:
+      xt = spectra[i][0].to(xt.dtype).detach()
+      xv = xv + (spectra[i][1].to(xv.dtype) - xv).detach()
+    t, v = xt.abs(), xv.abs()
+    if mag_weight > 0:
+      loss = loss + mag_weight * (t - v).abs().mean()
+    if logmag_weight > 0:
+      loss = loss + logmag_weight * (safe_log(t) - safe_log(v)).abs().mean()
+  return loss
+
+
 # Harmonic backward cases: (B, F, K, hop, sample_rate, amp method, f0 regime).  Every
 # hop (64: harmonic_backward2_kernel; 128 / 192 / 256: harmonic_backward_kernel), K,
 # F, method, rate and regime at least once; K = 7 / 9 / 100 / 260 reach the uniform
@@ -182,6 +247,56 @@ NOISE_CASES = [
     (1, 31, 129, 0, 64, False),
     (2, 32, 129, 101, 64, False),
 ]
+
+
+# Spectral-loss cases: (B, N, fft_sizes, mag_weight, logmag_weight, upstream).
+# N = 1000 is shorter than the 2048 / 4096-point frames; N = 12345 is a multiple of
+# no step, and with B = 3 its 2048-point STFT has an odd number of bins (the scalar
+# tail of spectral_l1_kernel).  `upstream`: the loss itself, 0.37 * loss, or loss +
+# an audio term (see test_gpu_backward_edges.py).
+DEFAULT_FFT_SIZES = (2048, 1024, 512, 256, 128, 64)
+SPECTRAL_CASES = [
+    (2, 1000, DEFAULT_FFT_SIZES, 1.0, 1.0, 'one'),
+    (1, 1000, (4096, 16), 0.3, 2.5, 'sum'),
+    (3, 12345, DEFAULT_FFT_SIZES, 1.0, 1.0, 'scaled'),
+    (3, 12345, DEFAULT_FFT_SIZES, 0.0, 1.0, 'one'),
+    (3, 12345, (4096, 16), 1.0, 0.0, 'scaled'),
+    (3, 12345, (4096, 16), 1.0, 1.0, 'sum'),
+    (1, 64000, DEFAULT_FFT_SIZES, 0.3, 2.5, 'sum'),
+    (2, 64000, DEFAULT_FFT_SIZES, 1.0, 0.0, 'scaled'),
+]
+
+
+def spectral_signals(B, N, fft_sizes, seed):
+  """(target, value) float32 [B, N] for the spectral-loss tests.
+
+  Below 2 * (largest frame + 64) + 768 samples both are independent white noise.
+  Longer signals have three stretches, separated by gaps where both are silent and
+  which are wider than any frame, so that every frame sees one stretch only:
+    1. target == value: both terms and their gradients are exactly 0;
+    2. target = 2 * value: exact in float32, so every |mag_t - mag_v| and every
+       log-magnitude difference (log 2) is far from 0 and no sign is decided by
+       rounding;
+    3. value silent, target white noise: the value's magnitudes are exactly 0
+       (safe_log's eps branch in the loss, the `ma > 0` guard in the gradient)."""
+  gen = torch.Generator().manual_seed(seed)
+  value = 0.1 * torch.randn(B, N, generator=gen)
+  other = 0.1 * torch.randn(B, N, generator=gen)
+  gap = max(fft_sizes) + 64
+  if N < 2 * gap + 768:
+    return other, value
+  r = (N - 2 * gap) // 3
+  b0 = N - 2 * gap - 2 * r              # [0, b0): equal
+  b1 = b0 + gap                         # [b1, b1 + r): target = 2 * value
+  b2 = b1 + r + gap                     # [b2, N): value silent, target noise
+  target = value.clone()
+  value[:, b0:b1] = 0.0
+  target[:, b0:b1] = 0.0
+  target[:, b1:b1 + r] *= 2.0
+  value[:, b1 + r:] = 0.0
+  target[:, b1 + r:b2] = 0.0
+  target[:, b2:] = other[:, b2:]
+  return target, value
 
 
 def low_f0_regime(regime, B, F, sample_rate, seed):

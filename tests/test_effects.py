@@ -10,6 +10,7 @@ import torch
 
 from oracle import ddsp_oracle as o
 from ddsp_b200 import core
+from tests.util import rel_err
 
 
 def _fft_path(audio, ir, padding, delay):
@@ -116,7 +117,6 @@ def test_filtered_noise_reverb_composition_matches_reference(monkeypatch, traina
 @pytest.mark.parametrize('taps,add_dry', [(3000, True), (48000, False), (200, True)])
 def test_reverb_matches_oracle(taps, add_dry):
   import ddsp_b200
-  from tests.util import rel_err
   rng = np.random.default_rng(taps)
   B, N = 2, 16000
   audio = rng.standard_normal((B, N)).astype(np.float32)
@@ -139,7 +139,6 @@ def test_reverb_matches_oracle(taps, add_dry):
 @pytest.mark.gpu
 def test_trainable_reverb_and_fir_filter():
   import ddsp_b200
-  from tests.util import rel_err
   rng = np.random.default_rng(3)
   B, N, F, nb = 2, 6400, 100, 65
   audio = rng.standard_normal((B, N)).astype(np.float32)
@@ -164,12 +163,22 @@ def test_trainable_reverb_and_fir_filter():
     (2, 16000, 2048, 2, 'same', -1),        # smallest IR on this route, auto delay
     (2, 5000, 9000, 2, 'valid', 0),         # IR longer than the audio, full tail
     (1, 1023, 2049, 1, 'same', 0),          # ragged against the 1024-sample blocks
-    (2, 4097, 4096, 2, 'same', 5)])
+    (2, 4097, 4096, 2, 'same', 5),
+    (2, 1, 2048, 2, 'same', 0),             # one-sample audio
+    (1, 2, 2049, 1, 'valid', 0),
+    (2, 1025, 3072, 2, 'same', 0),          # one sample past a block, S = 3 blocks
+    (2, 2047, 3073, 1, 'valid', 0),         # 'valid' with S > n, shared IR
+    (2, 16000, 48000, 2, 'same', -1),       # auto delay: start 23998, j_first = 15
+    (2, 4000, 3000, 2, 'same', 1500),       # positive delay past one block
+    (5, 3001, 2048, 1, 'same', 0)])         # IR batch 1 at B = 5
 def test_long_impulse_response_convolution_kernel(B, n, taps, ir_batch, padding, delay):
   """`ddsp_b200_fft_convolve_lti` (partitioned overlap-save, hand-written FFTs)
   behind core.fft_convolve for 2-D / single-frame impulse responses >= 2048 taps,
-  against the oracle's restatement of core.py:1382-1473."""
-  from tests.util import rel_err
+  against the oracle's restatement of core.py:1382-1473.  The kernel packs the two
+  time-halves of the audio (n2 = ceil(n / 2) samples apart) into one complex
+  signal and produces only the 1024-sample output blocks the crop reads, from
+  max(0, start - n2) on: the automatic delay of a 48000-tap IR over 16000 samples
+  starts that range at block 15."""
   rng = np.random.default_rng(n + taps)
   audio = rng.standard_normal((B, n)).astype(np.float32)
   ir = (rng.standard_normal((ir_batch, taps)) * np.exp(-np.arange(taps) / (taps / 5.0))
@@ -187,26 +196,118 @@ def test_long_impulse_response_convolution_kernel(B, n, taps, ir_batch, padding,
   assert float((acc - (got + 0.25)).abs().max()) < 1e-5
 
 
+# (B, n, S, ir_batch, padding, a, b): padding 'same' / 'valid' runs core.fft_convolve
+# with delay_compensation a (b unused); padding None runs FftConvolveLtiFn on the
+# crop [a, a + b), which the public API cannot always ask for.
+LONG_CONV_BACKWARD_CASES = [
+    (3, 6000, 5000, 1, 'same', 0, None),      # shared trainable IR, B > 1
+    (3, 6000, 5000, 3, 'same', 0, None),
+    (2, 16000, 48000, 2, 'same', 0, None),    # Reverb's crop with S > n: d IR past end
+    (2, 1000, 3000, 1, 'same', 0, None),      # n < 1024, S > n, shared
+    (2, 2047, 3073, 2, 'valid', 0, None),     # odd n, full tail
+    (2, 1600, 4800, 1, 'same', -1, None),     # auto delay: start > n - 1 (d IR off < 0)
+    (2, 5001, 2048, 2, None, 2500, 1500),     # start > S - 1: d audio off < 0
+    (1, 1000, 2048, 1, None, 2500, 500),      # both offsets < 0, S > end
+    (2, 3001, 9000, 2, None, 100, 3000),      # end = 3100: d IR zero past it
+]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize('shared', [True, False])
-def test_long_convolution_backward_matches_autograd(shared):
+@pytest.mark.parametrize('B,n,S,ir_batch,padding,a,b', LONG_CONV_BACKWARD_CASES)
+def test_long_convolution_backward_matches_autograd(B, n, S, ir_batch, padding, a, b):
   """FftConvolveLtiFn (the trainable Reverb): d audio and d impulse response from
-  the same kernels on reversed operands, against float64 autograd of torch.fft."""
+  the same kernels on reversed operands, each with its own crop offset
+  (S - 1 - start, n - 1 - start) and a padded-gradient branch where that offset is
+  negative.  Checked (a) elementwise against float64 autograd of
+  grad_ref.convolve_lti, (b) exactly 0 for samples and taps at or past start +
+  out_len, which reach no output, and (c) by the linearity identity against the
+  oracle's full convolution for three random directions of each operand."""
   from ddsp_b200 import autograd as ag
-  torch.manual_seed(3)
-  B, n, taps, start = 3, 6000, 5000, 0
-  audio = torch.randn(B, n, device='cuda')
-  ir = torch.randn(1 if shared else B, taps, device='cuda') * 0.02
-  g = torch.randn(B, n, device='cuda')
+  from tests import grad_ref
+  from tests.util import linearity
+  if padding is None:
+    start, out_len = a, b
+  else:
+    start, out_len, crop = core._crop_range(core.get_fft_size(n, S), n, S, padding, a)
+    assert out_len == crop
+  gen = torch.Generator().manual_seed(n + S)
+  audio = torch.randn(B, n, generator=gen).cuda()
+  ir = (torch.randn(ir_batch, S, generator=gen) *
+        torch.exp(-torch.arange(S) / (S / 5.0))).cuda()
+  g = torch.randn(B, out_len, generator=gen).cuda()
   a1, h1 = audio.clone().requires_grad_(True), ir.clone().requires_grad_(True)
-  y = core.fft_convolve(a1, h1, padding='same', delay_compensation=start)
+  if padding is None:
+    y = ag.FftConvolveLtiFn.apply(a1, h1, start, out_len)
+  else:
+    y = core.fft_convolve(a1, h1, padding=padding, delay_compensation=a)
   (y * g).sum().backward()
   a2, h2 = audio.double().requires_grad_(True), ir.double().requires_grad_(True)
-  m = n + taps - 1
-  yr = torch.fft.irfft(torch.fft.rfft(a2, m) * torch.fft.rfft(h2.expand(B, taps), m), m)
-  yr = yr[:, start:start + n]
+  yr = grad_ref.convolve_lti(a2, h2, start, out_len)
   (yr * g.double()).sum().backward()
-  assert float((y.double() - yr).abs().max() / yr.abs().max()) < 1e-4
-  for got, want in ((a1.grad, a2.grad), (h1.grad, h2.grad)):
-    err = float((got.double() - want).abs().max() / want.abs().max())
-    assert err < 2e-4, err
+  assert tuple(y.shape) == tuple(yr.shape) == (B, out_len)
+  for name, got, want, tol_max, tol_l2 in (('y', y, yr, 1e-4, 1e-4),
+                                           ('d audio', a1.grad, a2.grad, 2e-4, 1e-4),
+                                           ('d ir', h1.grad, h2.grad, 2e-4, 1e-4)):
+    assert torch.isfinite(got).all(), name
+    emax, el2 = rel_err(got.detach().cpu().numpy(), want.detach().cpu().numpy())
+    assert emax < tol_max and el2 < tol_l2, (name, emax, el2)
+  end = start + out_len
+  assert not a1.grad[:, end:].any() and not h1.grad[:, end:].any()
+  a64, h64 = audio.double().cpu().numpy(), ir.double().cpu().numpy()
+
+  def full(x, h):
+    h = np.broadcast_to(h, (B, h.shape[-1]))
+    return o.fft_convolve(x, h, padding='valid', delay_compensation=0)
+
+  linearity(a1.grad, g, lambda d: full(d, h64)[:, start:end], (B, n), seed=n)
+  linearity(h1.grad, g, lambda d: full(a64, d)[:, start:end], (ir_batch, S), seed=S)
+
+
+@pytest.mark.gpu
+def test_trainable_reverb_with_impulse_response_longer_than_audio():
+  """Reverb(trainable=True) at the default 48000 taps on one second of audio, with
+  the dry tap masked and the IR tiled over the batch, through .backward():
+  d audio and d IR against float64 autograd."""
+  import ddsp_b200
+  from tests import grad_ref
+  B, n, S = 2, 16000, 48000
+  gen = torch.Generator().manual_seed(11)
+  audio = torch.randn(B, n, generator=gen).cuda()
+  ir = (torch.randn(S, generator=gen) * torch.exp(-torch.arange(S) / 8000.0)).cuda()
+  g = torch.randn(B, n, generator=gen).cuda()
+  rev = ddsp_b200.Reverb(trainable=True, reverb_length=S)
+  rev._ir = ir.clone().requires_grad_(True)
+  a1 = audio.clone().requires_grad_(True)
+  out = rev(a1)
+  (out * g).sum().backward()
+  a2, h2 = audio.double().requires_grad_(True), ir.double().requires_grad_(True)
+  masked = torch.cat([h2.new_zeros(1), h2[1:]])[None, :]
+  ref = grad_ref.convolve_lti(a2, masked, 0, n) + a2
+  (ref * g.double()).sum().backward()
+  for name, got, want, tol_max in (('out', out, ref, 1e-4), ('d audio', a1.grad, a2.grad, 2e-4),
+                                   ('d ir', rev._ir.grad, h2.grad, 2e-4)):
+    emax, el2 = rel_err(got.detach().cpu().numpy(), want.detach().cpu().numpy())
+    assert emax < tol_max and el2 < 1e-4, (name, emax, el2)
+  assert float(rev._ir.grad[0]) == 0.0 and not rev._ir.grad[n:].any()
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('B,n,S,ir_batch,start,out_len', [
+    (2, 3001, 2048, 2, 0, 3001), (1, 1000, 5000, 1, 700, 4000), (3, 4096, 3000, 1, 2500, 3000)])
+def test_long_convolution_reverse_flags(B, n, S, ir_batch, start, out_len):
+  """LTI_REVERSE_AUDIO / LTI_REVERSE_IR of `ddsp_b200_fft_convolve_lti` (the
+  backward's time-reversed operands) against the same call on flipped tensors."""
+  from tests import grad_ref
+  gen = torch.Generator().manual_seed(n)
+  audio = torch.randn(B, n, generator=gen).cuda()
+  ir = torch.randn(ir_batch, S, generator=gen).cuda()
+  for ra, ri in ((True, False), (False, True), (True, True)):
+    got = core.fft_convolve_lti(audio, ir, start, out_len, reverse_audio=ra, reverse_ir=ri)
+    x = audio.flip(-1).contiguous() if ra else audio
+    h = ir.flip(-1).contiguous() if ri else ir
+    want = core.fft_convolve_lti(x, h, start, out_len)
+    peak = float(want.abs().max())
+    assert float((got - want).abs().max()) <= 1e-6 * peak, (ra, ri)
+    ref = grad_ref.convolve_lti(x.double(), h.double(), start, out_len)
+    emax, el2 = rel_err(got.cpu().numpy(), ref.cpu().numpy())
+    assert emax < 1e-4 and el2 < 1e-4, (ra, ri, emax, el2)

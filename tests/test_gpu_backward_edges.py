@@ -16,7 +16,7 @@ from ddsp_b200 import autograd as ag
 from ddsp_b200 import core
 from oracle import ddsp_oracle as o
 from tests import grad_ref
-from tests.util import synth_inputs
+from tests.util import linearity, synth_inputs
 
 pytestmark = pytest.mark.gpu
 
@@ -35,21 +35,6 @@ def _check(name, got, want, tol_max, tol_l2):
   assert torch.isfinite(got).all(), name
   emax, l2 = _errs(got, want)
   assert emax < tol_max and l2 < tol_l2, (name, emax, l2)
-
-
-def _linearity(grad, g, oracle_fn, shape, n_dirs=3, seed=0):
-  """(b): <grad, D> against sum g * oracle_fn(D) in float64 for random D >= 0,
-  relative to sum |g * oracle_fn(D)| (the inner product without cancellation)."""
-  rng = np.random.default_rng(seed)
-  gnp = g.double().cpu().numpy()
-  grad = grad.double().cpu().numpy()
-  for _ in range(n_dirs):
-    d = rng.uniform(0.0, 1.0, shape)
-    y = oracle_fn(d)
-    want = float((gnp * y).sum())
-    scale = float(np.abs(gnp * y).sum())
-    got = float((grad * d).sum())
-    assert abs(got - want) <= 1e-4 * scale, (got, want, scale)
 
 
 # ---------------------------------------------------------------------------
@@ -90,7 +75,7 @@ def test_harmonic_backward_every_hop_and_f0_regime(B, F, K, hop, sr, method, reg
   ag.HarmonicSynthesisFn.apply(f0, torch.ones_like(amp), ha, N, sr, method).mul(g).sum() \
       .backward()
   f0np = f0.cpu().numpy()
-  _linearity(ha.grad, g, lambda d: o.harmonic_synthesis(
+  linearity(ha.grad, g, lambda d: o.harmonic_synthesis(
       f0np, np.ones((B, F, 1)), harmonic_distribution=d, n_samples=N, sample_rate=sr,
       amp_resample_method=method), (B, F, K), seed=K)
 
@@ -234,7 +219,7 @@ def test_noise_backward_every_window_and_frame(B, F, nb, ws, frame, ragged):
   _check('audio', out, ref, 1e-4, 1e-4)
   _check('d mags', m1.grad, m2.grad, 2e-4, 1e-4)
   nnp = noise.double().cpu().numpy()
-  _linearity(m1.grad, g, lambda d: o.frequency_filter(nnp, d, window_size=ws),
+  linearity(m1.grad, g, lambda d: o.frequency_filter(nnp, d, window_size=ws),
              (B, F, nb), seed=nb)
 
 
@@ -302,17 +287,20 @@ def _reverb_reference(audio64, mags64, noise64, ws, bias):
   return wet + audio64
 
 
-@pytest.mark.parametrize('size', ['reduced', 'default'])
+@pytest.mark.parametrize('size', ['reduced', 'default', 'long_ir'])
 @pytest.mark.parametrize('trainable', [False, True])
 def test_filtered_noise_reverb(size, trainable):
   """FilteredNoiseReverb forward (given and learned magnitudes) against the float64
   oracle composition, and backward to the learned [n_frames, n_filter_banks]
   magnitudes and to the audio against float64 autograd.  'default' is the class
   defaults: 48000 taps from 1000 frames of 16 bands (48-sample frames, window 257
-  clamped to the 30-tap impulse response) on 64000-sample audio."""
+  clamped to the 30-tap impulse response) on 64000-sample audio.  'long_ir' has an
+  impulse response longer than the audio (8000 taps on 3000 samples)."""
   from ddsp_b200 import effects
   if size == 'reduced':
     B, n, L, F, nb, ws = 2, 6000, 4000, 50, 16, 257
+  elif size == 'long_ir':
+    B, n, L, F, nb, ws = 2, 3000, 8000, 50, 16, 257
   else:
     B, n, L, F, nb, ws = 2, 64000, 48000, 1000, 16, 257
   bias = -3.0
@@ -357,3 +345,73 @@ def test_filtered_noise_reverb(size, trainable):
   _check('audio', out, ref, 1e-4, 1e-4)
   _check('d audio', a1.grad, a2.grad, 2e-4, 1e-4)
   _check('d magnitudes', rev._magnitudes.grad, m2.grad[0], 2e-4, 1e-4)
+
+
+# ---------------------------------------------------------------------------
+# Multi-scale spectral loss: SpectralLossFn (spectral_l1_kernel, the windowed
+# overlap-add adjoint) and FrameWindowFn
+# ---------------------------------------------------------------------------
+@pytest.mark.parametrize('B,N,fft_sizes,mag_weight,logmag_weight,upstream',
+                         grad_ref.SPECTRAL_CASES)
+def test_spectral_loss_against_float64(B, N, fft_sizes, mag_weight, logmag_weight,
+                                       upstream):
+  """losses.SpectralLoss on CUDA (one SpectralLossFn node) against float64 autograd
+  of grad_ref.spectral_loss: the loss value, and d audio with the upstream gradient
+  1, 0.37 (read on the device by the adjoint of every FFT size, which accumulate
+  into one buffer) or 1 plus another term of the audio.  The signals
+  (grad_ref.spectral_signals) have silent stretches of the value, where its
+  magnitudes are exactly 0, and stretches equal to the target.  d audio is compared
+  with the reference evaluated at the float32 spectra the kernel saw (see
+  grad_ref.spectral_loss)."""
+  from ddsp_b200 import losses
+  from ddsp_b200 import spectral_ops
+  target, value = (x.to(DEV) for x in grad_ref.spectral_signals(B, N, fft_sizes,
+                                                                  seed=N))
+  loss_obj = losses.SpectralLoss(fft_sizes=fft_sizes, mag_weight=mag_weight,
+                                 logmag_weight=logmag_weight)
+  a1 = value.clone().requires_grad_(True)
+  assert loss_obj._fusable(target, a1, None)
+  loss = loss_obj(target, a1)
+  want = grad_ref.spectral_loss(target, value, fft_sizes, mag_weight, logmag_weight)
+  assert torch.isfinite(loss) and float(want) > 0
+  assert abs(float(loss) - float(want)) <= 2e-5 * float(want), (float(loss), float(want))
+  with torch.no_grad():
+    spectra = [(spectral_ops.stft_cuda(target, s), spectral_ops.stft_cuda(value, s))
+               for s in fft_sizes]
+  a2 = value.double().requires_grad_(True)
+  (g_ref,) = torch.autograd.grad(grad_ref.spectral_loss(
+      target, a2, fft_sizes, mag_weight, logmag_weight, spectra=spectra), a2)
+  if upstream == 'scaled':
+    (0.37 * loss).backward()
+    g_ref = 0.37 * g_ref
+  elif upstream == 'sum':
+    # another term of the audio, of the loss gradient's size
+    w = float(g_ref.abs().max()) * torch.randn(
+        B, N, device=DEV, generator=torch.Generator(device=DEV).manual_seed(B))
+    (loss + (a1 * w).sum()).backward()
+    g_ref = g_ref + w.double()
+  else:
+    loss.backward()
+  _check('d audio', a1.grad, g_ref, 2e-4, 1e-4)
+
+
+@pytest.mark.parametrize('B,N,frame_size', [(2, 1000, 2048), (3, 12345, 256),
+                                            (1, 64000, 64), (2, 999, 16)])
+def test_frame_window_backward(B, N, frame_size):
+  """FrameWindowFn (stft_cuda's framing + Hann, pad_end=True) and its adjoint, the
+  windowed overlap-add, against float64 autograd of grad_ref.stft_frames: frames
+  longer than the audio, N not a multiple of the step, the zero-padded tail."""
+  from ddsp_b200 import spectral_ops
+  gen = torch.Generator(device=DEV).manual_seed(N)
+  audio = torch.randn(B, N, device=DEV, generator=gen)
+  step = frame_size // 4
+  a1 = audio.clone().requires_grad_(True)
+  frames = spectral_ops.FrameWindowFn.apply(a1, frame_size, step)
+  gf = torch.randn(frames.shape, device=DEV, generator=gen)
+  (frames * gf).sum().backward()
+  a2 = audio.double().requires_grad_(True)
+  ref = grad_ref.stft_frames(a2, frame_size)
+  (ref * gf.double()).sum().backward()
+  assert frames.shape == ref.shape
+  _check('frames', frames, ref, 1e-6, 1e-6)
+  _check('d audio', a1.grad, a2.grad, 1e-5, 1e-5)

@@ -1,7 +1,7 @@
 """The float64 references of the backward tests (tests/grad_ref.py) against the
-oracle, which is pinned to the reference itself: both must reproduce
-`oracle.harmonic_synthesis` / `oracle.frequency_filter` to 1e-12 of the peak on
-every shape the GPU tests use."""
+oracle, which is pinned to the reference itself: they must reproduce
+`oracle.harmonic_synthesis`, `oracle.frequency_filter`, `oracle.fft_convolve` and
+`oracle.spectral_loss` to 1e-12 of the peak on the shapes the GPU tests use."""
 import numpy as np
 import pytest
 import torch
@@ -57,6 +57,52 @@ def test_noise_reference_matches_oracle(B, F, nb, ws, frame, ragged):
   assert _rel(got.numpy(), want) <= 1e-12
 
 
+@pytest.mark.parametrize('B,n,S,ir_batch,padding,delay', [
+    (2, 4000, 3000, 2, 'same', 0),
+    (2, 4000, 3000, 1, 'same', -1),
+    (3, 1001, 2049, 1, 'same', 0),          # S > n, odd n
+    (2, 999, 5000, 2, 'valid', 0),          # S > n, odd n, full tail
+    (2, 1025, 3073, 2, 'same', 1500),       # positive delay past one 1024 block
+    (1, 2, 2048, 1, 'same', 0),
+    (1, 1, 2049, 1, 'valid', 0),
+    (2, 1600, 4800, 2, 'same', -1),         # automatic delay, S = 3 n
+])
+def test_convolve_lti_reference_matches_oracle(B, n, S, ir_batch, padding, delay):
+  from ddsp_b200 import core
+  rng = np.random.default_rng(n + S)
+  audio = rng.standard_normal((B, n))
+  ir = rng.standard_normal((ir_batch, S)) * np.exp(-np.arange(S) / (S / 5.0))
+  want = o.fft_convolve(audio, np.broadcast_to(ir, (B, S)), padding=padding,
+                        delay_compensation=delay)
+  start, out_len, crop = core._crop_range(core.get_fft_size(n, S), n, S, padding, delay)
+  assert out_len == crop
+  got = grad_ref.convolve_lti(torch.from_numpy(audio), torch.from_numpy(ir), start, out_len)
+  assert got.shape == want.shape == (B, crop)
+  assert _rel(got.numpy(), want) <= 1e-12
+
+
+@pytest.mark.parametrize('B,N,fft_sizes,mag_weight,logmag_weight',
+                         [c[:5] for c in grad_ref.SPECTRAL_CASES] +
+                         [(2, 3000, (64,), 0.5, 0.0)])
+def test_spectral_loss_reference_matches_oracle(B, N, fft_sizes, mag_weight,
+                                                logmag_weight):
+  """On the GPU tests' own signals: N shorter than the largest FFT, silent
+  stretches of the value (magnitudes exactly 0), stretches equal to the target."""
+  target, value = grad_ref.spectral_signals(B, N, fft_sizes, seed=N)
+  got = grad_ref.spectral_loss(target, value, fft_sizes, mag_weight, logmag_weight)
+  want = o.spectral_loss(target.numpy(), value.numpy(), fft_sizes=fft_sizes,
+                         mag_weight=mag_weight, logmag_weight=logmag_weight)
+  assert np.isfinite(want) and want > 0
+  assert abs(float(got) - want) <= 1e-12 * want
+  if N >= 2 * max(fft_sizes) + 896:
+    frames = grad_ref.stft_frames(value, max(fft_sizes))
+    assert (frames.abs().amax(-1) == 0).any()          # a silent frame of the value
+  np.testing.assert_allclose(
+      grad_ref.stft_frames(value, 256).numpy(),
+      o.frame_pad_end(value.numpy().astype(np.float64), 256, 64) * o.hann_window(256),
+      rtol=0, atol=1e-15)
+
+
 def test_references_are_differentiable_in_float64():
   f0 = grad_ref.low_f0_regime('jump', 1, 4, 16000, seed=1)
   amp = torch.rand(1, 4, 1, dtype=torch.float64, requires_grad=True)
@@ -67,3 +113,12 @@ def test_references_are_differentiable_in_float64():
   mags = torch.rand(1, 4, 9, dtype=torch.float64, requires_grad=True)
   grad_ref.frequency_filter(torch.rand(1, 200, dtype=torch.float64), mags, 7).sum().backward()
   assert mags.grad is not None and torch.isfinite(mags.grad).all()
+  audio = torch.rand(2, 300, dtype=torch.float64, requires_grad=True)
+  ir = torch.rand(1, 500, dtype=torch.float64, requires_grad=True)
+  grad_ref.convolve_lti(audio, ir, 7, 400).sum().backward()
+  assert all(t.grad is not None and torch.isfinite(t.grad).all() for t in (audio, ir))
+  target, value = grad_ref.spectral_signals(1, 3000, (256, 64), seed=2)
+  value = value.double().requires_grad_(True)
+  grad_ref.spectral_loss(target, value, (256, 64), 1.0, 1.0).backward()
+  assert value.grad.dtype == torch.float64 and torch.isfinite(value.grad).all()
+  assert float(value.grad.abs().max()) > 0

@@ -33,3 +33,21 @@ def rel_err(a, b):
   peak = max(np.abs(b).max(), 1e-30)
   l2 = np.sqrt(((a - b)**2).sum() / max((b**2).sum(), 1e-60))
   return np.abs(a - b).max() / peak, l2
+
+
+def linearity(grad, g, oracle_fn, shape, n_dirs=3, seed=0):
+  """For an output y linear in the differentiated input x, with upstream gradient
+  g and dL/dx = grad: <grad, D> against sum g * oracle_fn(D) in float64 for random
+  directions D >= 0, relative to sum |g * oracle_fn(D)| (the inner product without
+  cancellation).  oracle_fn(D) is the oracle's output for input D; no restatement
+  of the operation is involved."""
+  rng = np.random.default_rng(seed)
+  gnp = g.double().cpu().numpy()
+  grad = grad.double().cpu().numpy()
+  for _ in range(n_dirs):
+    d = rng.uniform(0.0, 1.0, shape)
+    y = oracle_fn(d)
+    want = float((gnp * y).sum())
+    scale = float(np.abs(gnp * y).sum())
+    got = float((grad * d).sum())
+    assert abs(got - want) <= 1e-4 * scale, (got, want, scale)
