@@ -1151,4 +1151,20 @@ int ddsp_b200_debug_noise_timing(unsigned* host_out) {
 }
 #endif
 
+#ifdef DDSP_HV4_TIMING
+// measurement builds only (tools/harm_timing.py): the harmonic_v4 phase counters
+// summed since the previous call, [kMaxSMs][8 phases + warps counted] cycles; the
+// counters are zeroed after the copy
+int ddsp_b200_debug_harm_timing(unsigned long long* host_out) {
+  const size_t bytes = sizeof(unsigned long long) * kMaxSMs * (ddsp::hv4::kTimingPhases + 1);
+  cudaError_t e = cudaMemcpyFromSymbol(host_out, ddsp::hv4::g_hv4_timing, bytes);
+  if (e != cudaSuccess) return DDSP_B200_E_CUDA;
+  void* dev = nullptr;
+  e = cudaGetSymbolAddress(&dev, ddsp::hv4::g_hv4_timing);
+  if (e == cudaSuccess) e = cudaMemset(dev, 0, bytes);
+  if (e == cudaSuccess) e = cudaDeviceSynchronize();
+  return e == cudaSuccess ? 0 : DDSP_B200_E_CUDA;
+}
+#endif
+
 }  // extern "C"

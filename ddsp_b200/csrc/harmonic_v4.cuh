@@ -24,6 +24,13 @@
 //     has live count kc, row x0 is zero above kc by construction and row x1 is
 //     zero above its own count; if that is <= kc the frame runs ceil(kc / 4)
 //     unmasked groups.  Only the other frames take a masked group.
+//
+// On sm_90a (each f32x2 operation is two scalar instructions) the group loops run
+// pairs of groups on one 32-bit shared address (2 loop instructions per group,
+// 9 before), the first group of a uniform frame writes the accumulators instead
+// of zeroing them, and a CTA is four warps over 32 frames: one record warp builds
+// the 32 frame records while the other three transform the 33 rows, so that one
+// prologue serves 32 frames and the two run side by side (DESIGN.md 3.1, 4).
 #pragma once
 #include "harmonic_common.cuh"
 
@@ -31,7 +38,7 @@ namespace ddsp {
 namespace hv4 {
 
 #ifndef DDSP_HV4_NW
-#define DDSP_HV4_NW 1
+#define DDSP_HV4_NW 4
 #endif
 constexpr int NW = DDSP_HV4_NW;  // warps per CTA
 constexpr int NT = NW * 32;
@@ -41,6 +48,37 @@ constexpr int NT = NW * 32;
 #endif
 #ifndef DDSP_HV4_MIN_CTAS
 #define DDSP_HV4_MIN_CTAS (24 / DDSP_HV4_NW)
+#endif
+
+// -DDDSP_HV4_TIMING: per-SM totals of each warp's clock() cycles by kernel phase,
+// summed over every CTA the SM ran (tools/harm_timing.py reads them back through
+// ddsp_b200_debug_harm_timing); measurement builds only.
+#ifdef DDSP_HV4_TIMING
+constexpr int kTimingPhases = 8;     // + 1 slot: warps counted
+__device__ unsigned long long g_hv4_timing[kMaxSMs * (kTimingPhases + 1)];
+#define HV4_TIMING_DECL                                                                 \
+  unsigned tacc__[kTimingPhases] = {0, 0, 0, 0, 0, 0, 0, 0};                            \
+  unsigned tprev__ = (unsigned)clock()
+#define HV4_LAP(i)                                                                      \
+  do {                                                                                  \
+    const unsigned n__ = (unsigned)clock();                                             \
+    tacc__[i] += n__ - tprev__;                                                         \
+    tprev__ = n__;                                                                      \
+  } while (0)
+#define HV4_TIMING_FLUSH()                                                              \
+  do {                                                                                  \
+    if (lane == 0) {                                                                    \
+      unsigned smid__;                                                                  \
+      asm volatile("mov.u32 %0, %%smid;" : "=r"(smid__));                               \
+      unsigned long long* t__ = g_hv4_timing + (smid__ % kMaxSMs) * (kTimingPhases + 1); \
+      for (int i__ = 0; i__ < kTimingPhases; ++i__) atomicAdd(t__ + i__, (unsigned long long)tacc__[i__]); \
+      atomicAdd(t__ + kTimingPhases, 1ull);                                             \
+    }                                                                                   \
+  } while (0)
+#else
+#define HV4_TIMING_DECL
+#define HV4_LAP(i)
+#define HV4_TIMING_FLUSH()
 #endif
 
 // 2^32 * (phase + 2^-9 turn): the table index is the top byte of the ROUNDED-UP
@@ -80,6 +118,16 @@ __host__ __device__ inline Smem smem_layout(int FW, int Kp, int hop) {
 }
 
 using hcm::phase32;
+
+// 16-byte shared-memory load at a 32-bit shared address: the group loops step one
+// such address (ptxas otherwise keeps a generic pointer and an index beside it)
+__device__ __forceinline__ float4 lds128(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "r"(a));
+  return v;
+}
 
 __device__ __forceinline__ float2 bffma2(float x, float2 v, float2 acc) {
   return ffma2(make_float2(x, x), v, acc);
@@ -128,6 +176,18 @@ __device__ __forceinline__ void controls_rows4(float* __restrict__ sXw,
   sum += __shfl_xor_sync(0xffffffffu, sum, 2);
   sum += __shfl_xor_sync(0xffffffffu, sum, 1);
   if (row_ok && l8 == 0) sInv[r] = __fdividef(1.0f, (sum == 0.0f) ? 1e-7f : sum);
+}
+
+// Frame-rate live count of a row (f0 * k < sr/2 in float32, core.py:888).
+__device__ __forceinline__ int row_live_count(float fq, int K, float nyquist, bool nyq) {
+  int live = K;
+  if (nyq && fq > 0.f) {
+    int k = (int)fminf(nyquist / fq, (float)K);
+    while (k < K && __fmul_rn(fq, (float)(k + 1)) < nyquist) ++k;
+    while (k > 0 && !(__fmul_rn(fq, (float)k) < nyquist)) --k;
+    live = k;
+  }
+  return live;
 }
 
 // The exact per-oscillator slow path (f0 < 1 Hz) behind one call.
@@ -287,7 +347,7 @@ __device__ __forceinline__ void frame_chunk(
     const float* __restrict__ sCos, int K, float nyquist, int lane,
     float* __restrict__ out, int accumulate) {
   const float* __restrict__ x0 = sX + xoff;
-  const float* __restrict__ x1 = x0 + Kp;
+  const uint32_t kp4 = (uint32_t)Kp << 2;               // bytes from row x0 to row x1
   const ulonglong2 PA = *reinterpret_cast<const ulonglong2*>(&rec->P);
   const uint4 Dk = *reinterpret_cast<const uint4*>(&rec->D);
   const float4 fa = *reinterpret_cast<const float4*>(&rec->f_lo);
@@ -320,25 +380,26 @@ __device__ __forceinline__ void frame_chunk(
     osc_seed2(st, qa, qb, sSin, sCos);
     if (ng > 0) {
       // every sample of the frame has the same live count: ng unmasked groups,
-      // then (rem != 0) one group masked with warp-uniform predicates.  (One
-      // loop from zeroed accumulators: peeling the first group to write the
-      // accumulators cost ptxas 28 MOVs per frame at the merge points.)
-      st.s0e = st.s0o = st.s1e = st.s1o = make_float2(0.f, 0.f);
-      st.t0e = st.t0o = st.t1e = st.t1o = make_float2(0.f, 0.f);
-      const int k_main = ng << 2;                   // ng >= 1
-      int k = 0;
-#pragma unroll 1
-      do {
-        const float4 X0 = *reinterpret_cast<const float4*>(x0 + k);
-        const float4 X1 = *reinterpret_cast<const float4*>(x1 + k);
-        osc_group(st, X0, X1);
-        k += 4;
-      } while (k < k_main);
-      if (rem != 0) {
-        const float4 X0 = mask4u(*reinterpret_cast<const float4*>(x0 + k), rem);
-        const float4 X1 = mask4u(*reinterpret_cast<const float4*>(x1 + k), rem);
-        osc_group(st, X0, X1);
+      // then (rem != 0) one group masked with warp-uniform predicates.  The
+      // first group writes the accumulators (no zeroing); an even count runs
+      // its second group alone; the loop runs pairs of groups on one 32-bit
+      // shared address into row x0 (row x1 is that address plus 4 Kp).  The
+      // harmonics stay in order, so the sums are those of one group at a time.
+      uint32_t a = smem_u32(x0);
+      const uint32_t a_end = a + (ng << 4);         // ng >= 1
+      osc_group_first(st, lds128(a), lds128(a + kp4));
+      a += 16;
+      if ((ng & 1) == 0) {
+        osc_group(st, lds128(a), lds128(a + kp4));
+        a += 16;
       }
+#pragma unroll 1
+      while (a != a_end) {
+        osc_group(st, lds128(a), lds128(a + kp4));
+        osc_group(st, lds128(a + 16), lds128(a + kp4 + 16));
+        a += 32;
+      }
+      if (rem != 0) osc_group(st, mask4u(lds128(a), rem), mask4u(lds128(a + kp4), rem));
     } else {                 // live count changes inside this frame (or is < 4)
       int ra = r0 + lane;
       asm volatile("" : "+r"(ra));
@@ -349,18 +410,21 @@ __device__ __forceinline__ void frame_chunk(
       const int kmax = __reduce_max_sync(0xffffffffu, max(ka, kb));
       st.s0e = st.s0o = st.s1e = st.s1o = make_float2(0.f, 0.f);
       st.t0e = st.t0o = st.t1e = st.t1o = make_float2(0.f, 0.f);
-      const int k_main = kmin & ~3;
-      int k = 0;
-      for (; k < k_main; k += 4) {
-        const float4 X0 = *reinterpret_cast<const float4*>(x0 + k);
-        const float4 X1 = *reinterpret_cast<const float4*>(x1 + k);
-        osc_group(st, X0, X1);
+      // the groups every sample keeps whole, addressed as in the uniform loop
+      uint32_t a = smem_u32(x0);
+      const uint32_t a_main = a + ((kmin & ~3) << 2);
+      if (kmin & 4) {
+        osc_group(st, lds128(a), lds128(a + kp4));
+        a += 16;
       }
-      for (; k < kmax; k += 4) {
-        const float4 X0 = *reinterpret_cast<const float4*>(x0 + k);
-        const float4 X1 = *reinterpret_cast<const float4*>(x1 + k);
-        osc_group_masked(st, X0, X1, k, ka, kb);
+#pragma unroll 1
+      while (a != a_main) {
+        osc_group(st, lds128(a), lds128(a + kp4));
+        osc_group(st, lds128(a + 16), lds128(a + kp4 + 16));
+        a += 32;
       }
+      for (int k = kmin & ~3; k < kmax; k += 4, a += 16)
+        osc_group_masked(st, lds128(a), lds128(a + kp4), k, ka, kb);
     }
     const float2 t0 = ffma2(st.sg, fadd2(st.s0o, st.t0o), fadd2(st.s0e, st.t0e));
     const float2 t1 = ffma2(st.sg, fadd2(st.s1o, st.t1o), fadd2(st.s1e, st.t1e));
@@ -404,6 +468,7 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
   // Programmatic dependent launch: the noise kernel of the decoder may start
   // its prologue on SMs this grid has vacated.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  HV4_TIMING_DECL;
   // ---- 0. the frame slab: one TMA bulk copy, issued before anything else ----
   if (use_tma && tid == 0) {
     mbar_init(mbar, 1);
@@ -426,6 +491,17 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
   const int fr = warp * 32 + lane;                      // tile frame of a record lane
   const int cnt = max(0, min(32, nfr - warp * 32));     // frames of this record warp
   const bool raw_scale = p.ctl_flags & DDSP_B200_CTL_SCALE;
+  //         CONTROLS WARPS: get_controls rows are split over the warps that build
+  //         no records (over all warps when every warp builds records), so that
+  //         the transform runs while the records are built.
+  const int n_ctl = (NW > n_rec) ? NW - n_rec : NW;
+  const int cw = (NW > n_rec) ? warp - n_rec : warp;  // < 0: no rows
+  const int rw = (nfr + n_ctl - 1) / n_ctl;
+  const int c0 = cw * rw;                               // first row of the warp
+  const int ncr = (cw < 0) ? 0 : max(0, min(rw, nfr - c0));
+  const bool c_last = ncr > 0 && c0 + ncr == nfr;
+  const int nrows = ncr + ((c_last && rows_in > nfr) ? 1 : 0);   // + the real row after the tile
+  const float f_row = (lane < nrows) ? f0b[min(i0 + c0 + lane, F - 1)] : 0.f;
   float f = 0.f, a = 0.f, f_tile = 0.f, f_first = 0.f;
   float f_x = 0.f, a_x = 0.f;      // lane 31 of a full record warp: the frame after its range
   if (rec_warp && cnt > 0) {
@@ -499,6 +575,9 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
         sX[idx] = (idx % Kp == 0) ? 1.0f : 0.f;
     }
   }
+  HV4_LAP(0);
+  __syncthreads();            // tables, mbarrier init, partial sums, (LDG slab)
+  HV4_LAP(1);
 
   // ---- 2. frame records (record warps, lane = frame) ----
   const bool have_ctl = (p.ctl_flags != 0) && (p.hd != nullptr);
@@ -531,20 +610,10 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
     }
     excl = incl - tot;
     if (lane == 31) sWarpTot[warp] = incl;             // total of the record warp's frames
-    // frame-rate live count of a row (f0 * k < sr/2 in float32, core.py:888)
-    auto row_live = [&](float fq) {
-      int live = K;
-      if ((p.ctl_flags & DDSP_B200_CTL_NYQUIST) && fq > 0.f) {
-        int k = (int)fminf(p.nyquist / fq, (float)K);
-        while (k < K && __fmul_rn(fq, (float)(k + 1)) < p.nyquist) ++k;
-        while (k > 0 && !(__fmul_rn(fq, (float)k) < p.nyquist)) --k;
-        live = k;
-      }
-      return live;
-    };
-    const int live = row_live(f);
+    const bool nyq = p.ctl_flags & DDSP_B200_CTL_NYQUIST;
+    const int live = row_live_count(f, K, p.nyquist, nyq);
     int live_next = __shfl_down_sync(0xffffffffu, live, 1);
-    if (lane == 31 && cnt == 32) live_next = row_live(f_n);
+    if (lane == 31 && cnt == 32) live_next = row_live_count(f_n, K, p.nyquist, nyq);
     int ng = -1, rem = 0;                              // exact slow path
     if (lane < cnt && f >= 1.0f && f_n >= 1.0f) {
       const int kca = live_harmonics(f, f_n, 0.0f, K, p.nyquist);
@@ -572,14 +641,13 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
       r.f_lo = f; r.f_hi = f_n; r.amp0 = a; r.amp1 = a_n;
       sRec[fr] = r;
     }
-    if (lane <= cnt) sLive[fr] = live;
-    if (lane == 31 && cnt == 32) sLive[fr + 1] = live_next;
-  }
-  __syncthreads();            // tables, mbarrier init, partial sums, records, (LDG slab)
+    // the record warps' totals (sWarpTot) are shared among the record warps only
+    const int n_act = (nfr + 31) >> 5;
+    if (n_act > 1) asm volatile("bar.sync 1, %0;" ::"r"(32 * n_act) : "memory");
+    HV4_LAP(2);
 
-  // phase at the start of the tile (telescoped closed form, one double-precision
-  // evaluation: <= 2^15 turns, 2^-38 turn resolution), then the record warp's offset
-  if (rec_warp && cnt > 0) {
+    // phase at the start of the tile (telescoped closed form, one double-precision
+    // evaluation: <= 2^15 turns, 2^-38 turn resolution), then the record warp's offset
     double base_sum = 0.0;
 #pragma unroll
     for (int w = 0; w < NW; ++w) base_sum += sRedD[w];
@@ -600,38 +668,45 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
 #endif
     }
   }
-  if (use_tma) mbar_wait(mbar, 0);
+  HV4_LAP(3);
 
-  // ---- 3. get_controls on the warp's own rows (synths.py:110-117) ----
-  const int w0f = warp * FW;
-  const int nfw = max(0, min(FW, nfr - w0f));
-  if (nfw > 0) {
-    float* sXw = sX + (size_t)w0f * Kp;
-    const bool last = (w0f + nfw == nfr);
-    int nrows = nfw;
-    if (last && rows_in > nfr) nrows = nfw + 1;         // the real row after the tile
+  // ---- 3. get_controls on the controls warp's rows (synths.py:110-117) ----
+  if (ncr > 0) {
+    float* sXw = sX + (size_t)c0 * Kp;
+    if (have_ctl) {
+      const bool nyq = p.ctl_flags & DDSP_B200_CTL_NYQUIST;
+      for (int r = lane; r < nrows; r += 32)
+        sLive[c0 + r] = row_live_count(r == lane ? f_row : f0b[min(i0 + c0 + r, F - 1)], K,
+                                       p.nyquist, nyq);
+      __syncwarp();
+    }
+    if (use_tma) mbar_wait(mbar, 0);
+    HV4_LAP(4);
     if (have_ctl) {
       if (Kp <= 128) {
         for (int r0 = 0; r0 < nrows; r0 += 4)
-          controls_rows4(sXw, sLive + w0f, sInv + w0f, r0, nrows, Kp, raw_scale, lane);
+          controls_rows4(sXw, sLive + c0, sInv + c0, r0, nrows, Kp, raw_scale, lane);
       } else {
         for (int r0 = 0; r0 < nrows; r0 += 4)
-          hcm::controls_rows(sXw, sLive + w0f, r0, nrows, Kp, raw_scale, lane);
-        for (int r = lane; r < nrows; r += 32) sInv[w0f + r] = 1.0f;
+          hcm::controls_rows(sXw, sLive + c0, r0, nrows, Kp, raw_scale, lane);
+        for (int r = lane; r < nrows; r += 32) sInv[c0 + r] = 1.0f;
       }
     } else {
-      for (int r = lane; r < nrows; r += 32) sInv[w0f + r] = 1.0f;
+      for (int r = lane; r < nrows; r += 32) sInv[c0 + r] = 1.0f;
     }
-    if (last && rows_in < nfr + 1) {                    // frame F := frame F-1
+    if (c_last && rows_in < nfr + 1) {                  // frame F := frame F-1
       __syncwarp();
-      for (int c = lane; c < Kp; c += 32) sXw[nfw * Kp + c] = sXw[(nfw - 1) * Kp + c];
-      if (lane == 0) sInv[w0f + nfw] = sInv[w0f + nfw - 1];
+      for (int c = lane; c < Kp; c += 32) sXw[ncr * Kp + c] = sXw[(ncr - 1) * Kp + c];
+      if (lane == 0) sInv[c0 + ncr] = sInv[c0 + ncr - 1];
     }
   }
-  __syncthreads();   // the row after a warp's block (and its 1 / sum) is its neighbour's;
-                     // the records' phases
+  HV4_LAP(5);
+  __syncthreads();   // the records, the transformed rows and their 1 / sum
+  HV4_LAP(6);
 
-  // ---- 4. samples ----
+  // ---- 4. samples: the warp's own FW frames ----
+  const int w0f = warp * FW;
+  const int nfw = max(0, min(FW, nfr - w0f));
   if (nfw > 0) {
     FrameRec* rec = sRec + w0f;
     if (lane < nfw) {                                   // amp / row sum
@@ -658,6 +733,8 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
       }
     }
   }
+  HV4_LAP(7);
+  HV4_TIMING_FLUSH();
 }
 
 template <bool WINDOW, int HOPT>
@@ -681,9 +758,10 @@ inline int launch_harmonic_v4(HarmonicParams p, cudaStream_t st) {
   using namespace hv4;
   p.Kp = (p.K + 3) & ~3;
   static const int env_fw = [] { const char* e = getenv("DDSP_B200_HARM_FW"); return e ? atoi(e) : 0; }();
-  // One warp per CTA and 11 frames per warp (12 rows = three get_controls passes);
-  // DDSP_B200_HARM_FW overrides the frames per warp for A/B timing.  Small grids
-  // shrink the tile until every SM has one.
+  // Four warps per CTA and 8 frames per warp: one full record warp for the 32-frame
+  // tile while the other three transform its 33 rows (11 frames per warp with one
+  // warp per CTA); DDSP_B200_HARM_FW overrides the frames per warp for A/B timing.
+  // Small grids shrink the tile until every SM has one.
   int FW = (NW == 1) ? 11 : 8;
   const long long want_ctas = 8ll * num_sms() * (4 / NW);        // 32 warps per SM
   while (FW > 4 && (long long)p.B * ((p.F + FW * NW - 1) / (FW * NW)) < want_ctas) FW = (FW + 1) >> 1;
