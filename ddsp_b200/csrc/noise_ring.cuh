@@ -26,19 +26,20 @@
 //   * TRIANGULAR TRIMMING at compile time: the rows of frames q+1 and q-1 cover
 //     complementary triangles of the (n, i) square; fully unrolled bodies skip the
 //     (n, i) pairs whose taps are out of range.
-//   * producers: three groups of 4 warps take turns on tiles; a group takes its tile
-//     from raw magnitudes (TMA) through exp_sigmoid, the cosine sums (odd k, and the
-//     even k split once more by quarter-wave symmetry: 1601 MACs per frame instead
-//     of 4225; in registers as f32x2, no exchange) and the windowed taps to the
-//     Philox rows, and asks for its ring slot only when the sums are done.
+//   * producers: groups of 4 warps take turns on tiles; a group takes its tile from
+//     raw magnitudes (TMA) through exp_sigmoid, the cosine sums and the windowed taps
+//     to the Philox rows, and asks for its ring slot only when the sums are done.
+//     The cosine sums are a matrix product with a constant operand, [32 frames x 65
+//     magnitudes] x [65 x 65 cosines], split into its even-k and odd-k halves
+//     (h0[n] = E[n] + O[n], h0[64 - n] = E[n] - O[n]) and run on the FP64 tensor
+//     cores (mma.m16n8k4.f64, 154 per tile); each tap is rounded to float once.
 #pragma once
 #include "noise_fused.cuh"
 
 namespace ddsp {
 
 namespace nr_ {
-constexpr int NB = 65, FRAME = 64, S = 128, S0 = 128, Q = 32, QP = 36;
-constexpr int NE = 33, NO = 32, SHIFT = 64;
+constexpr int NB = 65, FRAME = 64, S = 128, S0 = 128, Q = 32, SHIFT = 64;
 // A consumer warp owns a UNIT of R outputs of 32 frames: R accumulators and the R
 // inputs of a body in registers.  R = 16 (four units per frame, 9 KB of FIR bodies)
 // is the product; R = 32 (two units, half the shared-memory loads per FMA, 35 KB
@@ -50,28 +51,49 @@ constexpr int NE = 33, NO = 32, SHIFT = 64;
 constexpr int R = DDSP_NR_UNIT;
 static_assert(R == 16 || R == 32, "noise_ring unit: 16 or 32 outputs");
 constexpr int UPT = FRAME / R;                     // units per 64-sample frame
-// Producer groups and ring slots.  The consumer tile groups hold NTG + 1 slots
-// between them; what is left decouples producers from consumers.  227 KB of
-// shared memory hold 7 slots next to three raw-magnitude staging buffers or 8 next
-// to two; the default is 3 groups / 7 slots (with two groups the consumers wait on
-// the producers' cosine sums).
+// Consumer warps, producer groups and ring slots.  The consumer tile groups hold
+// NTG + 1 slots between them; what is left decouples producers from consumers.
+// 227 KB of shared memory hold 7 slots next to the cosine table and up to three
+// raw-magnitude staging buffers.  The consumer warp count (8 or 16) and the group
+// count (1 .. 3) are build knobs for A/B timing (DESIGN.md 3.2).
+#ifndef DDSP_NR_CONS_WARPS
+#define DDSP_NR_CONS_WARPS 8
+#endif
 #ifndef DDSP_NR_PROD_GROUPS
 #define DDSP_NR_PROD_GROUPS 3
 #endif
 #ifndef DDSP_NR_MAX_SLOTS
 #define DDSP_NR_MAX_SLOTS 7
 #endif
-constexpr int CONS_WARPS = 8, PROD_GROUPS = DDSP_NR_PROD_GROUPS, PROD_WARPS = 4 * PROD_GROUPS;
+constexpr int CONS_WARPS = DDSP_NR_CONS_WARPS, PROD_GROUPS = DDSP_NR_PROD_GROUPS;
+constexpr int GROUP_WARPS = 4, PROD_WARPS = GROUP_WARPS * PROD_GROUPS;
+static_assert(CONS_WARPS == 8 || CONS_WARPS == 16, "noise_ring consumers: 8 or 16 warps");
+static_assert(PROD_GROUPS >= 1 && PROD_GROUPS <= 3, "noise_ring producers: 1 .. 3 groups");
 constexpr int NTG = CONS_WARPS / UPT;              // consumption tiles in flight
 static_assert((NTG & (NTG - 1)) == 0, "tile groups: a power of two");
 constexpr int SLOTS = DDSP_NR_MAX_SLOTS;
 static_assert(SLOTS > NTG + 1, "the ring must leave slots to the producers");
 constexpr int RING = 32 * SLOTS;
 // Every warp runs under the launch budget (65536 / THREADS registers: 96 for 640
-// threads); the scalar FIR needs no more, so there is no register split.
+// threads); the scalar FIR needs no more, so there is no register split, and a
+// shape with more warps than that would starve the consumers of registers.
 constexpr int THREADS = 32 * (CONS_WARPS + PROD_WARPS);
+static_assert(THREADS <= 640, "noise_ring: the FIR needs 96 registers per thread");
 constexpr int HPAD = 2, HS = 134, XS = 66, MS = 65;   // row strides (floats)
 constexpr int NQ = FRAME / 4;
+
+// IR synthesis on the FP64 tensor cores: per tile, H[f][n] = sum_k M[f][k] C[k][n]
+// as mma.m16n8k4 (A = 16 frames x 4 k, B = 4 k x 8 n), once over the even k (E)
+// and once over the odd k (O), for n = 0 .. 31 (four n-tiles) plus E at n = 32
+// (a fifth n-tile, one live column: O[32] = 0).  Within k-step s, lane (g, t) =
+// (lane / 4, lane % 4) takes index kk = 16 (s / 4) + 4 t + s % 4 of its half (k = 2 kk
+// or 2 kk + 1): frames g and g + 8 then read the magnitude rows (stride 65 floats)
+// on 32 distinct banks.  The table C[k][n] c_k / S0 (c_k = 1 at k = 0, 64, else 2)
+// is stored as B fragments, one double per lane, in that k order.
+constexpr int E_STEPS = 9, O_STEPS = 8;            // 33 even k (padded to 36), 32 odd k
+constexpr int E_NT = 5, O_NT = 4;                  // n-tiles of 8 columns
+constexpr int TAB_E = E_STEPS * E_NT * 32, TAB = TAB_E + O_STEPS * O_NT * 32;   // doubles
+__host__ __device__ constexpr int ir_kk(int s, int t) { return 16 * (s >> 2) + 4 * t + (s & 3); }
 
 // -DDDSP_NR_TIMING: per-warp cycle counters by phase (tools/noise_timing.py reads
 // them back through ddsp_b200_debug_noise_timing); measurement builds only.
@@ -90,8 +112,7 @@ __device__ unsigned g_nr_timing[kMaxSMs * 32 * 8];
 #endif
 
 struct Smem {
-  float te[NE * QP];
-  float to[NO * QP];
+  double ctab[TAB];
   float win[S];
   alignas(16) float raw[PROD_GROUPS][32 * NB + 8];
   alignas(16) float h[RING * HS];
@@ -143,6 +164,16 @@ __device__ __forceinline__ float lds32v(const float* p) {
   float v;
   asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(smem_u32(p)));
   return v;
+}
+
+// d += a b on the FP64 tensor cores: A 16 x 4 (a0: row lane / 4, a1: row lane / 4 + 8,
+// column lane % 4), B 4 x 8 (row lane % 4, column lane / 4), D 16 x 8 (d[0..1]: row
+// lane / 4, d[2..3]: row lane / 4 + 8, columns 2 (lane % 4) + {0, 1}).
+__device__ __forceinline__ void dmma_16x8x4(double (&d)[4], double a0, double a1, double b) {
+  asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0, %1, %2, %3}, {%4, %5}, {%6}, "
+      "{%0, %1, %2, %3};"
+      : "+d"(d[0]), "+d"(d[1]), "+d"(d[2]), "+d"(d[3])
+      : "d"(a0), "d"(a1), "d"(b));
 }
 
 __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c,
@@ -256,28 +287,20 @@ __global__ void __launch_bounds__(nr_::THREADS, 1)
 noise_ring_kernel(Params p) {
   Smem& sm = *reinterpret_cast<Smem*>(nr_smem);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const float invS0 = 1.0f / (float)S0;
 
   // ---- once: tables, window, zeroed ring (pads stay zero), barriers ----
-  for (int e = tid; e < NE * QP; e += THREADS) {
-    const int k = e / QP, n = e - k * QP;
-    const int ph = (2 * k * n) % S0;
-    const float ck = (k == 0 || 2 * k == NB - 1) ? invS0 : 2.0f * invS0;
-    sm.te[e] = (n <= Q) ? ck * cospif(2.0f * (float)ph * invS0) : 0.f;
-  }
-  for (int e = tid; e < NO * QP; e += THREADS) {
-    // odd-k table, laid out by producer warp: columns 8 w + c hold n = 4 w + c
-    // (c < 4) and its mirror n = 32 - 4 w - (c - 4) (c >= 4); column 32 holds n = 16
-    const int k = e / QP, col = e - k * QP;
-    int n = -1;
-    if (col < 32) {
-      const int w = col >> 3, c = col & 7;
-      n = (c < 4) ? 4 * w + c : 32 - 4 * w - (c - 4);
-    } else if (col == 32) {
-      n = 16;
+  for (int e = tid; e < TAB; e += THREADS) {
+    // B fragment (half, k-step s, n-tile nt), lane l: C[k][8 nt + l / 4] c_k / S0
+    const bool even = e < TAB_E;
+    const int ee = even ? e : e - TAB_E, nts = even ? E_NT : O_NT;
+    const int l = ee & 31, s = (ee >> 5) / nts, nt = (ee >> 5) - s * nts;
+    const int kk = ir_kk(s, l & 3), k = even ? 2 * kk : 2 * kk + 1, n = 8 * nt + (l >> 2);
+    double v = 0.0;
+    if (k < NB && n <= Q) {
+      const double ck = (k == 0 || k == NB - 1) ? 1.0 : 2.0;
+      v = ck / S0 * cospi(2.0 * (double)((k * n) % S0) / S0);
     }
-    const int ph = ((2 * k + 1) * max(n, 0)) % S0;
-    sm.to[e] = (n >= 0) ? 2.0f * invS0 * cospif(2.0f * (float)ph * invS0) : 0.f;
+    sm.ctab[e] = v;
   }
   for (int j = tid; j < S; j += THREADS)
     sm.win[j] = 0.5f - 0.5f * cospif(2.0f * (float)j / (float)S0);   // core.py:1498,1515
@@ -288,7 +311,7 @@ noise_ring_kernel(Params p) {
 #endif
   if (tid == 0) {
     for (int i = 0; i < SLOTS; ++i) {
-      mbar_init(&sm.full[i], 4);
+      mbar_init(&sm.full[i], GROUP_WARPS);          // one arrive per producer warp
       mbar_init(&sm.empty[i], 2 * UPT);
     }
     for (int i = 0; i < PROD_GROUPS; ++i) mbar_init(&sm.rawbar[i], 1);
@@ -393,10 +416,10 @@ noise_ring_kernel(Params p) {
     // both cosine half-sums -> windowed taps, then the tile's noise rows.  A group
     // has PROD_GROUPS tile periods for one tile, so its latency chains (TMA, MUFU,
     // LDS) stay off the consumers' critical path.
-    const int grp = (warp - CONS_WARPS) >> 2;
-    const int iw = (warp - CONS_WARPS) & 3;           // column block / slice
-    const int ptid = tid - (CONS_WARPS + 4 * grp) * 32;   // 0..127 within the group
-    constexpr int PT = 128;
+    const int grp = (warp - CONS_WARPS) / GROUP_WARPS;
+    const int iw = (warp - CONS_WARPS) % GROUP_WARPS;   // column block / slice
+    const int ptid = tid - (CONS_WARPS + GROUP_WARPS * grp) * 32;   // 0..127 within the group
+    constexpr int PT = 32 * GROUP_WARPS;
     const int bar_id = 1 + grp;
     float* s_raw = sm.raw[grp];
     void* rawbar = &sm.rawbar[grp];
@@ -470,7 +493,6 @@ noise_ring_kernel(Params p) {
       mbar_wait(rawbar, n_mine & 1);
       NR_LAP(0);
       const bool row_ok = (jb + lane >= 0) && (jb + lane < p.F);
-      const float* mrow = row_ok ? s_raw + roff + lane * NB : s_raw;
       if (p.raw && row_ok) {
         float* src = s_raw + roff + lane * NB + iw * 17;
         float v[17];
@@ -492,66 +514,41 @@ noise_ring_kernel(Params p) {
       const bool interior = (jb >= 0) && (jb + 32 <= p.F) &&
                             (p_lo + 32ll * FRAME <= p.N) && !nzb;
       constexpr int PER = 32 * NQ / 4;                 // 128 quads per warp
-      // B. the cosine sums, with the quarter-wave symmetry of the even-k half:
-      //    h0[n] = E[n] + O[n], h0[64 - n] = E[n] - O[n] (SURVEY A.5), and, splitting
-      //    the even k = 2 j by the parity of j, E[n] = EE[n] + EO[n], E[32 - n] =
-      //    EE[n] - EO[n]: 289 + 256 + 1056 MACs per frame instead of 1089 + 1024.
-      //    Warp w owns n = 4 w .. 4 w + 3 and their mirrors 32 - n (warp 3 also the
-      //    self-mirrored n = 16, where EO vanishes).
+      // B. the cosine sums as FP64 tensor-core products (see ir_kk): warp iw takes the
+      //    frames of m-tile iw / 2 and the n-tiles 2 (iw % 2), 2 (iw % 2) + 1 of both
+      //    halves; warps 1 and 3 also the n = 32 column of E.  Magnitude rows of
+      //    frames outside [0, F) are read from the buffer's start and their taps
+      //    forced to zero below; k past 64 (the even half's padding) reads zero.
       {
-        const int c0 = 4 * iw;
-        float2 aEE[2], aEO[2], aOa[2], aOb[2];
-        float ee16 = 0.f, o16 = 0.f;
+        const int g = lane >> 2, t = lane & 3;
+        const int ntb = 2 * (iw & 1);
+        const bool mid = iw & 1;
+        const int f0 = 16 * (iw >> 1) + g, f1 = f0 + 8;
+        const bool ok0 = (jb + f0 >= 0) && (jb + f0 < p.F);
+        const bool ok1 = (jb + f1 >= 0) && (jb + f1 < p.F);
+        const float* m0 = ok0 ? s_raw + roff + f0 * NB : s_raw;
+        const float* m1 = ok1 ? s_raw + roff + f1 * NB : s_raw;
+        const double* tb = sm.ctab + lane;
+        double aE[3][4], aO[2][4];
 #pragma unroll
-        for (int c = 0; c < 2; ++c) aEE[c] = aEO[c] = aOa[c] = aOb[c] = make_float2(0.f, 0.f);
-        // Software-pipelined over groups of four k (two register sets: the loads of
-        // group j2 + 1 are in flight while group j2 is multiplied); volatile loads so
-        // that their order and their distinct destinations stay.
-        struct Term { float m0, m1, m2, m3; float4 e0, e1, oa0, ob0, oa1, ob1; };
-        auto load_term = [&](Term& t, int j2) {
-          const float* pm = mrow + 4 * j2;               // k = 4 j2 .. 4 j2 + 3
-          const float* pe = sm.te + (2 * j2) * QP + c0;
-          const float* po = sm.to + (2 * j2) * QP + 8 * iw;
-          t.m0 = lds32v(pm); t.m1 = lds32v(pm + 1);
-          t.m2 = lds32v(pm + 2); t.m3 = lds32v(pm + 3);
-          t.e0 = lds128v(pe); t.e1 = lds128v(pe + QP);
-          t.oa0 = lds128v(po); t.ob0 = lds128v(po + 4);
-          t.oa1 = lds128v(po + QP); t.ob1 = lds128v(po + QP + 4);
-        };
-        auto mac_term = [&](const Term& t, int j2) {
-          aEE[0] = nf_ffma2(t.m0, make_float2(t.e0.x, t.e0.y), aEE[0]);
-          aEE[1] = nf_ffma2(t.m0, make_float2(t.e0.z, t.e0.w), aEE[1]);
-          aOa[0] = nf_ffma2(t.m1, make_float2(t.oa0.x, t.oa0.y), aOa[0]);
-          aOa[1] = nf_ffma2(t.m1, make_float2(t.oa0.z, t.oa0.w), aOa[1]);
-          aOb[0] = nf_ffma2(t.m1, make_float2(t.ob0.x, t.ob0.y), aOb[0]);
-          aOb[1] = nf_ffma2(t.m1, make_float2(t.ob0.z, t.ob0.w), aOb[1]);
-          aEO[0] = nf_ffma2(t.m2, make_float2(t.e1.x, t.e1.y), aEO[0]);
-          aEO[1] = nf_ffma2(t.m2, make_float2(t.e1.z, t.e1.w), aEO[1]);
-          aOa[0] = nf_ffma2(t.m3, make_float2(t.oa1.x, t.oa1.y), aOa[0]);
-          aOa[1] = nf_ffma2(t.m3, make_float2(t.oa1.z, t.oa1.w), aOa[1]);
-          aOb[0] = nf_ffma2(t.m3, make_float2(t.ob1.x, t.ob1.y), aOb[0]);
-          aOb[1] = nf_ffma2(t.m3, make_float2(t.ob1.z, t.ob1.w), aOb[1]);
-          if (iw == 3) {
-            ee16 = fmaf(t.m0, sm.te[(2 * j2) * QP + 16], ee16);
-            o16 = fmaf(t.m1, sm.to[(2 * j2) * QP + 32], o16);
-            o16 = fmaf(t.m3, sm.to[(2 * j2 + 1) * QP + 32], o16);
-          }
-        };
-        Term tA, tB;
-        load_term(tA, 0);
-#pragma unroll 1
-        for (int j2 = 0; j2 < NO / 2; j2 += 2) {
-          load_term(tB, j2 + 1);
-          mac_term(tA, j2);
-          // j2 + 2 = 16 is k = 64, the last even-even term: the rest of that group is
-          // read (table rows past the end run into the next array, mrow[65 .. 67] into
-          // the next row / the pad) and never used
-          load_term(tA, j2 + 2);
-          mac_term(tB, j2 + 1);
+        for (int c = 0; c < 4; ++c) {
+          aE[0][c] = aE[1][c] = aE[2][c] = 0.0;
+          aO[0][c] = aO[1][c] = 0.0;
         }
-        aEE[0] = nf_ffma2(tA.m0, make_float2(tA.e0.x, tA.e0.y), aEE[0]);
-        aEE[1] = nf_ffma2(tA.m0, make_float2(tA.e0.z, tA.e0.w), aEE[1]);
-        if (iw == 3) ee16 = fmaf(tA.m0, sm.te[NO * QP + 16], ee16);
+#pragma unroll
+        for (int s = 0; s < E_STEPS; ++s) {
+          const int k = 2 * ir_kk(s, t);
+          const bool kin = s < E_STEPS - 1 || k < NB;
+          const double e0 = kin ? (double)m0[k] : 0.0, e1 = kin ? (double)m1[k] : 0.0;
+          dmma_16x8x4(aE[0], e0, e1, tb[(s * E_NT + ntb) * 32]);
+          dmma_16x8x4(aE[1], e0, e1, tb[(s * E_NT + ntb + 1) * 32]);
+          if (mid) dmma_16x8x4(aE[2], e0, e1, tb[(s * E_NT + 4) * 32]);
+          if (s < O_STEPS) {
+            const double o0 = m0[k + 1], o1 = m1[k + 1];
+            dmma_16x8x4(aO[0], o0, o1, tb[TAB_E + (s * O_NT + ntb) * 32]);
+            dmma_16x8x4(aO[1], o0, o1, tb[TAB_E + (s * O_NT + ntb + 1) * 32]);
+          }
+        }
         NR_LAP(3);
         named_bar(bar_id, PT);     // the group is done reading the rows
         if (nxt.ok) roff = prefetch(nxt.sg, nxt.tau);
@@ -559,53 +556,40 @@ noise_ring_kernel(Params p) {
         // Only now does the group need its ring slot: the sums above live in registers.
         if (P >= SLOTS) mbar_wait(&sm.empty[slot], ((P / SLOTS) - 1) & 1);
         NR_LAP(2);
-        float* hr = sm.h + (slot * 32 + lane) * HS + HPAD;
-        const float EEv[4] = {aEE[0].x, aEE[0].y, aEE[1].x, aEE[1].y};
-        const float EOv[4] = {aEO[0].x, aEO[0].y, aEO[1].x, aEO[1].y};
-        const float OA[4] = {aOa[0].x, aOa[0].y, aOa[1].x, aOa[1].y};
-        const float OB[4] = {aOb[0].x, aOb[0].y, aOb[1].x, aOb[1].y};
-        // window values as 16-byte loads: the periodic Hann window has win[128 - i] ==
-        // win[i], so the mirrors' win[64 + (32 - n)] = win[32 + n], win[32 - n] = win[96 + n]
-        const float4 wpa4 = *reinterpret_cast<const float4*>(sm.win + SHIFT + c0);
-        const float4 wma4 = *reinterpret_cast<const float4*>(sm.win + c0);
-        const float4 wpb4 = *reinterpret_cast<const float4*>(sm.win + Q + c0);
-        const float4 wmb4 = *reinterpret_cast<const float4*>(sm.win + SHIFT + Q + c0);
-        const float WPA[4] = {wpa4.x, wpa4.y, wpa4.z, wpa4.w}, WMA[4] = {wma4.x, wma4.y, wma4.z, wma4.w};
-        const float WPB[4] = {wpb4.x, wpb4.y, wpb4.z, wpb4.w}, WMB[4] = {wmb4.x, wmb4.y, wmb4.z, wmb4.w};
-        float vpa[4], vma[4], vpb[4], vmb[4];
+        // h0[n] = E + O and h0[64 - n] = E - O, each rounded to float once, times the
+        // periodic Hann window (win[128 - i] == win[i]): taps 64 +- n and n, 128 - n
+        float* hs = sm.h + slot * 32 * HS + HPAD;
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const float Ea = EEv[c] + EOv[c], Eb = EEv[c] - EOv[c];     // E[n], E[32 - n]
-          vpa[c] = row_ok ? WPA[c] * (Ea + OA[c]) : 0.f;   // n:      taps 64 +- n
-          vma[c] = row_ok ? WMA[c] * (Ea - OA[c]) : 0.f;   //         taps n, 128 - n
-          vpb[c] = row_ok ? WPB[c] * (Eb + OB[c]) : 0.f;   // 32 - n: taps 96 - n, 32 + n
-          vmb[c] = row_ok ? WMB[c] * (Eb - OB[c]) : 0.f;   //         taps 32 - n, 96 + n
+        for (int j = 0; j < 2; ++j) {
+          const int n = 8 * (ntb + j) + 2 * t;          // this lane's columns n, n + 1
+          const float2 wp = *reinterpret_cast<const float2*>(sm.win + SHIFT + n);
+          const float2 wm = *reinterpret_cast<const float2*>(sm.win + n);
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const bool ok = r ? ok1 : ok0;
+            float* hr = hs + (r ? f1 : f0) * HS;
+            const double E0 = aE[j][2 * r], E1 = aE[j][2 * r + 1];
+            const double O0 = aO[j][2 * r], O1 = aO[j][2 * r + 1];
+            const float p0 = ok ? wp.x * (float)(E0 + O0) : 0.f;
+            const float p1 = ok ? wp.y * (float)(E1 + O1) : 0.f;
+            const float q0 = ok ? wm.x * (float)(E0 - O0) : 0.f;
+            const float q1 = ok ? wm.y * (float)(E1 - O1) : 0.f;
+            *reinterpret_cast<float2*>(hr + SHIFT + n) = make_float2(p0, p1);
+            hr[SHIFT - n] = p0;
+            hr[SHIFT - n - 1] = p1;
+            *reinterpret_cast<float2*>(hr + n) = make_float2(q0, q1);
+            if (n != 0) hr[S - n] = q0;                  // tap 128 does not exist
+            hr[S - n - 1] = q1;
+          }
         }
-        // v[c] to hr[base + c] / hr[base - c]; 8-byte stores where the pair starts even
-        auto st_up = [&](int base, const float* v) {
-          *reinterpret_cast<float2*>(hr + base) = make_float2(v[0], v[1]);
-          *reinterpret_cast<float2*>(hr + base + 2) = make_float2(v[2], v[3]);
-        };
-        auto st_down = [&](int base, const float* v, bool first) {
-          if (first) hr[base] = v[0];
-          *reinterpret_cast<float2*>(hr + base - 2) = make_float2(v[2], v[1]);
-          hr[base - 3] = v[3];
-        };
-        st_up(SHIFT + c0, vpa);                          // 64 + n
-        st_down(SHIFT - c0, vpa, true);                  // 64 - n
-        st_up(c0, vma);                                  // n
-        st_down(S - c0, vma, c0 != 0);                   // 128 - n (tap 128 does not exist)
-        st_down(SHIFT + Q - c0, vpb, true);              // 64 + (32 - n)
-        st_up(Q + c0, vpb);                              // 64 - (32 - n)
-        st_down(Q - c0, vmb, true);                      // 32 - n
-        st_up(SHIFT + Q + c0, vmb);                      // 128 - (32 - n)
-        if (iw == 3) {                                   // n = 16
-          const float vp16 = row_ok ? sm.win[SHIFT + 16] * (ee16 + o16) : 0.f;
-          const float vm16 = row_ok ? sm.win[16] * (ee16 - o16) : 0.f;
-          hr[SHIFT + 16] = vp16;
-          hr[SHIFT - 16] = vp16;
-          hr[16] = vm16;
-          hr[S - 16] = vm16;
+        if (mid && t == 0) {                             // n = 32: taps 32 and 96
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const float v = (r ? ok1 : ok0) ? sm.win[Q] * (float)aE[2][2 * r] : 0.f;
+            float* hr = hs + (r ? f1 : f0) * HS;
+            hr[Q] = v;
+            hr[S - Q] = v;
+          }
         }
       }
       NR_LAP(5);

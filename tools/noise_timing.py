@@ -33,12 +33,14 @@ t = buf.astype(np.float64)
 t = t[t.sum(axis=(1, 2)) > 0]                    # the CTAs of the grid
 N_SMS = len(t)
 n_warps = int((t.sum(axis=(0, 2)) > 0).sum())
-cons, prod = t[:, :8], t[:, 8:n_warps]
+# consumer warps come first and record phases 0..3 only
+n_cons = int((t[:, :n_warps, 4:].sum(axis=(0, 2)) == 0).sum())
+cons, prod = t[:, :n_cons], t[:, n_cons:n_warps]
 cn = ['wait full', 'FIR', 'release + store', 'loop / skip']
-pn = ['wait raw (TMA)', 'exp_sigmoid + bar', 'wait empty', 'cosine sums', 'bar + prefetch',
+pn = ['wait raw (TMA)', 'exp_sigmoid + bar', 'wait empty', 'IR sums (DMMA)', 'bar + prefetch',
       'taps epilogue', 'Philox rows + arrive', 'iterate']
-print('%s: B=%d, %d warps per CTA; cycles per warp, mean over %d CTAs (min .. max of the per-CTA means)' %
-      (os.path.basename(path), B, n_warps, N_SMS))
+print('%s: B=%d, %d warps per CTA (%d consumers); cycles per warp, mean over %d CTAs '
+      '(min .. max of the per-CTA means)' % (os.path.basename(path), B, n_warps, n_cons, N_SMS))
 tot = cons.sum(axis=2).mean()
 print('consumers: %.0f cycles in the tile loop' % tot)
 for i, nm in enumerate(cn):

@@ -63,10 +63,10 @@ def main(tag):
         f.write('  %-12s %5d\n' % (op, n))
       marks = {k: ops.get(k, 0) for k in ('FFMA2', 'FADD2', 'FMUL2', 'UBLKCP', 'SYNCS',
                                           'UTMALDG', 'MUFU', 'LDS', 'STS', 'LDG', 'STG',
-                                          'RED', 'IMAD', 'SHFL')}
+                                          'RED', 'IMAD', 'SHFL', 'DMMA')}
       f.write('\nmarkers: %s\n' % marks)
-      f.write('  (UBLKCP = cp.async.bulk 1-D TMA copies, SYNCS = mbarrier ops; no UTC*MMA: '
-              'the path uses no tensor cores by design)\n')
+      f.write('  (UBLKCP = cp.async.bulk 1-D TMA copies, SYNCS = mbarrier ops; DMMA = FP64 '
+              'tensor-core MMA, only in noise_ring\'s impulse-response synthesis)\n')
       f.write('\nhot loop excerpt (lines %d..%d):\n' % (lo, hi))
       f.write('\n'.join(l.rstrip() for l in lines[lo:hi]))
       f.write('\n')
