@@ -94,6 +94,10 @@ SIGNATURES = {
     'ddsp_b200_frame_window_adjoint':
         (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     'ddsp_b200_spectral_l1': (_i, [_vp, _vp, _vp, _vp, _i64, _f, _f, _i, _i, _vp]),
+    'ddsp_b200_mod_delay_forward':
+        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _i, _vp]),
+    'ddsp_b200_mod_delay_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _i, _vp]),
 }
 
 _lib = None

@@ -224,6 +224,36 @@ class FilteredNoiseFn(torch.autograd.Function):
     return dmags, None, None, None, None, None
 
 
+class ModDelayFn(torch.autograd.Function):
+  """core.mod_delay (ModDelay.get_signal, effects.py:370-394, and
+  core.variable_length_delay, core.py:1285-1314) on [B, N] operands,
+  differentiable in audio, gain and phase; one backward kernel writes the three
+  gradients (csrc/mod_delay.cuh).  gain may be None (variable_length_delay)."""
+
+  @staticmethod
+  def forward(ctx, audio, gain, phase, max_length, scale, offset, add_dry):
+    ctx.save_for_backward(audio, gain, phase)
+    ctx.cfg = (max_length, scale, offset, add_dry)
+    return core.mod_delay_forward(audio, gain, phase, max_length, scale, offset,
+                                  add_dry)
+
+  @staticmethod
+  def backward(ctx, grad_out):
+    audio, gain, phase = ctx.saved_tensors
+    max_length, scale, offset, add_dry = ctx.cfg
+    g = grad_out.contiguous().to(torch.float32)
+    want = ctx.needs_input_grad
+    d_audio = torch.empty_like(audio) if want[0] else None
+    d_gain = torch.empty_like(gain) if gain is not None and want[1] else None
+    d_phase = torch.empty_like(phase) if want[2] else None
+    b, n = audio.shape
+    _lib.check(_lib.load().ddsp_b200_mod_delay_backward(
+        audio.data_ptr(), phase.data_ptr(), core._ptr(gain), g.data_ptr(),
+        core._ptr(d_audio), core._ptr(d_gain), core._ptr(d_phase), b, n, max_length,
+        scale, offset, int(add_dry), _stream()))
+    return d_audio, d_gain, d_phase, None, None, None, None
+
+
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):
   """core.exp_sigmoid (core.py:386-404) as differentiable torch ops."""
   return max_value * torch.sigmoid(x)**math.log(exponent) + threshold

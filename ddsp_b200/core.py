@@ -968,6 +968,72 @@ def frequency_filter(audio, magnitudes, window_size: int = 0,
   return fft_convolve(audio, impulse_response, padding=padding)
 
 
+# ----------------------------------------------------------------------------
+# Modulated delay (core.py:1168-1214, 1285-1314; effects.py:328-394)
+# ----------------------------------------------------------------------------
+def _per_sample_shape(x, batch_size, n_samples, name):
+  """The [B, N] or [B, 1] shape of a [B, N, 1] / [B, N] control or of the
+  per-item [B, 1, 1] / [B, 1] that TensorFlow broadcasts (static shape only)."""
+  shape = _shape(x)
+  if len(shape) == 3 and shape[2] == 1:
+    shape = shape[:2]
+  if len(shape) != 2 or shape[0] != batch_size or shape[1] not in (1, n_samples):
+    raise ValueError(f'{name} must be [batch, n_samples(, 1)] or [batch, 1(, 1)] '
+                     f'for audio of shape ({batch_size}, {n_samples}); got '
+                     f'{_shape(x)}.')
+  return shape
+
+
+def _per_sample(x, shape, batch_size, n_samples):
+  return torch_float32(x).reshape(shape).expand(batch_size, n_samples).contiguous()
+
+
+def mod_delay(audio, gain, phase, max_length, scale=1.0, offset=0.0, add_dry=False):
+  """`[add_dry] audio + gain * variable_length_delay(phase * scale + offset, audio,
+  max_length)` in one kernel (csrc/mod_delay.cuh); `phase * scale + offset` is two
+  float32 roundings, as ModDelay's host arithmetic.  gain None means 1.  Routes to
+  `autograd.ModDelayFn` when grad is enabled and an input requires it."""
+  sa = _shape(audio)
+  if len(sa) != 2:
+    raise ValueError(f'audio must be [batch, n_samples]; got {sa}.')
+  batch_size, n_samples = sa
+  if int(max_length) != max_length or max_length < 1:
+    raise ValueError(f'max_length must be a positive integer; got {max_length}.')
+  if n_samples < 1:
+    raise ValueError(f'audio must have at least one sample; got {sa}.')
+  phase_shape = _per_sample_shape(phase, batch_size, n_samples, 'phase')
+  if gain is not None:
+    gain = _per_sample(gain, _per_sample_shape(gain, batch_size, n_samples, 'gain'),
+                       batch_size, n_samples)
+  phase = _per_sample(phase, phase_shape, batch_size, n_samples)
+  audio = torch_float32(audio)
+  args = (int(max_length), float(np.float32(scale)), float(np.float32(offset)),
+          bool(add_dry))
+  if torch.is_grad_enabled() and any(t is not None and t.requires_grad
+                                     for t in (audio, gain, phase)):
+    from ddsp_b200 import autograd as _ag
+    return _ag.ModDelayFn.apply(audio, gain, phase, *args)
+  return mod_delay_forward(audio, gain, phase, *args)
+
+
+def mod_delay_forward(audio, gain, phase, max_length, scale, offset, add_dry):
+  """The forward kernel on [B, N] float32 CUDA tensors (gain may be None)."""
+  out = torch.empty_like(audio)
+  with _on_device_of(audio, gain, phase):
+    _lib.check(_lib.load().ddsp_b200_mod_delay_forward(
+        _ptr(audio), _ptr(phase), _ptr(gain), _ptr(out), audio.shape[0],
+        audio.shape[1], max_length, scale, offset, int(add_dry), _stream()))
+  return out
+
+
+def variable_length_delay(phase, audio, max_length: int = 512):
+  """core.variable_length_delay (core.py:1285-1314): audio delayed by
+  phase * max_length samples with linear interpolation, the reference's wrap
+  included (phase in ((L-1)/L, 1] blends the oldest sample with the current one;
+  phase 1 is no delay)."""
+  return mod_delay(audio, None, phase, max_length)
+
+
 def uniform_noise(batch_size, n_samples, seed=0, offset=0, device=None):
   """Stand-in for tf.random.uniform([B, N], -1, 1) (synths.py:192-193):
   Philox4x32-10 keyed by `seed`, counter (sample/4, batch, offset)."""

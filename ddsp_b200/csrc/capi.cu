@@ -22,6 +22,7 @@
 #include "sinusoidal.cuh"
 #include "longconv.cuh"
 #include "spectral.cuh"
+#include "mod_delay.cuh"
 
 namespace ddsp {
 
@@ -1138,6 +1139,46 @@ int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
       reinterpret_cast<float2*>(grad_value), sums, n_bins_total, mag_weight, logmag_weight,
       1.0f / (float)n_bins_total, 1e-5f, n_bins, irfft_size);
   DDSP_CHECK_LAUNCH("spectral_l1");
+  return 0;
+}
+
+// ---- modulated delay ----------------------------------------------------------
+int ddsp_b200_mod_delay_forward(const float* audio, const float* phase, const float* gain,
+                                float* out, int B, int N, int max_length, float scale,
+                                float offset, int add_dry, void* stream) {
+  DDSP_REQUIRE(audio && phase && out, DDSP_B200_E_INVALID, "mod_delay_forward: null pointer");
+  DDSP_REQUIRE(B >= 0 && B <= 65535 && N >= 1 && max_length >= 1 && max_length < (1 << 29),
+               DDSP_B200_E_INVALID, "mod_delay_forward: bad shape B=%d N=%d max_length=%d",
+               B, N, max_length);
+  if (B == 0) return 0;
+  dim3 grid((unsigned)((N + md_::kThreads - 1) / md_::kThreads), B);
+  md_::mod_delay_forward_kernel<<<grid, md_::kThreads, 0, (cudaStream_t)stream>>>(
+      audio, phase, gain, out, N, max_length, scale, offset, add_dry);
+  DDSP_CHECK_LAUNCH("mod_delay_forward");
+  return 0;
+}
+
+int ddsp_b200_mod_delay_backward(const float* audio, const float* phase, const float* gain,
+                                 const float* grad_out, float* grad_audio, float* grad_gain,
+                                 float* grad_phase, int B, int N, int max_length, float scale,
+                                 float offset, int add_dry, void* stream) {
+  DDSP_REQUIRE(audio && phase && grad_out, DDSP_B200_E_INVALID,
+               "mod_delay_backward: null pointer");
+  DDSP_REQUIRE(grad_gain == nullptr || gain != nullptr, DDSP_B200_E_INVALID,
+               "mod_delay_backward: grad_gain asked for without a gain");
+  DDSP_REQUIRE(B >= 0 && B <= 65535 && N >= 1 && max_length >= 1 && max_length < (1 << 29),
+               DDSP_B200_E_INVALID, "mod_delay_backward: bad shape B=%d N=%d max_length=%d",
+               B, N, max_length);
+  if (B == 0 || (!grad_audio && !grad_gain && !grad_phase)) return 0;
+  const size_t smem = grad_audio ? md_::backward_smem_bytes() : 0;
+  int rc = set_smem(md_::mod_delay_backward_kernel, md_::backward_smem_bytes(),
+                    "mod_delay_backward");
+  if (rc) return rc;
+  dim3 grid((unsigned)((N + md_::kTile - 1) / md_::kTile), B);
+  md_::mod_delay_backward_kernel<<<grid, md_::kThreads, smem, (cudaStream_t)stream>>>(
+      audio, phase, gain, grad_out, grad_audio, grad_gain, grad_phase, N, max_length, scale,
+      offset, add_dry);
+  DDSP_CHECK_LAUNCH("mod_delay_backward");
   return 0;
 }
 

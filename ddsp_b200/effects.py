@@ -140,3 +140,40 @@ class FIRFilter(processors.Processor):
 
   def get_signal(self, audio, magnitudes):
     return core.frequency_filter(audio, magnitudes, window_size=self.window_size)
+
+
+class ModDelay(processors.Processor):
+  """Modulated delay behind chorus, flanger and vibrato (effects.py:328-394).
+
+  `get_signal` is one kernel: the phase mapping `phase * depth / max + center / max`,
+  the delay line, the gain and the dry mix (core.mod_delay).  As in the reference,
+  the mapped phase of the default `sigmoid` lies in (center / max, 1), which
+  reaches the wrap region of core.variable_length_delay near 1 (no delay there)."""
+
+  def __init__(self, center_ms=15.0, depth_ms=10.0, sample_rate=16000,
+               gain_scale_fn=core.exp_sigmoid, phase_scale_fn=torch.sigmoid,
+               add_dry=True, name='mod_delay'):
+    super().__init__(name=name)
+    self.center_ms = center_ms
+    self.depth_ms = depth_ms
+    self.sample_rate = sample_rate
+    self.gain_scale_fn = gain_scale_fn
+    self.phase_scale_fn = phase_scale_fn
+    self.add_dry = add_dry
+
+  def get_controls(self, audio, gain, phase):
+    """effects.py:349-366."""
+    if self.gain_scale_fn is not None:
+      gain = self.gain_scale_fn(core.torch_float32(gain))
+    if self.phase_scale_fn is not None:
+      phase = self.phase_scale_fn(core.torch_float32(phase))
+    return {'audio': audio, 'gain': gain, 'phase': phase}
+
+  def get_signal(self, audio, gain, phase):
+    """effects.py:368-394."""
+    max_delay_ms = self.center_ms + self.depth_ms
+    max_length_samples = int(self.sample_rate / 1000.0 * max_delay_ms)
+    depth_phase = self.depth_ms / max_delay_ms
+    center_phase = self.center_ms / max_delay_ms
+    return core.mod_delay(audio, gain, phase, max_length_samples, scale=depth_phase,
+                          offset=center_phase, add_dry=self.add_dry)

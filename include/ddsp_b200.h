@@ -346,6 +346,33 @@ int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
 int ddsp_b200_add(const float* a, const float* b, float* out, int64_t n,
                   void* stream);
 
+/* Modulated delay: core.variable_length_delay (core.py:1285-1314) and
+ * effects.ModDelay.get_signal (effects.py:328-394).
+ *   out[b,t] = (add_dry ? audio[b,t] : 0) + gain[b,t] * delay[b,t],
+ *   delay[b,t] = (1 - frac) v_{j0} + frac v_{j0+1},  pos = phase' * max_length,
+ *   phase' = phase[b,t] * scale + offset (two float32 roundings, no FMA),
+ *   j0 = floor(pos), frac = pos - j0,  v_j = audio[b, t - j] for 0 <= j < max_length
+ *   (0 for t - j < 0), v_{max_length} = audio[b, t] (the reference's wrap column),
+ *   v_j = 0 for j < 0 or j > max_length.
+ * audio, phase, out: [B, N]; gain: [B, N] or NULL (= 1).  core.variable_length_delay
+ * is scale = 1, offset = 0, gain = NULL, add_dry = 0.  1 <= max_length < 2^29.
+ * out must not alias audio.
+ *
+ * backward: for the upstream gradient grad_out [B, N], writes any of
+ *   grad_audio [B, N]  (d out / d audio, dry path included),
+ *   grad_gain  [B, N]  (= grad_out * delay; needs gain),
+ *   grad_phase [B, N]  (w.r.t. `phase`, i.e. times scale; 0 where pos is an integer:
+ *                       TensorFlow's subgradients of |.| and relu at 0);
+ * a NULL output is not computed.  No atomics: every element is written once and
+ * the result is bit-reproducible. */
+int ddsp_b200_mod_delay_forward(const float* audio, const float* phase, const float* gain,
+                                float* out, int B, int N, int max_length, float scale,
+                                float offset, int add_dry, void* stream);
+int ddsp_b200_mod_delay_backward(const float* audio, const float* phase, const float* gain,
+                                 const float* grad_out, float* grad_audio, float* grad_gain,
+                                 float* grad_phase, int B, int N, int max_length, float scale,
+                                 float offset, int add_dry, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
