@@ -31,8 +31,7 @@ def _newest_mtime():
 
 def _command(verbose=False):
   nvcc = os.environ.get('NVCC', 'nvcc')
-  extra = os.environ.get('DDSP_B200_NVCC_EXTRA', '').split()   # e.g. -DDDSP_HV4_NW=4
-  return [nvcc] + NVCC_FLAGS + extra + (['-Xptxas', '-v'] if verbose else []) + [
+  return [nvcc] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + [
       '-o', LIB_PATH] + _sources()
 
 
@@ -46,7 +45,7 @@ def _built_with():
 
 def is_stale():
   """True if the library is missing, older than its sources, or was built by
-  another nvcc command line (flags, arch, DDSP_B200_NVCC_EXTRA)."""
+  another nvcc command line (compiler, flags, arch)."""
   return (not os.path.exists(LIB_PATH) or
           os.path.getmtime(LIB_PATH) < _newest_mtime() or
           _built_with() != ' '.join(_command()))

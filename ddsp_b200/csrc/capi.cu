@@ -2,7 +2,6 @@
 // See include/ddsp_b200.h for the contract and the reference file:line each
 // entry point replaces.
 #include <stdarg.h>
-#include <string.h>
 
 #include <algorithm>
 
@@ -63,12 +62,6 @@ static int set_smem(K kernel, size_t bytes, const char* name) {
 }  // namespace ddsp
 
 using namespace ddsp;
-
-namespace ddsp {
-static inline int launch_harmonic_best(const HarmonicParams& p, cudaStream_t st) {
-  return launch_harmonic_v4(p, st);
-}
-}  // namespace ddsp
 
 extern "C" {
 
@@ -145,7 +138,7 @@ int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
   cudaStream_t st = (cudaStream_t)stream;
 
   if (phase_mode == DDSP_B200_PHASE_RECURRENCE && harmonic_fused_supported(p)) {
-    int rc = launch_harmonic_best(p, st);
+    int rc = launch_harmonic_v4(p, st);
     if (rc != 1) return rc;   // 1 = declined, fall through to the generic path
   }
 
@@ -418,7 +411,7 @@ static int decoder_forward_impl(const float* amps_raw, const float* hd_raw,
                "decoder_forward: shape outside the fused decoder path "
                "(needs hop %% 64 == 0, n_frequencies <= %d)", kNfMaxNb);
   cudaStream_t st = (cudaStream_t)stream;
-  int rc = launch_harmonic_best(p, st);
+  int rc = launch_harmonic_v4(p, st);
   if (rc == 1) {
     set_error("decoder_forward: harmonic tile does not fit shared memory");
     return DDSP_B200_E_UNSUPPORTED;
@@ -629,11 +622,7 @@ int ddsp_b200_harmonic_backward(const float* f0_hz, const float* grad_audio,
                DDSP_B200_E_UNSUPPORTED,
                "harmonic_backward: needs hop %% 64 == 0 (hop = %d)", p.hop);
   cudaStream_t st = (cudaStream_t)stream;
-  static const bool use_v1 = [] {
-    const char* e = getenv("DDSP_B200_HARM_BWD");
-    return e != nullptr && strcmp(e, "v1") == 0;
-  }();
-  if (!use_v1 && harmonic_backward2_supported(p))
+  if (harmonic_backward2_supported(p))
     return launch_harmonic_backward2(p, grad_audio, g0, g1, st);
   const size_t gbytes = sizeof(float) * (size_t)B * F * K;
   DDSP_CUDA_TRY(cudaMemsetAsync(g0, 0, gbytes, st), "harmonic_backward: memset g0");

@@ -152,26 +152,7 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src,
       "l"(src), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
-// DDSP_MBAR_HINT_NS > 0: pass a suspend-time hint to try_wait, so that a waiting
-// warp sleeps in hardware (and is woken by the phase flip) instead of coming back
-// to the issue stage every few hundred cycles.
-#ifndef DDSP_MBAR_HINT_NS
-#define DDSP_MBAR_HINT_NS 0
-#endif
 __device__ __forceinline__ void mbar_wait(void* bar, uint32_t phase) {
-#if DDSP_MBAR_HINT_NS > 0
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "WAIT_%=:\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n"
-      "@p bra DONE_%=;\n"
-      "bra WAIT_%=;\n"
-      "DONE_%=:\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(phase), "r"((uint32_t)DDSP_MBAR_HINT_NS)
-      : "memory");
-#else
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
@@ -183,7 +164,6 @@ __device__ __forceinline__ void mbar_wait(void* bar, uint32_t phase) {
       "}\n" ::"r"(smem_u32(bar)),
       "r"(phase)
       : "memory");
-#endif
 }
 
 __device__ __forceinline__ void mbar_arrive(void* bar) {

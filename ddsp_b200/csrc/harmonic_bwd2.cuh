@@ -13,9 +13,17 @@
 namespace ddsp {
 namespace hb2 {
 
-using hcm::FrameRec;
-constexpr int NW = hcm::kBwdWarps;
+constexpr int NW = 4;     // warps per CTA
 constexpr int NT = NW * 32;
+
+// Frame record of the third forward generation.
+struct __align__(16) FrameRec {
+  unsigned long long P, A;       // P carries the +2^31 rounding offset
+  unsigned long long D;
+  int kca, kcb;                  // live counts at r = 0 / r = hop-1; kca < 0: exact path
+  float f_lo, f_hi, amp0, amp1;
+};
+static_assert(sizeof(FrameRec) == 48, "FrameRec must be three 16-byte words");
 
 struct Smem {
   size_t off_tab, off_red, off_warp, warp_stride, total;
@@ -31,7 +39,8 @@ __host__ __device__ inline Smem smem_layout(int FW) {
   return s;
 }
 
-// Signed chain state of one sample.  The forward kernel's chain (v, d) steps as
+// Signed chain state of one sample: .x = odd-harmonic chain sin((1+2j) phi), .y =
+// even-harmonic chain sin((2+2j) phi).  The forward kernel's chain (v, d) steps as
 //   d' = d + na v,  v' = v + d'
 // on the angle 2 phi reduced to [-pi/2, pi/2]; where the reduction shifted it by half
 // a turn (sigma = -1) the true value is sin((1+2j) phi) = sigma^j v_j.  Here the sign
@@ -45,12 +54,23 @@ struct Chain {
 
 __device__ __forceinline__ void chain_seed(Chain& c, uint32_t p,
                                            const float2* __restrict__ tab) {
-  hcm::Osc o;
-  hcm::osc_seed(o, p, tab);
-  c.S = o.v;
-  c.sigma = o.sigma;
-  c.Dd = o.d;
-  c.sna = make_float2(o.sigma * o.na.x, o.sigma * o.na.y);
+  const uint32_t i = (p + (1u << (31 - kSinTabBits))) >> (32 - kSinTabBits);
+  const int r = (int)(p - (i << (32 - kSinTabBits)));
+  const float2 t = tab[i & (kSinTab - 1)];
+  const float eps = (float)r * 1.4629180792671596e-9f;           // 2 pi / 2^32
+  const float e2 = eps * eps;
+  const float ce = fmaf(e2, -0.5f, 1.0f);
+  const float se = eps * fmaf(e2, -0.16666667f, 1.0f);
+  const float s1 = fmaf(t.y, se, t.x * ce);
+  const float c1 = fmaf(-t.x, se, t.y * ce);
+  const float ss = s1 * s1, cc = c1 * c1;
+  const bool flip = ss > cc;                                     // cos(2 phi) < 0
+  const float s2 = (s1 + s1) * c1;                               // sin(2 phi)
+  const float na = -4.0f * fminf(ss, cc);
+  c.S = make_float2(s1, s2);
+  c.sigma = flip ? -1.0f : 1.0f;
+  c.Dd = make_float2(flip ? 0.0f : s1 + s1, s2);
+  c.sna = make_float2(c.sigma * na, c.sigma * na);
 }
 __device__ __forceinline__ void chain_step(Chain& c) {
   const float2 sg = make_float2(c.sigma, c.sigma);

@@ -13,10 +13,7 @@
 //     are f32x2 over the two samples: no cross-half sums, eight accumulator
 //     registers less;
 //   * the per-sample phase is 4 IMADs on the 64-bit fixed-point frame phase
-//     (hcm::phase32).  DDSP_HV4_PHASE_F64=1 builds the alternative, off by
-//     default: two DFMAs on the FP64 pipe, y = P' + c1 A + c2 D with
-//     P' = P + 1.5 * 2^20, whose low mantissa word IS the 32-bit fixed-point
-//     phase (the in-frame offset is < 2^13 turns, so the rounding is <= 2^-32 turn);
+//     (hcm::phase32);
 //   * get_controls writes each row once: exp_sigmoid on the live prefix, zeros
 //     above it, and the row's 1 / sum goes into the frame amplitude (amp / sum),
 //     not into a second pass over the row;
@@ -35,20 +32,31 @@
 #include "harmonic_common.cuh"
 
 namespace ddsp {
+
+// Slow, exact per-oscillator evaluation of one sample (frames with f0 < 1 Hz,
+// where the live-count shortcut is not valid).
+__device__ __noinline__ float harmonic_sample_exact(const float* x0,
+                                                    const float* x1, float w0,
+                                                    float w1, uint32_t p32,
+                                                    float f_lo, float f_hi,
+                                                    float frac, int K,
+                                                    float nyq) {
+  float acc = 0.f;
+  uint32_t pk = 0;
+  for (int k = 1; k <= K; ++k) {
+    pk += p32;
+    if (!(ref_harmonic_freq(f_lo, f_hi, frac, k) < nyq)) continue;
+    float a = x0[k - 1] * w0 + x1[k - 1] * w1;
+    acc = fmaf(a, sinpif((float)(int)pk * 4.656612873077393e-10f), acc);
+  }
+  return acc;
+}
+
 namespace hv4 {
 
-#ifndef DDSP_HV4_NW
-#define DDSP_HV4_NW 4
-#endif
-constexpr int NW = DDSP_HV4_NW;  // warps per CTA
+constexpr int NW = 4;            // warps per CTA
 constexpr int NT = NW * 32;
-
-#ifndef DDSP_HV4_PHASE_F64
-#define DDSP_HV4_PHASE_F64 0
-#endif
-#ifndef DDSP_HV4_MIN_CTAS
-#define DDSP_HV4_MIN_CTAS (24 / DDSP_HV4_NW)
-#endif
+constexpr int MIN_CTAS = 6;      // per SM: 24 warps, 80 registers
 
 // -DDDSP_HV4_TIMING: per-SM totals of each warp's clock() cycles by kernel phase,
 // summed over every CTA the SM ran (tools/harm_timing.py reads them back through
@@ -81,12 +89,8 @@ __device__ unsigned long long g_hv4_timing[kMaxSMs * (kTimingPhases + 1)];
 #define HV4_TIMING_FLUSH()
 #endif
 
-// 2^32 * (phase + 2^-9 turn): the table index is the top byte of the ROUNDED-UP
-// phase, the residual its low 24 bits minus 2^23.
-constexpr double kMagic = 1572864.0 + 0.001953125;          // 1.5 * 2^20 + 2^-9
-
 struct __align__(16) FrameRec {
-  unsigned long long P, A;       // F64 phase: bit patterns of doubles
+  unsigned long long P, A;       // P carries the +2^31 rounding and +2^-9 turn offsets
   unsigned long long D;
   int ng;                        // > 0: uniform frame, ng unmasked groups; 0: per-sample
                                  // live counts; < 0: exact path (f0 < 1 Hz)
@@ -176,6 +180,54 @@ __device__ __forceinline__ void controls_rows4(float* __restrict__ sXw,
   sum += __shfl_xor_sync(0xffffffffu, sum, 2);
   sum += __shfl_xor_sync(0xffffffffu, sum, 1);
   if (row_ok && l8 == 0) sInv[r] = __fdividef(1.0f, (sum == 0.0f) ? 1e-7f : sum);
+}
+
+// Harmonic.get_controls for up to four rows (r0 .. r0+3 of this warp's block) in
+// shared memory, 8 lanes per row: exp_sigmoid on the live prefix, zeros above it,
+// row normalisation with safe_divide (synths.py:110-117, core.py:894-907).  The
+// frame-rate live count of each row (f0*k < sr/2 in float32) was computed once
+// per row by the caller.
+__device__ __forceinline__ void controls_rows(float* __restrict__ sXw,
+                                              const int* __restrict__ sLive, int r0,
+                                              int nrows, int Kp, bool raw_scale,
+                                              int lane) {
+  const int K4 = Kp >> 2;
+  const int sub = lane >> 3, l8 = lane & 7;
+  const int r = r0 + sub;
+  const bool row_ok = r < nrows;
+  float4* row4 = reinterpret_cast<float4*>(sXw + (row_ok ? r : r0) * Kp);
+  const int live = sLive[row_ok ? r : r0];
+  float sum = 0.f;
+  if (row_ok) {
+    for (int c4 = l8; c4 < K4; c4 += 8) {
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (4 * c4 < live) {
+        v = row4[c4];
+        float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          float w = e[u];
+          if (raw_scale) w = exp_sigmoid_f(w);
+          if (4 * c4 + u >= live) w = 0.f;
+          e[u] = w;
+          sum += w;
+        }
+        v = make_float4(e[0], e[1], e[2], e[3]);
+      }
+      row4[c4] = v;
+    }
+  }
+  sum += __shfl_xor_sync(0xffffffffu, sum, 4);
+  sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+  sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+  const float inv = 1.0f / ((sum == 0.0f) ? 1e-7f : sum);
+  if (row_ok) {
+    for (int c4 = l8; 4 * c4 < live; c4 += 8) {
+      float4 v = row4[c4];
+      v.x *= inv; v.y *= inv; v.z *= inv; v.w *= inv;
+      row4[c4] = v;
+    }
+  }
 }
 
 // Frame-rate live count of a row (f0 * k < sr/2 in float32, core.py:888).
@@ -300,11 +352,7 @@ __device__ __forceinline__ float4 mask4u(const float4& X, int rem) {
 }
 
 struct LaneConst {
-#if DDSP_HV4_PHASE_F64
-  double c1a, c2a, c1b, c2b;     // r + 1, r (r + 1) / 2 for the lane's two samples
-#else
-  uint32_t c1a, c2a, c1b, c2b;
-#endif
+  uint32_t c1a, c2a, c1b, c2b;   // r + 1, r (r + 1) / 2 for the lane's two samples
   float2 w1;                     // amplitude weight of row x1 (Hann or linear)
 };
 
@@ -313,20 +361,11 @@ __device__ __forceinline__ LaneConst lane_const(int r0, int lane, float inv_hop,
                                                 const float* __restrict__ sW) {
   LaneConst c;
   const uint32_t ra = r0 + lane, rb = ra + 32;
-#if DDSP_HV4_PHASE_F64
-  c.c1a = (double)(ra + 1); c.c2a = (double)((ra * (ra + 1)) >> 1);
-  c.c1b = (double)(rb + 1); c.c2b = (double)((rb * (rb + 1)) >> 1);
-#else
   c.c1a = ra + 1; c.c2a = (ra * (ra + 1)) >> 1;
   c.c1b = rb + 1; c.c2b = (rb * (rb + 1)) >> 1;
-#endif
   // keep the constants in registers: ptxas otherwise re-derives them (and their
   // integer feeds) in every frame
-#if DDSP_HV4_PHASE_F64
-  asm volatile("" : "+d"(c.c1a), "+d"(c.c2a), "+d"(c.c1b), "+d"(c.c2b));
-#else
   asm volatile("" : "+r"(c.c1a), "+r"(c.c2a), "+r"(c.c1b), "+r"(c.c2b));
-#endif
   if (sW != nullptr) {
     c.w1 = make_float2(sW[ra], sW[rb]);
   } else {
@@ -353,16 +392,8 @@ __device__ __forceinline__ void frame_chunk(
   const float4 fa = *reinterpret_cast<const float4*>(&rec->f_lo);
   const unsigned long long D = ((unsigned long long)Dk.y << 32) | Dk.x;
   const int ng = (int)Dk.z, rem = (int)Dk.w;
-#if DDSP_HV4_PHASE_F64
-  const double Pd = __longlong_as_double((long long)PA.x);
-  const double Ad = __longlong_as_double((long long)PA.y);
-  const double Dd = __longlong_as_double((long long)D);
-  const uint32_t qa = (uint32_t)__double2loint(fma(lc.c2a, Dd, fma(lc.c1a, Ad, Pd)));
-  const uint32_t qb = (uint32_t)__double2loint(fma(lc.c2b, Dd, fma(lc.c1b, Ad, Pd)));
-#else
   const uint32_t qa = phase32(PA.x, PA.y, D, lc.c1a, lc.c2a);
   const uint32_t qb = phase32(PA.x, PA.y, D, lc.c1b, lc.c2b);
-#endif
   // (1 - w1) amp0, w1 amp1
   const float2 w0 = ffma2(make_float2(-lc.w1.x, -lc.w1.y), make_float2(fa.z, fa.z),
                                make_float2(fa.z, fa.z));
@@ -439,7 +470,7 @@ __device__ __forceinline__ void frame_chunk(
 }
 
 template <bool WINDOW, int HOPT>
-__global__ void __launch_bounds__(NT, DDSP_HV4_MIN_CTAS)
+__global__ void __launch_bounds__(NT, MIN_CTAS)
 harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int hop = HOPT ? HOPT : p.hop;
@@ -630,13 +661,7 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
     }
     if (lane < cnt) {
       FrameRec r;
-#if DDSP_HV4_PHASE_F64
-      r.P = 0;
-      r.A = (unsigned long long)__double_as_longlong(a0);
-      r.D = (unsigned long long)__double_as_longlong(dd);
-#else
       r.P = 0; r.A = turns_to_fix64(a0); r.D = turns_to_fix64(dd);
-#endif
       r.ng = ng; r.rem = rem;
       r.f_lo = f; r.f_hi = f_n; r.amp0 = a; r.amp1 = a_n;
       sRec[fr] = r;
@@ -658,14 +683,7 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
     for (int w = 0; w < warp; ++w) P0 += sWarpTot[w];
     if (lane < cnt) {
       const unsigned long long Pf = P0 + excl;         // exact frame phase, 2^64 = 1 turn
-#if DDSP_HV4_PHASE_F64
-      // top 53 bits as a double in [0, 1), plus the magic that makes the low
-      // mantissa word of P' + offsets the rounded 32-bit phase (+ 2^-9 turn)
-      const double Pd = (double)(Pf >> 11) * 1.1102230246251565e-16 + kMagic;
-      sRec[fr].P = (unsigned long long)__double_as_longlong(Pd);
-#else
       sRec[fr].P = Pf + 0x80000000ull + (1ull << (63 - kSinTabBits));
-#endif
     }
   }
   HV4_LAP(3);
@@ -688,7 +706,7 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
           controls_rows4(sXw, sLive + c0, sInv + c0, r0, nrows, Kp, raw_scale, lane);
       } else {
         for (int r0 = 0; r0 < nrows; r0 += 4)
-          hcm::controls_rows(sXw, sLive + c0, r0, nrows, Kp, raw_scale, lane);
+          controls_rows(sXw, sLive + c0, r0, nrows, Kp, raw_scale, lane);
         for (int r = lane; r < nrows; r += 32) sInv[c0 + r] = 1.0f;
       }
     } else {
@@ -757,17 +775,14 @@ inline cudaError_t launch_one(const HarmonicParams& p, int use_tma, int FW, dim3
 inline int launch_harmonic_v4(HarmonicParams p, cudaStream_t st) {
   using namespace hv4;
   p.Kp = (p.K + 3) & ~3;
-  static const int env_fw = [] { const char* e = getenv("DDSP_B200_HARM_FW"); return e ? atoi(e) : 0; }();
   // Four warps per CTA and 8 frames per warp: one full record warp for the 32-frame
-  // tile while the other three transform its 33 rows (11 frames per warp with one
-  // warp per CTA); DDSP_B200_HARM_FW overrides the frames per warp for A/B timing.
-  // Small grids shrink the tile until every SM has one.
-  int FW = (NW == 1) ? 11 : 8;
-  const long long want_ctas = 8ll * num_sms() * (4 / NW);        // 32 warps per SM
+  // tile while the other three transform its 33 rows.  Small grids shrink the tile
+  // until every SM has one.
+  int FW = 8;
+  const long long want_ctas = 8ll * num_sms();                   // 32 warps per SM
   while (FW > 4 && (long long)p.B * ((p.F + FW * NW - 1) / (FW * NW)) < want_ctas) FW = (FW + 1) >> 1;
   while (FW > 1 && (long long)p.B * ((p.F + FW * NW - 1) / (FW * NW)) < num_sms()) FW = (FW + 1) >> 1;
-  if (env_fw > 0) FW = std::min(32, env_fw);
-  FW = std::max(1, std::min(FW, (p.F + NW - 1) / NW));
+  FW =std::max(1, std::min(FW, (p.F + NW - 1) / NW));
   while (FW > 1 && smem_layout(FW, p.Kp, p.hop).total > 64 * 1024) FW = (FW + 1) / 2;
   const size_t smem = smem_layout(FW, p.Kp, p.hop).total;
   if (smem > 200 * 1024) return 1;

@@ -14,7 +14,7 @@
 //     and writes it straight to HBM (st / red.add for the fused Add) - consumer
 //     warps never talk to each other.
 //   * ROW RING, NO HALO.  A persistent CTA walks a contiguous range of frames; the
-//     impulse responses and noise rows live in a ring of eight 32-row slots in shared
+//     impulse responses and noise rows live in a ring of seven 32-row slots in shared
 //     memory (lane-private rows, strides = 2 mod 4 floats: conflict-free LDS.64),
 //     so neighbouring tiles share their edge rows instead of recomputing them.
 //   * ONE ACCUMULATOR PER OUTPUT, TAP-STATIONARY ORDER.  A consumer warp owns a
@@ -41,37 +41,19 @@ namespace ddsp {
 namespace nr_ {
 constexpr int NB = 65, FRAME = 64, S = 128, S0 = 128, Q = 32, SHIFT = 64;
 // A consumer warp owns a UNIT of R outputs of 32 frames: R accumulators and the R
-// inputs of a body in registers.  R = 16 (four units per frame, 9 KB of FIR bodies)
-// is the product; R = 32 (two units, half the shared-memory loads per FMA, 35 KB
-// of bodies) compiles (-DDDSP_NR_UNIT=32) for A/B timing.  Timed on the H100, the
-// smaller block wins (DESIGN.md 3.2).
-#ifndef DDSP_NR_UNIT
-#define DDSP_NR_UNIT 16
-#endif
-constexpr int R = DDSP_NR_UNIT;
-static_assert(R == 16 || R == 32, "noise_ring unit: 16 or 32 outputs");
+// inputs of a body in registers.  R = 16: four units per frame, 9 KB of FIR bodies
+// (a 32-output unit was timed slower on the H100, DESIGN.md 3.2).
+constexpr int R = 16;
 constexpr int UPT = FRAME / R;                     // units per 64-sample frame
 // Consumer warps, producer groups and ring slots.  The consumer tile groups hold
 // NTG + 1 slots between them; what is left decouples producers from consumers.
-// 227 KB of shared memory hold 7 slots next to the cosine table and up to three
-// raw-magnitude staging buffers.  The consumer warp count (8 or 16) and the group
-// count (1 .. 3) are build knobs for A/B timing (DESIGN.md 3.2).
-#ifndef DDSP_NR_CONS_WARPS
-#define DDSP_NR_CONS_WARPS 8
-#endif
-#ifndef DDSP_NR_PROD_GROUPS
-#define DDSP_NR_PROD_GROUPS 3
-#endif
-#ifndef DDSP_NR_MAX_SLOTS
-#define DDSP_NR_MAX_SLOTS 7
-#endif
-constexpr int CONS_WARPS = DDSP_NR_CONS_WARPS, PROD_GROUPS = DDSP_NR_PROD_GROUPS;
+// 227 KB of shared memory hold 7 slots next to the cosine table and the three
+// raw-magnitude staging buffers.  Other warp shapes were timed slower (DESIGN.md 3.2).
+constexpr int CONS_WARPS = 8, PROD_GROUPS = 3;
 constexpr int GROUP_WARPS = 4, PROD_WARPS = GROUP_WARPS * PROD_GROUPS;
-static_assert(CONS_WARPS == 8 || CONS_WARPS == 16, "noise_ring consumers: 8 or 16 warps");
-static_assert(PROD_GROUPS >= 1 && PROD_GROUPS <= 3, "noise_ring producers: 1 .. 3 groups");
 constexpr int NTG = CONS_WARPS / UPT;              // consumption tiles in flight
 static_assert((NTG & (NTG - 1)) == 0, "tile groups: a power of two");
-constexpr int SLOTS = DDSP_NR_MAX_SLOTS;
+constexpr int SLOTS = 7;
 static_assert(SLOTS > NTG + 1, "the ring must leave slots to the producers");
 constexpr int RING = 32 * SLOTS;
 // Every warp runs under the launch budget (65536 / THREADS registers: 96 for 640
