@@ -9,6 +9,12 @@ kernels, exposed as `torch.autograd.Function`s:
     phase path, `models/inverse_synthesis.py:84-117`; computed only when f0
     requires grad);
   * `FilteredNoiseFn`      - d magnitudes (the filter is linear in them);
+  * `SinusoidalSynthesisFn` - d amplitudes and d frequencies of the frame-rate
+    oscillator bank (`Sinusoidal.get_signal`, the synthesizer of
+    `models/inverse_synthesis.py:84-105`; d frequencies only when they require
+    grad); `core.sinusoidal_synthesis` routes to it under grad;
+  * `FftConvolveLtiFn` / `ModDelayFn` - the reverb convolution and the modulated
+    delay, routed to by `core.fft_convolve` / `core.mod_delay` under grad;
   * `DecoderFn` / `decoder_train` - the whole `ae.gin` decoder from RAW network
     outputs: forward is the fused two-kernel pipeline (`get_controls` in shared
     memory), backward is the two synthesizer backward kernels plus the
@@ -222,6 +228,42 @@ class FilteredNoiseFn(torch.autograd.Function):
         seed & (2**64 - 1), offset & (2**64 - 1), dmags.data_ptr(), b, f, nb,
         n_samples, window_size, _stream()))
     return dmags, None, None, None, None, None
+
+
+class SinusoidalSynthesisFn(torch.autograd.Function):
+  """core.sinusoidal_synthesis (Sinusoidal.get_signal, synths.py:305-323, on the
+  fused route: 'window' / 'linear' amplitudes, an integer hop), differentiable in
+  frequencies and amplitudes.  One backward call of `ddsp_b200_sinusoidal_backward`
+  (csrc/sinusoidal.cuh); d frequencies, the phase path, only when asked for.  The
+  Nyquist mask has subgradient 0 (tf.where)."""
+
+  @staticmethod
+  def forward(ctx, frequencies, amplitudes, n_samples, sample_rate, amp_resample_method):
+    frequencies = core.torch_float32(frequencies)
+    amplitudes = core.torch_float32(amplitudes)
+    ctx.save_for_backward(frequencies, amplitudes)
+    ctx.cfg = (int(n_samples), float(sample_rate), amp_resample_method)
+    return core.sinusoidal_synthesis(frequencies, amplitudes, n_samples=n_samples,
+                                     sample_rate=sample_rate,
+                                     amp_resample_method=amp_resample_method)
+
+  @staticmethod
+  def backward(ctx, grad_audio):
+    frequencies, amplitudes = ctx.saved_tensors
+    n_samples, sample_rate, method = ctx.cfg
+    b, f, k = amplitudes.shape
+    g = grad_audio.contiguous().to(torch.float32)
+    lib = _lib.load()
+    with core._on_device_of(frequencies, amplitudes, g):
+      d_amp = torch.empty_like(amplitudes)
+      d_freq = torch.empty_like(frequencies) if ctx.needs_input_grad[0] else None
+      nbytes = lib.ddsp_b200_sinusoidal_backward_workspace(b, f, k)
+      ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=amplitudes.device)
+      _lib.check(lib.ddsp_b200_sinusoidal_backward(
+          frequencies.data_ptr(), amplitudes.data_ptr(), g.data_ptr(), core._ptr(d_freq),
+          d_amp.data_ptr(), b, f, k, n_samples, sample_rate, core.AMP_METHODS[method],
+          ws.data_ptr(), nbytes, _stream()))
+    return d_freq, d_amp if ctx.needs_input_grad[1] else None, None, None, None
 
 
 class ModDelayFn(torch.autograd.Function):

@@ -506,16 +506,26 @@ def sinusoidal_synthesis(frequencies, amplitudes, n_samples: int = 64000,
   """Frame-rate bank of sinusoids with per-sinusoid frequencies
   [batch, n_frames, n_sinusoids] -> audio [batch, n_samples]: the fused form of
   resample + resample + core.oscillator_bank (synths.py:305-323) - the
-  [batch, n_samples, n_sinusoids] envelopes are never materialised."""
+  [batch, n_samples, n_sinusoids] envelopes are never materialised.  Routes to
+  `autograd.SinusoidalSynthesisFn` when grad is enabled and an input requires
+  it; `out=` / `accumulate=` are refused there."""
   sf, sa = _shape(frequencies), _shape(amplitudes)
   if len(sf) != 3 or sf != sa:
     raise ValueError(f'frequencies {sf} and amplitudes {sa} must both be '
                      '[batch, n_frames, n_sinusoids].')
   b, f, k = sf
   n_samples = int(n_samples)
+  if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad
+                                     for t in (frequencies, amplitudes)):
+    if out is not None or accumulate:
+      raise ValueError('sinusoidal_synthesis: out= and accumulate= write audio that '
+                       'autograd cannot track; they are not available when an input '
+                       'requires grad.')
+    from ddsp_b200 import autograd as _ag
+    return _ag.SinusoidalSynthesisFn.apply(frequencies, amplitudes, n_samples,
+                                           sample_rate, amp_resample_method)
   freqs = torch_float32(frequencies)
   amps = torch_float32(amplitudes)
-  _no_grad_path('sinusoidal_synthesis', freqs, amps)
   if out is None:
     out = torch.empty((b, n_samples), dtype=torch.float32, device=freqs.device)
     accumulate = False

@@ -971,6 +971,49 @@ size_t ddsp_b200_sinusoidal_workspace(int B, int F, int K) {
   return sizeof(unsigned long long) * (size_t)B * n_tiles * K + 256;
 }
 
+// The shape, method and workspace checks shared by the forward and the backward;
+// `name` prefixes the messages.  The caller returns 0 for B == 0 afterwards.
+static int sinus_check(const char* name, int B, int F, int K, int N, float sample_rate,
+                       int amp_method, const void* workspace, size_t workspace_bytes,
+                       size_t need) {
+  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1 && N >= 1, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d F=%d K=%d N=%d", name, B, F, K, N);
+  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW || amp_method == DDSP_B200_AMP_LINEAR,
+               DDSP_B200_E_INVALID, "%s: bad amp_method %d", name, amp_method);
+  DDSP_REQUIRE(N % F == 0, DDSP_B200_E_INVALID,
+               "%s: n_samples (%d) must be divisible by the number "
+               "of frames (%d)", name, N, F);
+  DDSP_REQUIRE(amp_method != DDSP_B200_AMP_WINDOW || F < N, DDSP_B200_E_INVALID,
+               "%s: window upsampling cannot downsample (frames %d "
+               ">= timesteps %d)", name, F, N);
+  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
+               "%s: sample_rate must be positive", name);
+  if (B == 0) return 0;
+  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
+               "%s: B=%d exceeds the 65535 grid limit", name, B);
+  DDSP_REQUIRE(sf_smem(sinus_tile_frames(F, K), K).total <= kMaxDynSmem,
+               DDSP_B200_E_UNSUPPORTED,
+               "%s: K=%d needs more shared memory than one CTA has", name, K);
+  DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
+               "%s: workspace of %zu B needed, %zu given", name, need, workspace_bytes);
+  return 0;
+}
+
+// Passes 1-2: the exclusive scan of the tile phase totals, into the workspace.
+static int sinus_tile_offsets(const float* frequencies, unsigned long long* sums, int B,
+                              int F, int K, int hop, int FT, double inv_sr,
+                              cudaStream_t st, const char* name) {
+  const int n_tiles = (F + FT - 1) / FT;
+  sinus_tile_sums<<<dim3(n_tiles, B), kSfThreads, 0, st>>>(frequencies, sums, F, K, hop,
+                                                           FT, n_tiles, inv_sr);
+  DDSP_CHECK_LAUNCH(name);
+  const int64_t BK = (int64_t)B * K;
+  oscbank_scan_chunks<<<(int)((BK + kObThreads - 1) / kObThreads), kObThreads, 0, st>>>(
+      sums, K, n_tiles, BK);
+  DDSP_CHECK_LAUNCH(name);
+  return 0;
+}
+
 int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitudes,
                                  float* audio, int B, int F, int K, int N,
                                  float sample_rate, int amp_method, int accumulate,
@@ -978,29 +1021,11 @@ int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitud
                                  void* stream) {
   DDSP_REQUIRE(frequencies && amplitudes && audio, DDSP_B200_E_INVALID,
                "sinusoidal_forward: null pointer");
-  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1 && N >= 1, DDSP_B200_E_INVALID,
-               "sinusoidal_forward: bad shape B=%d F=%d K=%d N=%d", B, F, K, N);
-  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW || amp_method == DDSP_B200_AMP_LINEAR,
-               DDSP_B200_E_INVALID, "sinusoidal_forward: bad amp_method %d", amp_method);
-  DDSP_REQUIRE(N % F == 0, DDSP_B200_E_INVALID,
-               "sinusoidal_forward: n_samples (%d) must be divisible by the number "
-               "of frames (%d)", N, F);
-  DDSP_REQUIRE(amp_method != DDSP_B200_AMP_WINDOW || F < N, DDSP_B200_E_INVALID,
-               "sinusoidal_forward: window upsampling cannot downsample (frames %d "
-               ">= timesteps %d)", F, N);
-  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
-               "sinusoidal_forward: sample_rate must be positive");
-  if (B == 0) return 0;
-  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
-               "sinusoidal_forward: B=%d exceeds the 65535 grid limit", B);
+  int rc = sinus_check("sinusoidal_forward", B, F, K, N, sample_rate, amp_method, workspace,
+                       workspace_bytes, ddsp_b200_sinusoidal_workspace(B, F, K));
+  if (rc || B == 0) return rc;
   const int FT = sinus_tile_frames(F, K);
   const SfSmem L = sf_smem(FT, K);
-  DDSP_REQUIRE(L.total <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
-               "sinusoidal_forward: K=%d needs more shared memory than one CTA has", K);
-  const size_t need = ddsp_b200_sinusoidal_workspace(B, F, K);
-  DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
-               "sinusoidal_forward: workspace of %zu B needed, %zu given", need,
-               workspace_bytes);
   unsigned long long* sums = reinterpret_cast<unsigned long long*>(
       ((uintptr_t)workspace + 255) & ~(uintptr_t)255);
   const int n_tiles = (F + FT - 1) / FT;
@@ -1008,27 +1033,68 @@ int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitud
   const double inv_sr = 1.0 / (double)sample_rate;
   cudaStream_t st = (cudaStream_t)stream;
   dim3 grid(n_tiles, B);
-  sinus_tile_sums<<<grid, kSfThreads, 0, st>>>(frequencies, sums, F, K, hop, FT, n_tiles,
-                                              inv_sr);
-  DDSP_CHECK_LAUNCH("sinusoidal_forward(tile sums)");
-  const int64_t BK = (int64_t)B * K;
-  oscbank_scan_chunks<<<(int)((BK + kObThreads - 1) / kObThreads), kObThreads, 0, st>>>(
-      sums, K, n_tiles, BK);
-  DDSP_CHECK_LAUNCH("sinusoidal_forward(scan)");
+  rc = sinus_tile_offsets(frequencies, sums, B, F, K, hop, FT, inv_sr, st,
+                          "sinusoidal_forward(tile offsets)");
+  if (rc) return rc;
   if (amp_method == DDSP_B200_AMP_WINDOW) {
-    int rc = set_smem(sinus_apply<true>, L.total, "sinusoidal_forward");
+    rc = set_smem(sinus_apply<true>, L.total, "sinusoidal_forward");
     if (rc) return rc;
     sinus_apply<true><<<grid, kSfThreads, L.total, st>>>(
         frequencies, amplitudes, sums, audio, F, K, N, hop, FT, n_tiles, inv_sr,
         sample_rate * 0.5f, accumulate);
   } else {
-    int rc = set_smem(sinus_apply<false>, L.total, "sinusoidal_forward");
+    rc = set_smem(sinus_apply<false>, L.total, "sinusoidal_forward");
     if (rc) return rc;
     sinus_apply<false><<<grid, kSfThreads, L.total, st>>>(
         frequencies, amplitudes, sums, audio, F, K, N, hop, FT, n_tiles, inv_sr,
         sample_rate * 0.5f, accumulate);
   }
   DDSP_CHECK_LAUNCH("sinusoidal_forward(apply)");
+  return 0;
+}
+
+size_t ddsp_b200_sinusoidal_backward_workspace(int B, int F, int K) {
+  if (B <= 0 || F <= 0 || K <= 0) return 0;
+  return ddsp_b200_sinusoidal_workspace(B, F, K) + sizeof(float) * 5 * (size_t)B * F * K +
+         256;
+}
+
+int ddsp_b200_sinusoidal_backward(const float* frequencies, const float* amplitudes,
+                                  const float* grad_audio, float* d_frequencies,
+                                  float* d_amplitudes, int B, int F, int K, int N,
+                                  float sample_rate, int amp_method, void* workspace,
+                                  size_t workspace_bytes, void* stream) {
+  DDSP_REQUIRE(frequencies && amplitudes && grad_audio && d_amplitudes, DDSP_B200_E_INVALID,
+               "sinusoidal_backward: null pointer");
+  int rc = sinus_check("sinusoidal_backward", B, F, K, N, sample_rate, amp_method,
+                       workspace, workspace_bytes,
+                       ddsp_b200_sinusoidal_backward_workspace(B, F, K));
+  if (rc || B == 0) return rc;
+  const int FT = sinus_tile_frames(F, K);
+  const int n_tiles = (F + FT - 1) / FT;
+  const int hop = N / F;
+  const double inv_sr = 1.0 / (double)sample_rate;
+  cudaStream_t st = (cudaStream_t)stream;
+  unsigned long long* sums = reinterpret_cast<unsigned long long*>(
+      ((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  float* part = reinterpret_cast<float*>(
+      ((uintptr_t)(sums + (size_t)B * n_tiles * K) + 255) & ~(uintptr_t)255);
+  rc = sinus_tile_offsets(frequencies, sums, B, F, K, hop, FT, inv_sr, st,
+                          "sinusoidal_backward(tile offsets)");
+  if (rc) return rc;
+  const int64_t BFK = (int64_t)B * F * K;
+  const unsigned n_blocks = (unsigned)((BFK + 31) / 32);
+  const bool phase = d_frequencies != nullptr;
+  auto kern = amp_method == DDSP_B200_AMP_WINDOW
+                  ? (phase ? sinus_bwd_frames<true, true> : sinus_bwd_frames<true, false>)
+                  : (phase ? sinus_bwd_frames<false, true> : sinus_bwd_frames<false, false>);
+  kern<<<n_blocks, kSbThreads, 0, st>>>(frequencies, amplitudes, grad_audio, sums, part, F,
+                                        K, N, hop, FT, n_tiles, BFK, inv_sr,
+                                        sample_rate * 0.5f);
+  DDSP_CHECK_LAUNCH("sinusoidal_backward(frames)");
+  sinus_bwd_finalize<<<dim3((K + 31) / 32, B), 32 * kSfinWarps, 0, st>>>(
+      part, d_amplitudes, d_frequencies, F, K, hop, BFK, inv_sr);
+  DDSP_CHECK_LAUNCH("sinusoidal_backward(finalize)");
   return 0;
 }
 

@@ -137,4 +137,180 @@ sinus_apply(const float* __restrict__ f, const float* __restrict__ a,
   }
 }
 
+// ---------------------------------------------------------------------------
+// Backward.  For one (b, k), upstream gradient g, s = sin 2 pi phi, m the
+// forward's own float32 Nyquist decision and c = g m amp 2 pi cos 2 pi phi:
+//   G0_i = sum_{t in i} g m s w0(r),  G1_i = sum_{t in i} g m s w1(r)
+//   d A_i = G0_i + G1_{i-1}  (+ G1_{F-1} on the last frame, frame F := F-1)
+// and with p1(r) = r(r+1)/(2 hop), p0(r) = (r+1) - p1(r), S_i = sum c,
+// Q0_i = sum c p0, Q1_i = sum c p1 (sr phi is linear in the frame frequencies:
+// alpha = (hop+1)/2, beta = (hop-1)/2 weigh the completed frames):
+//   sr d f_j = (alpha + beta [j>=1]) sum_{i>j} S_i + beta [j>=1] S_j + Q0_j
+//              + Q1_{j-1} [j>=1] + Q1_{F-1} [j == F-1].
+// Two passes after the forward's passes 1-2 (the tile phase offsets):
+//   4. sinus_bwd_frames: a CTA owns 32 consecutive (b, i, k) (one per lane) and
+//      splits the frame's hop samples into kSbWarps contiguous segments, one per
+//      warp.  A segment starts from the closed-form fixed-point phase and steps
+//      it by exact wrapping adds, so every phase is bit-identical to the
+//      forward's.  The warps' float partials are summed in warp order through
+//      shared memory: G0, G1 (and S, Q0, Q1) per (b, i, k) are written once.
+//   5. sinus_bwd_finalize: d A, and the frame-rate suffix sum of S and d f in
+//      double, per (b, k) over frame chunks combined in a fixed order.
+// No atomics, no memset: the gradients are bit-reproducible.  Without d f
+// (PHASE false) there is no cos, no S/Q sum and no scan.
+// ---------------------------------------------------------------------------
+constexpr int kSbWarps = 4;
+constexpr int kSbThreads = 32 * kSbWarps;
+
+template <bool WINDOW, bool PHASE>
+__global__ void __launch_bounds__(kSbThreads)
+sinus_bwd_frames(const float* __restrict__ f, const float* __restrict__ a,
+                 const float* __restrict__ g, const unsigned long long* __restrict__ offs,
+                 float* __restrict__ part /* [5][B*F*K]: G0, G1, S, Q0, Q1 */,
+                 int F, int K, int N, int hop, int FT, int n_tiles, int64_t BFK,
+                 double inv_sr, float nyquist) {
+  __shared__ float red[kSbWarps - 1][PHASE ? 5 : 2][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t p = (int64_t)blockIdx.x * 32 + lane;          // flat (b, i, k)
+  const bool live = p < BFK;
+  const int64_t pc = live ? p : BFK - 1;
+  const int k = (int)(pc % K);
+  const int64_t bi = pc / K;
+  const int i = (int)(bi % F), b = (int)(bi / F);
+  const int tile = i / FT, inx = min(i + 1, F - 1);
+  const float* fb = f + (size_t)b * F * K + k;
+
+  // the frame's phase: the tile offset plus the tile's frames before i
+  unsigned long long P = offs[((size_t)b * n_tiles + tile) * K + k];
+  for (int j = tile * FT; j < i; ++j)
+    P += sf_frame_total(fb[(size_t)j * K], fb[(size_t)(j + 1) * K], hop, inv_sr);
+  const float lo = fb[(size_t)i * K], hi = fb[(size_t)inx * K];
+  const double a0 = (double)lo * inv_sr, a1 = (double)hi * inv_sr;
+  const unsigned long long A = turns_to_fix64(a0);
+  const unsigned long long D = turns_to_fix64((a1 - a0) / (double)hop);
+  const float am0 = PHASE ? a[(size_t)bi * K + k] : 0.f;
+  const float am1 = PHASE ? a[((size_t)b * F + inx) * K + k] : 0.f;
+
+  // this warp's segment [r0, r1) of the frame
+  const int seg = (hop + kSbWarps - 1) / kSbWarps;
+  const int r0 = min(hop, warp * seg), r1 = min(hop, r0 + seg);
+  const unsigned long long ur0 = (unsigned long long)r0;
+  unsigned long long ph = P + 0x80000000ull + (ur0 + 1) * A + ((ur0 * (ur0 + 1)) >> 1) * D;
+  unsigned long long inc = A + (ur0 + 1) * D;                  // ph(r + 1) - ph(r)
+  const float inv_hop = 1.0f / (float)hop;
+  const float* gp = g + (size_t)b * N + (size_t)i * hop;
+  float G0 = 0.f, G1 = 0.f, S = 0.f, Q0 = 0.f, Q1 = 0.f;
+#pragma unroll 2
+  for (int r = r0; r < r1; ++r) {
+    const float frac = (float)r * inv_hop;
+    const float w1 = WINDOW ? (0.5f - 0.5f * cospif(frac)) : frac;
+    const float w0 = 1.0f - w1;
+    const float fe = __fadd_rn(lo, __fmul_rn(__fsub_rn(hi, lo), frac));   // as the forward
+    const float gm = (fe >= nyquist) ? 0.f : gp[r];
+    const float x = (float)(int)(uint32_t)(ph >> 32) * 4.656612873077393e-10f;
+    float s, c;
+    sincospif(x, &s, &c);        // one call on both paths: d A does not depend on PHASE
+    const float gs = gm * s;
+    G0 = fmaf(gs, w0, G0);
+    G1 = fmaf(gs, w1, G1);
+    if (PHASE) {
+      const float cc = gm * fmaf(am1, w1, am0 * w0) * c;
+      const float tri = (float)r * (float)(r + 1) * (0.5f * inv_hop);
+      S += cc;
+      Q0 = fmaf(cc, (float)(r + 1) - tri, Q0);
+      Q1 = fmaf(cc, tri, Q1);
+    }
+    ph += inc;
+    inc += D;
+  }
+
+  // segment partials, summed in warp order
+  if (warp > 0) {
+    red[warp - 1][0][lane] = G0;
+    red[warp - 1][1][lane] = G1;
+    if (PHASE) {
+      red[warp - 1][2][lane] = S;
+      red[warp - 1][3][lane] = Q0;
+      red[warp - 1][4][lane] = Q1;
+    }
+  }
+  __syncthreads();
+  if (warp == 0 && live) {
+#pragma unroll
+    for (int w = 0; w < kSbWarps - 1; ++w) {
+      G0 += red[w][0][lane];
+      G1 += red[w][1][lane];
+      if (PHASE) {
+        S += red[w][2][lane];
+        Q0 += red[w][3][lane];
+        Q1 += red[w][4][lane];
+      }
+    }
+    part[p] = G0;
+    part[BFK + p] = G1;
+    if (PHASE) {
+      part[2 * BFK + p] = S * 6.283185307179586f;
+      part[3 * BFK + p] = Q0 * 6.283185307179586f;
+      part[4 * BFK + p] = Q1 * 6.283185307179586f;
+    }
+  }
+}
+
+// pass 5.  A CTA owns one b and 32 sinusoids (one per lane); its warps own
+// contiguous frame chunks.  The suffix sum of S is the later chunks' totals,
+// added in warp order, then the running sum inside the chunk.  d_f may be NULL
+// (then S/Q were not computed).
+constexpr int kSfinWarps = 16;
+
+__global__ void __launch_bounds__(32 * kSfinWarps)
+sinus_bwd_finalize(const float* __restrict__ part, float* __restrict__ d_a,
+                   float* __restrict__ d_f, int F, int K, int hop, int64_t BFK,
+                   double inv_sr) {
+  __shared__ double tot[kSfinWarps][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int k = blockIdx.x * 32 + lane, b = blockIdx.y;
+  const bool live = k < K;
+  const int chunk = (F + kSfinWarps - 1) / kSfinWarps;
+  const int j0 = min(F, warp * chunk), j1 = min(F, j0 + chunk);
+  const size_t base = (size_t)b * F * K + (live ? k : 0);
+  const float* G0 = part + base;
+  const float* G1 = G0 + BFK;
+  float* da = d_a + base;
+  if (live) {
+#pragma unroll 4
+    for (int j = j0; j < j1; ++j) {
+      float v = G0[(size_t)j * K];
+      if (j >= 1) v += G1[(size_t)(j - 1) * K];
+      if (j == F - 1) v += G1[(size_t)j * K];
+      da[(size_t)j * K] = v;
+    }
+  }
+  if (d_f == nullptr) return;
+  const float* S = G1 + BFK;
+  const float* Q0 = S + BFK;
+  const float* Q1 = Q0 + BFK;
+  float* df = d_f + base;
+  double t = 0.0;
+  if (live) {
+#pragma unroll 4
+    for (int j = j0; j < j1; ++j) t += (double)S[(size_t)j * K];
+  }
+  tot[warp][lane] = t;
+  __syncthreads();
+  if (!live) return;
+  const double alpha = 0.5 * (double)(hop + 1), beta = 0.5 * (double)(hop - 1);
+  double suf = 0.0;                                            // sum_{i>j} S_i
+  for (int w = kSfinWarps - 1; w > warp; --w) suf += tot[w][lane];
+#pragma unroll 4
+  for (int j = j1 - 1; j >= j0; --j) {
+    const double s = (double)S[(size_t)j * K];
+    double v = (double)Q0[(size_t)j * K];
+    if (j >= 1) v += (alpha + beta) * suf + beta * s + (double)Q1[(size_t)(j - 1) * K];
+    else v += alpha * suf;
+    if (j == F - 1) v += (double)Q1[(size_t)j * K];
+    df[(size_t)j * K] = (float)(v * inv_sr);
+    suf += s;
+  }
+}
+
 }  // namespace ddsp

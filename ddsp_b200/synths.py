@@ -146,8 +146,9 @@ class Sinusoidal(processors.Processor):
 
   def get_signal(self, amplitudes, frequencies):
     """synths.py:305-323.  One fused frame-rate kernel when the hop is an integer
-    and the amplitudes are resampled by 'window' / 'linear'; otherwise the
-    reference's own decomposition on the stand-alone kernels."""
+    and the amplitudes are resampled by 'window' / 'linear' (differentiable in
+    both inputs); otherwise the reference's own decomposition on the stand-alone
+    kernels, which has no backward."""
     sa = core._shape(amplitudes)  # pylint: disable=protected-access
     if (self.amp_resample_method in core.AMP_METHODS and len(sa) == 3 and
         sa[1] > 0 and self.n_samples % sa[1] == 0 and
@@ -156,6 +157,8 @@ class Sinusoidal(processors.Processor):
           frequencies, amplitudes, n_samples=self.n_samples,
           sample_rate=self.sample_rate,
           amp_resample_method=self.amp_resample_method)
+    # the resampled envelopes would be detached: refuse rather than drop the gradient
+    core._no_grad_path('oscillator_bank', amplitudes, frequencies)  # pylint: disable=protected-access
     amplitude_envelopes = core.resample(amplitudes, self.n_samples,
                                         method=self.amp_resample_method)
     frequency_envelopes = core.resample(frequencies, self.n_samples)

@@ -305,6 +305,21 @@ int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitud
                                  void* workspace, size_t workspace_bytes,
                                  void* stream);
 
+/* Its backward: for the upstream gradient grad_audio [B,N], writes
+ * d_amplitudes [B,F,K] and, when d_frequencies [B,F,K] is not NULL, the
+ * gradient to the frequencies through the phase (a NULL d_frequencies skips
+ * the phase path: no cos, no phase sums, no frame scan).  The Nyquist mask is
+ * the forward's own float32 decision with subgradient 0, as tf.where gives.
+ * Same validation and error codes as the forward.  No atomics: the gradients
+ * are bit-reproducible.
+ * workspace: ddsp_b200_sinusoidal_backward_workspace(B,F,K) bytes. */
+size_t ddsp_b200_sinusoidal_backward_workspace(int B, int F, int K);
+int ddsp_b200_sinusoidal_backward(const float* frequencies, const float* amplitudes,
+                                  const float* grad_audio, float* d_frequencies,
+                                  float* d_amplitudes, int B, int F, int K, int N,
+                                  float sample_rate, int amp_method, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+
 /* core.resample / core.upsample_with_windows (core.py:573-714) stand-alone:
  * in [B,F,C] -> out [B,N,C].  method: 0 'window', 1 'linear', 2 'nearest',
  * 3 'cubic' (tf.compat.v1 bicubic, Keys A = -0.75).  add_endpoint as in the
