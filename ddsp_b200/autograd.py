@@ -31,10 +31,6 @@ from ddsp_b200 import _lib
 from ddsp_b200 import core
 
 
-def _stream():
-  return torch.cuda.current_stream().cuda_stream
-
-
 class HarmonicSynthesisFn(torch.autograd.Function):
   """core.harmonic_synthesis (core.py:1048-1111), differentiable in
   amplitudes and harmonic_distribution."""
@@ -62,7 +58,7 @@ class HarmonicSynthesisFn(torch.autograd.Function):
     g1 = torch.empty_like(hd)
     _lib.check(_lib.load().ddsp_b200_harmonic_backward(
         f0_hz.data_ptr(), grad_audio.data_ptr(), g0.data_ptr(), g1.data_ptr(),
-        b, f, k, n_samples, sample_rate, core.AMP_METHODS[method], _stream()))
+        b, f, k, n_samples, sample_rate, core.AMP_METHODS[method], core._stream()))
     # dL/d(amp * hd)[i] = g0[i] + g1[i-1], frame F being a copy of frame F-1
     dha = g0
     dha[:, 1:] += g1[:, :-1]
@@ -85,7 +81,7 @@ def _harmonic_d_f0(f0_hz, amplitudes, hd, grad_audio, n_samples, sample_rate, me
   _lib.check(_lib.load().ddsp_b200_harmonic_backward_f0(
       f0_hz.data_ptr(), amplitudes.data_ptr(), hd.data_ptr(), grad_audio.data_ptr(),
       d_f0.data_ptr(), b, f, k, n_samples, sample_rate, core.AMP_METHODS[method],
-      ws.data_ptr(), nbytes, _stream()))
+      ws.data_ptr(), nbytes, core._stream()))
   return d_f0
 
 
@@ -121,7 +117,7 @@ class DecoderFn(torch.autograd.Function):
     b, f, k = hd.shape
     nb = mags.shape[-1]
     lib = _lib.load()
-    st = _stream()
+    st = core._stream()
     g = grad_audio.contiguous().to(torch.float32)
     flags = _lib.CTL_SCALE | (_lib.CTL_NYQUIST if nyq else 0)
     # harmonic: sample-rate reductions, then get_controls transposed at frame rate
@@ -226,7 +222,7 @@ class FilteredNoiseFn(torch.autograd.Function):
     _lib.check(_lib.load().ddsp_b200_filtered_noise_backward(
         grad_audio.data_ptr(), 0 if ctx.noise is None else ctx.noise.data_ptr(),
         seed & (2**64 - 1), offset & (2**64 - 1), dmags.data_ptr(), b, f, nb,
-        n_samples, window_size, _stream()))
+        n_samples, window_size, core._stream()))
     return dmags, None, None, None, None, None
 
 
@@ -258,11 +254,11 @@ class SinusoidalSynthesisFn(torch.autograd.Function):
       d_amp = torch.empty_like(amplitudes)
       d_freq = torch.empty_like(frequencies) if ctx.needs_input_grad[0] else None
       nbytes = lib.ddsp_b200_sinusoidal_backward_workspace(b, f, k)
-      ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=amplitudes.device)
+      ws = core._workspace(nbytes, amplitudes.device)
       _lib.check(lib.ddsp_b200_sinusoidal_backward(
           frequencies.data_ptr(), amplitudes.data_ptr(), g.data_ptr(), core._ptr(d_freq),
           d_amp.data_ptr(), b, f, k, n_samples, sample_rate, core.AMP_METHODS[method],
-          ws.data_ptr(), nbytes, _stream()))
+          core._ptr(ws), nbytes, core._stream()))
     return d_freq, d_amp if ctx.needs_input_grad[1] else None, None, None, None
 
 
@@ -292,7 +288,7 @@ class ModDelayFn(torch.autograd.Function):
     _lib.check(_lib.load().ddsp_b200_mod_delay_backward(
         audio.data_ptr(), phase.data_ptr(), core._ptr(gain), g.data_ptr(),
         core._ptr(d_audio), core._ptr(d_gain), core._ptr(d_phase), b, n, max_length,
-        scale, offset, int(add_dry), _stream()))
+        scale, offset, int(add_dry), core._stream()))
     return d_audio, d_gain, d_phase, None, None, None, None
 
 

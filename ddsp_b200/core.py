@@ -98,6 +98,11 @@ def _stream():
   return torch.cuda.current_stream().cuda_stream
 
 
+def _workspace(nbytes, device):
+  """The scratch buffer a library call asked for, or None when it needs none."""
+  return torch.empty((nbytes,), dtype=torch.uint8, device=device) if nbytes else None
+
+
 class _on_device_of:
   """Context: make the device of the operands current (so the launch goes to
   THAT device's current stream), after checking they all live on one device."""
@@ -452,7 +457,7 @@ def angular_cumsum(angular_frequency, chunk_size: int = 1000,
           _stream()))
     else:
       nbytes = lib.ddsp_b200_oscillator_bank_workspace(b, n, max(c, 1))
-      ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=x3.device)
+      ws = _workspace(nbytes, x3.device)
       _lib.check(lib.ddsp_b200_angular_cumsum(
           _ptr(x3), _ptr(out), b, n, max(c, 1), int(chunk_size), 0, _ptr(ws),
           nbytes, _stream()))
@@ -492,7 +497,7 @@ def oscillator_bank(frequency_envelopes, amplitude_envelopes,
     out = torch.empty((b, n) if sum_sinusoids else (b, n, k), dtype=torch.float32,
                       device=f.device)
     nbytes = lib.ddsp_b200_oscillator_bank_workspace(b, n, k)
-    ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=f.device)
+    ws = _workspace(nbytes, f.device)
     _lib.check(lib.ddsp_b200_oscillator_bank(
         _ptr(f), _ptr(a), _ptr(out), b, n, k, float(sample_rate),
         int(bool(sum_sinusoids)), _ptr(ws), nbytes, _stream()))
@@ -534,7 +539,7 @@ def sinusoidal_synthesis(frequencies, amplitudes, n_samples: int = 64000,
   lib = _lib.load()
   with _on_device_of(freqs, amps, out):
     nbytes = lib.ddsp_b200_sinusoidal_workspace(b, f, k)
-    ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=freqs.device)
+    ws = _workspace(nbytes, freqs.device)
     _lib.check(lib.ddsp_b200_sinusoidal_forward(
         _ptr(freqs), _ptr(amps), _ptr(out), b, f, k, n_samples, float(sample_rate),
         AMP_METHODS[amp_resample_method], int(bool(accumulate)), _ptr(ws), nbytes,
@@ -866,7 +871,7 @@ def fft_convolve_lti(audio, impulse_response, start, out_len, out=None,
            (_lib.LTI_REVERSE_IR if reverse_ir else 0))
   with _on_device_of(audio, impulse_response, out):
     nbytes = lib.ddsp_b200_fft_convolve_lti_workspace(b, n, s_len, ir_batch)
-    ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=audio.device)
+    ws = _workspace(nbytes, audio.device)
     _lib.check(lib.ddsp_b200_fft_convolve_lti(
         _ptr(audio), _ptr(impulse_response), _ptr(out), b, n, s_len, ir_batch,
         int(start), int(out_len), int(bool(accumulate)), flags, _ptr(ws), nbytes,
@@ -1090,8 +1095,7 @@ def filtered_noise(magnitudes, n_samples, window_size=257, noise=None, seed=0,
   with _on_device_of(magnitudes, noise, out):
     ws_bytes = lib.ddsp_b200_filtered_noise_workspace(b, f, nb, n_samples,
                                                       int(window_size))
-    workspace = (torch.empty((ws_bytes,), dtype=torch.uint8,
-                             device=magnitudes.device) if ws_bytes else None)
+    workspace = _workspace(ws_bytes, magnitudes.device)
     _lib.check(lib.ddsp_b200_filtered_noise_forward(
         _ptr(magnitudes), _ptr(noise), int(seed) & (2**64 - 1),
         int(offset) & (2**64 - 1), _ptr(out), b, f, nb, n_samples,

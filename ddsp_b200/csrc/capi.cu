@@ -43,20 +43,61 @@ static inline int grid_for(int64_t n, int threads, int cap_per_sm = 8) {
   return (int)std::max<int64_t>(1, std::min(blocks, cap));
 }
 
-static constexpr size_t kMaxDynSmem = 200 * 1024;  // of 227 KB usable per CTA
-
-template <typename K>
-static int set_smem(K kernel, size_t bytes, const char* name) {
-  if (bytes > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(
-        kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) {
-      set_error("%s: cannot reserve %zu B of shared memory: %s", name, bytes,
-                cudaGetErrorString(e));
-      return DDSP_B200_E_CUDA;
-    }
-  }
+// The checks every harmonic entry point makes; `name` prefixes the messages.
+static int harm_check(const char* name, int B, int F, int K, int N, int amp_method,
+                      float sample_rate) {
+  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1 && N >= 1, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d F=%d K=%d N=%d", name, B, F, K, N);
+  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW || amp_method == DDSP_B200_AMP_LINEAR,
+               DDSP_B200_E_INVALID, "%s: bad amp_method %d", name, amp_method);
+  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
+               "%s: sample_rate must be positive", name);
   return 0;
+}
+
+// HarmonicParams of a harmonic entry point.  The caller sets the fields in which it
+// differs: accumulate, ctl_flags, the phase pointers, mask_nyquist and Kp.
+static HarmonicParams harm_params(const float* f0, const float* amps, const float* hd,
+                                  float* audio, int B, int F, int K, int N,
+                                  float sample_rate, int amp_method) {
+  HarmonicParams p;
+  p.f0 = f0; p.amps = amps; p.hd = hd; p.audio = audio;
+  p.B = B; p.F = F; p.K = K; p.N = N; p.hop = N / F;
+  p.sample_rate = sample_rate; p.nyquist = sample_rate * 0.5f;
+  p.inv_sr = 1.0 / (double)sample_rate;
+  p.amp_method = amp_method; p.accumulate = 0; p.ctl_flags = 0;
+  p.init_phase = nullptr; p.final_phase = nullptr; p.mask_nyquist = 1;
+  p.Kp = (K + 3) & ~3;
+  return p;
+}
+
+// Halves the frames per tile from FT until smem(FT, Kp) fits one CTA.  Returns the
+// tile, or 0 with the error set when not even one frame fits.
+static int fit_tile(const char* name, int FT, int K, int Kp, size_t (*smem)(int, int)) {
+  while (FT > 1 && smem(FT, Kp) > kMaxDynSmem) FT = (FT + 1) / 2;
+  DDSP_REQUIRE(smem(FT, Kp) <= kMaxDynSmem, 0,
+               "%s: K=%d needs more shared memory than one CTA has", name, K);
+  return FT;
+}
+
+// core.py:1446-1457: F impulse responses over N samples have frames of ceil(N / F)
+// samples, and framing the audio with that size (pad_end) must give F frames.
+// Returns the frame size, or 0 with the error set.
+static int ir_frame(int N, int F) {
+  const int frame = (N + F - 1) / F;
+  const int n_audio_frames = (N + frame - 1) / frame;
+  DDSP_REQUIRE(n_audio_frames == F, 0,
+               "Number of Audio frames (%d) and impulse response frames (%d) do "
+               "not match. For small hop size = ceil(audio_size / n_ir_frames), "
+               "number of impulse response frames must be a multiple of the "
+               "audio size.", n_audio_frames, F);
+  return frame;
+}
+
+// Workspaces are carved from the first 256-byte boundary at or after `p`.
+template <typename T>
+static T* align256(const void* p) {
+  return reinterpret_cast<T*>(((uintptr_t)p + 255) & ~(uintptr_t)255);
 }
 
 }  // namespace ddsp
@@ -98,14 +139,10 @@ int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
                                int phase_mode, int accumulate, void* stream) {
   DDSP_REQUIRE(f0_hz && amps && audio, DDSP_B200_E_INVALID,
                "harmonic_forward: null pointer");
-  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1 && N >= 1, DDSP_B200_E_INVALID,
-               "harmonic_forward: bad shape B=%d F=%d K=%d N=%d", B, F, K, N);
+  int rc = harm_check("harmonic_forward", B, F, K, N, amp_method, sample_rate);
+  if (rc) return rc;
   DDSP_REQUIRE(hd != nullptr || K == 1, DDSP_B200_E_INVALID,
                "harmonic_forward: harmonic_distribution is NULL but K=%d", K);
-  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW ||
-                   amp_method == DDSP_B200_AMP_LINEAR,
-               DDSP_B200_E_INVALID, "harmonic_forward: bad amp_method %d",
-               amp_method);
   DDSP_REQUIRE(phase_mode == DDSP_B200_PHASE_RECURRENCE ||
                    phase_mode == DDSP_B200_PHASE_DIRECT,
                DDSP_B200_E_INVALID, "harmonic_forward: bad phase_mode %d",
@@ -119,52 +156,34 @@ int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
                DDSP_B200_E_INVALID,
                "harmonic_forward: window upsampling cannot downsample "
                "(frames %d >= timesteps %d)", F, N);
-  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
-               "harmonic_forward: sample_rate must be positive");
   if (B == 0) return 0;
   DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
                "harmonic_forward: B=%d exceeds the 65535 grid limit", B);
 
-  HarmonicParams p;
-  p.f0 = f0_hz; p.amps = amps; p.hd = hd; p.audio = audio;
-  p.B = B; p.F = F; p.K = K; p.N = N; p.hop = N / F;
-  p.sample_rate = sample_rate;
-  p.nyquist = sample_rate * 0.5f;
-  p.inv_sr = 1.0 / (double)sample_rate;
-  p.amp_method = amp_method;
+  HarmonicParams p = harm_params(f0_hz, amps, hd, audio, B, F, K, N, sample_rate,
+                                 amp_method);
   p.accumulate = accumulate;
-  p.ctl_flags = 0;
-  p.init_phase = nullptr; p.final_phase = nullptr; p.mask_nyquist = 1;
   cudaStream_t st = (cudaStream_t)stream;
 
   if (phase_mode == DDSP_B200_PHASE_RECURRENCE && harmonic_fused_supported(p)) {
-    int rc = launch_harmonic_v4(p, st);
+    rc = launch_harmonic_v4(p, st);
     if (rc != 1) return rc;   // 1 = declined, fall through to the generic path
   }
 
-  p.Kp = (K + 3) & ~3;
   // frames per tile: ~2048 samples, enough CTAs to fill the chip, bounded smem
   int FT = std::max(1, 2048 / p.hop);
   const int64_t want_ctas = 4ll * num_sms();
   int ft_fill = (int)std::max<int64_t>(1, ((int64_t)B * F + want_ctas - 1) / want_ctas);
   FT = std::min(FT, std::max(ft_fill, std::min(4, F)));
   FT = std::min(FT, F);
-  while (FT > 1 && harm_smem_bytes(FT, p.Kp) > kMaxDynSmem) FT = (FT + 1) / 2;
-  DDSP_REQUIRE(harm_smem_bytes(FT, p.Kp) <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
-               "harmonic_forward: K=%d needs more shared memory than one CTA has",
-               K);
-  p.FT = FT;
-  const size_t smem = harm_smem_bytes(FT, p.Kp);
-  dim3 grid((F + FT - 1) / FT, B);
-  if (phase_mode == DDSP_B200_PHASE_DIRECT) {
-    int rc = set_smem(harmonic_generic_kernel<1>, smem, "harmonic_forward");
-    if (rc) return rc;
-    harmonic_generic_kernel<1><<<grid, kHarmThreads, smem, st>>>(p);
-  } else {
-    int rc = set_smem(harmonic_generic_kernel<0>, smem, "harmonic_forward");
-    if (rc) return rc;
-    harmonic_generic_kernel<0><<<grid, kHarmThreads, smem, st>>>(p);
-  }
+  p.FT = fit_tile("harmonic_forward", FT, K, p.Kp, harm_smem_bytes);
+  if (!p.FT) return DDSP_B200_E_UNSUPPORTED;
+  const size_t smem = harm_smem_bytes(p.FT, p.Kp);
+  auto kern = phase_mode == DDSP_B200_PHASE_DIRECT ? harmonic_generic_kernel<1>
+                                                   : harmonic_generic_kernel<0>;
+  rc = set_smem(kern, smem, "harmonic_forward");
+  if (rc) return rc;
+  kern<<<dim3((F + p.FT - 1) / p.FT, B), kHarmThreads, smem, st>>>(p);
   DDSP_CHECK_LAUNCH("harmonic_forward");
   return 0;
 }
@@ -176,39 +195,26 @@ int ddsp_b200_streaming_harmonic_forward(const float* f0_hz, const float* amps,
                                          int amp_method, void* stream) {
   DDSP_REQUIRE(f0_hz && amps && audio, DDSP_B200_E_INVALID,
                "streaming_harmonic_forward: null pointer");
-  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1 && N >= 1, DDSP_B200_E_INVALID,
-               "streaming_harmonic_forward: bad shape B=%d F=%d K=%d N=%d", B, F, K, N);
+  int rc = harm_check("streaming_harmonic_forward", B, F, K, N, amp_method, sample_rate);
+  if (rc) return rc;
   DDSP_REQUIRE(hd != nullptr || K == 1, DDSP_B200_E_INVALID,
                "streaming_harmonic_forward: harmonic_distribution is NULL but K=%d", K);
-  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW ||
-                   amp_method == DDSP_B200_AMP_LINEAR,
-               DDSP_B200_E_INVALID, "streaming_harmonic_forward: bad amp_method %d",
-               amp_method);
   DDSP_REQUIRE(N % F == 0, DDSP_B200_E_INVALID,
                "streaming_harmonic_forward: n_samples (%d) must be divisible by "
                "the number of frames (%d)", N, F);
-  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
-               "streaming_harmonic_forward: sample_rate must be positive");
   if (B == 0) return 0;
   DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
                "streaming_harmonic_forward: B=%d exceeds the 65535 grid limit", B);
-  HarmonicParams p;
-  p.f0 = f0_hz; p.amps = amps; p.hd = hd; p.audio = audio;
-  p.B = B; p.F = F; p.K = K; p.N = N; p.hop = N / F;
-  p.sample_rate = sample_rate; p.nyquist = sample_rate * 0.5f;
-  p.inv_sr = 1.0 / (double)sample_rate;
-  p.amp_method = amp_method; p.accumulate = 0; p.ctl_flags = 0;
+  HarmonicParams p = harm_params(f0_hz, amps, hd, audio, B, F, K, N, sample_rate,
+                                 amp_method);
   p.init_phase = initial_phase; p.final_phase = final_phase; p.mask_nyquist = 0;
-  p.Kp = (K + 3) & ~3;
-  int FT = std::max(1, std::min(F, 2048 / p.hop));
-  while (FT > 1 && harm_smem_bytes(FT, p.Kp) > kMaxDynSmem) FT = (FT + 1) / 2;
-  DDSP_REQUIRE(harm_smem_bytes(FT, p.Kp) <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
-               "streaming_harmonic_forward: K=%d needs too much shared memory", K);
-  p.FT = FT;
-  const size_t smem = harm_smem_bytes(FT, p.Kp);
-  int rc = set_smem(harmonic_generic_kernel<0>, smem, "streaming_harmonic_forward");
+  p.FT = fit_tile("streaming_harmonic_forward", std::max(1, std::min(F, 2048 / p.hop)),
+                  K, p.Kp, harm_smem_bytes);
+  if (!p.FT) return DDSP_B200_E_UNSUPPORTED;
+  const size_t smem = harm_smem_bytes(p.FT, p.Kp);
+  rc = set_smem(harmonic_generic_kernel<0>, smem, "streaming_harmonic_forward");
   if (rc) return rc;
-  dim3 grid((F + FT - 1) / FT, B);
+  dim3 grid((F + p.FT - 1) / p.FT, B);
   harmonic_generic_kernel<0><<<grid, kHarmThreads, smem, (cudaStream_t)stream>>>(p);
   DDSP_CHECK_LAUNCH("streaming_harmonic_forward");
   return 0;
@@ -269,14 +275,8 @@ int ddsp_b200_fir_time_varying(const float* audio, const float* ir, float* out,
   DDSP_REQUIRE(padding == DDSP_B200_PAD_SAME || padding == DDSP_B200_PAD_VALID,
                DDSP_B200_E_INVALID,
                "Padding must be 'valid' or 'same' (got code %d)", padding);
-  // core.py:1446-1457: frame = ceil(N / F); frame(pad_end) must yield F frames
-  const int frame = (N + F - 1) / F;
-  const int n_audio_frames = (N + frame - 1) / frame;
-  DDSP_REQUIRE(n_audio_frames == F, DDSP_B200_E_INVALID,
-               "Number of Audio frames (%d) and impulse response frames (%d) do "
-               "not match. For small hop size = ceil(audio_size / n_ir_frames), "
-               "number of impulse response frames must be a multiple of the "
-               "audio size.", n_audio_frames, F);
+  const int frame = ir_frame(N, F);
+  if (!frame) return DDSP_B200_E_INVALID;
   if (B == 0) return 0;
   DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
                "fir_time_varying: B=%d exceeds the 65535 grid limit", B);
@@ -334,13 +334,7 @@ int ddsp_b200_filtered_noise_forward(const float* mags, const float* noise,
                "filtered_noise_forward: bad shape B=%d F=%d N=%d", B, F, N);
   DDSP_REQUIRE(nb >= 2, DDSP_B200_E_INVALID,
                "filtered_noise_forward: need n_frequencies >= 2 (got %d)", nb);
-  const int frame = (N + F - 1) / F;
-  const int n_audio_frames = (N + frame - 1) / frame;
-  DDSP_REQUIRE(n_audio_frames == F, DDSP_B200_E_INVALID,
-               "Number of Audio frames (%d) and impulse response frames (%d) do "
-               "not match. For small hop size = ceil(audio_size / n_ir_frames), "
-               "number of impulse response frames must be a multiple of the "
-               "audio size.", n_audio_frames, F);
+  if (!ir_frame(N, F)) return DDSP_B200_E_INVALID;
   if (B == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (noise_fused_supported(F, nb, N, window_size)) {
@@ -353,8 +347,7 @@ int ddsp_b200_filtered_noise_forward(const float* mags, const float* noise,
                "filtered_noise_forward: workspace of %zu B needed, %zu given",
                need, workspace_bytes);
   IrGeom g = make_ir_geom(nb, window_size);
-  uintptr_t base = ((uintptr_t)workspace + 255) & ~(uintptr_t)255;
-  float* ir = reinterpret_cast<float*>(base);
+  float* ir = align256<float>(workspace);
   float* nz = ir + (size_t)B * F * g.S;
   int rc = ddsp_b200_frequency_impulse_response(mags, ir, (int64_t)B * F, nb,
                                                 window_size, stream);
@@ -378,31 +371,18 @@ static int decoder_forward_impl(const float* amps_raw, const float* hd_raw,
                                 float initial_bias, void* stream, int item_base) {
   DDSP_REQUIRE(amps_raw && hd_raw && f0_hz && mags_raw && audio,
                DDSP_B200_E_INVALID, "decoder_forward: null pointer");
-  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1 && N >= 1 && nb >= 2,
-               DDSP_B200_E_INVALID,
-               "decoder_forward: bad shape B=%d F=%d K=%d nb=%d N=%d", B, F, K,
-               nb, N);
-  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW ||
-                   amp_method == DDSP_B200_AMP_LINEAR,
-               DDSP_B200_E_INVALID, "decoder_forward: bad amp_method %d",
-               amp_method);
+  int rc = harm_check("decoder_forward", B, F, K, N, amp_method, sample_rate);
+  if (rc) return rc;
+  DDSP_REQUIRE(nb >= 2, DDSP_B200_E_INVALID,
+               "decoder_forward: need n_frequencies >= 2 (got %d)", nb);
   DDSP_REQUIRE(harmonic_flags != 0 &&
                    (harmonic_flags & ~(DDSP_B200_CTL_SCALE | DDSP_B200_CTL_NYQUIST)) == 0,
                DDSP_B200_E_INVALID, "decoder_forward: bad harmonic_flags %d",
                harmonic_flags);
-  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
-               "decoder_forward: sample_rate must be positive");
   if (B == 0) return 0;
-  HarmonicParams p;
-  p.f0 = f0_hz; p.amps = amps_raw; p.hd = hd_raw; p.audio = audio;
-  p.B = B; p.F = F; p.K = K; p.N = N; p.hop = N / F;
-  p.sample_rate = sample_rate;
-  p.nyquist = sample_rate * 0.5f;
-  p.inv_sr = 1.0 / (double)sample_rate;
-  p.amp_method = amp_method;
-  p.accumulate = 0;
+  HarmonicParams p = harm_params(f0_hz, amps_raw, hd_raw, audio, B, F, K, N,
+                                 sample_rate, amp_method);
   p.ctl_flags = harmonic_flags;
-  p.init_phase = nullptr; p.final_phase = nullptr; p.mask_nyquist = 1;
   // The single-pass pipeline exists for the decoder regime only; everything
   // else goes through get_controls + the two *_forward calls.
   DDSP_REQUIRE(N % F == 0 && B <= 65535 && harmonic_fused_supported(p) &&
@@ -411,7 +391,7 @@ static int decoder_forward_impl(const float* amps_raw, const float* hd_raw,
                "decoder_forward: shape outside the fused decoder path "
                "(needs hop %% 64 == 0, n_frequencies <= %d)", kNfMaxNb);
   cudaStream_t st = (cudaStream_t)stream;
-  int rc = launch_harmonic_v4(p, st);
+  rc = launch_harmonic_v4(p, st);
   if (rc == 1) {
     set_error("decoder_forward: harmonic tile does not fit shared memory");
     return DDSP_B200_E_UNSUPPORTED;
@@ -601,23 +581,14 @@ int ddsp_b200_harmonic_backward(const float* f0_hz, const float* grad_audio,
                                 float sample_rate, int amp_method, void* stream) {
   DDSP_REQUIRE(f0_hz && grad_audio && g0 && g1, DDSP_B200_E_INVALID,
                "harmonic_backward: null pointer");
-  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1 && N >= 1 && N % F == 0,
-               DDSP_B200_E_INVALID,
+  int rc = harm_check("harmonic_backward", B, F, K, N, amp_method, sample_rate);
+  if (rc) return rc;
+  DDSP_REQUIRE(N % F == 0, DDSP_B200_E_INVALID,
                "harmonic_backward: bad shape B=%d F=%d K=%d N=%d", B, F, K, N);
-  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW ||
-                   amp_method == DDSP_B200_AMP_LINEAR,
-               DDSP_B200_E_INVALID, "harmonic_backward: bad amp_method %d",
-               amp_method);
-  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
-               "harmonic_backward: sample_rate must be positive");
   if (B == 0) return 0;
-  HarmonicParams p;
-  p.f0 = f0_hz; p.amps = nullptr; p.hd = nullptr; p.audio = nullptr;
-  p.B = B; p.F = F; p.K = K; p.N = N; p.hop = N / F;
-  p.sample_rate = sample_rate; p.nyquist = sample_rate * 0.5f;
-  p.inv_sr = 1.0 / (double)sample_rate;
-  p.amp_method = amp_method; p.accumulate = 0; p.ctl_flags = 0; p.Kp = K;
-  p.init_phase = nullptr; p.final_phase = nullptr; p.mask_nyquist = 1;
+  HarmonicParams p = harm_params(f0_hz, nullptr, nullptr, nullptr, B, F, K, N,
+                                 sample_rate, amp_method);
+  p.Kp = K;
   DDSP_REQUIRE(p.hop % 64 == 0 && p.hop <= 8192 && B <= 65535,
                DDSP_B200_E_UNSUPPORTED,
                "harmonic_backward: needs hop %% 64 == 0 (hop = %d)", p.hop);
@@ -629,16 +600,11 @@ int ddsp_b200_harmonic_backward(const float* f0_hz, const float* grad_audio,
   DDSP_CUDA_TRY(cudaMemsetAsync(g1, 0, gbytes, st), "harmonic_backward: memset g1");
   p.FT = std::max(1, std::min(F, 2048 / p.hop));
   const size_t smem = harmonic_backward_smem(p.FT, p.hop);
-  dim3 grid((F + p.FT - 1) / p.FT, B);
-  if (amp_method == DDSP_B200_AMP_WINDOW) {
-    int rc = set_smem(harmonic_backward_kernel<true>, smem, "harmonic_backward");
-    if (rc) return rc;
-    harmonic_backward_kernel<true><<<grid, kHbThreads, smem, st>>>(p, grad_audio, g0, g1);
-  } else {
-    int rc = set_smem(harmonic_backward_kernel<false>, smem, "harmonic_backward");
-    if (rc) return rc;
-    harmonic_backward_kernel<false><<<grid, kHbThreads, smem, st>>>(p, grad_audio, g0, g1);
-  }
+  auto kern = amp_method == DDSP_B200_AMP_WINDOW ? harmonic_backward_kernel<true>
+                                                 : harmonic_backward_kernel<false>;
+  rc = set_smem(kern, smem, "harmonic_backward");
+  if (rc) return rc;
+  kern<<<dim3((F + p.FT - 1) / p.FT, B), kHbThreads, smem, st>>>(p, grad_audio, g0, g1);
   DDSP_CHECK_LAUNCH("harmonic_backward");
   return 0;
 }
@@ -651,14 +617,12 @@ int ddsp_b200_harmonic_backward_f0(const float* f0_hz, const float* amps,
                                    void* stream) {
   DDSP_REQUIRE(f0_hz && amps && grad_audio && d_f0, DDSP_B200_E_INVALID,
                "harmonic_backward_f0: null pointer");
-  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1 && N >= 1 && N % F == 0, DDSP_B200_E_INVALID,
+  int rc = harm_check("harmonic_backward_f0", B, F, K, N, amp_method, sample_rate);
+  if (rc) return rc;
+  DDSP_REQUIRE(N % F == 0, DDSP_B200_E_INVALID,
                "harmonic_backward_f0: bad shape B=%d F=%d K=%d N=%d", B, F, K, N);
   DDSP_REQUIRE(hd != nullptr || K == 1, DDSP_B200_E_INVALID,
                "harmonic_backward_f0: harmonic_distribution is NULL but K=%d", K);
-  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW || amp_method == DDSP_B200_AMP_LINEAR,
-               DDSP_B200_E_INVALID, "harmonic_backward_f0: bad amp_method %d", amp_method);
-  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
-               "harmonic_backward_f0: sample_rate must be positive");
   if (B == 0) return 0;
   DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
                "harmonic_backward_f0: B=%d exceeds the 65535 grid limit", B);
@@ -666,32 +630,19 @@ int ddsp_b200_harmonic_backward_f0(const float* f0_hz, const float* amps,
   DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
                "harmonic_backward_f0: workspace of %zu B needed, %zu given", need,
                workspace_bytes);
-  HarmonicParams p;
-  p.f0 = f0_hz; p.amps = amps; p.hd = hd; p.audio = nullptr;
-  p.B = B; p.F = F; p.K = K; p.N = N; p.hop = N / F;
-  p.sample_rate = sample_rate; p.nyquist = sample_rate * 0.5f;
-  p.inv_sr = 1.0 / (double)sample_rate;
-  p.amp_method = amp_method; p.accumulate = 0; p.ctl_flags = 0;
-  p.init_phase = nullptr; p.final_phase = nullptr; p.mask_nyquist = 1;
-  p.Kp = (K + 3) & ~3;
-  int FT = std::max(1, std::min(F, 2048 / p.hop));
-  while (FT > 1 && harmonic_df0_smem(FT, p.Kp) > kMaxDynSmem) FT = (FT + 1) / 2;
-  DDSP_REQUIRE(harmonic_df0_smem(FT, p.Kp) <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
-               "harmonic_backward_f0: K=%d needs too much shared memory", K);
-  p.FT = FT;
-  const size_t smem = harmonic_df0_smem(FT, p.Kp);
+  HarmonicParams p = harm_params(f0_hz, amps, hd, nullptr, B, F, K, N, sample_rate,
+                                 amp_method);
+  p.FT = fit_tile("harmonic_backward_f0", std::max(1, std::min(F, 2048 / p.hop)), K,
+                  p.Kp, harmonic_df0_smem);
+  if (!p.FT) return DDSP_B200_E_UNSUPPORTED;
+  const size_t smem = harmonic_df0_smem(p.FT, p.Kp);
   cudaStream_t st = (cudaStream_t)stream;
   float* sq = reinterpret_cast<float*>(workspace);
-  dim3 grid((F + FT - 1) / FT, B);
-  if (amp_method == DDSP_B200_AMP_WINDOW) {
-    int rc = set_smem(harmonic_df0_kernel<true>, smem, "harmonic_backward_f0");
-    if (rc) return rc;
-    harmonic_df0_kernel<true><<<grid, kDf0Threads, smem, st>>>(p, grad_audio, sq);
-  } else {
-    int rc = set_smem(harmonic_df0_kernel<false>, smem, "harmonic_backward_f0");
-    if (rc) return rc;
-    harmonic_df0_kernel<false><<<grid, kDf0Threads, smem, st>>>(p, grad_audio, sq);
-  }
+  auto kern = amp_method == DDSP_B200_AMP_WINDOW ? harmonic_df0_kernel<true>
+                                                 : harmonic_df0_kernel<false>;
+  rc = set_smem(kern, smem, "harmonic_backward_f0");
+  if (rc) return rc;
+  kern<<<dim3((F + p.FT - 1) / p.FT, B), kDf0Threads, smem, st>>>(p, grad_audio, sq);
   DDSP_CHECK_LAUNCH("harmonic_backward_f0");
   harmonic_df0_finalize<<<(B + 127) / 128, 128, 0, st>>>(sq, d_f0, B, F, p.hop,
                                                        (float)p.inv_sr);
@@ -742,9 +693,8 @@ int ddsp_b200_filtered_noise_backward(const float* grad_audio, const float* nois
                "filtered_noise_backward: null pointer");
   DDSP_REQUIRE(B >= 0 && F >= 1 && N >= 1 && nb >= 2, DDSP_B200_E_INVALID,
                "filtered_noise_backward: bad shape B=%d F=%d nb=%d N=%d", B, F, nb, N);
-  const int frame = (N + F - 1) / F;
-  DDSP_REQUIRE((N + frame - 1) / frame == F, DDSP_B200_E_INVALID,
-               "filtered_noise_backward: %d frames do not tile %d samples", F, N);
+  const int frame = ir_frame(N, F);
+  if (!frame) return DDSP_B200_E_INVALID;
   if (B == 0) return 0;
   NoiseBwdParams p;
   p.grad = grad_audio; p.noise = noise; p.dmags = dmags;
@@ -803,8 +753,7 @@ int ddsp_b200_oscillator_bank(const float* frequency_envelopes,
   DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
                "oscillator_bank: workspace of %zu B needed, %zu given", need,
                workspace_bytes);
-  unsigned long long* sums = reinterpret_cast<unsigned long long*>(
-      ((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  unsigned long long* sums = align256<unsigned long long>(workspace);
   const int n_chunks = (N + kObChunk - 1) / kObChunk;
   const double inv_sr = 1.0 / (double)sample_rate;
   cudaStream_t st = (cudaStream_t)stream;
@@ -816,14 +765,9 @@ int ddsp_b200_oscillator_bank(const float* frequency_envelopes,
   oscbank_scan_chunks<<<(int)((BK + kObThreads - 1) / kObThreads), kObThreads, 0, st>>>(
       sums, K, n_chunks, BK);
   DDSP_CHECK_LAUNCH("oscillator_bank(scan)");
-  if (sum_sinusoids)
-    oscbank_apply<true><<<grid, kObThreads, 0, st>>>(
-        frequency_envelopes, amplitude_envelopes, sums, out, N, K, n_chunks, inv_sr,
-        sample_rate * 0.5f);
-  else
-    oscbank_apply<false><<<grid, kObThreads, 0, st>>>(
-        frequency_envelopes, amplitude_envelopes, sums, out, N, K, n_chunks, inv_sr,
-        sample_rate * 0.5f);
+  auto apply = sum_sinusoids ? oscbank_apply<true> : oscbank_apply<false>;
+  apply<<<grid, kObThreads, 0, st>>>(frequency_envelopes, amplitude_envelopes, sums, out,
+                                     N, K, n_chunks, inv_sr, sample_rate * 0.5f);
   DDSP_CHECK_LAUNCH("oscillator_bank(apply)");
   return 0;
 }
@@ -861,7 +805,7 @@ int ddsp_b200_fft_convolve_lti(const float* audio, const float* impulse_response
                "fft_convolve_lti: workspace of %zu B needed, %zu given", need,
                workspace_bytes);
   const lc::Geom g = lc::geom(N, S);
-  float2* Z = reinterpret_cast<float2*>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  float2* Z = align256<float2>(workspace);
   float2* H = Z + (size_t)B * g.n_in * lc::M;
   float2* W = H + (size_t)ir_batch * g.P * lc::M;
   cudaStream_t st = (cudaStream_t)stream;
@@ -922,8 +866,7 @@ int ddsp_b200_angular_cumsum(const float* angular_frequency, float* phase, int B
   DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
                "angular_cumsum: workspace of %zu B needed, %zu given", need,
                workspace_bytes);
-  unsigned long long* sums = reinterpret_cast<unsigned long long*>(
-      ((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  unsigned long long* sums = align256<unsigned long long>(workspace);
   const int n_chunks = (N + kObChunk - 1) / kObChunk;
   const double inv_two_pi = 0.15915494309189535;
   dim3 grid(n_chunks, B);
@@ -1026,29 +969,20 @@ int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitud
   if (rc || B == 0) return rc;
   const int FT = sinus_tile_frames(F, K);
   const SfSmem L = sf_smem(FT, K);
-  unsigned long long* sums = reinterpret_cast<unsigned long long*>(
-      ((uintptr_t)workspace + 255) & ~(uintptr_t)255);
+  unsigned long long* sums = align256<unsigned long long>(workspace);
   const int n_tiles = (F + FT - 1) / FT;
   const int hop = N / F;
   const double inv_sr = 1.0 / (double)sample_rate;
   cudaStream_t st = (cudaStream_t)stream;
-  dim3 grid(n_tiles, B);
   rc = sinus_tile_offsets(frequencies, sums, B, F, K, hop, FT, inv_sr, st,
                           "sinusoidal_forward(tile offsets)");
   if (rc) return rc;
-  if (amp_method == DDSP_B200_AMP_WINDOW) {
-    rc = set_smem(sinus_apply<true>, L.total, "sinusoidal_forward");
-    if (rc) return rc;
-    sinus_apply<true><<<grid, kSfThreads, L.total, st>>>(
-        frequencies, amplitudes, sums, audio, F, K, N, hop, FT, n_tiles, inv_sr,
-        sample_rate * 0.5f, accumulate);
-  } else {
-    rc = set_smem(sinus_apply<false>, L.total, "sinusoidal_forward");
-    if (rc) return rc;
-    sinus_apply<false><<<grid, kSfThreads, L.total, st>>>(
-        frequencies, amplitudes, sums, audio, F, K, N, hop, FT, n_tiles, inv_sr,
-        sample_rate * 0.5f, accumulate);
-  }
+  auto kern = amp_method == DDSP_B200_AMP_WINDOW ? sinus_apply<true> : sinus_apply<false>;
+  rc = set_smem(kern, L.total, "sinusoidal_forward");
+  if (rc) return rc;
+  kern<<<dim3(n_tiles, B), kSfThreads, L.total, st>>>(
+      frequencies, amplitudes, sums, audio, F, K, N, hop, FT, n_tiles, inv_sr,
+      sample_rate * 0.5f, accumulate);
   DDSP_CHECK_LAUNCH("sinusoidal_forward(apply)");
   return 0;
 }
@@ -1075,10 +1009,8 @@ int ddsp_b200_sinusoidal_backward(const float* frequencies, const float* amplitu
   const int hop = N / F;
   const double inv_sr = 1.0 / (double)sample_rate;
   cudaStream_t st = (cudaStream_t)stream;
-  unsigned long long* sums = reinterpret_cast<unsigned long long*>(
-      ((uintptr_t)workspace + 255) & ~(uintptr_t)255);
-  float* part = reinterpret_cast<float*>(
-      ((uintptr_t)(sums + (size_t)B * n_tiles * K) + 255) & ~(uintptr_t)255);
+  unsigned long long* sums = align256<unsigned long long>(workspace);
+  float* part = align256<float>(sums + (size_t)B * n_tiles * K);
   rc = sinus_tile_offsets(frequencies, sums, B, F, K, hop, FT, inv_sr, st,
                           "sinusoidal_backward(tile offsets)");
   if (rc) return rc;

@@ -32,6 +32,26 @@ void count_launch();
     }                                                                   \
   } while (0)
 
+// Dynamic shared memory one CTA may reserve (of 227 KB usable per CTA).
+constexpr size_t kMaxDynSmem = 200 * 1024;
+
+// Allows `kernel` to launch with `bytes` of dynamic shared memory (past the default
+// 48 KB), or reports E_CUDA with `name` in front of the message.
+template <typename K>
+int set_smem(K kernel, size_t bytes, const char* name) {
+  if (bytes > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(
+        kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) {
+      (void)cudaGetLastError();   // reported here, not by the next launch check
+      set_error("%s: cannot reserve %zu B of shared memory: %s", name, bytes,
+                cudaGetErrorString(e));
+      return DDSP_B200_E_CUDA;
+    }
+  }
+  return 0;
+}
+
 // Upper bound on the SM count, for per-SM debug arrays (H100 SXM has 132).
 constexpr int kMaxSMs = 256;
 

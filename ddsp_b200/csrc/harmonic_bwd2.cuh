@@ -269,10 +269,9 @@ inline int launch_harmonic_backward2(HarmonicParams p, const float* grad, float*
   FW = std::max(1, std::min(FW, (p.F + NW - 1) / NW));
   const size_t smem = smem_layout(FW).total;
   dim3 grid((p.F + FW * NW - 1) / (FW * NW), p.B);
-  if (p.amp_method == DDSP_B200_AMP_WINDOW)
-    harmonic_backward2_kernel<true><<<grid, NT, smem, st>>>(p, grad, g0, g1, FW);
-  else
-    harmonic_backward2_kernel<false><<<grid, NT, smem, st>>>(p, grad, g0, g1, FW);
+  auto kern = p.amp_method == DDSP_B200_AMP_WINDOW ? harmonic_backward2_kernel<true>
+                                                   : harmonic_backward2_kernel<false>;
+  kern<<<grid, NT, smem, st>>>(p, grad, g0, g1, FW);
   DDSP_CHECK_LAUNCH("harmonic_backward(v2)");
   return 0;
 }

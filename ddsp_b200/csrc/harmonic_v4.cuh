@@ -755,19 +755,6 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
   HV4_TIMING_FLUSH();
 }
 
-template <bool WINDOW, int HOPT>
-inline cudaError_t launch_one(const HarmonicParams& p, int use_tma, int FW, dim3 grid,
-                              size_t smem, cudaStream_t st) {
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(harmonic_v4_kernel<WINDOW, HOPT>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem);
-    if (e != cudaSuccess) return e;
-  }
-  harmonic_v4_kernel<WINDOW, HOPT><<<grid, NT, smem, st>>>(p, use_tma, FW);
-  return cudaSuccess;
-}
-
 }  // namespace hv4
 
 // Returns 0 on success, negative on error, 1 if the tile cannot fit shared memory
@@ -785,24 +772,16 @@ inline int launch_harmonic_v4(HarmonicParams p, cudaStream_t st) {
   FW =std::max(1, std::min(FW, (p.F + NW - 1) / NW));
   while (FW > 1 && smem_layout(FW, p.Kp, p.hop).total > 64 * 1024) FW = (FW + 1) / 2;
   const size_t smem = smem_layout(FW, p.Kp, p.hop).total;
-  if (smem > 200 * 1024) return 1;
+  if (smem > kMaxDynSmem) return 1;
   const int use_tma = (p.hd != nullptr) && (p.K % 4 == 0) &&
                       (((uintptr_t)p.hd & 15) == 0);
   dim3 grid((p.F + FW * NW - 1) / (FW * NW), p.B);
-  cudaError_t e;
   const bool win = p.amp_method == DDSP_B200_AMP_WINDOW;
-  if (p.hop == 64) {
-    e = win ? launch_one<true, 64>(p, use_tma, FW, grid, smem, st)
-            : launch_one<false, 64>(p, use_tma, FW, grid, smem, st);
-  } else {
-    e = win ? launch_one<true, 0>(p, use_tma, FW, grid, smem, st)
-            : launch_one<false, 0>(p, use_tma, FW, grid, smem, st);
-  }
-  if (e != cudaSuccess) {
-    (void)cudaGetLastError();
-    set_error("harmonic_forward(v4): %s", cudaGetErrorString(e));
-    return DDSP_B200_E_CUDA;
-  }
+  auto kern = p.hop == 64 ? (win ? harmonic_v4_kernel<true, 64> : harmonic_v4_kernel<false, 64>)
+                          : (win ? harmonic_v4_kernel<true, 0> : harmonic_v4_kernel<false, 0>);
+  int rc = set_smem(kern, smem, "harmonic_forward(v4)");
+  if (rc) return rc;
+  kern<<<grid, NT, smem, st>>>(p, use_tma, FW);
   DDSP_CHECK_LAUNCH("harmonic_forward(v4)");
   return 0;
 }

@@ -465,7 +465,7 @@ inline bool nf_configure(NoiseFusedParams& p, int F, int nb, int N,
   p.nblk = (p.ylen + kNfR - 1) / kNfR;
   p.ngrp = (p.nblk * kNfR + p.frame - 1) / p.frame;
   p.outLen = (p.frame + 1) * (32 + p.ngrp) + 16;
-  return nf_smem_layout(p).total <= 200 * 1024;
+  return nf_smem_layout(p).total <= kMaxDynSmem;
 }
 
 inline bool noise_fused_supported(int F, int nb, int N, int window_size) {
@@ -494,13 +494,8 @@ inline int launch_noise_fused(const float* mags, const float* noise,
   }
   p.n_tiles = (int)n_tiles;
   const size_t smem = nf_smem_layout(p).total;
-  cudaError_t e = cudaFuncSetAttribute(
-      noise_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) {
-    set_error("filtered_noise_forward: cannot reserve %zu B smem: %s", smem,
-              cudaGetErrorString(e));
-    return DDSP_B200_E_CUDA;
-  }
+  int rc = set_smem(noise_fused_kernel, smem, "filtered_noise_forward");
+  if (rc) return rc;
   const int ctas_per_sm = smem <= 110 * 1024 ? 2 : 1;
   const int grid = (int)std::min<long long>(n_tiles, (long long)num_sms() * ctas_per_sm);
   noise_fused_kernel<<<grid, kNfThreads, smem, st>>>(p);

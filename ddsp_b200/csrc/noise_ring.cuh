@@ -642,13 +642,8 @@ inline int launch_noise_ring(const float* mags, const float* noise, uint64_t see
   const long long T = (long long)B * F;
   const size_t smem = sizeof(nr_::Smem);
   static_assert(sizeof(nr_::Smem) <= 227 * 1024, "noise_ring shared memory");
-  cudaError_t e = cudaFuncSetAttribute(
-      nr_::noise_ring_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  if (e != cudaSuccess) {
-    set_error("filtered_noise_forward: cannot reserve %zu B smem: %s", smem,
-              cudaGetErrorString(e));
-    return DDSP_B200_E_CUDA;
-  }
+  int rc = set_smem(nr_::noise_ring_kernel, smem, "filtered_noise_forward");
+  if (rc) return rc;
   // one persistent CTA per SM; tiny workloads get one CTA per 32-frame tile
   const int grid = (int)std::max<long long>(
       1, std::min<long long>((long long)num_sms(), (T + 31) / 32));
@@ -666,7 +661,7 @@ inline int launch_noise_ring(const float* mags, const float* noise, uint64_t see
   attr[0].val.programmaticStreamSerializationAllowed = overlap_previous ? 1 : 0;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  e = cudaLaunchKernelEx(&cfg, nr_::noise_ring_kernel, p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, nr_::noise_ring_kernel, p);
   if (e != cudaSuccess) {
     set_error("filtered_noise_forward(ring): launch failed: %s", cudaGetErrorString(e));
     return DDSP_B200_E_CUDA;
