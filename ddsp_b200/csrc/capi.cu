@@ -8,13 +8,13 @@
 #include "common.cuh"
 #include "controls.cuh"
 #include "harmonic.cuh"
-#include "harmonic_common.cuh"
 #include "harmonic_v4.cuh"
 #include "noise.cuh"
 #include "noise_fused.cuh"
 #include "noise_ring.cuh"
 #include "host_pipeline.cuh"
-#include "backward.cuh"
+#include "noise_backward.cuh"
+#include "harmonic_backward.cuh"
 #include "harmonic_bwd2.cuh"
 #include "controls_bwd.cuh"
 #include "oscbank.cuh"

@@ -13,65 +13,13 @@
 //   audio(t)= sum_{k: f_k(t) < sr/2} a_k(t) sin(2 pi k phi(t))
 // phi is 64-bit fixed point (wraps exactly); k*phi is a wrapping 32-bit multiply.
 #pragma once
-#include "common.cuh"
+#include "harmonic_common.cuh"
 
 namespace ddsp {
 
 constexpr int kHarmThreads = 256;
 
-struct HarmonicParams {
-  const float* __restrict__ f0;    // [B,F]
-  const float* __restrict__ amps;  // [B,F]
-  const float* __restrict__ hd;    // [B,F,K] or nullptr (K == 1, hd == 1)
-  float* __restrict__ audio;       // [B,N]
-  int B, F, K, N, hop;
-  int FT;          // frames per CTA tile
-  int Kp;          // smem row stride (floats)
-  float sample_rate;
-  float nyquist;
-  double inv_sr;
-  int amp_method;
-  int accumulate;
-  // 0: amps / hd are synthesizer CONTROLS (outputs of get_controls).
-  // DDSP_B200_CTL_*: they are raw network outputs; Harmonic.get_controls
-  // (synths.py:94-121) is applied while the frame slab is staged (fast path).
-  int ctl_flags;
-  // Streaming synthesis (core.harmonic_oscillator_bank, core.py:966-1025):
-  const float* init_phase;   // [B] radians added to the phase, or nullptr
-  float* final_phase;        // [B] phase after the last sample (radians), or nullptr
-  int mask_nyquist;          // 0: no audio-rate Nyquist mask (streaming bank has none)
-};
-
-// The reference's float32 evaluation of the k-th harmonic's audio-rate
-// frequency: hf = f0 * k (core.py:1044), then v1 bilinear
-// lo + (hi - lo) * frac (core.py:617-620).  Explicit _rn intrinsics forbid FMA
-// contraction so the Nyquist decision (core.py:888-890) matches op for op.
-__device__ __forceinline__ float ref_harmonic_freq(float f_lo, float f_hi,
-                                                   float frac, int k) {
-  float kf = (float)k;
-  float lo = __fmul_rn(f_lo, kf);
-  float hi = __fmul_rn(f_hi, kf);
-  return __fadd_rn(lo, __fmul_rn(__fsub_rn(hi, lo), frac));
-}
-
-// Number of harmonics k = 1..count that stay below Nyquist at this sample,
-// assuming f_k(t) is non-decreasing in k (true whenever both frame f0 >= 1 Hz).
-__device__ __forceinline__ int live_harmonics(float f_lo, float f_hi,
-                                              float frac, int K, float nyq) {
-  float ft = f_lo + (f_hi - f_lo) * frac;
-  int k = (int)fminf(nyq / fmaxf(ft, 1e-3f), (float)K);
-  k = max(0, min(k, K));
-  while (k < K && ref_harmonic_freq(f_lo, f_hi, frac, k + 1) < nyq) ++k;
-  while (k > 0 && !(ref_harmonic_freq(f_lo, f_hi, frac, k) < nyq)) --k;
-  return k;
-}
-
-struct HarmSmem {
-  // dynamic layout computed by harm_smem_bytes():
-  //   u64 P[FT], A[FT], D[FT]; u64 red[8];
-  //   float f0s[FT+1], amp[FT+1]; float xs[(FT+1)*Kp]
-};
-
+// u64 P[FT], A[FT], D[FT]; u64 red[8]; float f0s[FT+1], amp[FT+1]; float xs[(FT+1)*Kp]
 __host__ __device__ inline size_t harm_smem_bytes(int FT, int Kp) {
   return sizeof(unsigned long long) * (3 * (size_t)FT + 8) +
          sizeof(float) * (2 * (size_t)(FT + 1) + (size_t)(FT + 1) * Kp);
@@ -106,7 +54,7 @@ harmonic_generic_kernel(HarmonicParams p) {
   for (int j = tid; j < i0; j += kHarmThreads) {
     double a0 = (double)f0b[j] * p.inv_sr;
     double a1 = (double)f0b[min(j + 1, F - 1)] * p.inv_sr;
-    part += turns_to_fix64((double)hop * a0 + (a1 - a0) * (0.5 * (hop - 1)));
+    part += frame_total_fix64(a0, a1, hop);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
@@ -146,8 +94,8 @@ harmonic_generic_kernel(HarmonicParams p) {
       double a1 = (double)sF0[j + 1] * p.inv_sr;
       sP[j] = P;
       sA[j] = turns_to_fix64(a0);
-      sD[j] = turns_to_fix64((a1 - a0) / (double)hop);
-      P += turns_to_fix64((double)hop * a0 + (a1 - a0) * (0.5 * (hop - 1)));
+      sD[j] = frame_slope_fix64(a0, a1, hop);
+      P += frame_total_fix64(a0, a1, hop);
     }
     if (p.final_phase != nullptr && i0 + nfr == F) {
       // angular_cumsum's last value in [0, 2 pi) plus the initial phase

@@ -1,14 +1,13 @@
-// Harmonic backward, second generation (hop == 64): the transposes
+// Harmonic backward for hop == 64: the transposes
 //   G0[i,k] = sum_{t in frame i} g(t) w0(r) m_k(t) sin(k phi(t)),   G1 with w1
-// (backward.cuh) with sin(k phi) from the SAME Reinsch chains as the forward
-// kernel instead of one sinpif per oscillator: 10 packed instructions per sample
-// pair and harmonic pair, plus a 16-value transposing warp reduction per 8
-// harmonics.  Tiling, frame records and the phase prefix are those of the third
-// forward generation.  Every element of G0 / G1 is written (zeros above the live
-// count), so the caller needs no memset.
+// (harmonic_backward.cuh) with sin(k phi) from the SAME Reinsch chains as
+// harmonic_v4_kernel instead of one sinpif per oscillator: 10 packed instructions
+// per sample pair and harmonic pair, plus a 16-value transposing warp reduction
+// per 8 harmonics.  The frame records and the phase (tile_phase_base,
+// harmonic_common.cuh) are built as in harmonic_v4_kernel.  Every element of
+// G0 / G1 is written (zeros above the live count), so the caller needs no memset.
 #pragma once
-#include "backward.cuh"
-#include "harmonic_common.cuh"
+#include "harmonic_backward.cuh"
 
 namespace ddsp {
 namespace hb2 {
@@ -120,15 +119,10 @@ harmonic_backward2_kernel(HarmonicParams p, const float* __restrict__ grad,
       const double a0 = (double)f * p.inv_sr;
       const double a1 = (double)f_next * p.inv_sr;
       Af = turns_to_fix64(a0);
-      Df = turns_to_fix64((a1 - a0) / (double)hop);
-      tot = turns_to_fix64((double)hop * a0 + (a1 - a0) * (0.5 * (hop - 1)));
+      Df = frame_slope_fix64(a0, a1, hop);
+      tot = frame_total_fix64(a0, a1, hop);
     }
-    unsigned long long incl = tot;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned long long up = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += up;
-    }
+    const unsigned long long incl = warp_scan_frame_totals(tot, lane);
     excl = incl - tot;
     if (lane == 31) sWarpTot[warp] = incl;
     int kca = -1, kcb = -1;
@@ -151,8 +145,7 @@ harmonic_backward2_kernel(HarmonicParams p, const float* __restrict__ grad,
     for (int w = 0; w < NW; ++w) base_sum += sRedD[w];
     const double a_tile = (double)f0b[i0] * p.inv_sr;
     const double a_first = (double)f0b[0] * p.inv_sr;
-    unsigned long long P0 = turns_to_fix64(
-        (double)hop * (base_sum * p.inv_sr) + 0.5 * (hop - 1) * (a_tile - a_first));
+    unsigned long long P0 = tile_phase_base(base_sum, a_first, a_tile, hop, p.inv_sr);
     for (int w = 0; w < warp; ++w) P0 += sWarpTot[w];
     if (lane < nfw) sRec[lane].P = P0 + excl + 0x80000000ull;
   }

@@ -631,14 +631,9 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
       a0 = (double)f * p.inv_sr;
       const double a1 = (double)f_n * p.inv_sr;
       dd = (a1 - a0) * (1.0 / (double)hop);
-      tot = turns_to_fix64((double)hop * a0 + (a1 - a0) * (0.5 * (hop - 1)));
+      tot = frame_total_fix64(a0, a1, hop);
     }
-    unsigned long long incl = tot;                     // wrapping adds: exact
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned long long up = __shfl_up_sync(0xffffffffu, incl, o);
-      if (lane >= o) incl += up;
-    }
+    const unsigned long long incl = warp_scan_frame_totals(tot, lane);
     excl = incl - tot;
     if (lane == 31) sWarpTot[warp] = incl;             // total of the record warp's frames
     const bool nyq = p.ctl_flags & DDSP_B200_CTL_NYQUIST;
@@ -671,15 +666,13 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
     if (n_act > 1) asm volatile("bar.sync 1, %0;" ::"r"(32 * n_act) : "memory");
     HV4_LAP(2);
 
-    // phase at the start of the tile (telescoped closed form, one double-precision
-    // evaluation: <= 2^15 turns, 2^-38 turn resolution), then the record warp's offset
+    // phase at the start of the tile, then the record warp's offset
     double base_sum = 0.0;
 #pragma unroll
     for (int w = 0; w < NW; ++w) base_sum += sRedD[w];
     const double a_tile = (double)f_tile * p.inv_sr;
     const double a_first = (double)f_first * p.inv_sr;
-    unsigned long long P0 = turns_to_fix64(
-        (double)hop * (base_sum * p.inv_sr) + 0.5 * (hop - 1) * (a_tile - a_first));
+    unsigned long long P0 = tile_phase_base(base_sum, a_first, a_tile, hop, p.inv_sr);
     for (int w = 0; w < warp; ++w) P0 += sWarpTot[w];
     if (lane < cnt) {
       const unsigned long long Pf = P0 + excl;         // exact frame phase, 2^64 = 1 turn

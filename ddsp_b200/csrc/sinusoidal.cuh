@@ -18,18 +18,12 @@
 //      loops over k: phase -> sinpif, Nyquist mask on the reference's float32
 //      envelope (lo + (hi - lo) * frac, no FMA), two-row amplitude interpolation.
 #pragma once
-#include "common.cuh"
+#include "harmonic_common.cuh"
 #include "oscbank.cuh"
 
 namespace ddsp {
 
 constexpr int kSfThreads = 128;
-
-__device__ __forceinline__ unsigned long long sf_frame_total(float f_lo, float f_hi,
-                                                             int hop, double inv_sr) {
-  const double a0 = (double)f_lo * inv_sr, a1 = (double)f_hi * inv_sr;
-  return turns_to_fix64((double)hop * a0 + (a1 - a0) * (0.5 * (hop - 1)));
-}
 
 // pass 1.  sums[b, tile, k] = sum of the frame totals of the tile's frames.
 __global__ void __launch_bounds__(kSfThreads)
@@ -43,7 +37,7 @@ sinus_tile_sums(const float* __restrict__ f, unsigned long long* __restrict__ su
     float cur = fp[(size_t)i0 * K];
     for (int i = i0; i < i1; ++i) {
       const float nxt = fp[(size_t)min(i + 1, F - 1) * K];
-      acc += sf_frame_total(cur, nxt, hop, inv_sr);
+      acc += frame_total_fix64((double)cur * inv_sr, (double)nxt * inv_sr, hop);
       cur = nxt;
     }
     sums[((size_t)b * n_tiles + tile) * K + k] = acc;
@@ -99,8 +93,8 @@ sinus_apply(const float* __restrict__ f, const float* __restrict__ a,
       const double a0 = (double)f_lo * inv_sr, a1 = (double)f_hi * inv_sr;
       sP[j * K + k] = P + 0x80000000ull;          // rounding offset for the top 32 bits
       sA[j * K + k] = turns_to_fix64(a0);
-      sD[j * K + k] = turns_to_fix64((a1 - a0) / (double)hop);
-      P += sf_frame_total(f_lo, f_hi, hop, inv_sr);
+      sD[j * K + k] = frame_slope_fix64(a0, a1, hop);
+      P += frame_total_fix64(a0, a1, hop);
     }
   }
   __syncthreads();
@@ -183,11 +177,12 @@ sinus_bwd_frames(const float* __restrict__ f, const float* __restrict__ a,
   // the frame's phase: the tile offset plus the tile's frames before i
   unsigned long long P = offs[((size_t)b * n_tiles + tile) * K + k];
   for (int j = tile * FT; j < i; ++j)
-    P += sf_frame_total(fb[(size_t)j * K], fb[(size_t)(j + 1) * K], hop, inv_sr);
+    P += frame_total_fix64((double)fb[(size_t)j * K] * inv_sr,
+                           (double)fb[(size_t)(j + 1) * K] * inv_sr, hop);
   const float lo = fb[(size_t)i * K], hi = fb[(size_t)inx * K];
   const double a0 = (double)lo * inv_sr, a1 = (double)hi * inv_sr;
   const unsigned long long A = turns_to_fix64(a0);
-  const unsigned long long D = turns_to_fix64((a1 - a0) / (double)hop);
+  const unsigned long long D = frame_slope_fix64(a0, a1, hop);
   const float am0 = PHASE ? a[(size_t)bi * K + k] : 0.f;
   const float am1 = PHASE ? a[((size_t)b * F + inx) * K + k] : 0.f;
 
