@@ -299,6 +299,178 @@ def spectral_signals(B, N, fft_sizes, seed):
   return target, value
 
 
+# ---------------------------------------------------------------------------
+# Launch geometry of the fused forward kernels, restated from the launchers so
+# that the edge tests can say which kernel, tile and occupancy a case reaches.
+# tests/test_forward_routing.py pins these restatements to the library's own
+# routing (ddsp_b200_filtered_noise_workspace) without a GPU.
+# ---------------------------------------------------------------------------
+MAX_DYN_SMEM = 200 * 1024          # kMaxDynSmem (common.cuh)
+
+
+def ir_geometry(nb, window_size):
+  """make_ir_geom (noise.cuh): (S0, S, shift, padded)."""
+  s0 = 2 * (nb - 1)
+  ws = s0 if (window_size <= 0 or window_size > s0) else window_size
+  if s0 - ws > 0:
+    half = (ws + 1) // 2
+    return s0, 2 * half - 1, half - 2, True
+  return s0, s0, s0 // 2, False
+
+
+def noise_fused_geometry(F, nb, N, window_size):
+  """nf_configure + nf_smem_layout (noise_fused.cuh): None where
+  noise_fused_kernel declines the shape, else its tile geometry, shared memory
+  and CTAs per SM (launch_noise_fused)."""
+  if nb < 3 or nb > 129 or nb % 2 == 0:
+    return None
+  s0, s, _, _ = ir_geometry(nb, window_size)
+  frame = -(-N // F)
+  start = (s - 1) // 2 - 1
+  if start < 0 or frame < 16 or frame > 1024 or frame % 16:
+    return None
+  hb = (s - 1 - start + frame - 1) // frame
+  ha = (frame - 1 + start) // frame
+  tfo = 32 - hb - ha
+  if tfo < 16:
+    return None
+  q = s0 // 4
+  qp = (q + 1 + 3) & ~3
+  h_stride = ((s + 2 * 32 + 2 + 3) & ~3) + 2
+  x_stride = ((((frame + 15) & ~15) + 16 + 3) & ~3) + 2
+  nblk = (frame + s - 1 + 15) // 16
+  ngrp = (nblk * 16 + frame - 1) // frame
+  out_len = (frame + 1) * (32 + ngrp) + 16
+  floats = ((nb + 1) // 2 * qp + (nb - 1) // 2 * qp + ((s + 3) & ~3) + 32 * (nb | 1) +
+            32 * nb + 64 * h_stride + 32 * x_stride + out_len)
+  smem = (4 * floats + 15) & ~15
+  if smem > MAX_DYN_SMEM:
+    return None
+  return dict(frame=frame, S=s, TFo=tfo, Hb=hb, Ha=ha, tiles_per_item=-(-F // tfo),
+              smem=smem, ctas_per_sm=2 if smem <= 110 * 1024 else 1)
+
+
+def noise_route(F, nb, N, window_size):
+  """Which forward kernel core.filtered_noise runs: 'ring' (noise_ring_kernel: 65
+  bands, 64-sample frames, the unpadded 128-tap IR), 'fused'
+  (noise_fused_kernel) or 'generic' (IR kernel + FIR kernel)."""
+  if noise_fused_geometry(F, nb, N, window_size) is None:
+    return 'generic'
+  _, s, _, padded = ir_geometry(nb, window_size)
+  if nb == 65 and N % F == 0 and N // F == 64 and not padded and s == 128:
+    return 'ring'
+  return 'fused'
+
+
+def harmonic_v4_smem(fw, kp, hop):
+  """hv4::smem_layout(FW, Kp, hop).total."""
+  ft = 4 * fw
+  o = 16 + 2 * 4 * 256 + 4 * (ft + 1) * kp + (0 if hop == 64 else 4 * hop)
+  o = (o + 15) & ~15
+  o += 16 * 4 + 48 * ft + 4 * (ft + 1) + 4 * (ft + 1)
+  return (o + 15) & ~15
+
+
+def harmonic_v4_tile_width(B, F, K, hop, n_sms):
+  """The frames per warp (FW) launch_harmonic_v4 picks, or None where
+  core.harmonic_synthesis(phase_mode='recurrence') takes the generic kernel."""
+  if hop % 64 or hop > 8192 or K > 1024:
+    return None
+  kp = (K + 3) & ~3
+  fw = 8
+
+  def ctas(w):
+    return B * (-(-F // (4 * w)))
+  while fw > 4 and ctas(fw) < 8 * n_sms:
+    fw = (fw + 1) >> 1
+  while fw > 1 and ctas(fw) < n_sms:
+    fw = (fw + 1) >> 1
+  fw = max(1, min(fw, -(-F // 4)))
+  while fw > 1 and harmonic_v4_smem(fw, kp, hop) > 64 * 1024:
+    fw = (fw + 1) // 2
+  if harmonic_v4_smem(fw, kp, hop) > MAX_DYN_SMEM:
+    return None
+  return fw
+
+
+# Forward filtered-noise cases of tests/test_gpu_forward_edges.py: (B, F, nb,
+# frame, window_size, r, route) with N = F * frame - r (r < F keeps ceil(N / F) =
+# frame).  route: 'fused2' / 'fused1' = noise_fused_kernel at two / one CTAs per
+# SM, 'generic' = the IR + FIR kernels.  Each boundary is a fused case next to
+# the declined (or other-regime) neighbour one step over it.
+FWD_NOISE_CASES = [
+    (2, 40, 3, 16, 0, 0, 'fused2'),        # S = 4, the smallest frame
+    (2, 37, 3, 64, 3, 1, 'fused2'),        # S = 3 (window 3), ragged by 1
+    (1, 45, 3, 32, 4, 3, 'fused2'),        # S = 3 (even window 4), ragged by 3
+    (2, 33, 5, 16, 0, 8, 'fused2'),        # ragged by frame / 2
+    (2, 50, 17, 48, 0, 47, 'fused2'),      # frame 48 (no power-of-two quad count), ragged by frame - 1
+    (1, 40, 17, 512, 0, 0, 'fused1'),
+    (2, 50, 33, 32, 0, 0, 'fused2'),
+    (2, 45, 33, 80, 31, 40, 'fused2'),     # frame 80, odd padded window, ragged by frame / 2
+    (2, 30, 33, 64, 257, 0, 'fused2'),     # window clamped to the 64-tap IR
+    (1, 20, 33, 512, 0, 0, 'fused1'),      # ~179 KB: fused ...
+    (1, 20, 65, 512, 0, 0, 'generic'),     # ... ~210 KB > 200 KB: generic
+    (2, 30, 63, 128, 0, 0, 'fused2'),      # 108 KB: two CTAs per SM ...
+    (2, 30, 65, 128, 0, 0, 'fused1'),      # ... 111 KB > 110 KB: one
+    (2, 40, 65, 64, 101, 0, 'fused2'),     # ~88 KB
+    (2, 40, 129, 64, 64, 0, 'fused1'),     # ~119 KB, even padded window
+    (2, 40, 127, 16, 0, 0, 'fused1'),      # TFo = 16: fused ...
+    (2, 40, 129, 16, 0, 0, 'generic'),     # ... TFo = 15: generic
+    (2, 33, 65, 256, 65, 3, 'fused1'),
+    (1, 65, 127, 128, 0, 64, 'fused1'),
+    (1, 64, 129, 64, 0, 63, 'fused1'),     # the unpadded 256-tap IR, ragged by frame - 1
+    (2, 35, 65, 64, 32, 0, 'fused2'),      # even padded window off the ring shape
+    (2, 35, 65, 16, 31, 0, 'fused2'),
+    (2, 30, 65, 64, 4, 1, 'fused2'),       # S = 3 at 65 bands
+    (1, 21, 129, 48, 129, 0, 'fused1'),    # odd padded window at 129 bands
+    (1, 81, 63, 80, 64, 79, 'fused2'),
+]
+
+# Many tiles per CTA: B * ceil(F / TFo) >= 3 x (132 SMs x CTAs per SM), in both
+# occupancy regimes; F not a multiple of TFo, items of one frame and of fewer
+# frames than a tile, items of ~96000 samples (interior Philox tiles).
+FWD_NOISE_MANY_TILES = [
+    (16, 1501, 33, 64, 0, 5, 'fused2'),
+    (8, 1501, 129, 64, 64, 0, 'fused1'),
+    (800, 1, 33, 64, 0, 0, 'fused2'),
+    (400, 7, 129, 64, 64, 3, 'fused1'),
+]
+
+# decoder_forward off the ring shape: (B, F, K, nb, hop, sample_rate,
+# normalize_below_nyquist, window_size, initial_bias, noise, route).  noise:
+# 'injected' or 'philox'.  The last case has more noise tiles (288) than CTAs.
+FWD_DECODER_CASES = [
+    (2, 40, 60, 33, 128, 16000, True, 0, -5.0, 'injected', 'fused2'),
+    (2, 30, 100, 65, 192, 44100, False, 101, -2.0, 'philox', 'fused1'),
+    (1, 25, 80, 129, 256, 16000, True, 64, -8.0, 'injected', 'fused1'),
+    (2, 20, 40, 65, 128, 44100, True, 0, -2.0, 'philox', 'fused1'),
+    (12, 700, 20, 33, 128, 16000, False, 0, -8.0, 'philox', 'fused2'),
+]
+
+# harmonic_v4 forward cases: (B, F, K, hop, sample_rate, amp method, f0 regime,
+# accumulate, FW) where FW is the frames per warp launch_harmonic_v4 picks on a
+# 132-SM H100, or None for the generic kernel (hop 8256 > 8192, K 1025 > 1024).
+FWD_HARMONIC_CASES = [
+    (1, 1, 4, 64, 16000, 'window', 'glide', False, 1),
+    (2, 9, 1, 128, 16000, 'linear', 'unvoiced', True, 1),
+    (2, 13, 2, 192, 44100, 'window', 'subhertz', False, 1),
+    (1, 11, 3, 320, 48000, 'linear', 'cross1hz', False, 1),
+    (2, 7, 5, 512, 16000, 'window', 'jump', True, 1),
+    (1, 5, 63, 1024, 44100, 'window', 'nyquist', False, 1),
+    (1, 3, 64, 8192, 16000, 'linear', 'glide', False, 1),
+    (1, 3, 64, 8256, 16000, 'linear', 'glide', False, None),
+    (2, 1100, 4, 192, 16000, 'window', 'unvoiced', False, 4),
+    (1056, 32, 3, 128, 48000, 'linear', 'glide', True, 8),
+    (1, 1100, 100, 64, 44100, 'window', 'jump', False, 2),
+    (132, 16, 1024, 64, 16000, 'linear', 'cross1hz', False, 2),  # the 64 KB cap: 4 -> 2
+    (1, 7, 1024, 512, 44100, 'linear', 'subhertz', False, 1),
+    (1, 7, 1025, 512, 44100, 'linear', 'subhertz', False, None),
+    (2, 50, 100, 320, 48000, 'window', 'jump', True, 1),
+    (1, 33, 257, 192, 44100, 'linear', 'nyquist', False, 1),
+    (2, 17, 512, 128, 48000, 'window', 'cross1hz', False, 1),
+]
+
+
 def low_f0_regime(regime, B, F, sample_rate, seed):
   """[B, F, 1] float32 f0 tracks for the edges of the harmonic kernels:
     'unvoiced'  - runs of f0 = 0 between voiced frames;
