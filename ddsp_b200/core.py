@@ -430,12 +430,15 @@ def normalize_harmonics(harmonic_distribution, f0_hz=None, sample_rate=None):
 
 def angular_cumsum(angular_frequency, chunk_size: int = 1000,
                    tf_sequential: bool = False):
-  """core.angular_cumsum (core.py:799-866): accumulated phase in [0, 2 pi) of an
+  """core.angular_cumsum (core.py:799-866): accumulated phase in [0, 2 pi] of an
   angular frequency [batch, time, ...] in radians per sample.
 
   Default: the wrapped running sum computed EXACTLY (64-bit fixed-point turns,
   three-pass scan) - the quantity the reference's chunked float32 cumsum
-  approximates; `chunk_size` does not matter then.  tf_sequential=True reproduces
+  approximates; `chunk_size` does not matter then.  The exact phase lies in
+  [0, 2 pi); rounding it to float32 takes a phase within about 6e-8 rad below
+  2 pi up to float32(2 pi), so the result lies in [0, float32(2 pi)], the
+  [0, 2 pi] the reference documents.  tf_sequential=True reproduces
   the reference's own float32 arithmetic in its own order (chunks of
   `chunk_size`, mod-2pi stitching) - a debug mode for comparing against
   TensorFlow, one thread per (batch, channel)."""

@@ -97,7 +97,7 @@ oscbank_apply(const float* __restrict__ f, const float* __restrict__ a,
 }
 
 // core.angular_cumsum (core.py:799-866) done exactly: pass 3 variant that writes
-// the wrapped phase itself, in radians in [0, 2 pi) (f is then the angular
+// the wrapped phase itself, in radians in [0, float32(2 pi)] (f is then the angular
 // frequency in rad/sample and inv_sr = 1 / (2 pi)).
 __global__ void __launch_bounds__(kObThreads)
 oscbank_phase_out(const float* __restrict__ f, const unsigned long long* __restrict__ offs,

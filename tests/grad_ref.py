@@ -16,6 +16,10 @@ inputs live on.
   (symmetric Hann for odd windows, the padded / centred layout and its slicing,
   the `(S - 1) // 2 - 1` crop), and ragged frames (`frame = ceil(N / F)`, the last
   frame zero padded).
+* `fft_convolve`: shared (batch 1) or per-item impulse responses, 'valid' or
+  'same', any delay_compensation.
+* `oscillator_bank` / `angular_cumsum`: the stand-alone ops on audio-rate
+  envelopes (the Nyquist mask decided on the float32 frequencies).
 * `convolve_lti`: the long-impulse-response convolution (`FftConvolveLtiFn`,
   `Reverb`) at any crop.
 * `spectral_loss`: the multi-scale 'L1' spectrogram loss (`SpectralLossFn`) at any
@@ -88,6 +92,28 @@ def harmonic(f0_hz, amplitudes, harmonic_distribution, n_samples, sample_rate=16
   return (ae * torch.sin(phase)).sum(-1)
 
 
+def oscillator_bank(frequency_envelopes, amplitude_envelopes, sample_rate=16000,
+                    sum_sinusoids=True):
+  """core.oscillator_bank (core.py:911-962) on audio-rate envelopes [B, N, K]:
+  amplitude 0 where f >= sr / 2 (decided on the float32 frequencies, as the
+  reference decides it), phase = cumsum(f * 2 pi / sr), amp * sin(phase), summed
+  over K unless `sum_sinusoids` is False."""
+  f = frequency_envelopes.to(torch.float64)
+  a = amplitude_envelopes.to(torch.float64)
+  nyq = torch.tensor(sample_rate / 2.0, dtype=torch.float32)
+  a = torch.where(frequency_envelopes.to(torch.float32) >= nyq, torch.zeros_like(a), a)
+  phase = torch.cumsum(f * TWO_PI / float(sample_rate), dim=1)
+  audio = a * torch.sin(phase)
+  return audio.sum(-1) if sum_sinusoids else audio
+
+
+def angular_cumsum(angular_frequency):
+  """core.angular_cumsum (core.py:799-866) evaluated wide: the running sum of
+  [B, N, ...] angular frequencies over axis 1, wrapped into [0, 2 pi).  The
+  reference's chunking only changes its float32 rounding, so it is not restated."""
+  return torch.remainder(torch.cumsum(angular_frequency.to(torch.float64), dim=1), TWO_PI)
+
+
 def hann_window(n, dtype=torch.float64, device=None):
   """tf.signal.hann_window(n): periodic for even n, symmetric for odd n, [1] for
   n = 1 (oracle.hann_window)."""
@@ -121,11 +147,13 @@ def impulse_response(magnitudes, window_size=0):
   return torch.fft.fftshift(ir, dim=-1)
 
 
-def fft_convolve(audio, ir):
-  """core.fft_convolve(padding='same', delay_compensation=-1) (core.py:1382-1473)
-  of [B, N] audio with [B, F, S] impulse responses: frames of ceil(N / F) samples,
-  the last one zero padded, FFT size the next power of two of S + frame - 1."""
+def fft_convolve(audio, ir, padding='same', delay_compensation=-1):
+  """core.fft_convolve (core.py:1382-1473) of [B, N] audio with [B or 1, F, S]
+  impulse responses (batch 1 is shared by every item): frames of ceil(N / F)
+  samples, the last one zero padded, FFT size the next power of two of
+  S + frame - 1, then crop_and_compensate_delay with its Python slice."""
   audio = audio.to(torch.float64)
+  ir = ir.to(torch.float64)
   b, n = audio.shape
   _, f, s = ir.shape
   frame = -(-n // f)
@@ -143,8 +171,9 @@ def fft_convolve(audio, ir):
   out = out.reshape(b, (f + m - 1) * frame)[:, :total]
   # crop_and_compensate_delay, sliced as the reference slices (a window of one or
   # two taps gives start = -1)
-  start = (s - 1) // 2 - 1
-  end = total - n - start
+  crop_size = s + n - 1 if padding == 'valid' else n
+  start = (s - 1) // 2 - 1 if delay_compensation < 0 else delay_compensation
+  end = total - crop_size - start
   return out[:, start:-end]
 
 
@@ -393,6 +422,69 @@ def harmonic_v4_tile_width(B, F, K, hop, n_sms):
   return fw
 
 
+def harm_smem_bytes(ft, kp):
+  """harm_smem_bytes (harmonic.cuh): u64 P, A, D [FT] + red[8]; float f0, amp
+  [FT + 1]; float rows [(FT + 1) * Kp]."""
+  return 8 * (3 * ft + 8) + 4 * (2 * (ft + 1) + (ft + 1) * kp)
+
+
+def harmonic_generic_tile(B, F, K, hop, n_sms):
+  """The frames per tile (FT) ddsp_b200_harmonic_forward gives
+  harmonic_generic_kernel: FT = min(2048 / hop, max(ft_fill, min(4, F)), F), with
+  ft_fill = ceil(B F / (4 SMs)), then halved (fit_tile) until harm_smem_bytes fits
+  one CTA.  None where even one frame does not fit (E_UNSUPPORTED)."""
+  kp = (K + 3) & ~3
+  ft = max(1, 2048 // hop)
+  ft_fill = max(1, -(-(B * F) // (4 * n_sms)))
+  ft = min(ft, max(ft_fill, min(4, F)), F)
+  while ft > 1 and harm_smem_bytes(ft, kp) > MAX_DYN_SMEM:
+    ft = (ft + 1) // 2
+  return ft if harm_smem_bytes(ft, kp) <= MAX_DYN_SMEM else None
+
+
+def harmonic_route(B, F, K, hop, phase_mode, n_sms):
+  """'v4' or 'generic': the kernel core.harmonic_synthesis runs for an integer
+  hop and 'window' / 'linear' amplitudes."""
+  if phase_mode == 'recurrence' and harmonic_v4_tile_width(B, F, K, hop, n_sms) is not None:
+    return 'v4'
+  return 'generic'
+
+
+# harmonic_generic_kernel cases of tests/test_gpu_generic_edges.py: (B, F, K, hop,
+# sample_rate, amp method, f0 regime, phase_mode, accumulate, FT) with FT the frames
+# per tile harmonic_generic_tile gives on a 132-SM H100.  Every hop, K, mode,
+# method, rate and regime; FT = 2048 (hop 1), FT set by ft_fill with many tiles per
+# item, FT = F, FT = 1 at hop 8256, and halved by fit_tile (K = 10229 is the
+# smallest K that halves the 4-frame tile, K = 20000 halves 2 frames to 1).
+GENERIC_HARMONIC_CASES = [
+    (2, 600, 1, 1, 16000, 'linear', 'glide', 'recurrence', False, 4),
+    (64, 16896, 1, 1, 16000, 'linear', 'unvoiced', 'recurrence', False, 2048),
+    (3, 500, 60, 2, 44100, 'window', 'cross1hz', 'recurrence', True, 4),
+    (2, 70, 100, 31, 48000, 'linear', 'jump', 'direct', False, 4),
+    (8, 2000, 60, 33, 16000, 'window', 'glide', 'recurrence', False, 31),
+    (2, 40, 100, 63, 44100, 'linear', 'subhertz', 'recurrence', False, 4),
+    (2, 40, 100, 64, 16000, 'window', 'glide', 'direct', False, 4),
+    (1, 1, 60, 100, 16000, 'window', 'glide', 'recurrence', False, 1),
+    (3, 45, 60, 100, 48000, 'linear', 'nyquist', 'direct', True, 4),
+    (2, 50, 100, 160, 16000, 'linear', 'unvoiced', 'direct', False, 4),
+    (2, 3, 1025, 441, 44100, 'window', 'glide', 'recurrence', False, 3),
+    (1, 100, 60, 441, 44100, 'window', 'nyquist', 'recurrence', True, 4),
+    (2, 41, 60, 441, 44100, 'linear', 'glide', 'direct', False, 4),
+    (1, 33, 100, 480, 48000, 'window', 'jump', 'recurrence', False, 4),
+    (2, 7, 60, 1000, 16000, 'linear', 'cross1hz', 'direct', True, 2),
+    (1, 3, 60, 8256, 16000, 'window', 'subhertz', 'recurrence', False, 1),
+    (2, 25, 2048, 100, 48000, 'window', 'glide', 'recurrence', False, 4),
+    (1, 9, 10229, 441, 44100, 'linear', 'glide', 'recurrence', False, 2),
+    (1, 3, 20000, 1000, 48000, 'window', 'unvoiced', 'recurrence', False, 1),
+    # every harmonic live: the recurrence's whole chain at every sample
+    (2, 40, 100, 441, 44100, 'window', 'alllive', 'recurrence', False, 4),
+    (1, 30, 1024, 160, 16000, 'linear', 'alllive', 'recurrence', False, 4),
+    (1, 20, 2048, 480, 48000, 'window', 'alllive', 'recurrence', False, 4),
+    (1, 20, 4096, 441, 44100, 'window', 'alllive', 'recurrence', False, 4),
+    (1, 8, 4096, 441, 44100, 'linear', 'alllive', 'direct', False, 4),
+]
+
+
 # Forward filtered-noise cases of tests/test_gpu_forward_edges.py: (B, F, nb,
 # frame, window_size, r, route) with N = F * frame - r (r < F keeps ceil(N / F) =
 # frame).  route: 'fused2' / 'fused1' = noise_fused_kernel at two / one CTAs per
@@ -471,7 +563,7 @@ FWD_HARMONIC_CASES = [
 ]
 
 
-def low_f0_regime(regime, B, F, sample_rate, seed):
+def low_f0_regime(regime, B, F, sample_rate, seed, n_harmonics=None):
   """[B, F, 1] float32 f0 tracks for the edges of the harmonic kernels:
     'unvoiced'  - runs of f0 = 0 between voiced frames;
     'subhertz'  - runs of 0 < f0 < 1 Hz;
@@ -480,6 +572,9 @@ def low_f0_regime(regime, B, F, sample_rate, seed):
                   mask of the exact (f0 < 1 Hz) branch silences upper harmonics;
     'glide'     - fast glides whose live harmonic count changes inside most frames;
     'nyquist'   - runs of frames at or above sr / 2 (no live harmonic at all).
+    'alllive'   - every frame in [1.5 Hz, sr / (2 K)) for the K of `n_harmonics`:
+                  all K harmonics below Nyquist and no frame under 1 Hz, so the
+                  recurrence runs its whole chain at every sample.
   Voiced frames elsewhere sit at 80 .. 600 Hz."""
   g = torch.Generator().manual_seed(seed)
   base = 80.0 + 520.0 * torch.rand(B, F, 1, generator=g, dtype=torch.float64)
@@ -506,6 +601,11 @@ def low_f0_regime(regime, B, F, sample_rate, seed):
     f0 = torch.where(run, (0.5 + 0.2 * torch.rand(B, F, 1, generator=g,
                                                    dtype=torch.float64)) * sample_rate,
                      base)
+  elif regime == 'alllive':
+    # the top of the range stays 1e-3 below sr / (2 K), far more than the float32
+    # rounding of f0 * K and of the lerp
+    top = sample_rate / (2.0 * n_harmonics) * (1.0 - 1e-3)
+    f0 = 1.5 + (top - 1.5) * torch.rand(B, F, 1, generator=g, dtype=torch.float64)
   else:
     raise ValueError(regime)
   return f0.to(torch.float32)

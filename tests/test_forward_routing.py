@@ -101,3 +101,56 @@ def test_forward_harmonic_table_reaches_every_tile_width_and_hop():
   # the 64 KB shared-memory cap is what brings K = 1024 down to FW = 2
   assert grad_ref.harmonic_v4_smem(4, 1024, 64) > 64 * 1024
   assert grad_ref.harmonic_v4_tile_width(132, 16, 4, 64, H100_SMS) == 4
+
+
+@pytest.mark.parametrize('B,F,K,hop,sr,method,regime,mode,acc,ft',
+                         grad_ref.GENERIC_HARMONIC_CASES)
+def test_generic_harmonic_cases_tile_as_tabled(B, F, K, hop, sr, method, regime, mode, acc,
+                                               ft):
+  assert grad_ref.harmonic_route(B, F, K, hop, mode, H100_SMS) == 'generic'
+  assert grad_ref.harmonic_generic_tile(B, F, K, hop, H100_SMS) == ft
+
+
+def test_generic_harmonic_table_reaches_every_tile_regime():
+  """FT = 2048 (hop 1), FT set by ft_fill, FT = F, FT = 1 through fit_tile's halving
+  (and halved 4 -> 2 at the smallest K that needs it); every hop, K, mode, regime
+  and rate the generic kernel is asked for."""
+  rows = grad_ref.GENERIC_HARMONIC_CASES
+  tile = grad_ref.harmonic_generic_tile
+
+  def unhalved(B, F, hop):
+    ft_fill = max(1, -(-(B * F) // (4 * H100_SMS)))
+    return min(max(1, 2048 // hop), max(ft_fill, min(4, F)), F), ft_fill
+
+  regimes = set()
+  for B, F, K, hop, *_, ft in rows:
+    ft0, ft_fill = unhalved(B, F, hop)
+    if ft == 2048:
+      regimes.add('2048')
+    if ft == ft0 == ft_fill and ft_fill > min(4, F):
+      regimes.add('ft_fill')
+    if ft == F and F > 1:
+      regimes.add('F')
+    if ft < ft0:
+      regimes.add('halved to %d' % ft)
+  assert regimes >= {'2048', 'ft_fill', 'F', 'halved to 1', 'halved to 2'}
+  # K = 10229 is the smallest K for which the 4-frame tile must halve
+  assert tile(1, 9, 10228, 441, H100_SMS) == 4 and tile(1, 9, 10229, 441, H100_SMS) == 2
+  # K = 25584 fits one frame, one more does not (E_UNSUPPORTED)
+  assert tile(1, 3, 25584, 8256, H100_SMS) == 1 and tile(1, 3, 25585, 8256, H100_SMS) is None
+  # ft_fill's tiles leave > 256 frames before most tiles: a strided f0 prefix
+  assert any(F - ft > 256 and unhalved(B, F, hop)[1] == ft
+             for B, F, _, hop, *_, ft in rows)
+  assert {hop for _, _, _, hop, *_ in rows} >= {1, 2, 31, 33, 63, 64, 100, 160, 441, 480,
+                                                1000, 8256}
+  assert {K for _, _, K, *_ in rows} >= {1, 60, 100, 1025, 2048, 4096, 10229, 20000}
+  assert {r[6] for r in rows} == {'unvoiced', 'subhertz', 'cross1hz', 'jump', 'glide',
+                                  'nyquist', 'alllive'}
+  assert {r[2] for r in rows if r[6] == 'alllive'} >= {100, 1024, 2048, 4096}
+  assert {r[7] for r in rows} == {'recurrence', 'direct'}
+  assert {r[5] for r in rows} == {'window', 'linear'}
+  assert {r[4] for r in rows} == {16000, 44100, 48000}
+  assert any(r[8] for r in rows) and any(r[1] == 1 for r in rows)
+  # 'direct' at hop 64, where 'recurrence' would take harmonic_v4_kernel
+  assert grad_ref.harmonic_route(2, 40, 100, 64, 'recurrence', H100_SMS) == 'v4'
+  assert (2, 40, 100, 64, 16000, 'window', 'glide', 'direct', False, 4) in rows

@@ -122,3 +122,75 @@ def test_references_are_differentiable_in_float64():
   grad_ref.spectral_loss(target, value, (256, 64), 1.0, 1.0).backward()
   assert value.grad.dtype == torch.float64 and torch.isfinite(value.grad).all()
   assert float(value.grad.abs().max()) > 0
+
+
+@pytest.mark.parametrize('B,N,K,sr,sum_sinusoids', [(2, 300, 5, 16000, True),
+                                                    (1, 1, 1, 44100, True),
+                                                    (3, 700, 129, 48000, False)])
+def test_oscillator_bank_reference_matches_oracle(B, N, K, sr, sum_sinusoids):
+  """Negative frequencies, frequencies above Nyquist, and exactly at and one
+  float32 ulp below it (silenced and live: the mask is >=)."""
+  rng = np.random.default_rng(N + K)
+  f = (rng.uniform(-0.3, 0.55, (B, N, K)) * sr).astype(np.float32)
+  f[:, ::7, 0] = np.float32(sr / 2)
+  if K > 1:
+    f[:, ::7, 1] = np.nextafter(np.float32(sr / 2), np.float32(0))
+  a = rng.uniform(0.1, 1.0, (B, N, K)).astype(np.float32)
+  got = grad_ref.oscillator_bank(torch.from_numpy(f), torch.from_numpy(a), sr, sum_sinusoids)
+  want = o.oscillator_bank(f, a, sample_rate=sr, sum_sinusoids=sum_sinusoids)
+  assert got.shape == want.shape
+  assert _rel(got.numpy(), want) <= 1e-12
+  if not sum_sinusoids:
+    assert not want[:, ::7, 0].any() and want[:, 7::7, 1].any()
+
+
+@pytest.mark.parametrize('shape', [(2, 1), (3, 2500), (2, 1001, 3), (1, 999, 2, 3)])
+def test_angular_cumsum_reference_matches_oracle(shape):
+  """The wrapped running sum against the oracle's chunked angular_cumsum in float64
+  (chunks of 1000, the default), compared on the circle."""
+  x = np.random.default_rng(len(shape) + shape[1]).uniform(-np.pi, np.pi, shape)
+  got = grad_ref.angular_cumsum(torch.from_numpy(x)).numpy()
+  want = o.angular_cumsum(x)
+  assert got.shape == want.shape
+  assert got.min() >= 0.0 and got.max() < 2 * np.pi
+  d = np.mod(got - want, 2 * np.pi)
+  assert np.minimum(d, 2 * np.pi - d).max() <= 1e-12
+
+
+@pytest.mark.parametrize('B,N,F,S,ir_batch,padding,delay', [
+    (2, 1000, 7, 129, 2, 'valid', 0),
+    (3, 1000, 7, 128, 1, 'same', -1),
+    (2, 1000, 1, 129, 1, 'same', 300),
+    (2, 64, 64, 2047, 2, 'same', 1023),
+    (3, 6000, 5, 3000, 1, 'valid', -1),
+    (2, 4001, 5, 4096, 2, 'same', -1),
+])
+def test_fft_convolve_reference_matches_oracle(B, N, F, S, ir_batch, padding, delay):
+  """grad_ref.fft_convolve with shared (batch 1) and per-item impulse responses,
+  'valid' and 'same', automatic and explicit delays."""
+  rng = np.random.default_rng(N + S)
+  audio = rng.standard_normal((B, N))
+  ir = rng.standard_normal((ir_batch, F, S)) / np.sqrt(S)
+  got = grad_ref.fft_convolve(torch.from_numpy(audio), torch.from_numpy(ir), padding, delay)
+  want = o.fft_convolve(audio, np.broadcast_to(ir, (B, F, S)), padding=padding,
+                        delay_compensation=delay)
+  assert got.shape == want.shape and want.shape[1] > 0
+  assert _rel(got.numpy(), want) <= 1e-12
+
+
+@pytest.mark.parametrize('K,sr', [(100, 44100), (1024, 16000), (4096, 44100)])
+def test_alllive_regime_keeps_every_harmonic_live(K, sr):
+  """'alllive' f0 tracks: every frame in [1.5 Hz, sr / (2 K)), so the float32
+  Nyquist decision keeps all K harmonics at every sample, and the harmonic
+  reference matches the oracle there."""
+  f0 = grad_ref.low_f0_regime('alllive', 2, 12, sr, seed=K, n_harmonics=K)
+  assert float(f0.min()) >= 1.5 and float(f0.max()) * K < sr / 2
+  assert not grad_ref.nyquist_mask(f0, K, 12 * 50, sr).any()
+  g = torch.Generator().manual_seed(K)
+  amp = torch.rand(2, 12, 1, generator=g) + 0.2
+  hd = torch.rand(2, 12, K, generator=g)
+  hd = hd / hd.sum(-1, keepdim=True)
+  got = grad_ref.harmonic(f0, amp, hd, 12 * 50, sr, 'linear')
+  want = o.harmonic_synthesis(f0.numpy(), amp.numpy(), harmonic_distribution=hd.numpy(),
+                              n_samples=12 * 50, sample_rate=sr, amp_resample_method='linear')
+  assert _rel(got.numpy(), want) <= 1e-12
