@@ -75,6 +75,15 @@ SIGNATURES = {
     'ddsp_b200_noise_controls_backward': (_i, [_vp, _vp, _vp, _i64, _f, _vp]),
     'ddsp_b200_filtered_noise_backward':
         (_i, [_vp, _vp, _u64, _u64, _vp, _i, _i, _i, _i, _i, _vp]),
+    'ddsp_b200_fir_time_varying_backward_workspace': (_sz, [_i, _i, _i, _i, _i]),
+    'ddsp_b200_fir_time_varying_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+    'ddsp_b200_frequency_impulse_response_backward':
+        (_i, [_vp, _vp, _i64, _i, _i, _vp]),
+    'ddsp_b200_frequency_filter_backward_workspace':
+        (_sz, [_i, _i, _i, _i, _i, _i, _i]),
+    'ddsp_b200_frequency_filter_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
     'ddsp_b200_oscillator_bank_workspace': (_sz, [_i, _i, _i]),
     'ddsp_b200_oscillator_bank':
         (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _i, _vp, _sz, _vp]),

@@ -15,6 +15,11 @@ kernels, exposed as `torch.autograd.Function`s:
     grad); `core.sinusoidal_synthesis` routes to it under grad;
   * `FftConvolveLtiFn` / `ModDelayFn` - the reverb convolution and the modulated
     delay, routed to by `core.fft_convolve` / `core.mod_delay` under grad;
+  * `FirTimeVaryingFn` / `FrequencyImpulseResponseFn` / `FrequencyFilterFn` - the
+    direct-form time-varying FIR (impulse responses under 2048 taps: FIRFilter,
+    short reverbs), the impulse-response synthesis and their composition, routed to
+    by `core.fft_convolve` / `core.frequency_impulse_response` /
+    `core.frequency_filter` under grad;
   * `DecoderFn` / `decoder_train` - the whole `ae.gin` decoder from RAW network
     outputs: forward is the fused two-kernel pipeline (`get_controls` in shared
     memory), backward is the two synthesizer backward kernels plus the
@@ -200,6 +205,105 @@ class FftConvolveLtiFn(torch.autograd.Function):
       if ir_batch == 1 and b > 1:
         d_ir = d_ir.sum(0, keepdim=True)
     return d_audio, d_ir, None, None
+
+
+class FirTimeVaryingFn(torch.autograd.Function):
+  """core.fft_convolve on its direct-form route (impulse responses [1 or B, F, S]
+  with S < FFT_CONVOLVE_MIN_IR), differentiable in audio and impulse response: one
+  backward call of `ddsp_b200_fir_time_varying_backward` (csrc/fir_backward.cuh)
+  computes the gradients asked for.  `delay` is the crop start (< 0: automatic)."""
+
+  @staticmethod
+  def forward(ctx, audio, ir, padding, delay):
+    audio = core.torch_float32(audio)
+    ir = core.torch_float32(ir)
+    ctx.save_for_backward(audio, ir)
+    ctx.cfg = (padding, int(delay))
+    return core.fft_convolve(audio, ir, padding=padding, delay_compensation=delay)
+
+  @staticmethod
+  def backward(ctx, g):
+    audio, ir = ctx.saved_tensors
+    padding, delay = ctx.cfg
+    b, n = audio.shape
+    ir_batch, f, s = ir.shape
+    g = g.contiguous().to(torch.float32)
+    lib = _lib.load()
+    with core._on_device_of(audio, ir, g):
+      d_audio = torch.empty_like(audio) if ctx.needs_input_grad[0] else None
+      d_ir = torch.empty_like(ir) if ctx.needs_input_grad[1] else None
+      nbytes = (lib.ddsp_b200_fir_time_varying_backward_workspace(b, n, f, s, ir_batch)
+                if d_ir is not None else 0)
+      ws = core._workspace(nbytes, audio.device)
+      _lib.check(lib.ddsp_b200_fir_time_varying_backward(
+          audio.data_ptr(), ir.data_ptr(), g.data_ptr(), core._ptr(d_audio),
+          core._ptr(d_ir), b, n, f, s, ir_batch,
+          _lib.PAD_SAME if padding == 'same' else _lib.PAD_VALID, delay, core._ptr(ws),
+          nbytes, core._stream()))
+    return d_audio, d_ir, None, None
+
+
+class FrequencyImpulseResponseFn(torch.autograd.Function):
+  """core.frequency_impulse_response, differentiable in the magnitudes:
+  `ddsp_b200_frequency_impulse_response_backward` is the transpose of the windowed
+  cosine sum."""
+
+  @staticmethod
+  def forward(ctx, magnitudes, window_size):
+    magnitudes = core.torch_float32(magnitudes)
+    ctx.cfg = (tuple(magnitudes.shape), int(window_size))
+    return core.frequency_impulse_response(magnitudes, window_size=window_size)
+
+  @staticmethod
+  def backward(ctx, d_ir):
+    shape, window_size = ctx.cfg
+    nb = shape[-1]
+    d_ir = d_ir.contiguous().to(torch.float32)
+    with core._on_device_of(d_ir):
+      d_mags = torch.empty(shape, dtype=torch.float32, device=d_ir.device)
+      _lib.check(_lib.load().ddsp_b200_frequency_impulse_response_backward(
+          d_ir.data_ptr(), d_mags.data_ptr(), d_mags.numel() // nb, nb, window_size,
+          core._stream()))
+    return d_mags, None
+
+
+class FrequencyFilterFn(torch.autograd.Function):
+  """core.frequency_filter on the direct-form route (impulse responses shorter than
+  FFT_CONVOLVE_MIN_IR), differentiable in audio and magnitudes.  The forward's
+  impulse responses are saved, not recomputed; one backward call of
+  `ddsp_b200_frequency_filter_backward`, which picks the d magnitudes route."""
+
+  @staticmethod
+  def forward(ctx, audio, magnitudes, window_size, padding):
+    audio = core.torch_float32(audio)
+    magnitudes = core.torch_float32(magnitudes)
+    ir = core.frequency_impulse_response(magnitudes, window_size=window_size)
+    ctx.save_for_backward(audio, ir)
+    ctx.cfg = (tuple(magnitudes.shape), int(window_size), padding)
+    return core.fft_convolve(audio, ir, padding=padding)
+
+  @staticmethod
+  def backward(ctx, g):
+    audio, ir = ctx.saved_tensors
+    shape, window_size, padding = ctx.cfg
+    b, n = audio.shape
+    mb, nb = shape[0], shape[-1]
+    f = shape[1] if len(shape) == 3 else 1
+    pad = _lib.PAD_SAME if padding == 'same' else _lib.PAD_VALID
+    g = g.contiguous().to(torch.float32)
+    lib = _lib.load()
+    with core._on_device_of(audio, ir, g):
+      d_audio = torch.empty_like(audio) if ctx.needs_input_grad[0] else None
+      d_mags = (torch.empty(shape, dtype=torch.float32, device=audio.device)
+                if ctx.needs_input_grad[1] else None)
+      nbytes = (lib.ddsp_b200_frequency_filter_backward_workspace(
+          b, f, nb, n, mb, window_size, pad) if d_mags is not None else 0)
+      ws = core._workspace(nbytes, audio.device)
+      _lib.check(lib.ddsp_b200_frequency_filter_backward(
+          audio.data_ptr(), ir.data_ptr(), g.data_ptr(), core._ptr(d_audio),
+          core._ptr(d_mags), b, f, nb, n, mb, window_size, pad, core._ptr(ws), nbytes,
+          core._stream()))
+    return d_audio, d_mags, None, None
 
 
 class FilteredNoiseFn(torch.autograd.Function):

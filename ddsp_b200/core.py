@@ -745,13 +745,35 @@ def get_fft_size(frame_size: int, ir_size: int, power_of_2: bool = True) -> int:
   raise NotImplementedError('power_of_2=False needs scipy.fftpack.')
 
 
+def _ir_size(nb, window_size):
+  """Taps of the windowed impulse response of nb bins (`ddsp_b200_ir_size`):
+  window_size if odd, one less if even, 2 (nb - 1) without a window."""
+  s0 = 2 * (nb - 1)
+  ws = s0 if window_size <= 0 or window_size > s0 else window_size
+  return 2 * ((ws + 1) // 2) - 1 if ws < s0 else s0
+
+
+def _check_n_frequencies(nb):
+  if nb < 2:
+    raise ValueError(f'frequency_impulse_response needs >= 2 frequencies, got {nb}.')
+
+
+def _requires_grad(*tensors):
+  return torch.is_grad_enabled() and any(
+      isinstance(t, torch.Tensor) and t.requires_grad for t in tensors)
+
+
 def frequency_impulse_response(magnitudes, window_size: int = 0):
-  """core.frequency_impulse_response (core.py:1534-1565)."""
+  """core.frequency_impulse_response (core.py:1534-1565).  Routes to
+  `autograd.FrequencyImpulseResponseFn` when grad is enabled and the magnitudes
+  require it."""
   nb = int(_shape(magnitudes)[-1])
+  _check_n_frequencies(nb)
+  if _requires_grad(magnitudes):
+    from ddsp_b200 import autograd as _ag
+    return _ag.FrequencyImpulseResponseFn.apply(magnitudes, int(window_size))
   lib = _lib.load()
   s = lib.ddsp_b200_ir_size(nb, int(window_size))
-  if s < 0:
-    raise ValueError(f'frequency_impulse_response needs >= 2 frequencies, got {nb}.')
   magnitudes = torch_float32(magnitudes)
   ir = torch.empty(tuple(magnitudes.shape[:-1]) + (s,), dtype=torch.float32,
                    device=magnitudes.device)
@@ -882,15 +904,11 @@ def fft_convolve_lti(audio, impulse_response, start, out_len, out=None,
   return out
 
 
-def fft_convolve(audio, impulse_response, padding: Text = 'same',
-                 delay_compensation: int = -1, out=None, accumulate=False):
-  """core.fft_convolve (core.py:1382-1473).
-
-  Computed as the mathematically identical direct-form time-varying FIR
-  (frame / rfft / multiply / irfft / overlap_and_add / crop folded into index
-  math; SURVEY.md A.6) - the name is kept for drop-in compatibility.
-  """
-  sa, si = _shape(audio), _shape(impulse_response)
+def _fft_convolve_geometry(sa, si, padding, delay_compensation):
+  """The shape checks of core.fft_convolve (core.py:1382-1473) on the static shapes
+  of audio and impulse response, and what follows from them: (batch, audio size,
+  [ir_batch, n_ir_frames, ir_size], frame size, FFT size, crop start, crop length,
+  crop size)."""
   if len(sa) != 2 or len(si) not in (2, 3):
     raise ValueError(f'audio must be [batch, time] and impulse_response 2-D or '
                      f'3-D; got {sa} and {si}.')
@@ -915,6 +933,22 @@ def fft_convolve(audio, impulse_response, padding: Text = 'same',
   total_size = (n_ir_frames - 1) * frame_size + fft_size
   start, out_len, crop_size = _crop_range(total_size, audio_size, ir_size,
                                           padding, delay_compensation)
+  return (batch_size, audio_size, si, frame_size, fft_size, start, out_len,
+          crop_size)
+
+
+def fft_convolve(audio, impulse_response, padding: Text = 'same',
+                 delay_compensation: int = -1, out=None, accumulate=False):
+  """core.fft_convolve (core.py:1382-1473).
+
+  Computed as the mathematically identical direct-form time-varying FIR
+  (frame / rfft / multiply / irfft / overlap_and_add / crop folded into index
+  math; SURVEY.md A.6) - the name is kept for drop-in compatibility.
+  """
+  sa, si = _shape(audio), _shape(impulse_response)
+  (batch_size, audio_size, si, frame_size, fft_size, start, out_len,
+   crop_size) = _fft_convolve_geometry(sa, si, padding, delay_compensation)
+  ir_batch, n_ir_frames, ir_size = si
   if out_len != crop_size:
     # The reference's `audio[:, start:-end]` degenerates when end <= 0 (e.g.
     # end == 0 yields an empty tensor).  Reproduce the empty case; refuse the
@@ -961,6 +995,20 @@ def fft_convolve(audio, impulse_response, padding: Text = 'same',
     else:
       out.copy_(wet)
     return out
+  if _requires_grad(audio, impulse_response):
+    # time-varying FIR under training (FIRFilter, short reverbs): CUDA backward
+    # kernels for both operands (csrc/fir_backward.cuh)
+    if out is not None:
+      _check_out(out, (batch_size, crop_size), audio)
+    from ddsp_b200 import autograd as _ag
+    wet = _ag.FirTimeVaryingFn.apply(audio, impulse_response, padding, int(start))
+    if out is None:
+      return wet
+    if accumulate:
+      out += wet
+    else:
+      out.copy_(wet)
+    return out
   if out is None:
     out = torch.empty((batch_size, crop_size), dtype=torch.float32,
                       device=audio.device)
@@ -968,7 +1016,6 @@ def fft_convolve(audio, impulse_response, padding: Text = 'same',
   else:
     _check_out(out, (batch_size, crop_size), audio)
   impulse_response = impulse_response.contiguous()
-  _no_grad_path('fft_convolve', audio, impulse_response)
   with _on_device_of(audio, impulse_response, out):
     _lib.check(_lib.load().ddsp_b200_fir_time_varying(
         _ptr(audio), _ptr(impulse_response), _ptr(out), batch_size,
@@ -980,7 +1027,20 @@ def fft_convolve(audio, impulse_response, padding: Text = 'same',
 
 def frequency_filter(audio, magnitudes, window_size: int = 0,
                      padding: Text = 'same'):
-  """core.frequency_filter (core.py:1628-1655)."""
+  """core.frequency_filter (core.py:1628-1655).  When grad is enabled and an input
+  requires it, impulse responses under FFT_CONVOLVE_MIN_IR taps route to
+  `autograd.FrequencyFilterFn` (one backward call for both gradients); longer ones
+  compose `FrequencyImpulseResponseFn` with fft_convolve's long-IR route."""
+  if _requires_grad(audio, magnitudes):
+    sm = _shape(magnitudes)
+    nb = int(sm[-1])
+    _check_n_frequencies(nb)
+    s = _ir_size(nb, int(window_size))
+    _, _, _, _, _, _, out_len, crop_size = _fft_convolve_geometry(
+        _shape(audio), tuple(sm[:-1]) + (s,), padding, -1)
+    if s < FFT_CONVOLVE_MIN_IR and out_len == crop_size:
+      from ddsp_b200 import autograd as _ag
+      return _ag.FrequencyFilterFn.apply(audio, magnitudes, int(window_size), padding)
   impulse_response = frequency_impulse_response(magnitudes,
                                                 window_size=window_size)
   return fft_convolve(audio, impulse_response, padding=padding)

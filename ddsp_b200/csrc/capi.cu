@@ -22,6 +22,7 @@
 #include "longconv.cuh"
 #include "spectral.cuh"
 #include "mod_delay.cuh"
+#include "fir_backward.cuh"
 
 namespace ddsp {
 
@@ -685,6 +686,45 @@ int ddsp_b200_noise_controls_backward(const float* mags_raw, const float* d_mags
   return 0;
 }
 
+// NoiseBwdParams of a filtered-noise (or frequency_filter) shape whose frame is
+// `frame`; *n_tiles and *smem are what the launch needs (the caller checks them).
+static NoiseBwdParams noise_bwd_params(const float* grad, const float* noise, uint64_t seed,
+                                       uint64_t offset, float* dmags, int B, int F, int nb,
+                                       int N, int frame, int window_size, long long* n_tiles,
+                                       size_t* smem) {
+  NoiseBwdParams p;
+  p.grad = grad; p.noise = noise; p.dmags = dmags;
+  p.seed = seed; p.offset = offset;
+  p.B = B; p.F = F; p.nb = nb; p.N = N; p.frame = frame;
+  p.g = make_ir_geom(nb, window_size);
+  p.S = p.g.S;
+  p.start = (p.S - 1) / 2 - 1;
+  p.ylen = frame + p.S - 1;
+  p.nh = p.g.S0 / 2 + 1;
+  p.xS = (((frame + 15) & ~15) + 1) | 1;
+  p.gS = (((frame + 15) & ~15) + p.S + 17) | 1;
+  p.hS = (p.S + p.nh) | 1;
+  p.tiles_per_item = (F + 31) / 32;
+  *n_tiles = (long long)B * p.tiles_per_item;
+  p.n_tiles = (int)std::min<long long>(*n_tiles, INT32_MAX);
+  p.eo_tab = (nb == 65 && p.g.S0 == 128 && p.nh == 65) ? 1 : 0;
+  *smem = sizeof(float) * (noise_bwd_eo_offset(p) +
+                           (p.eo_tab ? (size_t)p.nh * kEoStride : 0));
+  return p;
+}
+
+// Launches noise_backward_kernel on checked parameters.
+static int noise_bwd_launch(const NoiseBwdParams& p, size_t smem, cudaStream_t st,
+                            const char* name) {
+  int rc = set_smem(noise_backward_kernel, smem, name);
+  if (rc) return rc;
+  const int per_sm = smem <= 100 * 1024 ? 2 : 1;
+  const int grid = (int)std::min<long long>(p.n_tiles, (long long)num_sms() * per_sm);
+  noise_backward_kernel<<<grid, kNbThreads, smem, st>>>(p);
+  DDSP_CHECK_LAUNCH(name);
+  return 0;
+}
+
 int ddsp_b200_filtered_noise_backward(const float* grad_audio, const float* noise,
                                       uint64_t seed, uint64_t offset, float* dmags,
                                       int B, int F, int nb, int N, int window_size,
@@ -696,37 +736,251 @@ int ddsp_b200_filtered_noise_backward(const float* grad_audio, const float* nois
   const int frame = ir_frame(N, F);
   if (!frame) return DDSP_B200_E_INVALID;
   if (B == 0) return 0;
-  NoiseBwdParams p;
-  p.grad = grad_audio; p.noise = noise; p.dmags = dmags;
-  p.seed = seed; p.offset = offset;
-  p.B = B; p.F = F; p.nb = nb; p.N = N; p.frame = frame;
-  p.g = make_ir_geom(nb, window_size);
-  p.S = p.g.S;
-  p.start = (p.S - 1) / 2 - 1;
+  long long n_tiles;
+  size_t smem;
+  NoiseBwdParams p = noise_bwd_params(grad_audio, noise, seed, offset, dmags, B, F, nb, N,
+                                      frame, window_size, &n_tiles, &smem);
   DDSP_REQUIRE(p.start >= 0, DDSP_B200_E_UNSUPPORTED,
                "filtered_noise_backward: impulse response too short");
-  p.ylen = frame + p.S - 1;
-  p.nh = p.g.S0 / 2 + 1;
-  p.xS = (((frame + 15) & ~15) + 1) | 1;
-  p.gS = (((frame + 15) & ~15) + p.S + 17) | 1;
-  p.hS = (p.S + p.nh) | 1;
-  p.tiles_per_item = (F + 31) / 32;
-  const long long n_tiles = (long long)B * p.tiles_per_item;
   DDSP_REQUIRE(n_tiles < (1ll << 31), DDSP_B200_E_INVALID,
                "filtered_noise_backward: too many tiles");
-  p.n_tiles = (int)n_tiles;
-  p.eo_tab = (nb == 65 && p.g.S0 == 128 && p.nh == 65) ? 1 : 0;
-  const size_t smem = sizeof(float) * (noise_bwd_eo_offset(p) +
-                                       (p.eo_tab ? (size_t)p.nh * kEoStride : 0));
   DDSP_REQUIRE(smem <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
                "filtered_noise_backward: shape needs %zu B of shared memory", smem);
-  int rc = set_smem(noise_backward_kernel, smem, "filtered_noise_backward");
-  if (rc) return rc;
-  const int per_sm = smem <= 100 * 1024 ? 2 : 1;
-  const int grid = (int)std::min<long long>(n_tiles, (long long)num_sms() * per_sm);
-  noise_backward_kernel<<<grid, kNbThreads, smem, (cudaStream_t)stream>>>(p);
-  DDSP_CHECK_LAUNCH("filtered_noise_backward");
+  return noise_bwd_launch(p, smem, (cudaStream_t)stream, "filtered_noise_backward");
+}
+
+// ---- backward of the time-varying FIR and of the impulse-response synthesis ----
+// The shared memory of ir_backward_kernel: the cosine table, padded to a float4, and
+// kIrFrames rows of nb folded taps.
+static size_t ir_backward_smem(const IrGeom& g) {
+  return sizeof(float) * ((((size_t)g.S0 + 3) & ~(size_t)3) + (size_t)kIrFrames * g.nb);
+}
+
+// FirDirParams of a shape (frame from ir_frame); out is set by the caller.
+static FirDirParams fir_dir_params(const float* x, const float* grad, int B, int N, int F,
+                                   int S, int frame, int start, int out_len) {
+  FirDirParams p;
+  p.x = x; p.g = grad; p.out = nullptr;
+  p.N = N; p.S = S; p.F = F; p.frame = frame; p.start = start; p.out_len = out_len;
+  fir_dir_segments(frame, &p.n_chunk, &p.seg);
+  p.segp = (p.seg + 15) & ~15;
+  p.xS = p.segp + 1;
+  p.gS = p.segp + kDirTaps + 1;
+  p.n_rows = (long long)B * F * p.n_chunk;
+  return p;
+}
+
+// Bytes of partial d IR sums a shape needs: none when every frame is one segment and
+// every item has its own impulse response.
+static size_t fir_dir_part_bytes(int B, int N, int F, int S, int ir_batch, int frame) {
+  int n_chunk, seg;
+  fir_dir_segments(frame, &n_chunk, &seg);
+  (void)N;
+  if (n_chunk == 1 && !(ir_batch == 1 && B > 1)) return 0;
+  return sizeof(float) * (size_t)B * F * n_chunk * S;
+}
+
+// The checks of the FIR backward shared by both entry points, after the null-pointer
+// and shape checks; sets *frame, *start and *out_len.  The caller returns 0 for B == 0.
+static int fir_bwd_check(const char* name, int B, int N, int F, int S, int ir_batch,
+                         int padding, int delay_compensation, int* frame, int* start,
+                         int* out_len) {
+  // core.py:1441-1443
+  DDSP_REQUIRE(ir_batch == B || ir_batch == 1, DDSP_B200_E_INVALID,
+               "Batch size of audio (%d) and impulse response (%d) must be the "
+               "same.", B, ir_batch);
+  DDSP_REQUIRE(padding == DDSP_B200_PAD_SAME || padding == DDSP_B200_PAD_VALID,
+               DDSP_B200_E_INVALID,
+               "Padding must be 'valid' or 'same' (got code %d)", padding);
+  *frame = ir_frame(N, F);
+  if (!*frame) return DDSP_B200_E_INVALID;
+  if (B == 0) return 0;
+  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID, "%s: B=%d exceeds the 65535 grid limit",
+               name, B);
+  *out_len = (padding == DDSP_B200_PAD_VALID) ? (N + S - 1) : N;
+  *start = delay_compensation < 0 ? ((S - 1) / 2 - 1) : delay_compensation;
+  DDSP_REQUIRE(*start >= 0, DDSP_B200_E_UNSUPPORTED,
+               "%s: impulse response of %d taps gives a negative automatic delay", name,
+               S);
+  DDSP_REQUIRE(sizeof(float) * ((size_t)kFadjThreads + S - 1) <= kMaxDynSmem,
+               DDSP_B200_E_UNSUPPORTED,
+               "%s: impulse response of %d taps is beyond the shared-memory FIR", name, S);
+  int n_chunk, seg;
+  fir_dir_segments(*frame, &n_chunk, &seg);
+  DDSP_REQUIRE((long long)B * F * n_chunk / kDirRows < (1ll << 31) &&
+                   (long long)ir_batch * F / kIrFrames < (1ll << 31),
+               DDSP_B200_E_INVALID, "%s: too many frames", name);
   return 0;
+}
+
+// Launches d audio (when d_audio is set) and d IR (when d_ir is set) of a checked shape.
+// `part` holds fir_dir_part_bytes of partial sums when that is not 0.
+static int fir_bwd_launch(const float* audio, const float* ir, const float* grad,
+                          float* d_audio, float* d_ir, int B, int N, int F, int S,
+                          int ir_batch, int frame, int start, int out_len, float* part,
+                          cudaStream_t st, const char* name) {
+  if (d_audio) {
+    const size_t smem = sizeof(float) * ((size_t)kFadjThreads + S - 1);
+    int rc = set_smem(fir_adjoint_kernel, smem, name);
+    if (rc) return rc;
+    dim3 grid((N + kFadjThreads - 1) / kFadjThreads, B);
+    fir_adjoint_kernel<<<grid, kFadjThreads, smem, st>>>(
+        grad, ir, d_audio, N, S, frame, ir_batch == 1 ? 0 : F * S, start, out_len);
+    DDSP_CHECK_LAUNCH(name);
+  }
+  if (d_ir) {
+    FirDirParams p = fir_dir_params(audio, grad, B, N, F, S, frame, start, out_len);
+    p.out = part ? part : d_ir;
+    const size_t smem = fir_dir_smem(p);
+    int rc = set_smem(fir_dir_kernel, smem, name);
+    if (rc) return rc;
+    dim3 grid((unsigned)((p.n_rows + kDirRows - 1) / kDirRows),
+              (unsigned)((S + kDirTaps - 1) / kDirTaps));
+    fir_dir_kernel<<<grid, kDirThreads, smem, st>>>(p);
+    DDSP_CHECK_LAUNCH(name);
+    if (part) {
+      const long long n_out = (long long)ir_batch * F * S;
+      fir_dir_reduce<<<grid_for(n_out, 256), 256, 0, st>>>(
+          part, d_ir, B, F, S, p.n_chunk, ir_batch == 1 && B > 1, n_out);
+      DDSP_CHECK_LAUNCH(name);
+    }
+  }
+  return 0;
+}
+
+// The route of frequency_filter's d magnitudes: the fused noise_backward_kernel reads
+// the audio as its noise when the padding is 'same', every item has its own magnitudes
+// and the shape fits its shared memory; otherwise d IR (fir_dir_kernel) and the IR
+// adjoint (ir_backward_kernel) through the workspace.
+static bool freq_filter_fused(int B, int F, int nb, int N, int frame, int mags_batch,
+                              int window_size, int padding) {
+  if (padding != DDSP_B200_PAD_SAME || mags_batch != B) return false;
+  long long n_tiles;
+  size_t smem;
+  noise_bwd_params(nullptr, nullptr, 0, 0, nullptr, B, F, nb, N, frame, window_size,
+                   &n_tiles, &smem);
+  return n_tiles < (1ll << 31) && smem <= kMaxDynSmem;
+}
+
+size_t ddsp_b200_fir_time_varying_backward_workspace(int B, int N, int F, int S,
+                                                     int ir_batch) {
+  if (B <= 0 || N <= 0 || F <= 0 || S <= 0 || (ir_batch != 1 && ir_batch != B)) return 0;
+  const int frame = (N + F - 1) / F;
+  if ((N + frame - 1) / frame != F) return 0;
+  const size_t part = fir_dir_part_bytes(B, N, F, S, ir_batch, frame);
+  return part ? part + 256 : 0;
+}
+
+int ddsp_b200_fir_time_varying_backward(const float* audio, const float* ir,
+                                        const float* grad, float* d_audio, float* d_ir,
+                                        int B, int N, int F, int S, int ir_batch,
+                                        int padding, int delay_compensation,
+                                        void* workspace, size_t workspace_bytes,
+                                        void* stream) {
+  const char* name = "fir_time_varying_backward";
+  DDSP_REQUIRE(audio && ir && grad, DDSP_B200_E_INVALID, "%s: null pointer", name);
+  DDSP_REQUIRE(B >= 0 && N >= 1 && F >= 1 && S >= 1, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d N=%d F=%d S=%d", name, B, N, F, S);
+  int frame = 0, start = 0, out_len = 0;
+  int rc = fir_bwd_check(name, B, N, F, S, ir_batch, padding, delay_compensation, &frame,
+                         &start, &out_len);
+  if (rc || B == 0) return rc;
+  const size_t need =
+      d_ir ? ddsp_b200_fir_time_varying_backward_workspace(B, N, F, S, ir_batch) : 0;
+  DDSP_REQUIRE(need == 0 || (workspace != nullptr && workspace_bytes >= need),
+               DDSP_B200_E_WORKSPACE, "%s: workspace of %zu B needed, %zu given", name,
+               need, workspace_bytes);
+  return fir_bwd_launch(audio, ir, grad, d_audio, d_ir, B, N, F, S, ir_batch, frame, start,
+                        out_len, need ? align256<float>(workspace) : nullptr,
+                        (cudaStream_t)stream, name);
+}
+
+int ddsp_b200_frequency_impulse_response_backward(const float* d_ir, float* d_mags,
+                                                  int64_t BF, int nb, int window_size,
+                                                  void* stream) {
+  DDSP_REQUIRE(d_ir && d_mags, DDSP_B200_E_INVALID,
+               "frequency_impulse_response_backward: null pointer");
+  DDSP_REQUIRE(nb >= 2 && BF >= 0, DDSP_B200_E_INVALID,
+               "frequency_impulse_response_backward: need n_frequencies >= 2 (got %d)", nb);
+  if (BF == 0) return 0;
+  const IrGeom g = make_ir_geom(nb, window_size);
+  const size_t smem = ir_backward_smem(g);
+  DDSP_REQUIRE(smem <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
+               "frequency_impulse_response_backward: n_frequencies=%d too large", nb);
+  const int64_t blocks = (BF + kIrFrames - 1) / kIrFrames;
+  DDSP_REQUIRE(blocks < (1ll << 31), DDSP_B200_E_INVALID,
+               "frequency_impulse_response_backward: too many frames");
+  int rc = set_smem(ir_backward_kernel, smem, "frequency_impulse_response_backward");
+  if (rc) return rc;
+  ir_backward_kernel<<<(int)blocks, kIrThreads, smem, (cudaStream_t)stream>>>(d_ir, d_mags,
+                                                                              BF, g);
+  DDSP_CHECK_LAUNCH("frequency_impulse_response_backward");
+  return 0;
+}
+
+size_t ddsp_b200_frequency_filter_backward_workspace(int B, int F, int nb, int N,
+                                                     int mags_batch, int window_size,
+                                                     int padding) {
+  if (B <= 0 || F <= 0 || N <= 0 || nb < 2 || (mags_batch != 1 && mags_batch != B))
+    return 0;
+  const int frame = (N + F - 1) / F;
+  if ((N + frame - 1) / frame != F) return 0;
+  if (freq_filter_fused(B, F, nb, N, frame, mags_batch, window_size, padding)) return 0;
+  const int S = make_ir_geom(nb, window_size).S;
+  // d IR [mags_batch, F, S], then the partial sums of fir_dir_kernel
+  const size_t d_ir = (sizeof(float) * (size_t)mags_batch * F * S + 255) & ~(size_t)255;
+  return 256 + d_ir + fir_dir_part_bytes(B, N, F, S, mags_batch, frame);
+}
+
+int ddsp_b200_frequency_filter_backward(const float* audio, const float* ir,
+                                        const float* grad, float* d_audio, float* d_mags,
+                                        int B, int F, int nb, int N, int mags_batch,
+                                        int window_size, int padding, void* workspace,
+                                        size_t workspace_bytes, void* stream) {
+  const char* name = "frequency_filter_backward";
+  DDSP_REQUIRE(audio && ir && grad, DDSP_B200_E_INVALID, "%s: null pointer", name);
+  DDSP_REQUIRE(B >= 0 && F >= 1 && N >= 1 && nb >= 2, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d F=%d nb=%d N=%d", name, B, F, nb, N);
+  const IrGeom g = make_ir_geom(nb, window_size);
+  const int S = g.S;
+  int frame = 0, start = 0, out_len = 0;
+  int rc = fir_bwd_check(name, B, N, F, S, mags_batch, padding, -1, &frame, &start,
+                         &out_len);
+  if (rc || B == 0) return rc;
+  const bool fused =
+      freq_filter_fused(B, F, nb, N, frame, mags_batch, window_size, padding);
+  DDSP_REQUIRE(!d_mags || fused || ir_backward_smem(g) <= kMaxDynSmem,
+               DDSP_B200_E_UNSUPPORTED, "%s: n_frequencies=%d too large", name, nb);
+  const size_t need =
+      d_mags ? ddsp_b200_frequency_filter_backward_workspace(B, F, nb, N, mags_batch,
+                                                             window_size, padding)
+             : 0;
+  DDSP_REQUIRE(need == 0 || (workspace != nullptr && workspace_bytes >= need),
+               DDSP_B200_E_WORKSPACE, "%s: workspace of %zu B needed, %zu given", name,
+               need, workspace_bytes);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (d_audio) {
+    rc = fir_bwd_launch(audio, ir, grad, d_audio, nullptr, B, N, F, S, mags_batch, frame,
+                        start, out_len, nullptr, st, name);
+    if (rc) return rc;
+  }
+  if (!d_mags) return 0;
+  if (fused) {
+    long long n_tiles;
+    size_t smem;
+    NoiseBwdParams p = noise_bwd_params(grad, audio, 0, 0, d_mags, B, F, nb, N, frame,
+                                        window_size, &n_tiles, &smem);
+    return noise_bwd_launch(p, smem, st, name);
+  }
+  float* d_ir = align256<float>(workspace);
+  float* part = d_ir + (((size_t)mags_batch * F * S + 63) & ~(size_t)63);
+  rc = fir_bwd_launch(audio, ir, grad, nullptr, d_ir, B, N, F, S, mags_batch, frame, start,
+                      out_len,
+                      fir_dir_part_bytes(B, N, F, S, mags_batch, frame) ? part : nullptr, st,
+                      name);
+  if (rc) return rc;
+  return ddsp_b200_frequency_impulse_response_backward(d_ir, d_mags, (int64_t)mags_batch * F,
+                                                       nb, window_size, stream);
 }
 
 size_t ddsp_b200_oscillator_bank_workspace(int B, int N, int K) {

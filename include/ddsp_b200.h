@@ -242,6 +242,46 @@ int ddsp_b200_filtered_noise_backward(const float* grad_audio, const float* nois
                                       int B, int F, int nb, int N, int window_size,
                                       void* stream);
 
+/* Backward of ddsp_b200_fir_time_varying for the upstream gradient grad [B, out_len]
+ * (out_len = N for 'same', N+S-1 for 'valid'): d_audio [B,N] and d_ir
+ * [ir_batch,F,S], each skipped when NULL.  A shared impulse response (ir_batch 1)
+ * gets the sum over the batch.  Same arguments, checks and status codes as the
+ * forward (E_UNSUPPORTED for a negative automatic delay).  No atomics: both
+ * gradients are bit-reproducible.  workspace: ddsp_b200_fir_time_varying_backward_
+ * workspace(B,N,F,S,ir_batch) bytes (needed only when d_ir is set; 0 when every
+ * frame is at most 256 samples and the impulse responses are per item). */
+size_t ddsp_b200_fir_time_varying_backward_workspace(int B, int N, int F, int S,
+                                                     int ir_batch);
+int ddsp_b200_fir_time_varying_backward(const float* audio, const float* ir,
+                                        const float* grad, float* d_audio, float* d_ir,
+                                        int B, int N, int F, int S, int ir_batch,
+                                        int padding, int delay_compensation,
+                                        void* workspace, size_t workspace_bytes,
+                                        void* stream);
+
+/* Backward of ddsp_b200_frequency_impulse_response: d_ir [BF, S] -> d_mags [BF, nb].
+ * Same limits as the forward (nb <= 5120). */
+int ddsp_b200_frequency_impulse_response_backward(const float* d_ir, float* d_mags,
+                                                  int64_t BF, int nb, int window_size,
+                                                  void* stream);
+
+/* Backward of core.frequency_filter (core.py:1628-1655): audio [B,N], the forward's
+ * impulse responses ir [mags_batch,F,S] and grad [B, out_len] -> d_audio [B,N] and
+ * d_mags [mags_batch,F,nb], each skipped when NULL (shared magnitudes, mags_batch 1,
+ * get the sum over the batch).  d_mags takes the fused filtered-noise backward kernel
+ * (the audio as its noise) for 'same' padding and per-item magnitudes when the shape
+ * fits it, and d IR plus the IR adjoint through the workspace otherwise.
+ * workspace: ddsp_b200_frequency_filter_backward_workspace(...) bytes (needed only
+ * when d_mags is set; 0 on the fused route). */
+size_t ddsp_b200_frequency_filter_backward_workspace(int B, int F, int nb, int N,
+                                                     int mags_batch, int window_size,
+                                                     int padding);
+int ddsp_b200_frequency_filter_backward(const float* audio, const float* ir,
+                                        const float* grad, float* d_audio, float* d_mags,
+                                        int B, int F, int nb, int N, int mags_batch,
+                                        int window_size, int padding, void* workspace,
+                                        size_t workspace_bytes, void* stream);
+
 /* core.oscillator_bank (core.py:911-962) on audio-rate envelopes [B,N,K]:
  * Nyquist mask, exact wrapped phase accumulation (three-pass chunked scan in
  * 64-bit fixed point), amp * sin(phase), summed over k when sum_sinusoids != 0
