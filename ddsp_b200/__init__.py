@@ -11,9 +11,10 @@ from ddsp_b200 import effects
 from ddsp_b200 import host
 from ddsp_b200 import processors
 from ddsp_b200 import synths
-from ddsp_b200.effects import FIRFilter, FilteredNoiseReverb, ModDelay, Reverb
+from ddsp_b200.effects import (ExpDecayReverb, FIRFilter, FilteredNoiseReverb,
+                               ModDelay, Reverb)
 from ddsp_b200.host import HostDecoder
-from ddsp_b200.processors import Add, Processor, ProcessorGroup
-from ddsp_b200.synths import FilteredNoise, Harmonic, Sinusoidal
+from ddsp_b200.processors import Add, Crop, Mix, Processor, ProcessorGroup
+from ddsp_b200.synths import FilteredNoise, Harmonic, Sinusoidal, TensorToAudio
 
 __version__ = '0.1.0'

@@ -110,6 +110,13 @@ SIGNATURES = {
         (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _i, _vp]),
     'ddsp_b200_mod_delay_backward':
         (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _i, _vp]),
+    'ddsp_b200_resample_backward': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    'ddsp_b200_mix_forward': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    'ddsp_b200_mix_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
+    'ddsp_b200_exp_decay_ir': (_i, [_vp, _vp, _vp, _u64, _u64, _vp, _i, _i, _vp]),
+    'ddsp_b200_exp_decay_ir_backward':
+        (_i, [_vp, _vp, _vp, _u64, _u64, _vp, _vp, _vp, _i, _i, _vp]),
 }
 
 _lib = None

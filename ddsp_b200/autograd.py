@@ -15,6 +15,10 @@ kernels, exposed as `torch.autograd.Function`s:
     grad); `core.sinusoidal_synthesis` routes to it under grad;
   * `FftConvolveLtiFn` / `ModDelayFn` - the reverb convolution and the modulated
     delay, routed to by `core.fft_convolve` / `core.mod_delay` under grad;
+  * `ResampleFn` / `AddFn` - core.resample (the transpose kernel) and core.add,
+    routed to under grad;
+  * `MixFn` / `ExpDecayIrFn` - processors.Mix's crossfade and the exponential
+    decay impulse response of effects.ExpDecayReverb;
   * `FirTimeVaryingFn` / `FrequencyImpulseResponseFn` / `FrequencyFilterFn` - the
     direct-form time-varying FIR (impulse responses under 2048 taps: FIRFilter,
     short reverbs), the impulse-response synthesis and their composition, routed to
@@ -394,6 +398,100 @@ class ModDelayFn(torch.autograd.Function):
         core._ptr(d_audio), core._ptr(d_gain), core._ptr(d_phase), b, n, max_length,
         scale, offset, int(add_dry), core._stream()))
     return d_audio, d_gain, d_phase, None, None, None, None
+
+
+class ResampleFn(torch.autograd.Function):
+  """core.resample / core.upsample_with_windows on [B, F, C] (core.py:573-714),
+  differentiable in the input: the backward kernel is the forward's transpose
+  (csrc/routing.cuh), every method and add_endpoint value."""
+
+  @staticmethod
+  def forward(ctx, inputs, n_timesteps, method, add_endpoint):
+    ctx.cfg = (tuple(inputs.shape), int(n_timesteps), method, bool(add_endpoint))
+    return core.resample_forward(inputs, n_timesteps, method, add_endpoint)
+
+  @staticmethod
+  def backward(ctx, g):
+    (b, f, c), n, method, add_endpoint = ctx.cfg
+    g = g.contiguous().to(torch.float32)
+    with core._on_device_of(g):
+      d_in = torch.empty((b, f, c), dtype=torch.float32, device=g.device)
+      _lib.check(_lib.load().ddsp_b200_resample_backward(
+          g.data_ptr(), d_in.data_ptr(), b, f, c, n, core._RESAMPLE_METHODS[method],
+          int(add_endpoint), core._stream()))
+    return d_in, None, None, None
+
+
+class AddFn(torch.autograd.Function):
+  """core.add (processors.Add, processors.py:174-176): the gradient goes to each
+  input, summed over the dimensions it was broadcast along."""
+
+  @staticmethod
+  def forward(ctx, a, b):
+    ctx.shapes = (a.shape, b.shape)
+    return core.add_forward(a, b)
+
+  @staticmethod
+  def backward(ctx, g):
+    sa, sb = ctx.shapes
+    want = ctx.needs_input_grad
+    return (g.sum_to_size(sa) if want[0] else None,
+            g.sum_to_size(sb) if want[1] else None)
+
+
+class MixFn(torch.autograd.Function):
+  """core.mix (processors.Mix.get_signal, processors.py:217-233), differentiable in
+  both signals and the mix level: one backward kernel writes the gradients asked
+  for (csrc/routing.cuh).  d mix_level is NaN where the level is exactly 0 or 1,
+  as in the reference."""
+
+  @staticmethod
+  def forward(ctx, signal_one, signal_two, mix_level):
+    ctx.save_for_backward(signal_one, signal_two, mix_level)
+    return core.mix_forward(signal_one, signal_two, mix_level)
+
+  @staticmethod
+  def backward(ctx, g):
+    s1, s2, m = ctx.saved_tensors
+    b, n, c = s1.shape
+    g = g.contiguous().to(torch.float32)
+    want = ctx.needs_input_grad
+    with core._on_device_of(s1, s2, m, g):
+      d1 = torch.empty_like(s1) if want[0] else None
+      d2 = torch.empty_like(s2) if want[1] else None
+      dm = torch.empty_like(m) if want[2] else None
+      _lib.check(_lib.load().ddsp_b200_mix_backward(
+          s1.data_ptr(), s2.data_ptr(), m.data_ptr(), g.data_ptr(), core._ptr(d1),
+          core._ptr(d2), core._ptr(dm), b, n, c, core._stream()))
+    return d1, d2, dm
+
+
+class ExpDecayIrFn(torch.autograd.Function):
+  """core.exp_decay_ir (ExpDecayReverb._get_ir, effects.py:144-151) on [rows] scaled
+  gain and raw decay, differentiable in both.  The backward regenerates the noise
+  (or reads the injected row) instead of saving the impulse response."""
+
+  @staticmethod
+  def forward(ctx, gain, decay, reverb_length, noise, seed, offset):
+    ctx.save_for_backward(gain, decay)
+    ctx.noise = noise
+    ctx.cfg = (int(reverb_length), int(seed), int(offset))
+    return core.exp_decay_ir_forward(gain, decay, reverb_length, noise, seed, offset)
+
+  @staticmethod
+  def backward(ctx, g):
+    gain, decay = ctx.saved_tensors
+    length, seed, offset = ctx.cfg
+    g = g.contiguous().to(torch.float32)
+    want = ctx.needs_input_grad
+    with core._on_device_of(gain, decay, g):
+      d_gain = torch.empty_like(gain) if want[0] else None
+      d_decay = torch.empty_like(decay) if want[1] else None
+      _lib.check(_lib.load().ddsp_b200_exp_decay_ir_backward(
+          gain.data_ptr(), decay.data_ptr(), core._ptr(ctx.noise), seed & (2**64 - 1),
+          offset & (2**64 - 1), g.data_ptr(), core._ptr(d_gain), core._ptr(d_decay),
+          gain.shape[0], length, core._stream()))
+    return d_gain, d_decay, None, None, None, None
 
 
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):

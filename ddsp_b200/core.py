@@ -289,7 +289,17 @@ _RESAMPLE_METHODS = {'window': 0, 'linear': 1, 'nearest': 2, 'cubic': 3}
 
 
 def _resample_3d(inputs, n_timesteps, method, add_endpoint):
+  """[B, F, C] -> [B, N, C]; routes to `autograd.ResampleFn` when grad is enabled
+  and the input requires it."""
   inputs = torch_float32(inputs)
+  if torch.is_grad_enabled() and inputs.requires_grad:
+    from ddsp_b200 import autograd as _ag
+    return _ag.ResampleFn.apply(inputs, int(n_timesteps), method, bool(add_endpoint))
+  return resample_forward(inputs, n_timesteps, method, add_endpoint)
+
+
+def resample_forward(inputs, n_timesteps, method, add_endpoint):
+  """The resample kernel on a [B, F, C] float32 CUDA tensor."""
   b, f, c = inputs.shape
   out = torch.empty((b, int(n_timesteps), c), dtype=torch.float32,
                     device=inputs.device)
@@ -1112,6 +1122,96 @@ def variable_length_delay(phase, audio, max_length: int = 512):
   return mod_delay(audio, None, phase, max_length)
 
 
+# ----------------------------------------------------------------------------
+# Mix (processors.py:179-233) and the exponential-decay impulse response
+# (effects.py:121-199)
+# ----------------------------------------------------------------------------
+def _mix_shapes(signal_one, signal_two, mix_level=None):
+  """Static checks of Mix: two [B, N, C] signals of one shape and a [B, N, 1] mix
+  level.  Returns (B, N, C)."""
+  s1, s2 = _shape(signal_one), _shape(signal_two)
+  if len(s1) != 3 or len(s2) != 3:
+    raise ValueError(
+        f'Mix takes 3-D signals [batch, n_samples, n_channels]; got {s1} and {s2}. '
+        'The mix level is [batch, n_samples, 1], and broadcasting it against a 2-D '
+        'signal [batch, n_samples] gives no crossfade of the two signals.')
+  if s1 != s2:
+    raise ValueError(f'Mix signals must have one shape; got {s1} and {s2}.')
+  if mix_level is not None and _shape(mix_level) != (s1[0], s1[1], 1):
+    raise ValueError(f'mix_level must be [{s1[0]}, {s1[1]}, 1]; got {_shape(mix_level)}.')
+  return s1
+
+
+def mix(signal_one, signal_two, mix_level):
+  """processors.Mix.get_signal (processors.py:217-233): the constant-power crossfade
+  sqrt(|m|) s1 + (1 - sqrt(|m - 1|)) s2 in one kernel (csrc/routing.cuh).  Routes to
+  `autograd.MixFn` when grad is enabled and an input requires it."""
+  _mix_shapes(signal_one, signal_two, mix_level)
+  s1, s2, m = (torch_float32(x) for x in (signal_one, signal_two, mix_level))
+  if torch.is_grad_enabled() and any(t.requires_grad for t in (s1, s2, m)):
+    from ddsp_b200 import autograd as _ag
+    return _ag.MixFn.apply(s1, s2, m)
+  return mix_forward(s1, s2, m)
+
+
+def mix_forward(signal_one, signal_two, mix_level):
+  """The mix kernel on [B, N, C] / [B, N, 1] float32 CUDA tensors."""
+  b, n, c = signal_one.shape
+  out = torch.empty_like(signal_one)
+  with _on_device_of(signal_one, signal_two, mix_level):
+    _lib.check(_lib.load().ddsp_b200_mix_forward(
+        _ptr(signal_one), _ptr(signal_two), _ptr(mix_level), _ptr(out), b, n, c,
+        _stream()))
+  return out
+
+
+def _ir_rows(x, name):
+  """[rows, 1] or [rows] (the reference's [batch, 1] gain and decay) -> rows."""
+  shape = _shape(x)
+  if len(shape) not in (1, 2) or (len(shape) == 2 and shape[1] != 1):
+    raise ValueError(f'{name} must be [batch, 1]; got {shape}.')
+  return shape[0]
+
+
+def exp_decay_ir(gain, decay, reverb_length, noise=None, seed=0, offset=0):
+  """ExpDecayReverb._get_ir (effects.py:144-151) on the SCALED gain:
+  `(gain * exp(-(2 + exp(decay)) * linspace(0, 1, L))) * noise`, [rows, L], one
+  kernel (csrc/routing.cuh).  gain and decay are [rows, 1] (or [1, 1], broadcast);
+  the noise is one [1, L] row for every item, `noise` when given, else the Philox
+  stream's row 0 at (seed, offset) - `uniform_noise(1, L, seed, offset)`.  Routes to
+  `autograd.ExpDecayIrFn` when grad is enabled and gain or decay requires it."""
+  rows_g, rows_d = _ir_rows(gain, 'gain'), _ir_rows(decay, 'decay')
+  if rows_g != rows_d and 1 not in (rows_g, rows_d):
+    raise ValueError(f'gain ({_shape(gain)}) and decay ({_shape(decay)}) do not '
+                     'broadcast.')
+  length = int(reverb_length)
+  if length != reverb_length or length < 1:
+    raise ValueError(f'reverb_length must be a positive integer; got {reverb_length}.')
+  if noise is not None and _shape(noise) not in ((1, length), (length,)):
+    raise ValueError(f'noise must be [1, {length}]; got {_shape(noise)}.')
+  rows = max(rows_g, rows_d)
+  gain = torch_float32(gain).reshape(-1).expand(rows).contiguous()
+  decay = torch_float32(decay).reshape(-1).expand(rows).contiguous()
+  if noise is not None:
+    noise = torch_float32(noise).reshape(length)
+  args = (length, noise, int(seed), int(offset))
+  if torch.is_grad_enabled() and (gain.requires_grad or decay.requires_grad):
+    from ddsp_b200 import autograd as _ag
+    return _ag.ExpDecayIrFn.apply(gain, decay, *args)
+  return exp_decay_ir_forward(gain, decay, *args)
+
+
+def exp_decay_ir_forward(gain, decay, reverb_length, noise, seed, offset):
+  """The impulse-response kernel on [rows] float32 CUDA gain and decay."""
+  rows = gain.shape[0]
+  ir = torch.empty((rows, reverb_length), dtype=torch.float32, device=gain.device)
+  with _on_device_of(gain, decay, noise):
+    _lib.check(_lib.load().ddsp_b200_exp_decay_ir(
+        _ptr(gain), _ptr(decay), _ptr(noise), seed & (2**64 - 1), offset & (2**64 - 1),
+        _ptr(ir), rows, reverb_length, _stream()))
+  return ir
+
+
 def uniform_noise(batch_size, n_samples, seed=0, offset=0, device=None):
   """Stand-in for tf.random.uniform([B, N], -1, 1) (synths.py:192-193):
   Philox4x32-10 keyed by `seed`, counter (sample/4, batch, offset)."""
@@ -1221,9 +1321,19 @@ def noise_controls(magnitudes, initial_bias=-5.0, scale=True):
 
 
 def add(signal_one, signal_two, out=None):
-  """processors.Add.get_signal (processors.py:174-176)."""
+  """processors.Add.get_signal (processors.py:174-176).  Routes to
+  `autograd.AddFn` when grad is enabled, an input requires it and no `out` is
+  given."""
   a = torch_float32(signal_one)
   b = torch_float32(signal_two)
+  if out is None and torch.is_grad_enabled() and (a.requires_grad or b.requires_grad):
+    from ddsp_b200 import autograd as _ag
+    return _ag.AddFn.apply(a, b)
+  return add_forward(a, b, out)
+
+
+def add_forward(a, b, out=None):
+  """The add kernel on float32 CUDA tensors that broadcast against each other."""
   if a.shape != b.shape:
     a, b = torch.broadcast_tensors(a, b)
     a, b = a.contiguous(), b.contiguous()

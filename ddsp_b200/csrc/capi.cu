@@ -23,6 +23,7 @@
 #include "spectral.cuh"
 #include "mod_delay.cuh"
 #include "fir_backward.cuh"
+#include "routing.cuh"
 
 namespace ddsp {
 
@@ -1319,6 +1320,106 @@ int ddsp_b200_add(const float* a, const float* b, float* out, int64_t n,
   if (n == 0) return 0;
   add_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(a, b, out, n);
   DDSP_CHECK_LAUNCH("add");
+  return 0;
+}
+
+// ---- routing: resample backward, Mix, ExpDecayReverb impulse response -----------
+int ddsp_b200_resample_backward(const float* grad_out, float* grad_in, int B, int F, int C,
+                                int N, int method, int add_endpoint, void* stream) {
+  DDSP_REQUIRE(grad_out && grad_in, DDSP_B200_E_INVALID, "resample_backward: null pointer");
+  DDSP_REQUIRE(B >= 0 && F >= 1 && C >= 1 && N >= 1, DDSP_B200_E_INVALID,
+               "resample_backward: bad shape B=%d F=%d C=%d N=%d", B, F, C, N);
+  DDSP_REQUIRE(method >= 0 && method <= 3, DDSP_B200_E_INVALID,
+               "resample_backward: bad method %d", method);
+  if (method == 0) {
+    // upsample_with_windows (core.py:676-693)
+    const int n_frames = add_endpoint ? F + 1 : F;
+    const int n_intervals = n_frames - 1;
+    DDSP_REQUIRE(n_frames < N, DDSP_B200_E_INVALID,
+                 "Upsample with windows cannot be used for downsampling"
+                 "More input frames (%d) than output timesteps (%d)", n_frames, N);
+    DDSP_REQUIRE(n_intervals > 0 && N % n_intervals == 0, DDSP_B200_E_INVALID,
+                 "For upsampling, the target the number of timesteps must be "
+                 "divisible by the number of input frames%s. (timesteps:%d, "
+                 "frames:%d, add_endpoint=%s).", add_endpoint ? "" : " - 1", N,
+                 n_frames, add_endpoint ? "True" : "False");
+  }
+  if (B == 0) return 0;
+  const rt_::ResampleGeom g = rt_::resample_geom(F, N, method, add_endpoint);
+  const int64_t total = (int64_t)B * F * C;
+  if (N >= 8 * F) {   // long frames: a warp per frame
+    rt_::resample_backward_kernel<32>
+        <<<grid_for(total * 32, rt_::kThreads, 16), rt_::kThreads, 0, (cudaStream_t)stream>>>(
+            grad_out, grad_in, B, C, g);
+  } else {
+    rt_::resample_backward_kernel<1>
+        <<<grid_for(total, rt_::kThreads, 16), rt_::kThreads, 0, (cudaStream_t)stream>>>(
+            grad_out, grad_in, B, C, g);
+  }
+  DDSP_CHECK_LAUNCH("resample_backward");
+  return 0;
+}
+
+int ddsp_b200_mix_forward(const float* signal_one, const float* signal_two,
+                          const float* mix_level, float* out, int B, int N, int C,
+                          void* stream) {
+  DDSP_REQUIRE(signal_one && signal_two && mix_level && out, DDSP_B200_E_INVALID,
+               "mix_forward: null pointer");
+  DDSP_REQUIRE(B >= 0 && N >= 1 && C >= 1, DDSP_B200_E_INVALID,
+               "mix_forward: bad shape B=%d N=%d C=%d", B, N, C);
+  if (B == 0) return 0;
+  const int64_t total = (int64_t)B * N * C;
+  rt_::mix_kernel<<<grid_for(total, rt_::kThreads), rt_::kThreads, 0, (cudaStream_t)stream>>>(
+      signal_one, signal_two, mix_level, out, (int64_t)B * N, C);
+  DDSP_CHECK_LAUNCH("mix_forward");
+  return 0;
+}
+
+int ddsp_b200_mix_backward(const float* signal_one, const float* signal_two,
+                           const float* mix_level, const float* grad_out,
+                           float* grad_signal_one, float* grad_signal_two,
+                           float* grad_mix_level, int B, int N, int C, void* stream) {
+  DDSP_REQUIRE(signal_one && signal_two && mix_level && grad_out, DDSP_B200_E_INVALID,
+               "mix_backward: null pointer");
+  DDSP_REQUIRE(B >= 0 && N >= 1 && C >= 1, DDSP_B200_E_INVALID,
+               "mix_backward: bad shape B=%d N=%d C=%d", B, N, C);
+  if (B == 0 || (!grad_signal_one && !grad_signal_two && !grad_mix_level)) return 0;
+  const int64_t rows = (int64_t)B * N;
+  rt_::mix_backward_kernel<<<grid_for(rows, rt_::kThreads), rt_::kThreads, 0,
+                             (cudaStream_t)stream>>>(
+      signal_one, signal_two, mix_level, grad_out, grad_signal_one, grad_signal_two,
+      grad_mix_level, rows, C);
+  DDSP_CHECK_LAUNCH("mix_backward");
+  return 0;
+}
+
+int ddsp_b200_exp_decay_ir(const float* gain, const float* decay, const float* noise,
+                           uint64_t seed, uint64_t offset, float* ir, int rows, int L,
+                           void* stream) {
+  DDSP_REQUIRE(gain && decay && ir, DDSP_B200_E_INVALID, "exp_decay_ir: null pointer");
+  DDSP_REQUIRE(rows >= 0 && L >= 1, DDSP_B200_E_INVALID,
+               "exp_decay_ir: bad shape rows=%d L=%d", rows, L);
+  if (rows == 0) return 0;
+  const int64_t total = (int64_t)rows * ((L + 3) / 4);
+  rt_::exp_decay_ir_kernel<<<grid_for(total, rt_::kThreads), rt_::kThreads, 0,
+                             (cudaStream_t)stream>>>(gain, decay, noise, seed, offset, ir,
+                                                     rows, L);
+  DDSP_CHECK_LAUNCH("exp_decay_ir");
+  return 0;
+}
+
+int ddsp_b200_exp_decay_ir_backward(const float* gain, const float* decay,
+                                    const float* noise, uint64_t seed, uint64_t offset,
+                                    const float* grad_ir, float* grad_gain,
+                                    float* grad_decay, int rows, int L, void* stream) {
+  DDSP_REQUIRE(gain && decay && grad_ir, DDSP_B200_E_INVALID,
+               "exp_decay_ir_backward: null pointer");
+  DDSP_REQUIRE(rows >= 0 && L >= 1, DDSP_B200_E_INVALID,
+               "exp_decay_ir_backward: bad shape rows=%d L=%d", rows, L);
+  if (rows == 0 || (!grad_gain && !grad_decay)) return 0;
+  rt_::exp_decay_ir_backward_kernel<<<rows, rt_::kIrBwdThreads, 0, (cudaStream_t)stream>>>(
+      gain, decay, noise, seed, offset, grad_ir, grad_gain, grad_decay, L);
+  DDSP_CHECK_LAUNCH("exp_decay_ir_backward");
   return 0;
 }
 

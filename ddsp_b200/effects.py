@@ -1,7 +1,7 @@
 """Effects processors that consume the decoder's audio: `Reverb`,
-`FilteredNoiseReverb` and `FIRFilter` with the reference's constructors and
-semantics (`ddsp/effects.py:28-117, 202-278, 283-325`; SURVEY 8f-3; the next
-node after `Add` in `solo_instrument.gin:26-40`).
+`ExpDecayReverb`, `FilteredNoiseReverb`, `FIRFilter` and `ModDelay` with the
+reference's constructors and semantics (`ddsp/effects.py:28-394`; SURVEY 8f-3; the
+next node after `Add` in `solo_instrument.gin:26-40`).
 
 `Reverb` is a long linear time-invariant convolution (48000-tap impulse
 response): `core.fft_convolve` routes one impulse response of 2048 taps and more
@@ -9,6 +9,8 @@ per item to the hand-written partitioned overlap-save convolution
 (csrc/longconv.cuh); `FilteredNoiseReverb` draws that impulse response from a
 `FilteredNoise` synthesizer; `FIRFilter` is the time-varying filter of
 `FilteredNoise` applied to given audio and runs on the IR + FIR kernels."""
+import itertools
+
 import torch
 
 from ddsp_b200 import core
@@ -63,6 +65,63 @@ class Reverb(processors.Processor):
     ir = self._mask_dry_ir(ir)
     wet = core.fft_convolve(audio, ir, padding='same', delay_compensation=0)
     return (wet + audio) if self._add_dry else wet
+
+
+class ExpDecayReverb(Reverb):
+  """Impulse response = an exponential decay of white noise (effects.py:121-199):
+  `(scale_fn(gain) * exp(-(2 + exp(decay)) * linspace(0, 1, L))) * noise`, one
+  [1, L] noise row shared by the batch.  The noise is the library's Philox stream
+  keyed by `seed` with a fresh offset per call (the reference draws fresh
+  `tf.random.uniform` noise per call); set `injected_noise` to a [1, L] tensor to
+  use that row instead.  The impulse response is one kernel with a CUDA backward to
+  gain and decay; `get_signal` is Reverb's."""
+
+  def __init__(self, trainable=False, reverb_length=48000, scale_fn=core.exp_sigmoid,
+               add_dry=True, name='exp_decay_reverb', seed=0):
+    super().__init__(name=name, add_dry=add_dry, trainable=trainable)
+    self._reverb_length = reverb_length
+    self._scale_fn = scale_fn
+    self.seed = seed
+    self._calls = itertools.count()
+    self._gain = None
+    self._decay = None
+    # Test hook: a [1, reverb_length] tensor used instead of the Philox stream.
+    self.injected_noise = None
+
+  def next_offset(self):
+    """Per-call Philox counter offset, so successive calls draw fresh noise."""
+    return next(self._calls)
+
+  def build(self, device=None):
+    """effects.py:153-166: the learned gain 2.0 and decay 4.0, shape [1]."""
+    if self.trainable and self._gain is None:
+      self._gain = torch.full((1,), 2.0, dtype=torch.float32,
+                              device=device).requires_grad_(True)
+      self._decay = torch.full((1,), 4.0, dtype=torch.float32,
+                               device=device).requires_grad_(True)
+
+  def _get_ir(self, gain, decay):
+    """effects.py:144-151."""
+    gain = core.torch_float32(gain)
+    if self._scale_fn is not None:
+      gain = self._scale_fn(gain)
+    return core.exp_decay_ir(gain, core.torch_float32(decay), self._reverb_length,
+                             noise=self.injected_noise, seed=self.seed,
+                             offset=self.next_offset())
+
+  def get_controls(self, audio, gain=None, decay=None):
+    """effects.py:168-198."""
+    if not self.trainable and (gain is None or decay is None):  # before device work
+      raise ValueError('Must provide "gain" and "decay" tensors if '
+                       'ExpDecayReverb trainable=False.')
+    audio = core.torch_float32(audio)
+    if self.trainable:
+      self.build(audio.device)
+      gain, decay = self._gain[None, :], self._decay[None, :]
+    ir = self._get_ir(gain, decay)
+    if self.trainable:
+      ir = self._match_dimensions(audio, ir)
+    return {'audio': audio, 'ir': ir}
 
 
 class FilteredNoiseReverb(Reverb):

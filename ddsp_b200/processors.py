@@ -1,9 +1,11 @@
-"""Processor / ProcessorGroup / Add with the reference's protocol
-(`ddsp/processors.py:37-176`) - the drop-in boundary of this library.
+"""Processor / ProcessorGroup / Add / Mix / Crop with the reference's protocol
+(`ddsp/processors.py:37-263`) - the drop-in boundary of this library.
 
 Tensors are torch CUDA float32; the arithmetic runs in libddsp_b200.so.
 """
 from typing import Dict, Text, Any
+
+import torch
 
 from ddsp_b200 import core
 from ddsp_b200 import dags
@@ -166,3 +168,59 @@ class Add(Processor):
 
   def get_signal(self, signal_one, signal_two):
     return core.add(signal_one, signal_two)
+
+
+class Mix(Processor):
+  """Constant-power crossfade between two signals (processors.py:179-233).
+
+  The signals are [batch, n_samples, n_channels] and the mix level
+  [batch, n_samples, 1], the shapes the reference's own test uses: broadcasting the
+  mix level against 2-D signals gives no crossfade, so those are refused."""
+
+  def __init__(self, name: Text = 'mix'):
+    super().__init__(name=name)
+
+  def get_controls(self, signal_one, signal_two, nn_out_mix_level) -> TensorDict:
+    """processors.py:192-215: sigmoid of the mix logits at frame rate, resampled
+    ('linear') to the signals' length - differentiable under grad."""
+    n_time_one = int(core._shape(signal_one)[1])   # pylint: disable=protected-access
+    n_time_two = int(core._shape(signal_two)[1])   # pylint: disable=protected-access
+    if n_time_one != n_time_two:
+      raise ValueError('The two signals must have the same length instead of'
+                       '{} and {}'.format(n_time_one, n_time_two))
+    core._mix_shapes(signal_one, signal_two)       # pylint: disable=protected-access
+    mix_level = torch.sigmoid(core.torch_float32(nn_out_mix_level))
+    mix_level = core.resample(mix_level, n_time_one)
+    return {'signal_one': signal_one, 'signal_two': signal_two,
+            'mix_level': mix_level}
+
+  def get_signal(self, signal_one, signal_two, mix_level):
+    """processors.py:217-233."""
+    return core.mix(signal_one, signal_two, mix_level)
+
+
+class Crop(Processor):
+  """Remove audio generated from padding frames (processors.py:236-263): torch
+  slicing of the time axis of 2-D or 3-D audio, a view."""
+
+  def __init__(self, frame_size: int, crop_location: Text = 'back',
+               name: Text = 'crop'):
+    super().__init__(name=name)
+    self.frame_size = frame_size
+    self.crop_location = crop_location
+
+  def get_controls(self, audio) -> TensorDict:
+    return {'audio': audio}
+
+  def get_signal(self, audio):
+    half_pad_amount = int(self.frame_size // 2)  # Symmetric even.
+    pad_amount = 2 * half_pad_amount
+    if self.crop_location == 'front':
+      return audio[:, pad_amount:]
+    elif self.crop_location == 'center':
+      return audio[:, half_pad_amount:-half_pad_amount]
+    elif self.crop_location == 'back':
+      return audio[:, :-pad_amount]
+    else:
+      raise ValueError(f'Crop_location: ({self.crop_location}), must be '
+                       '"front", "center", or "back".')

@@ -1,9 +1,29 @@
-"""Harmonic and FilteredNoise synthesizers with the reference's constructor
-arguments, method names and dict keys (`ddsp/synths.py:55-196`)."""
+"""TensorToAudio, Harmonic, FilteredNoise and Sinusoidal synthesizers with the
+reference's constructor arguments, method names and dict keys
+(`ddsp/synths.py:23-196, 260-323`)."""
 import itertools
 
 from ddsp_b200 import core
 from ddsp_b200 import processors
+
+
+class TensorToAudio(processors.Processor):
+  """Identity "synth": the input samples without their channel axis
+  (synths.py:23-52); a view."""
+
+  def __init__(self, name='tensor_to_audio'):
+    super().__init__(name=name)
+
+  def get_controls(self, samples):
+    return {'samples': samples}
+
+  def get_signal(self, samples):
+    """`tf.squeeze(samples, 2)`, which fails unless samples is [batch, time, 1]."""
+    shape = core._shape(samples)   # pylint: disable=protected-access
+    if len(shape) != 3 or shape[2] != 1:
+      raise ValueError(f'TensorToAudio takes samples of shape [batch, time, 1]; got '
+                       f'{shape}.')
+    return samples[:, :, 0]
 
 
 class Harmonic(processors.Processor):

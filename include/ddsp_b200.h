@@ -428,6 +428,46 @@ int ddsp_b200_mod_delay_backward(const float* audio, const float* phase, const f
                                  float* grad_phase, int B, int N, int max_length, float scale,
                                  float offset, int add_dry, void* stream);
 
+/* Transpose of ddsp_b200_resample: grad_out [B,N,C] -> grad_in [B,F,C], same
+ * arguments and checks.  Every tap of the forward (its float32 index and weight,
+ * the clamped taps included) is added in double; bit-reproducible. */
+int ddsp_b200_resample_backward(const float* grad_out, float* grad_in, int B, int F, int C,
+                                int N, int method, int add_endpoint, void* stream);
+
+/* processors.Mix.get_signal (processors.py:217-233):
+ *   out = sqrt(|m|) * s1 + (1 - sqrt(|m - 1|)) * s2
+ * in float32, in that operation order.  signal_one, signal_two, out: [B,N,C];
+ * mix_level m: [B,N,1], broadcast over C.
+ * backward: writes any of grad_signal_one, grad_signal_two [B,N,C] and
+ * grad_mix_level [B,N,1] (summed over C in channel order); NULL outputs are not
+ * computed.  grad_mix_level is NaN where m is exactly 0 or 1, as the reference's
+ * autodiff gives it (0 * inf). */
+int ddsp_b200_mix_forward(const float* signal_one, const float* signal_two,
+                          const float* mix_level, float* out, int B, int N, int C,
+                          void* stream);
+int ddsp_b200_mix_backward(const float* signal_one, const float* signal_two,
+                           const float* mix_level, const float* grad_out,
+                           float* grad_signal_one, float* grad_signal_two,
+                           float* grad_mix_level, int B, int N, int C, void* stream);
+
+/* effects.ExpDecayReverb._get_ir (effects.py:144-151), on the scaled gain:
+ *   ir[r,t] = (gain[r] * exp(-(2 + exp(decay[r])) * time[t])) * noise[t]
+ * in float32, time = tf.linspace(0, 1, L).  gain, decay: [rows]; ir: [rows, L];
+ * noise: one [L] row shared by every row, or NULL for the Philox stream's batch row
+ * 0 at (seed, offset) (= ddsp_b200_uniform_noise(1, L, seed, offset)).
+ * backward: for grad_ir [rows, L], writes any of
+ *   grad_gain[r]  = sum_t grad_ir e n,
+ *   grad_decay[r] = -exp(decay[r]) gain[r] sum_t grad_ir time e n
+ * (NULL outputs are not computed); the noise is regenerated, the sums are in double
+ * in a fixed order. */
+int ddsp_b200_exp_decay_ir(const float* gain, const float* decay, const float* noise,
+                           uint64_t seed, uint64_t offset, float* ir, int rows, int L,
+                           void* stream);
+int ddsp_b200_exp_decay_ir_backward(const float* gain, const float* decay,
+                                    const float* noise, uint64_t seed, uint64_t offset,
+                                    const float* grad_ir, float* grad_gain,
+                                    float* grad_decay, int rows, int L, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
