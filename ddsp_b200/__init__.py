@@ -15,6 +15,7 @@ from ddsp_b200.effects import (ExpDecayReverb, FIRFilter, FilteredNoiseReverb,
                                ModDelay, Reverb)
 from ddsp_b200.host import HostDecoder
 from ddsp_b200.processors import Add, Crop, Mix, Processor, ProcessorGroup
-from ddsp_b200.synths import FilteredNoise, Harmonic, Sinusoidal, TensorToAudio
+from ddsp_b200.synths import (FilteredNoise, Harmonic, Sinusoidal, TensorToAudio,
+                              Wavetable)
 
 __version__ = '0.1.0'

@@ -117,6 +117,13 @@ SIGNATURES = {
     'ddsp_b200_exp_decay_ir': (_i, [_vp, _vp, _vp, _u64, _u64, _vp, _i, _i, _vp]),
     'ddsp_b200_exp_decay_ir_backward':
         (_i, [_vp, _vp, _vp, _u64, _u64, _vp, _vp, _vp, _i, _i, _vp]),
+    'ddsp_b200_wavetable_workspace': (_sz, [_i, _i]),
+    'ddsp_b200_wavetable_forward':
+        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
+    'ddsp_b200_wavetable_backward_workspace': (_sz, [_i, _i, _i, _i, _i]),
+    'ddsp_b200_wavetable_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _sz,
+              _vp]),
 }
 
 _lib = None

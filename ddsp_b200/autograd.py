@@ -13,6 +13,9 @@ kernels, exposed as `torch.autograd.Function`s:
     oscillator bank (`Sinusoidal.get_signal`, the synthesizer of
     `models/inverse_synthesis.py:84-105`; d frequencies only when they require
     grad); `core.sinusoidal_synthesis` routes to it under grad;
+  * `WavetableSynthesisFn` - d f0, d amplitudes and d wavetables of the wavetable
+    synthesizer (`Wavetable.get_signal`); `core.wavetable_synthesis` routes to it
+    under grad;
   * `FftConvolveLtiFn` / `ModDelayFn` - the reverb convolution and the modulated
     delay, routed to by `core.fft_convolve` / `core.mod_delay` under grad;
   * `ResampleFn` / `AddFn` - core.resample (the transpose kernel) and core.add,
@@ -368,6 +371,42 @@ class SinusoidalSynthesisFn(torch.autograd.Function):
           d_amp.data_ptr(), b, f, k, n_samples, sample_rate, core.AMP_METHODS[method],
           core._ptr(ws), nbytes, core._stream()))
     return d_freq, d_amp if ctx.needs_input_grad[1] else None, None, None, None
+
+
+class WavetableSynthesisFn(torch.autograd.Function):
+  """core.wavetable_synthesis on the kernel's operands (f0 and amplitudes [B, F],
+  tables [B, Fw, W]), differentiable in all three: one backward call of
+  `ddsp_b200_wavetable_backward` (csrc/wavetable.cuh) computes the gradients that
+  are asked for.  d f0 is 0 where the lookup position is an integer, TensorFlow's
+  subgradient of linear_lookup."""
+
+  @staticmethod
+  def forward(ctx, f0, amplitudes, wavetables, n_samples, sample_rate, method):
+    ctx.save_for_backward(f0, amplitudes, wavetables)
+    ctx.cfg = (n_samples, sample_rate, method)
+    return core.wavetable_forward(f0, amplitudes, wavetables, n_samples, sample_rate,
+                                  method)
+
+  @staticmethod
+  def backward(ctx, grad_audio):
+    f0, amplitudes, wavetables = ctx.saved_tensors
+    n_samples, sample_rate, method = ctx.cfg
+    b, f = amplitudes.shape
+    _, fw, w = wavetables.shape
+    g = grad_audio.contiguous().to(torch.float32)
+    want = ctx.needs_input_grad
+    lib = _lib.load()
+    with core._on_device_of(f0, amplitudes, wavetables, g):
+      d_f0 = torch.empty_like(f0) if want[0] else None
+      d_amp = torch.empty_like(amplitudes) if want[1] else None
+      d_tab = torch.empty_like(wavetables) if want[2] else None
+      nbytes = lib.ddsp_b200_wavetable_backward_workspace(b, f, n_samples, fw, w)
+      ws = core._workspace(nbytes, amplitudes.device)
+      _lib.check(lib.ddsp_b200_wavetable_backward(
+          f0.data_ptr(), amplitudes.data_ptr(), wavetables.data_ptr(), g.data_ptr(),
+          core._ptr(d_f0), core._ptr(d_amp), core._ptr(d_tab), b, f, n_samples, fw, w,
+          sample_rate, core.AMP_METHODS[method], core._ptr(ws), nbytes, core._stream()))
+    return d_f0, d_amp, d_tab, None, None, None
 
 
 class ModDelayFn(torch.autograd.Function):

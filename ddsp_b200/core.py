@@ -312,7 +312,12 @@ def resample_forward(inputs, n_timesteps, method, add_endpoint):
 
 def upsample_with_windows(inputs, n_timesteps: int, add_endpoint: bool = True):
   """core.upsample_with_windows (core.py:645-714)."""
-  shape = _shape(inputs)
+  _check_window_upsample(_shape(inputs), n_timesteps, add_endpoint)
+  return _resample_3d(inputs, n_timesteps, 'window', add_endpoint)
+
+
+def _check_window_upsample(shape, n_timesteps, add_endpoint):
+  """The ValueErrors of core.upsample_with_windows (core.py:670-693)."""
   if len(shape) != 3:
     raise ValueError('Upsample_with_windows() only supports 3 dimensions, '
                      'not {}.'.format(list(shape)))
@@ -328,7 +333,6 @@ def upsample_with_windows(inputs, n_timesteps: int, add_endpoint: bool = True):
         'For upsampling, the target the number of timesteps must be divisible '
         'by the number of input frames{}. (timesteps:{}, frames:{}, '
         'add_endpoint={}).'.format(minus_one, n_timesteps, n_frames, add_endpoint))
-  return _resample_3d(inputs, n_timesteps, 'window', add_endpoint)
 
 
 def resample(inputs, n_timesteps: int, method: Text = 'linear',
@@ -1120,6 +1124,85 @@ def variable_length_delay(phase, audio, max_length: int = 512):
   included (phase in ((L-1)/L, 1] blends the oldest sample with the current one;
   phase 1 is no delay)."""
   return mod_delay(audio, None, phase, max_length)
+
+
+# ----------------------------------------------------------------------------
+# Wavetable synthesis (core.py:1217-1282)
+# ----------------------------------------------------------------------------
+def harmonic_distribution_to_wavetable(harmonic_distribution, n_wavetable=2048):
+  """core.harmonic_distribution_to_wavetable (core.py:1217-1235): one period of
+  the harmonic series [batch, time, n_harmonics] as [batch, time, n_wavetable]
+  samples, irfft of the distribution padded with DC in front, times W / 2.  A
+  differentiable torch op on the input's device and floating dtype."""
+  hd = (harmonic_distribution if torch.is_tensor(harmonic_distribution)
+        else torch.as_tensor(np.asarray(harmonic_distribution, np.float32)))
+  n_pad = int(n_wavetable / 2 - hd.shape[-1])
+  fft_in = torch.nn.functional.pad(hd, (1, n_pad))
+  return torch.fft.irfft(fft_in) * (n_wavetable / 2)
+
+
+def _frame_rows(x, name):
+  """(B, F) of a [B, F, 1] or [B, F] control (static shape only)."""
+  shape = _shape(x)
+  if len(shape) == 3 and shape[2] == 1:
+    shape = shape[:2]
+  if len(shape) != 2:
+    raise ValueError(f'{name} must be [batch, n_frames, 1]; got {_shape(x)}.')
+  return shape
+
+
+def wavetable_synthesis(frequencies, amplitudes, wavetables, n_samples: int = 64000,
+                        sample_rate: int = 16000):
+  """core.wavetable_synthesis (core.py:1238-1282) on one fused kernel
+  (csrc/wavetable.cuh): the phase is exact and the tables are read at frame rate.
+
+  frequencies, amplitudes: [batch, n_frames, 1]; wavetables: [batch, n_wavetable]
+  or [batch, 1, n_wavetable] (static) or [batch, n_frames_w, n_wavetable], which
+  is interpolated in time with core.resample's 'linear' taps.  When f0 and the
+  amplitudes have one frame count that divides n_samples, the kernel reads them
+  at frame rate; otherwise both are first resampled to n_samples (f0 'linear',
+  amplitudes 'window') and the same kernel runs at hop 1.  Routes to
+  `autograd.WavetableSynthesisFn` when grad is enabled and an input requires it."""
+  n = int(n_samples)
+  bf, ff = _frame_rows(frequencies, 'frequencies')
+  ba, fa = _frame_rows(amplitudes, 'amplitudes')
+  sw = _shape(wavetables)
+  if len(sw) == 2:
+    sw = (sw[0], 1, sw[1])
+  if len(sw) != 3 or not bf == ba == sw[0]:
+    raise ValueError(f'frequencies {_shape(frequencies)}, amplitudes '
+                     f'{_shape(amplitudes)} and wavetables {_shape(wavetables)} must '
+                     'share the batch size; wavetables are [batch, n_wavetable] or '
+                     '[batch, n_frames, n_wavetable].')
+  _check_window_upsample((ba, fa, 1), n, True)
+  f0 = torch_float32(frequencies).reshape(bf, ff)
+  amps = torch_float32(amplitudes).reshape(ba, fa)
+  tab = torch_float32(wavetables).reshape(sw)
+  if ff == fa and n % ff == 0:
+    method = 'window'
+  else:
+    f0 = resample(f0[:, :, None], n)[:, :, 0].contiguous()
+    amps = resample(amps[:, :, None], n, method='window')[:, :, 0].contiguous()
+    method = 'linear'
+  if torch.is_grad_enabled() and any(t.requires_grad for t in (f0, amps, tab)):
+    from ddsp_b200 import autograd as _ag
+    return _ag.WavetableSynthesisFn.apply(f0, amps, tab, n, float(sample_rate), method)
+  return wavetable_forward(f0, amps, tab, n, float(sample_rate), method)
+
+
+def wavetable_forward(f0, amps, tab, n_samples, sample_rate, method):
+  """The wavetable kernel: f0, amps [B, F] and tables [B, Fw, W], float32 CUDA."""
+  b, f = amps.shape
+  _, fw, w = tab.shape
+  out = torch.empty((b, n_samples), dtype=torch.float32, device=amps.device)
+  lib = _lib.load()
+  with _on_device_of(f0, amps, tab):
+    nbytes = lib.ddsp_b200_wavetable_workspace(b, f)
+    ws = _workspace(nbytes, amps.device)
+    _lib.check(lib.ddsp_b200_wavetable_forward(
+        _ptr(f0), _ptr(amps), _ptr(tab), _ptr(out), b, f, n_samples, fw, w,
+        sample_rate, AMP_METHODS[method], _ptr(ws), nbytes, _stream()))
+  return out
 
 
 # ----------------------------------------------------------------------------

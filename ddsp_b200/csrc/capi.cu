@@ -24,6 +24,7 @@
 #include "mod_delay.cuh"
 #include "fir_backward.cuh"
 #include "routing.cuh"
+#include "wavetable.cuh"
 
 namespace ddsp {
 
@@ -1521,6 +1522,161 @@ int ddsp_b200_mod_delay_backward(const float* audio, const float* phase, const f
       audio, phase, gain, grad_out, grad_audio, grad_gain, grad_phase, N, max_length, scale,
       offset, add_dry);
   DDSP_CHECK_LAUNCH("mod_delay_backward");
+  return 0;
+}
+
+size_t ddsp_b200_wavetable_workspace(int B, int F) {
+  if (B <= 0 || F <= 0) return 0;
+  const size_t n_tiles = ((size_t)F + wt_::kFT - 1) / wt_::kFT;
+  return sizeof(unsigned long long) * ((size_t)B * n_tiles + 3 * (size_t)B * F) + 4 * 256;
+}
+
+size_t ddsp_b200_wavetable_backward_workspace(int B, int F, int N, int Fw, int W) {
+  if (B <= 0 || F <= 0 || N <= 0 || Fw <= 0 || W <= 0) return 0;
+  const int n_seg = wt_::table_segments(N, Fw);
+  size_t bytes = ddsp_b200_wavetable_workspace(B, F) + sizeof(float) * 6 * (size_t)B * F + 512;
+  if (n_seg > 1) bytes += sizeof(float) * (size_t)B * Fw * n_seg * W + 256;
+  return bytes;
+}
+
+// The checks the forward and the backward share; `name` prefixes the messages.  The
+// caller returns 0 for B == 0 afterwards.
+static int wt_check(const char* name, int B, int F, int N, int Fw, int W, float sample_rate,
+                    int amp_method, const void* workspace, size_t workspace_bytes,
+                    size_t need) {
+  DDSP_REQUIRE(B >= 0 && F >= 1 && N >= 1 && Fw >= 1 && W >= 1, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d F=%d N=%d Fw=%d W=%d", name, B, F, N, Fw, W);
+  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW || amp_method == DDSP_B200_AMP_LINEAR,
+               DDSP_B200_E_INVALID, "%s: bad amp_method %d", name, amp_method);
+  DDSP_REQUIRE(N % F == 0, DDSP_B200_E_INVALID,
+               "%s: n_samples (%d) must be divisible by the number of frames (%d)", name,
+               N, F);
+  DDSP_REQUIRE(amp_method != DDSP_B200_AMP_WINDOW || F < N, DDSP_B200_E_INVALID,
+               "%s: window upsampling cannot downsample (frames %d >= timesteps %d)",
+               name, F, N);
+  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
+               "%s: sample_rate must be positive", name);
+  DDSP_REQUIRE(W <= wt_::kMaxW, DDSP_B200_E_UNSUPPORTED,
+               "%s: W=%d exceeds the %d wavetable columns supported", name, W, wt_::kMaxW);
+  DDSP_REQUIRE((int64_t)Fw * wt_::table_segments(N, Fw) * wt_::table_col_tiles(W) < (1ll << 31),
+               DDSP_B200_E_UNSUPPORTED, "%s: Fw=%d W=%d exceeds the grid limit", name, Fw,
+               W);
+  if (B == 0) return 0;
+  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
+               "%s: B=%d exceeds the 65535 grid limit", name, B);
+  DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
+               "%s: workspace of %zu B needed, %zu given", name, need, workspace_bytes);
+  return 0;
+}
+
+// Passes 1-3 of wavetable.cuh: the fixed-point phase P, A, D of every frame.
+struct WtPhase {
+  unsigned long long *sums, *P, *A, *D;
+  void* end;
+};
+static WtPhase wt_phase_layout(void* workspace, int B, int F) {
+  WtPhase w;
+  const int n_tiles = (F + wt_::kFT - 1) / wt_::kFT;
+  w.sums = align256<unsigned long long>(workspace);
+  w.P = align256<unsigned long long>(w.sums + (size_t)B * n_tiles);
+  w.A = align256<unsigned long long>(w.P + (size_t)B * F);
+  w.D = align256<unsigned long long>(w.A + (size_t)B * F);
+  w.end = w.D + (size_t)B * F;
+  return w;
+}
+static int wt_frame_phases(const WtPhase& w, const float* f0, int B, int F, int hop,
+                           float sample_rate, cudaStream_t st, const char* name) {
+  const int n_tiles = (F + wt_::kFT - 1) / wt_::kFT;
+  const double sr = (double)sample_rate;
+  wt_::wt_tile_sums<<<dim3(n_tiles, B), wt_::kFT, 0, st>>>(f0, w.sums, F, hop, n_tiles, sr);
+  DDSP_CHECK_LAUNCH(name);
+  oscbank_scan_chunks<<<(B + kObThreads - 1) / kObThreads, kObThreads, 0, st>>>(
+      w.sums, 1, n_tiles, (int64_t)B);
+  DDSP_CHECK_LAUNCH(name);
+  wt_::wt_frame_phase<<<dim3(n_tiles, B), wt_::kFT, 0, st>>>(f0, w.sums, w.P, w.A, w.D, F,
+                                                             hop, n_tiles, sr);
+  DDSP_CHECK_LAUNCH(name);
+  return 0;
+}
+
+int ddsp_b200_wavetable_forward(const float* f0_hz, const float* amplitudes,
+                                const float* wavetables, float* audio, int B, int F,
+                                int N, int Fw, int W, float sample_rate, int amp_method,
+                                void* workspace, size_t workspace_bytes, void* stream) {
+  DDSP_REQUIRE(f0_hz && amplitudes && wavetables && audio, DDSP_B200_E_INVALID,
+               "wavetable_forward: null pointer");
+  int rc = wt_check("wavetable_forward", B, F, N, Fw, W, sample_rate, amp_method, workspace,
+                    workspace_bytes, ddsp_b200_wavetable_workspace(B, F));
+  if (rc || B == 0) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int hop = N / F;
+  const WtPhase w = wt_phase_layout(workspace, B, F);
+  rc = wt_frame_phases(w, f0_hz, B, F, hop, sample_rate, st, "wavetable_forward(phase)");
+  if (rc) return rc;
+  auto kern = amp_method == DDSP_B200_AMP_WINDOW ? wt_::wt_forward<true>
+                                                 : wt_::wt_forward<false>;
+  kern<<<dim3((unsigned)((N + wt_::kThreads - 1) / wt_::kThreads), B), wt_::kThreads, 0, st>>>(
+      amplitudes, wavetables, w.P, w.A, w.D, audio, F, N, hop, Fw, W);
+  DDSP_CHECK_LAUNCH("wavetable_forward");
+  return 0;
+}
+
+int ddsp_b200_wavetable_backward(const float* f0_hz, const float* amplitudes,
+                                 const float* wavetables, const float* grad_audio,
+                                 float* d_f0, float* d_amplitudes, float* d_wavetables,
+                                 int B, int F, int N, int Fw, int W, float sample_rate,
+                                 int amp_method, void* workspace, size_t workspace_bytes,
+                                 void* stream) {
+  DDSP_REQUIRE(f0_hz && amplitudes && wavetables && grad_audio, DDSP_B200_E_INVALID,
+               "wavetable_backward: null pointer");
+  int rc = wt_check("wavetable_backward", B, F, N, Fw, W, sample_rate, amp_method, workspace,
+                    workspace_bytes, ddsp_b200_wavetable_backward_workspace(B, F, N, Fw, W));
+  if (rc || B == 0 || (!d_f0 && !d_amplitudes && !d_wavetables)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int hop = N / F;
+  const bool window = amp_method == DDSP_B200_AMP_WINDOW;
+  const WtPhase w = wt_phase_layout(workspace, B, F);
+  float* part = align256<float>(w.end);                    // [5][B F]
+  const int64_t BF = (int64_t)B * F;
+  float* d_amp_scratch = align256<float>(part + 5 * (size_t)BF);
+  float* tab_part = align256<float>(d_amp_scratch + (size_t)BF);
+  rc = wt_frame_phases(w, f0_hz, B, F, hop, sample_rate, st, "wavetable_backward(phase)");
+  if (rc) return rc;
+
+  if (d_f0 || d_amplitudes) {
+    const bool phase = d_f0 != nullptr;
+    auto kern = window ? (phase ? wt_::wt_bwd_frames<true, true>
+                                : wt_::wt_bwd_frames<true, false>)
+                       : (phase ? wt_::wt_bwd_frames<false, true>
+                                : wt_::wt_bwd_frames<false, false>);
+    kern<<<(unsigned)((BF + 31) / 32), kSbThreads, 0, st>>>(
+        amplitudes, wavetables, grad_audio, w.P, w.A, w.D, part, F, N, hop, Fw, W, BF);
+    DDSP_CHECK_LAUNCH("wavetable_backward(frames)");
+    // K = 1; sinus_bwd_finalize always writes d amplitudes
+    sinus_bwd_finalize<<<dim3(1, B), 32 * kSfinWarps, 0, st>>>(
+        part, d_amplitudes ? d_amplitudes : d_amp_scratch, d_f0, F, 1, hop, BF,
+        1.0 / (double)sample_rate);
+    DDSP_CHECK_LAUNCH("wavetable_backward(finalize)");
+  }
+
+  if (d_wavetables) {
+    const int n_seg = wt_::table_segments(N, Fw);
+    const size_t smem = wt_::table_smem_bytes(W);
+    auto kern = window ? wt_::wt_bwd_table<true> : wt_::wt_bwd_table<false>;
+    rc = set_smem(kern, smem, "wavetable_backward");
+    if (rc) return rc;
+    const unsigned gx = (unsigned)((int64_t)Fw * n_seg * wt_::table_col_tiles(W));
+    kern<<<dim3(gx, B), wt_::kTabWarps * 32, smem, st>>>(
+        amplitudes, grad_audio, w.P, w.A, w.D, n_seg > 1 ? tab_part : d_wavetables, F, N,
+        hop, Fw, W, n_seg);
+    DDSP_CHECK_LAUNCH("wavetable_backward(wavetables)");
+    if (n_seg > 1) {
+      const int64_t RW = (int64_t)B * Fw * W;
+      wt_::wt_table_reduce<<<grid_for(RW, 256), 256, 0, st>>>(tab_part, d_wavetables, RW, W,
+                                                            n_seg);
+      DDSP_CHECK_LAUNCH("wavetable_backward(reduce)");
+    }
+  }
   return 0;
 }
 

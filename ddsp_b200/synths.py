@@ -1,6 +1,6 @@
-"""TensorToAudio, Harmonic, FilteredNoise and Sinusoidal synthesizers with the
-reference's constructor arguments, method names and dict keys
-(`ddsp/synths.py:23-196, 260-323`)."""
+"""TensorToAudio, Harmonic, FilteredNoise, Wavetable and Sinusoidal synthesizers
+with the reference's constructor arguments, method names and dict keys
+(`ddsp/synths.py:23-323`)."""
 import itertools
 
 from ddsp_b200 import core
@@ -185,3 +185,42 @@ class Sinusoidal(processors.Processor):
     return core.oscillator_bank(frequency_envelopes=frequency_envelopes,
                                 amplitude_envelopes=amplitude_envelopes,
                                 sample_rate=self.sample_rate)
+
+
+class Wavetable(processors.Processor):
+  """Synthesize audio from a series of wavetables (synths.py:199-257).
+
+  get_signal is one fused kernel (`core.wavetable_synthesis`) that reads the
+  tables at frame rate; the reference's [batch, n_samples, n_wavetable] tables
+  are never built."""
+
+  def __init__(self,
+               n_samples=64000,
+               sample_rate=16000,
+               scale_fn=core.exp_sigmoid,
+               name='wavetable'):
+    super().__init__(name=name)
+    self.n_samples = n_samples
+    self.sample_rate = sample_rate
+    self.scale_fn = scale_fn
+
+  def get_controls(self, amplitudes, wavetables, f0_hz):
+    """synths.py:213-238: scale_fn on the amplitudes and the wavetables."""
+    amplitudes = core.torch_float32(amplitudes)
+    wavetables = core.torch_float32(wavetables)
+    if self.scale_fn is not None:
+      amplitudes = self.scale_fn(amplitudes)
+      wavetables = self.scale_fn(wavetables)
+    return {'amplitudes': amplitudes, 'wavetables': wavetables, 'f0_hz': f0_hz}
+
+  def get_signal(self, amplitudes, wavetables, f0_hz):
+    """synths.py:240-257.  The reference resamples 3-D tables to n_samples
+    ('linear') and wavetable_synthesis then reads them one frame per sample; the
+    kernel applies the same taps at frame rate.  2-D [batch, n_wavetable] tables
+    are resampled along n_wavetable as time, as the reference does, and read as
+    one static table of n_samples entries."""
+    if len(core._shape(wavetables)) == 2:  # pylint: disable=protected-access
+      wavetables = core.resample(wavetables, self.n_samples)
+    return core.wavetable_synthesis(amplitudes=amplitudes, wavetables=wavetables,
+                                    frequencies=f0_hz, n_samples=self.n_samples,
+                                    sample_rate=self.sample_rate)

@@ -468,6 +468,33 @@ int ddsp_b200_exp_decay_ir_backward(const float* gain, const float* decay,
                                     const float* grad_ir, float* grad_gain,
                                     float* grad_decay, int rows, int L, void* stream);
 
+/* core.wavetable_synthesis (core.py:1238-1282) with the tables kept at frame rate:
+ *   audio[b,t] = amp(t) * ((1 - frac) T_t[j0] + frac T_t[(j0 + 1) mod W]),
+ *   pos = phi(t) W, j0 = floor(pos), phi(t) = sum_{s<t} f0(s) / sr mod 1,
+ * with phi exact (64-bit fixed-point turns of the linearly interpolated f0).
+ * f0_hz, amplitudes: [B,F], N % F == 0; amplitudes upsampled with amp_method
+ * ('window' needs F < N).  wavetables: [B,Fw,W]; Fw == 1 is a static table, Fw > 1
+ * is interpolated in time with core.resample's 'linear' taps (add_endpoint), any
+ * Fw.  1 <= W <= 1048576, else E_UNSUPPORTED; B <= 65535.
+ * workspace: ddsp_b200_wavetable_workspace(B,F) bytes.
+ * backward: for grad_audio [B,N], writes any of d_f0 [B,F], d_amplitudes [B,F] and
+ * d_wavetables [B,Fw,W]; a NULL output is not computed.  d_f0 follows TensorFlow's
+ * subgradients: 0 where pos is an integer.  Table entries no sample reads are 0.
+ * No atomics: the gradients are bit-reproducible.
+ * workspace: ddsp_b200_wavetable_backward_workspace(B,F,N,Fw,W) bytes. */
+size_t ddsp_b200_wavetable_workspace(int B, int F);
+int ddsp_b200_wavetable_forward(const float* f0_hz, const float* amplitudes,
+                                const float* wavetables, float* audio, int B, int F,
+                                int N, int Fw, int W, float sample_rate, int amp_method,
+                                void* workspace, size_t workspace_bytes, void* stream);
+size_t ddsp_b200_wavetable_backward_workspace(int B, int F, int N, int Fw, int W);
+int ddsp_b200_wavetable_backward(const float* f0_hz, const float* amplitudes,
+                                 const float* wavetables, const float* grad_audio,
+                                 float* d_f0, float* d_amplitudes, float* d_wavetables,
+                                 int B, int F, int N, int Fw, int W, float sample_rate,
+                                 int amp_method, void* workspace, size_t workspace_bytes,
+                                 void* stream);
+
 #ifdef __cplusplus
 }
 #endif
