@@ -24,6 +24,7 @@ CTL_SCALE = 1
 CTL_NYQUIST = 2
 PAD_SAME = 0
 PAD_VALID = 1
+PAD_CENTER = 2
 LTI_REVERSE_AUDIO = 1
 LTI_REVERSE_IR = 2
 
@@ -124,6 +125,11 @@ SIGNATURES = {
     'ddsp_b200_wavetable_backward':
         (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _sz,
               _vp]),
+    'ddsp_b200_loudness_forward':
+        (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    'ddsp_b200_loudness_backward':
+        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    'ddsp_b200_rms_power': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
 }
 
 _lib = None

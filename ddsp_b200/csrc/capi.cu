@@ -25,6 +25,7 @@
 #include "fir_backward.cuh"
 #include "routing.cuh"
 #include "wavetable.cuh"
+#include "loudness.cuh"
 
 namespace ddsp {
 
@@ -1677,6 +1678,143 @@ int ddsp_b200_wavetable_backward(const float* f0_hz, const float* amplitudes,
       DDSP_CHECK_LAUNCH("wavetable_backward(reduce)");
     }
   }
+  return 0;
+}
+
+// ---- loudness and RMS power ----------------------------------------------------
+// The checks every framing entry point makes (spectral_ops.pad and
+// get_framed_lengths); sets *pad_left.  `name` prefixes the messages.
+static int framing_check(const char* name, int B, int N, int n_frames, int frame, int hop,
+                         int padding, int* pad_left) {
+  DDSP_REQUIRE(B >= 0 && N >= 1 && n_frames >= 0 && frame >= 1 && hop >= 1,
+               DDSP_B200_E_INVALID, "%s: bad shape B=%d N=%d T=%d frame=%d hop=%d", name, B,
+               N, n_frames, frame, hop);
+  DDSP_REQUIRE(padding == DDSP_B200_PAD_SAME || padding == DDSP_B200_PAD_VALID ||
+                   padding == DDSP_B200_PAD_CENTER,
+               DDSP_B200_E_INVALID, "%s: bad padding %d", name, padding);
+  DDSP_REQUIRE(padding == DDSP_B200_PAD_VALID || hop <= frame, DDSP_B200_E_INVALID,
+               "%s: frame_size (%d) must be greater than hop_size (%d)", name, frame, hop);
+  *pad_left = padding == DDSP_B200_PAD_CENTER ? frame / 2 : 0;
+  long long want;
+  if (padding == DDSP_B200_PAD_SAME) {
+    want = ((long long)N + hop - 1) / hop;
+  } else {
+    const long long padded = (long long)N + 2ll * *pad_left;
+    want = padded >= frame ? 1 + (padded - frame) / hop : 0;
+  }
+  DDSP_REQUIRE(n_frames == want, DDSP_B200_E_INVALID, "%s: n_frames=%d, the padding gives %lld",
+               name, n_frames, want);
+  if (B == 0) return 0;
+  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID, "%s: B=%d exceeds the 65535 grid limit", name,
+               B);
+  return 0;
+}
+
+static size_t ld_fwd_smem(int M, int warps, int64_t span) {
+  return sizeof(float2) * (size_t)M * (warps + 1) + sizeof(float) * (size_t)span;
+}
+static int ld_own(int n_fft) { return std::max(ld_::kMinOwn, n_fft); }
+static size_t ld_bwd_smem(int M, int warps, int own) {
+  return sizeof(float2) * (size_t)M * (warps + 1) + sizeof(float) * (size_t)own +
+         sizeof(int) * warps;
+}
+// Warps per CTA: the most of 8, 4, 2, 1 whose slices fit both kernels.  n_fft up to
+// ld_::kMaxFft always fits one.
+static int ld_warps(int n_fft) {
+  const int M = n_fft / 2;
+  int w = 8;
+  while (w > 1 && (ld_fwd_smem(M, w, n_fft) > kMaxDynSmem ||
+                   ld_bwd_smem(M, w, ld_own(n_fft)) > kMaxDynSmem))
+    w /= 2;
+  return w;
+}
+
+static int loud_check(const char* name, int B, int N, int n_frames, int n_fft, int hop,
+                      int padding, ld_::LoudParams* p) {
+  int pad_left = 0;
+  int rc = framing_check(name, B, N, n_frames, n_fft, hop, padding, &pad_left);
+  if (rc) return rc;
+  DDSP_REQUIRE(n_fft >= 2 && (n_fft & (n_fft - 1)) == 0, DDSP_B200_E_INVALID,
+               "%s: n_fft (%d) must be a power of two", name, n_fft);
+  DDSP_REQUIRE(n_fft <= ld_::kMaxFft, DDSP_B200_E_UNSUPPORTED,
+               "%s: n_fft=%d exceeds the %d supported", name, n_fft, ld_::kMaxFft);
+  p->N = N; p->T = n_frames; p->n_fft = n_fft; p->M = n_fft / 2; p->hop = hop;
+  p->pad_left = pad_left;
+  p->log2M = 0;
+  while ((1 << p->log2M) < p->M) ++p->log2M;
+  return 0;
+}
+
+static void db_params(ld_::LoudParams* p, float range_db, float ref_db) {
+  p->pmin = pow(10.0, -(double)range_db / 10.0);
+  p->range_db = (double)range_db;
+  p->ref_db = (double)ref_db;
+}
+
+int ddsp_b200_loudness_forward(const float* audio, const float* weights, float* loudness,
+                               int B, int N, int n_frames, int n_fft, int hop, int padding,
+                               float range_db, float ref_db, void* stream) {
+  DDSP_REQUIRE(audio && weights && (loudness || n_frames == 0), DDSP_B200_E_INVALID,
+               "loudness_forward: null pointer");
+  ld_::LoudParams p;
+  int rc = loud_check("loudness_forward", B, N, n_frames, n_fft, hop, padding, &p);
+  if (rc || B == 0 || n_frames == 0) return rc;
+  p.audio = audio; p.weights = weights;
+  db_params(&p, range_db, ref_db);
+  const int warps = ld_warps(n_fft);
+  int per_cta = 4 * warps;
+  while (per_cta > 1 &&
+         ld_fwd_smem(p.M, warps, (int64_t)(per_cta - 1) * hop + n_fft) > kMaxDynSmem)
+    per_cta /= 2;
+  const int span = (int)((int64_t)(per_cta - 1) * hop + n_fft);
+  const size_t smem = ld_fwd_smem(p.M, warps, span);
+  rc = set_smem(ld_::loudness_kernel, smem, "loudness_forward");
+  if (rc) return rc;
+  dim3 grid((unsigned)((n_frames + per_cta - 1) / per_cta), B);
+  ld_::loudness_kernel<<<grid, 32 * warps, smem, (cudaStream_t)stream>>>(p, loudness, per_cta,
+                                                                         span);
+  DDSP_CHECK_LAUNCH("loudness_forward");
+  return 0;
+}
+
+int ddsp_b200_loudness_backward(const float* audio, const float* weights,
+                                const float* grad_loudness, float* grad_audio, int B, int N,
+                                int n_frames, int n_fft, int hop, int padding, float range_db,
+                                float ref_db, void* stream) {
+  DDSP_REQUIRE(audio && weights && (grad_loudness || n_frames == 0) && grad_audio,
+               DDSP_B200_E_INVALID, "loudness_backward: null pointer");
+  ld_::LoudParams p;
+  int rc = loud_check("loudness_backward", B, N, n_frames, n_fft, hop, padding, &p);
+  if (rc || B == 0) return rc;
+  p.audio = audio; p.weights = weights;
+  db_params(&p, range_db, ref_db);
+  const int warps = ld_warps(n_fft), own = ld_own(n_fft);
+  const size_t smem = ld_bwd_smem(p.M, warps, own);
+  rc = set_smem(ld_::loudness_backward_kernel, smem, "loudness_backward");
+  if (rc) return rc;
+  dim3 grid((unsigned)((N + own - 1) / own), B);
+  ld_::loudness_backward_kernel<<<grid, 32 * warps, smem, (cudaStream_t)stream>>>(
+      p, grad_loudness, grad_audio, own);
+  DDSP_CHECK_LAUNCH("loudness_backward");
+  return 0;
+}
+
+int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n_frames,
+                        int frame_size, int hop, int padding, int in_db, float range_db,
+                        float ref_db, void* stream) {
+  DDSP_REQUIRE(audio && (power_db || n_frames == 0), DDSP_B200_E_INVALID,
+               "rms_power: null pointer");
+  int pad_left = 0;
+  int rc = framing_check("rms_power", B, N, n_frames, frame_size, hop, padding, &pad_left);
+  if (rc || B == 0 || n_frames == 0) return rc;
+  ld_::LoudParams d;
+  db_params(&d, range_db, ref_db);
+  const int64_t total = (int64_t)B * n_frames;
+  ld_::rms_power_kernel<<<grid_for(total * 32, ld_::kRmsThreads), ld_::kRmsThreads, 0,
+                          (cudaStream_t)stream>>>(audio, power_db, N, n_frames, total,
+                                                  frame_size, hop, pad_left, in_db, d.pmin,
+                                                  d.range_db, d.ref_db);
+  DDSP_CHECK_LAUNCH("rms_power");
   return 0;
 }
 

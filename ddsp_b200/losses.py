@@ -46,10 +46,6 @@ class SpectralLoss:
     self.cumsum_freq_weight = cumsum_freq_weight
     self.logmag_weight = logmag_weight
     self.loudness_weight = loudness_weight
-    if loudness_weight > 0:
-      raise NotImplementedError(
-          'loudness_weight needs spectral_ops.compute_loudness (A-weighting), '
-          'which is outside the decoder path (ae.gin:39-41 uses mag + logmag).')
     self.spectrogram_ops = [
         functools.partial(spectral_ops.compute_mag, size=size)
         for size in self.fft_sizes]
@@ -82,7 +78,19 @@ class SpectralLoss:
 
   def call(self, target_audio, audio, weights=None):
     if self._fusable(target_audio, audio, weights):
-      return self._call_fused(target_audio, audio)
+      loss = self._call_fused(target_audio, audio)
+    else:
+      loss = self._call_spectrograms(target_audio, audio, weights)
+    if self.loudness_weight > 0:
+      # losses.py:236-241: n_fft = 2048 and every other argument at its default,
+      # whatever the audio's sample rate
+      target = spectral_ops.compute_loudness(target_audio, n_fft=2048)
+      value = spectral_ops.compute_loudness(audio, n_fft=2048)
+      loss = loss + self.loudness_weight * mean_difference(
+          target, value, self.loss_type, weights=weights)
+    return loss
+
+  def _call_spectrograms(self, target_audio, audio, weights):
     loss = 0.0
     diff = lambda x, axis: torch.diff(x, dim=axis)
     for loss_op in self.spectrogram_ops:

@@ -4,7 +4,11 @@ Consumer of the decoder's audio in the C4 configuration (decoder -> multi-scale
 SpectralLoss).  Built on torch's cuFFT-backed FFT as SURVEY.md section 8f-1
 prescribes ("torch (cuFFT) first, not a hand kernel"); device-agnostic, so the
 CPU tests can pin it against the NumPy oracle.
+
+compute_loudness and compute_power run on hand-written CUDA kernels
+(csrc/loudness.cuh) instead: the framed audio would be 32x the input.
 """
+import numpy as np
 import torch
 
 
@@ -217,3 +221,158 @@ def stft_cuda(audio, frame_size, overlap=0.75):
   fft_length = 1 << (int(frame_size) - 1).bit_length()
   frames = FrameWindowFn.apply(audio.to(torch.float32), int(frame_size), step)
   return torch.fft.rfft(frames, n=fft_length, dim=-1)
+
+
+# ---- loudness and RMS power (spectral_ops.py:136-324, csrc/loudness.cuh) ------
+DB_RANGE = 80.0
+_A_WEIGHTS = {}
+
+
+def get_framed_lengths(input_length, frame_size, hop_size, padding='center'):
+  """spectral_ops.get_framed_lengths (spectral_ops.py:136-170): (n_frames,
+  padded_length) of a strided framing.  'valid' frames the signal as it is,
+  'center' adds frame_size samples (n_t / hop + 1 frames) and 'same' pads the end
+  so that n_frames = ceil(n_t / hop)."""
+  def n_frames(length):
+    return (length - frame_size) // hop_size + 1
+  if padding == 'valid':
+    return n_frames(input_length), input_length
+  if padding == 'center':
+    return n_frames(input_length + frame_size), input_length + frame_size
+  if padding == 'same':
+    n = -(-input_length // hop_size)
+    return n, (n - 1) * hop_size + frame_size
+  raise ValueError('`padding` must be one of [\'center\', \'same\', \'valid\'], '
+                   f'received ({padding}).')
+
+
+def _framing(audio, frame_size, hop_size, padding):
+  """spectral_ops.pad's checks in its order, on the shape alone: returns (B, N,
+  is_1d, n_frames, padding code).  n_frames is what tf.signal.frame gives on the
+  padded signal, 0 when 'valid' audio is shorter than a frame."""
+  from ddsp_b200 import _lib
+  shape = tuple(audio.shape) if torch.is_tensor(audio) else np.shape(audio)
+  if len(shape) == 3 and shape[-1] == 1:
+    shape = shape[:2]
+  if len(shape) not in (1, 2) or shape[-1] < 1:
+    raise ValueError(f'audio must be [batch, n_samples], [n_samples] or '
+                     f'[batch, n_samples, 1], got shape {tuple(shape)}')
+  if padding != 'valid' and hop_size > frame_size:
+    raise ValueError(f'During padding, frame_size ({frame_size}) must be greater '
+                     f'than hop_size ({hop_size}).')
+  if padding not in ('center', 'same', 'valid'):
+    raise ValueError('`padding` must be one of [\'center\', \'same\', \'valid\'], '
+                     f'received ({padding}).')
+  n = shape[-1]
+  if padding == 'same':
+    n_frames = -(-n // hop_size)
+  else:
+    padded = n + 2 * (frame_size // 2) if padding == 'center' else n
+    n_frames = 1 + (padded - frame_size) // hop_size if padded >= frame_size else 0
+  code = {'same': _lib.PAD_SAME, 'valid': _lib.PAD_VALID, 'center': _lib.PAD_CENTER}
+  return (1 if len(shape) == 1 else shape[0]), n, len(shape) == 1, n_frames, code[padding]
+
+
+def _audio_2d(audio, b, n):
+  from ddsp_b200 import core
+  return core.torch_float32(audio).reshape(b, n)
+
+
+def a_weighting(sample_rate, n_fft, device):
+  """10^(A_k / 10) of librosa.A_weighting(librosa.fft_frequencies(sr, n_fft)) with its
+  min_db = -80 clip, computed in float64 and cached per (sr, n_fft, device): the
+  [n_fft // 2 + 1] float32 weights compute_loudness applies to |X_k|^2."""
+  key = (float(sample_rate), int(n_fft), str(device))
+  if key not in _A_WEIGHTS:
+    f_sq = (np.arange(n_fft // 2 + 1, dtype=np.float64) * (sample_rate / n_fft)) ** 2
+    c = np.array([12194.217, 20.598997, 107.65265, 737.86223]) ** 2
+    with np.errstate(divide='ignore'):
+      a = 2.0 + 20.0 * (np.log10(c[0]) + 2 * np.log10(f_sq) - np.log10(f_sq + c[0])
+                        - np.log10(f_sq + c[1]) - 0.5 * np.log10(f_sq + c[2])
+                        - 0.5 * np.log10(f_sq + c[3]))
+    a = np.maximum(-80.0, a)
+    _A_WEIGHTS[key] = torch.as_tensor(10.0 ** (a / 10.0), dtype=torch.float32,
+                                      device=device)
+  return _A_WEIGHTS[key]
+
+
+class LoudnessFn(torch.autograd.Function):
+  """compute_loudness as one CUDA kernel, and its gradient w.r.t. the audio [B, N]
+  (csrc/loudness.cuh: the spectrum is recomputed, never saved)."""
+
+  @staticmethod
+  def forward(ctx, audio, weights, n_frames, n_fft, hop, padding, range_db, ref_db):
+    from ddsp_b200 import _lib
+    b, n = audio.shape
+    out = torch.empty((b, n_frames), dtype=torch.float32, device=audio.device)
+    _lib.check(_lib.load().ddsp_b200_loudness_forward(
+        audio.data_ptr(), weights.data_ptr(), out.data_ptr(), b, n, n_frames, n_fft, hop,
+        padding, range_db, ref_db, _stream()))
+    ctx.save_for_backward(audio, weights)
+    ctx.meta = (n_frames, n_fft, hop, padding, range_db, ref_db)
+    return out
+
+  @staticmethod
+  def backward(ctx, grad):
+    from ddsp_b200 import _lib
+    audio, weights = ctx.saved_tensors
+    n_frames, n_fft, hop, padding, range_db, ref_db = ctx.meta
+    b, n = audio.shape
+    grad = grad.to(torch.float32).contiguous()
+    grad_audio = torch.empty_like(audio)
+    _lib.check(_lib.load().ddsp_b200_loudness_backward(
+        audio.data_ptr(), weights.data_ptr(), grad.data_ptr(), grad_audio.data_ptr(), b, n,
+        n_frames, n_fft, hop, padding, range_db, ref_db, _stream()))
+    return grad_audio, None, None, None, None, None, None, None
+
+
+def compute_loudness(audio, sample_rate=16000, frame_rate=250, n_fft=512,
+                     range_db=DB_RANGE, ref_db=0.0, use_tf=True, padding='center'):
+  """spectral_ops.compute_loudness (spectral_ops.py:254-324): A-weighted power in dB,
+  [B, N] -> [B, T] and [N] -> [T] ([B, N, 1] is read as [B, N]).  Differentiable
+  through LoudnessFn; use_tf=False returns the same values as a NumPy array.  n_fft
+  must be a power of two (the reference's weighting only broadcasts then)."""
+  from ddsp_b200 import core
+  hop = int(sample_rate // frame_rate)
+  n_fft = int(n_fft)
+  b, n, is_1d, n_frames, code = _framing(audio, n_fft, hop, padding)
+  if n_fft < 2 or n_fft & (n_fft - 1):
+    raise ValueError(f'n_fft ({n_fft}) must be a power of two')
+  x = _audio_2d(audio, b, n)
+  with core._on_device_of(x):
+    out = LoudnessFn.apply(x, a_weighting(sample_rate, n_fft, x.device), n_frames,
+                           n_fft, hop, code, float(range_db), float(ref_db))
+  out = out[0] if is_1d else out
+  return out if use_tf else out.detach().cpu().numpy()
+
+
+def _rms(audio, sample_rate, frame_rate, frame_size, padding, in_db, range_db, ref_db,
+         name):
+  from ddsp_b200 import _lib, core
+  hop = int(sample_rate // frame_rate)
+  frame_size = int(frame_size)
+  b, n, is_1d, n_frames, code = _framing(audio, frame_size, hop, padding)
+  core._no_grad_path(name, audio)
+  x = _audio_2d(audio, b, n)
+  out = torch.empty((b, n_frames), dtype=torch.float32, device=x.device)
+  with core._on_device_of(x):
+    _lib.check(_lib.load().ddsp_b200_rms_power(
+        x.data_ptr(), out.data_ptr(), b, n, n_frames, frame_size, hop, code, int(in_db),
+        float(range_db), float(ref_db), _stream()))
+  return out[0] if is_1d else out
+
+
+def compute_rms_energy(audio, sample_rate=16000, frame_rate=250, frame_size=512,
+                       padding='center'):
+  """spectral_ops.compute_rms_energy (spectral_ops.py:223-231): mean(frame^2)^0.5 per
+  frame.  Forward only: an input that requires grad raises."""
+  return _rms(audio, sample_rate, frame_rate, frame_size, padding, False, DB_RANGE, 0.0,
+              'compute_rms_energy')
+
+
+def compute_power(audio, sample_rate=16000, frame_rate=250, frame_size=512, ref_db=0.0,
+                  range_db=DB_RANGE, padding='center'):
+  """spectral_ops.compute_power (spectral_ops.py:234-249): amplitude_to_db of the RMS
+  energy, i.e. power_to_db(mean(frame^2)).  Forward only."""
+  return _rms(audio, sample_rate, frame_rate, frame_size, padding, True, range_db, ref_db,
+              'compute_power')

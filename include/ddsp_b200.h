@@ -60,8 +60,9 @@ enum {
   DDSP_B200_CTL_NYQUIST = 2           /* normalize_below_nyquist=True          */
 };
 
-/* padding of ddsp_b200_fir_time_varying (core.py:1338-1379) */
-enum { DDSP_B200_PAD_SAME = 0, DDSP_B200_PAD_VALID = 1 };
+/* padding of ddsp_b200_fir_time_varying (core.py:1338-1379); the framing entry points
+ * (loudness, rms_power: spectral_ops.pad) also take CENTER */
+enum { DDSP_B200_PAD_SAME = 0, DDSP_B200_PAD_VALID = 1, DDSP_B200_PAD_CENTER = 2 };
 
 int ddsp_b200_version(void);
 /* Thread-local description of the last non-zero return on this thread. */
@@ -494,6 +495,31 @@ int ddsp_b200_wavetable_backward(const float* f0_hz, const float* amplitudes,
                                  int B, int F, int N, int Fw, int W, float sample_rate,
                                  int amp_method, void* workspace, size_t workspace_bytes,
                                  void* stream);
+
+/* spectral_ops.compute_loudness (spectral_ops.py:254-324) on audio [B,N]: frames of
+ * n_fft samples every hop under `padding` (DDSP_B200_PAD_*; CENTER pads n_fft/2 zeros
+ * on both sides, SAME pads the end to (ceil(N/hop) - 1) hop + n_fft, VALID nothing),
+ * periodic Hann window, loudness[b,t] = power_to_db(mean_k weights[k] |X_k|^2) with
+ * ref_db and range_db.  weights: [n_fft/2 + 1] device floats, the linear A-weighting.
+ * n_frames must be the frame count of that padding (1 + (padded - n_fft) / hop, or
+ * ceil(N/hop) for SAME).  n_fft is a power of two, hop <= n_fft unless VALID;
+ * n_fft > 16384 is E_UNSUPPORTED.  B <= 65535.
+ * backward: grad_audio [B,N] for grad_loudness [B,T], with tf.maximum's tie rule (no
+ * gradient through an active clamp).  No atomics: bit-reproducible. */
+int ddsp_b200_loudness_forward(const float* audio, const float* weights, float* loudness,
+                               int B, int N, int n_frames, int n_fft, int hop, int padding,
+                               float range_db, float ref_db, void* stream);
+int ddsp_b200_loudness_backward(const float* audio, const float* weights,
+                                const float* grad_loudness, float* grad_audio, int B, int N,
+                                int n_frames, int n_fft, int hop, int padding, float range_db,
+                                float ref_db, void* stream);
+/* spectral_ops.compute_power (spectral_ops.py:223-249): power_db[b,t] =
+ * power_to_db(mean(frame^2)) with frames of any frame_size every hop, padded as above
+ * (CENTER pads frame_size/2 zeros on both sides).  in_db == 0 writes
+ * compute_rms_energy's mean(frame^2)^0.5 instead.  Forward only. */
+int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n_frames,
+                        int frame_size, int hop, int padding, int in_db, float range_db,
+                        float ref_db, void* stream);
 
 #ifdef __cplusplus
 }
