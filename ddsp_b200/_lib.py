@@ -25,6 +25,9 @@ CTL_NYQUIST = 2
 PAD_SAME = 0
 PAD_VALID = 1
 PAD_CENTER = 2
+MEL = 0
+LOGMEL = 1
+MFCC = 2
 LTI_REVERSE_AUDIO = 1
 LTI_REVERSE_IR = 2
 
@@ -130,6 +133,10 @@ SIGNATURES = {
     'ddsp_b200_loudness_backward':
         (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
     'ddsp_b200_rms_power': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
+    'ddsp_b200_mel_forward':
+        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    'ddsp_b200_mel_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
 }
 
 _lib = None

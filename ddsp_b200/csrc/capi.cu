@@ -26,6 +26,7 @@
 #include "routing.cuh"
 #include "wavetable.cuh"
 #include "loudness.cuh"
+#include "mel.cuh"
 
 namespace ddsp {
 
@@ -1815,6 +1816,140 @@ int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n
                                                   frame_size, hop, pad_left, in_db, d.pmin,
                                                   d.range_db, d.ref_db);
   DDSP_CHECK_LAUNCH("rms_power");
+  return 0;
+}
+
+// ---- mel, log-mel and MFCC -------------------------------------------------------
+// Twiddles and one FFT slice per warp, one [bins] row per warp, and the MFCC's
+// 4 bins cosine table.
+static size_t mel_fixed_smem(int M, int warps, int bins, int mode) {
+  return sizeof(float2) * (size_t)M * (warps + 1) +
+         sizeof(float) * (size_t)bins * (warps + (mode == DDSP_B200_MFCC ? 4 : 0));
+}
+static size_t mel_bwd_smem(int M, int warps, int bins, int mode, int own) {
+  return mel_fixed_smem(M, warps, bins, mode) + sizeof(float) * (size_t)own +
+         sizeof(int) * warps;
+}
+// Warps per CTA: the most of 8, 4, 2, 1 whose backward fits with the smallest owned
+// span.  bins <= mel_::kMaxBins fits one warp at every fft_length.
+static int mel_warps(int M, int bins, int mode) {
+  int w = 8;
+  while (w > 1 && mel_bwd_smem(M, w, bins, mode, mel_::kOwnFloor) > kMaxDynSmem) w /= 2;
+  return w;
+}
+// Backward: samples a CTA owns, max(kMinOwn, fft_size) halved until it fits.
+static int mel_own(int fft_size, int M, int warps, int bins, int mode) {
+  int own = std::max(mel_::kMinOwn, fft_size);
+  while (own > mel_::kOwnFloor && mel_bwd_smem(M, warps, bins, mode, own) > kMaxDynSmem)
+    own /= 2;
+  return own;
+}
+
+static int mel_check(const char* name, int B, int N, int n_frames, int fft_size,
+                     int fft_length, int hop, int pad_end, int bins, int n_out, int mode,
+                     mel_::MelParams* p) {
+  DDSP_REQUIRE(B >= 0 && N >= 1 && n_frames >= 0 && fft_size >= 1 && hop >= 1,
+               DDSP_B200_E_INVALID, "%s: bad shape B=%d N=%d T=%d fft_size=%d hop=%d", name,
+               B, N, n_frames, fft_size, hop);
+  DDSP_REQUIRE(pad_end == 0 || pad_end == 1, DDSP_B200_E_INVALID, "%s: bad pad_end %d", name,
+               pad_end);
+  DDSP_REQUIRE(mode == DDSP_B200_MEL || mode == DDSP_B200_LOGMEL || mode == DDSP_B200_MFCC,
+               DDSP_B200_E_INVALID, "%s: bad mode %d", name, mode);
+  DDSP_REQUIRE(bins >= 1 && (mode == DDSP_B200_MFCC ? n_out >= 0 && n_out <= bins
+                                                    : n_out == bins),
+               DDSP_B200_E_INVALID, "%s: bad bins=%d n_out=%d for mode %d", name, bins, n_out,
+               mode);
+  DDSP_REQUIRE(fft_length >= 1 && (fft_length & (fft_length - 1)) == 0, DDSP_B200_E_INVALID,
+               "%s: fft_length (%d) must be a power of two", name, fft_length);
+  DDSP_REQUIRE(fft_length >= 2 && fft_length <= ld_::kMaxFft, DDSP_B200_E_UNSUPPORTED,
+               "%s: fft_length=%d is outside the 2..%d supported", name, fft_length,
+               ld_::kMaxFft);
+  DDSP_REQUIRE(fft_size <= fft_length, DDSP_B200_E_INVALID,
+               "%s: fft_size (%d) exceeds fft_length (%d)", name, fft_size, fft_length);
+  DDSP_REQUIRE(bins <= mel_::kMaxBins, DDSP_B200_E_UNSUPPORTED,
+               "%s: bins=%d exceeds the %d supported", name, bins, mel_::kMaxBins);
+  const long long want = pad_end ? ((long long)N + hop - 1) / hop
+                                 : (N >= fft_size ? 1 + (long long)(N - fft_size) / hop : 0);
+  DDSP_REQUIRE(n_frames == want, DDSP_B200_E_INVALID, "%s: n_frames=%d, the padding gives %lld",
+               name, n_frames, want);
+  if (B == 0) return 0;
+  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID, "%s: B=%d exceeds the 65535 grid limit", name,
+               B);
+  p->N = N; p->T = n_frames; p->fft_size = fft_size; p->M = fft_length / 2; p->hop = hop;
+  p->bins = bins; p->C = n_out;
+  p->log2M = 0;
+  while ((1 << p->log2M) < p->M) ++p->log2M;
+  return 0;
+}
+
+static void mel_tables(mel_::MelParams* p, const float* audio, const float* window,
+                       const void* mel_table, int fft_length, int bins) {
+  const int K = fft_length / 2 + 1;
+  p->audio = audio; p->window = window;
+  p->wpair = static_cast<const float2*>(mel_table);
+  p->band = reinterpret_cast<const int*>(p->wpair + K);
+  p->band_lo = p->band + K;
+  p->band_hi = p->band_lo + bins;
+}
+
+int ddsp_b200_mel_forward(const float* audio, const float* window, const void* mel_table,
+                          float* out, int B, int N, int n_frames, int fft_size, int fft_length,
+                          int hop, int pad_end, int bins, int n_out, int mode, void* stream) {
+  DDSP_REQUIRE(audio && window && mel_table && (out || n_frames == 0 || n_out == 0),
+               DDSP_B200_E_INVALID, "mel_forward: null pointer");
+  mel_::MelParams p;
+  int rc = mel_check("mel_forward", B, N, n_frames, fft_size, fft_length, hop, pad_end, bins,
+                     n_out, mode, &p);
+  if (rc || B == 0 || n_frames == 0 || n_out == 0) return rc;
+  mel_tables(&p, audio, window, mel_table, fft_length, bins);
+  const int warps = mel_warps(p.M, bins, mode);
+  const size_t fixed = mel_fixed_smem(p.M, warps, bins, mode);
+  // stage the audio span of per_cta frames; when not even two fit, each warp reads
+  // its own frame from global memory
+  int per_cta = 4 * warps;
+  while (per_cta > 1 &&
+         fixed + sizeof(float) * ((int64_t)(per_cta - 1) * hop + fft_size) > kMaxDynSmem)
+    per_cta /= 2;
+  int span = (int)((int64_t)(per_cta - 1) * hop + fft_size);
+  if (per_cta == 1) {
+    per_cta = warps;
+    span = 0;
+  }
+  const size_t smem = fixed + sizeof(float) * (size_t)span;
+  auto kern = mode == DDSP_B200_MEL      ? mel_::mel_kernel<mel_::kMel>
+              : mode == DDSP_B200_LOGMEL ? mel_::mel_kernel<mel_::kLogMel>
+                                         : mel_::mel_kernel<mel_::kMfcc>;
+  rc = set_smem(kern, smem, "mel_forward");
+  if (rc) return rc;
+  dim3 grid((unsigned)((n_frames + per_cta - 1) / per_cta), B);
+  kern<<<grid, 32 * warps, smem, (cudaStream_t)stream>>>(p, out, per_cta, span);
+  DDSP_CHECK_LAUNCH("mel_forward");
+  return 0;
+}
+
+int ddsp_b200_mel_backward(const float* audio, const float* window, const void* mel_table,
+                           const float* grad_out, float* grad_audio, int B, int N,
+                           int n_frames, int fft_size, int fft_length, int hop, int pad_end,
+                           int bins, int n_out, int mode, void* stream) {
+  DDSP_REQUIRE(audio && window && mel_table && (grad_out || n_frames == 0 || n_out == 0) &&
+                   grad_audio,
+               DDSP_B200_E_INVALID, "mel_backward: null pointer");
+  mel_::MelParams p;
+  int rc = mel_check("mel_backward", B, N, n_frames, fft_size, fft_length, hop, pad_end, bins,
+                     n_out, mode, &p);
+  if (rc || B == 0 || n_frames == 0 || n_out == 0) return rc;
+  mel_tables(&p, audio, window, mel_table, fft_length, bins);
+  const int warps = mel_warps(p.M, bins, mode);
+  const int own = mel_own(fft_size, p.M, warps, bins, mode);
+  const size_t smem = mel_bwd_smem(p.M, warps, bins, mode, own);
+  auto kern = mode == DDSP_B200_MEL      ? mel_::mel_backward_kernel<mel_::kMel>
+              : mode == DDSP_B200_LOGMEL ? mel_::mel_backward_kernel<mel_::kLogMel>
+                                         : mel_::mel_backward_kernel<mel_::kMfcc>;
+  rc = set_smem(kern, smem, "mel_backward");
+  if (rc) return rc;
+  dim3 grid((unsigned)((N + own - 1) / own), B);
+  kern<<<grid, 32 * warps, smem, (cudaStream_t)stream>>>(p, grad_out, grad_audio, own);
+  DDSP_CHECK_LAUNCH("mel_backward");
   return 0;
 }
 

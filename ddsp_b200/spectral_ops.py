@@ -6,7 +6,8 @@ prescribes ("torch (cuFFT) first, not a hand kernel"); device-agnostic, so the
 CPU tests can pin it against the NumPy oracle.
 
 compute_loudness and compute_power run on hand-written CUDA kernels
-(csrc/loudness.cuh) instead: the framed audio would be 32x the input.
+(csrc/loudness.cuh) instead: the framed audio would be 32x the input.  So do
+compute_mel, compute_logmel and compute_mfcc (csrc/mel.cuh).
 """
 import numpy as np
 import torch
@@ -376,3 +377,199 @@ def compute_power(audio, sample_rate=16000, frame_rate=250, frame_size=512, ref_
   energy, i.e. power_to_db(mean(frame^2)).  Forward only."""
   return _rms(audio, sample_rate, frame_rate, frame_size, padding, True, range_db, ref_db,
               'compute_power')
+
+
+# ---- mel, log-mel, MFCC and log magnitude (spectral_ops.py:67-133, csrc/mel.cuh) --
+MAX_MEL_FFT = 16384
+MAX_MEL_BINS = 1024
+_MEL_TABLES = {}
+_MEL_WINDOWS = {}
+
+
+def compute_logmag(audio, size=2048, overlap=0.75, pad_end=True):
+  """spectral_ops.compute_logmag (spectral_ops.py:92-94): safe_log of compute_mag."""
+  return safe_log(compute_mag(audio, size, overlap, pad_end))
+
+
+def _mel_arguments(num_mel_bins, sample_rate, lower_edge_hertz, upper_edge_hertz):
+  """The checks of tf.signal.linear_to_mel_weight_matrix, in its order."""
+  if num_mel_bins <= 0:
+    raise ValueError('num_mel_bins must be positive. Got: %s' % num_mel_bins)
+  if lower_edge_hertz < 0.0:
+    raise ValueError('lower_edge_hertz must be non-negative. Got: %s' % lower_edge_hertz)
+  if lower_edge_hertz >= upper_edge_hertz:
+    raise ValueError('lower_edge_hertz %.1f >= upper_edge_hertz %.1f' %
+                     (lower_edge_hertz, upper_edge_hertz))
+  if sample_rate <= 0.0:
+    raise ValueError('sample_rate must be positive. Got: %s' % sample_rate)
+  if upper_edge_hertz > sample_rate / 2:
+    raise ValueError('upper_edge_hertz must not be larger than the Nyquist frequency '
+                     '(sample_rate / 2). Got %s for sample_rate: %s' %
+                     (upper_edge_hertz, sample_rate))
+
+
+def linear_to_mel_weight_matrix(num_mel_bins=20, num_spectrogram_bins=129,
+                                sample_rate=8000, lower_edge_hertz=125.0,
+                                upper_edge_hertz=3800.0):
+  """tf.signal.linear_to_mel_weight_matrix in float64 NumPy, [K, bins]: HTK mel scale
+  1127 ln(1 + f / 700), bin frequencies linspace(0, sr / 2, K) with the DC row zero,
+  band edges linspace(mel(lo), mel(hi), bins + 2), and each weight
+  max(0, min(rising, falling)) in mel space."""
+  _mel_arguments(num_mel_bins, sample_rate, lower_edge_hertz, upper_edge_hertz)
+  def mel(f):
+    return 1127.0 * np.log(1.0 + np.asarray(f, np.float64) / 700.0)
+  freqs = np.linspace(0.0, sample_rate / 2.0, num_spectrogram_bins)[1:]
+  spec_mel = mel(freqs)[:, None]
+  edges = np.linspace(mel(lower_edge_hertz), mel(upper_edge_hertz), num_mel_bins + 2)
+  lower, center, upper = edges[None, :-2], edges[None, 1:-1], edges[None, 2:]
+  rising = (spec_mel - lower) / (center - lower)
+  falling = (upper - spec_mel) / (upper - center)
+  w = np.maximum(0.0, np.minimum(rising, falling))
+  return np.pad(w, [[1, 0], [0, 0]])
+
+
+def mel_table(bins, n_spectrogram_bins, sample_rate, lo_hz, hi_hz, device):
+  """linear_to_mel_weight_matrix in the sparse layout csrc/mel.cuh reads (one int32
+  tensor of 3 K + 2 bins words, include/ddsp_b200.h): per bin its first band and the
+  float32 weights into that band and the next, per band its bin range.  Computed in
+  float64 and cached per (bins, K, sr, lo, hi, device)."""
+  key = (int(bins), int(n_spectrogram_bins), float(sample_rate), float(lo_hz),
+         float(hi_hz), str(device))
+  if key not in _MEL_TABLES:
+    w = linear_to_mel_weight_matrix(bins, n_spectrogram_bins, sample_rate, lo_hz, hi_hz)
+    nz = w != 0.0
+    rows = np.arange(w.shape[0])
+    count = nz.sum(1)
+    first = np.where(count > 0, nz.argmax(1), -1)
+    nxt = np.minimum(first + 1, bins - 1)
+    if (count > 2).any() or ((count == 2) & ~nz[rows, nxt]).any():
+      raise AssertionError('mel weights outside two adjacent bands')
+    pair = np.zeros((w.shape[0], 2), np.float64)
+    pair[:, 0] = np.where(first >= 0, w[rows, np.maximum(first, 0)], 0.0)
+    pair[:, 1] = np.where((first >= 0) & (first + 1 < bins), w[rows, nxt], 0.0)
+    band_lo = np.zeros(bins, np.int32)
+    band_hi = np.zeros(bins, np.int32)
+    for j in range(bins):
+      ks = np.flatnonzero(nz[:, j])
+      if ks.size:
+        if ks[-1] + 1 - ks[0] != ks.size:
+          raise AssertionError('mel band %d is not one run of bins' % j)
+        band_lo[j], band_hi[j] = ks[0], ks[-1] + 1
+    words = np.concatenate([pair.astype(np.float32).reshape(-1).view(np.int32),
+                            first.astype(np.int32), band_lo, band_hi])
+    _MEL_TABLES[key] = torch.as_tensor(words, device=device)
+  return _MEL_TABLES[key]
+
+
+def mel_window(fft_size, device):
+  """tf.signal.hann_window(fft_size): periodic for even lengths, symmetric for odd
+  ones, computed in float64 and cached as float32 per (fft_size, device)."""
+  key = (int(fft_size), str(device))
+  if key not in _MEL_WINDOWS:
+    n = np.arange(fft_size, dtype=np.float64)
+    d = fft_size if fft_size % 2 == 0 else fft_size - 1
+    w = 0.5 - 0.5 * np.cos(2.0 * np.pi * n / d) if fft_size > 1 else np.ones(1)
+    _MEL_WINDOWS[key] = torch.as_tensor(w, dtype=torch.float32, device=device)
+  return _MEL_WINDOWS[key]
+
+
+class MelFn(torch.autograd.Function):
+  """compute_mel / compute_logmel / compute_mfcc as one CUDA kernel, and the gradient
+  w.r.t. the audio [B, N] (csrc/mel.cuh: the spectrum and the mel values are
+  recomputed, never saved).  meta = (n_frames, fft_size, fft_length, hop, pad_end,
+  bins, n_out, mode)."""
+
+  @staticmethod
+  def forward(ctx, audio, window, table, meta):
+    from ddsp_b200 import _lib
+    n_frames, fft_size, fft_length, hop, pad_end, bins, n_out, mode = meta
+    b, n = audio.shape
+    out = torch.empty((b, n_frames, n_out), dtype=torch.float32, device=audio.device)
+    _lib.check(_lib.load().ddsp_b200_mel_forward(
+        audio.data_ptr(), window.data_ptr(), table.data_ptr(), out.data_ptr(), b, n,
+        n_frames, fft_size, fft_length, hop, pad_end, bins, n_out, mode, _stream()))
+    ctx.save_for_backward(audio, window, table)
+    ctx.meta = meta
+    return out
+
+  @staticmethod
+  def backward(ctx, grad):
+    from ddsp_b200 import _lib
+    audio, window, table = ctx.saved_tensors
+    n_frames, fft_size, fft_length, hop, pad_end, bins, n_out, mode = ctx.meta
+    b, n = audio.shape
+    if n_frames == 0 or n_out == 0:
+      return torch.zeros_like(audio), None, None, None
+    grad = grad.to(torch.float32).contiguous()
+    grad_audio = torch.empty_like(audio)
+    _lib.check(_lib.load().ddsp_b200_mel_backward(
+        audio.data_ptr(), window.data_ptr(), table.data_ptr(), grad.data_ptr(),
+        grad_audio.data_ptr(), b, n, n_frames, fft_size, fft_length, hop, pad_end, bins,
+        n_out, mode, _stream()))
+    return grad_audio, None, None, None
+
+
+def _mel(audio, lo_hz, hi_hz, bins, fft_size, overlap, pad_end, sample_rate, mode,
+         mfcc_bins=None, name='compute_mel'):
+  """The shape and argument checks (all before any device work), then MelFn."""
+  from ddsp_b200 import _lib, core
+  shape = tuple(audio.shape) if torch.is_tensor(audio) else np.shape(audio)
+  if len(shape) == 3 and shape[-1] == 1:
+    shape = shape[:2]
+  if len(shape) not in (1, 2) or shape[-1] < 1:
+    raise ValueError(f'audio must be [batch, n_samples], [n_samples] or '
+                     f'[batch, n_samples, 1], got shape {tuple(shape)}')
+  fft_size = int(fft_size)
+  if fft_size < 1:
+    raise ValueError(f'fft_size must be positive, got {fft_size}')
+  hop = int(fft_size * (1.0 - overlap))
+  if hop < 1:
+    raise ValueError(f'frame_step = int(fft_size * (1 - overlap)) must be positive, got '
+                     f'{hop} (fft_size {fft_size}, overlap {overlap})')
+  bins = int(bins)
+  _mel_arguments(bins, sample_rate, lo_hz, hi_hz)
+  fft_length = 1 << (fft_size - 1).bit_length()
+  if not 2 <= fft_length <= MAX_MEL_FFT:
+    raise NotImplementedError(f'{name}: fft_size={fft_size} gives fft_length={fft_length}, '
+                              f'outside the 2..{MAX_MEL_FFT} supported')
+  if bins > MAX_MEL_BINS:
+    raise NotImplementedError(f'{name}: bins={bins} exceeds the {MAX_MEL_BINS} supported')
+  n = shape[-1]
+  b = 1 if len(shape) == 1 else shape[0]
+  n_frames = -(-n // hop) if pad_end else max(0, 1 + (n - fft_size) // hop)
+  n_out = len(range(bins)[:mfcc_bins]) if mode == _lib.MFCC else bins
+  x = _audio_2d(audio, b, n)
+  with core._on_device_of(x):
+    meta = (n_frames, fft_size, fft_length, hop, int(bool(pad_end)), bins, n_out, mode)
+    out = MelFn.apply(x, mel_window(fft_size, x.device),
+                      mel_table(bins, fft_length // 2 + 1, sample_rate, lo_hz, hi_hz,
+                                x.device), meta)
+  return out[0] if len(shape) == 1 else out
+
+
+def compute_mel(audio, lo_hz=0.0, hi_hz=8000.0, bins=64, fft_size=2048, overlap=0.75,
+                pad_end=True, sample_rate=16000):
+  """spectral_ops.compute_mel (spectral_ops.py:73-89): |stft| projected on
+  linear_to_mel_weight_matrix, [B, N] -> [B, T, bins] and [N] -> [T, bins] ([B, N, 1]
+  is read as [B, N]).  Differentiable through MelFn."""
+  from ddsp_b200 import _lib
+  return _mel(audio, lo_hz, hi_hz, bins, fft_size, overlap, pad_end, sample_rate,
+              _lib.MEL)
+
+
+def compute_logmel(audio, lo_hz=80.0, hi_hz=7600.0, bins=64, fft_size=2048, overlap=0.75,
+                   pad_end=True, sample_rate=16000):
+  """spectral_ops.compute_logmel (spectral_ops.py:97-109): safe_log of compute_mel."""
+  from ddsp_b200 import _lib
+  return _mel(audio, lo_hz, hi_hz, bins, fft_size, overlap, pad_end, sample_rate,
+              _lib.LOGMEL, name='compute_logmel')
+
+
+def compute_mfcc(audio, lo_hz=20.0, hi_hz=8000.0, fft_size=1024, mel_bins=128,
+                 mfcc_bins=13, overlap=0.75, pad_end=True, sample_rate=16000):
+  """spectral_ops.compute_mfcc (spectral_ops.py:112-133):
+  tf.signal.mfccs_from_log_mel_spectrograms of compute_logmel (the unnormalised DCT-II
+  times rsqrt(2 mel_bins)), cut to [..., :mfcc_bins] with Python's slice rules."""
+  from ddsp_b200 import _lib
+  return _mel(audio, lo_hz, hi_hz, mel_bins, fft_size, overlap, pad_end, sample_rate,
+              _lib.MFCC, mfcc_bins=mfcc_bins, name='compute_mfcc')

@@ -521,6 +521,33 @@ int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n
                         int frame_size, int hop, int padding, int in_db, float range_db,
                         float ref_db, void* stream);
 
+/* output stage of ddsp_b200_mel_forward / _backward */
+enum { DDSP_B200_MEL = 0, DDSP_B200_LOGMEL = 1, DDSP_B200_MFCC = 2 };
+
+/* spectral_ops.compute_mel / compute_logmel / compute_mfcc (spectral_ops.py:73-133) on
+ * audio [B,N]: tf.signal.stft frames of fft_size samples every hop (pad_end = 1 pads
+ * zeros past the end, n_frames = ceil(N / hop); pad_end = 0 pads nothing, n_frames =
+ * 1 + (N - fft_size) / hop, or 0 when N < fft_size), times window[fft_size], zero
+ * padded to fft_length (a power of two >= fft_size), real FFT of K = fft_length/2 + 1
+ * bins; mel[t,j] = sum_k W[k,j] |X_k|.  mode MEL writes out[B,T,bins] = mel, LOGMEL
+ * log(mel <= 0 ? 1e-5 : mel), MFCC the first n_out coefficients of the log-mel's
+ * unnormalised DCT-II times rsqrt(2 bins), out[B,T,n_out] (n_out == bins otherwise).
+ * mel_table: W in sparse form, 3K + 2 bins 32-bit words: [K] float pairs (w_lo, w_hi),
+ * [K] int32 band, [bins] int32 band_lo, [bins] int32 band_hi.  Bin k weighs w_lo into
+ * band[k] (when >= 0) and w_hi into band[k] + 1 (when < bins), band j sums its bins
+ * k in [band_lo[j], band_hi[j]), and band[] must lie in {j - 1, j} there.  fft_length
+ * outside 2..16384 and bins > 1024 are E_UNSUPPORTED.  B <= 65535.  B = 0, n_frames = 0
+ * and n_out = 0 return before any launch (backward: grad_audio is then not written).
+ * backward: grad_audio [B,N] for grad_out [B,T,C], TensorFlow's gradient (no gradient
+ * through mel <= 0 in the log, none through |X_k| = 0).  No atomics: bit-reproducible. */
+int ddsp_b200_mel_forward(const float* audio, const float* window, const void* mel_table,
+                          float* out, int B, int N, int n_frames, int fft_size, int fft_length,
+                          int hop, int pad_end, int bins, int n_out, int mode, void* stream);
+int ddsp_b200_mel_backward(const float* audio, const float* window, const void* mel_table,
+                           const float* grad_out, float* grad_audio, int B, int N,
+                           int n_frames, int fft_size, int fft_length, int hop, int pad_end,
+                           int bins, int n_out, int mode, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
