@@ -137,6 +137,14 @@ SIGNATURES = {
         (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
     'ddsp_b200_mel_backward':
         (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    'ddsp_b200_mixture_nll_forward':
+        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
+    'ddsp_b200_mixture_nll_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
+    'ddsp_b200_comb_nll_forward':
+        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
+    'ddsp_b200_comb_nll_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
 }
 
 _lib = None

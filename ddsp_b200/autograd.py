@@ -27,6 +27,9 @@ kernels, exposed as `torch.autograd.Function`s:
     short reverbs), the impulse-response synthesis and their composition, routed to
     by `core.fft_convolve` / `core.frequency_impulse_response` /
     `core.frequency_filter` under grad;
+  * `MixtureNLLFn` / `CombNLLFn` - the Gaussian-mixture NLLs of the consistency
+    losses (`losses.KDEConsistencyLoss`, `losses.TWMLoss`), evaluated per frame
+    on-chip with gradients to every input;
   * `DecoderFn` / `decoder_train` - the whole `ae.gin` decoder from RAW network
     outputs: forward is the fused two-kernel pipeline (`get_controls` in shared
     memory), backward is the two synthesizer backward kernels plus the
@@ -531,6 +534,92 @@ class ExpDecayIrFn(torch.autograd.Function):
           offset & (2**64 - 1), g.data_ptr(), core._ptr(d_gain), core._ptr(d_decay),
           gain.shape[0], length, core._stream()))
     return d_gain, d_decay, None, None, None, None
+
+
+class MixtureNLLFn(torch.autograd.Function):
+  """-log p(x | mixture) per query (csrc/consistency.cuh, mode A): for queries x
+  [B, T, Q], components mu and log-weights lw [B, T, J] and a scalar scale, the
+  Gaussian mixture NLL of each query under its own frame's mixture, [B, T, Q].  The
+  mixture of `KDEConsistencyLoss.nll` and `TWMLoss`'s p(harmonics | sinusoids);
+  differentiable in x, mu and lw by one backward launch.  With no components the
+  logsumexp is over nothing: the NLL is +inf and every gradient 0."""
+
+  @staticmethod
+  def forward(ctx, x, mu, lw, scale):
+    x, mu, lw = (t.contiguous().to(torch.float32) for t in (x, mu, lw))
+    b, t, q = x.shape
+    j = mu.shape[-1]
+    ctx.save_for_backward(x, mu, lw)
+    ctx.scale = float(scale)
+    with core._on_device_of(x, mu, lw):
+      if j == 0:
+        return torch.full_like(x, math.inf)
+      nll = torch.empty_like(x)
+      _lib.check(_lib.load().ddsp_b200_mixture_nll_forward(
+          x.data_ptr(), mu.data_ptr(), lw.data_ptr(), nll.data_ptr(), b, t, q, j,
+          ctx.scale, core._stream()))
+    return nll
+
+  @staticmethod
+  def backward(ctx, grad):
+    x, mu, lw = ctx.saved_tensors
+    b, t, q = x.shape
+    j = mu.shape[-1]
+    g = grad.contiguous().to(torch.float32)
+    with core._on_device_of(x, mu, lw, g):
+      if j == 0:
+        dx, dmu, dlw = torch.zeros_like(x), torch.zeros_like(mu), torch.zeros_like(lw)
+      else:
+        dx, dmu, dlw = torch.empty_like(x), torch.empty_like(mu), torch.empty_like(lw)
+        _lib.check(_lib.load().ddsp_b200_mixture_nll_backward(
+            x.data_ptr(), mu.data_ptr(), lw.data_ptr(), g.data_ptr(), dx.data_ptr(),
+            dmu.data_ptr(), dlw.data_ptr(), b, t, q, j, ctx.scale, core._stream()))
+    want = ctx.needs_input_grad
+    return (dx if want[0] else None, dmu if want[1] else None,
+            dlw if want[2] else None, None)
+
+
+class CombNLLFn(torch.autograd.Function):
+  """`TWMLoss`'s amplitude-weighted -log p(sinusoids | harmonics) (csrc/consistency.cuh,
+  mode B): for candidates f0 [B, T, C], points f and amplitudes a [B, T, P], the
+  `safe_divide`d mean over points of the comb NLL of f_p / f0_c, [B, T, C];
+  differentiable in f0, f and a by one backward launch.  With no points the mean is
+  0 / 1e-7 = 0."""
+
+  @staticmethod
+  def forward(ctx, f0, f, a, n_gaussians, scale):
+    f0, f, a = (t.contiguous().to(torch.float32) for t in (f0, f, a))
+    b, t, c = f0.shape
+    p = f.shape[-1]
+    ctx.save_for_backward(f0, f, a)
+    ctx.cfg = (int(n_gaussians), float(scale))
+    with core._on_device_of(f0, f, a):
+      if p == 0:
+        return torch.zeros_like(f0)
+      out = torch.empty_like(f0)
+      _lib.check(_lib.load().ddsp_b200_comb_nll_forward(
+          f0.data_ptr(), f.data_ptr(), a.data_ptr(), out.data_ptr(), b, t, c, p,
+          ctx.cfg[0], ctx.cfg[1], core._stream()))
+    return out
+
+  @staticmethod
+  def backward(ctx, grad):
+    f0, f, a = ctx.saved_tensors
+    b, t, c = f0.shape
+    p = f.shape[-1]
+    g = grad.contiguous().to(torch.float32)
+    with core._on_device_of(f0, f, a, g):
+      if p == 0 or c == 0:
+        d_f0, d_f, d_a = torch.zeros_like(f0), torch.zeros_like(f), torch.zeros_like(a)
+      else:
+        d_f0, d_f, d_a = torch.empty_like(f0), torch.empty_like(f), torch.empty_like(a)
+        _lib.check(_lib.load().ddsp_b200_comb_nll_backward(
+            f0.data_ptr(), f.data_ptr(), a.data_ptr(), g.data_ptr(), d_f0.data_ptr(),
+            d_f.data_ptr(), d_a.data_ptr(), b, t, c, p, ctx.cfg[0], ctx.cfg[1],
+            core._stream()))
+    want = ctx.needs_input_grad
+    return (d_f0 if want[0] else None, d_f if want[1] else None,
+            d_a if want[2] else None, None, None)
 
 
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):

@@ -193,6 +193,11 @@ def logb(x, base=2.0, eps=1e-5):
   return safe_log(x, eps) / den
 
 
+def log10(x, eps=1e-5):
+  """core.log10 (core.py:224-226)."""
+  return logb(x, base=10, eps=eps)
+
+
 def midi_to_hz(notes, midi_zero_silence: bool = False):
   """core.midi_to_hz (core.py:280-297)."""
   notes = _as_f32(notes)
@@ -424,6 +429,20 @@ def remove_above_nyquist(frequency_envelopes, amplitude_envelopes,
   amplitude_envelopes = torch_float32(amplitude_envelopes)
   return torch.where(frequency_envelopes >= sample_rate / 2.0,
                      torch.zeros_like(amplitude_envelopes), amplitude_envelopes)
+
+
+def harmonic_to_sinusoidal(harm_amp, harm_dist, f0_hz, sample_rate=16000):
+  """core.harmonic_to_sinusoidal (core.py:784-794): the harmonic synthesizer's
+  controls as sinusoids, amps [B, T, K] and freqs f0 * [1..K], with the harmonics
+  at or above Nyquist dropped and the rest renormalised.  Frame-rate differentiable
+  torch ops on the inputs' device, like hz_to_midi."""
+  harm_amp, harm_dist, f0_hz = _as_f32(harm_amp), _as_f32(harm_dist), _as_f32(f0_hz)
+  k = int(harm_dist.shape[-1])
+  freqs = f0_hz * torch.linspace(1.0, float(k), k, device=f0_hz.device)[None, None, :]
+  harm_dist = torch.where(freqs >= sample_rate / 2.0, torch.zeros_like(harm_dist),
+                          harm_dist)
+  harm_dist = safe_divide(harm_dist, torch.sum(harm_dist, dim=-1, keepdim=True))
+  return harm_amp * harm_dist, freqs
 
 
 def normalize_harmonics(harmonic_distribution, f0_hz=None, sample_rate=None):

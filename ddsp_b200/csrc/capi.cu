@@ -4,6 +4,9 @@
 #include <stdarg.h>
 
 #include <algorithm>
+#include <cfloat>
+#include <cmath>
+#include <vector>
 
 #include "common.cuh"
 #include "controls.cuh"
@@ -27,6 +30,7 @@
 #include "wavetable.cuh"
 #include "loudness.cuh"
 #include "mel.cuh"
+#include "consistency.cuh"
 
 namespace ddsp {
 
@@ -1950,6 +1954,148 @@ int ddsp_b200_mel_backward(const float* audio, const float* window, const void* 
   dim3 grid((unsigned)((N + own - 1) / own), B);
   kern<<<grid, 32 * warps, smem, (cudaStream_t)stream>>>(p, grad_out, grad_audio, own);
   DDSP_CHECK_LAUNCH("mel_backward");
+  return 0;
+}
+
+// ---- consistency-loss mixture NLLs -------------------------------------------------
+static int cons_rows(const char* name, int B, int T, int64_t* rows) {
+  DDSP_REQUIRE((int64_t)B * T <= INT32_MAX, DDSP_B200_E_INVALID,
+               "%s: B*T=%lld exceeds the 2^31 - 1 grid limit", name, (long long)B * T);
+  *rows = (int64_t)B * T;
+  return 0;
+}
+
+static int mix_check(const char* name, int B, int T, int Q, int J, float scale,
+                     cons_::MixParams* p, int64_t* rows) {
+  DDSP_REQUIRE(B >= 0 && T >= 0 && Q >= 0 && J >= 0, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d T=%d Q=%d J=%d", name, B, T, Q, J);
+  DDSP_REQUIRE(scale > 0.f && scale <= FLT_MAX, DDSP_B200_E_INVALID,
+               "%s: scale must be positive and finite, got %g", name, (double)scale);
+  DDSP_REQUIRE(J <= cons_::kMaxStaged, DDSP_B200_E_UNSUPPORTED,
+               "%s: J=%d components exceed the %d supported", name, J, cons_::kMaxStaged);
+  int rc = cons_rows(name, B, T, rows);
+  if (rc) return rc;
+  p->Q = Q;
+  p->J = J;
+  p->inv_scale = (float)(1.0 / scale);
+  p->log_norm = (float)(std::log((double)scale) + 0.5 * std::log(2.0 * M_PI));
+  return 0;
+}
+
+int ddsp_b200_mixture_nll_forward(const float* x, const float* mu, const float* lw,
+                                  float* nll, int B, int T, int Q, int J, float scale,
+                                  void* stream) {
+  const bool empty = B == 0 || T == 0 || Q == 0 || J == 0;
+  DDSP_REQUIRE(empty || (x && mu && lw && nll), DDSP_B200_E_INVALID,
+               "mixture_nll_forward: null pointer");
+  cons_::MixParams p;
+  int64_t rows = 0;
+  int rc = mix_check("mixture_nll_forward", B, T, Q, J, scale, &p, &rows);
+  if (rc || rows == 0 || Q == 0 || J == 0) return rc;
+  p.x = x; p.mu = mu; p.lw = lw;
+  const size_t smem = sizeof(float) * 2 * (size_t)J;
+  rc = set_smem(cons_::mixture_nll_kernel, smem, "mixture_nll_forward");
+  if (rc) return rc;
+  cons_::mixture_nll_kernel<<<(unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream>>>(
+      p, nll);
+  DDSP_CHECK_LAUNCH("mixture_nll_forward");
+  return 0;
+}
+
+int ddsp_b200_mixture_nll_backward(const float* x, const float* mu, const float* lw,
+                                   const float* grad, float* dx, float* dmu, float* dlw,
+                                   int B, int T, int Q, int J, float scale, void* stream) {
+  const bool empty = B == 0 || T == 0 || Q == 0 || J == 0;
+  DDSP_REQUIRE(empty || (x && mu && lw && grad && dx && dmu && dlw), DDSP_B200_E_INVALID,
+               "mixture_nll_backward: null pointer");
+  cons_::MixParams p;
+  int64_t rows = 0;
+  int rc = mix_check("mixture_nll_backward", B, T, Q, J, scale, &p, &rows);
+  if (rc || rows == 0 || Q == 0 || J == 0) return rc;
+  p.x = x; p.mu = mu; p.lw = lw;
+  const size_t smem = sizeof(float) * (4 * (size_t)J + 5 * cons_::kChunk);
+  rc = set_smem(cons_::mixture_nll_backward_kernel, smem, "mixture_nll_backward");
+  if (rc) return rc;
+  cons_::mixture_nll_backward_kernel<<<(unsigned)rows, cons_::kThreads, smem,
+                                       (cudaStream_t)stream>>>(p, grad, dx, dmu, dlw);
+  DDSP_CHECK_LAUNCH("mixture_nll_backward");
+  return 0;
+}
+
+// Half-width W of the comb window: the smallest W for which the terms |k - k0| > W
+// sum to less than 2^-25 of the largest term, counting each with the weight 1 + |z_k|
+// it carries into d nu / dq.  With k0 the nearest integer, |q - k0| <= 1/2 inside
+// [1/2, G + 1/2], so term n = |k - k0| is at most exp(-n (n - 1) / (2 s^2)) of the
+// largest (outside, every term is further: at most exp(-n^2 / (2 s^2))), twice for the
+// two sides, and |z_k| <= (n + 1/2) / s.
+static int comb_window(int G, double scale) {
+  std::vector<double> tail(G + 2, 0.0);
+  for (int n = G; n >= 1; --n)
+    tail[n] = tail[n + 1] +
+              2.0 * (1.0 + (n + 0.5) / scale) * std::exp(-0.5 * n * (n - 1.0) / (scale * scale));
+  int W = 0;
+  while (W < G && tail[W + 1] >= std::ldexp(1.0, -25)) ++W;
+  return W;
+}
+
+static int comb_check(const char* name, int B, int T, int C, int P, int G, float scale,
+                      cons_::CombParams* p, int64_t* rows) {
+  DDSP_REQUIRE(B >= 0 && T >= 0 && C >= 0 && P >= 0 && G >= 1, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d T=%d C=%d P=%d G=%d", name, B, T, C, P, G);
+  DDSP_REQUIRE(scale > 0.f && scale <= FLT_MAX, DDSP_B200_E_INVALID,
+               "%s: scale must be positive and finite, got %g", name, (double)scale);
+  DDSP_REQUIRE(C <= cons_::kMaxStaged && P <= cons_::kMaxStaged, DDSP_B200_E_UNSUPPORTED,
+               "%s: C=%d candidates or P=%d points exceed the %d supported", name, C, P,
+               cons_::kMaxStaged);
+  int rc = cons_rows(name, B, T, rows);
+  if (rc) return rc;
+  p->C = C;
+  p->P = P;
+  p->G = G;
+  p->inv_scale = (float)(1.0 / scale);
+  p->log_norm = (float)(std::log((double)G) + std::log((double)scale) +
+                        0.5 * std::log(2.0 * M_PI));
+  if (*rows && C && P) p->W = comb_window(G, scale);
+  return 0;
+}
+
+int ddsp_b200_comb_nll_forward(const float* f0, const float* f, const float* a, float* out,
+                               int B, int T, int C, int P, int G, float scale, void* stream) {
+  const bool empty = B == 0 || T == 0 || C == 0 || P == 0;
+  DDSP_REQUIRE(empty || (f0 && f && a && out), DDSP_B200_E_INVALID,
+               "comb_nll_forward: null pointer");
+  cons_::CombParams p;
+  int64_t rows = 0;
+  int rc = comb_check("comb_nll_forward", B, T, C, P, G, scale, &p, &rows);
+  if (rc || rows == 0 || C == 0 || P == 0) return rc;
+  p.f0 = f0; p.f = f; p.a = a;
+  const size_t smem = sizeof(float) * (2 * (size_t)P + C + 1);
+  rc = set_smem(cons_::comb_nll_kernel, smem, "comb_nll_forward");
+  if (rc) return rc;
+  cons_::comb_nll_kernel<<<(unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream>>>(
+      p, out);
+  DDSP_CHECK_LAUNCH("comb_nll_forward");
+  return 0;
+}
+
+int ddsp_b200_comb_nll_backward(const float* f0, const float* f, const float* a,
+                                const float* grad, float* d_f0, float* d_f, float* d_a,
+                                int B, int T, int C, int P, int G, float scale,
+                                void* stream) {
+  const bool empty = B == 0 || T == 0 || C == 0 || P == 0;
+  DDSP_REQUIRE(empty || (f0 && f && a && grad && d_f0 && d_f && d_a), DDSP_B200_E_INVALID,
+               "comb_nll_backward: null pointer");
+  cons_::CombParams p;
+  int64_t rows = 0;
+  int rc = comb_check("comb_nll_backward", B, T, C, P, G, scale, &p, &rows);
+  if (rc || rows == 0 || C == 0 || P == 0) return rc;
+  p.f0 = f0; p.f = f; p.a = a;
+  const size_t smem = sizeof(float) * (2 * (size_t)P + 3 * (size_t)C + 1);
+  rc = set_smem(cons_::comb_nll_backward_kernel, smem, "comb_nll_backward");
+  if (rc) return rc;
+  cons_::comb_nll_backward_kernel<<<(unsigned)rows, cons_::kThreads, smem,
+                                    (cudaStream_t)stream>>>(p, grad, d_f0, d_f, d_a);
+  DDSP_CHECK_LAUNCH("comb_nll_backward");
   return 0;
 }
 

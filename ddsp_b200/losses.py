@@ -1,10 +1,19 @@
-"""Multi-scale spectral loss with the reference's constructor and semantics
-(`ddsp/losses.py:102-243`), in torch (cuFFT on the GPU)."""
+"""Losses with the reference's constructors and semantics (`ddsp/losses.py`): the
+multi-scale spectral loss (`losses.py:102-243`, torch with cuFFT on the GPU) and the
+consistency losses of the self-supervised pitch model (`losses.py:489-1076`).  The
+Gaussian mixtures of `KDEConsistencyLoss` and `TWMLoss` are evaluated per frame by
+the CUDA kernels of `csrc/consistency.cuh` (`autograd.MixtureNLLFn`, `CombNLLFn`);
+the [B, T, K]-sized elementwise work around them is torch autograd."""
 import functools
+import math
+import re
 
 import torch
 
+from ddsp_b200 import autograd
+from ddsp_b200 import core
 from ddsp_b200 import spectral_ops
+from ddsp_b200.core import hz_to_midi, safe_divide
 
 
 def mean_difference(target, value, loss_type='L1', weights=None):
@@ -22,6 +31,26 @@ def mean_difference(target, value, loss_type='L1', weights=None):
   else:
     raise ValueError('Loss type ({}), must be '
                      '"L1", "L2", or "COSINE"'.format(loss_type))
+
+
+def _snake_case(name):
+  """A Keras layer's default name: its class name in snake case."""
+  name = re.sub(r'(.)([A-Z][a-z]+)', r'\1_\2', name)
+  return re.sub(r'([a-z])([A-Z])', r'\1_\2', name).lower()
+
+
+class Loss:
+  """losses.Loss (losses.py:41-47): a callable with a `name`; `get_losses_dict`
+  returns {name: call(...)}."""
+
+  def __init__(self, name=None):
+    self.name = name if name is not None else _snake_case(type(self).__name__)
+
+  def __call__(self, *args, **kwargs):
+    return self.call(*args, **kwargs)
+
+  def get_losses_dict(self, *args, **kwargs):
+    return {self.name: self(*args, **kwargs)}
 
 
 class SpectralLoss:
@@ -116,3 +145,259 @@ class SpectralLoss:
             spectral_ops.safe_log(target_mag), spectral_ops.safe_log(value_mag),
             self.loss_type, weights=weights)
     return loss
+
+
+# ------------------------------------------------------------------------------
+# Consistency losses (losses.py:489-578, 689-1076)
+# ------------------------------------------------------------------------------
+def amp_loss(amp, amp_target, loss_type='L1', weights=None, log=False, amin=1e-5):
+  """losses.amp_loss (losses.py:492-504): optionally on a log10 scale."""
+  amp = core.torch_float32(amp)
+  amp_target = core.torch_float32(amp_target)
+  if log:
+    amp = core.log10(torch.clamp(amp, min=amin))
+    amp_target = core.log10(torch.clamp(amp_target, min=amin))
+  return mean_difference(amp, amp_target, loss_type, weights)
+
+
+def freq_loss(f_hz, f_hz_target, loss_type='L1', weights=None):
+  """losses.freq_loss (losses.py:507-513): compared in MIDI."""
+  f_midi = hz_to_midi(core.torch_float32(f_hz))
+  f_midi_target = hz_to_midi(core.torch_float32(f_hz_target))
+  return mean_difference(f_midi, f_midi_target, loss_type, weights)
+
+
+class FilteredNoiseConsistencyLoss(Loss):
+  """losses.FilteredNoiseConsistencyLoss (losses.py:516-530)."""
+
+  def __init__(self, weight=1.0, name=None):
+    super().__init__(name)
+    self.weight = weight
+
+  def call(self, noise_magnitudes, noise_magnitudes_target):
+    return self.weight * amp_loss(noise_magnitudes, noise_magnitudes_target)
+
+
+class HarmonicConsistencyLoss(Loss):
+  """losses.HarmonicConsistencyLoss (losses.py:533-578): a dict of three losses,
+  the distribution and f0 terms masked where the target amplitude is below
+  `amp_threshold`."""
+
+  def __init__(self, amp_weight=1.0, dist_weight=1.0, f0_weight=1.0, amp_threshold=1e-4,
+               name=None):
+    super().__init__(name)
+    self.amp_weight = amp_weight
+    self.dist_weight = dist_weight
+    self.f0_weight = f0_weight
+    self.amp_threshold = amp_threshold
+
+  def call(self, harm_amp, harm_amp_target, harm_dist, harm_dist_target, f0_hz,
+           f0_hz_target):
+    harm_amp_target = core.torch_float32(harm_amp_target)
+    weights = (harm_amp_target >= self.amp_threshold).to(torch.float32)
+    return {
+        'harm_amp_loss': self.amp_weight * amp_loss(harm_amp, harm_amp_target),
+        'harm_dist_loss': self.dist_weight * amp_loss(harm_dist, harm_dist_target,
+                                                      weights=weights),
+        'f0_hz_loss': self.f0_weight * freq_loss(f0_hz, f0_hz_target, weights=weights),
+    }
+
+
+class ParamLoss(Loss):
+  """losses.ParamLoss (losses.py:1064-1076)."""
+
+  def __init__(self, weight=1.0, loss_type='L1', name=None):
+    super().__init__(name)
+    self.weight = weight
+    self.loss_type = loss_type
+
+  def call(self, pred, target, weights=None):
+    loss = mean_difference(core.torch_float32(pred), core.torch_float32(target),
+                           self.loss_type, weights)
+    return self.weight * loss
+
+
+def _check_sinusoids(name, pairs):
+  """Shape checks made before any device work: each (label, amps, freqs) pair is
+  [batch, time, n] with amps and freqs alike, and all share batch and time."""
+  frames = None
+  for label, a, f in pairs:
+    sa, sf = core._shape(a), core._shape(f)
+    if len(sa) != 3 or sa != sf:
+      raise ValueError(f'{name}: {label} must be two [batch, time, n] arrays of one '
+                       f'shape, got {sa} and {sf}')
+    if frames is not None and sa[:2] != frames:
+      raise ValueError(f'{name}: {label} has [batch, time] {sa[:2]}, the other inputs '
+                       f'{frames}')
+    frames = sa[:2]
+
+
+def _check_scale(name, label, scale):
+  if not (scale > 0.0 and math.isfinite(scale)):
+    raise ValueError(f'{name}: {label} must be positive and finite, got {scale}')
+
+
+def _log_weights(amps):
+  """The mixture weights of `Categorical(probs=amps_norm)` as MixtureSameFamily uses
+  them, log_softmax(log p), with exact zeros raised to 1e-7 before normalising
+  (losses.py:807-813, 1044-1051)."""
+  amps = torch.where(amps == 0.0, torch.full_like(amps, 1e-7), amps)
+  probs = safe_divide(amps, torch.sum(amps, dim=-1, keepdim=True))
+  return torch.log_softmax(torch.log(probs), dim=-1)
+
+
+class KDEConsistencyLoss(Loss):
+  """losses.KDEConsistencyLoss (losses.py:689-813): -log p(a | b) and -log p(b | a)
+  under Gaussian kernel density estimates in MIDI, plus the mean-amplitude match.
+  Each direction is one `autograd.MixtureNLLFn` launch forward and one backward;
+  gradients reach all four inputs."""
+
+  def __init__(self, weight_a=1.0, weight_b=1.0, weight_mean_amp=1.0, scale_a=0.1,
+               scale_b=0.1, name=None):
+    super().__init__(name)
+    self.weight_a = weight_a
+    self.weight_b = weight_b
+    self.weight_mean_amp = weight_mean_amp
+    self.scale_a = scale_a
+    self.scale_b = scale_b
+
+  def call(self, amps_a, freqs_a, amps_b, freqs_b):
+    """Scalar: weighted -log p(a|b) - log p(b|a) + the mean-amplitude L1."""
+    _check_sinusoids('KDEConsistencyLoss', [('amps_a, freqs_a', amps_a, freqs_a),
+                                            ('amps_b, freqs_b', amps_b, freqs_b)])
+    if self.weight_a > 0.0:
+      _check_scale('KDEConsistencyLoss', 'scale_b', self.scale_b)
+    if self.weight_b > 0.0:
+      _check_scale('KDEConsistencyLoss', 'scale_a', self.scale_a)
+    amps_a, freqs_a, amps_b, freqs_b = (
+        core.torch_float32(x) for x in (amps_a, freqs_a, amps_b, freqs_b))
+    loss = 0.0
+    if self.weight_a > 0.0:
+      loss_a = self.nll(amps_a, freqs_a, amps_b, freqs_b, self.scale_b)
+      loss = loss + torch.mean(self.weight_a * loss_a)
+    if self.weight_b > 0.0:
+      loss_b = self.nll(amps_b, freqs_b, amps_a, freqs_a, self.scale_a)
+      loss = loss + torch.mean(self.weight_b * loss_b)
+    if self.weight_mean_amp > 0.0:
+      mean_amp_a = torch.mean(amps_a, dim=-1)
+      mean_amp_b = torch.mean(amps_b, dim=-1)
+      loss = loss + self.weight_mean_amp * torch.mean(torch.abs(mean_amp_a - mean_amp_b))
+    return loss
+
+  def nll(self, amps, freqs, amps_target, freqs_target, scale_target):
+    """-log p(source | target), the amplitude-weighted mean over the source
+    sinusoids, [batch, time]."""
+    _check_sinusoids('KDEConsistencyLoss.nll',
+                     [('amps, freqs', amps, freqs),
+                      ('amps_target, freqs_target', amps_target, freqs_target)])
+    _check_scale('KDEConsistencyLoss.nll', 'scale_target', scale_target)
+    amps, freqs, amps_target, freqs_target = (
+        core.torch_float32(x) for x in (amps, freqs, amps_target, freqs_target))
+    nll = autograd.MixtureNLLFn.apply(hz_to_midi(freqs), hz_to_midi(freqs_target),
+                                      _log_weights(amps_target), scale_target)
+    amps_norm = safe_divide(amps, torch.sum(amps, dim=-1, keepdim=True))
+    return torch.mean(nll * amps_norm, dim=-1)
+
+
+class TWMLoss(Loss):
+  """losses.TWMLoss (losses.py:819-1061), the differentiable two-way mismatch.
+
+  -log p(sinusoids | harmonics) is the comb of `n_harmonic_gaussians` Gaussians of
+  width `harmonics_scale` at the harmonic numbers, on f / f0 (`autograd.CombNLLFn`);
+  -log p(harmonics | sinusoids) is the kernel density estimate of width
+  `sinusoids_scale` around the sinusoids in MIDI, at each candidate's first
+  `n_harmonic_points` harmonics (`autograd.MixtureNLLFn`).  (The reference's
+  constructor comments pair the scales the other way round; its code, followed
+  here, pairs them so.)  Gradients reach f0_candidates, freqs and amps."""
+
+  def __init__(self, sinusoids_weight=1.0, harmonics_weight=1.0, sinusoids_scale=0.5,
+               harmonics_scale=0.2, n_harmonic_points=10, n_harmonic_gaussians=30,
+               softmin_temperature=1.0, sample_rate=16000, name=None):
+    super().__init__(name)
+    self.softmin_temperature = softmin_temperature
+    self.sample_rate = sample_rate
+    self.sinusoids_weight = sinusoids_weight
+    self.harmonics_weight = harmonics_weight
+    self.sinusoids_scale = sinusoids_scale
+    self.n_harmonic_points = n_harmonic_points
+    self.harmonics_scale = harmonics_scale
+    self.n_harmonic_gaussians = n_harmonic_gaussians
+
+  def call(self, f0_candidates, freqs, amps):
+    """Scalar: the softmin over candidates of the weighted two terms."""
+    sinusoids_loss, harmonics_loss = self.get_loss_tensors(f0_candidates, freqs, amps)
+    combined_loss = (self.sinusoids_weight * sinusoids_loss +
+                     self.harmonics_weight * harmonics_loss)
+    softmin_loss = combined_loss * torch.softmax(
+        -combined_loss / self.softmin_temperature, dim=-1)
+    return torch.mean(softmin_loss)
+
+  def predict_f0(self, f0_candidates, freqs, amps):
+    """The candidate of least combined loss per frame, [batch, time, 1], on the
+    inputs' device.  NaN losses are skipped and ties go to the first index, as with
+    np.nanargmin; a frame whose losses are all NaN raises ValueError as it does."""
+    with torch.no_grad():
+      sinusoids_loss, harmonics_loss = self.get_loss_tensors(f0_candidates, freqs, amps)
+      loss = (self.sinusoids_weight * sinusoids_loss +
+              self.harmonics_weight * harmonics_loss)
+      nan = torch.isnan(loss)
+      if bool(torch.any(torch.all(nan, dim=-1))):
+        raise ValueError('All-NaN slice encountered')
+      idx = torch.argmin(torch.where(nan, torch.full_like(loss, math.inf), loss), dim=-1)
+      # a frame whose least loss is +inf: the first +inf, not a skipped NaN before it
+      first_inf = torch.argmax((loss == math.inf).to(torch.int32), dim=-1)
+      least = torch.gather(loss, -1, idx[..., None])[..., 0]
+      idx = torch.where(least == math.inf, first_inf, idx)
+      return torch.gather(core.torch_float32(f0_candidates), -1, idx[..., None])
+
+  def _check(self, f0_candidates, freqs, amps):
+    _check_sinusoids('TWMLoss', [('amps, freqs', amps, freqs)])
+    sc = core._shape(f0_candidates)
+    if len(sc) != 3 or sc[:2] != core._shape(freqs)[:2]:
+      raise ValueError(f'TWMLoss: f0_candidates must be [batch, time, candidates] with '
+                       f'the [batch, time] of freqs {core._shape(freqs)[:2]}, got {sc}')
+    if int(self.n_harmonic_points) < 1 or int(self.n_harmonic_gaussians) < 1:
+      raise ValueError('TWMLoss: n_harmonic_points (%s) and n_harmonic_gaussians (%s) '
+                       'must be at least 1' % (self.n_harmonic_points,
+                                               self.n_harmonic_gaussians))
+    _check_scale('TWMLoss', 'sinusoids_scale', self.sinusoids_scale)
+    _check_scale('TWMLoss', 'harmonics_scale', self.harmonics_scale)
+
+  def get_loss_tensors(self, f0_candidates, freqs, amps):
+    """-log p(sinusoids | harmonics) and -log p(harmonics | sinusoids), each
+    [batch, time, candidate]."""
+    self._check(f0_candidates, freqs, amps)
+    f0_candidates, freqs, amps = (
+        core.torch_float32(x) for x in (f0_candidates, freqs, amps))
+    sinusoids_loss = autograd.CombNLLFn.apply(
+        f0_candidates, freqs, amps, int(self.n_harmonic_gaussians),
+        float(self.harmonics_scale))
+
+    harmonics = self.get_candidate_harmonics(f0_candidates, as_midi=True)
+    b, t, c, n = harmonics.shape
+    nll = autograd.MixtureNLLFn.apply(
+        harmonics.reshape(b, t, c * n), hz_to_midi(freqs), _log_weights(amps),
+        float(self.sinusoids_scale)).reshape(b, t, c, n)
+    with torch.no_grad():
+      # the prior on upper harmonics and the Nyquist mask, reweighted by the
+      # number of harmonics below Nyquist: constants of the graph
+      amps_prior = torch.linspace(1.0, 1.0 / n, n, device=harmonics.device)
+      nyquist_mask = (harmonics < hz_to_midi(self.sample_rate / 2.0)).to(torch.float32)
+      weights = amps_prior * safe_divide(
+          nyquist_mask, torch.mean(nyquist_mask, dim=-1, keepdim=True))
+    harmonics_loss = torch.mean(nll * weights, dim=-1)
+    return sinusoids_loss, harmonics_loss
+
+  def get_candidate_harmonics(self, f0_candidates, as_midi=True):
+    """The harmonic series f0 * [1..n_harmonic_points] of each candidate,
+    [batch, time, candidate, harmonic], in MIDI or in hertz.  In MIDI it is formed
+    as hz_to_midi(f0) + 12 log2(n) (0 where f0 <= 0, as hz_to_midi(f0 n) gives),
+    which keeps one [batch, time, candidate, harmonic] tensor in the graph instead
+    of hz_to_midi's chain of them."""
+    f0_candidates = core.torch_float32(f0_candidates)
+    n = torch.arange(1, int(self.n_harmonic_points) + 1, dtype=torch.float32,
+                     device=f0_candidates.device)
+    if not as_midi:
+      return f0_candidates[..., None] * n
+    midi = hz_to_midi(f0_candidates)[..., None] + 12.0 * torch.log2(n)
+    return torch.where(f0_candidates[..., None] <= 0.0, torch.zeros_like(midi), midi)

@@ -548,6 +548,46 @@ int ddsp_b200_mel_backward(const float* audio, const float* window, const void* 
                            int n_frames, int fft_size, int fft_length, int hop, int pad_end,
                            int bins, int n_out, int mode, void* stream);
 
+/* Mixture NLL of the consistency losses (losses.KDEConsistencyLoss.nll and
+ * TWMLoss's p(harmonics | sinusoids), losses.py:759-813, 982-990): per frame (b, t),
+ *   nll[b,t,q] = -logsumexp_j(lw[b,t,j] - ((x[b,t,q] - mu[b,t,j]) / scale)^2 / 2)
+ *                + log(scale) + log(2 pi) / 2
+ * for x [B,T,Q], mu and lw [B,T,J] (lw: log-weights, normalised by the caller), the
+ * logsumexp shifted by its largest term.  1 <= J <= 4096 is staged per frame; J > 4096
+ * is E_UNSUPPORTED.  Q is unbounded.  scale must be positive and finite.  B*T <=
+ * 2^31 - 1.  B, T, Q or J = 0 return before any launch and write nothing; the
+ * pointers may then be null.
+ * backward: for g [B,T,Q], with responsibilities r_qj and z_qj = (x_q - mu_j) / scale,
+ *   dx = g_q / scale sum_j r_qj z_qj, dmu = -1/scale sum_q g_q r_qj z_qj,
+ *   dlw = -sum_q g_q r_qj;
+ * every sum in a fixed order, no atomics: bit-reproducible. */
+int ddsp_b200_mixture_nll_forward(const float* x, const float* mu, const float* lw,
+                                  float* nll, int B, int T, int Q, int J, float scale,
+                                  void* stream);
+int ddsp_b200_mixture_nll_backward(const float* x, const float* mu, const float* lw,
+                                   const float* grad, float* dx, float* dmu, float* dlw,
+                                   int B, int T, int Q, int J, float scale, void* stream);
+
+/* Harmonic-comb NLL of TWMLoss's p(sinusoids | harmonics), amplitude-reduced
+ * (losses.py:956-977): for candidates f0 [B,T,C], points f and amplitudes a [B,T,P],
+ *   out[b,t,c] = safe_divide(sum_p a_p nu(safe_divide(f_p, f0_c)), sum_p a_p),
+ *   nu(q) = -logsumexp_{k=1..G}(-log G - ((q - k) / scale)^2 / 2) + log(scale)
+ *           + log(2 pi) / 2,
+ * safe_divide's zero denominators being the constant 1e-7.  Only the comb terms within
+ * a window around the nearest k are summed, its half-width chosen from scale and G so
+ * that the omitted terms stay below 2^-25 of the sum.  1 <= C, P <= 4096 (more is
+ * E_UNSUPPORTED), G >= 1, scale positive and finite, B*T <= 2^31 - 1.  B, T, C or P = 0
+ * return before any launch and write nothing; the pointers may then be null.
+ * backward: d_f0 [B,T,C], d_f and d_a [B,T,P] for g [B,T,C]; no gradient through a
+ * safe_divide denominator that was 0 (d_f0 = 0 at f0 = 0).  Fixed-order sums, no
+ * atomics: bit-reproducible. */
+int ddsp_b200_comb_nll_forward(const float* f0, const float* f, const float* a, float* out,
+                               int B, int T, int C, int P, int G, float scale, void* stream);
+int ddsp_b200_comb_nll_backward(const float* f0, const float* f, const float* a,
+                                const float* grad, float* d_f0, float* d_f, float* d_a,
+                                int B, int T, int C, int P, int G, float scale,
+                                void* stream);
+
 #ifdef __cplusplus
 }
 #endif
