@@ -88,6 +88,14 @@ SIGNATURES = {
         (_sz, [_i, _i, _i, _i, _i, _i, _i]),
     'ddsp_b200_frequency_filter_backward':
         (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+    'ddsp_b200_sinc_impulse_response': (_i, [_vp, _vp, _i64, _i, _f, _i, _vp]),
+    'ddsp_b200_sinc_impulse_response_backward':
+        (_i, [_vp, _vp, _vp, _i64, _i, _f, _i, _vp]),
+    'ddsp_b200_sinc_filter':
+        (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _i, _i, _vp]),
+    'ddsp_b200_sinc_filter_backward_workspace': (_sz, [_i, _i, _i, _i, _i]),
+    'ddsp_b200_sinc_filter_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _i, _vp, _sz, _vp]),
     'ddsp_b200_oscillator_bank_workspace': (_sz, [_i, _i, _i]),
     'ddsp_b200_oscillator_bank':
         (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _i, _vp, _sz, _vp]),

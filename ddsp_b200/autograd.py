@@ -27,6 +27,9 @@ kernels, exposed as `torch.autograd.Function`s:
     short reverbs), the impulse-response synthesis and their composition, routed to
     by `core.fft_convolve` / `core.frequency_impulse_response` /
     `core.frequency_filter` under grad;
+  * `SincImpulseResponseFn` / `SincFilterFn` - core.sinc_impulse_response and the
+    fused core.sinc_filter, differentiable in the cutoff (and the audio); the taps
+    are rebuilt on chip in the backward, never stored;
   * `MixtureNLLFn` / `CombNLLFn` - the Gaussian-mixture NLLs of the consistency
     losses (`losses.KDEConsistencyLoss`, `losses.TWMLoss`), evaluated per frame
     on-chip with gradients to every input;
@@ -314,6 +317,64 @@ class FrequencyFilterFn(torch.autograd.Function):
           core._ptr(d_mags), b, f, nb, n, mb, window_size, pad, core._ptr(ws), nbytes,
           core._stream()))
     return d_audio, d_mags, None, None
+
+
+class SincImpulseResponseFn(torch.autograd.Function):
+  """core.sinc_impulse_response, differentiable in the cutoff:
+  `ddsp_b200_sinc_impulse_response_backward` recomputes each frame's taps and their
+  derivative on chip (csrc/sinc.cuh)."""
+
+  @staticmethod
+  def forward(ctx, cutoff, s, shape, scale, high_pass):
+    ctx.save_for_backward(cutoff)
+    ctx.cfg = (s, scale, high_pass)
+    return core.sinc_impulse_response_forward(cutoff, s, shape, scale, high_pass)
+
+  @staticmethod
+  def backward(ctx, d_ir):
+    cutoff, = ctx.saved_tensors
+    s, scale, high_pass = ctx.cfg
+    d_ir = d_ir.contiguous().to(torch.float32)
+    with core._on_device_of(cutoff, d_ir):
+      d_cutoff = torch.empty_like(cutoff)
+      _lib.check(_lib.load().ddsp_b200_sinc_impulse_response_backward(
+          cutoff.data_ptr(), d_ir.data_ptr(), d_cutoff.data_ptr(), cutoff.numel(), s,
+          scale, int(high_pass), core._stream()))
+    return d_cutoff, None, None, None, None
+
+
+class SincFilterFn(torch.autograd.Function):
+  """core.sinc_filter on the fused route (fewer than FFT_CONVOLVE_MIN_IR taps),
+  differentiable in audio and cutoff.  Nothing but the inputs is saved: one call of
+  `ddsp_b200_sinc_filter_backward` rebuilds each frame's taps and computes the
+  gradients asked for."""
+
+  @staticmethod
+  def forward(ctx, audio, cutoff, s, scale, high_pass, padding, cutoff_batch, n_frames):
+    ctx.save_for_backward(audio, cutoff)
+    ctx.cfg = (s, scale, high_pass, padding, cutoff_batch, n_frames)
+    return core.sinc_filter_forward(audio, cutoff, s, scale, high_pass, padding,
+                                    cutoff_batch, n_frames)
+
+  @staticmethod
+  def backward(ctx, g):
+    audio, cutoff = ctx.saved_tensors
+    s, scale, high_pass, padding, cutoff_batch, n_frames = ctx.cfg
+    b, n = audio.shape
+    g = g.contiguous().to(torch.float32)
+    lib = _lib.load()
+    with core._on_device_of(audio, cutoff, g):
+      d_audio = torch.empty_like(audio) if ctx.needs_input_grad[0] else None
+      d_cutoff = torch.empty_like(cutoff) if ctx.needs_input_grad[1] else None
+      nbytes = (lib.ddsp_b200_sinc_filter_backward_workspace(b, n, n_frames, s, cutoff_batch)
+                if d_cutoff is not None else 0)
+      ws = core._workspace(nbytes, audio.device)
+      _lib.check(lib.ddsp_b200_sinc_filter_backward(
+          audio.data_ptr(), cutoff.data_ptr(), g.data_ptr(), core._ptr(d_audio),
+          core._ptr(d_cutoff), b, n, n_frames, s, cutoff_batch, scale, int(high_pass),
+          _lib.PAD_SAME if padding == 'same' else _lib.PAD_VALID, core._ptr(ws), nbytes,
+          core._stream()))
+    return d_audio, d_cutoff, None, None, None, None, None, None
 
 
 class FilteredNoiseFn(torch.autograd.Function):

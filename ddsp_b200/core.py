@@ -1080,6 +1080,101 @@ def frequency_filter(audio, magnitudes, window_size: int = 0,
 
 
 # ----------------------------------------------------------------------------
+# Windowed-sinc filters (core.py:1568-1625, 1658-1690)
+# ----------------------------------------------------------------------------
+def sinc(x, threshold=1e-20):
+  """core.sinc (core.py:1568-1573): sin(pi x) / (pi x), with |x| < threshold
+  replaced by threshold.  Elementwise torch on whatever device x lives on."""
+  x = _as_f32(x)
+  x = torch.where(torch.abs(x) < threshold, torch.full_like(x, threshold), x)
+  x = np.pi * x
+  return torch.sin(x) / x
+
+
+def _sinc_geometry(cutoff_shape, window_size, sample_rate):
+  """Taps, impulse-response shape and cutoff scale of sinc_impulse_response
+  (core.py:1576-1625), from static shapes only.  The response has the broadcast
+  shape of cutoff [..., 1] and [1, 1, S]: a scalar gives [1, 1, S], [B, F, 1] gives
+  [B, F, S] and [F, 1] gives one shared response of F frames, [1, F, S]."""
+  if isinstance(window_size, bool) or int(window_size) != window_size or window_size < 0:
+    raise ValueError(f'window_size must be a non-negative integer, got {window_size}.')
+  if len(cutoff_shape) and cutoff_shape[-1] != 1:
+    raise ValueError('cutoff_frequency must have a last axis of size 1 ([batch, '
+                     f'n_frames, 1]); got shape {tuple(cutoff_shape)}.')
+  s = 2 * (int(window_size) // 2) + 1
+  lead = tuple(cutoff_shape[:-1]) if len(cutoff_shape) else ()
+  shape = (1,) * max(0, 2 - len(lead)) + lead + (s,)
+  # the reference scales with `*=` in float32; here the caller's array is left alone.
+  # As there, a rate of 0 raises ZeroDivisionError and a negative one is accepted
+  # (sinc is even, so it gives the positive rate's response and gradient).
+  scale = 1.0 if sample_rate is None else float(np.float32(2.0 / float(sample_rate)))
+  return s, shape, scale
+
+
+def sinc_impulse_response_forward(cutoff, s, shape, scale, high_pass):
+  """`ddsp_b200_sinc_impulse_response` on a float32 CUDA cutoff -> [shape] taps."""
+  ir = torch.empty(shape, dtype=torch.float32, device=cutoff.device)
+  with _on_device_of(cutoff):
+    _lib.check(_lib.load().ddsp_b200_sinc_impulse_response(
+        _ptr(cutoff), _ptr(ir), cutoff.numel(), s, scale, int(bool(high_pass)), _stream()))
+  return ir
+
+
+def sinc_impulse_response(cutoff_frequency, window_size: int = 512,
+                          sample_rate: Optional[int] = None, high_pass: bool = False):
+  """core.sinc_impulse_response (core.py:1576-1625): Hamming-windowed sinc low-pass
+  (or, with high_pass, its complement) of 2 (window_size // 2) + 1 taps, normalised to
+  unit DC gain.  Routes to `autograd.SincImpulseResponseFn` when grad is enabled and the
+  cutoff requires it."""
+  s, shape, scale = _sinc_geometry(_shape(cutoff_frequency), window_size, sample_rate)
+  cutoff = torch_float32(cutoff_frequency)
+  if _requires_grad(cutoff):
+    from ddsp_b200 import autograd as _ag
+    return _ag.SincImpulseResponseFn.apply(cutoff, s, shape, scale, bool(high_pass))
+  return sinc_impulse_response_forward(cutoff, s, shape, scale, high_pass)
+
+
+def sinc_filter_forward(audio, cutoff, s, scale, high_pass, padding, cutoff_batch, n_frames):
+  """`ddsp_b200_sinc_filter` on float32 CUDA audio [B, N] and cutoff
+  [cutoff_batch * n_frames] -> [B, N] ('same') or [B, N + S - 1] ('valid')."""
+  b, n = audio.shape
+  out_len = n if padding == 'same' else n + s - 1
+  out = torch.empty((b, out_len), dtype=torch.float32, device=audio.device)
+  with _on_device_of(audio, cutoff):
+    _lib.check(_lib.load().ddsp_b200_sinc_filter(
+        _ptr(audio), _ptr(cutoff), _ptr(out), b, n, n_frames, s, cutoff_batch, scale,
+        int(bool(high_pass)), _lib.PAD_SAME if padding == 'same' else _lib.PAD_VALID, 0,
+        _stream()))
+  return out
+
+
+def sinc_filter(audio, cutoff_frequency, window_size: int = 512,
+                sample_rate: Optional[int] = None, padding: Text = 'same',
+                high_pass: bool = False):
+  """core.sinc_filter (core.py:1658-1690): audio [B, N] through the sinc filters of
+  cutoff_frequency [B or 1, F, 1] (or a scalar, or [F, 1]), with fft_convolve's framing
+  and delay compensation.  Under FFT_CONVOLVE_MIN_IR taps, and where the reference's
+  crop is not empty, the fused kernels build the taps on chip (under grad through
+  `autograd.SincFilterFn`); otherwise sinc_impulse_response feeds fft_convolve."""
+  s, ir_shape, scale = _sinc_geometry(_shape(cutoff_frequency), window_size, sample_rate)
+  _, _, si, _, _, _, out_len, crop_size = _fft_convolve_geometry(
+      _shape(audio), ir_shape, padding, -1)
+  if s < FFT_CONVOLVE_MIN_IR and out_len == crop_size:
+    cutoff_batch, n_frames = si[0], si[1]
+    audio = torch_float32(audio)
+    cutoff = torch_float32(cutoff_frequency)
+    if _requires_grad(audio, cutoff):
+      from ddsp_b200 import autograd as _ag
+      return _ag.SincFilterFn.apply(audio, cutoff, s, scale, bool(high_pass), padding,
+                                    cutoff_batch, n_frames)
+    return sinc_filter_forward(audio, cutoff, s, scale, high_pass, padding, cutoff_batch,
+                               n_frames)
+  impulse_response = sinc_impulse_response(cutoff_frequency, window_size=window_size,
+                                            sample_rate=sample_rate, high_pass=high_pass)
+  return fft_convolve(audio, impulse_response, padding=padding)
+
+
+# ----------------------------------------------------------------------------
 # Modulated delay (core.py:1168-1214, 1285-1314; effects.py:328-394)
 # ----------------------------------------------------------------------------
 def _per_sample_shape(x, batch_size, n_samples, name):

@@ -31,6 +31,7 @@
 #include "loudness.cuh"
 #include "mel.cuh"
 #include "consistency.cuh"
+#include "sinc.cuh"
 
 namespace ddsp {
 
@@ -989,6 +990,154 @@ int ddsp_b200_frequency_filter_backward(const float* audio, const float* ir,
   if (rc) return rc;
   return ddsp_b200_frequency_impulse_response_backward(d_ir, d_mags, (int64_t)mags_batch * F,
                                                        nb, window_size, stream);
+}
+
+// ---- windowed-sinc filters (csrc/sinc.cuh) --------------------------------------------
+int ddsp_b200_sinc_impulse_response(const float* cutoff, float* ir, int64_t BF, int S,
+                                    float scale, int high_pass, void* stream) {
+  const char* name = "sinc_impulse_response";
+  DDSP_REQUIRE(cutoff && ir, DDSP_B200_E_INVALID, "%s: null pointer", name);
+  DDSP_REQUIRE(BF >= 0 && S >= 1 && (S & 1), DDSP_B200_E_INVALID,
+               "%s: bad shape BF=%lld S=%d (S must be odd)", name, (long long)BF, S);
+  DDSP_REQUIRE(BF < (1ll << 31), DDSP_B200_E_INVALID, "%s: too many frames", name);
+  if (BF == 0) return 0;
+  sinc_ir_kernel<<<(unsigned)BF, kSincThreads, 0, (cudaStream_t)stream>>>(cutoff, ir, S, scale,
+                                                                          high_pass);
+  DDSP_CHECK_LAUNCH(name);
+  return 0;
+}
+
+int ddsp_b200_sinc_impulse_response_backward(const float* cutoff, const float* d_ir,
+                                             float* d_cutoff, int64_t BF, int S, float scale,
+                                             int high_pass, void* stream) {
+  const char* name = "sinc_impulse_response_backward";
+  DDSP_REQUIRE(cutoff && d_ir && d_cutoff, DDSP_B200_E_INVALID, "%s: null pointer", name);
+  DDSP_REQUIRE(BF >= 0 && S >= 1 && (S & 1), DDSP_B200_E_INVALID,
+               "%s: bad shape BF=%lld S=%d (S must be odd)", name, (long long)BF, S);
+  DDSP_REQUIRE(BF < (1ll << 31), DDSP_B200_E_INVALID, "%s: too many frames", name);
+  if (BF == 0) return 0;
+  sinc_ir_backward_kernel<<<(unsigned)BF, kSincThreads, 0, (cudaStream_t)stream>>>(
+      cutoff, d_ir, d_cutoff, S, scale, high_pass);
+  DDSP_CHECK_LAUNCH(name);
+  return 0;
+}
+
+// The checks both sinc_filter entry points make after the null-pointer check; sets
+// *frame, *start and *out_len.  The caller returns 0 for B == 0.
+static int sinc_filter_check(const char* name, int B, int N, int F, int S, int cutoff_batch,
+                             int padding, int* frame, int* start, int* out_len) {
+  DDSP_REQUIRE(B >= 0 && N >= 1 && F >= 1 && S >= 1 && (S & 1), DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d N=%d F=%d S=%d (S must be odd)", name, B, N, F, S);
+  // core.py:1441-1443
+  DDSP_REQUIRE(cutoff_batch == B || cutoff_batch == 1, DDSP_B200_E_INVALID,
+               "Batch size of audio (%d) and impulse response (%d) must be the "
+               "same.", B, cutoff_batch);
+  DDSP_REQUIRE(padding == DDSP_B200_PAD_SAME || padding == DDSP_B200_PAD_VALID,
+               DDSP_B200_E_INVALID,
+               "Padding must be 'valid' or 'same' (got code %d)", padding);
+  *frame = ir_frame(N, F);
+  if (!*frame) return DDSP_B200_E_INVALID;
+  if (B == 0) return 0;
+  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID, "%s: B=%d exceeds the 65535 grid limit",
+               name, B);
+  DDSP_REQUIRE(S >= 3, DDSP_B200_E_UNSUPPORTED,
+               "%s: %d tap gives a negative automatic delay (the reference's crop is "
+               "empty); compose sinc_impulse_response and fft_convolve", name, S);
+  DDSP_REQUIRE(S < 2048, DDSP_B200_E_UNSUPPORTED,
+               "%s: %d taps is beyond the fused kernels (2047 at most); compose "
+               "sinc_impulse_response and fft_convolve", name, S);
+  DDSP_REQUIRE((long long)N + S + 4 * kSincTile < (1ll << 31), DDSP_B200_E_INVALID,
+               "%s: N=%d is too long", name, N);
+  *out_len = (padding == DDSP_B200_PAD_VALID) ? (N + S - 1) : N;
+  *start = (S - 1) / 2 - 1;
+  return 0;
+}
+
+int ddsp_b200_sinc_filter(const float* audio, const float* cutoff, float* out, int B, int N,
+                          int F, int S, int cutoff_batch, float scale, int high_pass,
+                          int padding, int accumulate, void* stream) {
+  const char* name = "sinc_filter";
+  DDSP_REQUIRE(audio && cutoff && out, DDSP_B200_E_INVALID, "%s: null pointer", name);
+  int frame = 0, start = 0, out_len = 0;
+  int rc = sinc_filter_check(name, B, N, F, S, cutoff_batch, padding, &frame, &start,
+                             &out_len);
+  if (rc || B == 0) return rc;
+  const size_t smem = sinc_filter_smem(S);
+  rc = set_smem(sinc_filter_kernel, smem, name);
+  if (rc) return rc;
+  SincFilterParams p;
+  p.x = audio; p.cutoff = cutoff; p.out = out;
+  p.N = N; p.F = F; p.frame = frame; p.S = S; p.cutoff_stride = cutoff_batch == 1 ? 0 : F;
+  p.scale = scale; p.high_pass = high_pass ? 1 : 0; p.start = start; p.out_len = out_len;
+  p.accumulate = accumulate ? 1 : 0;
+  dim3 grid((out_len + kSincTile - 1) / kSincTile, B);
+  sinc_filter_kernel<<<grid, kSincThreads, smem, (cudaStream_t)stream>>>(p);
+  DDSP_CHECK_LAUNCH(name);
+  return 0;
+}
+
+// Partial d cutoff sums the backward needs: none when every frame is one tile and every
+// item has its own cutoff.
+static size_t sinc_bwd_part_bytes(int B, int N, int F, int cutoff_batch, int frame) {
+  int fpt, n_seg, seg, tiles;
+  sinc_bwd_tiles(N, F, frame, &fpt, &n_seg, &seg, &tiles);
+  if (n_seg == 1 && !(cutoff_batch == 1 && B > 1)) return 0;
+  return sizeof(float) * (size_t)B * F * n_seg;
+}
+
+size_t ddsp_b200_sinc_filter_backward_workspace(int B, int N, int F, int S, int cutoff_batch) {
+  if (B <= 0 || N <= 0 || F <= 0 || S <= 0 || (cutoff_batch != 1 && cutoff_batch != B))
+    return 0;
+  const int frame = (N + F - 1) / F;
+  if ((N + frame - 1) / frame != F) return 0;
+  const size_t part = sinc_bwd_part_bytes(B, N, F, cutoff_batch, frame);
+  return part ? part + 256 : 0;
+}
+
+int ddsp_b200_sinc_filter_backward(const float* audio, const float* cutoff, const float* grad,
+                                   float* d_audio, float* d_cutoff, int B, int N, int F,
+                                   int S, int cutoff_batch, float scale, int high_pass,
+                                   int padding, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+  const char* name = "sinc_filter_backward";
+  DDSP_REQUIRE(audio && cutoff && grad, DDSP_B200_E_INVALID, "%s: null pointer", name);
+  int frame = 0, start = 0, out_len = 0;
+  int rc = sinc_filter_check(name, B, N, F, S, cutoff_batch, padding, &frame, &start,
+                             &out_len);
+  if (rc || B == 0) return rc;
+  const size_t need =
+      d_cutoff ? ddsp_b200_sinc_filter_backward_workspace(B, N, F, S, cutoff_batch) : 0;
+  DDSP_REQUIRE(need == 0 || (workspace != nullptr && workspace_bytes >= need),
+               DDSP_B200_E_WORKSPACE, "%s: workspace of %zu B needed, %zu given", name,
+               need, workspace_bytes);
+  if (!d_audio && !d_cutoff) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  SincBwdParams p;
+  p.x = audio; p.cutoff = cutoff; p.g = grad; p.dx = d_audio;
+  float* part = need ? align256<float>(workspace) : nullptr;
+  p.dc = part ? part : d_cutoff;
+  p.N = N; p.F = F; p.frame = frame; p.S = S; p.cutoff_stride = cutoff_batch == 1 ? 0 : F;
+  p.scale = scale; p.high_pass = high_pass ? 1 : 0; p.start = start; p.out_len = out_len;
+  sinc_bwd_tiles(N, F, frame, &p.fpt, &p.n_seg, &p.seg, &p.tiles);
+  const size_t smem = sinc_bwd_smem(S);
+  dim3 grid((unsigned)p.tiles, B);
+  if (d_cutoff) {
+    rc = set_smem(sinc_filter_backward_kernel<true>, smem, name);
+    if (rc) return rc;
+    sinc_filter_backward_kernel<true><<<grid, kSincThreads, smem, st>>>(p);
+  } else {
+    rc = set_smem(sinc_filter_backward_kernel<false>, smem, name);
+    if (rc) return rc;
+    sinc_filter_backward_kernel<false><<<grid, kSincThreads, smem, st>>>(p);
+  }
+  DDSP_CHECK_LAUNCH(name);
+  if (part) {
+    const long long n_out = (long long)cutoff_batch * F;
+    sinc_dc_reduce<<<grid_for(n_out, 256), 256, 0, st>>>(part, d_cutoff, B, F, p.n_seg,
+                                                         cutoff_batch == 1 && B > 1, n_out);
+    DDSP_CHECK_LAUNCH(name);
+  }
+  return 0;
 }
 
 size_t ddsp_b200_oscillator_bank_workspace(int B, int N, int K) {

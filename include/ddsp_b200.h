@@ -283,6 +283,38 @@ int ddsp_b200_frequency_filter_backward(const float* audio, const float* ir,
                                         int window_size, int padding, void* workspace,
                                         size_t workspace_bytes, void* stream);
 
+/* core.sinc_impulse_response (core.py:1576-1625): cutoff [BF] -> ir [BF, S] for
+ * S = 2 (window_size / 2) + 1 taps (odd).  The cutoff is multiplied by `scale` in
+ * float32 first (1, or float32(2 / sample_rate)); high_pass != 0 gives delta - h. */
+int ddsp_b200_sinc_impulse_response(const float* cutoff, float* ir, int64_t BF, int S,
+                                    float scale, int high_pass, void* stream);
+/* Its backward: d_ir [BF, S] -> d_cutoff [BF] (the gradient of the unscaled cutoff). */
+int ddsp_b200_sinc_impulse_response_backward(const float* cutoff, const float* d_ir,
+                                             float* d_cutoff, int64_t BF, int S, float scale,
+                                             int high_pass, void* stream);
+
+/* core.sinc_filter (core.py:1658-1690) fused: fft_convolve of audio [B,N] with the
+ * sinc impulse responses of cutoff [cutoff_batch, F] (cutoff_batch 1 or B), automatic
+ * delay compensation, taps built in shared memory and never stored.  out [B, N] for
+ * 'same', [B, N+S-1] for 'valid'; accumulate != 0: out += result.  The reference's
+ * errors for batch, frames and padding; E_UNSUPPORTED for S < 3 (an empty crop) and
+ * S >= 2048. */
+int ddsp_b200_sinc_filter(const float* audio, const float* cutoff, float* out, int B, int N,
+                          int F, int S, int cutoff_batch, float scale, int high_pass,
+                          int padding, int accumulate, void* stream);
+/* Backward of ddsp_b200_sinc_filter for grad [B, out_len]: d_audio [B,N] and d_cutoff
+ * [cutoff_batch, F], each skipped when NULL; a shared cutoff gets the sum over the
+ * batch.  Same checks as the forward.  No atomics: both gradients are bit-reproducible.
+ * workspace: ddsp_b200_sinc_filter_backward_workspace(B,N,F,S,cutoff_batch) bytes
+ * (needed only when d_cutoff is set; 0 when frames are at most 1024 samples and the
+ * cutoffs are per item). */
+size_t ddsp_b200_sinc_filter_backward_workspace(int B, int N, int F, int S, int cutoff_batch);
+int ddsp_b200_sinc_filter_backward(const float* audio, const float* cutoff, const float* grad,
+                                   float* d_audio, float* d_cutoff, int B, int N, int F,
+                                   int S, int cutoff_batch, float scale, int high_pass,
+                                   int padding, void* workspace, size_t workspace_bytes,
+                                   void* stream);
+
 /* core.oscillator_bank (core.py:911-962) on audio-rate envelopes [B,N,K]:
  * Nyquist mask, exact wrapped phase accumulation (three-pass chunked scan in
  * 64-bit fixed point), amp * sin(phase), summed over k when sum_sinusoids != 0

@@ -71,7 +71,16 @@ f0g[:, 5:9] = 0.3
 f0g.requires_grad_(True)
 ag.decoder_train(feats['amps'], feats['harmonic_distribution'], f0g,
                  feats['noise_magnitudes'], n_samples=N, window_size=0).abs().mean().backward()
+# windowed-sinc filters: impulse response and its backward, the fused filter forward
+# and backward (ragged frames, a shared cutoff, frames split into segments)
+sc = (0.5 * torch.rand(2, 7, 1, device='cuda')).requires_grad_(True)
+core.sinc_impulse_response(sc, window_size=64, high_pass=True).square().mean().backward()
+xs = torch.randn(2, 3000, device='cuda', requires_grad=True)
+core.sinc_filter(xs, sc, window_size=64).square().mean().backward()
+scs = (0.5 * torch.rand(1, 1, 1, device='cuda')).requires_grad_(True)
+core.sinc_filter(xs, scs, window_size=512, padding='valid').square().mean().backward()
 torch.cuda.synchronize()
+assert torch.isfinite(sc.grad).all() and torch.isfinite(scs.grad).all()
 assert torch.isfinite(h2).all() and torch.isfinite(r4).all() and torch.isfinite(ob).all()
 assert torch.isfinite(xa.grad).all() and torch.isfinite(hi.grad).all() and torch.isfinite(f0g.grad).all()
 assert torch.isfinite(e).all() and torch.isfinite(f).all() and torch.isfinite(g).all()
