@@ -5,6 +5,7 @@ cited per function); the arithmetic happens in libddsp_b200.so (hand-written
 sm_90a kernels) through the ctypes C ABI in `_lib.py`.  torch is plumbing:
 device memory and streams.  There is no CPU fallback.
 """
+import functools
 from collections import abc
 from typing import Any, Dict, Optional, Sequence, Text
 
@@ -122,6 +123,33 @@ class _on_device_of:
 
   def __exit__(self, *exc):
     return self._ctx.__exit__(*exc)
+
+
+def _cuda_tensors(xs):
+  for x in xs:
+    if isinstance(x, torch.Tensor):
+      if x.is_cuda:
+        yield x
+    elif isinstance(x, dict):
+      yield from _cuda_tensors(x.values())
+    elif isinstance(x, (list, tuple)):
+      yield from _cuda_tensors(x)
+
+
+def on_operands_device(fn):
+  """Runs `fn` with the device of its CUDA tensor arguments current (those inside
+  dicts, lists and tuples included), after checking that they share one device: its
+  host arithmetic, allocations and launches then go to that device and its current
+  stream, and operands on two devices raise ValueError before any device work.
+  Without CUDA tensor arguments (numpy arrays, CPU tensors) it changes nothing."""
+  @functools.wraps(fn)
+  def wrapper(*args, **kwargs):
+    tensors = list(_cuda_tensors(args)) + list(_cuda_tensors(kwargs.values()))
+    if not tensors:
+      return fn(*args, **kwargs)
+    with _on_device_of(*tensors):
+      return fn(*args, **kwargs)
+  return wrapper
 
 
 def _check_out(out, shape, like, name='out'):
@@ -379,6 +407,7 @@ def resample(inputs, n_timesteps: int, method: Text = 'linear',
 # ----------------------------------------------------------------------------
 # Harmonic synthesis (core.py:1048-1111)
 # ----------------------------------------------------------------------------
+@on_operands_device
 def harmonic_controls(amplitudes, harmonic_distribution, f0_hz, sample_rate,
                       scale=True, normalize_below_nyquist=True):
   """synths.Harmonic.get_controls arithmetic (synths.py:94-121): exp_sigmoid,
@@ -422,6 +451,7 @@ def get_harmonic_frequencies(frequencies, n_harmonics: int):
   return frequencies * ratios[None, None, :]
 
 
+@on_operands_device
 def remove_above_nyquist(frequency_envelopes, amplitude_envelopes,
                          sample_rate: int = 16000):
   """core.remove_above_nyquist (core.py:869-891)."""
@@ -445,6 +475,7 @@ def harmonic_to_sinusoidal(harm_amp, harm_dist, f0_hz, sample_rate=16000):
   return harm_amp * harm_dist, freqs
 
 
+@on_operands_device
 def normalize_harmonics(harmonic_distribution, f0_hz=None, sample_rate=None):
   """core.normalize_harmonics (core.py:894-907) on the controls kernel."""
   sh = _shape(harmonic_distribution)
@@ -500,6 +531,7 @@ def angular_cumsum(angular_frequency, chunk_size: int = 1000,
   return out.reshape(shape)
 
 
+@on_operands_device
 def oscillator_bank(frequency_envelopes, amplitude_envelopes,
                     sample_rate: int = 16000, sum_sinusoids: bool = True,
                     use_angular_cumsum: bool = False,
@@ -540,6 +572,7 @@ def oscillator_bank(frequency_envelopes, amplitude_envelopes,
   return out
 
 
+@on_operands_device
 def sinusoidal_synthesis(frequencies, amplitudes, n_samples: int = 64000,
                          sample_rate: int = 16000,
                          amp_resample_method: Text = 'window', out=None,
@@ -583,6 +616,7 @@ def sinusoidal_synthesis(frequencies, amplitudes, n_samples: int = 64000,
   return out
 
 
+@on_operands_device
 def harmonic_synthesis(frequencies,
                        amplitudes,
                        harmonic_shifts=None,
@@ -715,6 +749,7 @@ def harmonic_synthesis(frequencies,
   return out
 
 
+@on_operands_device
 def streaming_harmonic_synthesis(frequencies,
                                  amplitudes,
                                  harmonic_distribution=None,
@@ -751,19 +786,21 @@ def streaming_harmonic_synthesis(frequencies,
     # normalize_harmonics (core.py:1143-1146): Nyquist mask + row normalisation
     hd_n = torch.empty_like(hd)
     amp_copy = torch.empty_like(amplitudes)
-    _lib.check(lib.ddsp_b200_harmonic_controls(
-        _ptr(amplitudes), _ptr(hd), _ptr(frequencies), _ptr(amp_copy), _ptr(hd_n),
-        b, f, k, float(sample_rate), _lib.CTL_NYQUIST, _stream()))
+    with _on_device_of(frequencies, amplitudes, hd):
+      _lib.check(lib.ddsp_b200_harmonic_controls(
+          _ptr(amplitudes), _ptr(hd), _ptr(frequencies), _ptr(amp_copy), _ptr(hd_n),
+          b, f, k, float(sample_rate), _lib.CTL_NYQUIST, _stream()))
     hd = hd_n
   init = None
   if initial_phase is not None:
     init = torch_float32(initial_phase).reshape(b).contiguous()
   audio = torch.empty((b, n_samples), dtype=torch.float32, device=frequencies.device)
   final_phase = torch.empty((b,), dtype=torch.float32, device=frequencies.device)
-  _lib.check(lib.ddsp_b200_streaming_harmonic_forward(
-      _ptr(frequencies), _ptr(amplitudes), _ptr(hd), _ptr(init), _ptr(audio),
-      _ptr(final_phase), b, f, k, n_samples, float(sample_rate),
-      AMP_METHODS[amp_resample_method], _stream()))
+  with _on_device_of(frequencies, amplitudes, hd, init):
+    _lib.check(lib.ddsp_b200_streaming_harmonic_forward(
+        _ptr(frequencies), _ptr(amplitudes), _ptr(hd), _ptr(init), _ptr(audio),
+        _ptr(final_phase), b, f, k, n_samples, float(sample_rate),
+        AMP_METHODS[amp_resample_method], _stream()))
   return audio, final_phase.reshape(b, 1, 1)
 
 
@@ -811,8 +848,9 @@ def frequency_impulse_response(magnitudes, window_size: int = 0):
   ir = torch.empty(tuple(magnitudes.shape[:-1]) + (s,), dtype=torch.float32,
                    device=magnitudes.device)
   bf = magnitudes.numel() // nb
-  _lib.check(lib.ddsp_b200_frequency_impulse_response(
-      _ptr(magnitudes), _ptr(ir), bf, nb, int(window_size), _stream()))
+  with _on_device_of(magnitudes):
+    _lib.check(lib.ddsp_b200_frequency_impulse_response(
+        _ptr(magnitudes), _ptr(ir), bf, nb, int(window_size), _stream()))
   return ir
 
 
@@ -913,12 +951,15 @@ def _fft_convolve_cufft(audio, impulse_response, n_ir_frames, frame_size, fft_si
   return total[:, start:start + crop_size].contiguous()
 
 
+@on_operands_device
 def fft_convolve_lti(audio, impulse_response, start, out_len, out=None,
                      accumulate=False, reverse_audio=False, reverse_ir=False):
   """Full linear convolution of audio [B, N] with ONE impulse response per item
   [1 or B, S], cropped to [start, start + out_len): `ddsp_b200_fft_convolve_lti`
   (partitioned overlap-save, hand-written FFTs).  reverse_*: read that operand back
   to front (what the backward pass needs)."""
+  audio = torch_float32(audio)
+  impulse_response = torch_float32(impulse_response)
   b, n = audio.shape
   ir_batch, s_len = impulse_response.shape
   if out is None:
@@ -970,6 +1011,7 @@ def _fft_convolve_geometry(sa, si, padding, delay_compensation):
           crop_size)
 
 
+@on_operands_device
 def fft_convolve(audio, impulse_response, padding: Text = 'same',
                  delay_compensation: int = -1, out=None, accumulate=False):
   """core.fft_convolve (core.py:1382-1473).
@@ -1058,6 +1100,7 @@ def fft_convolve(audio, impulse_response, padding: Text = 'same',
   return out
 
 
+@on_operands_device
 def frequency_filter(audio, magnitudes, window_size: int = 0,
                      padding: Text = 'same'):
   """core.frequency_filter (core.py:1628-1655).  When grad is enabled and an input
@@ -1148,6 +1191,7 @@ def sinc_filter_forward(audio, cutoff, s, scale, high_pass, padding, cutoff_batc
   return out
 
 
+@on_operands_device
 def sinc_filter(audio, cutoff_frequency, window_size: int = 512,
                 sample_rate: Optional[int] = None, padding: Text = 'same',
                 high_pass: bool = False):
@@ -1194,6 +1238,7 @@ def _per_sample(x, shape, batch_size, n_samples):
   return torch_float32(x).reshape(shape).expand(batch_size, n_samples).contiguous()
 
 
+@on_operands_device
 def mod_delay(audio, gain, phase, max_length, scale=1.0, offset=0.0, add_dry=False):
   """`[add_dry] audio + gain * variable_length_delay(phase * scale + offset, audio,
   max_length)` in one kernel (csrc/mod_delay.cuh); `phase * scale + offset` is two
@@ -1232,6 +1277,7 @@ def mod_delay_forward(audio, gain, phase, max_length, scale, offset, add_dry):
   return out
 
 
+@on_operands_device
 def variable_length_delay(phase, audio, max_length: int = 512):
   """core.variable_length_delay (core.py:1285-1314): audio delayed by
   phase * max_length samples with linear interpolation, the reference's wrap
@@ -1265,6 +1311,7 @@ def _frame_rows(x, name):
   return shape
 
 
+@on_operands_device
 def wavetable_synthesis(frequencies, amplitudes, wavetables, n_samples: int = 64000,
                         sample_rate: int = 16000):
   """core.wavetable_synthesis (core.py:1238-1282) on one fused kernel
@@ -1339,6 +1386,7 @@ def _mix_shapes(signal_one, signal_two, mix_level=None):
   return s1
 
 
+@on_operands_device
 def mix(signal_one, signal_two, mix_level):
   """processors.Mix.get_signal (processors.py:217-233): the constant-power crossfade
   sqrt(|m|) s1 + (1 - sqrt(|m - 1|)) s2 in one kernel (csrc/routing.cuh).  Routes to
@@ -1370,6 +1418,7 @@ def _ir_rows(x, name):
   return shape[0]
 
 
+@on_operands_device
 def exp_decay_ir(gain, decay, reverb_length, noise=None, seed=0, offset=0):
   """ExpDecayReverb._get_ir (effects.py:144-151) on the SCALED gain:
   `(gain * exp(-(2 + exp(decay)) * linspace(0, 1, L))) * noise`, [rows, L], one
@@ -1414,12 +1463,14 @@ def uniform_noise(batch_size, n_samples, seed=0, offset=0, device=None):
   Philox4x32-10 keyed by `seed`, counter (sample/4, batch, offset)."""
   out = torch.empty((batch_size, n_samples), dtype=torch.float32,
                     device=device or _device())
-  _lib.check(_lib.load().ddsp_b200_uniform_noise(
-      _ptr(out), batch_size, n_samples, int(seed) & (2**64 - 1),
-      int(offset) & (2**64 - 1), _stream()))
+  with _on_device_of(out):
+    _lib.check(_lib.load().ddsp_b200_uniform_noise(
+        _ptr(out), batch_size, n_samples, int(seed) & (2**64 - 1),
+        int(offset) & (2**64 - 1), _stream()))
   return out
 
 
+@on_operands_device
 def filtered_noise(magnitudes, n_samples, window_size=257, noise=None, seed=0,
                    offset=0, out=None, accumulate=False):
   """FilteredNoise.get_signal arithmetic (synths.py:181-196): uniform noise ->
@@ -1464,6 +1515,7 @@ def filtered_noise(magnitudes, n_samples, window_size=257, noise=None, seed=0,
   return out
 
 
+@on_operands_device
 def decoder_forward(amps, harmonic_distribution, f0_hz, noise_magnitudes,
                     n_samples, sample_rate=16000, amp_resample_method='window',
                     normalize_below_nyquist=True, window_size=0,
@@ -1517,6 +1569,7 @@ def noise_controls(magnitudes, initial_bias=-5.0, scale=True):
   return out
 
 
+@on_operands_device
 def add(signal_one, signal_two, out=None):
   """processors.Add.get_signal (processors.py:174-176).  Routes to
   `autograd.AddFn` when grad is enabled, an input requires it and no `out` is
@@ -1531,11 +1584,12 @@ def add(signal_one, signal_two, out=None):
 
 def add_forward(a, b, out=None):
   """The add kernel on float32 CUDA tensors that broadcast against each other."""
-  if a.shape != b.shape:
-    a, b = torch.broadcast_tensors(a, b)
-    a, b = a.contiguous(), b.contiguous()
-  if out is None:
-    out = torch.empty_like(a)
-  _lib.check(_lib.load().ddsp_b200_add(_ptr(a), _ptr(b), _ptr(out), a.numel(),
-                                       _stream()))
+  with _on_device_of(a, b, out):
+    if a.shape != b.shape:
+      a, b = torch.broadcast_tensors(a, b)
+      a, b = a.contiguous(), b.contiguous()
+    if out is None:
+      out = torch.empty_like(a)
+    _lib.check(_lib.load().ddsp_b200_add(_ptr(a), _ptr(b), _ptr(out), a.numel(),
+                                         _stream()))
   return out

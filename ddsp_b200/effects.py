@@ -158,6 +158,8 @@ class FilteredNoiseReverb(Reverb):
         torch.is_grad_enabled()):
       from ddsp_b200 import autograd as _ag
       syn = self._synth
+      # the controls in float32, as on the inference path, whatever the caller's dtype
+      magnitudes = core.torch_float32(magnitudes)
       if syn.scale_fn is core.exp_sigmoid:
         mags = _ag.exp_sigmoid(magnitudes + syn.initial_bias)
       elif syn.scale_fn is not None:

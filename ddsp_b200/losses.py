@@ -46,6 +46,7 @@ class Loss:
   def __init__(self, name=None):
     self.name = name if name is not None else _snake_case(type(self).__name__)
 
+  @core.on_operands_device
   def __call__(self, *args, **kwargs):
     return self.call(*args, **kwargs)
 
@@ -79,6 +80,7 @@ class SpectralLoss:
         functools.partial(spectral_ops.compute_mag, size=size)
         for size in self.fft_sizes]
 
+  @core.on_operands_device
   def __call__(self, target_audio, audio, weights=None):
     return self.call(target_audio, audio, weights=weights)
 

@@ -20,6 +20,7 @@ class Processor:
     self.name = name
     self.trainable = trainable
 
+  @core.on_operands_device
   def __call__(self, *args, return_outputs_dict: bool = False, **kwargs):
     return self.call(*args, return_outputs_dict=return_outputs_dict, **kwargs)
 
@@ -54,6 +55,7 @@ class ProcessorGroup(dags.DAGLayer):
   def processors(self):
     return [getattr(self, name) for name in self.processor_names]
 
+  @core.on_operands_device
   def __call__(self, inputs: TensorDict, return_outputs_dict: bool = False,
                **kwargs):
     return self.call(inputs, return_outputs_dict=return_outputs_dict, **kwargs)

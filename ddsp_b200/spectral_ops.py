@@ -71,16 +71,8 @@ class FrameWindowFn(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, audio, frame_size, step):
-    from ddsp_b200 import _lib
-    audio = audio.contiguous()
-    b, n = audio.shape
-    n_frames = -(-n // step)
-    frames = torch.empty((b, n_frames, frame_size), dtype=torch.float32,
-                         device=audio.device)
-    _lib.check(_lib.load().ddsp_b200_frame_window(
-        audio.data_ptr(), _hann(frame_size, audio.device).data_ptr(),
-        frames.data_ptr(), b, n, n_frames, frame_size, step, _stream()))
-    ctx.meta = (b, n, n_frames, frame_size, step)
+    frames = _frame_window(audio, frame_size, step)
+    ctx.meta = (audio.shape[0], audio.shape[1], frames.shape[1], frame_size, step)
     return frames
 
   @staticmethod
@@ -96,15 +88,16 @@ class FrameWindowFn(torch.autograd.Function):
 
 
 def _frame_window(audio, frame_size, step):
-  from ddsp_b200 import _lib
+  from ddsp_b200 import _lib, core
   audio = audio.contiguous()
   b, n = audio.shape
   n_frames = -(-n // step)
   frames = torch.empty((b, n_frames, frame_size), dtype=torch.float32,
                        device=audio.device)
-  _lib.check(_lib.load().ddsp_b200_frame_window(
-      audio.data_ptr(), _hann(frame_size, audio.device).data_ptr(),
-      frames.data_ptr(), b, n, n_frames, frame_size, step, _stream()))
+  with core._on_device_of(audio):
+    _lib.check(_lib.load().ddsp_b200_frame_window(
+        audio.data_ptr(), _hann(frame_size, audio.device).data_ptr(),
+        frames.data_ptr(), b, n, n_frames, frame_size, step, _stream()))
   return frames
 
 
@@ -120,26 +113,28 @@ class SpectralTermFn(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, stft_target, audio, frame_size, step, mag_weight, logmag_weight):
-    from ddsp_b200 import _lib
-    audio = audio.to(torch.float32).contiguous()
-    frames = _frame_window(audio, frame_size, step)
-    xv = torch.fft.rfft(frames, n=frame_size, dim=-1)
-    del frames
-    xt = stft_target.contiguous()
-    if xt.shape != xv.shape:
-      raise ValueError(f'target STFT {tuple(xt.shape)} vs value STFT {tuple(xv.shape)}')
-    grad = torch.empty_like(xv)
-    sums = torch.zeros(2, dtype=torch.float64, device=xv.device)
-    m = xv.numel()
-    _lib.check(_lib.load().ddsp_b200_spectral_l1(
-        xt.data_ptr(), xv.data_ptr(), grad.data_ptr(), sums.data_ptr(), m,
-        float(mag_weight), float(logmag_weight), xv.shape[-1], frame_size,
-        _stream()))
-    ctx.save_for_backward(grad)
-    ctx.meta = (audio.shape[0], audio.shape[1], xv.shape[1], frame_size, step)
-    w = torch.tensor([mag_weight / m, logmag_weight / m], dtype=torch.float64,
-                     device=xv.device)
-    return (sums * w).sum().to(torch.float32)
+    from ddsp_b200 import _lib, core
+    with core._on_device_of(stft_target, audio):
+      audio = audio.to(torch.float32).contiguous()
+      frames = _frame_window(audio, frame_size, step)
+      xv = torch.fft.rfft(frames, n=frame_size, dim=-1)
+      del frames
+      xt = stft_target.to(torch.complex64).contiguous()
+      if xt.data_ptr() % 16:
+        xt = xt.clone()   # spectral_l1 reads 16-byte vectors: a view at an odd offset
+      if xt.shape != xv.shape:
+        raise ValueError(f'target STFT {tuple(xt.shape)} vs value STFT {tuple(xv.shape)}')
+      grad = torch.empty_like(xv)
+      sums = torch.zeros(2, dtype=torch.float64, device=xv.device)
+      m = xv.numel()
+      _lib.check(_lib.load().ddsp_b200_spectral_l1(
+          xt.data_ptr(), xv.data_ptr(), grad.data_ptr(), sums.data_ptr(), m,
+          float(mag_weight), float(logmag_weight), xv.shape[-1], frame_size,
+          _stream()))
+      ctx.save_for_backward(grad)
+      ctx.meta = (audio.shape[0], audio.shape[1], xv.shape[1], frame_size, step)
+      w = _loss_weights((m,), mag_weight, logmag_weight, xv.device)
+      return (sums * w).sum().to(torch.float32)
 
   @staticmethod
   def backward(ctx, grad_out):
@@ -157,6 +152,17 @@ class SpectralTermFn(torch.autograd.Function):
 _LOSS_WEIGHTS = {}
 
 
+def _loss_weights(counts, mag_weight, logmag_weight, device):
+  """[[mag_weight / m, logmag_weight / m] per term] in float64, cached per device: a
+  host-to-device copy on every call would keep the loss out of CUDA graph capture."""
+  key = (tuple(counts), float(mag_weight), float(logmag_weight), str(device))
+  if key not in _LOSS_WEIGHTS:
+    _LOSS_WEIGHTS[key] = torch.tensor(
+        [[mag_weight / m, logmag_weight / m] for m in counts], dtype=torch.float64,
+        device=device)
+  return _LOSS_WEIGHTS[key]
+
+
 class SpectralLossFn(torch.autograd.Function):
   """The whole multi-scale 'L1' spectrogram loss (losses.SpectralLoss.call,
   losses.py:194-243, `ae.gin` weights) as ONE autograd node: per FFT size framing +
@@ -168,33 +174,30 @@ class SpectralLossFn(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, target, audio, fft_sizes, mag_weight, logmag_weight):
-    from ddsp_b200 import _lib
+    from ddsp_b200 import _lib, core
     lib = _lib.load()
-    audio = audio.to(torch.float32).contiguous()
-    target = target.to(torch.float32).contiguous()
-    b, n = audio.shape
-    sums = torch.zeros((len(fft_sizes), 2), dtype=torch.float64, device=audio.device)
-    grads, counts = [], []
-    for idx, size in enumerate(fft_sizes):
-      size = int(size)
-      step = int(size * 0.25)
-      xt = torch.fft.rfft(_frame_window(target, size, step), n=size, dim=-1)
-      xv = torch.fft.rfft(_frame_window(audio, size, step), n=size, dim=-1)
-      m = xv.numel()
-      _lib.check(lib.ddsp_b200_spectral_l1(
-          xt.data_ptr(), xv.data_ptr(), xv.data_ptr(), sums[idx].data_ptr(), m,
-          float(mag_weight), float(logmag_weight), xv.shape[-1], -1, _stream()))
-      del xt
-      grads.append(xv)                   # now holds d loss_size / d X_value, irfft-ready
-      counts.append(m)
-    key = (tuple(counts), float(mag_weight), float(logmag_weight), str(audio.device))
-    if key not in _LOSS_WEIGHTS:
-      _LOSS_WEIGHTS[key] = torch.tensor(
-          [[mag_weight / m, logmag_weight / m] for m in counts], dtype=torch.float64,
-          device=audio.device)
-    ctx.save_for_backward(*grads)
-    ctx.meta = (b, n, tuple(int(sz) for sz in fft_sizes))
-    return (sums * _LOSS_WEIGHTS[key]).sum().to(torch.float32)
+    with core._on_device_of(target, audio):
+      audio = audio.to(torch.float32).contiguous()
+      target = target.to(torch.float32).contiguous()
+      b, n = audio.shape
+      sums = torch.zeros((len(fft_sizes), 2), dtype=torch.float64, device=audio.device)
+      grads, counts = [], []
+      for idx, size in enumerate(fft_sizes):
+        size = int(size)
+        step = int(size * 0.25)
+        xt = torch.fft.rfft(_frame_window(target, size, step), n=size, dim=-1)
+        xv = torch.fft.rfft(_frame_window(audio, size, step), n=size, dim=-1)
+        m = xv.numel()
+        _lib.check(lib.ddsp_b200_spectral_l1(
+            xt.data_ptr(), xv.data_ptr(), xv.data_ptr(), sums[idx].data_ptr(), m,
+            float(mag_weight), float(logmag_weight), xv.shape[-1], -1, _stream()))
+        del xt
+        grads.append(xv)                 # now holds d loss_size / d X_value, irfft-ready
+        counts.append(m)
+      ctx.save_for_backward(*grads)
+      ctx.meta = (b, n, tuple(int(sz) for sz in fft_sizes))
+      w = _loss_weights(counts, mag_weight, logmag_weight, audio.device)
+      return (sums * w).sum().to(torch.float32)
 
   @staticmethod
   def backward(ctx, grad_out):
@@ -220,8 +223,10 @@ def stft_cuda(audio, frame_size, overlap=0.75):
   """stft(pad_end=True) for CUDA tensors through FrameWindowFn + cuFFT."""
   step = int(frame_size * (1.0 - overlap))
   fft_length = 1 << (int(frame_size) - 1).bit_length()
-  frames = FrameWindowFn.apply(audio.to(torch.float32), int(frame_size), step)
-  return torch.fft.rfft(frames, n=fft_length, dim=-1)
+  from ddsp_b200 import core
+  with core._on_device_of(audio):
+    frames = FrameWindowFn.apply(core.torch_float32(audio), int(frame_size), step)
+    return torch.fft.rfft(frames, n=fft_length, dim=-1)
 
 
 # ---- loudness and RMS power (spectral_ops.py:136-324, csrc/loudness.cuh) ------
