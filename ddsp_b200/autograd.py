@@ -603,7 +603,8 @@ class MixtureNLLFn(torch.autograd.Function):
   Gaussian mixture NLL of each query under its own frame's mixture, [B, T, Q].  The
   mixture of `KDEConsistencyLoss.nll` and `TWMLoss`'s p(harmonics | sinusoids);
   differentiable in x, mu and lw by one backward launch.  With no components the
-  logsumexp is over nothing: the NLL is +inf and every gradient 0."""
+  logsumexp is over nothing: the NLL is +inf and every gradient 0.  With no queries
+  the NLL is empty and nothing depends on mu or lw: their gradients are 0."""
 
   @staticmethod
   def forward(ctx, x, mu, lw, scale):
@@ -628,7 +629,8 @@ class MixtureNLLFn(torch.autograd.Function):
     j = mu.shape[-1]
     g = grad.contiguous().to(torch.float32)
     with core._on_device_of(x, mu, lw, g):
-      if j == 0:
+      if j == 0 or q == 0:
+        # the kernel writes nothing when either is empty (include/ddsp_b200.h)
         dx, dmu, dlw = torch.zeros_like(x), torch.zeros_like(mu), torch.zeros_like(lw)
       else:
         dx, dmu, dlw = torch.empty_like(x), torch.empty_like(mu), torch.empty_like(lw)

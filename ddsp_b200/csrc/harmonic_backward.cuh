@@ -198,6 +198,7 @@ inline size_t harmonic_backward_smem(int FT, int hop) {
 // harmonic_distribution).  One thread per sample, one sincospif per oscillator.
 // ---------------------------------------------------------------------------
 constexpr int kDf0Threads = 256;
+constexpr int kDf0Warps = kDf0Threads / 32;
 
 template <bool WINDOW>
 __global__ void __launch_bounds__(kDf0Threads)
@@ -211,8 +212,9 @@ harmonic_df0_kernel(HarmonicParams p, const float* __restrict__ grad,
   unsigned long long* sRed = sD + FT;
   float* sF0 = reinterpret_cast<float*>(sRed + 8);
   float* sAmp = sF0 + (FT + 1);
-  float* sAcc = sAmp + (FT + 1);                 // [FT][3]
-  float* sX = sAcc + 3 * FT + ((3 * FT) & 1);
+  float* sAcc = sAmp + (FT + 1);                 // [kDf0Warps][FT][3]
+  const int n_acc = kDf0Warps * 3 * FT;
+  float* sX = sAcc + n_acc + (n_acc & 1);
   const int b = blockIdx.y;
   const int i0 = blockIdx.x * FT;
   const int nfr = min(FT, F - i0);
@@ -234,7 +236,7 @@ harmonic_df0_kernel(HarmonicParams p, const float* __restrict__ grad,
     sF0[j] = f0b[g];
     sAmp[j] = ampb[g];
   }
-  for (int j = tid; j < 3 * FT; j += kDf0Threads) sAcc[j] = 0.f;
+  for (int j = tid; j < n_acc; j += kDf0Threads) sAcc[j] = 0.f;
   if (p.hd != nullptr) {
     const float* hdb = p.hd + ((size_t)b * F + i0) * K;
     const int rows_in = min(nfr + 1, F - i0);
@@ -268,10 +270,14 @@ harmonic_df0_kernel(HarmonicParams p, const float* __restrict__ grad,
   const float inv_hop = 1.0f / (float)hop;
   const float* gb = grad + (size_t)b * p.N + (size_t)i0 * hop;
   const int n_iter = (n_tile + kDf0Threads - 1) / kDf0Threads;
+  const int lane = tid & 31;
+  float* acc_w = sAcc + (tid >> 5) * 3 * FT;
+  int cur = -1;                        // lane 0: the frame rc / rq0 / rq1 belong to
+  float rc = 0.f, rq0 = 0.f, rq1 = 0.f;
   for (int it = 0; it < n_iter; ++it) {
     const int lt = it * kDf0Threads + tid;
     const bool ok = lt < n_tile;
-    const int li = ok ? lt / hop : 0;
+    const int li = ok ? lt / hop : -1;
     float c = 0.f, q0 = 0.f, q1 = 0.f;
     if (ok) {
       const int r = lt - li * hop;
@@ -300,37 +306,56 @@ harmonic_df0_kernel(HarmonicParams p, const float* __restrict__ grad,
       q1 = c * tri;
       q0 = c * ((float)(r + 1) - tri);
     }
-    // per-frame reduction: a warp whose lanes all sit in one frame reduces by
-    // shuffles; otherwise shared-memory atomics
+    // per-frame reduction in a fixed order, so d f0 is bit-reproducible: a warp's
+    // samples are consecutive, so its frames ascend (one frame when hop is a multiple
+    // of 32); each is reduced by shuffles and added to lane 0's running sums, which
+    // go to the warp's own row of sAcc when the frame changes.  No atomics.
     const unsigned full = 0xffffffffu;
-    const int li0 = __shfl_sync(full, li, 0);
-    const bool same = __all_sync(full, ok && li == li0);
-    if (same) {
+    const int first = __shfl_sync(full, li, 0);
+    if (first >= 0) {
+      const int last = __reduce_max_sync(full, li);
+      for (int fr = first; fr <= last; ++fr) {
+        float sc = li == fr ? c : 0.f, s0 = li == fr ? q0 : 0.f, s1 = li == fr ? q1 : 0.f;
 #pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        c += __shfl_xor_sync(full, c, o);
-        q0 += __shfl_xor_sync(full, q0, o);
-        q1 += __shfl_xor_sync(full, q1, o);
+        for (int o = 16; o > 0; o >>= 1) {
+          sc += __shfl_xor_sync(full, sc, o);
+          s0 += __shfl_xor_sync(full, s0, o);
+          s1 += __shfl_xor_sync(full, s1, o);
+        }
+        if (lane == 0) {
+          if (fr != cur) {
+            if (cur >= 0) {
+              acc_w[3 * cur + 0] = rc;
+              acc_w[3 * cur + 1] = rq0;
+              acc_w[3 * cur + 2] = rq1;
+            }
+            cur = fr;
+            rc = rq0 = rq1 = 0.f;
+          }
+          rc += sc;
+          rq0 += s0;
+          rq1 += s1;
+        }
       }
-      if ((tid & 31) == 0) {
-        atomicAdd(&sAcc[3 * li0 + 0], c);
-        atomicAdd(&sAcc[3 * li0 + 1], q0);
-        atomicAdd(&sAcc[3 * li0 + 2], q1);
-      }
-    } else if (ok) {
-      atomicAdd(&sAcc[3 * li + 0], c);
-      atomicAdd(&sAcc[3 * li + 1], q0);
-      atomicAdd(&sAcc[3 * li + 2], q1);
     }
   }
+  if (lane == 0 && cur >= 0) {
+    acc_w[3 * cur + 0] = rc;
+    acc_w[3 * cur + 1] = rq0;
+    acc_w[3 * cur + 2] = rq1;
+  }
   __syncthreads();
-  for (int j = tid; j < 3 * nfr; j += kDf0Threads)
-    sq[((size_t)b * F + i0) * 3 + j] = sAcc[j];
+  for (int j = tid; j < 3 * nfr; j += kDf0Threads) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < kDf0Warps; ++w) s += sAcc[w * 3 * FT + j];
+    sq[((size_t)b * F + i0) * 3 + j] = s;
+  }
 }
 
 inline size_t harmonic_df0_smem(int FT, int Kp) {
   return sizeof(unsigned long long) * (3 * (size_t)FT + 8) +
-         sizeof(float) * (2 * (size_t)(FT + 1) + 3 * (size_t)FT + 1 +
+         sizeof(float) * (2 * (size_t)(FT + 1) + kDf0Warps * 3 * (size_t)FT + 1 +
                           (size_t)(FT + 1) * Kp);
 }
 

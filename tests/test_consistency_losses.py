@@ -563,6 +563,16 @@ def test_zero_sizes():
   ws, wh = ref.twm_loss_tensors(f0, e, e)
   assert np.array_equal(s.cpu().numpy(), ws.numpy())
   assert np.array_equal(np.isinf(h.cpu().numpy()), np.isinf(wh.numpy()))
+  # no queries but components (Q = 0 < J): the mixture's gradients are exactly 0.
+  # Freed NaN memory first, so that gradients left unwritten come back as NaN.
+  torch.full((1 << 16,), math.nan, device=DEV)
+  x = torch.zeros((2, 3, 0), device=DEV, requires_grad=True)
+  mu, lw = _cuda(np.full((2, 3, 5), 60.0), np.full((2, 3, 5), -1.6), grad=True)
+  nll = autograd.MixtureNLLFn.apply(x, mu, lw, 0.1)
+  assert nll.shape == (2, 3, 0)
+  nll.sum().backward()
+  assert torch.equal(mu.grad, torch.zeros_like(mu)), mu.grad
+  assert torch.equal(lw.grad, torch.zeros_like(lw)), lw.grad
 
 
 @pytest.mark.gpu
