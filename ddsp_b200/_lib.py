@@ -25,6 +25,7 @@ CTL_NYQUIST = 2
 PAD_SAME = 0
 PAD_VALID = 1
 PAD_CENTER = 2
+PADDING = {'same': PAD_SAME, 'valid': PAD_VALID, 'center': PAD_CENTER}
 MEL = 0
 LOGMEL = 1
 MFCC = 2

@@ -74,9 +74,8 @@ class HarmonicSynthesisFn(torch.autograd.Function):
     grad_audio = grad_audio.contiguous().to(torch.float32)
     g0 = torch.empty_like(hd)
     g1 = torch.empty_like(hd)
-    _lib.check(_lib.load().ddsp_b200_harmonic_backward(
-        f0_hz.data_ptr(), grad_audio.data_ptr(), g0.data_ptr(), g1.data_ptr(),
-        b, f, k, n_samples, sample_rate, core.AMP_METHODS[method], core._stream()))
+    core._launch('ddsp_b200_harmonic_backward', f0_hz, grad_audio, g0, g1, b, f, k,
+                 n_samples, sample_rate, core.AMP_METHODS[method])
     # dL/d(amp * hd)[i] = g0[i] + g1[i-1], frame F being a copy of frame F-1
     dha = g0
     dha[:, 1:] += g1[:, :-1]
@@ -94,12 +93,9 @@ def _harmonic_d_f0(f0_hz, amplitudes, hd, grad_audio, n_samples, sample_rate, me
   """dL/d f0_hz [B, F, 1] through the phase (`ddsp_b200_harmonic_backward_f0`)."""
   b, f, k = hd.shape
   d_f0 = torch.empty((b, f, 1), dtype=torch.float32, device=hd.device)
-  nbytes = 12 * b * f
-  ws = torch.empty((max(nbytes, 1),), dtype=torch.uint8, device=hd.device)
-  _lib.check(_lib.load().ddsp_b200_harmonic_backward_f0(
-      f0_hz.data_ptr(), amplitudes.data_ptr(), hd.data_ptr(), grad_audio.data_ptr(),
-      d_f0.data_ptr(), b, f, k, n_samples, sample_rate, core.AMP_METHODS[method],
-      ws.data_ptr(), nbytes, core._stream()))
+  core._launch('ddsp_b200_harmonic_backward_f0', f0_hz, amplitudes, hd, grad_audio, d_f0,
+               b, f, k, n_samples, sample_rate, core.AMP_METHODS[method],
+               *core._workspace(12 * b * f, hd.device))
   return d_f0
 
 
@@ -134,30 +130,24 @@ class DecoderFn(torch.autograd.Function):
     n_samples, sample_rate, method, nyq, window_size, bias, seed, offset = ctx.cfg
     b, f, k = hd.shape
     nb = mags.shape[-1]
-    lib = _lib.load()
-    st = core._stream()
     g = grad_audio.contiguous().to(torch.float32)
     flags = _lib.CTL_SCALE | (_lib.CTL_NYQUIST if nyq else 0)
     # harmonic: sample-rate reductions, then get_controls transposed at frame rate
     g0 = torch.empty_like(hd)
     g1 = torch.empty_like(hd)
-    _lib.check(lib.ddsp_b200_harmonic_backward(
-        f0_hz.data_ptr(), g.data_ptr(), g0.data_ptr(), g1.data_ptr(), b, f, k,
-        n_samples, sample_rate, core.AMP_METHODS[method], st))
+    core._launch('ddsp_b200_harmonic_backward', f0_hz, g, g0, g1, b, f, k, n_samples,
+                 sample_rate, core.AMP_METHODS[method])
     d_amps = torch.empty_like(amps)
     d_hd = torch.empty_like(hd)
-    _lib.check(lib.ddsp_b200_harmonic_controls_backward(
-        amps.data_ptr(), hd.data_ptr(), f0_hz.data_ptr(), g0.data_ptr(), g1.data_ptr(),
-        d_amps.data_ptr(), d_hd.data_ptr(), b, f, k, sample_rate, flags, st))
+    core._launch('ddsp_b200_harmonic_controls_backward', amps, hd, f0_hz, g0, g1, d_amps,
+                 d_hd, b, f, k, sample_rate, flags)
     # noise: the filter is linear in the magnitudes
     dmags = torch.empty_like(mags)
-    _lib.check(lib.ddsp_b200_filtered_noise_backward(
-        g.data_ptr(), 0 if ctx.noise is None else ctx.noise.data_ptr(),
-        seed & (2**64 - 1), offset & (2**64 - 1), dmags.data_ptr(), b, f, nb,
-        n_samples, window_size, st))
+    core._launch('ddsp_b200_filtered_noise_backward', g, ctx.noise, seed, offset, dmags, b,
+                 f, nb, n_samples, window_size)
     d_mags = torch.empty_like(mags)
-    _lib.check(lib.ddsp_b200_noise_controls_backward(
-        mags.data_ptr(), dmags.data_ptr(), d_mags.data_ptr(), mags.numel(), bias, st))
+    core._launch('ddsp_b200_noise_controls_backward', mags, dmags, d_mags, mags.numel(),
+                 bias)
     d_f0 = None
     if ctx.needs_input_grad[2]:
       # the phase path needs the synthesizer controls: one controls launch
@@ -241,18 +231,12 @@ class FirTimeVaryingFn(torch.autograd.Function):
     b, n = audio.shape
     ir_batch, f, s = ir.shape
     g = g.contiguous().to(torch.float32)
-    lib = _lib.load()
-    with core._on_device_of(audio, ir, g):
-      d_audio = torch.empty_like(audio) if ctx.needs_input_grad[0] else None
-      d_ir = torch.empty_like(ir) if ctx.needs_input_grad[1] else None
-      nbytes = (lib.ddsp_b200_fir_time_varying_backward_workspace(b, n, f, s, ir_batch)
-                if d_ir is not None else 0)
-      ws = core._workspace(nbytes, audio.device)
-      _lib.check(lib.ddsp_b200_fir_time_varying_backward(
-          audio.data_ptr(), ir.data_ptr(), g.data_ptr(), core._ptr(d_audio),
-          core._ptr(d_ir), b, n, f, s, ir_batch,
-          _lib.PAD_SAME if padding == 'same' else _lib.PAD_VALID, delay, core._ptr(ws),
-          nbytes, core._stream()))
+    d_audio = torch.empty_like(audio) if ctx.needs_input_grad[0] else None
+    d_ir = torch.empty_like(ir) if ctx.needs_input_grad[1] else None
+    ws = (core._workspace('ddsp_b200_fir_time_varying_backward_workspace', audio.device, b,
+                          n, f, s, ir_batch) if d_ir is not None else (None, 0))
+    core._launch('ddsp_b200_fir_time_varying_backward', audio, ir, g, d_audio, d_ir, b, n,
+                 f, s, ir_batch, _lib.PADDING[padding], delay, *ws)
     return d_audio, d_ir, None, None
 
 
@@ -272,11 +256,9 @@ class FrequencyImpulseResponseFn(torch.autograd.Function):
     shape, window_size = ctx.cfg
     nb = shape[-1]
     d_ir = d_ir.contiguous().to(torch.float32)
-    with core._on_device_of(d_ir):
-      d_mags = torch.empty(shape, dtype=torch.float32, device=d_ir.device)
-      _lib.check(_lib.load().ddsp_b200_frequency_impulse_response_backward(
-          d_ir.data_ptr(), d_mags.data_ptr(), d_mags.numel() // nb, nb, window_size,
-          core._stream()))
+    d_mags = torch.empty(shape, dtype=torch.float32, device=d_ir.device)
+    core._launch('ddsp_b200_frequency_impulse_response_backward', d_ir, d_mags,
+                 d_mags.numel() // nb, nb, window_size)
     return d_mags, None
 
 
@@ -302,20 +284,15 @@ class FrequencyFilterFn(torch.autograd.Function):
     b, n = audio.shape
     mb, nb = shape[0], shape[-1]
     f = shape[1] if len(shape) == 3 else 1
-    pad = _lib.PAD_SAME if padding == 'same' else _lib.PAD_VALID
+    pad = _lib.PADDING[padding]
     g = g.contiguous().to(torch.float32)
-    lib = _lib.load()
-    with core._on_device_of(audio, ir, g):
-      d_audio = torch.empty_like(audio) if ctx.needs_input_grad[0] else None
-      d_mags = (torch.empty(shape, dtype=torch.float32, device=audio.device)
-                if ctx.needs_input_grad[1] else None)
-      nbytes = (lib.ddsp_b200_frequency_filter_backward_workspace(
-          b, f, nb, n, mb, window_size, pad) if d_mags is not None else 0)
-      ws = core._workspace(nbytes, audio.device)
-      _lib.check(lib.ddsp_b200_frequency_filter_backward(
-          audio.data_ptr(), ir.data_ptr(), g.data_ptr(), core._ptr(d_audio),
-          core._ptr(d_mags), b, f, nb, n, mb, window_size, pad, core._ptr(ws), nbytes,
-          core._stream()))
+    d_audio = torch.empty_like(audio) if ctx.needs_input_grad[0] else None
+    d_mags = (torch.empty(shape, dtype=torch.float32, device=audio.device)
+              if ctx.needs_input_grad[1] else None)
+    ws = (core._workspace('ddsp_b200_frequency_filter_backward_workspace', audio.device, b,
+                          f, nb, n, mb, window_size, pad) if d_mags is not None else (None, 0))
+    core._launch('ddsp_b200_frequency_filter_backward', audio, ir, g, d_audio, d_mags, b, f,
+                 nb, n, mb, window_size, pad, *ws)
     return d_audio, d_mags, None, None
 
 
@@ -335,11 +312,9 @@ class SincImpulseResponseFn(torch.autograd.Function):
     cutoff, = ctx.saved_tensors
     s, scale, high_pass = ctx.cfg
     d_ir = d_ir.contiguous().to(torch.float32)
-    with core._on_device_of(cutoff, d_ir):
-      d_cutoff = torch.empty_like(cutoff)
-      _lib.check(_lib.load().ddsp_b200_sinc_impulse_response_backward(
-          cutoff.data_ptr(), d_ir.data_ptr(), d_cutoff.data_ptr(), cutoff.numel(), s,
-          scale, int(high_pass), core._stream()))
+    d_cutoff = torch.empty_like(cutoff)
+    core._launch('ddsp_b200_sinc_impulse_response_backward', cutoff, d_ir, d_cutoff,
+                 cutoff.numel(), s, scale, int(high_pass))
     return d_cutoff, None, None, None, None
 
 
@@ -362,18 +337,13 @@ class SincFilterFn(torch.autograd.Function):
     s, scale, high_pass, padding, cutoff_batch, n_frames = ctx.cfg
     b, n = audio.shape
     g = g.contiguous().to(torch.float32)
-    lib = _lib.load()
-    with core._on_device_of(audio, cutoff, g):
-      d_audio = torch.empty_like(audio) if ctx.needs_input_grad[0] else None
-      d_cutoff = torch.empty_like(cutoff) if ctx.needs_input_grad[1] else None
-      nbytes = (lib.ddsp_b200_sinc_filter_backward_workspace(b, n, n_frames, s, cutoff_batch)
-                if d_cutoff is not None else 0)
-      ws = core._workspace(nbytes, audio.device)
-      _lib.check(lib.ddsp_b200_sinc_filter_backward(
-          audio.data_ptr(), cutoff.data_ptr(), g.data_ptr(), core._ptr(d_audio),
-          core._ptr(d_cutoff), b, n, n_frames, s, cutoff_batch, scale, int(high_pass),
-          _lib.PAD_SAME if padding == 'same' else _lib.PAD_VALID, core._ptr(ws), nbytes,
-          core._stream()))
+    d_audio = torch.empty_like(audio) if ctx.needs_input_grad[0] else None
+    d_cutoff = torch.empty_like(cutoff) if ctx.needs_input_grad[1] else None
+    ws = (core._workspace('ddsp_b200_sinc_filter_backward_workspace', audio.device, b, n,
+                          n_frames, s, cutoff_batch) if d_cutoff is not None else (None, 0))
+    core._launch('ddsp_b200_sinc_filter_backward', audio, cutoff, g, d_audio, d_cutoff, b, n,
+                 n_frames, s, cutoff_batch, scale, int(high_pass), _lib.PADDING[padding],
+                 *ws)
     return d_audio, d_cutoff, None, None, None, None, None, None
 
 
@@ -394,10 +364,8 @@ class FilteredNoiseFn(torch.autograd.Function):
     n_samples, window_size, seed, offset, (b, f, nb) = ctx.cfg
     grad_audio = grad_audio.contiguous().to(torch.float32)
     dmags = torch.empty((b, f, nb), dtype=torch.float32, device=grad_audio.device)
-    _lib.check(_lib.load().ddsp_b200_filtered_noise_backward(
-        grad_audio.data_ptr(), 0 if ctx.noise is None else ctx.noise.data_ptr(),
-        seed & (2**64 - 1), offset & (2**64 - 1), dmags.data_ptr(), b, f, nb,
-        n_samples, window_size, core._stream()))
+    core._launch('ddsp_b200_filtered_noise_backward', grad_audio, ctx.noise, seed, offset,
+                 dmags, b, f, nb, n_samples, window_size)
     return dmags, None, None, None, None, None
 
 
@@ -424,16 +392,12 @@ class SinusoidalSynthesisFn(torch.autograd.Function):
     n_samples, sample_rate, method = ctx.cfg
     b, f, k = amplitudes.shape
     g = grad_audio.contiguous().to(torch.float32)
-    lib = _lib.load()
-    with core._on_device_of(frequencies, amplitudes, g):
-      d_amp = torch.empty_like(amplitudes)
-      d_freq = torch.empty_like(frequencies) if ctx.needs_input_grad[0] else None
-      nbytes = lib.ddsp_b200_sinusoidal_backward_workspace(b, f, k)
-      ws = core._workspace(nbytes, amplitudes.device)
-      _lib.check(lib.ddsp_b200_sinusoidal_backward(
-          frequencies.data_ptr(), amplitudes.data_ptr(), g.data_ptr(), core._ptr(d_freq),
-          d_amp.data_ptr(), b, f, k, n_samples, sample_rate, core.AMP_METHODS[method],
-          core._ptr(ws), nbytes, core._stream()))
+    d_amp = torch.empty_like(amplitudes)
+    d_freq = torch.empty_like(frequencies) if ctx.needs_input_grad[0] else None
+    core._launch('ddsp_b200_sinusoidal_backward', frequencies, amplitudes, g, d_freq, d_amp,
+                 b, f, k, n_samples, sample_rate, core.AMP_METHODS[method],
+                 *core._workspace('ddsp_b200_sinusoidal_backward_workspace',
+                                  amplitudes.device, b, f, k))
     return d_freq, d_amp if ctx.needs_input_grad[1] else None, None, None, None
 
 
@@ -459,17 +423,13 @@ class WavetableSynthesisFn(torch.autograd.Function):
     _, fw, w = wavetables.shape
     g = grad_audio.contiguous().to(torch.float32)
     want = ctx.needs_input_grad
-    lib = _lib.load()
-    with core._on_device_of(f0, amplitudes, wavetables, g):
-      d_f0 = torch.empty_like(f0) if want[0] else None
-      d_amp = torch.empty_like(amplitudes) if want[1] else None
-      d_tab = torch.empty_like(wavetables) if want[2] else None
-      nbytes = lib.ddsp_b200_wavetable_backward_workspace(b, f, n_samples, fw, w)
-      ws = core._workspace(nbytes, amplitudes.device)
-      _lib.check(lib.ddsp_b200_wavetable_backward(
-          f0.data_ptr(), amplitudes.data_ptr(), wavetables.data_ptr(), g.data_ptr(),
-          core._ptr(d_f0), core._ptr(d_amp), core._ptr(d_tab), b, f, n_samples, fw, w,
-          sample_rate, core.AMP_METHODS[method], core._ptr(ws), nbytes, core._stream()))
+    d_f0 = torch.empty_like(f0) if want[0] else None
+    d_amp = torch.empty_like(amplitudes) if want[1] else None
+    d_tab = torch.empty_like(wavetables) if want[2] else None
+    core._launch('ddsp_b200_wavetable_backward', f0, amplitudes, wavetables, g, d_f0, d_amp,
+                 d_tab, b, f, n_samples, fw, w, sample_rate, core.AMP_METHODS[method],
+                 *core._workspace('ddsp_b200_wavetable_backward_workspace',
+                                  amplitudes.device, b, f, n_samples, fw, w))
     return d_f0, d_amp, d_tab, None, None, None
 
 
@@ -496,10 +456,8 @@ class ModDelayFn(torch.autograd.Function):
     d_gain = torch.empty_like(gain) if gain is not None and want[1] else None
     d_phase = torch.empty_like(phase) if want[2] else None
     b, n = audio.shape
-    _lib.check(_lib.load().ddsp_b200_mod_delay_backward(
-        audio.data_ptr(), phase.data_ptr(), core._ptr(gain), g.data_ptr(),
-        core._ptr(d_audio), core._ptr(d_gain), core._ptr(d_phase), b, n, max_length,
-        scale, offset, int(add_dry), core._stream()))
+    core._launch('ddsp_b200_mod_delay_backward', audio, phase, gain, g, d_audio, d_gain,
+                 d_phase, b, n, max_length, scale, offset, int(add_dry))
     return d_audio, d_gain, d_phase, None, None, None, None
 
 
@@ -517,11 +475,9 @@ class ResampleFn(torch.autograd.Function):
   def backward(ctx, g):
     (b, f, c), n, method, add_endpoint = ctx.cfg
     g = g.contiguous().to(torch.float32)
-    with core._on_device_of(g):
-      d_in = torch.empty((b, f, c), dtype=torch.float32, device=g.device)
-      _lib.check(_lib.load().ddsp_b200_resample_backward(
-          g.data_ptr(), d_in.data_ptr(), b, f, c, n, core._RESAMPLE_METHODS[method],
-          int(add_endpoint), core._stream()))
+    d_in = torch.empty((b, f, c), dtype=torch.float32, device=g.device)
+    core._launch('ddsp_b200_resample_backward', g, d_in, b, f, c, n,
+                 core._RESAMPLE_METHODS[method], int(add_endpoint))
     return d_in, None, None, None
 
 
@@ -559,13 +515,10 @@ class MixFn(torch.autograd.Function):
     b, n, c = s1.shape
     g = g.contiguous().to(torch.float32)
     want = ctx.needs_input_grad
-    with core._on_device_of(s1, s2, m, g):
-      d1 = torch.empty_like(s1) if want[0] else None
-      d2 = torch.empty_like(s2) if want[1] else None
-      dm = torch.empty_like(m) if want[2] else None
-      _lib.check(_lib.load().ddsp_b200_mix_backward(
-          s1.data_ptr(), s2.data_ptr(), m.data_ptr(), g.data_ptr(), core._ptr(d1),
-          core._ptr(d2), core._ptr(dm), b, n, c, core._stream()))
+    d1 = torch.empty_like(s1) if want[0] else None
+    d2 = torch.empty_like(s2) if want[1] else None
+    dm = torch.empty_like(m) if want[2] else None
+    core._launch('ddsp_b200_mix_backward', s1, s2, m, g, d1, d2, dm, b, n, c)
     return d1, d2, dm
 
 
@@ -587,13 +540,10 @@ class ExpDecayIrFn(torch.autograd.Function):
     length, seed, offset = ctx.cfg
     g = g.contiguous().to(torch.float32)
     want = ctx.needs_input_grad
-    with core._on_device_of(gain, decay, g):
-      d_gain = torch.empty_like(gain) if want[0] else None
-      d_decay = torch.empty_like(decay) if want[1] else None
-      _lib.check(_lib.load().ddsp_b200_exp_decay_ir_backward(
-          gain.data_ptr(), decay.data_ptr(), core._ptr(ctx.noise), seed & (2**64 - 1),
-          offset & (2**64 - 1), g.data_ptr(), core._ptr(d_gain), core._ptr(d_decay),
-          gain.shape[0], length, core._stream()))
+    d_gain = torch.empty_like(gain) if want[0] else None
+    d_decay = torch.empty_like(decay) if want[1] else None
+    core._launch('ddsp_b200_exp_decay_ir_backward', gain, decay, ctx.noise, seed, offset, g,
+                 d_gain, d_decay, gain.shape[0], length)
     return d_gain, d_decay, None, None, None, None
 
 
@@ -613,13 +563,10 @@ class MixtureNLLFn(torch.autograd.Function):
     j = mu.shape[-1]
     ctx.save_for_backward(x, mu, lw)
     ctx.scale = float(scale)
-    with core._on_device_of(x, mu, lw):
-      if j == 0:
-        return torch.full_like(x, math.inf)
-      nll = torch.empty_like(x)
-      _lib.check(_lib.load().ddsp_b200_mixture_nll_forward(
-          x.data_ptr(), mu.data_ptr(), lw.data_ptr(), nll.data_ptr(), b, t, q, j,
-          ctx.scale, core._stream()))
+    if j == 0:
+      return torch.full_like(x, math.inf)
+    nll = torch.empty_like(x)
+    core._launch('ddsp_b200_mixture_nll_forward', x, mu, lw, nll, b, t, q, j, ctx.scale)
     return nll
 
   @staticmethod
@@ -628,15 +575,13 @@ class MixtureNLLFn(torch.autograd.Function):
     b, t, q = x.shape
     j = mu.shape[-1]
     g = grad.contiguous().to(torch.float32)
-    with core._on_device_of(x, mu, lw, g):
-      if j == 0 or q == 0:
-        # the kernel writes nothing when either is empty (include/ddsp_b200.h)
-        dx, dmu, dlw = torch.zeros_like(x), torch.zeros_like(mu), torch.zeros_like(lw)
-      else:
-        dx, dmu, dlw = torch.empty_like(x), torch.empty_like(mu), torch.empty_like(lw)
-        _lib.check(_lib.load().ddsp_b200_mixture_nll_backward(
-            x.data_ptr(), mu.data_ptr(), lw.data_ptr(), g.data_ptr(), dx.data_ptr(),
-            dmu.data_ptr(), dlw.data_ptr(), b, t, q, j, ctx.scale, core._stream()))
+    if j == 0 or q == 0:
+      # the kernel writes nothing when either is empty (include/ddsp_b200.h)
+      dx, dmu, dlw = torch.zeros_like(x), torch.zeros_like(mu), torch.zeros_like(lw)
+    else:
+      dx, dmu, dlw = torch.empty_like(x), torch.empty_like(mu), torch.empty_like(lw)
+      core._launch('ddsp_b200_mixture_nll_backward', x, mu, lw, g, dx, dmu, dlw, b, t, q,
+                   j, ctx.scale)
     want = ctx.needs_input_grad
     return (dx if want[0] else None, dmu if want[1] else None,
             dlw if want[2] else None, None)
@@ -656,13 +601,10 @@ class CombNLLFn(torch.autograd.Function):
     p = f.shape[-1]
     ctx.save_for_backward(f0, f, a)
     ctx.cfg = (int(n_gaussians), float(scale))
-    with core._on_device_of(f0, f, a):
-      if p == 0:
-        return torch.zeros_like(f0)
-      out = torch.empty_like(f0)
-      _lib.check(_lib.load().ddsp_b200_comb_nll_forward(
-          f0.data_ptr(), f.data_ptr(), a.data_ptr(), out.data_ptr(), b, t, c, p,
-          ctx.cfg[0], ctx.cfg[1], core._stream()))
+    if p == 0:
+      return torch.zeros_like(f0)
+    out = torch.empty_like(f0)
+    core._launch('ddsp_b200_comb_nll_forward', f0, f, a, out, b, t, c, p, *ctx.cfg)
     return out
 
   @staticmethod
@@ -671,15 +613,12 @@ class CombNLLFn(torch.autograd.Function):
     b, t, c = f0.shape
     p = f.shape[-1]
     g = grad.contiguous().to(torch.float32)
-    with core._on_device_of(f0, f, a, g):
-      if p == 0 or c == 0:
-        d_f0, d_f, d_a = torch.zeros_like(f0), torch.zeros_like(f), torch.zeros_like(a)
-      else:
-        d_f0, d_f, d_a = torch.empty_like(f0), torch.empty_like(f), torch.empty_like(a)
-        _lib.check(_lib.load().ddsp_b200_comb_nll_backward(
-            f0.data_ptr(), f.data_ptr(), a.data_ptr(), g.data_ptr(), d_f0.data_ptr(),
-            d_f.data_ptr(), d_a.data_ptr(), b, t, c, p, ctx.cfg[0], ctx.cfg[1],
-            core._stream()))
+    if p == 0 or c == 0:
+      d_f0, d_f, d_a = torch.zeros_like(f0), torch.zeros_like(f), torch.zeros_like(a)
+    else:
+      d_f0, d_f, d_a = torch.empty_like(f0), torch.empty_like(f), torch.empty_like(a)
+      core._launch('ddsp_b200_comb_nll_backward', f0, f, a, g, d_f0, d_f, d_a, b, t, c, p,
+                   *ctx.cfg)
     want = ctx.needs_input_grad
     return (d_f0 if want[0] else None, d_f if want[1] else None,
             d_a if want[2] else None, None, None)

@@ -95,13 +95,37 @@ def _shape(x):
   return tuple(x.shape) if hasattr(x, 'shape') else tuple(np.shape(x))
 
 
-def _stream():
-  return torch.cuda.current_stream().cuda_stream
+def _workspace(query, device, *shape):
+  """The scratch space of one launch as the (buffer, bytes) pair its parameters take,
+  for `_launch(..., *_workspace(...))`.  `query` is the name of the entry point's
+  workspace query, called with `shape`, or the byte count itself where the header
+  states it.  A launch that needs none gets (None, 0): NULL and 0."""
+  nbytes = query if isinstance(query, int) else getattr(_lib.load(), query)(*shape)
+  return (torch.empty((nbytes,), dtype=torch.uint8, device=device) if nbytes else None,
+          nbytes)
 
 
-def _workspace(nbytes, device):
-  """The scratch buffer a library call asked for, or None when it needs none."""
-  return torch.empty((nbytes,), dtype=torch.uint8, device=device) if nbytes else None
+def _launch(symbol, *args):
+  """Calls the launching entry point `symbol` (its full C name) of the library with
+  `args` and the current stream of the operands' device as its last argument, with
+  that device current, and raises its status.  A tensor argument goes as its
+  data_ptr() and must be a contiguous CUDA tensor, all of them on one device; None
+  goes as NULL; anything else as it is.  Every check raises ValueError before the
+  launch."""
+  tensors, c_args = [], []
+  for i, a in enumerate(args):
+    if isinstance(a, torch.Tensor):
+      if not a.is_contiguous():
+        raise ValueError(f'{symbol}: argument {i} is not contiguous (shape '
+                         f'{tuple(a.shape)}, strides {a.stride()}).')
+      if not a.is_cuda:
+        raise ValueError(f'{symbol}: argument {i} is on {a.device}, not a CUDA device.')
+      tensors.append(a)
+      a = a.data_ptr()
+    c_args.append(0 if a is None else a)
+  with _on_device_of(*tensors):
+    _lib.check(getattr(_lib.load(), symbol)(
+        *c_args, torch.cuda.current_stream().cuda_stream))
 
 
 class _on_device_of:
@@ -153,7 +177,7 @@ def on_operands_device(fn):
 
 
 def _check_out(out, shape, like, name='out'):
-  """`out=` of the synthesizers is written by a kernel: B*N floats at data_ptr."""
+  """`out=` of the synthesizers is written by a kernel: B*N contiguous floats."""
   if (not isinstance(out, torch.Tensor) or not out.is_cuda or
       out.dtype != torch.float32 or not out.is_contiguous() or
       tuple(out.shape) != tuple(shape) or out.device != like.device):
@@ -177,10 +201,6 @@ def _no_grad_path(name, *tensors):
         'kernels), or wrap the call in torch.no_grad().')
 
 
-def _ptr(t):
-  return 0 if t is None else t.data_ptr()
-
-
 # ----------------------------------------------------------------------------
 # Scaling (core.py:386-404) - used by callers that want the bare function; the
 # processors call the fused controls kernels instead.
@@ -191,9 +211,7 @@ def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):
   if (exponent, max_value, threshold) == (10.0, 2.0, 1e-7) and not (
       torch.is_grad_enabled() and x.requires_grad):
     out = torch.empty_like(x)
-    with _on_device_of(x):
-      _lib.check(_lib.load().ddsp_b200_noise_controls(
-          _ptr(x), _ptr(out), x.numel(), 0.0, 1, _stream()))
+    _launch('ddsp_b200_noise_controls', x, out, x.numel(), 0.0, 1)
     return out
   return max_value * torch.sigmoid(x)**float(np.log(exponent)) + threshold
 
@@ -336,10 +354,8 @@ def resample_forward(inputs, n_timesteps, method, add_endpoint):
   b, f, c = inputs.shape
   out = torch.empty((b, int(n_timesteps), c), dtype=torch.float32,
                     device=inputs.device)
-  with _on_device_of(inputs):
-    _lib.check(_lib.load().ddsp_b200_resample(
-        _ptr(inputs), _ptr(out), b, f, c, int(n_timesteps),
-        _RESAMPLE_METHODS[method], int(bool(add_endpoint)), _stream()))
+  _launch('ddsp_b200_resample', inputs, out, b, f, c, int(n_timesteps),
+          _RESAMPLE_METHODS[method], int(bool(add_endpoint)))
   return out
 
 
@@ -429,10 +445,8 @@ def harmonic_controls(amplitudes, harmonic_distribution, f0_hz, sample_rate,
   flags = ((_lib.CTL_SCALE if scale else 0) |
            (_lib.CTL_NYQUIST if normalize_below_nyquist else 0))
   _no_grad_path('harmonic_controls', amplitudes, hd, f0_hz)
-  with _on_device_of(amplitudes, hd, f0_hz):
-    _lib.check(_lib.load().ddsp_b200_harmonic_controls(
-        _ptr(amplitudes), _ptr(hd), _ptr(f0_hz), _ptr(amps_out), _ptr(hd_out),
-        b, f, k, float(sample_rate), flags, _stream()))
+  _launch('ddsp_b200_harmonic_controls', amplitudes, hd, f0_hz, amps_out, hd_out, b, f, k,
+          float(sample_rate), flags)
   return amps_out, hd_out
 
 
@@ -516,18 +530,12 @@ def angular_cumsum(angular_frequency, chunk_size: int = 1000,
     c *= int(d)
   x3 = x.reshape(b, n, max(c, 1))
   out = torch.empty_like(x3)
-  lib = _lib.load()
-  with _on_device_of(x3):
-    if tf_sequential:
-      _lib.check(lib.ddsp_b200_angular_cumsum(
-          _ptr(x3), _ptr(out), b, n, max(c, 1), int(chunk_size), 2, None, 0,
-          _stream()))
-    else:
-      nbytes = lib.ddsp_b200_oscillator_bank_workspace(b, n, max(c, 1))
-      ws = _workspace(nbytes, x3.device)
-      _lib.check(lib.ddsp_b200_angular_cumsum(
-          _ptr(x3), _ptr(out), b, n, max(c, 1), int(chunk_size), 0, _ptr(ws),
-          nbytes, _stream()))
+  if tf_sequential:
+    _launch('ddsp_b200_angular_cumsum', x3, out, b, n, max(c, 1), int(chunk_size), 2,
+            None, 0)
+  else:
+    _launch('ddsp_b200_angular_cumsum', x3, out, b, n, max(c, 1), int(chunk_size), 0,
+            *_workspace('ddsp_b200_oscillator_bank_workspace', x3.device, b, n, max(c, 1)))
   return out.reshape(shape)
 
 
@@ -554,21 +562,16 @@ def oscillator_bank(frequency_envelopes, amplitude_envelopes,
   f = torch_float32(frequency_envelopes)
   a = torch_float32(amplitude_envelopes)
   _no_grad_path('oscillator_bank', f, a)
-  lib = _lib.load()
-  with _on_device_of(f, a):
-    if phase_mode == 'tf_sequential':
-      wavs = torch.empty((b, n, k), dtype=torch.float32, device=f.device)
-      _lib.check(lib.ddsp_b200_oscillator_bank_tf_sequential(
-          _ptr(f), _ptr(a), _ptr(wavs), b, n, k, float(sample_rate),
-          int(bool(use_angular_cumsum)), 1000, _stream()))
-      return wavs.sum(-1) if sum_sinusoids else wavs
-    out = torch.empty((b, n) if sum_sinusoids else (b, n, k), dtype=torch.float32,
-                      device=f.device)
-    nbytes = lib.ddsp_b200_oscillator_bank_workspace(b, n, k)
-    ws = _workspace(nbytes, f.device)
-    _lib.check(lib.ddsp_b200_oscillator_bank(
-        _ptr(f), _ptr(a), _ptr(out), b, n, k, float(sample_rate),
-        int(bool(sum_sinusoids)), _ptr(ws), nbytes, _stream()))
+  if phase_mode == 'tf_sequential':
+    wavs = torch.empty((b, n, k), dtype=torch.float32, device=f.device)
+    _launch('ddsp_b200_oscillator_bank_tf_sequential', f, a, wavs, b, n, k,
+            float(sample_rate), int(bool(use_angular_cumsum)), 1000)
+    return wavs.sum(-1) if sum_sinusoids else wavs
+  out = torch.empty((b, n) if sum_sinusoids else (b, n, k), dtype=torch.float32,
+                    device=f.device)
+  _launch('ddsp_b200_oscillator_bank', f, a, out, b, n, k, float(sample_rate),
+          int(bool(sum_sinusoids)),
+          *_workspace('ddsp_b200_oscillator_bank_workspace', f.device, b, n, k))
   return out
 
 
@@ -605,14 +608,9 @@ def sinusoidal_synthesis(frequencies, amplitudes, n_samples: int = 64000,
     accumulate = False
   else:
     _check_out(out, (b, n_samples), freqs)
-  lib = _lib.load()
-  with _on_device_of(freqs, amps, out):
-    nbytes = lib.ddsp_b200_sinusoidal_workspace(b, f, k)
-    ws = _workspace(nbytes, freqs.device)
-    _lib.check(lib.ddsp_b200_sinusoidal_forward(
-        _ptr(freqs), _ptr(amps), _ptr(out), b, f, k, n_samples, float(sample_rate),
-        AMP_METHODS[amp_resample_method], int(bool(accumulate)), _ptr(ws), nbytes,
-        _stream()))
+  _launch('ddsp_b200_sinusoidal_forward', freqs, amps, out, b, f, k, n_samples,
+          float(sample_rate), AMP_METHODS[amp_resample_method], int(bool(accumulate)),
+          *_workspace('ddsp_b200_sinusoidal_workspace', freqs.device, b, f, k))
   return out
 
 
@@ -711,35 +709,32 @@ def harmonic_synthesis(frequencies,
     if out is None:
       out = torch.empty((b, n_samples), dtype=torch.float32,
                         device=frequencies.device)
-    with _on_device_of(frequencies, amplitudes, harmonic_distribution, out):
-      _lib.check(_lib.load().ddsp_b200_harmonic_forward(
-          _ptr(frequencies), _ptr(amplitudes), _ptr(harmonic_distribution),
-          _ptr(out), b, f, k, n_samples, float(sample_rate),
-          AMP_METHODS[amp_resample_method], mode, int(bool(accumulate)), _stream()))
+    _launch('ddsp_b200_harmonic_forward', frequencies, amplitudes, harmonic_distribution,
+            out, b, f, k, n_samples, float(sample_rate), AMP_METHODS[amp_resample_method],
+            mode, int(bool(accumulate)))
     return out
 
   # frame-rate harmonic frequencies / amplitudes, float32 op for op as the
   # reference (core.py:1091-1099): (f0 * k) * (1 + shifts), amplitudes * hd
-  with _on_device_of(frequencies, amplitudes, harmonic_distribution, harmonic_shifts):
-    harmonic_frequencies = get_harmonic_frequencies(frequencies, k)
-    if harmonic_shifts is not None:
-      harmonic_frequencies = harmonic_frequencies * (1.0 + harmonic_shifts)
-    harmonic_amplitudes = (amplitudes * harmonic_distribution
-                           if harmonic_distribution is not None
-                           else amplitudes.expand(b, f, k).contiguous())
-    if fused_ok:
-      return sinusoidal_synthesis(harmonic_frequencies, harmonic_amplitudes,
-                                  n_samples=n_samples, sample_rate=sample_rate,
-                                  amp_resample_method=amp_resample_method, out=out,
-                                  accumulate=accumulate)
-    # core.py:1101-1110 on the stand-alone kernels (audio-rate envelopes exist)
-    frequency_envelopes = resample(harmonic_frequencies, n_samples)
-    amplitude_envelopes = resample(harmonic_amplitudes, n_samples,
-                                   method=amp_resample_method)
-    audio = oscillator_bank(
-        frequency_envelopes, amplitude_envelopes, sample_rate=sample_rate,
-        use_angular_cumsum=use_angular_cumsum,
-        phase_mode='tf_sequential' if phase_mode == 'tf_sequential' else 'exact')
+  harmonic_frequencies = get_harmonic_frequencies(frequencies, k)
+  if harmonic_shifts is not None:
+    harmonic_frequencies = harmonic_frequencies * (1.0 + harmonic_shifts)
+  harmonic_amplitudes = (amplitudes * harmonic_distribution
+                         if harmonic_distribution is not None
+                         else amplitudes.expand(b, f, k).contiguous())
+  if fused_ok:
+    return sinusoidal_synthesis(harmonic_frequencies, harmonic_amplitudes,
+                                n_samples=n_samples, sample_rate=sample_rate,
+                                amp_resample_method=amp_resample_method, out=out,
+                                accumulate=accumulate)
+  # core.py:1101-1110 on the stand-alone kernels (audio-rate envelopes exist)
+  frequency_envelopes = resample(harmonic_frequencies, n_samples)
+  amplitude_envelopes = resample(harmonic_amplitudes, n_samples,
+                                 method=amp_resample_method)
+  audio = oscillator_bank(
+      frequency_envelopes, amplitude_envelopes, sample_rate=sample_rate,
+      use_angular_cumsum=use_angular_cumsum,
+      phase_mode='tf_sequential' if phase_mode == 'tf_sequential' else 'exact')
   if out is None:
     return audio
   if accumulate:
@@ -779,28 +774,23 @@ def streaming_harmonic_synthesis(frequencies,
   amplitudes = torch_float32(amplitudes)
   k = 1
   hd = None
-  lib = _lib.load()
   if harmonic_distribution is not None:
     hd = torch_float32(harmonic_distribution)
     k = int(hd.shape[-1])
     # normalize_harmonics (core.py:1143-1146): Nyquist mask + row normalisation
     hd_n = torch.empty_like(hd)
     amp_copy = torch.empty_like(amplitudes)
-    with _on_device_of(frequencies, amplitudes, hd):
-      _lib.check(lib.ddsp_b200_harmonic_controls(
-          _ptr(amplitudes), _ptr(hd), _ptr(frequencies), _ptr(amp_copy), _ptr(hd_n),
-          b, f, k, float(sample_rate), _lib.CTL_NYQUIST, _stream()))
+    _launch('ddsp_b200_harmonic_controls', amplitudes, hd, frequencies, amp_copy, hd_n,
+            b, f, k, float(sample_rate), _lib.CTL_NYQUIST)
     hd = hd_n
   init = None
   if initial_phase is not None:
     init = torch_float32(initial_phase).reshape(b).contiguous()
   audio = torch.empty((b, n_samples), dtype=torch.float32, device=frequencies.device)
   final_phase = torch.empty((b,), dtype=torch.float32, device=frequencies.device)
-  with _on_device_of(frequencies, amplitudes, hd, init):
-    _lib.check(lib.ddsp_b200_streaming_harmonic_forward(
-        _ptr(frequencies), _ptr(amplitudes), _ptr(hd), _ptr(init), _ptr(audio),
-        _ptr(final_phase), b, f, k, n_samples, float(sample_rate),
-        AMP_METHODS[amp_resample_method], _stream()))
+  _launch('ddsp_b200_streaming_harmonic_forward', frequencies, amplitudes, hd, init, audio,
+          final_phase, b, f, k, n_samples, float(sample_rate),
+          AMP_METHODS[amp_resample_method])
   return audio, final_phase.reshape(b, 1, 1)
 
 
@@ -842,15 +832,12 @@ def frequency_impulse_response(magnitudes, window_size: int = 0):
   if _requires_grad(magnitudes):
     from ddsp_b200 import autograd as _ag
     return _ag.FrequencyImpulseResponseFn.apply(magnitudes, int(window_size))
-  lib = _lib.load()
-  s = lib.ddsp_b200_ir_size(nb, int(window_size))
+  s = _lib.load().ddsp_b200_ir_size(nb, int(window_size))
   magnitudes = torch_float32(magnitudes)
   ir = torch.empty(tuple(magnitudes.shape[:-1]) + (s,), dtype=torch.float32,
                    device=magnitudes.device)
-  bf = magnitudes.numel() // nb
-  with _on_device_of(magnitudes):
-    _lib.check(lib.ddsp_b200_frequency_impulse_response(
-        _ptr(magnitudes), _ptr(ir), bf, nb, int(window_size), _stream()))
+  _launch('ddsp_b200_frequency_impulse_response', magnitudes, ir, magnitudes.numel() // nb,
+          nb, int(window_size))
   return ir
 
 
@@ -965,16 +952,12 @@ def fft_convolve_lti(audio, impulse_response, start, out_len, out=None,
   if out is None:
     out = torch.empty((b, out_len), dtype=torch.float32, device=audio.device)
     accumulate = False
-  lib = _lib.load()
   flags = ((_lib.LTI_REVERSE_AUDIO if reverse_audio else 0) |
            (_lib.LTI_REVERSE_IR if reverse_ir else 0))
-  with _on_device_of(audio, impulse_response, out):
-    nbytes = lib.ddsp_b200_fft_convolve_lti_workspace(b, n, s_len, ir_batch)
-    ws = _workspace(nbytes, audio.device)
-    _lib.check(lib.ddsp_b200_fft_convolve_lti(
-        _ptr(audio), _ptr(impulse_response), _ptr(out), b, n, s_len, ir_batch,
-        int(start), int(out_len), int(bool(accumulate)), flags, _ptr(ws), nbytes,
-        _stream()))
+  _launch('ddsp_b200_fft_convolve_lti', audio, impulse_response, out, b, n, s_len, ir_batch,
+          int(start), int(out_len), int(bool(accumulate)), flags,
+          *_workspace('ddsp_b200_fft_convolve_lti_workspace', audio.device, b, n, s_len,
+                      ir_batch))
   return out
 
 
@@ -1091,12 +1074,9 @@ def fft_convolve(audio, impulse_response, padding: Text = 'same',
   else:
     _check_out(out, (batch_size, crop_size), audio)
   impulse_response = impulse_response.contiguous()
-  with _on_device_of(audio, impulse_response, out):
-    _lib.check(_lib.load().ddsp_b200_fir_time_varying(
-        _ptr(audio), _ptr(impulse_response), _ptr(out), batch_size,
-        audio_size, n_ir_frames, ir_size, ir_batch,
-        _lib.PAD_SAME if padding == 'same' else _lib.PAD_VALID,
-        int(start), int(bool(accumulate)), _stream()))
+  _launch('ddsp_b200_fir_time_varying', audio, impulse_response, out, batch_size,
+          audio_size, n_ir_frames, ir_size, ir_batch, _lib.PADDING[padding], int(start),
+          int(bool(accumulate)))
   return out
 
 
@@ -1157,9 +1137,8 @@ def _sinc_geometry(cutoff_shape, window_size, sample_rate):
 def sinc_impulse_response_forward(cutoff, s, shape, scale, high_pass):
   """`ddsp_b200_sinc_impulse_response` on a float32 CUDA cutoff -> [shape] taps."""
   ir = torch.empty(shape, dtype=torch.float32, device=cutoff.device)
-  with _on_device_of(cutoff):
-    _lib.check(_lib.load().ddsp_b200_sinc_impulse_response(
-        _ptr(cutoff), _ptr(ir), cutoff.numel(), s, scale, int(bool(high_pass)), _stream()))
+  _launch('ddsp_b200_sinc_impulse_response', cutoff, ir, cutoff.numel(), s, scale,
+          int(bool(high_pass)))
   return ir
 
 
@@ -1183,11 +1162,8 @@ def sinc_filter_forward(audio, cutoff, s, scale, high_pass, padding, cutoff_batc
   b, n = audio.shape
   out_len = n if padding == 'same' else n + s - 1
   out = torch.empty((b, out_len), dtype=torch.float32, device=audio.device)
-  with _on_device_of(audio, cutoff):
-    _lib.check(_lib.load().ddsp_b200_sinc_filter(
-        _ptr(audio), _ptr(cutoff), _ptr(out), b, n, n_frames, s, cutoff_batch, scale,
-        int(bool(high_pass)), _lib.PAD_SAME if padding == 'same' else _lib.PAD_VALID, 0,
-        _stream()))
+  _launch('ddsp_b200_sinc_filter', audio, cutoff, out, b, n, n_frames, s, cutoff_batch,
+          scale, int(bool(high_pass)), _lib.PADDING[padding], 0)
   return out
 
 
@@ -1270,10 +1246,8 @@ def mod_delay(audio, gain, phase, max_length, scale=1.0, offset=0.0, add_dry=Fal
 def mod_delay_forward(audio, gain, phase, max_length, scale, offset, add_dry):
   """The forward kernel on [B, N] float32 CUDA tensors (gain may be None)."""
   out = torch.empty_like(audio)
-  with _on_device_of(audio, gain, phase):
-    _lib.check(_lib.load().ddsp_b200_mod_delay_forward(
-        _ptr(audio), _ptr(phase), _ptr(gain), _ptr(out), audio.shape[0],
-        audio.shape[1], max_length, scale, offset, int(add_dry), _stream()))
+  _launch('ddsp_b200_mod_delay_forward', audio, phase, gain, out, audio.shape[0],
+          audio.shape[1], max_length, scale, offset, int(add_dry))
   return out
 
 
@@ -1356,13 +1330,9 @@ def wavetable_forward(f0, amps, tab, n_samples, sample_rate, method):
   b, f = amps.shape
   _, fw, w = tab.shape
   out = torch.empty((b, n_samples), dtype=torch.float32, device=amps.device)
-  lib = _lib.load()
-  with _on_device_of(f0, amps, tab):
-    nbytes = lib.ddsp_b200_wavetable_workspace(b, f)
-    ws = _workspace(nbytes, amps.device)
-    _lib.check(lib.ddsp_b200_wavetable_forward(
-        _ptr(f0), _ptr(amps), _ptr(tab), _ptr(out), b, f, n_samples, fw, w,
-        sample_rate, AMP_METHODS[method], _ptr(ws), nbytes, _stream()))
+  _launch('ddsp_b200_wavetable_forward', f0, amps, tab, out, b, f, n_samples, fw, w,
+          sample_rate, AMP_METHODS[method],
+          *_workspace('ddsp_b200_wavetable_workspace', amps.device, b, f))
   return out
 
 
@@ -1403,10 +1373,7 @@ def mix_forward(signal_one, signal_two, mix_level):
   """The mix kernel on [B, N, C] / [B, N, 1] float32 CUDA tensors."""
   b, n, c = signal_one.shape
   out = torch.empty_like(signal_one)
-  with _on_device_of(signal_one, signal_two, mix_level):
-    _lib.check(_lib.load().ddsp_b200_mix_forward(
-        _ptr(signal_one), _ptr(signal_two), _ptr(mix_level), _ptr(out), b, n, c,
-        _stream()))
+  _launch('ddsp_b200_mix_forward', signal_one, signal_two, mix_level, out, b, n, c)
   return out
 
 
@@ -1451,10 +1418,8 @@ def exp_decay_ir_forward(gain, decay, reverb_length, noise, seed, offset):
   """The impulse-response kernel on [rows] float32 CUDA gain and decay."""
   rows = gain.shape[0]
   ir = torch.empty((rows, reverb_length), dtype=torch.float32, device=gain.device)
-  with _on_device_of(gain, decay, noise):
-    _lib.check(_lib.load().ddsp_b200_exp_decay_ir(
-        _ptr(gain), _ptr(decay), _ptr(noise), seed & (2**64 - 1), offset & (2**64 - 1),
-        _ptr(ir), rows, reverb_length, _stream()))
+  _launch('ddsp_b200_exp_decay_ir', gain, decay, noise, seed, offset, ir, rows,
+          reverb_length)
   return ir
 
 
@@ -1463,10 +1428,7 @@ def uniform_noise(batch_size, n_samples, seed=0, offset=0, device=None):
   Philox4x32-10 keyed by `seed`, counter (sample/4, batch, offset)."""
   out = torch.empty((batch_size, n_samples), dtype=torch.float32,
                     device=device or _device())
-  with _on_device_of(out):
-    _lib.check(_lib.load().ddsp_b200_uniform_noise(
-        _ptr(out), batch_size, n_samples, int(seed) & (2**64 - 1),
-        int(offset) & (2**64 - 1), _stream()))
+  _launch('ddsp_b200_uniform_noise', out, batch_size, n_samples, int(seed), int(offset))
   return out
 
 
@@ -1492,7 +1454,6 @@ def filtered_noise(magnitudes, n_samples, window_size=257, noise=None, seed=0,
         'match. For small hop size = ceil(audio_size / n_ir_frames), '
         'number of impulse response frames must be a multiple of the audio '
         'size.'.format(n_audio_frames, f))
-  lib = _lib.load()
   magnitudes = torch_float32(magnitudes)
   if noise is not None:
     noise = torch_float32(noise)
@@ -1503,15 +1464,10 @@ def filtered_noise(magnitudes, n_samples, window_size=257, noise=None, seed=0,
   else:
     _check_out(out, (b, n_samples), magnitudes)
   _no_grad_path('filtered_noise', magnitudes)
-  with _on_device_of(magnitudes, noise, out):
-    ws_bytes = lib.ddsp_b200_filtered_noise_workspace(b, f, nb, n_samples,
-                                                      int(window_size))
-    workspace = _workspace(ws_bytes, magnitudes.device)
-    _lib.check(lib.ddsp_b200_filtered_noise_forward(
-        _ptr(magnitudes), _ptr(noise), int(seed) & (2**64 - 1),
-        int(offset) & (2**64 - 1), _ptr(out), b, f, nb, n_samples,
-        int(window_size), int(bool(accumulate)), _ptr(workspace), ws_bytes,
-        _stream()))
+  _launch('ddsp_b200_filtered_noise_forward', magnitudes, noise, int(seed), int(offset),
+          out, b, f, nb, n_samples, int(window_size), int(bool(accumulate)),
+          *_workspace('ddsp_b200_filtered_noise_workspace', magnitudes.device, b, f, nb,
+                      n_samples, int(window_size)))
   return out
 
 
@@ -1548,12 +1504,9 @@ def decoder_forward(amps, harmonic_distribution, f0_hz, noise_magnitudes,
   _no_grad_path('decoder_forward', amps, hd, f0_hz, mags)
   out = torch.empty((b, n_samples), dtype=torch.float32, device=hd.device)
   flags = _lib.CTL_SCALE | (_lib.CTL_NYQUIST if normalize_below_nyquist else 0)
-  with _on_device_of(amps, hd, f0_hz, mags, noise):
-    _lib.check(_lib.load().ddsp_b200_decoder_forward(
-        _ptr(amps), _ptr(hd), _ptr(f0_hz), _ptr(mags), _ptr(noise),
-        int(seed) & (2**64 - 1), int(offset) & (2**64 - 1), _ptr(out), b, f, k,
-        sm[2], n_samples, float(sample_rate), AMP_METHODS[amp_resample_method],
-        flags, int(window_size), float(initial_bias), _stream()))
+  _launch('ddsp_b200_decoder_forward', amps, hd, f0_hz, mags, noise, int(seed),
+          int(offset), out, b, f, k, sm[2], n_samples, float(sample_rate),
+          AMP_METHODS[amp_resample_method], flags, int(window_size), float(initial_bias))
   return out
 
 
@@ -1562,10 +1515,8 @@ def noise_controls(magnitudes, initial_bias=-5.0, scale=True):
   magnitudes = torch_float32(magnitudes)
   _no_grad_path('noise_controls', magnitudes)
   out = torch.empty_like(magnitudes)
-  with _on_device_of(magnitudes):
-    _lib.check(_lib.load().ddsp_b200_noise_controls(
-        _ptr(magnitudes), _ptr(out), magnitudes.numel(), float(initial_bias),
-        int(bool(scale)), _stream()))
+  _launch('ddsp_b200_noise_controls', magnitudes, out, magnitudes.numel(),
+          float(initial_bias), int(bool(scale)))
   return out
 
 
@@ -1584,12 +1535,10 @@ def add(signal_one, signal_two, out=None):
 
 def add_forward(a, b, out=None):
   """The add kernel on float32 CUDA tensors that broadcast against each other."""
-  with _on_device_of(a, b, out):
-    if a.shape != b.shape:
-      a, b = torch.broadcast_tensors(a, b)
-      a, b = a.contiguous(), b.contiguous()
-    if out is None:
-      out = torch.empty_like(a)
-    _lib.check(_lib.load().ddsp_b200_add(_ptr(a), _ptr(b), _ptr(out), a.numel(),
-                                         _stream()))
+  if a.shape != b.shape:
+    a, b = torch.broadcast_tensors(a, b)
+    a, b = a.contiguous(), b.contiguous()
+  if out is None:
+    out = torch.empty_like(a)
+  _launch('ddsp_b200_add', a, b, out, a.numel())
   return out

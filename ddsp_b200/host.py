@@ -168,8 +168,8 @@ class HostDecoder:
       stream = torch.cuda.current_stream()
       _lib.check(_lib.load().ddsp_b200_decoder_forward_host(
           self._handle, amps.data_ptr(), hd.data_ptr(), f0.data_ptr(),
-          mags.data_ptr(), int(self.noise.seed) & (2**64 - 1),
-          int(self.noise.next_offset()) & (2**64 - 1), out.data_ptr(), b,
+          mags.data_ptr(), int(self.noise.seed), int(self.noise.next_offset()),
+          out.data_ptr(), b,
           self.n_chunks, float(self.harm.sample_rate),
           core.AMP_METHODS[self.harm.amp_resample_method], flags,
           int(self.noise.window_size), float(self.noise.initial_bias),

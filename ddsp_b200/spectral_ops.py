@@ -12,6 +12,9 @@ compute_mel, compute_logmel and compute_mfcc (csrc/mel.cuh).
 import numpy as np
 import torch
 
+from ddsp_b200 import _lib
+from ddsp_b200 import core
+
 
 def safe_log(x, eps=1e-5):
   """core.safe_log (core.py:213-216)."""
@@ -60,10 +63,6 @@ def _hann(frame_size, device):
   return _WINDOWS[key]
 
 
-def _stream():
-  return torch.cuda.current_stream().cuda_stream
-
-
 class FrameWindowFn(torch.autograd.Function):
   """stft's framing + periodic Hann window (pad_end=True) as one CUDA kernel,
   and its transpose (windowed overlap-add of the frame gradients) for backward.
@@ -77,27 +76,23 @@ class FrameWindowFn(torch.autograd.Function):
 
   @staticmethod
   def backward(ctx, grad_frames):
-    from ddsp_b200 import _lib
     b, n, n_frames, frame_size, step = ctx.meta
     grad_frames = grad_frames.contiguous()
     grad_audio = torch.empty((b, n), dtype=torch.float32, device=grad_frames.device)
-    _lib.check(_lib.load().ddsp_b200_frame_window_adjoint(
-        grad_frames.data_ptr(), _hann(frame_size, grad_frames.device).data_ptr(),
-        grad_audio.data_ptr(), b, n, n_frames, frame_size, step, None, 0, _stream()))
+    core._launch('ddsp_b200_frame_window_adjoint', grad_frames,
+                 _hann(frame_size, grad_frames.device), grad_audio, b, n, n_frames,
+                 frame_size, step, None, 0)
     return grad_audio, None, None
 
 
 def _frame_window(audio, frame_size, step):
-  from ddsp_b200 import _lib, core
   audio = audio.contiguous()
   b, n = audio.shape
   n_frames = -(-n // step)
   frames = torch.empty((b, n_frames, frame_size), dtype=torch.float32,
                        device=audio.device)
-  with core._on_device_of(audio):
-    _lib.check(_lib.load().ddsp_b200_frame_window(
-        audio.data_ptr(), _hann(frame_size, audio.device).data_ptr(),
-        frames.data_ptr(), b, n, n_frames, frame_size, step, _stream()))
+  core._launch('ddsp_b200_frame_window', audio, _hann(frame_size, audio.device), frames,
+               b, n, n_frames, frame_size, step)
   return frames
 
 
@@ -113,7 +108,6 @@ class SpectralTermFn(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, stft_target, audio, frame_size, step, mag_weight, logmag_weight):
-    from ddsp_b200 import _lib, core
     with core._on_device_of(stft_target, audio):
       audio = audio.to(torch.float32).contiguous()
       frames = _frame_window(audio, frame_size, step)
@@ -127,10 +121,8 @@ class SpectralTermFn(torch.autograd.Function):
       grad = torch.empty_like(xv)
       sums = torch.zeros(2, dtype=torch.float64, device=xv.device)
       m = xv.numel()
-      _lib.check(_lib.load().ddsp_b200_spectral_l1(
-          xt.data_ptr(), xv.data_ptr(), grad.data_ptr(), sums.data_ptr(), m,
-          float(mag_weight), float(logmag_weight), xv.shape[-1], frame_size,
-          _stream()))
+      core._launch('ddsp_b200_spectral_l1', xt, xv, grad, sums, m, float(mag_weight),
+                   float(logmag_weight), xv.shape[-1], frame_size)
       ctx.save_for_backward(grad)
       ctx.meta = (audio.shape[0], audio.shape[1], xv.shape[1], frame_size, step)
       w = _loss_weights((m,), mag_weight, logmag_weight, xv.device)
@@ -138,14 +130,13 @@ class SpectralTermFn(torch.autograd.Function):
 
   @staticmethod
   def backward(ctx, grad_out):
-    from ddsp_b200 import _lib
     (grad,) = ctx.saved_tensors
     b, n, n_frames, frame_size, step = ctx.meta
     grad_frames = torch.fft.irfft(grad, n=frame_size, dim=-1).contiguous()
     grad_audio = torch.empty((b, n), dtype=torch.float32, device=grad.device)
-    _lib.check(_lib.load().ddsp_b200_frame_window_adjoint(
-        grad_frames.data_ptr(), _hann(frame_size, grad.device).data_ptr(),
-        grad_audio.data_ptr(), b, n, n_frames, frame_size, step, None, 0, _stream()))
+    core._launch('ddsp_b200_frame_window_adjoint', grad_frames,
+                 _hann(frame_size, grad.device), grad_audio, b, n, n_frames, frame_size,
+                 step, None, 0)
     return None, grad_audio * grad_out, None, None, None, None
 
 
@@ -174,8 +165,6 @@ class SpectralLossFn(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, target, audio, fft_sizes, mag_weight, logmag_weight):
-    from ddsp_b200 import _lib, core
-    lib = _lib.load()
     with core._on_device_of(target, audio):
       audio = audio.to(torch.float32).contiguous()
       target = target.to(torch.float32).contiguous()
@@ -188,9 +177,8 @@ class SpectralLossFn(torch.autograd.Function):
         xt = torch.fft.rfft(_frame_window(target, size, step), n=size, dim=-1)
         xv = torch.fft.rfft(_frame_window(audio, size, step), n=size, dim=-1)
         m = xv.numel()
-        _lib.check(lib.ddsp_b200_spectral_l1(
-            xt.data_ptr(), xv.data_ptr(), xv.data_ptr(), sums[idx].data_ptr(), m,
-            float(mag_weight), float(logmag_weight), xv.shape[-1], -1, _stream()))
+        core._launch('ddsp_b200_spectral_l1', xt, xv, xv, sums[idx], m, float(mag_weight),
+                     float(logmag_weight), xv.shape[-1], -1)
         del xt
         grads.append(xv)                 # now holds d loss_size / d X_value, irfft-ready
         counts.append(m)
@@ -201,8 +189,6 @@ class SpectralLossFn(torch.autograd.Function):
 
   @staticmethod
   def backward(ctx, grad_out):
-    from ddsp_b200 import _lib
-    lib = _lib.load()
     b, n, sizes = ctx.meta
     grads = ctx.saved_tensors
     go = grad_out.to(torch.float32).contiguous()
@@ -213,9 +199,8 @@ class SpectralLossFn(torch.autograd.Function):
       # unnormalised inverse (the 1/n pass would be an elementwise kernel over the
       # frames; spectral_l1 left the spectrum scaled for exactly this)
       gf = torch.fft.irfft(grads[idx], n=size, dim=-1, norm='forward').contiguous()
-      _lib.check(lib.ddsp_b200_frame_window_adjoint(
-          gf.data_ptr(), _hann(size, go.device).data_ptr(), grad_audio.data_ptr(), b, n,
-          n_frames, size, step, go.data_ptr(), int(idx > 0), _stream()))
+      core._launch('ddsp_b200_frame_window_adjoint', gf, _hann(size, go.device), grad_audio,
+                   b, n, n_frames, size, step, go, int(idx > 0))
     return None, grad_audio, None, None, None
 
 
@@ -223,10 +208,8 @@ def stft_cuda(audio, frame_size, overlap=0.75):
   """stft(pad_end=True) for CUDA tensors through FrameWindowFn + cuFFT."""
   step = int(frame_size * (1.0 - overlap))
   fft_length = 1 << (int(frame_size) - 1).bit_length()
-  from ddsp_b200 import core
-  with core._on_device_of(audio):
-    frames = FrameWindowFn.apply(core.torch_float32(audio), int(frame_size), step)
-    return torch.fft.rfft(frames, n=fft_length, dim=-1)
+  frames = FrameWindowFn.apply(core.torch_float32(audio), int(frame_size), step)
+  return torch.fft.rfft(frames, n=fft_length, dim=-1)
 
 
 # ---- loudness and RMS power (spectral_ops.py:136-324, csrc/loudness.cuh) ------
@@ -256,7 +239,6 @@ def _framing(audio, frame_size, hop_size, padding):
   """spectral_ops.pad's checks in its order, on the shape alone: returns (B, N,
   is_1d, n_frames, padding code).  n_frames is what tf.signal.frame gives on the
   padded signal, 0 when 'valid' audio is shorter than a frame."""
-  from ddsp_b200 import _lib
   shape = tuple(audio.shape) if torch.is_tensor(audio) else np.shape(audio)
   if len(shape) == 3 and shape[-1] == 1:
     shape = shape[:2]
@@ -275,12 +257,11 @@ def _framing(audio, frame_size, hop_size, padding):
   else:
     padded = n + 2 * (frame_size // 2) if padding == 'center' else n
     n_frames = 1 + (padded - frame_size) // hop_size if padded >= frame_size else 0
-  code = {'same': _lib.PAD_SAME, 'valid': _lib.PAD_VALID, 'center': _lib.PAD_CENTER}
-  return (1 if len(shape) == 1 else shape[0]), n, len(shape) == 1, n_frames, code[padding]
+  return ((1 if len(shape) == 1 else shape[0]), n, len(shape) == 1, n_frames,
+          _lib.PADDING[padding])
 
 
 def _audio_2d(audio, b, n):
-  from ddsp_b200 import core
   return core.torch_float32(audio).reshape(b, n)
 
 
@@ -308,27 +289,23 @@ class LoudnessFn(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, audio, weights, n_frames, n_fft, hop, padding, range_db, ref_db):
-    from ddsp_b200 import _lib
     b, n = audio.shape
     out = torch.empty((b, n_frames), dtype=torch.float32, device=audio.device)
-    _lib.check(_lib.load().ddsp_b200_loudness_forward(
-        audio.data_ptr(), weights.data_ptr(), out.data_ptr(), b, n, n_frames, n_fft, hop,
-        padding, range_db, ref_db, _stream()))
+    core._launch('ddsp_b200_loudness_forward', audio, weights, out, b, n, n_frames, n_fft,
+                 hop, padding, range_db, ref_db)
     ctx.save_for_backward(audio, weights)
     ctx.meta = (n_frames, n_fft, hop, padding, range_db, ref_db)
     return out
 
   @staticmethod
   def backward(ctx, grad):
-    from ddsp_b200 import _lib
     audio, weights = ctx.saved_tensors
     n_frames, n_fft, hop, padding, range_db, ref_db = ctx.meta
     b, n = audio.shape
     grad = grad.to(torch.float32).contiguous()
     grad_audio = torch.empty_like(audio)
-    _lib.check(_lib.load().ddsp_b200_loudness_backward(
-        audio.data_ptr(), weights.data_ptr(), grad.data_ptr(), grad_audio.data_ptr(), b, n,
-        n_frames, n_fft, hop, padding, range_db, ref_db, _stream()))
+    core._launch('ddsp_b200_loudness_backward', audio, weights, grad, grad_audio, b, n,
+                 n_frames, n_fft, hop, padding, range_db, ref_db)
     return grad_audio, None, None, None, None, None, None, None
 
 
@@ -338,33 +315,28 @@ def compute_loudness(audio, sample_rate=16000, frame_rate=250, n_fft=512,
   [B, N] -> [B, T] and [N] -> [T] ([B, N, 1] is read as [B, N]).  Differentiable
   through LoudnessFn; use_tf=False returns the same values as a NumPy array.  n_fft
   must be a power of two (the reference's weighting only broadcasts then)."""
-  from ddsp_b200 import core
   hop = int(sample_rate // frame_rate)
   n_fft = int(n_fft)
   b, n, is_1d, n_frames, code = _framing(audio, n_fft, hop, padding)
   if n_fft < 2 or n_fft & (n_fft - 1):
     raise ValueError(f'n_fft ({n_fft}) must be a power of two')
   x = _audio_2d(audio, b, n)
-  with core._on_device_of(x):
-    out = LoudnessFn.apply(x, a_weighting(sample_rate, n_fft, x.device), n_frames,
-                           n_fft, hop, code, float(range_db), float(ref_db))
+  out = LoudnessFn.apply(x, a_weighting(sample_rate, n_fft, x.device), n_frames, n_fft, hop,
+                         code, float(range_db), float(ref_db))
   out = out[0] if is_1d else out
   return out if use_tf else out.detach().cpu().numpy()
 
 
 def _rms(audio, sample_rate, frame_rate, frame_size, padding, in_db, range_db, ref_db,
          name):
-  from ddsp_b200 import _lib, core
   hop = int(sample_rate // frame_rate)
   frame_size = int(frame_size)
   b, n, is_1d, n_frames, code = _framing(audio, frame_size, hop, padding)
   core._no_grad_path(name, audio)
   x = _audio_2d(audio, b, n)
   out = torch.empty((b, n_frames), dtype=torch.float32, device=x.device)
-  with core._on_device_of(x):
-    _lib.check(_lib.load().ddsp_b200_rms_power(
-        x.data_ptr(), out.data_ptr(), b, n, n_frames, frame_size, hop, code, int(in_db),
-        float(range_db), float(ref_db), _stream()))
+  core._launch('ddsp_b200_rms_power', x, out, b, n, n_frames, frame_size, hop, code,
+               int(in_db), float(range_db), float(ref_db))
   return out[0] if is_1d else out
 
 
@@ -486,20 +458,17 @@ class MelFn(torch.autograd.Function):
 
   @staticmethod
   def forward(ctx, audio, window, table, meta):
-    from ddsp_b200 import _lib
     n_frames, fft_size, fft_length, hop, pad_end, bins, n_out, mode = meta
     b, n = audio.shape
     out = torch.empty((b, n_frames, n_out), dtype=torch.float32, device=audio.device)
-    _lib.check(_lib.load().ddsp_b200_mel_forward(
-        audio.data_ptr(), window.data_ptr(), table.data_ptr(), out.data_ptr(), b, n,
-        n_frames, fft_size, fft_length, hop, pad_end, bins, n_out, mode, _stream()))
+    core._launch('ddsp_b200_mel_forward', audio, window, table, out, b, n, n_frames,
+                 fft_size, fft_length, hop, pad_end, bins, n_out, mode)
     ctx.save_for_backward(audio, window, table)
     ctx.meta = meta
     return out
 
   @staticmethod
   def backward(ctx, grad):
-    from ddsp_b200 import _lib
     audio, window, table = ctx.saved_tensors
     n_frames, fft_size, fft_length, hop, pad_end, bins, n_out, mode = ctx.meta
     b, n = audio.shape
@@ -507,17 +476,14 @@ class MelFn(torch.autograd.Function):
       return torch.zeros_like(audio), None, None, None
     grad = grad.to(torch.float32).contiguous()
     grad_audio = torch.empty_like(audio)
-    _lib.check(_lib.load().ddsp_b200_mel_backward(
-        audio.data_ptr(), window.data_ptr(), table.data_ptr(), grad.data_ptr(),
-        grad_audio.data_ptr(), b, n, n_frames, fft_size, fft_length, hop, pad_end, bins,
-        n_out, mode, _stream()))
+    core._launch('ddsp_b200_mel_backward', audio, window, table, grad, grad_audio, b, n,
+                 n_frames, fft_size, fft_length, hop, pad_end, bins, n_out, mode)
     return grad_audio, None, None, None
 
 
 def _mel(audio, lo_hz, hi_hz, bins, fft_size, overlap, pad_end, sample_rate, mode,
          mfcc_bins=None, name='compute_mel'):
   """The shape and argument checks (all before any device work), then MelFn."""
-  from ddsp_b200 import _lib, core
   shape = tuple(audio.shape) if torch.is_tensor(audio) else np.shape(audio)
   if len(shape) == 3 and shape[-1] == 1:
     shape = shape[:2]
@@ -544,11 +510,10 @@ def _mel(audio, lo_hz, hi_hz, bins, fft_size, overlap, pad_end, sample_rate, mod
   n_frames = -(-n // hop) if pad_end else max(0, 1 + (n - fft_size) // hop)
   n_out = len(range(bins)[:mfcc_bins]) if mode == _lib.MFCC else bins
   x = _audio_2d(audio, b, n)
-  with core._on_device_of(x):
-    meta = (n_frames, fft_size, fft_length, hop, int(bool(pad_end)), bins, n_out, mode)
-    out = MelFn.apply(x, mel_window(fft_size, x.device),
-                      mel_table(bins, fft_length // 2 + 1, sample_rate, lo_hz, hi_hz,
-                                x.device), meta)
+  meta = (n_frames, fft_size, fft_length, hop, int(bool(pad_end)), bins, n_out, mode)
+  out = MelFn.apply(x, mel_window(fft_size, x.device),
+                    mel_table(bins, fft_length // 2 + 1, sample_rate, lo_hz, hi_hz,
+                              x.device), meta)
   return out[0] if len(shape) == 1 else out
 
 
@@ -557,7 +522,6 @@ def compute_mel(audio, lo_hz=0.0, hi_hz=8000.0, bins=64, fft_size=2048, overlap=
   """spectral_ops.compute_mel (spectral_ops.py:73-89): |stft| projected on
   linear_to_mel_weight_matrix, [B, N] -> [B, T, bins] and [N] -> [T, bins] ([B, N, 1]
   is read as [B, N]).  Differentiable through MelFn."""
-  from ddsp_b200 import _lib
   return _mel(audio, lo_hz, hi_hz, bins, fft_size, overlap, pad_end, sample_rate,
               _lib.MEL)
 
@@ -565,7 +529,6 @@ def compute_mel(audio, lo_hz=0.0, hi_hz=8000.0, bins=64, fft_size=2048, overlap=
 def compute_logmel(audio, lo_hz=80.0, hi_hz=7600.0, bins=64, fft_size=2048, overlap=0.75,
                    pad_end=True, sample_rate=16000):
   """spectral_ops.compute_logmel (spectral_ops.py:97-109): safe_log of compute_mel."""
-  from ddsp_b200 import _lib
   return _mel(audio, lo_hz, hi_hz, bins, fft_size, overlap, pad_end, sample_rate,
               _lib.LOGMEL, name='compute_logmel')
 
@@ -575,6 +538,5 @@ def compute_mfcc(audio, lo_hz=20.0, hi_hz=8000.0, fft_size=1024, mel_bins=128,
   """spectral_ops.compute_mfcc (spectral_ops.py:112-133):
   tf.signal.mfccs_from_log_mel_spectrograms of compute_logmel (the unnormalised DCT-II
   times rsqrt(2 mel_bins)), cut to [..., :mfcc_bins] with Python's slice rules."""
-  from ddsp_b200 import _lib
   return _mel(audio, lo_hz, hi_hz, mel_bins, fft_size, overlap, pad_end, sample_rate,
               _lib.MFCC, mfcc_bins=mfcc_bins, name='compute_mfcc')

@@ -75,7 +75,8 @@ def _backward_call(s, N, want, ws, nbytes, outs):
   d_f0, d_amp, d_tab = (o.data_ptr() if c in want else 0 for o, c in zip(outs, 'fat'))
   _lib.check(_lib.load().ddsp_b200_wavetable_backward(
       f0.data_ptr(), amps.data_ptr(), tab.data_ptr(), g.data_ptr(), d_f0, d_amp, d_tab,
-      B, F, N, Fw, W, 16000.0, _lib.AMP_WINDOW, ws.data_ptr(), nbytes, core._stream()))
+      B, F, N, Fw, W, 16000.0, _lib.AMP_WINDOW, ws.data_ptr(), nbytes,
+      torch.cuda.current_stream().cuda_stream))
 
 
 def _shape(B, F, Fw, W, N, iters, warmup, dev):
