@@ -154,6 +154,10 @@ SIGNATURES = {
         (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
     'ddsp_b200_comb_nll_backward':
         (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
+    'ddsp_b200_sinusoidal_to_harmonic':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _i, _vp]),
+    'ddsp_b200_sinusoidal_to_harmonic_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _i, _vp]),
 }
 
 _lib = None

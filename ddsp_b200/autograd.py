@@ -624,6 +624,34 @@ class CombNLLFn(torch.autograd.Function):
             d_a if want[2] else None, None, None)
 
 
+class SinusoidalToHarmonicFn(torch.autograd.Function):
+  """core.sinusoidal_to_harmonic, differentiable in sin_amps, sin_freqs and f0_hz.
+  Nothing but the inputs is saved: one call of
+  `ddsp_b200_sinusoidal_to_harmonic_backward` (csrc/consistency.cuh, mode C) recomputes
+  each frame's weights and writes all three gradients, zeros where nothing contributes."""
+
+  @staticmethod
+  def forward(ctx, sin_amps, sin_freqs, f0_hz, n_harmonics, harmonic_width, sample_rate,
+              normalize):
+    ctx.save_for_backward(sin_amps, sin_freqs, f0_hz)
+    ctx.cfg = (n_harmonics, harmonic_width, sample_rate, normalize)
+    return core.sinusoidal_to_harmonic_forward(sin_amps, sin_freqs, f0_hz, *ctx.cfg)
+
+  @staticmethod
+  def backward(ctx, g_amp, g_dist):
+    a, f, f0 = ctx.saved_tensors
+    k, width, sample_rate, normalize = ctx.cfg
+    b, t, s = a.shape
+    g_amp = g_amp.contiguous().to(torch.float32)
+    g_dist = g_dist.contiguous().to(torch.float32)
+    d_a, d_f, d_f0 = torch.empty_like(a), torch.empty_like(f), torch.empty_like(f0)
+    core._launch('ddsp_b200_sinusoidal_to_harmonic_backward', a, f, f0, g_amp, g_dist, d_a,
+                 d_f, d_f0, b, t, s, k, width, sample_rate, int(normalize))
+    want = ctx.needs_input_grad
+    return (d_a if want[0] else None, d_f if want[1] else None, d_f0 if want[2] else None,
+            None, None, None, None)
+
+
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):
   """core.exp_sigmoid (core.py:386-404) as differentiable torch ops."""
   return max_value * torch.sigmoid(x)**math.log(exponent) + threshold

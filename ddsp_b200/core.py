@@ -489,6 +489,62 @@ def harmonic_to_sinusoidal(harm_amp, harm_dist, f0_hz, sample_rate=16000):
   return harm_amp * harm_dist, freqs
 
 
+SIN_TO_HARM_MAX_SINUSOIDS = 4096    # staged per frame by the kernels
+
+
+def _sinusoidal_to_harmonic_shapes(sin_amps, sin_freqs, f0_hz, harmonic_width, n_harmonics):
+  """(B, T, S, K) of sinusoidal_to_harmonic from static shapes, or the error."""
+  sa, sf, s0 = _shape(sin_amps), _shape(sin_freqs), _shape(f0_hz)
+  if len(sa) != 3 or sf != sa or s0 != sa[:2] + (1,):
+    raise ValueError(f'sin_amps {sa} and sin_freqs {sf} must both be [batch, time, '
+                     f'n_sinusoids] and f0_hz {s0} [batch, time, 1].')
+  if isinstance(n_harmonics, bool) or int(n_harmonics) != n_harmonics or n_harmonics < 0:
+    raise ValueError(f'n_harmonics must be a non-negative integer, got {n_harmonics}.')
+  if np.float32(harmonic_width) == 0.0:
+    raise ValueError('harmonic_width must be nonzero (the reference divides by it), got '
+                     f'{harmonic_width}.')
+  if sa[2] > SIN_TO_HARM_MAX_SINUSOIDS:
+    raise NotImplementedError(
+        f'sinusoidal_to_harmonic: {sa[2]} sinusoids per frame exceed the '
+        f'{SIN_TO_HARM_MAX_SINUSOIDS} the kernels stage.')
+  return sa + (int(n_harmonics),)
+
+
+def sinusoidal_to_harmonic_forward(sin_amps, sin_freqs, f0_hz, n_harmonics, harmonic_width,
+                                   sample_rate, normalize):
+  """`ddsp_b200_sinusoidal_to_harmonic` on float32 CUDA operands -> (harm_amp [B, T, 1],
+  harm_dist [B, T, K])."""
+  b, t, s = sin_amps.shape
+  harm_amp = torch.empty((b, t, 1), dtype=torch.float32, device=sin_amps.device)
+  harm_dist = torch.empty((b, t, n_harmonics), dtype=torch.float32, device=sin_amps.device)
+  _launch('ddsp_b200_sinusoidal_to_harmonic', sin_amps, sin_freqs, f0_hz, harm_amp,
+          harm_dist, b, t, s, n_harmonics, harmonic_width, sample_rate, int(normalize))
+  return harm_amp, harm_dist
+
+
+@on_operands_device
+def sinusoidal_to_harmonic(sin_amps, sin_freqs, f0_hz, harmonic_width=0.1,
+                           n_harmonics=100, sample_rate=16000, normalize=False):
+  """core.sinusoidal_to_harmonic (core.py:733-781): the amplitude and distribution of K
+  harmonics of f0 that sinusoids [B, T, S] weighted by a Gaussian in their frequency
+  distance relative to f0 amount to, (harm_amp [B, T, 1], harm_dist [B, T, K]).  Each
+  frame is evaluated on chip (csrc/consistency.cuh, mode C); the reference's
+  [B, T, K, S] tensors are never formed.  Routes to `autograd.SinusoidalToHarmonicFn`
+  when grad is enabled and an input requires it.
+
+  The inputs must have exactly these shapes (the reference would broadcast size-1
+  axes); other shapes, a zero harmonic_width and more than 4096 sinusoids raise before
+  any device work."""
+  b, t, s, k = _sinusoidal_to_harmonic_shapes(sin_amps, sin_freqs, f0_hz, harmonic_width,
+                                              n_harmonics)
+  a, f, f0 = torch_float32(sin_amps), torch_float32(sin_freqs), torch_float32(f0_hz)
+  cfg = (k, float(harmonic_width), float(sample_rate), bool(normalize))
+  if _requires_grad(a, f, f0):
+    from ddsp_b200 import autograd as _ag
+    return _ag.SinusoidalToHarmonicFn.apply(a, f, f0, *cfg)
+  return sinusoidal_to_harmonic_forward(a, f, f0, *cfg)
+
+
 @on_operands_device
 def normalize_harmonics(harmonic_distribution, f0_hz=None, sample_rate=None):
   """core.normalize_harmonics (core.py:894-907) on the controls kernel."""

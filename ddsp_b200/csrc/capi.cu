@@ -2248,6 +2248,76 @@ int ddsp_b200_comb_nll_backward(const float* f0, const float* f, const float* a,
   return 0;
 }
 
+// ---- core.sinusoidal_to_harmonic ---------------------------------------------------
+static int s2h_check(const char* name, int B, int T, int S, int K, float width,
+                     float sample_rate, int normalize, cons_::S2HParams* p, int64_t* rows) {
+  DDSP_REQUIRE(B >= 0 && T >= 0 && S >= 0 && K >= 0, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d T=%d S=%d K=%d", name, B, T, S, K);
+  DDSP_REQUIRE(width != 0.f, DDSP_B200_E_INVALID, "%s: harmonic_width must be nonzero",
+               name);
+  DDSP_REQUIRE(normalize == 0 || normalize == 1, DDSP_B200_E_INVALID,
+               "%s: normalize must be 0 or 1, got %d", name, normalize);
+  DDSP_REQUIRE(S <= cons_::kMaxStaged, DDSP_B200_E_UNSUPPORTED,
+               "%s: S=%d sinusoids exceed the %d supported", name, S, cons_::kMaxStaged);
+  int rc = cons_rows(name, B, T, rows);
+  if (rc) return rc;
+  p->S = S;
+  p->K = K;
+  p->width = width;
+  p->nyquist = sample_rate * 0.5f;
+  p->normalize = normalize;
+  return 0;
+}
+
+int ddsp_b200_sinusoidal_to_harmonic(const float* sin_amps, const float* sin_freqs,
+                                     const float* f0_hz, float* harm_amp, float* harm_dist,
+                                     int B, int T, int S, int K, float width,
+                                     float sample_rate, int normalize, void* stream) {
+  const bool empty = B == 0 || T == 0;
+  DDSP_REQUIRE(empty || (f0_hz && harm_amp && (S == 0 || (sin_amps && sin_freqs)) &&
+                         (K == 0 || harm_dist)),
+               DDSP_B200_E_INVALID, "sinusoidal_to_harmonic: null pointer");
+  cons_::S2HParams p;
+  int64_t rows = 0;
+  int rc = s2h_check("sinusoidal_to_harmonic", B, T, S, K, width, sample_rate, normalize, &p,
+                     &rows);
+  if (rc || rows == 0) return rc;
+  p.a = sin_amps; p.f = sin_freqs; p.f0 = f0_hz;
+  const size_t smem = sizeof(float) * (2 * (size_t)S + cons_::kThreads + 1);
+  rc = set_smem(cons_::sin_to_harm_kernel, smem, "sinusoidal_to_harmonic");
+  if (rc) return rc;
+  cons_::sin_to_harm_kernel<<<(unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream>>>(
+      p, harm_amp, harm_dist);
+  DDSP_CHECK_LAUNCH("sinusoidal_to_harmonic");
+  return 0;
+}
+
+int ddsp_b200_sinusoidal_to_harmonic_backward(
+    const float* sin_amps, const float* sin_freqs, const float* f0_hz, const float* grad_amp,
+    const float* grad_dist, float* d_sin_amps, float* d_sin_freqs, float* d_f0_hz, int B,
+    int T, int S, int K, float width, float sample_rate, int normalize, void* stream) {
+  const bool empty = B == 0 || T == 0;
+  DDSP_REQUIRE(empty || (f0_hz && grad_amp && d_f0_hz &&
+                         (S == 0 || (sin_amps && sin_freqs && d_sin_amps && d_sin_freqs)) &&
+                         (K == 0 || grad_dist)),
+               DDSP_B200_E_INVALID, "sinusoidal_to_harmonic_backward: null pointer");
+  cons_::S2HParams p;
+  int64_t rows = 0;
+  int rc = s2h_check("sinusoidal_to_harmonic_backward", B, T, S, K, width, sample_rate,
+                     normalize, &p, &rows);
+  if (rc || rows == 0) return rc;
+  p.a = sin_amps; p.f = sin_freqs; p.f0 = f0_hz;
+  const size_t smem =
+      sizeof(float) * (4 * (size_t)S + 4 * cons_::kHarmChunk + cons_::kThreads + 1);
+  rc = set_smem(cons_::sin_to_harm_backward_kernel, smem, "sinusoidal_to_harmonic_backward");
+  if (rc) return rc;
+  cons_::sin_to_harm_backward_kernel<<<(unsigned)rows, cons_::kThreads, smem,
+                                       (cudaStream_t)stream>>>(
+      p, grad_amp, grad_dist, d_sin_amps, d_sin_freqs, d_f0_hz);
+  DDSP_CHECK_LAUNCH("sinusoidal_to_harmonic_backward");
+  return 0;
+}
+
 #ifdef DDSP_NR_TIMING
 // measurement builds only (tools/noise_timing.py): the noise_ring phase counters of
 // the last launch, [kMaxSMs CTAs][32 warps][8 phases] cycles (rows past the grid stay 0)

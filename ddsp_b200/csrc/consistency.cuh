@@ -35,6 +35,32 @@
 // (out_c and d f0_c = -g_c / (D f0_c) sum_p a_p nu'(q) q, 0 at f0_c = 0), then a thread
 // per point sums over the candidates in ascending c:
 //   d a_p = sum_c g_c (nu_pc - out_c [D != 0]) / D,  d f_p = sum_c g_c a_p nu'_pc / (D f0_c).
+//
+// Mode C, sin_to_harm_kernel (core.sinusoidal_to_harmonic, core.py:733-781): for
+// sinusoids a[r, s], f[r, s] and one f0[r], with den = f0 (1e-7 where f0 = 0),
+//   q_ks = (f_s - f0 k) / den,  w_ks = exp(-(|q_ks| / width)^2),  k = 1..K,
+//   W_ks = w_ks / sw_k where normalize and sw_k = sum_s w_ks > 1, else w_ks,
+//   HA_k = sum_s W_ks a_s (0 where f0 k >= nyquist),  D = sum_k HA_k,
+//   harm_amp[r] = D,  harm_dist[r, k] = HA_k / Ds  (Ds = D, 1e-7 where D = 0).
+// One CTA per frame stages a and f; a thread per harmonic sums over the sinusoids (q
+// and w in the reference's float32 op order; the normalised sum as sum_s w a / sw).
+// D is the sum of the threads' partial sums, added by thread 0 in thread order.
+//
+// Mode C backward, sin_to_harm_backward_kernel: with upstream g_A and g_k,
+//   dHA_k = g_A + (g_k - [D != 0] sum_j g_j HA_j / Ds) / Ds  (0 where masked),
+//   the same as TensorFlow's g_k / Ds + g_A - sum_j g_j HA_j / Ds^2 without its inf - inf
+//   at a tiny D,
+//   alpha_k = dHA_k / sw_k, beta_k = HA_k before the mask where normalised, else
+//   alpha_k = dHA_k, beta_k = 0;  e_ks = alpha_k (a_s - beta_k) w_ks q_ks,
+//   d a_s = sum_k alpha_k w_ks,  d f_s = -2 / (width^2 den) sum_k e_ks,
+//   d f0 = 2 / (width^2 den) sum_ks e_ks (k + [f0 != 0] q_ks)
+// (the f0 k path, and the denominator's unless safe_divide took its constant).  A first
+// pass recomputes D, a second sum_j g_j HA_j / Ds (from the first kHarmChunk rows kept in
+// shared memory, later rows recomputed).  Then harmonics are taken in chunks of
+// kHarmChunk: a thread per harmonic writes alpha and beta to shared memory, then a
+// thread per sinusoid adds the chunk's terms to its running sums in ascending k.
+// Harmonics with alpha_k = 0 (every masked one) and pairs whose float32 weight is 0
+// add exactly 0 and are skipped.  No atomics: bit-reproducible.
 #pragma once
 #include "common.cuh"
 
@@ -44,6 +70,7 @@ namespace cons_ {
 constexpr int kThreads = 128;
 constexpr int kMaxStaged = 4096;   // components (mode A), candidates and points (mode B)
 constexpr int kChunk = 512;        // queries per shared-memory chunk of the mode A backward
+constexpr int kHarmChunk = 256;    // harmonics per shared-memory chunk of the mode C backward
 
 struct MixParams {
   const float* x;      // [R, Q]
@@ -61,6 +88,16 @@ struct CombParams {
   int C, P, G, W;
   float inv_scale;     // 1 / s
   float log_norm;      // log G + log s + log(2 pi) / 2
+};
+
+struct S2HParams {
+  const float* a;      // [R, S]
+  const float* f;      // [R, S]
+  const float* f0;     // [R]
+  int S, K;
+  float width;         // harmonic_width, nonzero
+  float nyquist;       // sample_rate / 2
+  int normalize;
 };
 
 // One query against the staged components: the shift j* and the sums
@@ -291,6 +328,180 @@ __global__ void __launch_bounds__(kThreads) comb_nll_backward_kernel(
     dar[i] = da;
     dfr[i] = dfs * A[i];
   }
+}
+
+// The sum of one value per thread, added by thread 0 in thread order; every thread gets
+// it.  red: kThreads + 1 floats.
+__device__ __forceinline__ float ordered_block_sum(float v, float* red) {
+  red[threadIdx.x] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float s = 0.f;
+    for (int i = 0; i < kThreads; ++i) s += red[i];
+    red[kThreads] = s;
+  }
+  __syncthreads();
+  return red[kThreads];
+}
+
+__device__ __forceinline__ void stage_sinusoids(const S2HParams& p, int64_t r, float* A,
+                                                float* F) {
+  const float* a = p.a + r * p.S;
+  const float* f = p.f + r * p.S;
+  for (int s = threadIdx.x; s < p.S; s += blockDim.x) {
+    A[s] = a[s];
+    F[s] = f[s];
+  }
+}
+
+// w_ks as the reference forms it: freqs_ratio = |(f - hf) / den|, exp(-(ratio / width)^2)
+__device__ __forceinline__ float s2h_weight(float f, float hf, float den, float width,
+                                            float* q) {
+  *q = (f - hf) / den;
+  const float u = fabsf(*q) / width;
+  return expf(-(u * u));
+}
+
+// Harmonic k's sum of weights sw and its amplitude before the Nyquist mask,
+// hp = sum_s W_ks a_s.
+struct S2HRow {
+  float sw, hp;
+};
+
+__device__ __forceinline__ S2HRow s2h_row(const S2HParams& p, float hf, float den,
+                                          const float* A, const float* F) {
+  float sw = 0.f, swa = 0.f, q;
+  for (int s = 0; s < p.S; ++s) {
+    const float w = s2h_weight(F[s], hf, den, p.width, &q);
+    sw += w;
+    swa = fmaf(w, A[s], swa);
+  }
+  return {sw, p.normalize && sw > 1.f ? swa / sw : swa};
+}
+
+// grid: one CTA per frame; smem: 2 S + kThreads + 1 floats
+__global__ void __launch_bounds__(kThreads) sin_to_harm_kernel(S2HParams p, float* harm_amp,
+                                                               float* harm_dist) {
+  extern __shared__ float sm[];
+  float* A = sm;
+  float* F = A + p.S;
+  float* red = F + p.S;
+  const int64_t r = blockIdx.x;
+  stage_sinusoids(p, r, A, F);
+  const float f0 = p.f0[r];
+  const float den = f0 == 0.f ? 1e-7f : f0;
+  __syncthreads();
+  float* dist = harm_dist + r * p.K;
+  float part = 0.f;
+  for (int k = threadIdx.x; k < p.K; k += blockDim.x) {
+    const float hf = f0 * (float)(k + 1);
+    const float ha = hf >= p.nyquist ? 0.f : s2h_row(p, hf, den, A, F).hp;
+    dist[k] = ha;     // HA_k until D is known; read back by this thread only
+    part += ha;
+  }
+  const float D = ordered_block_sum(part, red);
+  const float Ds = D == 0.f ? 1e-7f : D;
+  for (int k = threadIdx.x; k < p.K; k += blockDim.x) dist[k] = dist[k] / Ds;
+  if (threadIdx.x == 0) harm_amp[r] = D;
+}
+
+// grid: one CTA per frame; smem: 4 S + 4 kHarmChunk + kThreads + 1 floats
+__global__ void __launch_bounds__(kThreads) sin_to_harm_backward_kernel(
+    S2HParams p, const float* g_amp, const float* g_dist, float* d_a, float* d_f,
+    float* d_f0) {
+  extern __shared__ float sm[];
+  float* A = sm;
+  float* F = A + p.S;
+  float* ES = F + p.S;             // sum_k e_ks, per sinusoid
+  float* AS = ES + p.S;            // sum_k alpha_k w_ks
+  float* cSW = AS + p.S;           // first chunk's sw_k, kept from the first pass
+  float* cHP = cSW + kHarmChunk;   //   and hp_k
+  float* cAl = cHP + kHarmChunk;   // per harmonic of the chunk: alpha_k
+  float* cBe = cAl + kHarmChunk;   //   beta_k
+  float* red = cBe + kHarmChunk;
+  const int64_t r = blockIdx.x;
+  stage_sinusoids(p, r, A, F);
+  for (int s = threadIdx.x; s < p.S; s += blockDim.x) {
+    ES[s] = 0.f;
+    AS[s] = 0.f;
+  }
+  const float f0 = p.f0[r];
+  const float den = f0 == 0.f ? 1e-7f : f0;
+  __syncthreads();
+  const float* gd = g_dist + r * p.K;
+  float pd = 0.f;
+  for (int k = threadIdx.x; k < p.K; k += blockDim.x) {
+    const float hf = f0 * (float)(k + 1);
+    S2HRow h = {0.f, 0.f};
+    if (!(hf >= p.nyquist)) h = s2h_row(p, hf, den, A, F);
+    pd += h.hp;
+    if (k < kHarmChunk) {
+      cSW[k] = h.sw;
+      cHP[k] = h.hp;
+    }
+  }
+  const float D = ordered_block_sum(pd, red);
+  const float Ds = D == 0.f ? 1e-7f : D;
+  // dHA_k = g_A + (g_k - Gd) / Ds with Gd = sum_j g_j dist_j (0 where D = 0): the two
+  // 1 / Ds terms are combined before the division, and dist_j = HA_j / Ds keeps its
+  // precision when HA and D are tiny, so a small D cancels instead of giving inf - inf
+  float pg = 0.f;
+  if (D != 0.f) {
+    for (int k = threadIdx.x; k < p.K; k += blockDim.x) {
+      const float hf = f0 * (float)(k + 1);
+      if (hf >= p.nyquist) continue;
+      const float hp = k < kHarmChunk ? cHP[k] : s2h_row(p, hf, den, A, F).hp;
+      pg = fmaf(gd[k], hp / Ds, pg);
+    }
+  }
+  const float Gd = ordered_block_sum(pg, red);
+  const float ga = g_amp[r];
+  float pf = 0.f;
+  for (int k0 = 0; k0 < p.K; k0 += kHarmChunk) {
+    const int n = min(kHarmChunk, p.K - k0);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+      const float hf = f0 * (float)(k0 + i + 1);
+      float al = 0.f, be = 0.f;
+      if (!(hf >= p.nyquist)) {
+        const S2HRow h = k0 == 0 ? S2HRow{cSW[i], cHP[i]} : s2h_row(p, hf, den, A, F);
+        const float dha = ga + (gd[k0 + i] - Gd) / Ds;
+        const bool sel = p.normalize && h.sw > 1.f;
+        al = sel ? dha / h.sw : dha;
+        be = sel ? h.hp : 0.f;
+      }
+      cAl[i] = al;
+      cBe[i] = be;
+    }
+    __syncthreads();
+    for (int s = threadIdx.x; s < p.S; s += blockDim.x) {
+      const float a = A[s], fs = F[s];
+      float es = ES[s], as = AS[s];
+      for (int i = 0; i < n; ++i) {
+        const float al = cAl[i];
+        if (al == 0.f) continue;
+        const float kf = (float)(k0 + i + 1);
+        float q;
+        const float w = s2h_weight(fs, f0 * kf, den, p.width, &q);
+        if (w == 0.f) continue;     // adds exactly 0 (alpha may be inf where D is tiny)
+        const float e = al * (a - cBe[i]) * w * q;
+        es += e;
+        as = fmaf(al, w, as);
+        pf = fmaf(e, f0 != 0.f ? kf + q : kf, pf);
+      }
+      ES[s] = es;
+      AS[s] = as;
+    }
+    __syncthreads();
+  }
+  const float F0 = ordered_block_sum(pf, red);
+  const float k2 = 2.f / (p.width * p.width);
+  float* dfr = d_f + r * p.S;
+  float* dar = d_a + r * p.S;
+  for (int s = threadIdx.x; s < p.S; s += blockDim.x) {
+    dfr[s] = -k2 * ES[s] / den;
+    dar[s] = AS[s];
+  }
+  if (threadIdx.x == 0) d_f0[r] = k2 * F0 / den;
 }
 
 }  // namespace cons_

@@ -620,6 +620,34 @@ int ddsp_b200_comb_nll_backward(const float* f0, const float* f, const float* a,
                                 int B, int T, int C, int P, int G, float scale,
                                 void* stream);
 
+/* core.sinusoidal_to_harmonic (core.py:733-781): for sinusoids sin_amps and sin_freqs
+ * [B,T,S] and f0_hz [B,T,1], per frame with den = f0 (1e-7 where f0 = 0) and k = 1..K,
+ *   w_ks = exp(-(|(sin_freqs_s - f0 k) / den| / width)^2),
+ *   W_ks = w_ks / sum_s w_ks where normalize and that sum is > 1, else w_ks,
+ *   HA_k = sum_s W_ks sin_amps_s, 0 where f0 k >= sample_rate / 2,
+ *   harm_amp [B,T,1] = sum_k HA_k,  harm_dist [B,T,K] = HA_k / harm_amp
+ *   (1e-7 for a zero harm_amp).
+ * width must be nonzero (0 is E_INVALID; a negative width acts as its magnitude),
+ * normalize 0 or 1.  S <= 4096 sinusoids are staged per frame; more is E_UNSUPPORTED.
+ * K is unbounded.  B*T <= 2^31 - 1.  No workspace.  B = 0 or T = 0 returns before any
+ * launch and writes nothing (the pointers may then be null).  Otherwise one launch
+ * writes every output: S = 0 gives harm_amp = 0 and harm_dist = 0; K = 0 gives
+ * harm_amp = 0.  Arrays of zero elements may be null.
+ * backward: for grad_amp [B,T,1] and grad_dist [B,T,K], d_sin_amps and d_sin_freqs
+ * [B,T,S] and d_f0_hz [B,T,1], all written, zeros where nothing contributes (K = 0 or
+ * S = 0).  TensorFlow's gradient: none through a safe_divide denominator that took its
+ * 1e-7 (f0 = 0, harm_amp = 0), sign(0) = 0 in |q|, none to the branch of normalize's
+ * where that was not taken, none through harmonics at or above Nyquist.  Every sum in a
+ * fixed order, no atomics: bit-reproducible. */
+int ddsp_b200_sinusoidal_to_harmonic(const float* sin_amps, const float* sin_freqs,
+                                     const float* f0_hz, float* harm_amp, float* harm_dist,
+                                     int B, int T, int S, int K, float width,
+                                     float sample_rate, int normalize, void* stream);
+int ddsp_b200_sinusoidal_to_harmonic_backward(
+    const float* sin_amps, const float* sin_freqs, const float* f0_hz, const float* grad_amp,
+    const float* grad_dist, float* d_sin_amps, float* d_sin_freqs, float* d_f0_hz, int B,
+    int T, int S, int K, float width, float sample_rate, int normalize, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

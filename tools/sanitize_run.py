@@ -79,8 +79,16 @@ xs = torch.randn(2, 3000, device='cuda', requires_grad=True)
 core.sinc_filter(xs, sc, window_size=64).square().mean().backward()
 scs = (0.5 * torch.rand(1, 1, 1, device='cuda')).requires_grad_(True)
 core.sinc_filter(xs, scs, window_size=512, padding='valid').square().mean().backward()
+# sinusoidal_to_harmonic forward and backward: two harmonic chunks, both normalize modes
+sa = torch.rand(2, 5, 37, device='cuda', requires_grad=True)
+sfq = (4000.0 * torch.rand(2, 5, 37, device='cuda')).requires_grad_(True)
+sf0 = (80.0 + 300.0 * torch.rand(2, 5, 1, device='cuda')).requires_grad_(True)
+for norm in (False, True):
+  ha, hd = core.sinusoidal_to_harmonic(sa, sfq, sf0, n_harmonics=300, normalize=norm)
+  (ha.sum() + hd.square().sum()).backward()
 torch.cuda.synchronize()
 assert torch.isfinite(sc.grad).all() and torch.isfinite(scs.grad).all()
+assert torch.isfinite(sa.grad).all() and torch.isfinite(sf0.grad).all()
 assert torch.isfinite(h2).all() and torch.isfinite(r4).all() and torch.isfinite(ob).all()
 assert torch.isfinite(xa.grad).all() and torch.isfinite(hi.grad).all() and torch.isfinite(f0g.grad).all()
 assert torch.isfinite(e).all() and torch.isfinite(f).all() and torch.isfinite(g).all()
