@@ -100,12 +100,15 @@ SIGNATURES = {
     'ddsp_b200_oscillator_bank_workspace': (_sz, [_i, _i, _i]),
     'ddsp_b200_oscillator_bank':
         (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
+    'ddsp_b200_oscillator_bank_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp]),
     'ddsp_b200_resample': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
     'ddsp_b200_fft_convolve_lti_workspace': (_sz, [_i, _i, _i, _i]),
     'ddsp_b200_fft_convolve_lti':
         (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
     'ddsp_b200_angular_cumsum':
         (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
+    'ddsp_b200_angular_cumsum_backward': (_i, [_vp, _vp, _i, _i, _i, _vp]),
     'ddsp_b200_oscillator_bank_tf_sequential':
         (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _i, _i, _vp]),
     'ddsp_b200_sinusoidal_workspace': (_sz, [_i, _i, _i]),

@@ -13,6 +13,10 @@ kernels, exposed as `torch.autograd.Function`s:
     oscillator bank (`Sinusoidal.get_signal`, the synthesizer of
     `models/inverse_synthesis.py:84-105`; d frequencies only when they require
     grad); `core.sinusoidal_synthesis` routes to it under grad;
+  * `OscillatorBankFn` / `AngularCumsumFn` - the stand-alone oscillator bank on
+    audio-rate envelopes (d frequency and d amplitude envelopes) and the phase
+    accumulation, routed to by `core.oscillator_bank` / `core.angular_cumsum` under
+    grad;
   * `WavetableSynthesisFn` - d f0, d amplitudes and d wavetables of the wavetable
     synthesizer (`Wavetable.get_signal`); `core.wavetable_synthesis` routes to it
     under grad;
@@ -399,6 +403,52 @@ class SinusoidalSynthesisFn(torch.autograd.Function):
                  *core._workspace('ddsp_b200_sinusoidal_backward_workspace',
                                   amplitudes.device, b, f, k))
     return d_freq, d_amp if ctx.needs_input_grad[1] else None, None, None, None
+
+
+class OscillatorBankFn(torch.autograd.Function):
+  """core.oscillator_bank (core.py:911-962) on audio-rate envelopes [B, N, K],
+  differentiable in frequency and amplitude envelopes.  One call of
+  `ddsp_b200_oscillator_bank_backward` (csrc/oscbank.cuh) computes the gradients asked
+  for from the saved inputs, on the forward's exact phase; the Nyquist mask has
+  subgradient 0 (tf.where)."""
+
+  @staticmethod
+  def forward(ctx, f, a, sample_rate, sum_sinusoids):
+    ctx.save_for_backward(f, a)
+    ctx.cfg = (sample_rate, sum_sinusoids)
+    return core.oscillator_bank_forward(f, a, sample_rate, sum_sinusoids)
+
+  @staticmethod
+  def backward(ctx, grad):
+    f, a = ctx.saved_tensors
+    sample_rate, sum_sinusoids = ctx.cfg
+    b, n, k = f.shape
+    g = grad.contiguous().to(torch.float32)
+    want = ctx.needs_input_grad
+    d_f = torch.empty_like(f) if want[0] else None
+    d_a = torch.empty_like(a) if want[1] else None
+    core._launch('ddsp_b200_oscillator_bank_backward', f, a, g, d_f, d_a, b, n, k,
+                 sample_rate, int(sum_sinusoids))
+    return d_f, d_a, None, None
+
+
+class AngularCumsumFn(torch.autograd.Function):
+  """core.angular_cumsum (core.py:799-866) on [batch, time, ...], differentiable in the
+  angular frequency: the gradient is the reverse running sum of the upstream gradient
+  along time (`ddsp_b200_angular_cumsum_backward`)."""
+
+  @staticmethod
+  def forward(ctx, x):
+    ctx.shape = tuple(x.shape)
+    return core.angular_cumsum_forward(x)
+
+  @staticmethod
+  def backward(ctx, grad):
+    b, n, c = core._bnc(ctx.shape)
+    g = grad.contiguous().to(torch.float32)
+    d_x = torch.empty(ctx.shape, dtype=torch.float32, device=g.device)
+    core._launch('ddsp_b200_angular_cumsum_backward', g, d_x, b, n, c)
+    return d_x
 
 
 class WavetableSynthesisFn(torch.autograd.Function):

@@ -575,23 +575,43 @@ def angular_cumsum(angular_frequency, chunk_size: int = 1000,
   [0, 2 pi] the reference documents.  tf_sequential=True reproduces
   the reference's own float32 arithmetic in its own order (chunks of
   `chunk_size`, mod-2pi stitching) - a debug mode for comparing against
-  TensorFlow, one thread per (batch, channel)."""
+  TensorFlow, one thread per (batch, channel).
+
+  Routes to `autograd.AngularCumsumFn` when grad is enabled and the input
+  requires it; tf_sequential=True is forward-only and raises NotImplementedError
+  there."""
   x = torch_float32(angular_frequency)
-  shape = tuple(x.shape)
-  if len(shape) < 2:
-    raise ValueError(f'angular_frequency must be [batch, time, ...], got {list(shape)}.')
-  b, n = shape[0], shape[1]
+  if len(x.shape) < 2:
+    raise ValueError(f'angular_frequency must be [batch, time, ...], got {list(x.shape)}.')
+  if _requires_grad(x):
+    if tf_sequential:
+      raise NotImplementedError('angular_cumsum: tf_sequential=True is a forward-only '
+                                'debug mode; it has no backward.')
+    from ddsp_b200 import autograd as _ag
+    return _ag.AngularCumsumFn.apply(x)
+  return angular_cumsum_forward(x, chunk_size, tf_sequential)
+
+
+def _bnc(shape):
+  """(B, N, C) of a [batch, time, ...] shape, C the product of the trailing axes
+  (at least 1)."""
   c = 1
   for d in shape[2:]:
     c *= int(d)
-  x3 = x.reshape(b, n, max(c, 1))
+  return shape[0], shape[1], max(c, 1)
+
+
+def angular_cumsum_forward(x, chunk_size=1000, tf_sequential=False):
+  """`ddsp_b200_angular_cumsum` on a float32 CUDA tensor [batch, time, ...]."""
+  shape = tuple(x.shape)
+  b, n, c = _bnc(shape)
+  x3 = x.reshape(b, n, c)
   out = torch.empty_like(x3)
   if tf_sequential:
-    _launch('ddsp_b200_angular_cumsum', x3, out, b, n, max(c, 1), int(chunk_size), 2,
-            None, 0)
+    _launch('ddsp_b200_angular_cumsum', x3, out, b, n, c, int(chunk_size), 2, None, 0)
   else:
-    _launch('ddsp_b200_angular_cumsum', x3, out, b, n, max(c, 1), int(chunk_size), 0,
-            *_workspace('ddsp_b200_oscillator_bank_workspace', x3.device, b, n, max(c, 1)))
+    _launch('ddsp_b200_angular_cumsum', x3, out, b, n, c, int(chunk_size), 0,
+            *_workspace('ddsp_b200_oscillator_bank_workspace', x3.device, b, n, c))
   return out.reshape(shape)
 
 
@@ -607,7 +627,11 @@ def oscillator_bank(frequency_envelopes, amplitude_envelopes,
   fixed point) whatever `use_angular_cumsum` says - both reference modes
   approximate this.  phase_mode='tf_sequential': the reference's own float32
   arithmetic in its own order - tf.cumsum, or angular_cumsum (chunks of 1000)
-  when use_angular_cumsum - reproducing TensorFlow's phase error (debug)."""
+  when use_angular_cumsum - reproducing TensorFlow's phase error (debug).
+
+  Routes to `autograd.OscillatorBankFn` when grad is enabled and an input
+  requires it (both `sum_sinusoids` values); phase_mode='tf_sequential' is
+  forward-only and raises NotImplementedError there."""
   if phase_mode not in ('exact', 'tf_sequential'):
     raise ValueError(f"phase_mode must be 'exact' or 'tf_sequential', got {phase_mode!r}.")
   sf, sa = _shape(frequency_envelopes), _shape(amplitude_envelopes)
@@ -617,12 +641,23 @@ def oscillator_bank(frequency_envelopes, amplitude_envelopes,
   b, n, k = sf
   f = torch_float32(frequency_envelopes)
   a = torch_float32(amplitude_envelopes)
-  _no_grad_path('oscillator_bank', f, a)
+  if _requires_grad(f, a):
+    if phase_mode == 'tf_sequential':
+      raise NotImplementedError("oscillator_bank: phase_mode='tf_sequential' is a "
+                                'forward-only debug mode; it has no backward.')
+    from ddsp_b200 import autograd as _ag
+    return _ag.OscillatorBankFn.apply(f, a, float(sample_rate), bool(sum_sinusoids))
   if phase_mode == 'tf_sequential':
     wavs = torch.empty((b, n, k), dtype=torch.float32, device=f.device)
     _launch('ddsp_b200_oscillator_bank_tf_sequential', f, a, wavs, b, n, k,
             float(sample_rate), int(bool(use_angular_cumsum)), 1000)
     return wavs.sum(-1) if sum_sinusoids else wavs
+  return oscillator_bank_forward(f, a, sample_rate, sum_sinusoids)
+
+
+def oscillator_bank_forward(f, a, sample_rate, sum_sinusoids):
+  """`ddsp_b200_oscillator_bank` (exact phase) on float32 CUDA envelopes [B, N, K]."""
+  b, n, k = f.shape
   out = torch.empty((b, n) if sum_sinusoids else (b, n, k), dtype=torch.float32,
                     device=f.device)
   _launch('ddsp_b200_oscillator_bank', f, a, out, b, n, k, float(sample_rate),

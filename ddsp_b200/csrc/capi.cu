@@ -1183,6 +1183,38 @@ int ddsp_b200_oscillator_bank(const float* frequency_envelopes,
   return 0;
 }
 
+// One cluster per (b, tile of kObbLanes oscillators) along x, batch along y.
+static dim3 oscbank_backward_grid(int B, int K) {
+  return dim3((unsigned)(kObbCluster * ((K + kObbLanes - 1) / kObbLanes)), (unsigned)B);
+}
+
+int ddsp_b200_oscillator_bank_backward(const float* frequency_envelopes,
+                                       const float* amplitude_envelopes, const float* grad,
+                                       float* d_frequency_envelopes,
+                                       float* d_amplitude_envelopes, int B, int N, int K,
+                                       float sample_rate, int sum_sinusoids, void* stream) {
+  const bool empty = B == 0 || N == 0 || K == 0;
+  DDSP_REQUIRE(empty || (frequency_envelopes && amplitude_envelopes && grad),
+               DDSP_B200_E_INVALID, "oscillator_bank_backward: null pointer");
+  DDSP_REQUIRE(B >= 0 && N >= 0 && K >= 0, DDSP_B200_E_INVALID,
+               "oscillator_bank_backward: bad shape B=%d N=%d K=%d", B, N, K);
+  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
+               "oscillator_bank_backward: sample_rate must be positive");
+  DDSP_REQUIRE(sum_sinusoids == 0 || sum_sinusoids == 1, DDSP_B200_E_INVALID,
+               "oscillator_bank_backward: sum_sinusoids must be 0 or 1, got %d",
+               sum_sinusoids);
+  if (empty || (!d_frequency_envelopes && !d_amplitude_envelopes)) return 0;
+  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
+               "oscillator_bank_backward: B=%d exceeds the 65535 grid limit", B);
+  auto kernel = sum_sinusoids ? oscbank_backward<kObbSum> : oscbank_backward<kObbFull>;
+  kernel<<<oscbank_backward_grid(B, K), kObbLanes * kObbWarps, 0, (cudaStream_t)stream>>>(
+      frequency_envelopes, amplitude_envelopes, grad, d_frequency_envelopes,
+      d_amplitude_envelopes, N, K, 1.0 / (double)sample_rate, sample_rate * 0.5f,
+      6.283185307179586 / (double)sample_rate);
+  DDSP_CHECK_LAUNCH("oscillator_bank_backward");
+  return 0;
+}
+
 size_t ddsp_b200_fft_convolve_lti_workspace(int B, int N, int S, int ir_batch) {
   if (B <= 0 || N <= 0 || S <= 0 || (ir_batch != 1 && ir_batch != B)) return 0;
   const lc::Geom g = lc::geom(N, S);
@@ -1291,6 +1323,23 @@ int ddsp_b200_angular_cumsum(const float* angular_frequency, float* phase, int B
   oscbank_phase_out<<<grid, kObThreads, 0, st>>>(angular_frequency, sums, phase, N, C,
                                                 n_chunks, inv_two_pi);
   DDSP_CHECK_LAUNCH("angular_cumsum(apply)");
+  return 0;
+}
+
+int ddsp_b200_angular_cumsum_backward(const float* grad, float* d_angular_frequency, int B,
+                                      int N, int C, void* stream) {
+  const bool empty = B == 0 || N == 0 || C == 0;
+  DDSP_REQUIRE(empty || (grad && d_angular_frequency), DDSP_B200_E_INVALID,
+               "angular_cumsum_backward: null pointer");
+  DDSP_REQUIRE(B >= 0 && N >= 0 && C >= 0, DDSP_B200_E_INVALID,
+               "angular_cumsum_backward: bad shape B=%d N=%d C=%d", B, N, C);
+  if (empty) return 0;
+  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
+               "angular_cumsum_backward: B=%d exceeds the 65535 grid limit", B);
+  oscbank_backward<kObbCumsum>
+      <<<oscbank_backward_grid(B, C), kObbLanes * kObbWarps, 0, (cudaStream_t)stream>>>(
+          nullptr, nullptr, grad, d_angular_frequency, nullptr, N, C, 0.0, 0.f, 1.0);
+  DDSP_CHECK_LAUNCH("angular_cumsum_backward");
   return 0;
 }
 

@@ -8,6 +8,8 @@
 // k (the contiguous axis), so every global access is coalesced; the path is
 // HBM-bound: f is read twice, amp once.
 #pragma once
+#include <cooperative_groups.h>
+
 #include "common.cuh"
 
 namespace ddsp {
@@ -114,6 +116,127 @@ oscbank_phase_out(const float* __restrict__ f, const unsigned long long* __restr
       *op = (float)((double)ph * 5.421010862427522e-20 * 6.283185307179586);   // 2^-64 turns -> rad
     }
   }
+}
+
+// ---- backward (TensorFlow's gradients of core.py:911-962 and 799-866) ----------
+//   phi_t = (2 pi / sr) sum_{u<=t} f_u  (the forward's exact fixed-point phase),
+//   m = [f < sr/2] (the forward's float32 decision; the mask passes no gradient):
+//   d a[t,k] = g m sin(phi),   d f[t,k] = (2 pi / sr) sum_{u>=t} g_u a_u m_u cos(phi_u);
+//   angular_cumsum: d omega[t] = sum_{u>=t} g_u (floormod has derivative 1).
+// One cluster of kObbCluster CTAs per (b, tile of 32 oscillators); lane = oscillator,
+// so every access is a coalesced row of 32 floats.  The cluster's 128 warps split time
+// into contiguous segments, one per warp, in (rank, warp) order.  Segment totals cross
+// warps through shared memory and CTAs through distributed shared memory, each added in
+// a fixed order, so no workspace, atomic or memset is needed and the result is
+// bit-reproducible:
+//   1. the segment's fixed-point phase total (u64, exact); exchange -> phase at the
+//      segment start;
+//   2. walk forward: d a, and the segment total of g a m cos(phi) in double;
+//      exchange -> suffix of the later segments;
+//   3. walk backward from the segment's end phase (ph -= fix(f) is exact), adding
+//      g a m cos(phi) in double; d f = float((2 pi / sr) * suffix), rounded once.
+// The phase is the forward's: the same turns_to_fix64 terms, rounded to 2^-32 turn, and
+// sin(phi) is the forward's sinpif, so d a is the gradient of the audio it produced and
+// does not depend on whether d f is asked for.  Without d f, step 2's sum and step 3
+// are skipped (no cosine); without d a, nothing is written in step 2.  KIND: SUM (g is [B, N]),
+// FULL (g is [B, N, K]) or CUMSUM (angular_cumsum: no phase, d omega is written as d f).
+constexpr int kObbLanes = 32;
+constexpr int kObbWarps = 16;
+constexpr int kObbCluster = 8;                       // the portable cluster size
+constexpr int kObbSegs = kObbWarps * kObbCluster;    // time segments per (b, tile)
+enum { kObbSum = 0, kObbFull = 1, kObbCumsum = 2 };
+
+template <int KIND>
+__global__ void __cluster_dims__(kObbCluster, 1, 1) __launch_bounds__(kObbLanes * kObbWarps)
+oscbank_backward(const float* __restrict__ f, const float* __restrict__ a,
+                 const float* __restrict__ g, float* __restrict__ df,
+                 float* __restrict__ da, int N, int K, double inv_sr, float nyquist,
+                 double scale) {
+  namespace cg = cooperative_groups;
+  cg::cluster_group cluster = cg::this_cluster();
+  __shared__ unsigned long long ph_seg[kObbWarps][kObbLanes], ph_cta[kObbLanes];
+  __shared__ double s_seg[kObbWarps][kObbLanes], s_cta[kObbLanes];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int rank = (int)cluster.block_rank();
+  const int b = blockIdx.y;
+  const int k = (blockIdx.x / kObbCluster) * kObbLanes + lane;
+  const bool live = k < K;
+  const int len = (N + kObbSegs - 1) / kObbSegs;
+  const int t0 = min(N, (rank * kObbWarps + w) * len);
+  const int t1 = t0 + min(len, N - t0);
+  const size_t row0 = (size_t)b * N;
+  // the term of d f at sample t, with the phase ph (inclusive of t)
+  auto term = [&](int t, unsigned long long ph) -> double {
+    const size_t i = (row0 + t) * K + k;
+    const float gv = g[KIND == kObbSum ? row0 + t : i];
+    if (KIND == kObbCumsum) return (double)gv;
+    const float fv = f[i];
+    const uint32_t p32 = (uint32_t)((ph + 0x80000000ull) >> 32);
+    const float c = cospif((float)(int)p32 * 4.656612873077393e-10f);
+    return (fv >= nyquist) ? 0.0 : (double)(gv * (a[i] * c));
+  };
+
+  unsigned long long ph = 0;     // phase before the segment, then after it
+  if (KIND != kObbCumsum) {
+    unsigned long long tot = 0;
+    if (live)
+      for (int t = t0; t < t1; ++t)
+        tot += turns_to_fix64((double)f[(row0 + t) * K + k] * inv_sr);
+    ph_seg[w][lane] = tot;
+    __syncthreads();
+    if (w == 0) {
+      unsigned long long c = 0;
+      for (int v = 0; v < kObbWarps; ++v) c += ph_seg[v][lane];
+      ph_cta[lane] = c;
+    }
+    cluster.sync();
+    for (int q = 0; q < rank; ++q) ph += cluster.map_shared_rank(&ph_cta[0], q)[lane];
+    for (int v = 0; v < w; ++v) ph += ph_seg[v][lane];
+  }
+
+  double tot = 0.0;
+  if (live) {
+    if (KIND == kObbCumsum) {
+      for (int t = t0; t < t1; ++t) tot += term(t, 0);
+    } else if (da != nullptr || df != nullptr) {
+      for (int t = t0; t < t1; ++t) {
+        const size_t i = (row0 + t) * K + k;
+        ph += turns_to_fix64((double)f[i] * inv_sr);
+        if (da != nullptr) {
+          const uint32_t p32 = (uint32_t)((ph + 0x80000000ull) >> 32);
+          const float s = sinpif((float)(int)p32 * 4.656612873077393e-10f);
+          da[i] = (f[i] >= nyquist) ? 0.f : g[KIND == kObbSum ? row0 + t : i] * s;
+        }
+        if (df != nullptr) tot += term(t, ph);
+      }
+    }
+  }
+  if (df == nullptr) {
+    cluster.sync();              // no CTA leaves while another reads its ph_cta
+    return;
+  }
+
+  s_seg[w][lane] = tot;
+  __syncthreads();
+  if (w == 0) {
+    double c = 0.0;
+    for (int v = 0; v < kObbWarps; ++v) c += s_seg[v][lane];
+    s_cta[lane] = c;
+  }
+  cluster.sync();
+  double acc = 0.0;              // the later segments, nearest last
+  for (int q = kObbCluster - 1; q > rank; --q)
+    acc += cluster.map_shared_rank(&s_cta[0], q)[lane];
+  for (int v = kObbWarps - 1; v > w; --v) acc += s_seg[v][lane];
+  if (live) {
+    for (int t = t1 - 1; t >= t0; --t) {
+      const size_t i = (row0 + t) * K + k;
+      acc += term(t, ph);
+      df[i] = (float)(acc * scale);
+      if (KIND != kObbCumsum) ph -= turns_to_fix64((double)f[i] * inv_sr);
+    }
+  }
+  cluster.sync();                // no CTA leaves while another reads its s_cta
 }
 
 // Debug mode `tf_sequential`: the reference's own float32 arithmetic, in its own

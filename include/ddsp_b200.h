@@ -325,6 +325,24 @@ int ddsp_b200_oscillator_bank(const float* frequency_envelopes,
                               int N, int K, float sample_rate, int sum_sinusoids,
                               void* workspace, size_t workspace_bytes,
                               void* stream);
+/* Backward of ddsp_b200_oscillator_bank for grad [B,N] (sum_sinusoids = 1) or [B,N,K]
+ * (0): TensorFlow's gradients of core.py:911-962.  With m = [f < sr/2] (the forward's
+ * float32 mask, which passes no gradient) and phi_t = (2 pi / sr) sum_{u<=t} f_u (the
+ * forward's exact phase, bit for bit):
+ *   d_amplitude_envelopes[t,k] = g m sin(phi_t),
+ *   d_frequency_envelopes[t,k] = (2 pi / sr) sum_{u>=t} g_u a_u m_u cos(phi_u)
+ * (the suffix summed in double, rounded once).  use_angular_cumsum does not change the
+ * gradient.  Each gradient is skipped when its pointer is NULL (d_frequency_envelopes =
+ * NULL skips the suffix scan and the cosine); d_amplitude_envelopes does not depend on
+ * whether d_frequency_envelopes is asked for.  No workspace and no atomics: one
+ * thread-block cluster per (b, 32 oscillators) exchanges segment totals in distributed
+ * shared memory, so both gradients are bit-reproducible.  Checks as the forward's, plus
+ * sum_sinusoids in {0, 1}; B, N or K = 0 is a no-op (NULL pointers allowed then). */
+int ddsp_b200_oscillator_bank_backward(const float* frequency_envelopes,
+                                       const float* amplitude_envelopes, const float* grad,
+                                       float* d_frequency_envelopes,
+                                       float* d_amplitude_envelopes, int B, int N, int K,
+                                       float sample_rate, int sum_sinusoids, void* stream);
 
 /* core.fft_convolve (core.py:1382-1473) with ONE impulse response per item of any
  * length (the LTI case: effects.Reverb, effects.py:103-117, 48000 taps): uniformly
@@ -358,6 +376,12 @@ int ddsp_b200_fft_convolve_lti(const float* audio, const float* impulse_response
 int ddsp_b200_angular_cumsum(const float* angular_frequency, float* phase, int B,
                              int N, int C, int chunk_size, int mode,
                              void* workspace, size_t workspace_bytes, void* stream);
+/* Backward of ddsp_b200_angular_cumsum (mode 0) for grad [B,N,C]: floormod has
+ * derivative 1, so d_angular_frequency[t] = sum_{u>=t} grad[u] along N, summed in
+ * double and rounded once.  No workspace, no atomics (the oscillator-bank backward's
+ * cluster scan); B, N or C = 0 is a no-op (NULL pointers allowed then). */
+int ddsp_b200_angular_cumsum_backward(const float* grad, float* d_angular_frequency, int B,
+                                      int N, int C, void* stream);
 int ddsp_b200_oscillator_bank_tf_sequential(const float* frequency_envelopes,
                                             const float* amplitude_envelopes,
                                             float* out, int B, int N, int K,

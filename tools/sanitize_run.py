@@ -86,7 +86,17 @@ sf0 = (80.0 + 300.0 * torch.rand(2, 5, 1, device='cuda')).requires_grad_(True)
 for norm in (False, True):
   ha, hd = core.sinusoidal_to_harmonic(sa, sfq, sf0, n_harmonics=300, normalize=norm)
   (ha.sum() + hd.square().sum()).backward()
+# oscillator_bank backward (both sum_sinusoids values, N past the 128 time segments)
+# and angular_cumsum backward
+obf = (200 + 9000 * torch.rand(2, 700, 37, device='cuda')).requires_grad_(True)
+oba = torch.rand(2, 700, 37, device='cuda', requires_grad=True)
+for ss in (True, False):
+  core.oscillator_bank(obf, oba, sum_sinusoids=ss).square().mean().backward()
+omg = om.clone().requires_grad_(True)
+core.angular_cumsum(omg).square().mean().backward()
 torch.cuda.synchronize()
+assert torch.isfinite(obf.grad).all() and torch.isfinite(oba.grad).all()
+assert torch.isfinite(omg.grad).all()
 assert torch.isfinite(sc.grad).all() and torch.isfinite(scs.grad).all()
 assert torch.isfinite(sa.grad).all() and torch.isfinite(sf0.grad).all()
 assert torch.isfinite(h2).all() and torch.isfinite(r4).all() and torch.isfinite(ob).all()
