@@ -77,6 +77,8 @@ SIGNATURES = {
         (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
     'ddsp_b200_harmonic_controls_backward':
         (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp]),
+    'ddsp_b200_harmonic_controls_vjp':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp]),
     'ddsp_b200_noise_controls_backward': (_i, [_vp, _vp, _vp, _i64, _f, _vp]),
     'ddsp_b200_filtered_noise_backward':
         (_i, [_vp, _vp, _u64, _u64, _vp, _i, _i, _i, _i, _i, _vp]),

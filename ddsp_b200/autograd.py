@@ -9,6 +9,14 @@ kernels, exposed as `torch.autograd.Function`s:
     phase path, `models/inverse_synthesis.py:84-117`; computed only when f0
     requires grad);
   * `FilteredNoiseFn`      - d magnitudes (the filter is linear in them);
+    `core.harmonic_synthesis` / `core.filtered_noise` route to these two under grad
+    (DESIGN.md section 3.15 has the table of which shape goes where);
+  * `HarmonicControlsFn` / `NoiseControlsFn` - `Harmonic.get_controls` and
+    `FilteredNoise.get_controls` for any upstream gradient (a loss on the controls
+    themselves as well as the synthesizer's), one backward launch each; routed to by
+    `core.harmonic_controls` / `core.noise_controls` under grad.  With them the
+    Processor API trains: `ProcessorGroup.get_controls` + `get_signal` and
+    `group(features, return_outputs_dict=True)`;
   * `SinusoidalSynthesisFn` - d amplitudes and d frequencies of the frame-rate
     oscillator bank (`Sinusoidal.get_signal`, the synthesizer of
     `models/inverse_synthesis.py:84-105`; d frequencies only when they require
@@ -159,6 +167,64 @@ class DecoderFn(torch.autograd.Function):
                                             normalize_below_nyquist=nyq)
       d_f0 = _harmonic_d_f0(f0_hz, a_ctl, h_ctl, g, n_samples, sample_rate, method)
     return (d_amps, d_hd, d_f0, d_mags) + (None,) * 9
+
+
+class HarmonicControlsFn(torch.autograd.Function):
+  """core.harmonic_controls (Harmonic.get_controls, synths.py:94-121), differentiable
+  in the raw amplitudes and harmonic distribution for any upstream gradient on the two
+  controls: one backward launch of `ddsp_b200_harmonic_controls_vjp`
+  (csrc/controls_bwd.cuh).  f0_hz gets none: the Nyquist mask is piecewise constant
+  (tf.where)."""
+
+  @staticmethod
+  def forward(ctx, amplitudes, harmonic_distribution, f0_hz, sample_rate, scale,
+              normalize_below_nyquist):
+    ctx.save_for_backward(amplitudes, harmonic_distribution, f0_hz)
+    ctx.cfg = (float(sample_rate), bool(scale), bool(normalize_below_nyquist))
+    ctx.set_materialize_grads(False)
+    return core.harmonic_controls(amplitudes, harmonic_distribution, f0_hz, *ctx.cfg)
+
+  @staticmethod
+  def backward(ctx, d_amplitudes, d_hd):
+    amps, hd, f0_hz = ctx.saved_tensors
+    sample_rate, scale, nyq = ctx.cfg
+    b, f, k = hd.shape
+    if d_amplitudes is not None:
+      d_amplitudes = d_amplitudes.contiguous().to(torch.float32)
+    if d_hd is not None:
+      d_hd = d_hd.contiguous().to(torch.float32)
+    d_amps_raw = torch.empty_like(amps)
+    d_hd_raw = torch.empty_like(hd)
+    flags = (_lib.CTL_SCALE if scale else 0) | (_lib.CTL_NYQUIST if nyq else 0)
+    core._launch('ddsp_b200_harmonic_controls_vjp', amps, hd, f0_hz, d_amplitudes, d_hd,
+                 d_amps_raw, d_hd_raw, b, f, k, sample_rate, flags)
+    want = ctx.needs_input_grad
+    return (d_amps_raw if want[0] else None, d_hd_raw if want[1] else None, None, None,
+            None, None)
+
+
+class NoiseControlsFn(torch.autograd.Function):
+  """core.noise_controls (FilteredNoise.get_controls, synths.py:165-179),
+  differentiable in the raw magnitudes: `ddsp_b200_noise_controls_backward`.  Without
+  `scale` the op is the identity and so is its gradient."""
+
+  @staticmethod
+  def forward(ctx, magnitudes, initial_bias, scale):
+    ctx.save_for_backward(magnitudes)
+    ctx.cfg = (float(initial_bias), bool(scale))
+    return core.noise_controls(magnitudes, *ctx.cfg)
+
+  @staticmethod
+  def backward(ctx, d_mags):
+    mags, = ctx.saved_tensors
+    bias, scale = ctx.cfg
+    if not scale:
+      return d_mags, None, None
+    d_mags = d_mags.contiguous().to(torch.float32)
+    d_raw = torch.empty_like(mags)
+    core._launch('ddsp_b200_noise_controls_backward', mags, d_mags, d_raw, mags.numel(),
+                 bias)
+    return d_raw, None, None
 
 
 class FftConvolveLtiFn(torch.autograd.Function):

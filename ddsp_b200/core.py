@@ -188,17 +188,22 @@ def _check_out(out, shape, like, name='out'):
 
 
 def _no_grad_path(name, *tensors):
-  """The kernels behind `core.*` / Processor / ProcessorGroup do not record an
-  autograd graph.  A training loop that relies on gradients must go through
-  ddsp_b200.autograd (decoder_train / HarmonicSynthesisFn / FilteredNoiseFn);
-  silently returning detached audio would train nothing."""
+  """Refuses to return detached audio.  The calls that end here record no autograd
+  graph: the fused signal-only `ProcessorGroup` call (`decoder_forward`), the
+  synthesizers writing through `out=` / `accumulate=`, and the shapes no backward
+  kernel takes.  A training loop gets gradients from the Processor API
+  (`group(features, return_outputs_dict=True)`, or `get_controls` + `get_signal`),
+  whose `core.*` ops route to ddsp_b200.autograd under grad, or from
+  `autograd.decoder_train`; silently returning detached audio would train nothing."""
   if torch.is_grad_enabled() and any(
       isinstance(t, torch.Tensor) and t.requires_grad for t in tensors):
     raise RuntimeError(
         f'ddsp_b200.core.{name}: an input requires grad, but this call is the '
-        'inference path and returns detached audio.  Use ddsp_b200.autograd.'
-        'decoder_train / HarmonicSynthesisFn / FilteredNoiseFn (CUDA backward '
-        'kernels), or wrap the call in torch.no_grad().')
+        'inference path and returns detached audio.  Train through the Processor '
+        'API - group(features, return_outputs_dict=True), or get_controls + '
+        'get_signal - or ddsp_b200.autograd.decoder_train / HarmonicSynthesisFn / '
+        'FilteredNoiseFn (CUDA backward kernels), or wrap the call in '
+        'torch.no_grad().')
 
 
 # ----------------------------------------------------------------------------
@@ -427,7 +432,9 @@ def resample(inputs, n_timesteps: int, method: Text = 'linear',
 def harmonic_controls(amplitudes, harmonic_distribution, f0_hz, sample_rate,
                       scale=True, normalize_below_nyquist=True):
   """synths.Harmonic.get_controls arithmetic (synths.py:94-121): exp_sigmoid,
-  core.normalize_harmonics (core.py:894-907)."""
+  core.normalize_harmonics (core.py:894-907).  Routes to
+  `autograd.HarmonicControlsFn` when grad is enabled and the amplitudes or the
+  distribution require it; f0_hz gets no gradient through the mask (tf.where)."""
   sa, sh, sf = _shape(amplitudes), _shape(harmonic_distribution), _shape(f0_hz)
   if len(sh) != 3 or len(sa) != 3 or len(sf) != 3:
     raise ValueError('Harmonic controls must be 3-D [batch, frames, channels]; '
@@ -440,11 +447,14 @@ def harmonic_controls(amplitudes, harmonic_distribution, f0_hz, sample_rate,
   amplitudes = torch_float32(amplitudes)
   hd = torch_float32(harmonic_distribution)
   f0_hz = torch_float32(f0_hz)
+  if _requires_grad(amplitudes, hd):
+    from ddsp_b200 import autograd as _ag
+    return _ag.HarmonicControlsFn.apply(amplitudes, hd, f0_hz, float(sample_rate),
+                                        bool(scale), bool(normalize_below_nyquist))
   amps_out = torch.empty_like(amplitudes)
   hd_out = torch.empty_like(hd)
   flags = ((_lib.CTL_SCALE if scale else 0) |
            (_lib.CTL_NYQUIST if normalize_below_nyquist else 0))
-  _no_grad_path('harmonic_controls', amplitudes, hd, f0_hz)
   _launch('ddsp_b200_harmonic_controls', amplitudes, hd, f0_hz, amps_out, hd_out, b, f, k,
           float(sample_rate), flags)
   return amps_out, hd_out
@@ -735,6 +745,14 @@ def harmonic_synthesis(frequencies,
   'tf_sequential' reproduces TensorFlow's float32 phase arithmetic in its own
   order (tf.cumsum, or angular_cumsum if use_angular_cumsum) - a debug mode for
   small shapes that materialises the envelopes.
+
+  When grad is enabled and an input requires it (DESIGN.md section 3.15): the fused
+  case at hops the harmonic backward kernel takes (a multiple of 64, at most 8192)
+  is `autograd.HarmonicSynthesisFn`; `harmonic_shifts`, or any other integer hop,
+  goes through `sinusoidal_synthesis` and its backward; 'nearest' / 'cubic' and
+  non-integer hops through `resample` and `oscillator_bank` and theirs.  `out=` is
+  refused there (RuntimeError), and phase_mode='tf_sequential' has no backward
+  (NotImplementedError).
   """
   if amp_resample_method not in ('nearest', 'linear', 'cubic', 'window'):
     # core.py:632-634
@@ -767,6 +785,13 @@ def harmonic_synthesis(frequencies,
                        f'{"=" + str(k) if harmonic_distribution is not None else ""}].')
     k = int(ss[-1])
   n_samples = int(n_samples)
+  grad = _requires_grad(frequencies, amplitudes, harmonic_distribution, harmonic_shifts)
+  if grad and out is not None:
+    _no_grad_path('harmonic_synthesis', frequencies, amplitudes, harmonic_distribution,
+                  harmonic_shifts)
+  if grad and phase_mode == 'tf_sequential':
+    raise NotImplementedError("harmonic_synthesis: phase_mode='tf_sequential' is a "
+                              'forward-only debug mode; it has no backward.')
   if amp_resample_method == 'window':
     if f >= n_samples:
       # core.py:682-685
@@ -785,8 +810,6 @@ def harmonic_synthesis(frequencies,
     harmonic_distribution = torch_float32(harmonic_distribution)
   if harmonic_shifts is not None:
     harmonic_shifts = torch_float32(harmonic_shifts)
-  _no_grad_path('harmonic_synthesis', frequencies, amplitudes, harmonic_distribution,
-                harmonic_shifts)
   if out is not None:
     _check_out(out, (b, n_samples), frequencies)
   else:
@@ -794,7 +817,14 @@ def harmonic_synthesis(frequencies,
 
   fused_ok = (amp_resample_method in AMP_METHODS and n_samples % f == 0 and
               phase_mode != 'tf_sequential')
-  if harmonic_shifts is None and fused_ok:
+  if grad and harmonic_shifts is None and fused_ok and _harmonic_backward_takes(
+      b, f, n_samples):
+    from ddsp_b200 import autograd as _ag
+    if harmonic_distribution is None:
+      harmonic_distribution = torch.ones_like(amplitudes)
+    return _ag.HarmonicSynthesisFn.apply(frequencies, amplitudes, harmonic_distribution,
+                                         n_samples, sample_rate, amp_resample_method)
+  if harmonic_shifts is None and fused_ok and not grad:
     mode = {'recurrence': _lib.PHASE_RECURRENCE, 'direct': _lib.PHASE_DIRECT}[
         phase_mode]
     if out is None:
@@ -833,6 +863,13 @@ def harmonic_synthesis(frequencies,
   else:
     out.copy_(audio)
   return out
+
+
+def _harmonic_backward_takes(b, f, n_samples):
+  """Whether `ddsp_b200_harmonic_backward` takes an integer-hop shape: a hop that is a
+  multiple of 64 and at most 8192, a batch within the grid limit."""
+  hop = n_samples // f
+  return hop % 64 == 0 and hop <= 8192 and b <= 65535
 
 
 @on_operands_device
@@ -1523,11 +1560,33 @@ def uniform_noise(batch_size, n_samples, seed=0, offset=0, device=None):
   return out
 
 
+def _noise_backward_takes(f, nb, n_samples, window_size):
+  """Whether `ddsp_b200_filtered_noise_backward` takes a shape: an impulse response of
+  at least three taps, and 32 frames of noise, gradient and taps within one CTA's
+  shared memory (the launcher's own layout, csrc/capi.cu noise_bwd_params)."""
+  if nb < 2:
+    return False
+  s0 = 2 * (nb - 1)
+  s = _ir_size(nb, window_size)
+  frame = -(-n_samples // f)
+  padded = (frame + 15) & ~15
+  x_stride = (padded + 1) | 1
+  g_stride = (padded + s + 17) | 1
+  h_stride = (s + nb) | 1
+  floats = (s0 + s + 32 * (x_stride + g_stride + h_stride) + 3) & ~3
+  if nb == 65:
+    floats += nb * 36       # the cosine table of the 65-band specialisation
+  return s >= 3 and 4 * floats <= 200 * 1024
+
+
 @on_operands_device
 def filtered_noise(magnitudes, n_samples, window_size=257, noise=None, seed=0,
                    offset=0, out=None, accumulate=False):
   """FilteredNoise.get_signal arithmetic (synths.py:181-196): uniform noise ->
-  core.frequency_filter (core.py:1628-1655), fused where the shape allows."""
+  core.frequency_filter (core.py:1628-1655), fused where the shape allows.  Routes to
+  `autograd.FilteredNoiseFn` when grad is enabled and the magnitudes require it,
+  for the shapes `ddsp_b200_filtered_noise_backward` takes; `out=` and the other
+  shapes are refused there (RuntimeError)."""
   sm = _shape(magnitudes)
   if len(sm) != 3:
     raise ValueError('magnitudes must be [batch, n_frames, n_filter_banks], got '
@@ -1545,6 +1604,12 @@ def filtered_noise(magnitudes, n_samples, window_size=257, noise=None, seed=0,
         'match. For small hop size = ceil(audio_size / n_ir_frames), '
         'number of impulse response frames must be a multiple of the audio '
         'size.'.format(n_audio_frames, f))
+  if _requires_grad(magnitudes):
+    if out is not None or not _noise_backward_takes(f, nb, n_samples, int(window_size)):
+      _no_grad_path('filtered_noise', magnitudes)
+    from ddsp_b200 import autograd as _ag
+    return _ag.FilteredNoiseFn.apply(magnitudes, n_samples, int(window_size), noise,
+                                     int(seed), int(offset))
   magnitudes = torch_float32(magnitudes)
   if noise is not None:
     noise = torch_float32(noise)
@@ -1554,7 +1619,6 @@ def filtered_noise(magnitudes, n_samples, window_size=257, noise=None, seed=0,
     accumulate = False
   else:
     _check_out(out, (b, n_samples), magnitudes)
-  _no_grad_path('filtered_noise', magnitudes)
   _launch('ddsp_b200_filtered_noise_forward', magnitudes, noise, int(seed), int(offset),
           out, b, f, nb, n_samples, int(window_size), int(bool(accumulate)),
           *_workspace('ddsp_b200_filtered_noise_workspace', magnitudes.device, b, f, nb,
@@ -1602,9 +1666,12 @@ def decoder_forward(amps, harmonic_distribution, f0_hz, noise_magnitudes,
 
 
 def noise_controls(magnitudes, initial_bias=-5.0, scale=True):
-  """FilteredNoise.get_controls arithmetic (synths.py:165-179)."""
+  """FilteredNoise.get_controls arithmetic (synths.py:165-179).  Routes to
+  `autograd.NoiseControlsFn` when grad is enabled and the magnitudes require it."""
   magnitudes = torch_float32(magnitudes)
-  _no_grad_path('noise_controls', magnitudes)
+  if _requires_grad(magnitudes):
+    from ddsp_b200 import autograd as _ag
+    return _ag.NoiseControlsFn.apply(magnitudes, float(initial_bias), bool(scale))
   out = torch.empty_like(magnitudes)
   _launch('ddsp_b200_noise_controls', magnitudes, out, magnitudes.numel(),
           float(initial_bias), int(bool(scale)))

@@ -682,6 +682,28 @@ int ddsp_b200_harmonic_controls_backward(const float* amps_raw, const float* hd_
   return 0;
 }
 
+int ddsp_b200_harmonic_controls_vjp(const float* amps_raw, const float* hd_raw,
+                                    const float* f0_hz, const float* d_amplitudes,
+                                    const float* d_hd, float* d_amps_raw, float* d_hd_raw,
+                                    int B, int F, int K, float sample_rate, int flags,
+                                    void* stream) {
+  DDSP_REQUIRE(amps_raw && hd_raw && f0_hz && d_amps_raw && d_hd_raw,
+               DDSP_B200_E_INVALID, "harmonic_controls_vjp: null pointer");
+  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1, DDSP_B200_E_INVALID,
+               "harmonic_controls_vjp: bad shape B=%d F=%d K=%d", B, F, K);
+  const int64_t rows = (int64_t)B * F;
+  if (rows == 0) return 0;
+  DDSP_REQUIRE(rows < (1ll << 31) / 32, DDSP_B200_E_INVALID,
+               "harmonic_controls_vjp: B*F too large");
+  const int threads = 256;
+  const int blocks = (int)((rows * 32 + threads - 1) / threads);
+  harmonic_controls_vjp_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(
+      amps_raw, hd_raw, f0_hz, d_amplitudes, d_hd, d_amps_raw, d_hd_raw, (int)rows, K,
+      sample_rate * 0.5f, flags);
+  DDSP_CHECK_LAUNCH("harmonic_controls_vjp");
+  return 0;
+}
+
 int ddsp_b200_noise_controls_backward(const float* mags_raw, const float* d_mags,
                                       float* d_raw, int64_t n, float initial_bias,
                                       void* stream) {

@@ -4,6 +4,14 @@
 
 namespace ddsp {
 
+// The Nyquist decision of Harmonic.get_controls for harmonic number k1 = 1..K:
+// get_harmonic_frequencies is f0 * linspace(1..K) in float32 (core.py:1042-1044),
+// silent at or above sr/2 (core.py:888-890).  The forward and both backward kernels
+// (controls_bwd.cuh) decide with this one expression.
+__device__ __forceinline__ bool harmonic_above_nyquist(float f0, int k1, float nyquist) {
+  return __fmul_rn(f0, (float)k1) >= nyquist;
+}
+
 // Harmonic.get_controls: one warp per (b, f) row of harmonic_distribution.
 //   hd = exp_sigmoid(hd)                    (synths.py:110-112, core.py:386-404)
 //   hd[k] = 0 where f0 * k >= sr/2          (core.py:894-901, 888-890)
@@ -25,8 +33,7 @@ harmonic_controls_kernel(const float* amps_in, const float* hd_in,
   for (int c = lane; c < K; c += 32) {
     float v = in[c];
     if (scale) v = exp_sigmoid_f(v);
-    // get_harmonic_frequencies: f0 * linspace(1..K) in float32 (core.py:1042-1044)
-    if (nyq && __fmul_rn(f, (float)(c + 1)) >= nyquist) v = 0.f;
+    if (nyq && harmonic_above_nyquist(f, c + 1, nyquist)) v = 0.f;
     out[c] = v;
     sum += v;
   }

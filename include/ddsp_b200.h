@@ -228,6 +228,21 @@ int ddsp_b200_harmonic_controls_backward(const float* amps_raw, const float* hd_
                                          float* d_hd_raw, int B, int F, int K,
                                          float sample_rate, int flags, void* stream);
 
+/* The vector-Jacobian product of Harmonic.get_controls (synths.py:94-121) for ANY
+ * upstream gradient: d_amplitudes [B,F,1] on the scaled amplitudes and d_hd [B,F,K] on
+ * the normalised harmonic distribution - what a loss on the controls themselves
+ * produces, summed with the synthesizer's own gradient.  Either may be NULL: zeros,
+ * and not read.  From the RAW inputs amps_raw [B,F,1], hd_raw [B,F,K] and f0_hz
+ * [B,F,1] to d_amps_raw [B,F,1] and d_hd_raw [B,F,K], every element written.
+ * flags as ddsp_b200_harmonic_controls (without DDSP_B200_CTL_SCALE the inputs are
+ * already scaled and only the mask and the normalisation are transposed).  f0_hz gets
+ * no gradient: the Nyquist mask is piecewise constant.  One launch. */
+int ddsp_b200_harmonic_controls_vjp(const float* amps_raw, const float* hd_raw,
+                                    const float* f0_hz, const float* d_amplitudes,
+                                    const float* d_hd, float* d_amps_raw, float* d_hd_raw,
+                                    int B, int F, int K, float sample_rate, int flags,
+                                    void* stream);
+
 /* Backward of FilteredNoise.get_controls (synths.py:165-179):
  * d raw = d magnitudes * exp_sigmoid'(raw + initial_bias), n elements. */
 int ddsp_b200_noise_controls_backward(const float* mags_raw, const float* d_mags,
