@@ -37,6 +37,7 @@ _i = ctypes.c_int
 _i64 = ctypes.c_int64
 _u64 = ctypes.c_uint64
 _f = ctypes.c_float
+_d = ctypes.c_double
 _vp = ctypes.c_void_p
 _sz = ctypes.c_size_t
 
@@ -163,6 +164,10 @@ SIGNATURES = {
         (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _i, _vp]),
     'ddsp_b200_sinusoidal_to_harmonic_backward':
         (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _i, _vp]),
+    'ddsp_b200_hmm_log_prob': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _d, _d, _vp]),
+    'ddsp_b200_hmm_log_prob_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _d, _d, _vp]),
+    'ddsp_b200_hmm_viterbi': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _d, _d, _vp]),
 }
 
 _lib = None

@@ -45,6 +45,9 @@ kernels, exposed as `torch.autograd.Function`s:
   * `MixtureNLLFn` / `CombNLLFn` - the Gaussian-mixture NLLs of the consistency
     losses (`losses.KDEConsistencyLoss`, `losses.TWMLoss`), evaluated per frame
     on-chip with gradients to every input;
+  * `HmmLogProbFn` - the HMM log-likelihood of `losses.HmmTranscriber`, with
+    gradients to the observations (pitch and amplitude); routed to by
+    `core.hmm_log_prob` under grad;
   * `DecoderFn` / `decoder_train` - the whole `ae.gin` decoder from RAW network
     outputs: forward is the fused two-kernel pipeline (`get_controls` in shared
     memory), backward is the two synthesizer backward kernels plus the
@@ -766,6 +769,32 @@ class SinusoidalToHarmonicFn(torch.autograd.Function):
     want = ctx.needs_input_grad
     return (d_a if want[0] else None, d_f if want[1] else None, d_f0 if want[2] else None,
             None, None, None, None)
+
+
+class HmmLogProbFn(torch.autograd.Function):
+  """core.hmm_log_prob, differentiable in the observations [B, T, 2].  Nothing but the
+  inputs is saved: `ddsp_b200_hmm_log_prob_backward` (csrc/hmm.cuh) re-runs the forward
+  algorithm with a checkpoint every ~sqrt(T) steps ([B, ceil(T / seg), K] floats of
+  scratch, 4 MB at B = 256, T = 1000, K = 128) and scans the posterior marginals back
+  segment by segment."""
+
+  @staticmethod
+  def forward(ctx, x, loc, scale, hold, other):
+    ctx.save_for_backward(x, loc, scale)
+    ctx.cfg = (hold, other)
+    return core.hmm_log_prob_forward(x, loc, scale, hold, other)
+
+  @staticmethod
+  def backward(ctx, g):
+    x, loc, scale = ctx.saved_tensors
+    b, t, _ = x.shape
+    k = loc.shape[0]
+    seg = core.hmm_segment(t, k)
+    d_x = torch.empty_like(x)
+    ckpt = torch.empty((b, -(-t // seg), k), dtype=torch.float32, device=x.device)
+    core._launch('ddsp_b200_hmm_log_prob_backward', x, loc, scale,
+                 g.contiguous().to(torch.float32), d_x, ckpt, seg, b, t, k, *ctx.cfg)
+    return d_x, None, None, None, None
 
 
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):

@@ -6,6 +6,7 @@ sm_90a kernels) through the ctypes C ABI in `_lib.py`.  torch is plumbing:
 device memory and streams.  There is no CPU fallback.
 """
 import functools
+import math
 from collections import abc
 from typing import Any, Dict, Optional, Sequence, Text
 
@@ -553,6 +554,108 @@ def sinusoidal_to_harmonic(sin_amps, sin_freqs, f0_hz, harmonic_width=0.1,
     from ddsp_b200 import autograd as _ag
     return _ag.SinusoidalToHarmonicFn.apply(a, f, f0, *cfg)
   return sinusoidal_to_harmonic_forward(a, f, f0, *cfg)
+
+
+# ----------------------------------------------------------------------------
+# The HMM of losses.HmmTranscriber (losses.py:247-345): csrc/hmm.cuh
+# ----------------------------------------------------------------------------
+HMM_MAX_STATES = 1024          # states one CTA runs, a thread each
+HMM_SEGMENT_FLOATS = 48 * 1024  # shared floats of the backward's segment buffer
+HMM_VITERBI_BYTES = 200 * 1024  # shared bytes of the Viterbi back pointers
+
+
+def _hmm_shapes(observations, loc, scale):
+  """(B, T, K) of an HMM call from static shapes, or the error."""
+  so, sl, ss = _shape(observations), _shape(loc), _shape(scale)
+  if len(so) != 3 or so[2] != 2 or so[1] < 1:
+    raise ValueError(f'observations {so} must be [batch, time >= 1, 2] (pitch, amps).')
+  if len(sl) != 2 or sl[1] != 2 or ss != sl:
+    raise ValueError(f'loc {sl} and scale {ss} must both be [n_states, 2].')
+  if sl[0] < 2:
+    raise ValueError(f'the HMM needs at least 2 states, got {sl[0]}.')
+  if sl[0] > HMM_MAX_STATES:
+    raise NotImplementedError(f'HMM: {sl[0]} states exceed the {HMM_MAX_STATES} the '
+                              'kernels run.')
+  return so[0], so[1], sl[0]
+
+
+def _hmm_transition(hold, other):
+  hold, other = float(hold), float(other)
+  if not (np.isfinite(hold) and np.isfinite(other) and hold >= 0.0 and other >= 0.0
+          and hold + other > 0.0):
+    raise ValueError(f'hold={hold} and other={other} must be finite, non-negative and '
+                     'not both 0.')
+  return hold, other
+
+
+def hmm_segment(t, k):
+  """Steps per checkpoint of the log-likelihood backward: about sqrt(T), so that the
+  checkpoints ([B, ceil(T / seg), K] floats) and the segment buffer (seg x K floats
+  of shared memory) are both O(K sqrt(T)); at most HMM_SEGMENT_FLOATS / K."""
+  return min(math.isqrt(t - 1) + 1, HMM_SEGMENT_FLOATS // k)
+
+
+def hmm_viterbi_takes(t, k):
+  """True where `ddsp_b200_hmm_viterbi` keeps T steps of K states' back pointers in
+  shared memory: 4 T (ceil(K / 32) + 1) <= 200 KiB."""
+  return 4 * t * ((k + 31) // 32 + 1) <= HMM_VITERBI_BYTES
+
+
+def _hmm_operands(observations, loc, scale):
+  x = torch_float32(observations)
+  return x, torch_float32(loc, device=x.device), torch_float32(scale, device=x.device)
+
+
+def hmm_log_prob_forward(x, loc, scale, hold, other):
+  """`ddsp_b200_hmm_log_prob` on float32 CUDA operands -> log_prob [B]."""
+  b, t, _ = x.shape
+  out = torch.empty((b,), dtype=torch.float32, device=x.device)
+  _launch('ddsp_b200_hmm_log_prob', x, loc, scale, out, b, t, loc.shape[0], hold, other)
+  return out
+
+
+@on_operands_device
+def hmm_log_prob(observations, loc, scale, hold, other):
+  """log p(observations) [B] under the HMM of losses.HmmTranscriber: K states, a
+  uniform initial distribution, transitions `hold` on the diagonal and `other`
+  elsewhere, observations [B, T, 2] under MultivariateNormalDiag(loc_j, scale_j) with
+  loc and scale [K, 2] (tfp's HiddenMarkovModel.log_prob).  The forward algorithm
+  runs in O(K) per step in one launch (csrc/hmm.cuh).  Routes to
+  `autograd.HmmLogProbFn` when grad is enabled and the observations require it;
+  loc and scale are constants.
+
+  Shapes, K < 2 and invalid hold / other raise ValueError, K > 1024
+  NotImplementedError, before any device work."""
+  _hmm_shapes(observations, loc, scale)
+  hold, other = _hmm_transition(hold, other)
+  if _requires_grad(loc, scale):
+    raise NotImplementedError('hmm_log_prob: gradients reach the observations only; '
+                              'loc and scale are constants.')
+  x, loc, scale = _hmm_operands(observations, loc, scale)
+  if _requires_grad(x):
+    from ddsp_b200 import autograd as _ag
+    return _ag.HmmLogProbFn.apply(x, loc, scale, hold, other)
+  return hmm_log_prob_forward(x, loc, scale, hold, other)
+
+
+@on_operands_device
+def hmm_posterior_mode(observations, loc, scale, hold, other):
+  """The most likely state sequence [B, T] (int64) of the HMM of `hmm_log_prob`
+  (tfp's HiddenMarkovModel.posterior_mode), by Viterbi in one launch with its back
+  pointers in shared memory.  Ties go to the lowest state index.  Besides the errors
+  of `hmm_log_prob`, T steps of K states beyond `hmm_viterbi_takes` raise
+  NotImplementedError before any device work."""
+  b, t, k = _hmm_shapes(observations, loc, scale)
+  hold, other = _hmm_transition(hold, other)
+  if not hmm_viterbi_takes(t, k):
+    raise NotImplementedError(
+        f'hmm_posterior_mode: {t} steps of {k} states exceed the back pointers the '
+        f'kernel keeps (4 T (ceil(K / 32) + 1) <= {HMM_VITERBI_BYTES} bytes).')
+  x, loc, scale = _hmm_operands(observations, loc, scale)
+  path = torch.empty((b, t), dtype=torch.int64, device=x.device)
+  _launch('ddsp_b200_hmm_viterbi', x.detach(), loc.detach(), scale.detach(), path, b, t,
+          k, hold, other)
+  return path
 
 
 @on_operands_device

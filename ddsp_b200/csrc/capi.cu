@@ -32,6 +32,7 @@
 #include "mel.cuh"
 #include "consistency.cuh"
 #include "sinc.cuh"
+#include "hmm.cuh"
 
 namespace ddsp {
 
@@ -2386,6 +2387,92 @@ int ddsp_b200_sinusoidal_to_harmonic_backward(
                                        (cudaStream_t)stream>>>(
       p, grad_amp, grad_dist, d_sin_amps, d_sin_freqs, d_f0_hz);
   DDSP_CHECK_LAUNCH("sinusoidal_to_harmonic_backward");
+  return 0;
+}
+
+// ---- losses.HmmTranscriber -----------------------------------------------------------
+// The checks every HMM entry point makes, and its kernel parameters.
+static int hmm_check(const char* name, const float* obs, const float* loc,
+                     const float* scale, int B, int T, int K, double hold, double other,
+                     hmm_::Params* p) {
+  DDSP_REQUIRE(B >= 0 && T >= 1 && K >= 2, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d T=%d K=%d", name, B, T, K);
+  DDSP_REQUIRE(std::isfinite(hold) && std::isfinite(other) && hold >= 0.0 && other >= 0.0 &&
+                   hold + other > 0.0,
+               DDSP_B200_E_INVALID,
+               "%s: hold=%g and other=%g must be finite, non-negative and not both 0",
+               name, hold, other);
+  DDSP_REQUIRE(K <= hmm_::kMaxStates, DDSP_B200_E_UNSUPPORTED,
+               "%s: K=%d states exceed the %d supported", name, K, hmm_::kMaxStates);
+  p->obs = reinterpret_cast<const float2*>(obs);
+  p->loc = reinterpret_cast<const float2*>(loc);
+  p->scale = reinterpret_cast<const float2*>(scale);
+  p->T = T;
+  p->K = K;
+  p->hold = (float)hold;
+  p->other = (float)other;
+  p->log_hold = (float)std::log(hold);
+  p->log_other = (float)std::log(other);
+  p->log_init = -std::log((double)K);
+  return 0;
+}
+
+static unsigned hmm_threads(int K) { return (unsigned)((K + 31) & ~31); }
+
+int ddsp_b200_hmm_log_prob(const float* obs, const float* loc, const float* scale,
+                           float* log_prob, int B, int T, int K, double hold, double other,
+                           void* stream) {
+  DDSP_REQUIRE(B == 0 || (obs && loc && scale && log_prob), DDSP_B200_E_INVALID,
+               "hmm_log_prob: null pointer");
+  hmm_::Params p;
+  int rc = hmm_check("hmm_log_prob", obs, loc, scale, B, T, K, hold, other, &p);
+  if (rc || B == 0) return rc;
+  hmm_::hmm_log_prob_kernel<<<(unsigned)B, hmm_threads(K), 0, (cudaStream_t)stream>>>(
+      p, log_prob);
+  DDSP_CHECK_LAUNCH("hmm_log_prob");
+  return 0;
+}
+
+int ddsp_b200_hmm_log_prob_backward(const float* obs, const float* loc, const float* scale,
+                                    const float* grad, float* d_obs, float* checkpoints,
+                                    int seg, int B, int T, int K, double hold, double other,
+                                    void* stream) {
+  DDSP_REQUIRE(B == 0 || (obs && loc && scale && grad && d_obs && checkpoints),
+               DDSP_B200_E_INVALID, "hmm_log_prob_backward: null pointer");
+  hmm_::Params p;
+  int rc = hmm_check("hmm_log_prob_backward", obs, loc, scale, B, T, K, hold, other, &p);
+  if (rc) return rc;
+  DDSP_REQUIRE(seg >= 1 && (int64_t)seg * K <= hmm_::kSegFloats, DDSP_B200_E_INVALID,
+               "hmm_log_prob_backward: seg=%d must be at least 1 with seg*K at most %d",
+               seg, hmm_::kSegFloats);
+  if (B == 0) return 0;
+  const size_t smem = sizeof(float) * (size_t)seg * K;
+  rc = set_smem(hmm_::hmm_backward_kernel, smem, "hmm_log_prob_backward");
+  if (rc) return rc;
+  hmm_::hmm_backward_kernel<<<(unsigned)B, hmm_threads(K), smem, (cudaStream_t)stream>>>(
+      p, seg, grad, reinterpret_cast<float2*>(d_obs), checkpoints);
+  DDSP_CHECK_LAUNCH("hmm_log_prob_backward");
+  return 0;
+}
+
+int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale,
+                          int64_t* path, int B, int T, int K, double hold, double other,
+                          void* stream) {
+  DDSP_REQUIRE(B == 0 || (obs && loc && scale && path), DDSP_B200_E_INVALID,
+               "hmm_viterbi: null pointer");
+  hmm_::Params p;
+  int rc = hmm_check("hmm_viterbi", obs, loc, scale, B, T, K, hold, other, &p);
+  if (rc) return rc;
+  const size_t smem = sizeof(uint32_t) * (size_t)T * ((K + 31) / 32 + 1);
+  DDSP_REQUIRE(smem <= hmm_::kViterbiBytes, DDSP_B200_E_UNSUPPORTED,
+               "hmm_viterbi: T=%d steps of K=%d states need %zu B of back pointers, more "
+               "than the %zu supported", T, K, smem, hmm_::kViterbiBytes);
+  if (B == 0) return 0;
+  rc = set_smem(hmm_::hmm_viterbi_kernel, smem, "hmm_viterbi");
+  if (rc) return rc;
+  hmm_::hmm_viterbi_kernel<<<(unsigned)B, hmm_threads(K), smem, (cudaStream_t)stream>>>(
+      p, path);
+  DDSP_CHECK_LAUNCH("hmm_viterbi");
   return 0;
 }
 

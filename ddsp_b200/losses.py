@@ -3,11 +3,13 @@ multi-scale spectral loss (`losses.py:102-243`, torch with cuFFT on the GPU) and
 consistency losses of the self-supervised pitch model (`losses.py:489-1076`).  The
 Gaussian mixtures of `KDEConsistencyLoss` and `TWMLoss` are evaluated per frame by
 the CUDA kernels of `csrc/consistency.cuh` (`autograd.MixtureNLLFn`, `CombNLLFn`);
-the [B, T, K]-sized elementwise work around them is torch autograd."""
+the [B, T, K]-sized elementwise work around them is torch autograd.  The HMM of
+`HmmTranscriber` (`losses.py:247-345`) runs on the kernels of `csrc/hmm.cuh`."""
 import functools
 import math
 import re
 
+import numpy as np
 import torch
 
 from ddsp_b200 import autograd
@@ -403,3 +405,131 @@ class TWMLoss(Loss):
       return f0_candidates[..., None] * n
     midi = hz_to_midi(f0_candidates)[..., None] + 12.0 * torch.log2(n)
     return torch.where(f0_candidates[..., None] <= 0.0, torch.zeros_like(midi), midi)
+
+
+# ------------------------------------------------------------------------------
+# HMM prior and MIDI transcription (losses.py:247-345)
+# ------------------------------------------------------------------------------
+class HmmTranscriber:
+  """losses.HmmTranscriber (losses.py:247-345): an HMM over MIDI with one state per
+  pitch 1..n_pitches - 1 and state 0 for "off", observing (f0 in MIDI, amplitude).
+
+  The reference subclasses tfp's HiddenMarkovModel; here the two methods it uses run on
+  the CUDA kernels of csrc/hmm.cuh: `log_prob` (the forward algorithm, differentiable in
+  pitch and amplitude through `autograd.HmmLogProbFn`) and `posterior_mode` (Viterbi,
+  ties to the lowest pitch).  The transitions are `hold` = 1 - 1 / avg_length on the
+  diagonal and `other` = (1 - hold) / (n_pitches - 1) elsewhere; the HMM's parameters
+  are constants.  Other tfp Distribution methods are not provided.
+
+  pitch and amps other than [batch, n_timesteps, 1], n_pitches < 2, n_timesteps < 1
+  and avg_length < 1 raise ValueError before any device work; n_pitches > 1024, and
+  for `posterior_mode` more steps than `core.hmm_viterbi_takes` allows, raise
+  NotImplementedError."""
+
+  def __init__(self,
+               avg_length=200,
+               midi_std=0.5,
+               amps_on_center=1.5,
+               amps_on_scale=0.5,
+               amps_off_center=0.0,
+               amps_off_scale=0.1,
+               n_timesteps=1000,
+               n_pitches=128,
+               weight=1.0,
+               name='HiddenMarkovModel'):
+    if not avg_length >= 1:
+      raise ValueError(f'HmmTranscriber: avg_length must be at least 1 (hold = 1 - '
+                       f'1 / avg_length), got {avg_length}')
+    if int(n_pitches) != n_pitches or n_pitches < 2:
+      raise ValueError(f'HmmTranscriber: n_pitches must be an integer >= 2, got {n_pitches}')
+    if int(n_timesteps) != n_timesteps or n_timesteps < 1:
+      raise ValueError(f'HmmTranscriber: n_timesteps must be an integer >= 1, got '
+                       f'{n_timesteps}')
+    self.avg_length = avg_length
+    self.midi_std = midi_std
+    self.n_timesteps = int(n_timesteps)
+    self.n_pitches = int(n_pitches)
+    self.weight = weight
+    self.name = name
+    self.hold = 1.0 - 1.0 / avg_length
+    self.other = (1.0 - self.hold) / (self.n_pitches - 1)
+    k = self.n_pitches
+    self.loc = np.stack([np.r_[k / 2.0, np.arange(1, k)],
+                         np.r_[amps_off_center, np.full(k - 1, amps_on_center)]],
+                        axis=-1).astype(np.float32)
+    self.scale = np.stack([np.r_[float(k), np.full(k - 1, midi_std)],
+                           np.r_[amps_off_scale, np.full(k - 1, amps_on_scale)]],
+                          axis=-1).astype(np.float32)
+    self._params = {}   # device -> (loc, scale) on it
+
+  def _on(self, device):
+    if device not in self._params:
+      self._params[device] = (core.torch_float32(self.loc, device=device),
+                              core.torch_float32(self.scale, device=device))
+    return self._params[device]
+
+  def _check(self, name, x, last):
+    s = core._shape(x)
+    if len(s) != 3 or s[1] != self.n_timesteps or s[2] != last:
+      raise ValueError(f'HmmTranscriber.{name}: expected [batch, {self.n_timesteps}, '
+                       f'{last}], got {s}')
+
+  def _supported(self, name, viterbi):
+    k, t = self.n_pitches, self.n_timesteps
+    if k > core.HMM_MAX_STATES:
+      raise NotImplementedError(f'HmmTranscriber.{name}: {k} pitches exceed the '
+                                f'{core.HMM_MAX_STATES} states the kernels run.')
+    if viterbi and not core.hmm_viterbi_takes(t, k):
+      raise NotImplementedError(f'HmmTranscriber.{name}: {t} steps of {k} states exceed '
+                                'the back pointers the Viterbi kernel keeps.')
+
+  def _observations(self, name, pitch, amps, viterbi=False):
+    self._check(name, pitch, 1)
+    self._check(name, amps, 1)
+    if core._shape(pitch) != core._shape(amps):
+      raise ValueError(f'HmmTranscriber.{name}: pitch {core._shape(pitch)} and amps '
+                       f'{core._shape(amps)} differ')
+    self._supported(name, viterbi)
+    pitch = core.torch_float32(pitch)
+    return torch.cat([pitch, core.torch_float32(amps, device=pitch.device)], dim=-1)
+
+  def __call__(self, pitch, amps):
+    return self.nll(pitch, amps)
+
+  @staticmethod
+  def straight_through(x, x_quant):
+    """Straight through estimation: the value of x_quant, the gradient of x."""
+    return x - (x - x_quant).detach()
+
+  @core.on_operands_device
+  def log_prob(self, pa):
+    """log p(pa) [batch] for observations pa [batch, n_timesteps, 2] (pitch, amps)."""
+    self._check('log_prob', pa, 2)
+    self._supported('log_prob', False)
+    x = core.torch_float32(pa)
+    return core.hmm_log_prob(x, *self._on(x.device), self.hold, self.other)
+
+  @core.on_operands_device
+  def posterior_mode(self, pa):
+    """The most likely state per step, [batch, n_timesteps] int64."""
+    self._check('posterior_mode', pa, 2)
+    self._supported('posterior_mode', True)
+    x = core.torch_float32(pa)
+    return core.hmm_posterior_mode(x, *self._on(x.device), self.hold, self.other)
+
+  @core.on_operands_device
+  def nll(self, pitch, amps, per_example_loss=False):
+    """Negative log-likelihood per timestep: weight * mean_b(-log p_b / T), or the
+    [batch] values with per_example_loss."""
+    pa = self._observations('nll', pitch, amps)
+    avg_nll = -self.log_prob(pa) / pa.shape[1]
+    loss = avg_nll if per_example_loss else torch.mean(avg_nll)
+    return self.weight * loss
+
+  @core.on_operands_device
+  def predict_midi(self, pitch, amps, channel_dim=True, dtype=torch.float32):
+    """Viterbi decode of the most likely state as the quantized MIDI pitch,
+    [batch, n_timesteps, 1] (or [batch, n_timesteps]) of `dtype`."""
+    pa = self._observations('predict_midi', pitch, amps, viterbi=True)
+    q_pitch = self.posterior_mode(pa).to(dtype)
+    return q_pitch[:, :, None] if channel_dim else q_pitch

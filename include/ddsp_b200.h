@@ -687,6 +687,35 @@ int ddsp_b200_sinusoidal_to_harmonic_backward(
     const float* grad_dist, float* d_sin_amps, float* d_sin_freqs, float* d_f0_hz, int B,
     int T, int S, int K, float width, float sample_rate, int normalize, void* stream);
 
+/* losses.HmmTranscriber (losses.py:247-345): tfp's HiddenMarkovModel over K states with
+ * a uniform initial distribution, transitions hold on the diagonal and other elsewhere,
+ * and observations obs [B,T,2] (pitch, amps) under MultivariateNormalDiag(loc_j, scale_j),
+ * loc and scale [K,2] (scale positive).
+ *   ddsp_b200_hmm_log_prob: log_prob [B] = log p(obs_b), the forward algorithm in O(K)
+ *     per step, its normalisers summed in double.
+ *   ddsp_b200_hmm_log_prob_backward: d_obs [B,T,2] = grad_b * d log_prob_b / d obs, from
+ *     the posterior marginals; loc and scale are constants.  checkpoints is scratch of
+ *     B * ceil(T / seg) * K floats: the kernel re-runs the forward and keeps its state
+ *     there every seg steps; 1 <= seg and seg * K <= 49152 (E_INVALID otherwise).  No
+ *     atomics: bit-reproducible.
+ *   ddsp_b200_hmm_viterbi: path [B,T] (int64), the most likely state sequence; ties go to
+ *     the lowest state index.  The back pointers stay in shared memory, which bounds
+ *     4 T (ceil(K / 32) + 1) <= 204800 bytes (E_UNSUPPORTED otherwise): K = 1024 takes
+ *     T <= 1551, K = 128 T <= 10240.
+ * All three take B >= 0, T >= 1, 2 <= K <= 1024 (more is E_UNSUPPORTED), hold and other
+ * finite, non-negative and not both 0.  B = 0 returns after the checks without a launch
+ * (the pointers may then be null). */
+int ddsp_b200_hmm_log_prob(const float* obs, const float* loc, const float* scale,
+                           float* log_prob, int B, int T, int K, double hold, double other,
+                           void* stream);
+int ddsp_b200_hmm_log_prob_backward(const float* obs, const float* loc, const float* scale,
+                                    const float* grad, float* d_obs, float* checkpoints,
+                                    int seg, int B, int T, int K, double hold, double other,
+                                    void* stream);
+int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale,
+                          int64_t* path, int B, int T, int K, double hold, double other,
+                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -102,6 +102,14 @@ assert torch.isfinite(sa.grad).all() and torch.isfinite(sf0.grad).all()
 assert torch.isfinite(h2).all() and torch.isfinite(r4).all() and torch.isfinite(ob).all()
 assert torch.isfinite(xa.grad).all() and torch.isfinite(hi.grad).all() and torch.isfinite(f0g.grad).all()
 assert torch.isfinite(e).all() and torch.isfinite(f).all() and torch.isfinite(g).all()
+# HmmTranscriber: log_prob with its backward (a partial last segment) and Viterbi
+hmm = losses.HmmTranscriber(n_timesteps=37, n_pitches=45)
+hp = (45.0 * torch.rand(2, 37, 1, device='cuda')).requires_grad_(True)
+ha = 1.5 * torch.rand(2, 37, 1, device='cuda')
+hmm.nll(hp, ha).backward()
+hq = hmm.predict_midi(hp, ha)
+torch.cuda.synchronize()
+assert torch.isfinite(hp.grad).all() and bool(((hq >= 0) & (hq < 45)).all())
 print('sanitize_run ok', float(a.abs().mean()), float(b.abs().mean()),
       float(c.abs().mean()), float(d.abs().mean()),
       float(raw['harmonic_distribution'].grad.abs().mean()))
