@@ -1666,7 +1666,7 @@ def uniform_noise(batch_size, n_samples, seed=0, offset=0, device=None):
 def _noise_backward_takes(f, nb, n_samples, window_size):
   """Whether `ddsp_b200_filtered_noise_backward` takes a shape: an impulse response of
   at least three taps, and 32 frames of noise, gradient and taps within one CTA's
-  shared memory (the launcher's own layout, csrc/capi.cu noise_bwd_params)."""
+  shared memory (the launcher's own layout, csrc/noise.cu noise_bwd_params)."""
   if nb < 2:
     return False
   s0 = 2 * (nb - 1)

@@ -1,7 +1,7 @@
-// Base of the harmonic kernel family: the parameters, the reference's float32
-// Nyquist decision, the 256-entry sin / cos table and the 64-bit fixed-point
-// phase arithmetic, which a backward kernel shares with its forward to
-// reproduce the forward's phase.  Derivations (closed-form phase, Reinsch
+// Base of the harmonic kernel family: the parameters and the entry points' checks
+// of them, the reference's float32 Nyquist decision, the 256-entry sin / cos table
+// and the 64-bit fixed-point phase arithmetic, which a backward kernel shares
+// with its forward to reproduce the forward's phase.  Derivations (closed-form phase, Reinsch
 // recurrence, per-row accumulators, live-count Nyquist culling): DESIGN.md 3.1.
 #pragma once
 #include <cmath>
@@ -63,6 +63,38 @@ constexpr int kSinTab = 1 << kSinTabBits;  // 256-entry (sin, cos) table
 // The fused kernels need whole 64-sample chunks per frame.
 inline bool harmonic_fused_supported(const HarmonicParams& p) {
   return (p.hop % 64 == 0) && p.hop <= 8192 && p.K <= 1024;
+}
+
+// The fused forward's launcher, defined in harmonic_v4.cuh and compiled in
+// harmonic.cu only; the decoder in noise.cu launches the kernel through it.
+int launch_harmonic_v4(HarmonicParams p, cudaStream_t st);
+
+// The checks every harmonic entry point makes; `name` prefixes the messages.
+static int harm_check(const char* name, int B, int F, int K, int N, int amp_method,
+                      float sample_rate) {
+  DDSP_REQUIRE(B >= 0 && F >= 1 && K >= 1 && N >= 1, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d F=%d K=%d N=%d", name, B, F, K, N);
+  DDSP_REQUIRE(amp_method == DDSP_B200_AMP_WINDOW || amp_method == DDSP_B200_AMP_LINEAR,
+               DDSP_B200_E_INVALID, "%s: bad amp_method %d", name, amp_method);
+  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID,
+               "%s: sample_rate must be positive", name);
+  return 0;
+}
+
+// HarmonicParams of a harmonic entry point.  The caller sets the fields in which it
+// differs: accumulate, ctl_flags, the phase pointers, mask_nyquist and Kp.
+static HarmonicParams harm_params(const float* f0, const float* amps, const float* hd,
+                                  float* audio, int B, int F, int K, int N,
+                                  float sample_rate, int amp_method) {
+  HarmonicParams p;
+  p.f0 = f0; p.amps = amps; p.hd = hd; p.audio = audio;
+  p.B = B; p.F = F; p.K = K; p.N = N; p.hop = N / F;
+  p.sample_rate = sample_rate; p.nyquist = sample_rate * 0.5f;
+  p.inv_sr = 1.0 / (double)sample_rate;
+  p.amp_method = amp_method; p.accumulate = 0; p.ctl_flags = 0;
+  p.init_phase = nullptr; p.final_phase = nullptr; p.mask_nyquist = 1;
+  p.Kp = (K + 3) & ~3;
+  return p;
 }
 
 // Fixed-point phase (2^64 = one turn) of a frame where a = f / sr goes linearly

@@ -752,7 +752,7 @@ harmonic_v4_kernel(HarmonicParams p, int use_tma, int FW) {
 
 // Returns 0 on success, negative on error, 1 if the tile cannot fit shared memory
 // (the caller then takes the generic kernel).
-inline int launch_harmonic_v4(HarmonicParams p, cudaStream_t st) {
+int launch_harmonic_v4(HarmonicParams p, cudaStream_t st) {
   using namespace hv4;
   p.Kp = (p.K + 3) & ~3;
   // Four warps per CTA and 8 frames per warp: one full record warp for the 32-frame

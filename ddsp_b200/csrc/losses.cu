@@ -1,0 +1,309 @@
+// C ABI of the loss family: the consistency mixture and comb NLLs,
+// sinusoidal_to_harmonic and the HMM, forward and backward.
+#include "capi.cuh"
+#include "consistency.cuh"
+#include "hmm.cuh"
+
+using namespace ddsp;
+
+extern "C" {
+
+// ---- consistency-loss mixture NLLs -------------------------------------------------
+static int cons_rows(const char* name, int B, int T, int64_t* rows) {
+  DDSP_REQUIRE((int64_t)B * T <= INT32_MAX, DDSP_B200_E_INVALID,
+               "%s: B*T=%lld exceeds the 2^31 - 1 grid limit", name, (long long)B * T);
+  *rows = (int64_t)B * T;
+  return 0;
+}
+
+static int mix_check(const char* name, int B, int T, int Q, int J, float scale,
+                     cons_::MixParams* p, int64_t* rows) {
+  DDSP_REQUIRE(B >= 0 && T >= 0 && Q >= 0 && J >= 0, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d T=%d Q=%d J=%d", name, B, T, Q, J);
+  DDSP_REQUIRE(scale > 0.f && scale <= FLT_MAX, DDSP_B200_E_INVALID,
+               "%s: scale must be positive and finite, got %g", name, (double)scale);
+  DDSP_REQUIRE(J <= cons_::kMaxStaged, DDSP_B200_E_UNSUPPORTED,
+               "%s: J=%d components exceed the %d supported", name, J, cons_::kMaxStaged);
+  int rc = cons_rows(name, B, T, rows);
+  if (rc) return rc;
+  p->Q = Q;
+  p->J = J;
+  p->inv_scale = (float)(1.0 / scale);
+  p->log_norm = (float)(std::log((double)scale) + 0.5 * std::log(2.0 * M_PI));
+  return 0;
+}
+
+int ddsp_b200_mixture_nll_forward(const float* x, const float* mu, const float* lw,
+                                  float* nll, int B, int T, int Q, int J, float scale,
+                                  void* stream) {
+  const bool empty = B == 0 || T == 0 || Q == 0 || J == 0;
+  DDSP_REQUIRE(empty || (x && mu && lw && nll), DDSP_B200_E_INVALID,
+               "mixture_nll_forward: null pointer");
+  cons_::MixParams p;
+  int64_t rows = 0;
+  int rc = mix_check("mixture_nll_forward", B, T, Q, J, scale, &p, &rows);
+  if (rc || rows == 0 || Q == 0 || J == 0) return rc;
+  p.x = x; p.mu = mu; p.lw = lw;
+  const size_t smem = sizeof(float) * 2 * (size_t)J;
+  rc = set_smem(cons_::mixture_nll_kernel, smem, "mixture_nll_forward");
+  if (rc) return rc;
+  cons_::mixture_nll_kernel<<<(unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream>>>(
+      p, nll);
+  DDSP_CHECK_LAUNCH("mixture_nll_forward");
+  return 0;
+}
+
+int ddsp_b200_mixture_nll_backward(const float* x, const float* mu, const float* lw,
+                                   const float* grad, float* dx, float* dmu, float* dlw,
+                                   int B, int T, int Q, int J, float scale, void* stream) {
+  const bool empty = B == 0 || T == 0 || Q == 0 || J == 0;
+  DDSP_REQUIRE(empty || (x && mu && lw && grad && dx && dmu && dlw), DDSP_B200_E_INVALID,
+               "mixture_nll_backward: null pointer");
+  cons_::MixParams p;
+  int64_t rows = 0;
+  int rc = mix_check("mixture_nll_backward", B, T, Q, J, scale, &p, &rows);
+  if (rc || rows == 0 || Q == 0 || J == 0) return rc;
+  p.x = x; p.mu = mu; p.lw = lw;
+  const size_t smem = sizeof(float) * (4 * (size_t)J + 5 * cons_::kChunk);
+  rc = set_smem(cons_::mixture_nll_backward_kernel, smem, "mixture_nll_backward");
+  if (rc) return rc;
+  cons_::mixture_nll_backward_kernel<<<(unsigned)rows, cons_::kThreads, smem,
+                                       (cudaStream_t)stream>>>(p, grad, dx, dmu, dlw);
+  DDSP_CHECK_LAUNCH("mixture_nll_backward");
+  return 0;
+}
+
+// Half-width W of the comb window: the smallest W for which the terms |k - k0| > W
+// sum to less than 2^-25 of the largest term, counting each with the weight 1 + |z_k|
+// it carries into d nu / dq.  With k0 the nearest integer, |q - k0| <= 1/2 inside
+// [1/2, G + 1/2], so term n = |k - k0| is at most exp(-n (n - 1) / (2 s^2)) of the
+// largest (outside, every term is further: at most exp(-n^2 / (2 s^2))), twice for the
+// two sides, and |z_k| <= (n + 1/2) / s.
+static int comb_window(int G, double scale) {
+  std::vector<double> tail(G + 2, 0.0);
+  for (int n = G; n >= 1; --n)
+    tail[n] = tail[n + 1] +
+              2.0 * (1.0 + (n + 0.5) / scale) * std::exp(-0.5 * n * (n - 1.0) / (scale * scale));
+  int W = 0;
+  while (W < G && tail[W + 1] >= std::ldexp(1.0, -25)) ++W;
+  return W;
+}
+
+static int comb_check(const char* name, int B, int T, int C, int P, int G, float scale,
+                      cons_::CombParams* p, int64_t* rows) {
+  DDSP_REQUIRE(B >= 0 && T >= 0 && C >= 0 && P >= 0 && G >= 1, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d T=%d C=%d P=%d G=%d", name, B, T, C, P, G);
+  DDSP_REQUIRE(scale > 0.f && scale <= FLT_MAX, DDSP_B200_E_INVALID,
+               "%s: scale must be positive and finite, got %g", name, (double)scale);
+  DDSP_REQUIRE(C <= cons_::kMaxStaged && P <= cons_::kMaxStaged, DDSP_B200_E_UNSUPPORTED,
+               "%s: C=%d candidates or P=%d points exceed the %d supported", name, C, P,
+               cons_::kMaxStaged);
+  int rc = cons_rows(name, B, T, rows);
+  if (rc) return rc;
+  p->C = C;
+  p->P = P;
+  p->G = G;
+  p->inv_scale = (float)(1.0 / scale);
+  p->log_norm = (float)(std::log((double)G) + std::log((double)scale) +
+                        0.5 * std::log(2.0 * M_PI));
+  if (*rows && C && P) p->W = comb_window(G, scale);
+  return 0;
+}
+
+int ddsp_b200_comb_nll_forward(const float* f0, const float* f, const float* a, float* out,
+                               int B, int T, int C, int P, int G, float scale, void* stream) {
+  const bool empty = B == 0 || T == 0 || C == 0 || P == 0;
+  DDSP_REQUIRE(empty || (f0 && f && a && out), DDSP_B200_E_INVALID,
+               "comb_nll_forward: null pointer");
+  cons_::CombParams p;
+  int64_t rows = 0;
+  int rc = comb_check("comb_nll_forward", B, T, C, P, G, scale, &p, &rows);
+  if (rc || rows == 0 || C == 0 || P == 0) return rc;
+  p.f0 = f0; p.f = f; p.a = a;
+  const size_t smem = sizeof(float) * (2 * (size_t)P + C + 1);
+  rc = set_smem(cons_::comb_nll_kernel, smem, "comb_nll_forward");
+  if (rc) return rc;
+  cons_::comb_nll_kernel<<<(unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream>>>(
+      p, out);
+  DDSP_CHECK_LAUNCH("comb_nll_forward");
+  return 0;
+}
+
+int ddsp_b200_comb_nll_backward(const float* f0, const float* f, const float* a,
+                                const float* grad, float* d_f0, float* d_f, float* d_a,
+                                int B, int T, int C, int P, int G, float scale,
+                                void* stream) {
+  const bool empty = B == 0 || T == 0 || C == 0 || P == 0;
+  DDSP_REQUIRE(empty || (f0 && f && a && grad && d_f0 && d_f && d_a), DDSP_B200_E_INVALID,
+               "comb_nll_backward: null pointer");
+  cons_::CombParams p;
+  int64_t rows = 0;
+  int rc = comb_check("comb_nll_backward", B, T, C, P, G, scale, &p, &rows);
+  if (rc || rows == 0 || C == 0 || P == 0) return rc;
+  p.f0 = f0; p.f = f; p.a = a;
+  const size_t smem = sizeof(float) * (2 * (size_t)P + 3 * (size_t)C + 1);
+  rc = set_smem(cons_::comb_nll_backward_kernel, smem, "comb_nll_backward");
+  if (rc) return rc;
+  cons_::comb_nll_backward_kernel<<<(unsigned)rows, cons_::kThreads, smem,
+                                    (cudaStream_t)stream>>>(p, grad, d_f0, d_f, d_a);
+  DDSP_CHECK_LAUNCH("comb_nll_backward");
+  return 0;
+}
+
+// ---- core.sinusoidal_to_harmonic ---------------------------------------------------
+static int s2h_check(const char* name, int B, int T, int S, int K, float width,
+                     float sample_rate, int normalize, cons_::S2HParams* p, int64_t* rows) {
+  DDSP_REQUIRE(B >= 0 && T >= 0 && S >= 0 && K >= 0, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d T=%d S=%d K=%d", name, B, T, S, K);
+  DDSP_REQUIRE(width != 0.f, DDSP_B200_E_INVALID, "%s: harmonic_width must be nonzero",
+               name);
+  DDSP_REQUIRE(normalize == 0 || normalize == 1, DDSP_B200_E_INVALID,
+               "%s: normalize must be 0 or 1, got %d", name, normalize);
+  DDSP_REQUIRE(S <= cons_::kMaxStaged, DDSP_B200_E_UNSUPPORTED,
+               "%s: S=%d sinusoids exceed the %d supported", name, S, cons_::kMaxStaged);
+  int rc = cons_rows(name, B, T, rows);
+  if (rc) return rc;
+  p->S = S;
+  p->K = K;
+  p->width = width;
+  p->nyquist = sample_rate * 0.5f;
+  p->normalize = normalize;
+  return 0;
+}
+
+int ddsp_b200_sinusoidal_to_harmonic(const float* sin_amps, const float* sin_freqs,
+                                     const float* f0_hz, float* harm_amp, float* harm_dist,
+                                     int B, int T, int S, int K, float width,
+                                     float sample_rate, int normalize, void* stream) {
+  const bool empty = B == 0 || T == 0;
+  DDSP_REQUIRE(empty || (f0_hz && harm_amp && (S == 0 || (sin_amps && sin_freqs)) &&
+                         (K == 0 || harm_dist)),
+               DDSP_B200_E_INVALID, "sinusoidal_to_harmonic: null pointer");
+  cons_::S2HParams p;
+  int64_t rows = 0;
+  int rc = s2h_check("sinusoidal_to_harmonic", B, T, S, K, width, sample_rate, normalize, &p,
+                     &rows);
+  if (rc || rows == 0) return rc;
+  p.a = sin_amps; p.f = sin_freqs; p.f0 = f0_hz;
+  const size_t smem = sizeof(float) * (2 * (size_t)S + cons_::kThreads + 1);
+  rc = set_smem(cons_::sin_to_harm_kernel, smem, "sinusoidal_to_harmonic");
+  if (rc) return rc;
+  cons_::sin_to_harm_kernel<<<(unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream>>>(
+      p, harm_amp, harm_dist);
+  DDSP_CHECK_LAUNCH("sinusoidal_to_harmonic");
+  return 0;
+}
+
+int ddsp_b200_sinusoidal_to_harmonic_backward(
+    const float* sin_amps, const float* sin_freqs, const float* f0_hz, const float* grad_amp,
+    const float* grad_dist, float* d_sin_amps, float* d_sin_freqs, float* d_f0_hz, int B,
+    int T, int S, int K, float width, float sample_rate, int normalize, void* stream) {
+  const bool empty = B == 0 || T == 0;
+  DDSP_REQUIRE(empty || (f0_hz && grad_amp && d_f0_hz &&
+                         (S == 0 || (sin_amps && sin_freqs && d_sin_amps && d_sin_freqs)) &&
+                         (K == 0 || grad_dist)),
+               DDSP_B200_E_INVALID, "sinusoidal_to_harmonic_backward: null pointer");
+  cons_::S2HParams p;
+  int64_t rows = 0;
+  int rc = s2h_check("sinusoidal_to_harmonic_backward", B, T, S, K, width, sample_rate,
+                     normalize, &p, &rows);
+  if (rc || rows == 0) return rc;
+  p.a = sin_amps; p.f = sin_freqs; p.f0 = f0_hz;
+  const size_t smem =
+      sizeof(float) * (4 * (size_t)S + 4 * cons_::kHarmChunk + cons_::kThreads + 1);
+  rc = set_smem(cons_::sin_to_harm_backward_kernel, smem, "sinusoidal_to_harmonic_backward");
+  if (rc) return rc;
+  cons_::sin_to_harm_backward_kernel<<<(unsigned)rows, cons_::kThreads, smem,
+                                       (cudaStream_t)stream>>>(
+      p, grad_amp, grad_dist, d_sin_amps, d_sin_freqs, d_f0_hz);
+  DDSP_CHECK_LAUNCH("sinusoidal_to_harmonic_backward");
+  return 0;
+}
+
+// ---- losses.HmmTranscriber -----------------------------------------------------------
+// The checks every HMM entry point makes, and its kernel parameters.
+static int hmm_check(const char* name, const float* obs, const float* loc,
+                     const float* scale, int B, int T, int K, double hold, double other,
+                     hmm_::Params* p) {
+  DDSP_REQUIRE(B >= 0 && T >= 1 && K >= 2, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d T=%d K=%d", name, B, T, K);
+  DDSP_REQUIRE(std::isfinite(hold) && std::isfinite(other) && hold >= 0.0 && other >= 0.0 &&
+                   hold + other > 0.0,
+               DDSP_B200_E_INVALID,
+               "%s: hold=%g and other=%g must be finite, non-negative and not both 0",
+               name, hold, other);
+  DDSP_REQUIRE(K <= hmm_::kMaxStates, DDSP_B200_E_UNSUPPORTED,
+               "%s: K=%d states exceed the %d supported", name, K, hmm_::kMaxStates);
+  p->obs = reinterpret_cast<const float2*>(obs);
+  p->loc = reinterpret_cast<const float2*>(loc);
+  p->scale = reinterpret_cast<const float2*>(scale);
+  p->T = T;
+  p->K = K;
+  p->hold = (float)hold;
+  p->other = (float)other;
+  p->log_hold = (float)std::log(hold);
+  p->log_other = (float)std::log(other);
+  p->log_init = -std::log((double)K);
+  return 0;
+}
+
+static unsigned hmm_threads(int K) { return (unsigned)((K + 31) & ~31); }
+
+int ddsp_b200_hmm_log_prob(const float* obs, const float* loc, const float* scale,
+                           float* log_prob, int B, int T, int K, double hold, double other,
+                           void* stream) {
+  DDSP_REQUIRE(B == 0 || (obs && loc && scale && log_prob), DDSP_B200_E_INVALID,
+               "hmm_log_prob: null pointer");
+  hmm_::Params p;
+  int rc = hmm_check("hmm_log_prob", obs, loc, scale, B, T, K, hold, other, &p);
+  if (rc || B == 0) return rc;
+  hmm_::hmm_log_prob_kernel<<<(unsigned)B, hmm_threads(K), 0, (cudaStream_t)stream>>>(
+      p, log_prob);
+  DDSP_CHECK_LAUNCH("hmm_log_prob");
+  return 0;
+}
+
+int ddsp_b200_hmm_log_prob_backward(const float* obs, const float* loc, const float* scale,
+                                    const float* grad, float* d_obs, float* checkpoints,
+                                    int seg, int B, int T, int K, double hold, double other,
+                                    void* stream) {
+  DDSP_REQUIRE(B == 0 || (obs && loc && scale && grad && d_obs && checkpoints),
+               DDSP_B200_E_INVALID, "hmm_log_prob_backward: null pointer");
+  hmm_::Params p;
+  int rc = hmm_check("hmm_log_prob_backward", obs, loc, scale, B, T, K, hold, other, &p);
+  if (rc) return rc;
+  DDSP_REQUIRE(seg >= 1 && (int64_t)seg * K <= hmm_::kSegFloats, DDSP_B200_E_INVALID,
+               "hmm_log_prob_backward: seg=%d must be at least 1 with seg*K at most %d",
+               seg, hmm_::kSegFloats);
+  if (B == 0) return 0;
+  const size_t smem = sizeof(float) * (size_t)seg * K;
+  rc = set_smem(hmm_::hmm_backward_kernel, smem, "hmm_log_prob_backward");
+  if (rc) return rc;
+  hmm_::hmm_backward_kernel<<<(unsigned)B, hmm_threads(K), smem, (cudaStream_t)stream>>>(
+      p, seg, grad, reinterpret_cast<float2*>(d_obs), checkpoints);
+  DDSP_CHECK_LAUNCH("hmm_log_prob_backward");
+  return 0;
+}
+
+int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale,
+                          int64_t* path, int B, int T, int K, double hold, double other,
+                          void* stream) {
+  DDSP_REQUIRE(B == 0 || (obs && loc && scale && path), DDSP_B200_E_INVALID,
+               "hmm_viterbi: null pointer");
+  hmm_::Params p;
+  int rc = hmm_check("hmm_viterbi", obs, loc, scale, B, T, K, hold, other, &p);
+  if (rc) return rc;
+  const size_t smem = sizeof(uint32_t) * (size_t)T * ((K + 31) / 32 + 1);
+  DDSP_REQUIRE(smem <= hmm_::kViterbiBytes, DDSP_B200_E_UNSUPPORTED,
+               "hmm_viterbi: T=%d steps of K=%d states need %zu B of back pointers, more "
+               "than the %zu supported", T, K, smem, hmm_::kViterbiBytes);
+  if (B == 0) return 0;
+  rc = set_smem(hmm_::hmm_viterbi_kernel, smem, "hmm_viterbi");
+  if (rc) return rc;
+  hmm_::hmm_viterbi_kernel<<<(unsigned)B, hmm_threads(K), smem, (cudaStream_t)stream>>>(
+      p, path);
+  DDSP_CHECK_LAUNCH("hmm_viterbi");
+  return 0;
+}
+
+}  // extern "C"

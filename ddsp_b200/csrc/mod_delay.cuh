@@ -27,7 +27,7 @@
 // d audio is written once per element, without atomics, bit-reproducibly.  The CTA
 // also writes d gain and d phase of the outputs inside its tile.
 #pragma once
-#include "common.cuh"
+#include "taps.cuh"
 
 namespace ddsp {
 namespace md_ {
@@ -94,36 +94,6 @@ mod_delay_forward_kernel(const float* __restrict__ audio, const float* __restric
   float wet = __fadd_rn(__fmul_rn(tp.w0, v0), __fmul_rn(tp.w1, v1));
   if (gain != nullptr) wet = __fmul_rn(wet, __ldg(gain + row + t));
   out[row + t] = add_dry ? __fadd_rn(wet, x[t]) : wet;
-}
-
-// Adds `val` of every lane whose `target` lies in the tile to buf[target - s0].
-// Fast path: valid targets strictly increasing over the lanes (every smooth phase),
-// so no two lanes share one.  Otherwise lanes with one target are summed by the
-// lowest of them, in lane order.  Both give the same bits: a lone lane adds its own
-// value either way.
-__device__ __forceinline__ void scatter_tap(float* buf, float* stage, int target,
-                                            float val, bool valid, int s0, int lane) {
-  int prev = valid ? target : -1;                 // inclusive max scan of valid targets
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, prev, o);
-    if (lane >= o) prev = max(prev, u);
-  }
-  int below = __shfl_up_sync(0xffffffffu, prev, 1);
-  if (lane == 0) below = -1;
-  if (__all_sync(0xffffffffu, !valid || target > below)) {
-    if (valid) buf[target - s0] += val;
-    return;
-  }
-  stage[lane] = val;
-  __syncwarp();
-  const unsigned peers = __match_any_sync(0xffffffffu, valid ? target : -1);
-  if (valid && (peers & ((1u << lane) - 1u)) == 0u) {
-    float sum = 0.f;
-    for (unsigned m = peers; m != 0u; m &= m - 1u) sum += stage[__ffs(m) - 1];
-    buf[target - s0] += sum;
-  }
-  __syncwarp();
 }
 
 // d audio (optional), d gain (optional, needs gain) and d phase (optional) of

@@ -147,4 +147,25 @@ fir_kernel(const float* __restrict__ x, const float* __restrict__ ir,
   ob[o] = acc;
 }
 
+// tf.random.uniform([B, N], -1, 1) stand-in (synths.py:192-193): Philox4x32-10.
+__global__ void __launch_bounds__(256)
+uniform_noise_kernel(float* __restrict__ out, int B, int N, uint64_t seed,
+                     uint64_t offset) {
+  const int n4 = (N + 3) >> 2;
+  const int64_t total = (int64_t)B * n4;
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (; i < total; i += stride) {
+    const int b = (int)(i / n4);
+    const int q = (int)(i - (int64_t)b * n4);
+    const float4 v = noise4((uint32_t)q, (uint32_t)b, seed, offset);
+    float* o = out + (size_t)b * N + 4 * (size_t)q;
+    const int rem = N - 4 * q;
+    o[0] = v.x;
+    if (rem > 1) o[1] = v.y;
+    if (rem > 2) o[2] = v.z;
+    if (rem > 3) o[3] = v.w;
+  }
+}
+
 }  // namespace ddsp

@@ -1,11 +1,11 @@
-// Signal routing and the exponential-decay reverb: the backward of core.resample
-// (core.py:573-714), processors.Mix (processors.py:179-233) forward and backward,
+// Signal routing and the exponential-decay reverb: processors.Add, core.resample
+// (core.py:573-714) and its backward, processors.Mix (processors.py:179-233) forward and backward,
 // and ExpDecayReverb._get_ir (effects.py:144-151) forward and backward.
 //
 // Every gradient is written once per element, without float atomics or memset,
 // and split sums are added in a fixed order, so each is bit-reproducible.
 //
-// resample_backward_kernel is the transpose of resample_kernel (controls.cuh) in
+// resample_backward_kernel is the transpose of resample_kernel (above) in
 // gather form.  Sample t of the forward reads frames lo(t) .. hi(t) (after the
 // clamps), and both are non-decreasing in t, so the samples that reach frame j are
 // one range [t0, t1): t0 the first t with hi(t) >= j, t1 the first t with
@@ -15,96 +15,87 @@
 // share one frame (G = 32 when frames span many samples): lane l walks t0 + l,
 // t0 + l + G, ..., and the lanes are summed by a fixed xor tree.
 #pragma once
-#include "common.cuh"
+#include "taps.cuh"
 
 namespace ddsp {
+
+// processors.Add.get_signal (processors.py:174-176)
+__global__ void __launch_bounds__(256)
+add_kernel(const float* a, const float* b, float* out, int64_t n) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (; i < n; i += stride) out[i] = a[i] + b[i];
+}
+
+// core.resample / core.upsample_with_windows (core.py:573-714) as a stand-alone
+// op: [B, F, C] -> [B, N, C].  method 0 = 'window' (Hann overlap-add ==
+// two-tap raised cosine, SURVEY A.2), 1 = 'linear' (tf v1 bilinear,
+// align_corners = !add_endpoint), 2 = 'nearest', 3 = 'cubic' (tf v1 bicubic).  Index math follows TF's
+// float32 scale * index for linear / nearest; the window method needs an integer
+// hop (checked by the caller, core.py:687-693).
+__global__ void __launch_bounds__(256)
+resample_kernel(const float* __restrict__ in, float* __restrict__ out, int B, int F,
+                int C, int N, int method, int add_endpoint) {
+  const int64_t total = (int64_t)B * N * C;
+  int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  const float scale = (!add_endpoint && N > 1) ? (float)(F - 1) / (float)(N - 1)
+                                               : (float)F / (float)N;
+  const int hop = add_endpoint ? N / max(F, 1) : N / max(F - 1, 1);
+  for (; idx < total; idx += stride) {
+    const int c = (int)(idx % C);
+    const int64_t bt = idx / C;
+    const int t = (int)(bt % N);
+    const int b = (int)(bt / N);
+    const float* x = in + (size_t)b * F * C + c;
+    float v;
+    if (method == 0) {
+      const int i = t / hop, r = t - i * hop;
+      const int i1 = min(i + 1, F - 1);            // add_endpoint: frame F := F-1
+      const float w1 = 0.5f - 0.5f * cospif((float)r / (float)hop);
+      v = x[(size_t)i * C] * (1.0f - w1) + x[(size_t)i1 * C] * w1;
+    } else if (method == 1) {
+      const float src = (float)t * scale;
+      const float fl = floorf(src);
+      const int lo = max((int)fl, 0);
+      const int hi = min((int)ceilf(src), F - 1);
+      const float top = x[(size_t)min(lo, F - 1) * C], bot = x[(size_t)hi * C];
+      v = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), src - fl));
+    } else if (method == 2) {
+      const float src = (float)t * scale;
+      const int i = min((int)(add_endpoint ? floorf(src) : roundf(src)), F - 1);
+      v = x[(size_t)i * C];
+    } else {
+      // 'cubic': TensorFlow's legacy bicubic kernel (resize_bicubic_op.cc, Keys
+      // A = -0.75, no half-pixel centres).  Its weights come from a 1025-entry
+      // float32 table indexed by lrintf(delta * 1024); the same entries are
+      // evaluated here in double and rounded to float32.
+      const float src = (float)t * scale;
+      const float fl = floorf(src);
+      const int loc = (int)fl;
+      const int off = (int)lrintf((src - fl) * 1024.0f);
+      const double A = -0.75;
+      const double xa = off * (1.0 / 1024.0), xb = (1024 - off) * (1.0 / 1024.0);
+      const float w1 = (float)(((A + 2) * xa - (A + 3)) * xa * xa + 1);
+      const float w2 = (float)(((A + 2) * xb - (A + 3)) * xb * xb + 1);
+      const double ya = xa + 1.0, yb = xb + 1.0;
+      const float w0 = (float)(((A * ya - 5 * A) * ya + 8 * A) * ya - 4 * A);
+      const float w3 = (float)(((A * yb - 5 * A) * yb + 8 * A) * yb - 4 * A);
+      const float v0 = x[(size_t)min(max(loc - 1, 0), F - 1) * C];
+      const float v1 = x[(size_t)min(max(loc, 0), F - 1) * C];
+      const float v2 = x[(size_t)min(max(loc + 1, 0), F - 1) * C];
+      const float v3 = x[(size_t)min(max(loc + 2, 0), F - 1) * C];
+      v = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(v0, w0), __fmul_rn(v1, w1)),
+                              __fmul_rn(v2, w2)), __fmul_rn(v3, w3));
+    }
+    out[idx] = v;
+  }
+}
+
 namespace rt_ {
 
 constexpr int kThreads = 256;
 constexpr int kIrBwdThreads = 512;
-
-struct ResampleGeom {
-  int F, N, method, add_endpoint;
-  float scale;   // the forward's float32 index scale
-  int hop;       // 'window' only
-};
-
-__host__ __device__ inline ResampleGeom resample_geom(int F, int N, int method,
-                                                       int add_endpoint) {
-  ResampleGeom g;
-  g.F = F; g.N = N; g.method = method; g.add_endpoint = add_endpoint;
-  g.scale = (!add_endpoint && N > 1) ? (float)(F - 1) / (float)(N - 1)
-                                     : (float)F / (float)N;
-  const int den = add_endpoint ? (F > 1 ? F : 1) : (F - 1 > 1 ? F - 1 : 1);
-  g.hop = N / den;
-  return g;
-}
-
-__device__ __forceinline__ int clampi(int v, int lo, int hi) { return min(max(v, lo), hi); }
-
-// The frames sample t reads, and their weights, exactly as resample_kernel
-// computes them.  Returns the tap count (1, 2 or 4).
-__device__ __forceinline__ int resample_taps(const ResampleGeom& g, int t, int* idx,
-                                             float* w) {
-  if (g.method == 0) {
-    const int i = t / g.hop, r = t - i * g.hop;
-    const float w1 = 0.5f - 0.5f * cospif((float)r / (float)g.hop);
-    idx[0] = i; w[0] = 1.0f - w1;
-    idx[1] = min(i + 1, g.F - 1); w[1] = w1;
-    return 2;
-  }
-  const float src = (float)t * g.scale;
-  const float fl = floorf(src);
-  if (g.method == 1) {
-    idx[0] = min(max((int)fl, 0), g.F - 1); w[0] = 1.0f - (src - fl);
-    idx[1] = min((int)ceilf(src), g.F - 1); w[1] = src - fl;
-    return 2;
-  }
-  if (g.method == 2) {
-    idx[0] = min((int)(g.add_endpoint ? floorf(src) : roundf(src)), g.F - 1);
-    w[0] = 1.0f;
-    return 1;
-  }
-  const int loc = (int)fl;
-  const int off = (int)lrintf((src - fl) * 1024.0f);
-  const double A = -0.75;
-  const double xa = off * (1.0 / 1024.0), xb = (1024 - off) * (1.0 / 1024.0);
-  const double ya = xa + 1.0, yb = xb + 1.0;
-  w[0] = (float)(((A * ya - 5 * A) * ya + 8 * A) * ya - 4 * A);
-  w[1] = (float)(((A + 2) * xa - (A + 3)) * xa * xa + 1);
-  w[2] = (float)(((A + 2) * xb - (A + 3)) * xb * xb + 1);
-  w[3] = (float)(((A * yb - 5 * A) * yb + 8 * A) * yb - 4 * A);
-#pragma unroll
-  for (int k = 0; k < 4; ++k) idx[k] = clampi(loc - 1 + k, 0, g.F - 1);
-  return 4;
-}
-
-// lowest / highest frame sample t reads (non-decreasing in t)
-__device__ __forceinline__ int resample_lo(const ResampleGeom& g, int t) {
-  if (g.method == 0) return t / g.hop;
-  const float src = (float)t * g.scale;
-  if (g.method == 1) return min(max((int)floorf(src), 0), g.F - 1);
-  if (g.method == 2) return min((int)(g.add_endpoint ? floorf(src) : roundf(src)), g.F - 1);
-  return clampi((int)floorf(src) - 1, 0, g.F - 1);
-}
-__device__ __forceinline__ int resample_hi(const ResampleGeom& g, int t) {
-  if (g.method == 0) return min(t / g.hop + 1, g.F - 1);
-  const float src = (float)t * g.scale;
-  if (g.method == 1) return min((int)ceilf(src), g.F - 1);
-  if (g.method == 2) return min((int)(g.add_endpoint ? floorf(src) : roundf(src)), g.F - 1);
-  return clampi((int)floorf(src) + 2, 0, g.F - 1);
-}
-
-// first t in [0, N) with hi(t) >= j (use_hi) or lo(t) > j (!use_hi); N if none
-__device__ __forceinline__ int resample_bound(const ResampleGeom& g, int j, bool use_hi) {
-  int a = 0, b = g.N;
-  while (a < b) {
-    const int m = a + ((b - a) >> 1);
-    const bool past = use_hi ? resample_hi(g, m) >= j : resample_lo(g, m) > j;
-    if (past) b = m; else a = m + 1;
-  }
-  return a;
-}
 
 // d in [B, F, C] from d out [B, N, C]: G lanes (1 or a whole warp) per (b, j, c),
 // grid-stride; for G = 32 the output index is warp-uniform.

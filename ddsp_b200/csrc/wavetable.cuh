@@ -27,7 +27,7 @@
 //        p1 = r (r - 1) / (2 hop), p0 = r - p1, then sinus_bwd_finalize (K = 1)
 //   6.   wt_bwd_table: d wavetables.  A CTA owns one table frame, one segment of
 //        the samples that read it and one range of columns; each warp scatters
-//        into its own shared buffer with mod_delay.cuh's scatter_tap (strictly
+//        into its own shared buffer with taps.cuh's scatter_tap (strictly
 //        increasing targets, else lanes with one target summed in lane order),
 //        and the warp buffers are added in warp order.  Several segments
 //        (static tables, few table frames) leave partial tables that
@@ -37,9 +37,8 @@
 // bit-reproducible.
 #pragma once
 #include "harmonic_common.cuh"
-#include "mod_delay.cuh"
-#include "routing.cuh"
 #include "sinusoidal.cuh"
+#include "taps.cuh"
 
 namespace ddsp {
 namespace wt_ {

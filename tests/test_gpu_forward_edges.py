@@ -413,7 +413,7 @@ def test_streaming_harmonic_several_tiles_wide(B, F, K, hop, method, init):
   fit shared memory, and initial phases near 0 and near 2 pi, against the oracle."""
   N = F * hop
   f0, amp, hd = _streaming_inputs(B, F, K, seed=F + K)
-  ft0 = min(F, 2048 // hop)           # frames per tile before fit_tile (capi.cu)
+  ft0 = min(F, 2048 // hop)           # frames per tile before fit_tile (harmonic.cu)
   ft = ft0
   while ft > 1 and 8 * (3 * ft + 8) + 4 * (2 * (ft + 1) + (ft + 1) * ((K + 3) & ~3)) > \
       200 * 1024:                      # harm_smem_bytes > kMaxDynSmem
