@@ -168,6 +168,10 @@ SIGNATURES = {
     'ddsp_b200_hmm_log_prob_backward':
         (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _d, _d, _vp]),
     'ddsp_b200_hmm_viterbi': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _d, _d, _vp]),
+    'ddsp_b200_wasserstein_forward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _f, _vp]),
+    'ddsp_b200_wasserstein_backward':
+        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _f, _vp]),
 }
 
 _lib = None

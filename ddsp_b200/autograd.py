@@ -797,6 +797,36 @@ class HmmLogProbFn(torch.autograd.Function):
     return d_x, None, None, None, None
 
 
+
+class WassersteinFn(torch.autograd.Function):
+  """losses.wasserstein_distance on [R, Nu] values u and weights wu, [R, Nv] values v and
+  weights wv (csrc/wasserstein.cuh): the [R] distances, differentiable in all four by one
+  backward launch that re-sorts each row.  Nothing but the inputs is saved.  Empty sides
+  are refused by the caller; R = 0 launches nothing."""
+
+  @staticmethod
+  def forward(ctx, u, v, wu, wv, p):
+    u, v, wu, wv = (t.contiguous().to(torch.float32) for t in (u, v, wu, wv))
+    ctx.save_for_backward(u, v, wu, wv)
+    ctx.p = float(p)
+    r, nu = u.shape
+    out = torch.empty((r,), dtype=torch.float32, device=u.device)
+    core._launch('ddsp_b200_wasserstein_forward', u, v, wu, wv, out, r, nu, v.shape[1],
+                 ctx.p)
+    return out
+
+  @staticmethod
+  def backward(ctx, grad):
+    u, v, wu, wv = ctx.saved_tensors
+    r, nu = u.shape
+    du, dv, dwu, dwv = (torch.empty_like(t) for t in (u, v, wu, wv))
+    core._launch('ddsp_b200_wasserstein_backward', u, v, wu, wv,
+                 grad.contiguous().to(torch.float32), du, dv, dwu, dwv, r, nu, v.shape[1],
+                 ctx.p)
+    want = ctx.needs_input_grad
+    return (du if want[0] else None, dv if want[1] else None, dwu if want[2] else None,
+            dwv if want[3] else None, None)
+
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):
   """core.exp_sigmoid (core.py:386-404) as differentiable torch ops."""
   return max_value * torch.sigmoid(x)**math.log(exponent) + threshold

@@ -557,6 +557,13 @@ def sinusoidal_to_harmonic(sin_amps, sin_freqs, f0_hz, harmonic_width=0.1,
 
 
 # ----------------------------------------------------------------------------
+# losses.wasserstein_distance (losses.py:641-686): csrc/wasserstein.cuh
+# ----------------------------------------------------------------------------
+WASSERSTEIN_MAX_SIDE = 4096    # values per side one CTA sorts in shared memory
+WASSERSTEIN_MAX_ROWS = 2**31 - 1
+
+
+# ----------------------------------------------------------------------------
 # The HMM of losses.HmmTranscriber (losses.py:247-345): csrc/hmm.cuh
 # ----------------------------------------------------------------------------
 HMM_MAX_STATES = 1024          # states one CTA runs, a thread each

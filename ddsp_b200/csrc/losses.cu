@@ -1,8 +1,9 @@
 // C ABI of the loss family: the consistency mixture and comb NLLs,
-// sinusoidal_to_harmonic and the HMM, forward and backward.
+// sinusoidal_to_harmonic, the HMM and the Wasserstein distance, forward and backward.
 #include "capi.cuh"
 #include "consistency.cuh"
 #include "hmm.cuh"
+#include "wasserstein.cuh"
 
 using namespace ddsp;
 
@@ -303,6 +304,65 @@ int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale
   hmm_::hmm_viterbi_kernel<<<(unsigned)B, hmm_threads(K), smem, (cudaStream_t)stream>>>(
       p, path);
   DDSP_CHECK_LAUNCH("hmm_viterbi");
+  return 0;
+}
+
+// ---- losses.wasserstein_distance ------------------------------------------------------
+static int ws_check(const char* name, int64_t R, int Nu, int Nv, float p, ws_::Params* wp) {
+  DDSP_REQUIRE(R >= 0 && Nu >= 0 && Nv >= 0, DDSP_B200_E_INVALID,
+               "%s: bad shape R=%lld Nu=%d Nv=%d", name, (long long)R, Nu, Nv);
+  DDSP_REQUIRE(p > 0.f && p <= FLT_MAX, DDSP_B200_E_INVALID,
+               "%s: p must be positive and finite, got %g", name, (double)p);
+  DDSP_REQUIRE(Nu <= ws_::kMaxSide && Nv <= ws_::kMaxSide, DDSP_B200_E_UNSUPPORTED,
+               "%s: Nu=%d or Nv=%d elements exceed the %d supported per side", name, Nu, Nv,
+               ws_::kMaxSide);
+  DDSP_REQUIRE(R <= INT32_MAX, DDSP_B200_E_INVALID,
+               "%s: R=%lld exceeds the 2^31 - 1 grid limit", name, (long long)R);
+  wp->Nu = Nu;
+  wp->Nv = Nv;
+  wp->p = p;
+  wp->inv_p = (float)(1.0 / (double)p);
+  return 0;
+}
+
+int ddsp_b200_wasserstein_forward(const float* u, const float* v, const float* wu,
+                                  const float* wv, float* out, int64_t R, int Nu, int Nv,
+                                  float p, void* stream) {
+  const bool empty = R == 0 || Nu == 0 || Nv == 0;
+  DDSP_REQUIRE(empty || (u && v && wu && wv && out), DDSP_B200_E_INVALID,
+               "wasserstein_forward: null pointer");
+  ws_::Params wp;
+  int rc = ws_check("wasserstein_forward", R, Nu, Nv, p, &wp);
+  if (rc || empty) return rc;
+  wp.u = u; wp.v = v; wp.wu = wu; wp.wv = wv;
+  const int m = ws_::padded(Nu + Nv);
+  const size_t smem = ws_::smem_bytes(m);
+  rc = set_smem(ws_::wasserstein_kernel, smem, "wasserstein_forward");
+  if (rc) return rc;
+  ws_::wasserstein_kernel<<<(unsigned)R, ws_::threads_for(m), smem, (cudaStream_t)stream>>>(
+      wp, out);
+  DDSP_CHECK_LAUNCH("wasserstein_forward");
+  return 0;
+}
+
+int ddsp_b200_wasserstein_backward(const float* u, const float* v, const float* wu,
+                                   const float* wv, const float* grad, float* du, float* dv,
+                                   float* dwu, float* dwv, int64_t R, int Nu, int Nv, float p,
+                                   void* stream) {
+  const bool empty = R == 0 || Nu == 0 || Nv == 0;
+  DDSP_REQUIRE(empty || (u && v && wu && wv && grad && du && dv && dwu && dwv),
+               DDSP_B200_E_INVALID, "wasserstein_backward: null pointer");
+  ws_::Params wp;
+  int rc = ws_check("wasserstein_backward", R, Nu, Nv, p, &wp);
+  if (rc || empty) return rc;
+  wp.u = u; wp.v = v; wp.wu = wu; wp.wv = wv;
+  const int m = ws_::padded(Nu + Nv);
+  const size_t smem = ws_::smem_bytes(m);
+  rc = set_smem(ws_::wasserstein_backward_kernel, smem, "wasserstein_backward");
+  if (rc) return rc;
+  ws_::wasserstein_backward_kernel<<<(unsigned)R, ws_::threads_for(m), smem,
+                                     (cudaStream_t)stream>>>(wp, grad, du, dv, dwu, dwv);
+  DDSP_CHECK_LAUNCH("wasserstein_backward");
   return 0;
 }
 

@@ -4,7 +4,9 @@ consistency losses of the self-supervised pitch model (`losses.py:489-1076`).  T
 Gaussian mixtures of `KDEConsistencyLoss` and `TWMLoss` are evaluated per frame by
 the CUDA kernels of `csrc/consistency.cuh` (`autograd.MixtureNLLFn`, `CombNLLFn`);
 the [B, T, K]-sized elementwise work around them is torch autograd.  The HMM of
-`HmmTranscriber` (`losses.py:247-345`) runs on the kernels of `csrc/hmm.cuh`."""
+`HmmTranscriber` (`losses.py:247-345`) runs on the kernels of `csrc/hmm.cuh`, and
+`wasserstein_distance` (`losses.py:641-686`) on those of `csrc/wasserstein.cuh`.
+`LossGroup` (`losses.py:50-98`) runs a DAG of losses."""
 import functools
 import math
 import re
@@ -14,6 +16,7 @@ import torch
 
 from ddsp_b200 import autograd
 from ddsp_b200 import core
+from ddsp_b200 import dags
 from ddsp_b200 import spectral_ops
 from ddsp_b200.core import hz_to_midi, safe_divide
 
@@ -54,6 +57,36 @@ class Loss:
 
   def get_losses_dict(self, *args, **kwargs):
     return {self.name: self(*args, **kwargs)}
+
+
+class LossGroup(dags.DAGLayer):
+  """losses.LossGroup (losses.py:50-98): the losses of a DAG, each node a loss (or its
+  keyword name) and the nested keys of its inputs, e.g.
+  [['f0_loss', ['f0_midi', 'f0_midi_pred', 'f0_loss_weights']], ...].  Keyword losses
+  become attributes of the group; `name=` is split off as the group's own name.  Called
+  on a dict of outputs, it returns the flat {loss.name: value} of every loss, in
+  `loss_names` order; a keyword loss that no node runs raises KeyError there."""
+
+  def __init__(self, dag, **kwarg_losses):
+    super().__init__(dag, **kwarg_losses)
+    if kwarg_losses.get('name') is None:
+      self.name = 'loss_group'
+    self.loss_names = self.module_names
+
+  @property
+  def losses(self):
+    return [getattr(self, name) for name in self.loss_names]
+
+  def call(self, outputs, **kwargs):
+    dag_outputs = super().call(outputs, **kwargs)
+    loss_outputs = {}
+    for k in self.loss_names:
+      loss_outputs.update(dag_outputs[k])
+    return loss_outputs
+
+  def get_losses_dict(self, outputs, **kwargs):
+    """The same dict as calling the group."""
+    return self(outputs, **kwargs)
 
 
 class SpectralLoss:
@@ -405,6 +438,89 @@ class TWMLoss(Loss):
       return f0_candidates[..., None] * n
     midi = hz_to_midi(f0_candidates)[..., None] + 12.0 * torch.log2(n)
     return torch.where(f0_candidates[..., None] <= 0.0, torch.zeros_like(midi), midi)
+
+
+# ------------------------------------------------------------------------------
+# Wasserstein consistency (losses.py:584-686)
+# ------------------------------------------------------------------------------
+def _check_wasserstein(u_values, v_values, u_weights, v_weights, p):
+  """The checks of wasserstein_distance, before any device work; returns the batch shape
+  and the two side lengths."""
+  name = 'wasserstein_distance'
+  if u_weights is None or v_weights is None:
+    raise ValueError(f'{name}: u_weights and v_weights are required.  The reference '
+                     'cannot evaluate None weights (it multiplies a float64 CDF by the '
+                     'float32 values), and no normalised variant is offered.')
+  su, sv = core._shape(u_values), core._shape(v_values)
+  swu, swv = core._shape(u_weights), core._shape(v_weights)
+  if len(su) < 1 or swu != su:
+    raise ValueError(f'{name}: u_values {su} and u_weights {swu} must be one shape '
+                     '[*batch, n_u]')
+  if len(sv) < 1 or swv != sv:
+    raise ValueError(f'{name}: v_values {sv} and v_weights {swv} must be one shape '
+                     '[*batch, n_v]')
+  if su[:-1] != sv[:-1]:
+    raise ValueError(f'{name}: u has batch shape {su[:-1]}, v {sv[:-1]}')
+  if su[-1] < 1 or sv[-1] < 1:
+    raise ValueError(f'{name}: each side needs at least one value, got n_u={su[-1]} and '
+                     f'n_v={sv[-1]} (the reference cannot evaluate an empty side)')
+  p = float(p)
+  if not (p > 0.0 and math.isfinite(p)):
+    raise ValueError(f'{name}: p must be positive and finite, got {p}')
+  limit = core.WASSERSTEIN_MAX_SIDE
+  if su[-1] > limit or sv[-1] > limit:
+    raise NotImplementedError(f'{name}: n_u={su[-1]} or n_v={sv[-1]} values exceed the '
+                              f'{limit} per side the kernel sorts.')
+  rows = math.prod(su[:-1])
+  if rows > core.WASSERSTEIN_MAX_ROWS:
+    raise NotImplementedError(f'{name}: {rows} rows exceed the {core.WASSERSTEIN_MAX_ROWS} '
+                              'the kernel launches.')
+  return su[:-1], su[-1], sv[-1]
+
+
+@core.on_operands_device
+def wasserstein_distance(u_values, v_values, u_weights, v_weights, p=1.0):
+  """losses.wasserstein_distance (losses.py:641-686), [*batch], for values and weights
+  [*batch, n_u] and [*batch, n_v]: (sum_i delta_i |U_i - V_i|^p)^(1/p) over the gaps
+  delta_i of the sorted union, with U_i and V_i the cumulative weights at or below its
+  i-th value.  As in the reference the cumulative weights are not normalised (its
+  normalisation is computed and discarded), so weight totals that differ add their
+  difference.  One launch of `autograd.WassersteinFn` forward and one backward, with
+  gradients to all four inputs.  None weights, shapes that differ, empty sides and p
+  not positive and finite raise ValueError, more than 4096 values per side
+  NotImplementedError, before any device work."""
+  batch, nu, nv = _check_wasserstein(u_values, v_values, u_weights, v_weights, p)
+  u, v, wu, wv = (core.torch_float32(x) for x in (u_values, v_values, u_weights, v_weights))
+  out = autograd.WassersteinFn.apply(u.reshape(-1, nu), v.reshape(-1, nv),
+                                     wu.reshape(-1, nu), wv.reshape(-1, nv), float(p))
+  return out.reshape(batch)
+
+
+class WassersteinConsistencyLoss(Loss):
+  """losses.WassersteinConsistencyLoss (losses.py:584-638): weight * the mean over
+  [batch, time] of the p = 1 Wasserstein distance between the sinusoids a and b in MIDI
+  (core.hz_to_midi: 0 Hz and below map to MIDI 0), amplitude-weighted.  As in the
+  reference it is the plain number 0.0 unless weight > 0 and midi is true.  amps_a and
+  freqs_a are [batch, time, n_a], amps_b and freqs_b [batch, time, n_b]; other shapes
+  raise ValueError before any device work."""
+
+  def __init__(self, weight=1.0, midi=True, name=None):
+    super().__init__(name)
+    self.weight = weight
+    self.midi = midi
+
+  def call(self, amps_a, freqs_a, amps_b, freqs_b):
+    _check_sinusoids('WassersteinConsistencyLoss',
+                     [('amps_a, freqs_a', amps_a, freqs_a),
+                      ('amps_b, freqs_b', amps_b, freqs_b)])
+    loss = 0.0
+    if self.weight > 0.0 and self.midi:
+      amps_a, freqs_a, amps_b, freqs_b = (
+          core.torch_float32(x) for x in (amps_a, freqs_a, amps_b, freqs_b))
+      dist = wasserstein_distance(hz_to_midi(freqs_a), hz_to_midi(freqs_b), amps_a, amps_b,
+                                  p=1.0)
+      loss = torch.mean(self.weight * dist)
+    return loss
 
 
 # ------------------------------------------------------------------------------

@@ -716,6 +716,32 @@ int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale
                           int64_t* path, int B, int T, int K, double hold, double other,
                           void* stream);
 
+/* losses.wasserstein_distance (losses.py:641-686): for R rows of values u [R,Nu] and
+ * v [R,Nv] with weights wu [R,Nu] and wv [R,Nv], s = sort(concat(u, v)) (stable: u before
+ * v, lower index first; -0 ties with +0, NaNs sort last), N = Nu + Nv and i = 0 .. N-2,
+ *   out[r] = (sum_i (s_{i+1} - s_i) |U_i - V_i|^p)^(1/p),
+ *   U_i = sum_k wu_k [u_k <= s_i],  V_i = sum_k wv_k [v_k <= s_i].
+ * The CDFs are raw cumulative weights, not normalised, as the reference computes them.
+ * p positive and finite; Nu, Nv <= 4096 (more is E_UNSUPPORTED); R <= 2^31 - 1.  No
+ * workspace.  R, Nu or Nv = 0 returns after the checks without a launch and writes
+ * nothing (the pointers may then be null).  One CTA per row sorts, scans and sums in
+ * shared memory: nothing but out is written.
+ * backward: for grad [R], du [R,Nu], dv [R,Nv], dwu [R,Nu] and dwv [R,Nv], all written.
+ * With c_i = |U_i - V_i|^p, S = sum_i delta_i c_i, G = grad (1/p) S^(1/p - 1) and
+ * g_i = G delta_i p |U_i - V_i|^(p-1) sgn(U_i - V_i):
+ *   the element sorted to position j gets G c_{j-1} [j >= 1] - G c_j [j <= N-2],
+ *   dwu_k = sum_{i: s_i >= u_k} g_i,  dwv_k = -sum_{i: s_i >= v_k} g_i.
+ * An exact U_i = V_i at p < 1, or S = 0 at p > 1, gives NaN (0 * inf) as autograd does;
+ * at p = 1 everything finite stays finite.  Fixed-order scans and sums, no atomics:
+ * bit-reproducible. */
+int ddsp_b200_wasserstein_forward(const float* u, const float* v, const float* wu,
+                                  const float* wv, float* out, int64_t R, int Nu, int Nv,
+                                  float p, void* stream);
+int ddsp_b200_wasserstein_backward(const float* u, const float* v, const float* wu,
+                                   const float* wv, const float* grad, float* du, float* dv,
+                                   float* dwu, float* dwv, int64_t R, int Nu, int Nv, float p,
+                                   void* stream);
+
 #ifdef __cplusplus
 }
 #endif

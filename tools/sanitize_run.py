@@ -110,6 +110,12 @@ hmm.nll(hp, ha).backward()
 hq = hmm.predict_midi(hp, ha)
 torch.cuda.synchronize()
 assert torch.isfinite(hp.grad).all() and bool(((hq >= 0) & (hq < 45)).all())
+# wasserstein_distance: unequal sides with ties, forward and backward
+wx = [torch.round(4.0 * torch.rand(3, n, device='cuda')).requires_grad_(True) for n in (37, 70)]
+ww = [torch.rand(3, n, device='cuda').requires_grad_(True) for n in (37, 70)]
+losses.wasserstein_distance(wx[0], wx[1], ww[0], ww[1]).sum().backward()
+torch.cuda.synchronize()
+assert all(torch.isfinite(t.grad).all() for t in wx + ww)
 print('sanitize_run ok', float(a.abs().mean()), float(b.abs().mean()),
       float(c.abs().mean()), float(d.abs().mean()),
       float(raw['harmonic_distribution'].grad.abs().mean()))
