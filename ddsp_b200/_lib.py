@@ -1,178 +1,89 @@
-"""ctypes binding of libddsp_b200.so (the C ABI in include/ddsp_b200.h).
+"""ctypes binding of libddsp_b200.so, derived at import from its C ABI,
+include/ddsp_b200.h: every `ddsp_b200_*` prototype becomes an entry of SIGNATURES,
+and every `DDSP_B200_*` enum value or integer #define a module attribute without
+the prefix (E_INVALID, PAD_SAME, HMM_MAX_STATES, ...).
 
 There is NO fallback: if the shared library is missing or fails to load, every
 op raises.  Build it with `python -m ddsp_b200.build` (needs nvcc, not a GPU).
 """
 import ctypes
 import os
+import re
 import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libddsp_b200.so')
+HEADER_PATH = os.path.join(_HERE, '..', 'include', 'ddsp_b200.h')
 
-OK = 0
-E_INVALID = -1
-E_UNSUPPORTED = -2
-E_CUDA = -3
-E_WORKSPACE = -4
+_sz = ctypes.c_size_t   # the type of every workspace size
 
-AMP_WINDOW = 0
-AMP_LINEAR = 1
-PHASE_RECURRENCE = 0
-PHASE_DIRECT = 1
-CTL_SCALE = 1
-CTL_NYQUIST = 2
-PAD_SAME = 0
-PAD_VALID = 1
-PAD_CENTER = 2
-PADDING = {'same': PAD_SAME, 'valid': PAD_VALID, 'center': PAD_CENTER}
-MEL = 0
-LOGMEL = 1
-MFCC = 2
-LTI_REVERSE_AUDIO = 1
-LTI_REVERSE_IR = 2
-
-_c_float_p = ctypes.c_void_p  # device pointers travel as integers
-_i = ctypes.c_int
-_i64 = ctypes.c_int64
-_u64 = ctypes.c_uint64
-_f = ctypes.c_float
-_d = ctypes.c_double
-_vp = ctypes.c_void_p
-_sz = ctypes.c_size_t
-
-# name -> (restype, argtypes); mirrors include/ddsp_b200.h one to one.
-SIGNATURES = {
-    'ddsp_b200_version': (_i, []),
-    'ddsp_b200_last_error': (ctypes.c_char_p, []),
-    'ddsp_b200_launch_count': (_u64, []),
-    'ddsp_b200_harmonic_controls':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp]),
-    'ddsp_b200_harmonic_forward':
-        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _i, _i, _vp]),
-    'ddsp_b200_streaming_harmonic_forward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp]),
-    'ddsp_b200_noise_controls': (_i, [_vp, _vp, _i64, _f, _i, _vp]),
-    'ddsp_b200_ir_size': (_i, [_i, _i]),
-    'ddsp_b200_frequency_impulse_response':
-        (_i, [_vp, _vp, _i64, _i, _i, _vp]),
-    'ddsp_b200_fir_time_varying':
-        (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
-    'ddsp_b200_uniform_noise': (_i, [_vp, _i, _i, _u64, _u64, _vp]),
-    'ddsp_b200_filtered_noise_workspace': (_sz, [_i, _i, _i, _i, _i]),
-    'ddsp_b200_filtered_noise_forward':
-        (_i, [_vp, _vp, _u64, _u64, _vp, _i, _i, _i, _i, _i, _i, _vp, _sz,
-              _vp]),
-    'ddsp_b200_decoder_forward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _u64, _u64, _vp, _i, _i, _i, _i, _i, _f,
-              _i, _i, _i, _f, _vp]),
-    'ddsp_b200_host_pipeline_create':
-        (_i, [ctypes.POINTER(_vp), _i, _i, _i, _i, _i, _i]),
-    'ddsp_b200_host_pipeline_destroy': (_i, [_vp]),
-    'ddsp_b200_decoder_forward_host':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _u64, _u64, _vp, _i, _i, _f, _i, _i, _i,
-              _f, _vp]),
-    'ddsp_b200_harmonic_backward':
-        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp]),
-    'ddsp_b200_harmonic_backward_f0':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
-    'ddsp_b200_harmonic_controls_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp]),
-    'ddsp_b200_harmonic_controls_vjp':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp]),
-    'ddsp_b200_noise_controls_backward': (_i, [_vp, _vp, _vp, _i64, _f, _vp]),
-    'ddsp_b200_filtered_noise_backward':
-        (_i, [_vp, _vp, _u64, _u64, _vp, _i, _i, _i, _i, _i, _vp]),
-    'ddsp_b200_fir_time_varying_backward_workspace': (_sz, [_i, _i, _i, _i, _i]),
-    'ddsp_b200_fir_time_varying_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
-    'ddsp_b200_frequency_impulse_response_backward':
-        (_i, [_vp, _vp, _i64, _i, _i, _vp]),
-    'ddsp_b200_frequency_filter_backward_workspace':
-        (_sz, [_i, _i, _i, _i, _i, _i, _i]),
-    'ddsp_b200_frequency_filter_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
-    'ddsp_b200_sinc_impulse_response': (_i, [_vp, _vp, _i64, _i, _f, _i, _vp]),
-    'ddsp_b200_sinc_impulse_response_backward':
-        (_i, [_vp, _vp, _vp, _i64, _i, _f, _i, _vp]),
-    'ddsp_b200_sinc_filter':
-        (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _i, _i, _vp]),
-    'ddsp_b200_sinc_filter_backward_workspace': (_sz, [_i, _i, _i, _i, _i]),
-    'ddsp_b200_sinc_filter_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _i, _vp, _sz, _vp]),
-    'ddsp_b200_oscillator_bank_workspace': (_sz, [_i, _i, _i]),
-    'ddsp_b200_oscillator_bank':
-        (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
-    'ddsp_b200_oscillator_bank_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _i, _vp]),
-    'ddsp_b200_resample': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
-    'ddsp_b200_fft_convolve_lti_workspace': (_sz, [_i, _i, _i, _i]),
-    'ddsp_b200_fft_convolve_lti':
-        (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
-    'ddsp_b200_angular_cumsum':
-        (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _sz, _vp]),
-    'ddsp_b200_angular_cumsum_backward': (_i, [_vp, _vp, _i, _i, _i, _vp]),
-    'ddsp_b200_oscillator_bank_tf_sequential':
-        (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _i, _i, _vp]),
-    'ddsp_b200_sinusoidal_workspace': (_sz, [_i, _i, _i]),
-    'ddsp_b200_sinusoidal_forward':
-        (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _i, _vp, _sz, _vp]),
-    'ddsp_b200_sinusoidal_backward_workspace': (_sz, [_i, _i, _i]),
-    'ddsp_b200_sinusoidal_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
-    'ddsp_b200_add': (_i, [_vp, _vp, _vp, _i64, _vp]),
-    'ddsp_b200_frame_window': (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp]),
-    'ddsp_b200_frame_window_adjoint':
-        (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
-    'ddsp_b200_spectral_l1': (_i, [_vp, _vp, _vp, _vp, _i64, _f, _f, _i, _i, _vp]),
-    'ddsp_b200_mod_delay_forward':
-        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _i, _vp]),
-    'ddsp_b200_mod_delay_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _f, _f, _i, _vp]),
-    'ddsp_b200_resample_backward': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp]),
-    'ddsp_b200_mix_forward': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
-    'ddsp_b200_mix_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _vp]),
-    'ddsp_b200_exp_decay_ir': (_i, [_vp, _vp, _vp, _u64, _u64, _vp, _i, _i, _vp]),
-    'ddsp_b200_exp_decay_ir_backward':
-        (_i, [_vp, _vp, _vp, _u64, _u64, _vp, _vp, _vp, _i, _i, _vp]),
-    'ddsp_b200_wavetable_workspace': (_sz, [_i, _i]),
-    'ddsp_b200_wavetable_forward':
-        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _sz, _vp]),
-    'ddsp_b200_wavetable_backward_workspace': (_sz, [_i, _i, _i, _i, _i]),
-    'ddsp_b200_wavetable_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _i, _vp, _sz,
-              _vp]),
-    'ddsp_b200_loudness_forward':
-        (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
-    'ddsp_b200_loudness_backward':
-        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
-    'ddsp_b200_rms_power': (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _f, _vp]),
-    'ddsp_b200_mel_forward':
-        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
-    'ddsp_b200_mel_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _vp]),
-    'ddsp_b200_mixture_nll_forward':
-        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
-    'ddsp_b200_mixture_nll_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp]),
-    'ddsp_b200_comb_nll_forward':
-        (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
-    'ddsp_b200_comb_nll_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _f, _vp]),
-    'ddsp_b200_sinusoidal_to_harmonic':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _i, _vp]),
-    'ddsp_b200_sinusoidal_to_harmonic_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _f, _f, _i, _vp]),
-    'ddsp_b200_hmm_log_prob': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _d, _d, _vp]),
-    'ddsp_b200_hmm_log_prob_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _d, _d, _vp]),
-    'ddsp_b200_hmm_viterbi': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _d, _d, _vp]),
-    'ddsp_b200_wasserstein_forward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _f, _vp]),
-    'ddsp_b200_wasserstein_backward':
-        (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i, _i, _f, _vp]),
+# C types of the header, spelled without `const` and whitespace.  Device pointers
+# travel as integers.
+_SCALARS = {
+    'int': ctypes.c_int,
+    'int64_t': ctypes.c_int64,
+    'uint64_t': ctypes.c_uint64,
+    'size_t': _sz,
+    'float': ctypes.c_float,
+    'double': ctypes.c_double,
 }
+
+
+def _ctype(spelling, is_return=False):
+  """The ctypes type of a C type as the header spells it; an unknown type raises, so
+  that a new type in the header is never bound by a guess."""
+  t = re.sub(r'\bconst\b|\s', '', spelling)
+  if is_return and t == 'char*':
+    return ctypes.c_char_p
+  if t == 'ddsp_b200_host_pipeline**':
+    return ctypes.POINTER(ctypes.c_void_p)
+  if t.endswith('*') and not t.endswith('**'):
+    return ctypes.c_void_p
+  if t in _SCALARS:
+    return _SCALARS[t]
+  raise TypeError(f'ddsp_b200: the C type {spelling.strip()!r} in the ABI header has no '
+                  'ctypes binding in ddsp_b200/_lib.py')
+
+
+def parse_header(text):
+  """(signatures, constants) of the C header `text`: {name: (restype, argtypes)} for
+  every ddsp_b200_* prototype and {NAME: value} for every DDSP_B200_NAME enum value
+  or integer #define."""
+  text = re.sub(r'/\*.*?\*/|//[^\n]*', ' ', text, flags=re.S)
+  constants = {m[1]: int(m[2]) for m in
+               re.finditer(r'^\s*#\s*define\s+DDSP_B200_(\w+)\s+(-?\d+)\s*$', text, re.M)}
+  for body in re.findall(r'\benum\s*\{([^}]*)\}', text):
+    for item in body.split(','):
+      m = re.fullmatch(r'\s*DDSP_B200_(\w+)\s*=\s*(-?\d+)\s*', item)
+      if not m:
+        raise ValueError(f'ddsp_b200: enumerator {item.strip()!r} of the ABI header is '
+                         'not DDSP_B200_NAME = integer')
+      constants[m[1]] = int(m[2])
+  text = re.sub(r'^\s*#[^\n]*', ' ', text, flags=re.M)
+  signatures = {}
+  for m in re.finditer(r'([\w\s*]+?)\b(ddsp_b200_\w+)\s*\(([^()]*)\)\s*;', text):
+    params = [p.strip() for p in m[3].split(',')]
+    if params == ['void']:
+      params = []
+    # a parameter is its type and a name: drop the name
+    argtypes = [_ctype(re.sub(r'\w+$', '', p)) for p in params]
+    signatures[m[2]] = (_ctype(m[1], is_return=True), argtypes)
+  return signatures, constants
+
+
+def _read_header():
+  if not os.path.exists(HEADER_PATH):
+    raise RuntimeError(
+        'ddsp_b200: %s is missing. The C ABI header declares what the binding '
+        'calls; it belongs next to the package, in the source tree.' % HEADER_PATH)
+  with open(HEADER_PATH) as f:
+    return f.read()
+
+
+SIGNATURES, _CONSTANTS = parse_header(_read_header())
+globals().update(_CONSTANTS)
+PADDING = {name[len('PAD_'):].lower(): value for name, value in _CONSTANTS.items()
+           if name.startswith('PAD_')}
 
 _lib = None
 _lock = threading.Lock()

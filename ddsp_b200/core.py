@@ -500,9 +500,6 @@ def harmonic_to_sinusoidal(harm_amp, harm_dist, f0_hz, sample_rate=16000):
   return harm_amp * harm_dist, freqs
 
 
-SIN_TO_HARM_MAX_SINUSOIDS = 4096    # staged per frame by the kernels
-
-
 def _sinusoidal_to_harmonic_shapes(sin_amps, sin_freqs, f0_hz, harmonic_width, n_harmonics):
   """(B, T, S, K) of sinusoidal_to_harmonic from static shapes, or the error."""
   sa, sf, s0 = _shape(sin_amps), _shape(sin_freqs), _shape(f0_hz)
@@ -514,10 +511,10 @@ def _sinusoidal_to_harmonic_shapes(sin_amps, sin_freqs, f0_hz, harmonic_width, n
   if np.float32(harmonic_width) == 0.0:
     raise ValueError('harmonic_width must be nonzero (the reference divides by it), got '
                      f'{harmonic_width}.')
-  if sa[2] > SIN_TO_HARM_MAX_SINUSOIDS:
+  if sa[2] > _lib.CONSISTENCY_MAX_STAGED:
     raise NotImplementedError(
         f'sinusoidal_to_harmonic: {sa[2]} sinusoids per frame exceed the '
-        f'{SIN_TO_HARM_MAX_SINUSOIDS} the kernels stage.')
+        f'{_lib.CONSISTENCY_MAX_STAGED} the kernels stage.')
   return sa + (int(n_harmonics),)
 
 
@@ -557,20 +554,8 @@ def sinusoidal_to_harmonic(sin_amps, sin_freqs, f0_hz, harmonic_width=0.1,
 
 
 # ----------------------------------------------------------------------------
-# losses.wasserstein_distance (losses.py:641-686): csrc/wasserstein.cuh
-# ----------------------------------------------------------------------------
-WASSERSTEIN_MAX_SIDE = 4096    # values per side one CTA sorts in shared memory
-WASSERSTEIN_MAX_ROWS = 2**31 - 1
-
-
-# ----------------------------------------------------------------------------
 # The HMM of losses.HmmTranscriber (losses.py:247-345): csrc/hmm.cuh
 # ----------------------------------------------------------------------------
-HMM_MAX_STATES = 1024          # states one CTA runs, a thread each
-HMM_SEGMENT_FLOATS = 48 * 1024  # shared floats of the backward's segment buffer
-HMM_VITERBI_BYTES = 200 * 1024  # shared bytes of the Viterbi back pointers
-
-
 def _hmm_shapes(observations, loc, scale):
   """(B, T, K) of an HMM call from static shapes, or the error."""
   so, sl, ss = _shape(observations), _shape(loc), _shape(scale)
@@ -580,8 +565,8 @@ def _hmm_shapes(observations, loc, scale):
     raise ValueError(f'loc {sl} and scale {ss} must both be [n_states, 2].')
   if sl[0] < 2:
     raise ValueError(f'the HMM needs at least 2 states, got {sl[0]}.')
-  if sl[0] > HMM_MAX_STATES:
-    raise NotImplementedError(f'HMM: {sl[0]} states exceed the {HMM_MAX_STATES} the '
+  if sl[0] > _lib.HMM_MAX_STATES:
+    raise NotImplementedError(f'HMM: {sl[0]} states exceed the {_lib.HMM_MAX_STATES} the '
                               'kernels run.')
   return so[0], so[1], sl[0]
 
@@ -599,13 +584,13 @@ def hmm_segment(t, k):
   """Steps per checkpoint of the log-likelihood backward: about sqrt(T), so that the
   checkpoints ([B, ceil(T / seg), K] floats) and the segment buffer (seg x K floats
   of shared memory) are both O(K sqrt(T)); at most HMM_SEGMENT_FLOATS / K."""
-  return min(math.isqrt(t - 1) + 1, HMM_SEGMENT_FLOATS // k)
+  return min(math.isqrt(t - 1) + 1, _lib.HMM_SEGMENT_FLOATS // k)
 
 
 def hmm_viterbi_takes(t, k):
   """True where `ddsp_b200_hmm_viterbi` keeps T steps of K states' back pointers in
-  shared memory: 4 T (ceil(K / 32) + 1) <= 200 KiB."""
-  return 4 * t * ((k + 31) // 32 + 1) <= HMM_VITERBI_BYTES
+  shared memory: 4 T (ceil(K / 32) + 1) <= HMM_VITERBI_BYTES."""
+  return bool(_lib.load().ddsp_b200_hmm_viterbi_takes(t, k))
 
 
 def _hmm_operands(observations, loc, scale):
@@ -657,7 +642,7 @@ def hmm_posterior_mode(observations, loc, scale, hold, other):
   if not hmm_viterbi_takes(t, k):
     raise NotImplementedError(
         f'hmm_posterior_mode: {t} steps of {k} states exceed the back pointers the '
-        f'kernel keeps (4 T (ceil(K / 32) + 1) <= {HMM_VITERBI_BYTES} bytes).')
+        f'kernel keeps (4 T (ceil(K / 32) + 1) <= {_lib.HMM_VITERBI_BYTES} bytes).')
   x, loc, scale = _hmm_operands(observations, loc, scale)
   path = torch.empty((b, t), dtype=torch.int64, device=x.device)
   _launch('ddsp_b200_hmm_viterbi', x.detach(), loc.detach(), scale.detach(), path, b, t,
@@ -978,8 +963,7 @@ def harmonic_synthesis(frequencies,
 def _harmonic_backward_takes(b, f, n_samples):
   """Whether `ddsp_b200_harmonic_backward` takes an integer-hop shape: a hop that is a
   multiple of 64 and at most 8192, a batch within the grid limit."""
-  hop = n_samples // f
-  return hop % 64 == 0 and hop <= 8192 and b <= 65535
+  return bool(_lib.load().ddsp_b200_harmonic_backward_takes(b, f, n_samples))
 
 
 @on_operands_device
@@ -1044,11 +1028,8 @@ def get_fft_size(frame_size: int, ir_size: int, power_of_2: bool = True) -> int:
 
 
 def _ir_size(nb, window_size):
-  """Taps of the windowed impulse response of nb bins (`ddsp_b200_ir_size`):
-  window_size if odd, one less if even, 2 (nb - 1) without a window."""
-  s0 = 2 * (nb - 1)
-  ws = s0 if window_size <= 0 or window_size > s0 else window_size
-  return 2 * ((ws + 1) // 2) - 1 if ws < s0 else s0
+  """Taps of the windowed impulse response of nb bins: `ddsp_b200_ir_size`."""
+  return _lib.load().ddsp_b200_ir_size(nb, window_size)
 
 
 def _check_n_frequencies(nb):
@@ -1070,7 +1051,7 @@ def frequency_impulse_response(magnitudes, window_size: int = 0):
   if _requires_grad(magnitudes):
     from ddsp_b200 import autograd as _ag
     return _ag.FrequencyImpulseResponseFn.apply(magnitudes, int(window_size))
-  s = _lib.load().ddsp_b200_ir_size(nb, int(window_size))
+  s = _ir_size(nb, int(window_size))
   magnitudes = torch_float32(magnitudes)
   ir = torch.empty(tuple(magnitudes.shape[:-1]) + (s,), dtype=torch.float32,
                    device=magnitudes.device)
@@ -1329,6 +1310,8 @@ def frequency_filter(audio, magnitudes, window_size: int = 0,
     sm = _shape(magnitudes)
     nb = int(sm[-1])
     _check_n_frequencies(nb)
+    # the shape checks do not depend on the taps: they raise before the library is asked
+    _fft_convolve_geometry(_shape(audio), tuple(sm[:-1]) + (1,), padding, -1)
     s = _ir_size(nb, int(window_size))
     _, _, _, _, _, _, out_len, crop_size = _fft_convolve_geometry(
         _shape(audio), tuple(sm[:-1]) + (s,), padding, -1)
@@ -1673,20 +1656,9 @@ def uniform_noise(batch_size, n_samples, seed=0, offset=0, device=None):
 def _noise_backward_takes(f, nb, n_samples, window_size):
   """Whether `ddsp_b200_filtered_noise_backward` takes a shape: an impulse response of
   at least three taps, and 32 frames of noise, gradient and taps within one CTA's
-  shared memory (the launcher's own layout, csrc/noise.cu noise_bwd_params)."""
-  if nb < 2:
-    return False
-  s0 = 2 * (nb - 1)
-  s = _ir_size(nb, window_size)
-  frame = -(-n_samples // f)
-  padded = (frame + 15) & ~15
-  x_stride = (padded + 1) | 1
-  g_stride = (padded + s + 17) | 1
-  h_stride = (s + nb) | 1
-  floats = (s0 + s + 32 * (x_stride + g_stride + h_stride) + 3) & ~3
-  if nb == 65:
-    floats += nb * 36       # the cosine table of the 65-band specialisation
-  return s >= 3 and 4 * floats <= 200 * 1024
+  shared memory."""
+  return bool(_lib.load().ddsp_b200_filtered_noise_backward_takes(f, nb, n_samples,
+                                                                  window_size))
 
 
 @on_operands_device

@@ -68,7 +68,8 @@ namespace ddsp {
 namespace cons_ {
 
 constexpr int kThreads = 128;
-constexpr int kMaxStaged = 4096;   // components (mode A), candidates and points (mode B)
+// components (mode A), candidates and points (mode B) staged per frame
+constexpr int kMaxStaged = DDSP_B200_CONSISTENCY_MAX_STAGED;
 constexpr int kChunk = 512;        // queries per shared-memory chunk of the mode A backward
 constexpr int kHarmChunk = 256;    // harmonics per shared-memory chunk of the mode C backward
 

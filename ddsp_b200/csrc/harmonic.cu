@@ -145,6 +145,12 @@ int ddsp_b200_noise_controls(const float* mag_in, float* mag_out, int64_t n,
   return 0;
 }
 
+int ddsp_b200_harmonic_backward_takes(int B, int F, int N) {
+  if (F < 1) return 0;
+  const int hop = N / F;
+  return hop >= 64 && hop % 64 == 0 && hop <= 8192 && B <= 65535;
+}
+
 int ddsp_b200_harmonic_backward(const float* f0_hz, const float* grad_audio,
                                 float* g0, float* g1, int B, int F, int K, int N,
                                 float sample_rate, int amp_method, void* stream) {
@@ -158,8 +164,7 @@ int ddsp_b200_harmonic_backward(const float* f0_hz, const float* grad_audio,
   HarmonicParams p = harm_params(f0_hz, nullptr, nullptr, nullptr, B, F, K, N,
                                  sample_rate, amp_method);
   p.Kp = K;
-  DDSP_REQUIRE(p.hop % 64 == 0 && p.hop <= 8192 && B <= 65535,
-               DDSP_B200_E_UNSUPPORTED,
+  DDSP_REQUIRE(ddsp_b200_harmonic_backward_takes(B, F, N), DDSP_B200_E_UNSUPPORTED,
                "harmonic_backward: needs hop %% 64 == 0 (hop = %d)", p.hop);
   cudaStream_t st = (cudaStream_t)stream;
   if (harmonic_backward2_supported(p))

@@ -41,11 +41,11 @@
 namespace ddsp {
 namespace hmm_ {
 
-constexpr int kMaxStates = 1024;
+constexpr int kMaxStates = DDSP_B200_HMM_MAX_STATES;
 // Shared floats of the backward's segment buffer: seg * K <= kSegFloats (192 KB).
-constexpr int kSegFloats = 48 * 1024;
+constexpr int kSegFloats = DDSP_B200_HMM_SEGMENT_FLOATS;
 // Shared bytes of the Viterbi back pointers: 4 T (ceil(K / 32) + 1) <= kViterbiBytes.
-constexpr size_t kViterbiBytes = 200 * 1024;
+constexpr size_t kViterbiBytes = DDSP_B200_HMM_VITERBI_BYTES;
 constexpr float kLog2Pi = 1.8378770664093453f;
 
 struct Params {

@@ -11,7 +11,7 @@ extern "C" {
 
 // ---- consistency-loss mixture NLLs -------------------------------------------------
 static int cons_rows(const char* name, int B, int T, int64_t* rows) {
-  DDSP_REQUIRE((int64_t)B * T <= INT32_MAX, DDSP_B200_E_INVALID,
+  DDSP_REQUIRE((int64_t)B * T <= DDSP_B200_MAX_ROWS, DDSP_B200_E_INVALID,
                "%s: B*T=%lld exceeds the 2^31 - 1 grid limit", name, (long long)B * T);
   *rows = (int64_t)B * T;
   return 0;
@@ -286,6 +286,15 @@ int ddsp_b200_hmm_log_prob_backward(const float* obs, const float* loc, const fl
   return 0;
 }
 
+// Shared bytes of the Viterbi back pointers of T steps of K states.
+static size_t hmm_viterbi_smem(int T, int K) {
+  return sizeof(uint32_t) * (size_t)T * ((K + 31) / 32 + 1);
+}
+
+int ddsp_b200_hmm_viterbi_takes(int T, int K) {
+  return T >= 1 && K >= 1 && hmm_viterbi_smem(T, K) <= hmm_::kViterbiBytes;
+}
+
 int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale,
                           int64_t* path, int B, int T, int K, double hold, double other,
                           void* stream) {
@@ -294,8 +303,8 @@ int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale
   hmm_::Params p;
   int rc = hmm_check("hmm_viterbi", obs, loc, scale, B, T, K, hold, other, &p);
   if (rc) return rc;
-  const size_t smem = sizeof(uint32_t) * (size_t)T * ((K + 31) / 32 + 1);
-  DDSP_REQUIRE(smem <= hmm_::kViterbiBytes, DDSP_B200_E_UNSUPPORTED,
+  const size_t smem = hmm_viterbi_smem(T, K);
+  DDSP_REQUIRE(ddsp_b200_hmm_viterbi_takes(T, K), DDSP_B200_E_UNSUPPORTED,
                "hmm_viterbi: T=%d steps of K=%d states need %zu B of back pointers, more "
                "than the %zu supported", T, K, smem, hmm_::kViterbiBytes);
   if (B == 0) return 0;
@@ -316,7 +325,7 @@ static int ws_check(const char* name, int64_t R, int Nu, int Nv, float p, ws_::P
   DDSP_REQUIRE(Nu <= ws_::kMaxSide && Nv <= ws_::kMaxSide, DDSP_B200_E_UNSUPPORTED,
                "%s: Nu=%d or Nv=%d elements exceed the %d supported per side", name, Nu, Nv,
                ws_::kMaxSide);
-  DDSP_REQUIRE(R <= INT32_MAX, DDSP_B200_E_INVALID,
+  DDSP_REQUIRE(R <= DDSP_B200_MAX_ROWS, DDSP_B200_E_INVALID,
                "%s: R=%lld exceeds the 2^31 - 1 grid limit", name, (long long)R);
   wp->Nu = Nu;
   wp->Nv = Nv;

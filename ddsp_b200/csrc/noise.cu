@@ -389,6 +389,17 @@ static int noise_bwd_launch(const NoiseBwdParams& p, size_t smem, cudaStream_t s
   return 0;
 }
 
+int ddsp_b200_filtered_noise_backward_takes(int F, int nb, int N, int window_size) {
+  if (F < 1 || N < 1 || nb < 2) return 0;
+  const int frame = (N + F - 1) / F;
+  if ((N + frame - 1) / frame != F) return 0;
+  long long n_tiles;
+  size_t smem;
+  const NoiseBwdParams p = noise_bwd_params(nullptr, nullptr, 0, 0, nullptr, 1, F, nb, N,
+                                            frame, window_size, &n_tiles, &smem);
+  return p.start >= 0 && smem <= kMaxDynSmem;
+}
+
 int ddsp_b200_filtered_noise_backward(const float* grad_audio, const float* noise,
                                       uint64_t seed, uint64_t offset, float* dmags,
                                       int B, int F, int nb, int N, int window_size,
@@ -404,12 +415,13 @@ int ddsp_b200_filtered_noise_backward(const float* grad_audio, const float* nois
   size_t smem;
   NoiseBwdParams p = noise_bwd_params(grad_audio, noise, seed, offset, dmags, B, F, nb, N,
                                       frame, window_size, &n_tiles, &smem);
-  DDSP_REQUIRE(p.start >= 0, DDSP_B200_E_UNSUPPORTED,
-               "filtered_noise_backward: impulse response too short");
+  DDSP_REQUIRE(ddsp_b200_filtered_noise_backward_takes(F, nb, N, window_size),
+               DDSP_B200_E_UNSUPPORTED,
+               p.start < 0 ? "filtered_noise_backward: impulse response too short"
+                           : "filtered_noise_backward: shape needs %zu B of shared memory",
+               smem);
   DDSP_REQUIRE(n_tiles < (1ll << 31), DDSP_B200_E_INVALID,
                "filtered_noise_backward: too many tiles");
-  DDSP_REQUIRE(smem <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
-               "filtered_noise_backward: shape needs %zu B of shared memory", smem);
   return noise_bwd_launch(p, smem, (cudaStream_t)stream, "filtered_noise_backward");
 }
 

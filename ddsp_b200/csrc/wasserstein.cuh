@@ -35,7 +35,7 @@
 namespace ddsp {
 namespace ws_ {
 
-constexpr int kMaxSide = 4096;   // elements per side
+constexpr int kMaxSide = DDSP_B200_WASSERSTEIN_MAX_SIDE;  // elements per side
 constexpr int kMinPadded = 64;
 constexpr int kMaxThreads = 512;
 

@@ -14,6 +14,7 @@ import re
 import numpy as np
 import torch
 
+from ddsp_b200 import _lib
 from ddsp_b200 import autograd
 from ddsp_b200 import core
 from ddsp_b200 import dags
@@ -467,13 +468,13 @@ def _check_wasserstein(u_values, v_values, u_weights, v_weights, p):
   p = float(p)
   if not (p > 0.0 and math.isfinite(p)):
     raise ValueError(f'{name}: p must be positive and finite, got {p}')
-  limit = core.WASSERSTEIN_MAX_SIDE
+  limit = _lib.WASSERSTEIN_MAX_SIDE
   if su[-1] > limit or sv[-1] > limit:
     raise NotImplementedError(f'{name}: n_u={su[-1]} or n_v={sv[-1]} values exceed the '
                               f'{limit} per side the kernel sorts.')
   rows = math.prod(su[:-1])
-  if rows > core.WASSERSTEIN_MAX_ROWS:
-    raise NotImplementedError(f'{name}: {rows} rows exceed the {core.WASSERSTEIN_MAX_ROWS} '
+  if rows > _lib.MAX_ROWS:
+    raise NotImplementedError(f'{name}: {rows} rows exceed the {_lib.MAX_ROWS} '
                               'the kernel launches.')
   return su[:-1], su[-1], sv[-1]
 
@@ -592,9 +593,9 @@ class HmmTranscriber:
 
   def _supported(self, name, viterbi):
     k, t = self.n_pitches, self.n_timesteps
-    if k > core.HMM_MAX_STATES:
+    if k > _lib.HMM_MAX_STATES:
       raise NotImplementedError(f'HmmTranscriber.{name}: {k} pitches exceed the '
-                                f'{core.HMM_MAX_STATES} states the kernels run.')
+                                f'{_lib.HMM_MAX_STATES} states the kernels run.')
     if viterbi and not core.hmm_viterbi_takes(t, k):
       raise NotImplementedError(f'HmmTranscriber.{name}: {t} steps of {k} states exceed '
                                 'the back pointers the Viterbi kernel keeps.')

@@ -19,6 +19,12 @@
  *     thread-local).
  *   - Return value: 0 = ok, negative = DDSP_B200_E_* below.  Shape/argument
  *     errors are detected BEFORE any launch.
+ *   - The *_workspace, *_takes and ddsp_b200_ir_size queries are pure host
+ *     functions: they launch nothing and set no error.
+ *
+ * The Python binding (ddsp_b200/_lib.py) is derived from this file at import:
+ * every ddsp_b200_* prototype and every DDSP_B200_* integer constant.  A C type
+ * it does not know stops the import, so a new type needs a line there.
  */
 #ifndef DDSP_B200_H_
 #define DDSP_B200_H_
@@ -201,7 +207,10 @@ int ddsp_b200_decoder_forward_host(ddsp_b200_host_pipeline* pipeline,
  * the reference gets it from TF autodiff).  grad_audio [B,N] -> g0, g1 [B,F,K]:
  *   g0[i,k] = sum_{t in frame i} grad(t) w0(r) m_k(t) sin(k phi(t)),  g1 with w1;
  *   dL/dha[i,k] = g0[i,k] + g1[i-1,k] (+ g1[F-1,k] when i == F-1).
- * The frame-rate recombination is left to the caller.  d f0 is not built. */
+ * The frame-rate recombination is left to the caller.  d f0 is not built.
+ * Shapes beyond ddsp_b200_harmonic_backward_takes(B, F, N) are E_UNSUPPORTED: it is
+ * 1 for a hop N / F that is a multiple of 64 up to 8192 and B <= 65535, else 0. */
+int ddsp_b200_harmonic_backward_takes(int B, int F, int N);
 int ddsp_b200_harmonic_backward(const float* f0_hz, const float* grad_audio,
                                 float* g0, float* g1, int B, int F, int K, int N,
                                 float sample_rate, int amp_method, void* stream);
@@ -252,7 +261,11 @@ int ddsp_b200_noise_controls_backward(const float* mags_raw, const float* d_mags
 /* Backward of FilteredNoise.get_signal w.r.t. magnitudes (controls): the
  * transpose of core.frequency_filter (core.py:1628-1655) for the same noise
  * (caller-supplied, or the Philox stream of (seed, offset)).
- * grad_audio [B,N] -> dmags [B,F,nb]. */
+ * grad_audio [B,N] -> dmags [B,F,nb].  Shapes beyond
+ * ddsp_b200_filtered_noise_backward_takes(F, nb, N, window_size) are E_UNSUPPORTED: it
+ * is 1 for a valid shape whose impulse response has at least 3 taps and whose tiles of
+ * 32 frames (noise, gradient and taps) fit one CTA's shared memory, else 0. */
+int ddsp_b200_filtered_noise_backward_takes(int F, int nb, int N, int window_size);
 int ddsp_b200_filtered_noise_backward(const float* grad_audio, const float* noise,
                                       uint64_t seed, uint64_t offset, float* dmags,
                                       int B, int F, int nb, int N, int window_size,
@@ -619,6 +632,11 @@ int ddsp_b200_mel_backward(const float* audio, const float* window, const void* 
                            int n_frames, int fft_size, int fft_length, int hop, int pad_end,
                            int bins, int n_out, int mode, void* stream);
 
+/* Limits of the loss kernels, which run one CTA per row (a frame, or a Wasserstein row):
+ * rows on the grid's x axis, and the components, candidates, points or sinusoids the
+ * consistency kernels stage per frame. */
+enum { DDSP_B200_MAX_ROWS = 2147483647, DDSP_B200_CONSISTENCY_MAX_STAGED = 4096 };
+
 /* Mixture NLL of the consistency losses (losses.KDEConsistencyLoss.nll and
  * TWMLoss's p(harmonics | sinusoids), losses.py:759-813, 982-990): per frame (b, t),
  *   nll[b,t,q] = -logsumexp_j(lw[b,t,j] - ((x[b,t,q] - mu[b,t,j]) / scale)^2 / 2)
@@ -696,15 +714,22 @@ int ddsp_b200_sinusoidal_to_harmonic_backward(
  *   ddsp_b200_hmm_log_prob_backward: d_obs [B,T,2] = grad_b * d log_prob_b / d obs, from
  *     the posterior marginals; loc and scale are constants.  checkpoints is scratch of
  *     B * ceil(T / seg) * K floats: the kernel re-runs the forward and keeps its state
- *     there every seg steps; 1 <= seg and seg * K <= 49152 (E_INVALID otherwise).  No
- *     atomics: bit-reproducible.
+ *     there every seg steps; 1 <= seg and seg * K <= DDSP_B200_HMM_SEGMENT_FLOATS
+ *     (E_INVALID otherwise).  No atomics: bit-reproducible.
  *   ddsp_b200_hmm_viterbi: path [B,T] (int64), the most likely state sequence; ties go to
  *     the lowest state index.  The back pointers stay in shared memory, which bounds
- *     4 T (ceil(K / 32) + 1) <= 204800 bytes (E_UNSUPPORTED otherwise): K = 1024 takes
- *     T <= 1551, K = 128 T <= 10240.
- * All three take B >= 0, T >= 1, 2 <= K <= 1024 (more is E_UNSUPPORTED), hold and other
- * finite, non-negative and not both 0.  B = 0 returns after the checks without a launch
- * (the pointers may then be null). */
+ *     4 T (ceil(K / 32) + 1) <= DDSP_B200_HMM_VITERBI_BYTES (E_UNSUPPORTED otherwise):
+ *     K = 1024 takes T <= 1551, K = 128 T <= 10240.  ddsp_b200_hmm_viterbi_takes(T, K) is
+ *     1 for T >= 1 steps of K >= 1 states within that bound, else 0.
+ * All three take B >= 0, T >= 1, 2 <= K <= DDSP_B200_HMM_MAX_STATES (more is
+ * E_UNSUPPORTED), hold and other finite, non-negative and not both 0.  B = 0 returns
+ * after the checks without a launch (the pointers may then be null). */
+enum {
+  DDSP_B200_HMM_MAX_STATES = 1024,      /* one CTA runs the states, a thread each      */
+  DDSP_B200_HMM_SEGMENT_FLOATS = 49152, /* the backward's segment buffer (192 KiB)     */
+  DDSP_B200_HMM_VITERBI_BYTES = 204800  /* the Viterbi back pointers (200 KiB)         */
+};
+int ddsp_b200_hmm_viterbi_takes(int T, int K);
 int ddsp_b200_hmm_log_prob(const float* obs, const float* loc, const float* scale,
                            float* log_prob, int B, int T, int K, double hold, double other,
                            void* stream);
@@ -722,9 +747,9 @@ int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale
  *   out[r] = (sum_i (s_{i+1} - s_i) |U_i - V_i|^p)^(1/p),
  *   U_i = sum_k wu_k [u_k <= s_i],  V_i = sum_k wv_k [v_k <= s_i].
  * The CDFs are raw cumulative weights, not normalised, as the reference computes them.
- * p positive and finite; Nu, Nv <= 4096 (more is E_UNSUPPORTED); R <= 2^31 - 1.  No
- * workspace.  R, Nu or Nv = 0 returns after the checks without a launch and writes
- * nothing (the pointers may then be null).  One CTA per row sorts, scans and sums in
+ * p positive and finite; Nu, Nv <= DDSP_B200_WASSERSTEIN_MAX_SIDE (more is
+ * E_UNSUPPORTED); R <= DDSP_B200_MAX_ROWS.  No workspace.  R, Nu or Nv = 0 returns after
+ * the checks without a launch and writes nothing (the pointers may then be null).  One CTA per row sorts, scans and sums in
  * shared memory: nothing but out is written.
  * backward: for grad [R], du [R,Nu], dv [R,Nv], dwu [R,Nu] and dwv [R,Nv], all written.
  * With c_i = |U_i - V_i|^p, S = sum_i delta_i c_i, G = grad (1/p) S^(1/p - 1) and
@@ -734,6 +759,7 @@ int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale
  * An exact U_i = V_i at p < 1, or S = 0 at p > 1, gives NaN (0 * inf) as autograd does;
  * at p = 1 everything finite stays finite.  Fixed-order scans and sums, no atomics:
  * bit-reproducible. */
+enum { DDSP_B200_WASSERSTEIN_MAX_SIDE = 4096 /* values per side one CTA sorts */ };
 int ddsp_b200_wasserstein_forward(const float* u, const float* v, const float* wu,
                                   const float* wv, float* out, int64_t R, int Nu, int Nv,
                                   float p, void* stream);

@@ -703,7 +703,7 @@ class Recorder:
     self.calls = []
 
   def __getattr__(self, name):
-    if name.endswith('_workspace') or name in _PASS_THROUGH:
+    if name.endswith(('_workspace', '_takes')) or name in _PASS_THROUGH:
       return getattr(self.real, name)
     assert name in _lib.SIGNATURES, name
 

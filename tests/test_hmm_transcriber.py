@@ -26,6 +26,7 @@ from ddsp_b200 import _lib, core, losses
 from oracle import ref_on_shim
 from tests import hmm_ref as ref
 from tests.golden import make_hmm_golden as mg
+from tests.util import HostQueriesOnly
 
 DEV = 'cuda'
 
@@ -89,13 +90,14 @@ def test_restatement_against_brute_force(k, t, avg_length):
       assert np.array_equal(path[i], best[i]), (i, path[i], best[i])
 
 
-def test_value_errors_before_device_work(monkeypatch):
+def test_value_errors_before_device_work_or_launches(monkeypatch):
   """Every error is raised from static shapes and arguments, before any tensor is moved
-  or the library is loaded."""
+  or anything but the library's host queries (the Viterbi size rule) is called."""
   def touched(*a, **k):
     raise AssertionError('device work before the argument checks')
   monkeypatch.setattr(core, 'torch_float32', touched)
-  monkeypatch.setattr(core._lib, 'load', touched)
+  rec = HostQueriesOnly(_lib.load())
+  monkeypatch.setattr(core._lib, 'load', lambda: rec)
   for kw in (dict(n_pitches=1), dict(n_pitches=0), dict(n_timesteps=0),
              dict(avg_length=0.999), dict(avg_length=-3.0), dict(n_pitches=2.5)):
     with pytest.raises(ValueError):
@@ -214,10 +216,10 @@ def test_abi_check_table(fn, args, want, msg):
     assert lib.ddsp_b200_last_error() == msg
 
 
-def test_no_workspace():
+def test_no_workspace_and_one_size_query():
   names = sorted(n for n in _lib.SIGNATURES if 'hmm' in n)
   assert names == ['ddsp_b200_hmm_log_prob', 'ddsp_b200_hmm_log_prob_backward',
-                   'ddsp_b200_hmm_viterbi']
+                   'ddsp_b200_hmm_viterbi', 'ddsp_b200_hmm_viterbi_takes']
   for n in names:
     assert _lib.SIGNATURES[n][1][-2] is not _lib._sz
 
