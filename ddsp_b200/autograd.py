@@ -25,6 +25,11 @@ kernels, exposed as `torch.autograd.Function`s:
     audio-rate envelopes (d frequency and d amplitude envelopes) and the phase
     accumulation, routed to by `core.oscillator_bank` / `core.angular_cumsum` under
     grad;
+  * `HarmonicOscillatorBankFn` - core.harmonic_oscillator_bank with a carried phase,
+    differentiable in f0, amplitude envelopes and initial phase through the audio and the
+    final phase; routed to by `core.harmonic_oscillator_bank` (and so by
+    `core.streaming_harmonic_synthesis`) under grad;
+  * `LinearLookupFn` - core.linear_lookup, d phase and d wavetables;
   * `WavetableSynthesisFn` - d f0, d amplitudes and d wavetables of the wavetable
     synthesizer (`Wavetable.get_signal`); `core.wavetable_synthesis` routes to it
     under grad;
@@ -518,6 +523,66 @@ class AngularCumsumFn(torch.autograd.Function):
     d_x = torch.empty(ctx.shape, dtype=torch.float32, device=g.device)
     core._launch('ddsp_b200_angular_cumsum_backward', g, d_x, b, n, c)
     return d_x
+
+
+class HarmonicOscillatorBankFn(torch.autograd.Function):
+  """core.harmonic_oscillator_bank (core.py:966-1025) on f [B, N, 1], a [B, N, K] and
+  init [B, 1, 1] or None, differentiable in all three through both outputs (audio and
+  final phase).  One call of `ddsp_b200_harmonic_oscillator_bank_backward`
+  (csrc/harmonic_bank.cuh) computes the gradients asked for on the forward's exact phase."""
+
+  @staticmethod
+  def forward(ctx, f, a, init, sample_rate, use_angular_cumsum):
+    ctx.save_for_backward(f, a, init)
+    ctx.sample_rate = sample_rate
+    return core.harmonic_oscillator_bank_forward(f, a, init, sample_rate,
+                                                 use_angular_cumsum)
+
+  @staticmethod
+  def backward(ctx, grad_audio, grad_final_phase):
+    f, a, init = ctx.saved_tensors
+    b, n, k = a.shape
+    g = (torch.zeros((b, n), dtype=torch.float32, device=a.device) if grad_audio is None
+         else grad_audio.contiguous().to(torch.float32))
+    g_phi = (None if grad_final_phase is None
+             else grad_final_phase.contiguous().to(torch.float32))
+    want = ctx.needs_input_grad
+    d_f = torch.empty_like(f) if want[0] else None
+    d_a = torch.empty_like(a) if want[1] else None
+    d_init = torch.empty_like(init) if init is not None and want[2] else None
+    if b == 0:
+      return d_f, d_a, d_init, None, None
+    core._launch('ddsp_b200_harmonic_oscillator_bank_backward', f, a, init, g, g_phi, d_f,
+                 d_a, d_init, b, n, k, ctx.sample_rate)
+    return d_f, d_a, d_init, None, None
+
+
+class LinearLookupFn(torch.autograd.Function):
+  """core.linear_lookup (core.py:1168-1214) on phase [B, N] (or [B, N, 1]) and tables
+  [B, W], [B, 1, W] or [B, N, W], differentiable in both: one call of
+  `ddsp_b200_linear_lookup_backward` (csrc/lookup.cuh).  d phase follows TensorFlow's
+  subgradients of abs and relu, so it is 0 on a grid point."""
+
+  @staticmethod
+  def forward(ctx, phase, wavetables, per_sample):
+    ctx.save_for_backward(phase, wavetables)
+    ctx.per_sample = per_sample
+    return core.linear_lookup_forward(phase, wavetables, per_sample)
+
+  @staticmethod
+  def backward(ctx, grad):
+    phase, wavetables = ctx.saved_tensors
+    b, n = phase.shape[:2]
+    w = wavetables.shape[-1]
+    g = grad.contiguous().to(torch.float32)
+    want = ctx.needs_input_grad
+    d_phase = torch.empty_like(phase) if want[0] else None
+    d_tab = torch.empty_like(wavetables) if want[1] else None
+    if b == 0:
+      return d_phase, d_tab, None
+    core._launch('ddsp_b200_linear_lookup_backward', phase, wavetables, g, d_phase, d_tab,
+                 b, n, w, int(ctx.per_sample))
+    return d_phase, d_tab, None
 
 
 class WavetableSynthesisFn(torch.autograd.Function):

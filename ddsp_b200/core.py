@@ -966,6 +966,64 @@ def _harmonic_backward_takes(b, f, n_samples):
   return bool(_lib.load().ddsp_b200_harmonic_backward_takes(b, f, n_samples))
 
 
+def _hob_shapes(frequency, amplitude_envelopes, initial_phase):
+  """(B, N, K) of harmonic_oscillator_bank's operands; ValueError otherwise."""
+  sf, sa = _shape(frequency), _shape(amplitude_envelopes)
+  if len(sf) != 3 or len(sa) != 3 or sf[2] != 1 or sa[:2] != sf[:2] or sf[1] < 1 or sa[2] < 1:
+    raise ValueError(f'frequency {sf} must be [batch, n_samples, 1] and amplitude_envelopes '
+                     f'{sa} [batch, n_samples, n_harmonics], with n_samples >= 1 and '
+                     'n_harmonics >= 1.')
+  if initial_phase is not None and _shape(initial_phase) != (sf[0], 1, 1):
+    raise ValueError(f'initial_phase {_shape(initial_phase)} must be [{sf[0]}, 1, 1].')
+  return sf[0], sf[1], sa[2]
+
+
+def _hob_backward_takes(b, n, k):
+  """Whether `ddsp_b200_harmonic_oscillator_bank_backward` takes the shape."""
+  return bool(_lib.load().ddsp_b200_harmonic_oscillator_bank_backward_takes(b, n, k))
+
+
+@on_operands_device
+def harmonic_oscillator_bank(frequency, amplitude_envelopes, initial_phase=None,
+                             sample_rate: int = 16000, use_angular_cumsum: bool = True):
+  """core.harmonic_oscillator_bank (core.py:966-1025): one audio-rate f0 [B, N, 1] drives
+  the harmonics k = 1..K of amplitude_envelopes [B, N, K] from initial_phase [B, 1, 1]
+  (None: 0).  Returns (audio [B, N], final_phase [B, 1, 1]); feed final_phase back as the
+  next call's initial_phase.
+
+  The phase is accumulated exactly in 64-bit fixed-point turns, and harmonic k's phase is
+  k times it, wrapping exactly; there is no Nyquist mask, as in the reference.
+  final_phase is the wrapped sum in [0, 2 pi) plus initial_phase with
+  use_angular_cumsum=True, else the unwrapped sum plus initial_phase; the audio is the same
+  in both modes.  Routes to `autograd.HarmonicOscillatorBankFn` when grad is enabled and an
+  input requires it."""
+  b, n, k = _hob_shapes(frequency, amplitude_envelopes, initial_phase)
+  grad = _requires_grad(frequency, amplitude_envelopes, initial_phase)
+  if grad and not _hob_backward_takes(b, n, k):
+    _no_grad_path('harmonic_oscillator_bank', frequency, amplitude_envelopes, initial_phase)
+  f = torch_float32(frequency)
+  a = torch_float32(amplitude_envelopes)
+  init = None if initial_phase is None else torch_float32(initial_phase, f.device)
+  if grad:
+    from ddsp_b200 import autograd as _ag
+    return _ag.HarmonicOscillatorBankFn.apply(f, a, init, float(sample_rate),
+                                              bool(use_angular_cumsum))
+  return harmonic_oscillator_bank_forward(f, a, init, sample_rate, use_angular_cumsum)
+
+
+def harmonic_oscillator_bank_forward(f, a, init, sample_rate, use_angular_cumsum):
+  """`ddsp_b200_harmonic_oscillator_bank` on float32 CUDA operands f [B, N, 1],
+  a [B, N, K] and init [B, 1, 1] or None."""
+  b, n, k = a.shape
+  audio = torch.empty((b, n), dtype=torch.float32, device=f.device)
+  final_phase = torch.empty((b, 1, 1), dtype=torch.float32, device=f.device)
+  if b == 0:
+    return audio, final_phase
+  _launch('ddsp_b200_harmonic_oscillator_bank', f, a, init, audio, final_phase, b, n, k,
+          float(sample_rate), int(bool(use_angular_cumsum)))
+  return audio, final_phase
+
+
 @on_operands_device
 def streaming_harmonic_synthesis(frequencies,
                                  amplitudes,
@@ -977,7 +1035,13 @@ def streaming_harmonic_synthesis(frequencies,
   """core.streaming_harmonic_synthesis (core.py:1114-1164): single-f0 harmonic
   bank with a carried phase.  Returns (audio [B, n_samples], final_phase
   [B, 1, 1]) - feed final_phase back as initial_phase for the next hop
-  (training/inference.py:463-478)."""
+  (training/inference.py:463-478).
+
+  Without grad, 'window' / 'linear' amplitudes at an integer hop run one fused kernel.
+  Other hops, 'nearest' / 'cubic' amplitudes, and every call under grad run the
+  reference's composition on our kernels: normalize_harmonics, resample and
+  harmonic_oscillator_bank, each with its backward, so gradients reach frequencies,
+  amplitudes, harmonic_distribution and initial_phase."""
   sf, sa = _shape(frequencies), _shape(amplitudes)
   if len(sf) != 3 or len(sa) != 3 or sa != sf or sf[2] != 1:
     raise ValueError(f'frequencies {sf} and amplitudes {sa} must both be '
@@ -985,20 +1049,28 @@ def streaming_harmonic_synthesis(frequencies,
   if amp_resample_method not in ('nearest', 'linear', 'cubic', 'window'):
     raise ValueError('Method ({}) is invalid. Must be one of {}.'.format(
         amp_resample_method, "['nearest', 'linear', 'cubic', 'window']"))
-  if amp_resample_method not in AMP_METHODS:
-    raise NotImplementedError(amp_resample_method)
   b, f, _ = sf
   n_samples = int(n_samples)
-  if n_samples % f != 0:
-    raise NotImplementedError(
-        f'n_samples ({n_samples}) must be a multiple of the number of frames ({f}).')
+  k = 1
+  if harmonic_distribution is not None:
+    sh = _shape(harmonic_distribution)
+    if len(sh) != 3 or sh[:2] != (b, f):
+      raise ValueError(f'harmonic_distribution {sh} must be [{b}, {f}, n_harmonics].')
+    k = int(sh[-1])
+  if _requires_grad(frequencies, amplitudes, harmonic_distribution, initial_phase):
+    if not _hob_backward_takes(b, n_samples, k):
+      _no_grad_path('streaming_harmonic_synthesis', frequencies, amplitudes,
+                    harmonic_distribution, initial_phase)
+    return _streaming_composition(frequencies, amplitudes, harmonic_distribution,
+                                  initial_phase, n_samples, sample_rate, amp_resample_method)
+  if amp_resample_method not in AMP_METHODS or n_samples % f != 0:
+    return _streaming_composition(frequencies, amplitudes, harmonic_distribution,
+                                  initial_phase, n_samples, sample_rate, amp_resample_method)
   frequencies = torch_float32(frequencies)
   amplitudes = torch_float32(amplitudes)
-  k = 1
   hd = None
   if harmonic_distribution is not None:
     hd = torch_float32(harmonic_distribution)
-    k = int(hd.shape[-1])
     # normalize_harmonics (core.py:1143-1146): Nyquist mask + row normalisation
     hd_n = torch.empty_like(hd)
     amp_copy = torch.empty_like(amplitudes)
@@ -1014,6 +1086,23 @@ def streaming_harmonic_synthesis(frequencies,
           final_phase, b, f, k, n_samples, float(sample_rate),
           AMP_METHODS[amp_resample_method])
   return audio, final_phase.reshape(b, 1, 1)
+
+
+def _streaming_composition(frequencies, amplitudes, harmonic_distribution, initial_phase,
+                           n_samples, sample_rate, amp_resample_method):
+  """core.py:1140-1164 op for op: normalize_harmonics, amplitudes * distribution,
+  resample and harmonic_oscillator_bank, each differentiable."""
+  frequencies = torch_float32(frequencies)
+  amplitudes = torch_float32(amplitudes)
+  if harmonic_distribution is not None:
+    hd = normalize_harmonics(torch_float32(harmonic_distribution), frequencies, sample_rate)
+    harmonic_amplitudes = amplitudes * hd
+  else:
+    harmonic_amplitudes = amplitudes
+  frequency_envelopes = resample(frequencies, n_samples)
+  amplitude_envelopes = resample(harmonic_amplitudes, n_samples, method=amp_resample_method)
+  return harmonic_oscillator_bank(frequency_envelopes, amplitude_envelopes, initial_phase,
+                                  sample_rate=sample_rate)
 
 
 # ----------------------------------------------------------------------------
@@ -1484,6 +1573,53 @@ def variable_length_delay(phase, audio, max_length: int = 512):
 # ----------------------------------------------------------------------------
 # Wavetable synthesis (core.py:1217-1282)
 # ----------------------------------------------------------------------------
+def _linear_lookup_shapes(phase, wavetables):
+  """(B, N, W, per_sample) of linear_lookup's operands; ValueError otherwise."""
+  sp, sw = _shape(phase), _shape(wavetables)
+  if len(sp) not in (2, 3) or (len(sp) == 3 and sp[2] != 1) or sp[1] < 1:
+    raise ValueError(f'phase {sp} must be [batch, n_samples] or [batch, n_samples, 1].')
+  b, n = sp[:2]
+  ok = (len(sw) == 2 and sw[0] == b) or (len(sw) == 3 and sw[0] == b and sw[1] in (1, n))
+  if not ok or sw[-1] < 1:
+    raise ValueError(f'wavetables {sw} must be [{b}, n_wavetable], [{b}, 1, n_wavetable] or '
+                     f'[{b}, {n}, n_wavetable] for phase {sp}.')
+  return b, n, sw[-1], len(sw) == 3 and sw[1] == n and n > 1
+
+
+@on_operands_device
+def linear_lookup(phase, wavetables):
+  """core.linear_lookup (core.py:1168-1214): phase [B, N] or [B, N, 1] reads
+  wavetables [B, W], [B, 1, W] (one table per item) or [B, N, W] (one per sample) with
+  linear interpolation, column W being column 0 again -> [B, N].
+
+  The weights are the reference's own, relu(1 - |phase - lin_j| W) with lin the float32
+  linspace(0, 1, W + 1), evaluated in float32 at the few columns that can carry weight: a
+  phase outside [0, 1] is not wrapped, it gets partial weights or none.  Routes to
+  `autograd.LinearLookupFn` when grad is enabled and an input requires it (TensorFlow's
+  subgradients: d phase is 0 on a grid point)."""
+  b, n, w, per_sample = _linear_lookup_shapes(phase, wavetables)
+  if w > _lib.LOOKUP_MAX_W:
+    raise NotImplementedError(f'linear_lookup: {w} wavetable columns; at most '
+                              f'{_lib.LOOKUP_MAX_W} are supported.')
+  p = torch_float32(phase)
+  tab = torch_float32(wavetables, p.device)
+  if _requires_grad(p, tab):
+    from ddsp_b200 import autograd as _ag
+    return _ag.LinearLookupFn.apply(p, tab, per_sample)
+  return linear_lookup_forward(p, tab, per_sample)
+
+
+def linear_lookup_forward(p, tab, per_sample):
+  """`ddsp_b200_linear_lookup_forward` on float32 CUDA operands."""
+  b, n = p.shape[:2]
+  out = torch.empty((b, n), dtype=torch.float32, device=p.device)
+  if b == 0:
+    return out
+  _launch('ddsp_b200_linear_lookup_forward', p, tab, out, b, n, tab.shape[-1],
+          int(per_sample))
+  return out
+
+
 def harmonic_distribution_to_wavetable(harmonic_distribution, n_wavetable=2048):
   """core.harmonic_distribution_to_wavetable (core.py:1217-1235): one period of
   the harmonic series [batch, time, n_harmonics] as [batch, time, n_wavetable]

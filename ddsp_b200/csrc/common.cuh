@@ -96,6 +96,19 @@ __device__ __forceinline__ unsigned long long turns_to_fix64(double turns) {
   return (unsigned long long)__double2ll_rn(fr * 18446744073709551616.0);
 }
 
+// sin and cos of a fixed-point phase, rounded to 2^-32 turn: how every oscillator-bank
+// kernel evaluates its oscillators (a backward recomputes the forward's bits).
+__device__ __forceinline__ float fix64_pi31(unsigned long long ph) {
+  const uint32_t p32 = (uint32_t)((ph + 0x80000000ull) >> 32);
+  return (float)(int)p32 * 4.656612873077393e-10f;   // 2^-31: [-1, 1) half turns
+}
+__device__ __forceinline__ float fix64_sin(unsigned long long ph) {
+  return sinpif(fix64_pi31(ph));
+}
+__device__ __forceinline__ float fix64_cos(unsigned long long ph) {
+  return cospif(fix64_pi31(ph));
+}
+
 // core.exp_sigmoid (core.py:386-404): 2 * sigmoid(x)^ln(10) + 1e-7, evaluated
 // as 2 * 2^(-ln10 * log2(1 + e^-x)) + 1e-7 on the SFU (3 MUFU ops): both limits
 // are exact (x -> -inf: 1e-7, x -> +inf: 2 + 1e-7) and nothing overflows to NaN.

@@ -75,8 +75,7 @@ oscbank_apply(const float* __restrict__ f, const float* __restrict__ a,
       if (live) {
         const float fv = *fp;
         ph += turns_to_fix64((double)fv * inv_sr);
-        const uint32_t p32 = (uint32_t)((ph + 0x80000000ull) >> 32);
-        const float s = sinpif((float)(int)p32 * 4.656612873077393e-10f);
+        const float s = fix64_sin(ph);
         v = (fv >= nyquist) ? 0.f : (*ap) * s;
         if (!SUM) out[((size_t)b * N + t) * K + k] = v;
       }
@@ -171,8 +170,7 @@ oscbank_backward(const float* __restrict__ f, const float* __restrict__ a,
     const float gv = g[KIND == kObbSum ? row0 + t : i];
     if (KIND == kObbCumsum) return (double)gv;
     const float fv = f[i];
-    const uint32_t p32 = (uint32_t)((ph + 0x80000000ull) >> 32);
-    const float c = cospif((float)(int)p32 * 4.656612873077393e-10f);
+    const float c = fix64_cos(ph);
     return (fv >= nyquist) ? 0.0 : (double)(gv * (a[i] * c));
   };
 
@@ -203,8 +201,7 @@ oscbank_backward(const float* __restrict__ f, const float* __restrict__ a,
         const size_t i = (row0 + t) * K + k;
         ph += turns_to_fix64((double)f[i] * inv_sr);
         if (da != nullptr) {
-          const uint32_t p32 = (uint32_t)((ph + 0x80000000ull) >> 32);
-          const float s = sinpif((float)(int)p32 * 4.656612873077393e-10f);
+          const float s = fix64_sin(ph);
           da[i] = (f[i] >= nyquist) ? 0.f : g[KIND == kObbSum ? row0 + t : i] * s;
         }
         if (df != nullptr) tot += term(t, ph);

@@ -1,6 +1,9 @@
-// C ABI of the oscillator family: the oscillator bank, angular_cumsum, the
-// sinusoidal and wavetable synthesizers, forward and backward.
+// C ABI of the oscillator family: the oscillator bank, the harmonic oscillator bank,
+// angular_cumsum, the sinusoidal and wavetable synthesizers and linear_lookup, forward and
+// backward.
 #include "capi.cuh"
+#include "harmonic_bank.cuh"
+#include "lookup.cuh"
 #include "oscbank.cuh"
 #include "sinusoidal.cuh"
 #include "wavetable.cuh"
@@ -443,6 +446,116 @@ int ddsp_b200_wavetable_backward(const float* f0_hz, const float* amplitudes,
       DDSP_CHECK_LAUNCH("wavetable_backward(reduce)");
     }
   }
+  return 0;
+}
+
+// ---- core.harmonic_oscillator_bank (harmonic_bank.cuh) ----------------------------------
+int ddsp_b200_harmonic_oscillator_bank_backward_takes(int B, int N, int K) {
+  return B >= 0 && B <= 65535 && N >= 1 && K >= 1;
+}
+
+static int hob_check(const char* name, int B, int N, int K, float sample_rate) {
+  DDSP_REQUIRE(B >= 0 && N >= 1 && K >= 1, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d N=%d K=%d", name, B, N, K);
+  DDSP_REQUIRE(sample_rate > 0.f, DDSP_B200_E_INVALID, "%s: sample_rate must be positive",
+               name);
+  return 0;
+}
+
+int ddsp_b200_harmonic_oscillator_bank(const float* frequency,
+                                       const float* amplitude_envelopes,
+                                       const float* initial_phase, float* audio,
+                                       float* final_phase, int B, int N, int K,
+                                       float sample_rate, int use_angular_cumsum,
+                                       void* stream) {
+  int rc = hob_check("harmonic_oscillator_bank", B, N, K, sample_rate);
+  if (rc || B == 0) return rc;
+  DDSP_REQUIRE(frequency && amplitude_envelopes && audio, DDSP_B200_E_INVALID,
+               "harmonic_oscillator_bank: null pointer");
+  hob_::hob_forward<<<dim3(B, hob_::n_spans(N)), hob_::kThreads, 0, (cudaStream_t)stream>>>(
+      frequency, amplitude_envelopes, initial_phase, audio, final_phase, N, K,
+      1.0 / (double)sample_rate, use_angular_cumsum ? 0 : 1);
+  DDSP_CHECK_LAUNCH("harmonic_oscillator_bank");
+  return 0;
+}
+
+int ddsp_b200_harmonic_oscillator_bank_backward(
+    const float* frequency, const float* amplitude_envelopes, const float* initial_phase,
+    const float* grad_audio, const float* grad_final_phase, float* d_frequency,
+    float* d_amplitude_envelopes, float* d_initial_phase, int B, int N, int K,
+    float sample_rate, void* stream) {
+  int rc = hob_check("harmonic_oscillator_bank_backward", B, N, K, sample_rate);
+  if (rc || B == 0) return rc;
+  DDSP_REQUIRE(ddsp_b200_harmonic_oscillator_bank_backward_takes(B, N, K),
+               DDSP_B200_E_UNSUPPORTED,
+               "harmonic_oscillator_bank_backward: B=%d exceeds the 65535 clusters of its grid",
+               B);
+  DDSP_REQUIRE(frequency && amplitude_envelopes && grad_audio, DDSP_B200_E_INVALID,
+               "harmonic_oscillator_bank_backward: null pointer");
+  if (!d_frequency && !d_amplitude_envelopes && !d_initial_phase) return 0;
+  hob_::hob_backward<<<dim3(hob_::kCl, B), hob_::kBwWarps * 32, 0, (cudaStream_t)stream>>>(
+      frequency, amplitude_envelopes, initial_phase, grad_audio, grad_final_phase,
+      d_frequency, d_amplitude_envelopes, d_initial_phase, N, K, 1.0 / (double)sample_rate,
+      6.283185307179586 / (double)sample_rate);
+  DDSP_CHECK_LAUNCH("harmonic_oscillator_bank_backward");
+  return 0;
+}
+
+// ---- core.linear_lookup (lookup.cuh) -------------------------------------------------
+static int ll_check(const char* name, int B, int N, int W, int per_sample) {
+  DDSP_REQUIRE(B >= 0 && N >= 1 && W >= 1 && (per_sample == 0 || per_sample == 1),
+               DDSP_B200_E_INVALID, "%s: bad shape B=%d N=%d W=%d per_sample=%d", name, B,
+               N, W, per_sample);
+  DDSP_REQUIRE(W <= DDSP_B200_LOOKUP_MAX_W, DDSP_B200_E_UNSUPPORTED,
+               "%s: W=%d exceeds the %d wavetable columns supported", name, W,
+               (int)DDSP_B200_LOOKUP_MAX_W);
+  DDSP_REQUIRE((int64_t)B * N < (1ll << 31) * (int64_t)ll_::kThreads, DDSP_B200_E_INVALID,
+               "%s: B=%d N=%d exceeds the grid limit", name, B, N);
+  return 0;
+}
+
+int ddsp_b200_linear_lookup_forward(const float* phase, const float* wavetables, float* out,
+                                    int B, int N, int W, int per_sample, void* stream) {
+  DDSP_REQUIRE(phase && wavetables && out, DDSP_B200_E_INVALID,
+               "linear_lookup_forward: null pointer");
+  int rc = ll_check("linear_lookup_forward", B, N, W, per_sample);
+  if (rc || B == 0) return rc;
+  auto kern = per_sample ? ll_::ll_samples<true, false> : ll_::ll_samples<false, false>;
+  const int64_t rows = (int64_t)B * N;
+  kern<<<(unsigned)((rows + ll_::kThreads - 1) / ll_::kThreads), ll_::kThreads, 0,
+         (cudaStream_t)stream>>>(phase, wavetables, nullptr, out, rows, N, W);
+  DDSP_CHECK_LAUNCH("linear_lookup_forward");
+  return 0;
+}
+
+int ddsp_b200_linear_lookup_backward(const float* phase, const float* wavetables,
+                                     const float* grad, float* d_phase, float* d_wavetables,
+                                     int B, int N, int W, int per_sample, void* stream) {
+  DDSP_REQUIRE(phase && wavetables && grad, DDSP_B200_E_INVALID,
+               "linear_lookup_backward: null pointer");
+  int rc = ll_check("linear_lookup_backward", B, N, W, per_sample);
+  if (rc || B == 0) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int64_t rows = (int64_t)B * N;
+  if (d_phase) {
+    auto kern = per_sample ? ll_::ll_samples<true, true> : ll_::ll_samples<false, true>;
+    kern<<<(unsigned)((rows + ll_::kThreads - 1) / ll_::kThreads), ll_::kThreads, 0, st>>>(
+        phase, wavetables, grad, d_phase, rows, N, W);
+    DDSP_CHECK_LAUNCH("linear_lookup_backward(phase)");
+  }
+  if (!d_wavetables) return 0;
+  if (per_sample) {
+    ll_::ll_dtab_rows<<<grid_for(rows * 32, ll_::kThreads), ll_::kThreads, 0, st>>>(
+        phase, grad, d_wavetables, rows, W);
+    DDSP_CHECK_LAUNCH("linear_lookup_backward(wavetables)");
+    return 0;
+  }
+  const size_t smem = wt_::table_smem_bytes(W);
+  rc = set_smem(ll_::ll_dtab_items, smem, "linear_lookup_backward");
+  if (rc) return rc;
+  ll_::ll_dtab_items<<<dim3((unsigned)(ll_::kCl * wt_::table_col_tiles(W)), std::min(B, 65535)),
+                       wt_::kTabWarps * 32, smem, st>>>(phase, grad, d_wavetables, B, N, W);
+  DDSP_CHECK_LAUNCH("linear_lookup_backward(wavetables)");
   return 0;
 }
 

@@ -416,6 +416,40 @@ int ddsp_b200_oscillator_bank_tf_sequential(const float* frequency_envelopes,
                                             float sample_rate, int use_angular_cumsum,
                                             int chunk_size, void* stream);
 
+/* core.harmonic_oscillator_bank (core.py:966-1025): frequency [B,N] (Hz, one f0 per
+ * sample), amplitude_envelopes [B,N,K], initial_phase [B] radians or NULL (0) ->
+ * audio [B,N] = sum_k a[t,k] sin(k phi_t), phi_t = initial_phase + (2 pi / sr) sum_{u<=t}
+ * f_u, with no Nyquist mask.  The phase is accumulated exactly in 64-bit fixed-point turns
+ * (one scan per item) and harmonic k's is the wrapping product k phi.  final_phase [B] (or
+ * NULL) is phi after the last sample: with use_angular_cumsum != 0 the wrapped sum in
+ * [0, 2 pi) plus initial_phase, else the unwrapped sum (accumulated exactly, rounded once)
+ * plus initial_phase.  The audio does not depend on use_angular_cumsum.  B = 0 is a no-op.
+ * No workspace. */
+int ddsp_b200_harmonic_oscillator_bank(const float* frequency,
+                                       const float* amplitude_envelopes,
+                                       const float* initial_phase, float* audio,
+                                       float* final_phase, int B, int N, int K,
+                                       float sample_rate, int use_angular_cumsum,
+                                       void* stream);
+/* Its backward for grad_audio [B,N] and grad_final_phase [B] (NULL: 0).  With
+ * c_t = g_t sum_k k a[t,k] cos(k phi_t) on the forward's exact phase:
+ *   d_amplitude_envelopes[t,k] = g_t sin(k phi_t),
+ *   d_frequency[t] = (2 pi / sr) (sum_{u>=t} c_u + g_phi),
+ *   d_initial_phase = sum_u c_u + g_phi
+ * (floormod passes gradient 1; the sums in double in a fixed order, rounded once).  A NULL
+ * output is not computed; without d_frequency and d_initial_phase there is no cosine and no
+ * suffix scan.  No atomics: bit-reproducible.  Checks as the forward's.
+ * The forward takes any B; the backward runs one thread-block cluster per item and takes
+ * B <= 65535 (more is E_UNSUPPORTED):
+ * ddsp_b200_harmonic_oscillator_bank_backward_takes(B, N, K) says whether a shape is taken.
+ * No workspace: one thread-block cluster per item exchanges segment totals. */
+int ddsp_b200_harmonic_oscillator_bank_backward_takes(int B, int N, int K);
+int ddsp_b200_harmonic_oscillator_bank_backward(
+    const float* frequency, const float* amplitude_envelopes, const float* initial_phase,
+    const float* grad_audio, const float* grad_final_phase, float* d_frequency,
+    float* d_amplitude_envelopes, float* d_initial_phase, int B, int N, int K,
+    float sample_rate, void* stream);
+
 /* Frame-rate oscillator bank with per-sinusoid frequencies: the fusion of
  * resample(frequencies) + resample(amplitudes, amp_method) + oscillator_bank
  * for synths.Sinusoidal.get_signal (synths.py:305-323) and for
@@ -579,6 +613,21 @@ int ddsp_b200_wavetable_backward(const float* f0_hz, const float* amplitudes,
                                  int B, int F, int N, int Fw, int W, float sample_rate,
                                  int amp_method, void* workspace, size_t workspace_bytes,
                                  void* stream);
+
+/* core.linear_lookup (core.py:1168-1214): phase [B,N] reads wavetables [B,W]
+ * (per_sample = 0, one table per item) or [B,N,W] (per_sample = 1) -> out [B,N] =
+ * sum_{j=0..W} relu(1 - |phase - lin_j| W) T[j mod W], lin = float32 linspace(0, 1, W + 1),
+ * every step in float32 as the reference computes it; phases outside [0, 1] are not
+ * wrapped.  W <= DDSP_B200_LOOKUP_MAX_W (more is E_UNSUPPORTED).
+ * The backward writes d_phase [B,N] (TensorFlow's subgradients: 0 on a grid point of a
+ * power-of-two W) and d_wavetables (the table's shape); a NULL output is not computed.
+ * No atomics and no workspace: bit-reproducible. */
+enum { DDSP_B200_LOOKUP_MAX_W = 4194304 /* the four candidate columns stay exact */ };
+int ddsp_b200_linear_lookup_forward(const float* phase, const float* wavetables, float* out,
+                                    int B, int N, int W, int per_sample, void* stream);
+int ddsp_b200_linear_lookup_backward(const float* phase, const float* wavetables,
+                                     const float* grad, float* d_phase, float* d_wavetables,
+                                     int B, int N, int W, int per_sample, void* stream);
 
 /* spectral_ops.compute_loudness (spectral_ops.py:254-324) on audio [B,N]: frames of
  * n_fft samples every hop under `padding` (DDSP_B200_PAD_*; CENTER pads n_fft/2 zeros
