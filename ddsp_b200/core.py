@@ -232,6 +232,17 @@ def _as_f32(x):
   return torch.as_tensor(np.asarray(x, dtype=np.float32))
 
 
+def diff(x, axis=-1):
+  """core.diff (core.py:171-198): the finite difference x[1:] - x[:-1] along `axis`,
+  one shorter there.  ValueError for axis >= x.ndim."""
+  x = x if torch.is_tensor(x) else _as_f32(x)
+  ndim = x.dim()
+  if axis >= ndim:
+    raise ValueError('Invalid axis index: %d for tensor with only %d axes.' % (axis, ndim))
+  n = x.shape[axis] - 1
+  return x.narrow(axis, 1, n) - x.narrow(axis, 0, n)
+
+
 def safe_log(x, eps=1e-5):
   """core.safe_log (core.py:213-216)."""
   x = _as_f32(x)

@@ -2,6 +2,7 @@
 // mel, log-mel and MFCC, forward and backward.
 #include "capi.cuh"
 #include "spectral.cuh"
+#include "spectral_terms.cuh"
 #include "loudness.cuh"
 #include "mel.cuh"
 
@@ -66,6 +67,50 @@ int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
       reinterpret_cast<float2*>(grad_value), sums, n_bins_total, mag_weight, logmag_weight,
       1.0f / (float)n_bins_total, 1e-5f, n_bins, irfft_size);
   DDSP_CHECK_LAUNCH("spectral_l1");
+  return 0;
+}
+
+int ddsp_b200_spectral_terms(const float* stft_target, const float* stft_value,
+                             float* grad_value, double* sums, int B, int T, int F, int terms,
+                             int loss_type, float mag_weight, float delta_time_weight,
+                             float delta_freq_weight, float cumsum_freq_weight,
+                             float logmag_weight, void* stream) {
+  DDSP_REQUIRE(stft_target && stft_value && grad_value && sums, DDSP_B200_E_INVALID,
+               "spectral_terms: null pointer");
+  DDSP_REQUIRE(B >= 0 && B <= 65535 && T >= 1 && F >= 2, DDSP_B200_E_INVALID,
+               "spectral_terms: bad shape B=%d T=%d F=%d", B, T, F);
+  DDSP_REQUIRE(terms >= 1 && terms <= st_::kAllTerms, DDSP_B200_E_INVALID,
+               "spectral_terms: bad terms %d", terms);
+  DDSP_REQUIRE(loss_type == DDSP_B200_LOSS_L1 || loss_type == DDSP_B200_LOSS_L2,
+               DDSP_B200_E_INVALID, "spectral_terms: bad loss_type %d", loss_type);
+  DDSP_REQUIRE((((uintptr_t)stft_target | (uintptr_t)stft_value | (uintptr_t)grad_value) & 7) == 0,
+               DDSP_B200_E_INVALID, "spectral_terms: STFTs must be 8-byte aligned");
+  const size_t bytes = sizeof(float2) * (size_t)B * T * F;
+  DDSP_REQUIRE(!(terms & DDSP_B200_TERM_DELTA_TIME) ||
+                   !(st_::overlaps(grad_value, stft_target, bytes) ||
+                     st_::overlaps(grad_value, stft_value, bytes)),
+               DDSP_B200_E_INVALID,
+               "spectral_terms: with delta_time, grad_value must not overlap either STFT");
+  DDSP_REQUIRE(F <= st_::kMaxBins, DDSP_B200_E_UNSUPPORTED,
+               "spectral_terms: F=%d bins exceed the %d per frame supported", F, st_::kMaxBins);
+  if (B == 0) return 0;
+  // per-term weight / element count; delta_time has none when T = 1
+  const double counts[5] = {(double)B * T * F, (double)B * (T - 1) * F,
+                            (double)B * T * (F - 1), (double)B * T * F, (double)B * T * F};
+  const float weights[5] = {mag_weight, delta_time_weight, delta_freq_weight,
+                            cumsum_freq_weight, logmag_weight};
+  st_::Coeffs k;
+  for (int j = 0; j < 5; ++j) k.c[j] = counts[j] > 0 ? (float)(weights[j] / counts[j]) : 0.f;
+  const int rows = st_::tile_rows(T, F);
+  const size_t smem = st_::tile_smem(rows, F, terms);
+  st_::Kernel kern = st_::pick<1>(terms, loss_type == DDSP_B200_LOSS_L2);
+  int rc = set_smem(kern, smem, "spectral_terms");
+  if (rc) return rc;
+  dim3 grid((unsigned)((T + rows - 1) / rows), B);
+  kern<<<grid, st_::kThreads, smem, (cudaStream_t)stream>>>(
+      reinterpret_cast<const float2*>(stft_target), reinterpret_cast<const float2*>(stft_value),
+      reinterpret_cast<float2*>(grad_value), sums, T, F, rows, k);
+  DDSP_CHECK_LAUNCH("spectral_terms");
   return 0;
 }
 

@@ -127,21 +127,27 @@ class SpectralLoss:
   def _fusable(self, target_audio, audio, weights):
     """The ae.gin configuration (L1 on magnitudes and log-magnitudes,
     ae.gin:39-41) on CUDA tensors runs through three hand-written kernels per FFT
-    size around cuFFT instead of ~70 elementwise launches."""
-    return (torch.is_tensor(audio) and audio.is_cuda and torch.is_tensor(target_audio)
+    size around cuFFT instead of ~70 elementwise launches.  So does any
+    configuration with a delta_time, delta_freq or cumsum_freq term, 'L1' or 'L2',
+    at FFT sizes up to 8192 (spectral_terms)."""
+    if not (torch.is_tensor(audio) and audio.is_cuda and torch.is_tensor(target_audio)
             and target_audio.is_cuda and weights is None
-            and self.loss_type.upper() == 'L1'
-            and self.delta_time_weight <= 0 and self.delta_freq_weight <= 0
-            and self.cumsum_freq_weight <= 0
-            and (self.mag_weight > 0 or self.logmag_weight > 0)
             and audio.dim() == 2 and target_audio.shape == audio.shape
             and all(int(sz) >= 16 and (int(sz) & (int(sz) - 1)) == 0
-                    for sz in self.fft_sizes))
+                    for sz in self.fft_sizes)):
+      return False
+    loss_type = self.loss_type.upper()
+    if max(self.delta_time_weight, self.delta_freq_weight, self.cumsum_freq_weight) > 0:
+      return (loss_type in ('L1', 'L2') and
+              all(int(sz) // 2 + 1 <= _lib.SPECTRAL_TERMS_MAX_BINS for sz in self.fft_sizes))
+    return loss_type == 'L1' and (self.mag_weight > 0 or self.logmag_weight > 0)
 
   def _call_fused(self, target_audio, audio):
     return spectral_ops.SpectralLossFn.apply(
         target_audio.detach(), audio, tuple(int(s) for s in self.fft_sizes),
-        max(self.mag_weight, 0.0), max(self.logmag_weight, 0.0))
+        max(self.mag_weight, 0.0), max(self.logmag_weight, 0.0),
+        max(self.delta_time_weight, 0.0), max(self.delta_freq_weight, 0.0),
+        max(self.cumsum_freq_weight, 0.0), self.loss_type)
 
   def call(self, target_audio, audio, weights=None):
     if self._fusable(target_audio, audio, weights):
@@ -159,7 +165,7 @@ class SpectralLoss:
 
   def _call_spectrograms(self, target_audio, audio, weights):
     loss = 0.0
-    diff = lambda x, axis: torch.diff(x, dim=axis)
+    diff = core.diff
     for loss_op in self.spectrogram_ops:
       target_mag = loss_op(target_audio)
       value_mag = loss_op(audio)

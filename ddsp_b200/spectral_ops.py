@@ -9,6 +9,8 @@ compute_loudness and compute_power run on hand-written CUDA kernels
 (csrc/loudness.cuh) instead: the framed audio would be 32x the input.  So do
 compute_mel, compute_logmel and compute_mfcc (csrc/mel.cuh).
 """
+import math
+
 import numpy as np
 import torch
 
@@ -154,37 +156,83 @@ def _loss_weights(counts, mag_weight, logmag_weight, device):
   return _LOSS_WEIGHTS[key]
 
 
+# the terms of losses.SpectralLoss in the order of their bits in `terms`
+# (DDSP_B200_TERM_*) and of their slots in spectral_terms' sums
+_TERMS = (_lib.TERM_MAG, _lib.TERM_DELTA_TIME, _lib.TERM_DELTA_FREQ, _lib.TERM_CUMSUM_FREQ,
+          _lib.TERM_LOGMAG)
+_TERM_WEIGHTS = {}
+
+
+def _term_weights(shapes, weights, device):
+  """[[weight / element count per term] per FFT size] in float64, cached per device.
+  An inactive term (weight <= 0) weighs 0; an active one with no elements (delta_time
+  of a single frame) weighs NaN: the mean of nothing, as in the reference."""
+  key = (tuple(shapes), tuple(weights), str(device))
+  if key not in _TERM_WEIGHTS:
+    rows = []
+    for b, t, f in shapes:
+      counts = (b * t * f, b * (t - 1) * f, b * t * (f - 1), b * t * f, b * t * f)
+      rows.append([0.0 if w <= 0 else (w / m if m > 0 else math.nan)
+                   for w, m in zip(weights, counts)])
+    _TERM_WEIGHTS[key] = torch.tensor(rows, dtype=torch.float64, device=device)
+  return _TERM_WEIGHTS[key]
+
+
 class SpectralLossFn(torch.autograd.Function):
-  """The whole multi-scale 'L1' spectrogram loss (losses.SpectralLoss.call,
-  losses.py:194-243, `ae.gin` weights) as ONE autograd node: per FFT size framing +
-  Hann (kernel), cuFFT r2c of target and value, one pass leaving both L1 sums and
-  the value-STFT gradient IN PLACE of the value STFT; backward is cuFFT c2r plus a
-  windowed overlap-add per size that accumulates, already scaled by the upstream
-  gradient (read on the device), into a single dL/d audio buffer.  No elementwise
-  torch op on either pass."""
+  """The whole multi-scale spectrogram loss (losses.SpectralLoss.call,
+  losses.py:194-243) as ONE autograd node: per FFT size framing + Hann (kernel),
+  cuFFT r2c of target and value, one pass leaving the loss sums and the value-STFT
+  gradient; backward is cuFFT c2r plus a windowed overlap-add per size that
+  accumulates, already scaled by the upstream gradient (read on the device), into a
+  single dL/d audio buffer.  No elementwise torch op on either pass.
+
+  The `ae.gin` configuration ('L1', mag and logmag only) runs spectral_l1, which
+  writes the gradient in place of the value STFT.  Any other configuration ('L1' or
+  'L2', any of the five terms) runs spectral_terms; with delta_time its gradient
+  goes to a buffer of its own (the kernel reads neighbouring frames)."""
 
   @staticmethod
-  def forward(ctx, target, audio, fft_sizes, mag_weight, logmag_weight):
+  def forward(ctx, target, audio, fft_sizes, mag_weight, logmag_weight,
+              delta_time_weight=0.0, delta_freq_weight=0.0, cumsum_freq_weight=0.0,
+              loss_type='L1'):
+    weights = tuple(float(w) for w in (mag_weight, delta_time_weight, delta_freq_weight,
+                                       cumsum_freq_weight, logmag_weight))
+    loss_type = loss_type.upper()
+    if loss_type not in ('L1', 'L2'):
+      raise ValueError(f"SpectralLossFn: loss_type must be 'L1' or 'L2', got {loss_type!r}")
+    l1_only = loss_type == 'L1' and max(weights[1:4]) <= 0
+    terms = sum(bit for bit, w in zip(_TERMS, weights) if w > 0)
     with core._on_device_of(target, audio):
       audio = audio.to(torch.float32).contiguous()
       target = target.to(torch.float32).contiguous()
       b, n = audio.shape
-      sums = torch.zeros((len(fft_sizes), 2), dtype=torch.float64, device=audio.device)
-      grads, counts = [], []
+      sums = torch.zeros((len(fft_sizes), 2 if l1_only else 5), dtype=torch.float64,
+                         device=audio.device)
+      grads, counts, shapes = [], [], []
       for idx, size in enumerate(fft_sizes):
         size = int(size)
         step = int(size * 0.25)
         xt = torch.fft.rfft(_frame_window(target, size, step), n=size, dim=-1)
         xv = torch.fft.rfft(_frame_window(audio, size, step), n=size, dim=-1)
         m = xv.numel()
-        core._launch('ddsp_b200_spectral_l1', xt, xv, xv, sums[idx], m, float(mag_weight),
-                     float(logmag_weight), xv.shape[-1], -1)
-        del xt
-        grads.append(xv)                 # now holds d loss_size / d X_value, irfft-ready
+        if l1_only:
+          core._launch('ddsp_b200_spectral_l1', xt, xv, xv, sums[idx], m, float(mag_weight),
+                       float(logmag_weight), xv.shape[-1], -1)
+          grad = xv
+        else:
+          grad = torch.empty_like(xv) if weights[1] > 0 else xv
+          core._launch('ddsp_b200_spectral_terms', xt, xv, grad, sums[idx], *xv.shape,
+                       terms, getattr(_lib, 'LOSS_' + loss_type), *weights)
+        del xt, xv
+        grads.append(grad)               # now holds d loss_size / d X_value, irfft-ready
         counts.append(m)
+        shapes.append(tuple(grad.shape))
       ctx.save_for_backward(*grads)
       ctx.meta = (b, n, tuple(int(sz) for sz in fft_sizes))
-      w = _loss_weights(counts, mag_weight, logmag_weight, audio.device)
+      if l1_only:
+        w = _loss_weights(counts, mag_weight, logmag_weight, audio.device)
+      else:
+        w = _term_weights(shapes, weights, audio.device)
       return (sums * w).sum().to(torch.float32)
 
   @staticmethod
@@ -197,11 +245,11 @@ class SpectralLossFn(torch.autograd.Function):
       step = int(size * 0.25)
       n_frames = -(-n // step)
       # unnormalised inverse (the 1/n pass would be an elementwise kernel over the
-      # frames; spectral_l1 left the spectrum scaled for exactly this)
+      # frames; the loss kernels left the spectrum scaled for exactly this)
       gf = torch.fft.irfft(grads[idx], n=size, dim=-1, norm='forward').contiguous()
       core._launch('ddsp_b200_frame_window_adjoint', gf, _hann(size, go.device), grad_audio,
                    b, n, n_frames, size, step, go, int(idx > 0))
-    return None, grad_audio, None, None, None
+    return None, grad_audio, None, None, None, None, None, None, None
 
 
 def stft_cuda(audio, frame_size, overlap=0.75):

@@ -516,6 +516,32 @@ int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
                           float mag_weight, float logmag_weight, int n_bins,
                           int irfft_size, void* stream);
 
+/* spectral_terms: every spectrogram term of losses.SpectralLoss (losses.py:194-234)
+ * for complex STFTs [B, T, F] (interleaved re/im, F = fft_size/2 + 1) of target and
+ * value, 'L1' or 'L2'.  For each term in `terms` (DDSP_B200_TERM_* flags) it adds
+ * the sum of |d| (L1) or d^2 (L2), d = target term - value term, to sums[bit index]
+ * (mag 0, delta_time 1, delta_freq 2, cumsum_freq 3, logmag 4; the caller zeroes
+ * them), and writes to grad_value d/dX_v of sum weight * mean(term), pre-scaled for
+ * an unnormalised inverse transform (spectral_l1's irfft_size = -1).  The terms of
+ * m = |X|: mag m, delta_time core.diff(m, axis=1), delta_freq core.diff(m, axis=2),
+ * cumsum_freq cumsum(m, axis=2), logmag safe_log(m).  grad_value may be
+ * stft_value unless delta_time is active, when it must overlap neither STFT.
+ * F > DDSP_B200_SPECTRAL_TERMS_MAX_BINS (fft_size 8192) is E_UNSUPPORTED. */
+enum {
+  DDSP_B200_TERM_MAG = 1,
+  DDSP_B200_TERM_DELTA_TIME = 2,
+  DDSP_B200_TERM_DELTA_FREQ = 4,
+  DDSP_B200_TERM_CUMSUM_FREQ = 8,
+  DDSP_B200_TERM_LOGMAG = 16
+};
+enum { DDSP_B200_LOSS_L1 = 0, DDSP_B200_LOSS_L2 = 1 };
+enum { DDSP_B200_SPECTRAL_TERMS_MAX_BINS = 4097 /* frame rows one CTA stages */ };
+int ddsp_b200_spectral_terms(const float* stft_target, const float* stft_value,
+                             float* grad_value, double* sums, int B, int T, int F, int terms,
+                             int loss_type, float mag_weight, float delta_time_weight,
+                             float delta_freq_weight, float cumsum_freq_weight,
+                             float logmag_weight, void* stream);
+
 /* processors.Add.get_signal (processors.py:174-176). out may alias a or b. */
 int ddsp_b200_add(const float* a, const float* b, float* out, int64_t n,
                   void* stream);
