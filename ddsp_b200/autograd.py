@@ -50,6 +50,8 @@ kernels, exposed as `torch.autograd.Function`s:
   * `MixtureNLLFn` / `CombNLLFn` - the Gaussian-mixture NLLs of the consistency
     losses (`losses.KDEConsistencyLoss`, `losses.TWMLoss`), evaluated per frame
     on-chip with gradients to every input;
+  * `NoteMomentsFn` - nn.get_note_moments and nn.pool_over_notes, d x through the
+    per-note mean and std;
   * `HmmLogProbFn` - the HMM log-likelihood of `losses.HmmTranscriber`, with
     gradients to the observations (pitch and amplitude); routed to by
     `core.hmm_log_prob` under grad;
@@ -891,6 +893,46 @@ class WassersteinFn(torch.autograd.Function):
     want = ctx.needs_input_grad
     return (du if want[0] else None, dv if want[1] else None, dwu if want[2] else None,
             dwv if want[3] else None, None)
+
+class NoteMomentsFn(torch.autograd.Function):
+  """nn.get_note_moments (pool=False) or nn.pool_over_notes (pool=True) on x [B,T,D] and
+  a float mask [B,T,N] (csrc/notes.cuh): (mean, std) per note [B,N,D], or pooled back to
+  the frames [B,T,D]; only the mean when `with_std` is false.  Differentiable in x only;
+  the mask is a constant.  Grads are not materialised, so an output nobody uses adds no
+  term: an unused std cannot turn the mean's gradient into 0 * inf = NaN.  Saves x, the
+  mask and the per-note moments."""
+
+  @staticmethod
+  def forward(ctx, x, mask, pool, with_std):
+    ctx.set_materialize_grads(False)
+    b, t, d = x.shape
+    n = mask.shape[2]
+    mean = torch.empty((b, n, d), dtype=torch.float32, device=x.device)
+    std = torch.empty_like(mean) if with_std else None
+    pm = torch.empty_like(x) if pool else None
+    ps = torch.empty_like(x) if pool and with_std else None
+    core._launch('ddsp_b200_note_moments', x, mask, mean, std, pm, ps, b, t, n, d)
+    ctx.save_for_backward(x, mask, mean, std)
+    ctx.pool = pool
+    outs = (pm, ps) if pool else (mean, std)
+    return outs if with_std else outs[0]
+
+  @staticmethod
+  def backward(ctx, *grads):
+    x, mask, mean, std = ctx.saved_tensors
+    g = [None if a is None else a.contiguous().to(torch.float32) for a in grads]
+    g += [None] * (2 - len(g))
+    if g[0] is None and g[1] is None:
+      return None, None, None, None
+    b, t, d = x.shape
+    n = mask.shape[2]
+    gm, gs, gpm, gps = (None, None, g[0], g[1]) if ctx.pool else (g[0], g[1], None, None)
+    dx = torch.empty_like(x)
+    nbytes = 8 * b * n * d + 256 if b and n and d else 0   # A and C, [B,N,D] each
+    core._launch('ddsp_b200_note_moments_backward', x, mask, mean, std, gm, gs, gpm, gps, dx,
+                 *core._workspace(nbytes, x.device), b, t, n, d)
+    return dx, None, None, None
+
 
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):
   """core.exp_sigmoid (core.py:386-404) as differentiable torch ops."""

@@ -472,6 +472,21 @@ def harmonic_controls(amplitudes, harmonic_distribution, f0_hz, sample_rate,
   return amps_out, hd_out
 
 
+def note_mask(q, onset, max_regions, note_on_only):
+  """The launch behind nn.get_note_mask (onset None) and nn.get_note_mask_from_onset:
+  the float32 mask [B, T_out, max_regions] of the contiguous float32 CUDA pitches q
+  [B, T] (and onsets [B, T]); T_out = T, or 2 for one frame under the edge rule."""
+  b, t = q.shape
+  t_out = t if onset is not None or t > 1 else 2
+  mask = torch.empty((b, t_out, max_regions), dtype=torch.float32, device=q.device)
+  flag = int(bool(note_on_only))
+  # the edge rule's per-region decisions: a byte per region that can hold a frame
+  nbytes = b * min(max_regions, t) if onset is None and flag else 0
+  _launch('ddsp_b200_note_mask', q, onset, mask, *_workspace(nbytes, q.device),
+          b, t, max_regions, flag)
+  return mask
+
+
 def safe_divide(numerator, denominator, eps=1e-7):
   """core.safe_divide (core.py:207-210)."""
   safe = torch.where(denominator == 0.0, torch.full_like(denominator, eps),

@@ -1,8 +1,10 @@
 // C ABI of the loss family: the consistency mixture and comb NLLs,
-// sinusoidal_to_harmonic, the HMM and the Wasserstein distance, forward and backward.
+// sinusoidal_to_harmonic, the HMM, the Wasserstein distance and the note functions of
+// the MIDI autoencoder, forward and backward.
 #include "capi.cuh"
 #include "consistency.cuh"
 #include "hmm.cuh"
+#include "notes.cuh"
 #include "wasserstein.cuh"
 
 using namespace ddsp;
@@ -372,6 +374,177 @@ int ddsp_b200_wasserstein_backward(const float* u, const float* v, const float* 
   ws_::wasserstein_backward_kernel<<<(unsigned)R, ws_::threads_for(m), smem,
                                      (cudaStream_t)stream>>>(wp, grad, du, dv, dwu, dwv);
   DDSP_CHECK_LAUNCH("wasserstein_backward");
+  return 0;
+}
+
+// ---- nn.get_note_mask, get_note_moments, pool_over_notes ---------------------------------
+// Region decisions of the edge rule with note_on_only: one byte per region that can hold a
+// frame (min(R, T)) per item.
+static size_t note_mask_regions(int B, int T, int R, int onset, int note_on_only) {
+  if (onset || !note_on_only || B <= 0 || T <= 0 || R <= 0) return 0;
+  return (size_t)B * (size_t)(R < T ? R : T);
+}
+
+int ddsp_b200_note_mask(const float* q, const float* onset, float* mask, void* workspace,
+                        size_t workspace_bytes, int B, int T, int R, int note_on_only,
+                        void* stream) {
+  DDSP_REQUIRE(B >= 0 && T >= 1 && R >= 0, DDSP_B200_E_INVALID,
+               "note_mask: bad shape B=%d T=%d R=%d", B, T, R);
+  DDSP_REQUIRE(note_on_only == 0 || note_on_only == 1, DDSP_B200_E_INVALID,
+               "note_mask: note_on_only must be 0 or 1, got %d", note_on_only);
+  const bool empty = B == 0 || R == 0;
+  DDSP_REQUIRE(empty || (q && mask), DDSP_B200_E_INVALID, "note_mask: null pointer");
+  const size_t need = note_mask_regions(B, T, R, onset != nullptr, note_on_only);
+  DDSP_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), DDSP_B200_E_WORKSPACE,
+               "note_mask: workspace of %zu B is smaller than the %zu B needed",
+               workspace_bytes, need);
+  if (empty) return 0;
+  notes_::MaskParams p;
+  p.q = q;
+  p.onset = onset;
+  p.on = static_cast<uint8_t*>(workspace);
+  p.T = T;
+  p.T_out = onset || T > 1 ? T : 2;
+  p.R = R;
+  p.Rf = R < T ? R : T;
+  p.note_on_only = note_on_only;
+  if (onset)
+    notes_::note_mask_kernel<true><<<(unsigned)B, notes_::kMaskThreads, 0,
+                                     (cudaStream_t)stream>>>(p, mask);
+  else
+    notes_::note_mask_kernel<false><<<(unsigned)B, notes_::kMaskThreads, 0,
+                                      (cudaStream_t)stream>>>(p, mask);
+  DDSP_CHECK_LAUNCH("note_mask");
+  return 0;
+}
+
+// The shape checks of the moments entry points, and the CTA count of a grid of tiles of
+// `rows` rows (notes or frames) by D dims per item.
+static int notes_check(const char* name, int B, int T, int N, int D, notes_::Params* p) {
+  DDSP_REQUIRE(B >= 0 && T >= 1 && N >= 0 && D >= 0, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d T=%d N=%d D=%d", name, B, T, N, D);
+  p->T = T;
+  p->N = N;
+  p->D = D;
+  p->tiles_d = (D + notes_::kDTile - 1) / notes_::kDTile;
+  return 0;
+}
+
+static int notes_grid(const char* name, int B, int rows, notes_::Params* p, unsigned* grid) {
+  p->tiles_r = (rows + notes_::kTile - 1) / notes_::kTile;
+  const int64_t ctas = (int64_t)B * p->tiles_r * p->tiles_d;
+  DDSP_REQUIRE(ctas <= DDSP_B200_MAX_ROWS, DDSP_B200_E_INVALID,
+               "%s: %lld tiles exceed the 2^31 - 1 grid limit", name, (long long)ctas);
+  *grid = (unsigned)ctas;
+  return 0;
+}
+
+int ddsp_b200_note_moments(const float* x, const float* mask, float* mean, float* stdev,
+                           float* pooled_mean, float* pooled_std, int B, int T, int N, int D,
+                           void* stream) {
+  notes_::Params p;
+  int rc = notes_check("note_moments", B, T, N, D, &p);
+  if (rc) return rc;
+  const bool empty = B == 0 || N == 0 || D == 0;
+  DDSP_REQUIRE(empty || (x && mask && mean), DDSP_B200_E_INVALID,
+               "note_moments: null pointer");
+  DDSP_REQUIRE(empty || !pooled_std || (stdev && pooled_mean), DDSP_B200_E_INVALID,
+               "note_moments: pooled_std needs std and pooled_mean");
+  unsigned grid_n = 0, grid_t = 0;
+  rc = notes_grid("note_moments", B, N, &p, &grid_n);
+  if (rc) return rc;
+  notes_::Params pt = p;
+  rc = notes_grid("note_moments", B, T, &pt, &grid_t);
+  if (rc) return rc;
+  if (B == 0 || D == 0) return 0;
+  if (N == 0) {   // nothing to pool: the pooled sums are zero
+    const size_t bytes = sizeof(float) * (size_t)B * T * D;
+    if (pooled_mean)
+      DDSP_CUDA_TRY(cudaMemsetAsync(pooled_mean, 0, bytes, (cudaStream_t)stream), "note_moments");
+    if (pooled_std)
+      DDSP_CUDA_TRY(cudaMemsetAsync(pooled_std, 0, bytes, (cudaStream_t)stream), "note_moments");
+    return 0;
+  }
+  p.x = pt.x = x;
+  p.m = pt.m = mask;
+  if (stdev)
+    notes_::note_moments_kernel<true><<<grid_n, notes_::kThreads, 0, (cudaStream_t)stream>>>(
+        p, mean, stdev);
+  else
+    notes_::note_moments_kernel<false><<<grid_n, notes_::kThreads, 0, (cudaStream_t)stream>>>(
+        p, mean, nullptr);
+  DDSP_CHECK_LAUNCH("note_moments");
+  if (!pooled_mean) return 0;
+  const notes_::OverN o{mean, stdev, nullptr};
+  if (pooled_std)
+    notes_::note_over_n_kernel<notes_::kPoolBoth><<<grid_t, notes_::kThreads, 0,
+                                                    (cudaStream_t)stream>>>(
+        pt, o, pooled_mean, pooled_std);
+  else
+    notes_::note_over_n_kernel<notes_::kPoolMean><<<grid_t, notes_::kThreads, 0,
+                                                    (cudaStream_t)stream>>>(
+        pt, o, pooled_mean, nullptr);
+  DDSP_CHECK_LAUNCH("note_pool");
+  return 0;
+}
+
+// The backward's A and C, [B,N,D] floats each, from a 256-byte boundary.
+static size_t note_backward_bytes(int B, int N, int D) {
+  if (B <= 0 || N <= 0 || D <= 0) return 0;
+  return 2 * sizeof(float) * (size_t)B * N * D + 256;
+}
+
+int ddsp_b200_note_moments_backward(const float* x, const float* mask, const float* mean,
+                                    const float* stdev, const float* grad_mean,
+                                    const float* grad_std, const float* grad_pooled_mean,
+                                    const float* grad_pooled_std, float* dx, void* workspace,
+                                    size_t workspace_bytes, int B, int T, int N, int D,
+                                    void* stream) {
+  notes_::Params p;
+  int rc = notes_check("note_moments_backward", B, T, N, D, &p);
+  if (rc) return rc;
+  const bool empty = B == 0 || D == 0;
+  DDSP_REQUIRE(empty || (x && dx && (N == 0 || (mask && mean))), DDSP_B200_E_INVALID,
+               "note_moments_backward: null pointer");
+  const bool with_std = grad_std || grad_pooled_std;
+  DDSP_REQUIRE(!with_std || stdev || N == 0, DDSP_B200_E_INVALID,
+               "note_moments_backward: a std gradient needs std");
+  const size_t need = note_backward_bytes(B, N, D);
+  DDSP_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), DDSP_B200_E_WORKSPACE,
+               "note_moments_backward: workspace of %zu B is smaller than the %zu B needed",
+               workspace_bytes, need);
+  unsigned grid_n = 0, grid_t = 0;
+  rc = notes_grid("note_moments_backward", B, N, &p, &grid_n);
+  if (rc) return rc;
+  notes_::Params pt = p;
+  rc = notes_grid("note_moments_backward", B, T, &pt, &grid_t);
+  if (rc) return rc;
+  if (empty) return 0;
+  if (N == 0) {   // x enters no note
+    DDSP_CUDA_TRY(cudaMemsetAsync(dx, 0, sizeof(float) * (size_t)B * T * D,
+                                  (cudaStream_t)stream), "note_moments_backward");
+    return 0;
+  }
+  p.x = pt.x = x;
+  p.m = pt.m = mask;
+  float* A = align256<float>(workspace);
+  float* C = A + (size_t)B * N * D;
+  const notes_::Grads g{mean, stdev, grad_mean, grad_std, grad_pooled_mean, grad_pooled_std};
+  if (with_std)
+    notes_::note_moments_backward_kernel<true><<<grid_n, notes_::kThreads, 0,
+                                                 (cudaStream_t)stream>>>(p, g, A, C);
+  else
+    notes_::note_moments_backward_kernel<false><<<grid_n, notes_::kThreads, 0,
+                                                  (cudaStream_t)stream>>>(p, g, A, nullptr);
+  DDSP_CHECK_LAUNCH("note_moments_backward");
+  const notes_::OverN o{A, C, mean};
+  if (with_std)
+    notes_::note_over_n_kernel<notes_::kDxBoth><<<grid_t, notes_::kThreads, 0,
+                                                  (cudaStream_t)stream>>>(pt, o, dx, nullptr);
+  else
+    notes_::note_over_n_kernel<notes_::kDxMean><<<grid_t, notes_::kThreads, 0,
+                                                  (cudaStream_t)stream>>>(pt, o, dx, nullptr);
+  DDSP_CHECK_LAUNCH("note_moments_backward");
   return 0;
 }
 

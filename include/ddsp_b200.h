@@ -843,6 +843,52 @@ int ddsp_b200_wasserstein_backward(const float* u, const float* v, const float* 
                                    float* dwu, float* dwv, int64_t R, int Nu, int Nv, float p,
                                    void* stream);
 
+/* training/nn.py:375-557, the note functions of the MIDI autoencoder.
+ * ddsp_b200_note_mask: the dense mask [B, T_out, R] of get_note_mask (onset null) or
+ *   get_note_mask_from_onset (onset [B,T]) for q [B,T] (channel 0 of a 3-D q_pitch).
+ *   Edge rule: frame 0 opens region 0; frame t in 1 .. T-2 opens a new region iff
+ *   |q_t - q_{t-1}| > 0 (NaN never does); the last frame joins the region before it.
+ *   T_out = T, except T = 1 gives two rows, both region 0.  Onset rule: frame t >= 1
+ *   adds (int)onset_t (truncation) to the region count, T_out = T; non-finite onsets and
+ *   onsets of magnitude 2^31 or more are outside the contract.  Row t is 1 at its region
+ *   index when 0 <= index < R and the note is on, else 0.  note_on_only: with the edge
+ *   rule a region is on iff the reference's mask-weighted sum of q over all T frames is
+ *   > 0, decided in double (a non-finite frame outside the region makes it NaN: off);
+ *   with the onset rule a frame is on iff q_t > 0.  workspace: scratch of at least
+ *   B * min(R, T) bytes with the edge rule and note_on_only, else none (E_WORKSPACE if
+ *   smaller).  B >= 0, T >= 1, R >= 0; B = 0 or R = 0
+ *   returns after the checks without a launch.
+ * ddsp_b200_note_moments: for x [B,T,D] and any float mask [B,T,N],
+ *   L_n = sum_t m_tn, Ls_n = L_n or 1e-7 where L_n = 0,
+ *   mean [B,N,D] = sum_t m_tn x_td / Ls_n, std [B,N,D] = (sum_t ((x_td - mean) m_tn)^2 / Ls_n)^0.5
+ *   (two passes; std may be null), and, when pooled_mean is not null, pooled_mean [B,T,D] =
+ *   sum_n m_tn mean_nd and (pooled_std not null, which needs std) pooled_std = sum_n m_tn std_nd.
+ *   One launch, or two when pooling.  N = 0 writes zero pooled values.
+ * ddsp_b200_note_moments_backward: dx [B,T,D] from any of grad_mean, grad_std [B,N,D] and
+ *   grad_pooled_mean, grad_pooled_std [B,T,D] (null for none; a std gradient needs std):
+ *   with Gmu = grad_mean + sum_t m grad_pooled_mean, Gs = grad_std + sum_t m grad_pooled_std,
+ *   Gv = Gs 0.5 / std, GQ = Gv / Ls, r_tnd = (x_td - mean_nd) m_tn,
+ *   Gmu' = Gmu - 2 GQ sum_t m_tn r_tnd, dx_td = sum_n m_tn (Gmu'_nd / Ls_n + 2 GQ_nd r_tnd);
+ *   without a std gradient the GQ terms are skipped.  std = 0 under a std gradient gives NaN
+ *   (0 * inf) through the whole (b, d), as autograd does.  workspace: scratch of at least
+ *   8 B N D + 256 bytes when B, N and D are positive (E_WORKSPACE if smaller).  Two launches.
+ * Both moment entry points take B >= 0, T >= 1, N, D >= 0 and at most 2^31 - 1 CTAs (B
+ * times the tiles of 32 notes or frames by 64 dims); B = 0 or D = 0 returns after the
+ * checks without a launch.  All three: no atomics, fixed summation orders,
+ * bit-reproducible. */
+int ddsp_b200_note_mask(const float* q, const float* onset, float* mask, void* workspace,
+                        size_t workspace_bytes, int B, int T, int R, int note_on_only,
+                        void* stream);
+int ddsp_b200_note_moments(const float* x, const float* mask, float* mean, float* std,
+                           float* pooled_mean, float* pooled_std, int B, int T, int N, int D,
+                           void* stream);
+int ddsp_b200_note_moments_backward(const float* x, const float* mask, const float* mean,
+                                    const float* std, const float* grad_mean,
+                                    const float* grad_std, const float* grad_pooled_mean,
+                                    const float* grad_pooled_std, float* dx, void* workspace,
+                                    size_t workspace_bytes, int B, int T, int N, int D,
+                                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif
