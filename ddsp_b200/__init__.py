@@ -10,6 +10,7 @@ from ddsp_b200 import dags
 from ddsp_b200 import effects
 from ddsp_b200 import host
 from ddsp_b200 import nn
+from ddsp_b200 import preprocessing
 from ddsp_b200 import processors
 from ddsp_b200 import synths
 from ddsp_b200.effects import (ExpDecayReverb, FIRFilter, FilteredNoiseReverb,

@@ -1,10 +1,11 @@
 // C ABI of the feature family: framing, the spectral loss, loudness, RMS power,
-// mel, log-mel and MFCC, forward and backward.
+// mel, log-mel and MFCC, forward and backward, and CREPE's frames, Viterbi path and f0.
 #include "capi.cuh"
 #include "spectral.cuh"
 #include "spectral_terms.cuh"
 #include "loudness.cuh"
 #include "mel.cuh"
+#include "crepe.cuh"
 
 using namespace ddsp;
 
@@ -248,6 +249,64 @@ int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n
                                                   frame_size, hop, pad_left, in_db, d.pmin,
                                                   d.range_db, d.ref_db);
   DDSP_CHECK_LAUNCH("rms_power");
+  return 0;
+}
+
+// ---- CREPE: frames, Viterbi path, f0 and confidence ------------------------------
+int ddsp_b200_crepe_frames(const float* audio, float* frames, int B, int N, int n_frames,
+                           int hop, int padding, void* stream) {
+  DDSP_REQUIRE(audio && (frames || n_frames == 0 || B == 0), DDSP_B200_E_INVALID,
+               "crepe_frames: null pointer");
+  int pad_left = 0;
+  // the kernel strides over all B * n_frames frames, so the batch has no grid limit
+  // and is checked here alone
+  DDSP_REQUIRE(B >= 0, DDSP_B200_E_INVALID, "crepe_frames: bad shape B=%d", B);
+  int rc = framing_check("crepe_frames", B > 0, N, n_frames, crepe_::kFrame, hop, padding,
+                         &pad_left);
+  if (rc || B == 0 || n_frames == 0) return rc;
+  const int64_t total = (int64_t)B * n_frames;
+  const int threads = 32 * crepe_::kFrameWarps;
+  crepe_::crepe_frames_kernel<<<grid_for(total * 32, threads, 16), threads, 0,
+                                (cudaStream_t)stream>>>(audio, frames, N, n_frames, total,
+                                                        hop, pad_left);
+  DDSP_CHECK_LAUNCH("crepe_frames");
+  return 0;
+}
+
+size_t ddsp_b200_crepe_viterbi_workspace_bytes(int B, int T) {
+  if (B <= 0 || T <= 1) return 0;
+  return sizeof(uint32_t) * crepe_::kRecordWords * (size_t)B * (size_t)(T - 1);
+}
+
+int ddsp_b200_crepe_viterbi(const float* activations, int* centers, void* workspace,
+                            size_t workspace_bytes, int B, int T, void* stream) {
+  DDSP_REQUIRE(B >= 0 && T >= 1, DDSP_B200_E_INVALID, "crepe_viterbi: bad shape B=%d T=%d",
+               B, T);
+  DDSP_REQUIRE(B == 0 || (activations && centers), DDSP_B200_E_INVALID,
+               "crepe_viterbi: null pointer");
+  const size_t need = ddsp_b200_crepe_viterbi_workspace_bytes(B, T);
+  DDSP_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), DDSP_B200_E_WORKSPACE,
+               "crepe_viterbi: workspace of %zu bytes, %zu needed", workspace_bytes, need);
+  DDSP_REQUIRE(((uintptr_t)workspace & 3) == 0, DDSP_B200_E_INVALID,
+               "crepe_viterbi: workspace must be 4-byte aligned");
+  if (B == 0) return 0;
+  crepe_::crepe_viterbi_kernel<<<B, crepe_::kThreads, 0, (cudaStream_t)stream>>>(
+      activations, centers, T, static_cast<uint32_t*>(workspace));
+  DDSP_CHECK_LAUNCH("crepe_viterbi");
+  return 0;
+}
+
+int ddsp_b200_crepe_decode(const float* activations, const int* centers, float* f0,
+                           float* confidence, int64_t M, void* stream) {
+  DDSP_REQUIRE(M >= 0, DDSP_B200_E_INVALID, "crepe_decode: bad shape M=%lld", (long long)M);
+  DDSP_REQUIRE(M == 0 || (activations && f0 && confidence), DDSP_B200_E_INVALID,
+               "crepe_decode: null pointer");
+  if (M == 0) return 0;
+  const int threads = 32 * crepe_::kDecodeWarps;
+  crepe_::crepe_decode_kernel<<<grid_for(M * 32, threads, 16), threads, 0,
+                                (cudaStream_t)stream>>>(activations, centers, f0,
+                                                        confidence, M);
+  DDSP_CHECK_LAUNCH("crepe_decode");
   return 0;
 }
 

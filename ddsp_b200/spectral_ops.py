@@ -7,9 +7,11 @@ CPU tests can pin it against the NumPy oracle.
 
 compute_loudness and compute_power run on hand-written CUDA kernels
 (csrc/loudness.cuh) instead: the framed audio would be 32x the input.  So do
-compute_mel, compute_logmel and compute_mfcc (csrc/mel.cuh).
+compute_mel, compute_logmel and compute_mfcc (csrc/mel.cuh), and everything
+PretrainedCREPE does around its network (csrc/crepe.cuh).
 """
 import math
+import os
 
 import numpy as np
 import torch
@@ -261,6 +263,7 @@ def stft_cuda(audio, frame_size, overlap=0.75):
 
 
 # ---- loudness and RMS power (spectral_ops.py:136-324, csrc/loudness.cuh) ------
+F0_RANGE = 127.0  # MIDI
 DB_RANGE = 80.0
 _A_WEIGHTS = {}
 
@@ -293,12 +296,7 @@ def _framing(audio, frame_size, hop_size, padding):
   if len(shape) not in (1, 2) or shape[-1] < 1:
     raise ValueError(f'audio must be [batch, n_samples], [n_samples] or '
                      f'[batch, n_samples, 1], got shape {tuple(shape)}')
-  if padding != 'valid' and hop_size > frame_size:
-    raise ValueError(f'During padding, frame_size ({frame_size}) must be greater '
-                     f'than hop_size ({hop_size}).')
-  if padding not in ('center', 'same', 'valid'):
-    raise ValueError('`padding` must be one of [\'center\', \'same\', \'valid\'], '
-                     f'received ({padding}).')
+  _padding_check(frame_size, hop_size, padding)
   n = shape[-1]
   if padding == 'same':
     n_frames = -(-n // hop_size)
@@ -588,3 +586,181 @@ def compute_mfcc(audio, lo_hz=20.0, hi_hz=8000.0, fft_size=1024, mel_bins=128,
   times rsqrt(2 mel_bins)), cut to [..., :mfcc_bins] with Python's slice rules."""
   return _mel(audio, lo_hz, hi_hz, mel_bins, fft_size, overlap, pad_end, sample_rate,
               _lib.MFCC, mfcc_bins=mfcc_bins, name='compute_mfcc')
+
+
+# ---- pad and CREPE (spectral_ops.py:171-220, 432-566, csrc/crepe.cuh) -------------
+CREPE_SAMPLE_RATE = 16000
+CREPE_FRAME_SIZE = 1024
+_CREPE_BINS = _lib.CREPE_BINS
+_CREPE_SIZES = ('full', 'large', 'small', 'tiny')
+
+
+def pad(x, frame_size, hop_size, padding='center', axis=1, mode='CONSTANT',
+        constant_values=0):
+  """spectral_ops.pad (spectral_ops.py:171-220): pads `x` (any shape; axis 0 when it has
+  one axis) for strided framing, on the device it is on.  'valid' returns x as float32
+  unchecked; 'same' pads the end to get_framed_lengths' padded length; 'center' pads
+  frame_size // 2 on both sides.  mode is tf.pad's: 'CONSTANT' (constant_values),
+  'REFLECT' (the edge not repeated) or 'SYMMETRIC' (the edge repeated), any case."""
+  x = core._as_f32(x)
+  if padding == 'valid':
+    return x
+  _padding_check(frame_size, hop_size, padding)
+  if x.dim() <= 1:
+    axis = 0
+  axis = axis % max(x.dim(), 1)
+  n_t = x.shape[axis]
+  if padding == 'same':
+    _, n_t_padded = get_framed_lengths(n_t, frame_size, hop_size, padding)
+    left, right = 0, int(n_t_padded - n_t)
+  else:
+    left = right = int(frame_size // 2)
+  mode = mode.upper()
+  if mode == 'CONSTANT':
+    shape = list(x.shape)
+    parts = []
+    for amount in (left, right):
+      shape[axis] = amount
+      parts.append(torch.full(shape, constant_values, dtype=x.dtype, device=x.device))
+    return torch.cat([parts[0], x, parts[1]], dim=axis)
+  if mode not in ('REFLECT', 'SYMMETRIC'):
+    raise ValueError(f'mode must be one of CONSTANT, REFLECT or SYMMETRIC, got {mode!r}')
+  # tf.pad's limits: REFLECT pads less than the axis, SYMMETRIC at most the axis
+  limit = n_t - 1 if mode == 'REFLECT' else n_t
+  if max(left, right) > limit:
+    raise ValueError(f'{mode} padding of {max(left, right)} on an axis of {n_t} elements')
+  i = torch.arange(-left, n_t + right, device=x.device)
+  if mode == 'REFLECT':
+    i = torch.where(i < 0, -i, torch.where(i >= n_t, 2 * (n_t - 1) - i, i))
+  else:
+    i = torch.where(i < 0, -i - 1, torch.where(i >= n_t, 2 * n_t - 1 - i, i))
+  return x.index_select(axis, i)
+
+
+def _padding_check(frame_size, hop_size, padding):
+  """pad's checks for the padding modes that pad, in its order."""
+  if padding != 'valid' and hop_size > frame_size:
+    raise ValueError(f'During padding, frame_size ({frame_size}) must be greater '
+                     f'than hop_size ({hop_size}).')
+  if padding not in ('center', 'same', 'valid'):
+    raise ValueError('`padding` must be one of [\'center\', \'same\', \'valid\'], '
+                     f'received ({padding}).')
+
+
+def _crepe_frames(audio, hop_size, padding):
+  """pad + batch_frames + normalize_frames as one kernel: [B * n_frames, 1024]."""
+  b, n, _, n_frames, code = _framing(audio, CREPE_FRAME_SIZE, hop_size, padding)
+  x = _audio_2d(audio, b, n)
+  frames = torch.empty((b * n_frames, CREPE_FRAME_SIZE), dtype=torch.float32,
+                       device=x.device)
+  core._launch('ddsp_b200_crepe_frames', x, frames, b, n, n_frames, hop_size, code)
+  return frames, b
+
+
+class PretrainedCREPE:
+  """spectral_ops.PretrainedCREPE (spectral_ops.py:432-566): pitch from a CREPE network,
+  with everything around the network on CUDA kernels (csrc/crepe.cuh).
+
+  model_size_or_path is the network, mapping normalised frames [M, 1024] to activations
+  [M, 360]: a torch.nn.Module or any callable, or the path of a TorchScript file (the
+  reference's SavedModel branch).  The sizes 'full', 'large', 'small' and 'tiny' name
+  the weights of the `crepe` package, which are not shipped here: they raise
+  NotImplementedError.  Nothing here is differentiable: inputs that require grad raise,
+  and the network runs under torch.no_grad()."""
+
+  def __init__(self, model_size_or_path, hop_size=160):
+    self.hop_size = int(hop_size)
+    self.frame_size = CREPE_FRAME_SIZE
+    self.sample_rate = CREPE_SAMPLE_RATE
+    if isinstance(model_size_or_path, str) and model_size_or_path in _CREPE_SIZES:
+      raise NotImplementedError(
+          f"PretrainedCREPE: the '{model_size_or_path}' weights come with the crepe "
+          'package and are not available here; pass the network as a torch module or '
+          'callable, or the path of a TorchScript file.')
+    if isinstance(model_size_or_path, (str, os.PathLike)):
+      self.core_model = torch.jit.load(os.fspath(model_size_or_path))
+    elif callable(model_size_or_path):
+      self.core_model = model_size_or_path
+    else:
+      raise TypeError('PretrainedCREPE: model_size_or_path must be a callable network or '
+                      f'a path, got {type(model_size_or_path).__name__}')
+    self.model_size_or_path = model_size_or_path
+
+  @classmethod
+  def activations_to_f0_and_confidence(cls, activations, centers=None):
+    """(f0_hz [M], confidence [M, 1]) of activations [M, 360]: the row max, and the
+    activation-weighted mean of the cents of the 10 bins centre - 4 .. centre + 5 (each
+    clamped into 0 .. 359) in Hz.  The centre is each row's first argmax, or centers [M]
+    (cast to int32 as the reference does).  Weights summing to 0 give NaN (0 / 0), as
+    in the reference."""
+    shape = core._shape(activations)
+    if len(shape) != 2 or shape[1] != _CREPE_BINS:
+      raise ValueError(f'activations must be [n_frames, {_CREPE_BINS}], got {shape}')
+    if centers is not None and tuple(core._shape(centers)) != shape[:1]:
+      raise ValueError(f'centers must be [{shape[0]}], got {tuple(core._shape(centers))}')
+    core._no_grad_path('PretrainedCREPE.activations_to_f0_and_confidence', activations)
+    acts = core.torch_float32(activations)
+    if centers is not None:
+      centers = torch.as_tensor(centers, device=acts.device).to(torch.int32).contiguous()
+    m = shape[0]
+    f0 = torch.empty((m,), dtype=torch.float32, device=acts.device)
+    confidence = torch.empty((m, 1), dtype=torch.float32, device=acts.device)
+    core._launch('ddsp_b200_crepe_decode', acts, centers, f0, confidence, m)
+    return f0, confidence
+
+  def batch_frames(self, audio):
+    """Frames of 1024 every hop_size of padded audio [B, N], stacked into [B * F, 1024]
+    (tf.signal.frame, pad_end=False); audio of exactly 1024 samples is one frame."""
+    audio = core._as_f32(audio)
+    if audio.shape[-1] == self.frame_size:
+      return audio
+    if audio.shape[-1] < self.frame_size:
+      return audio.new_zeros((0, self.frame_size))
+    frames = audio.unfold(-1, self.frame_size, self.hop_size)
+    return frames.reshape(-1, self.frame_size)
+
+  def normalize_frames(self, frames):
+    """(frames - mean) / std per frame [M, 1024], with tf.nn.moments' mean and
+    population variance (summed in double) and std = 1e-8 where the variance is 0."""
+    shape = core._shape(frames)
+    if len(shape) != 2 or shape[1] != self.frame_size:
+      raise ValueError(f'frames must be [n_frames, {self.frame_size}], got {shape}')
+    core._no_grad_path('PretrainedCREPE.normalize_frames', frames)
+    x = core.torch_float32(frames)
+    out = torch.empty_like(x)
+    if shape[0]:
+      core._launch('ddsp_b200_crepe_frames', x, out, shape[0], self.frame_size, 1,
+                   self.frame_size, _lib.PAD_VALID)
+    return out
+
+  def predict_f0_and_confidence(self, audio, viterbi=False, padding='center'):
+    """(f0_hz, confidence), each [B, F], of audio [B, N] or [N]: padding, framing and
+    normalisation in one kernel, the network, then Viterbi centres if asked for and the
+    local-average f0."""
+    core._no_grad_path('PretrainedCREPE.predict_f0_and_confidence', audio)
+    frames, b = _crepe_frames(audio, self.hop_size, padding)
+    with torch.no_grad():
+      acts = self.core_model(frames)
+    acts = core.torch_float32(acts, frames.device)
+    if tuple(acts.shape) != (frames.shape[0], _CREPE_BINS):
+      raise ValueError(f'the network mapped frames {tuple(frames.shape)} to '
+                       f'{tuple(acts.shape)}, not [{frames.shape[0]}, {_CREPE_BINS}]')
+    centers = None
+    if viterbi:
+      centers = self.viterbi_decode(acts.reshape(b, -1, _CREPE_BINS)).reshape(-1)
+    f0_hz, confidence = self.activations_to_f0_and_confidence(acts, centers)
+    return f0_hz.reshape(b, -1), confidence.reshape(b, -1)
+
+  def viterbi_decode(self, acts):
+    """centres [B, T] (int64) of activations [B, T, 360]: the posterior mode of
+    create_hmm's HMM (csrc/crepe.cuh), ties to the lowest bin as tf.argmax's."""
+    shape = core._shape(acts)
+    if len(shape) != 3 or shape[2] != _CREPE_BINS or shape[1] < 1:
+      raise ValueError(f'acts must be [batch, n_frames >= 1, {_CREPE_BINS}], got {shape}')
+    core._no_grad_path('PretrainedCREPE.viterbi_decode', acts)
+    x = core.torch_float32(acts)
+    b, t, _ = shape
+    centers = torch.empty((b, t), dtype=torch.int32, device=x.device)
+    core._launch('ddsp_b200_crepe_viterbi', x, centers,
+                 *core._workspace('ddsp_b200_crepe_viterbi_workspace_bytes', x.device, b, t), b, t)
+    return centers.to(torch.int64)

@@ -19,8 +19,8 @@
  *     thread-local).
  *   - Return value: 0 = ok, negative = DDSP_B200_E_* below.  Shape/argument
  *     errors are detected BEFORE any launch.
- *   - The *_workspace, *_takes and ddsp_b200_ir_size queries are pure host
- *     functions: they launch nothing and set no error.
+ *   - The *_workspace, *_workspace_bytes, *_takes and ddsp_b200_ir_size queries
+ *     are pure host functions: they launch nothing and set no error.
  *
  * The Python binding (ddsp_b200/_lib.py) is derived from this file at import:
  * every ddsp_b200_* prototype and every DDSP_B200_* integer constant.  A C type
@@ -679,6 +679,38 @@ int ddsp_b200_loudness_backward(const float* audio, const float* weights,
 int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n_frames,
                         int frame_size, int hop, int padding, int in_db, float range_db,
                         float ref_db, void* stream);
+
+/* spectral_ops.PretrainedCREPE (spectral_ops.py:432-566) around its network.  All three
+ * are forward only, with no atomics: bit-reproducible.
+ * ddsp_b200_crepe_frames: the network's input frames [B * n_frames, 1024] of audio [B,N]:
+ *   pad (padding DDSP_B200_PAD_*: CENTER pads 512 zeros on both sides, SAME pads the end
+ *   to (ceil(N/hop) - 1) hop + 1024, VALID nothing), frames of 1024 every hop
+ *   (tf.signal.frame, pad_end=False), each normalised to (x - mean) / std with the mean
+ *   and population variance of tf.nn.moments, summed in double, and std = 1e-8 where the
+ *   variance is 0.  n_frames must be that padding's frame count (0 for VALID audio
+ *   shorter than a frame); hop <= 1024 unless VALID.  B = 0 or n_frames = 0 returns after
+ *   the checks without a launch.
+ * ddsp_b200_crepe_viterbi: centers [B,T] (int32), HiddenMarkovModel.posterior_mode of
+ *   activations [B,T,360] under create_hmm's model (uniform start, transitions
+ *   max(12 - |i - j|, 1e-5) over their row sums, Multinomial(1, eye 0.1 + 0.9/360)
+ *   emissions); every tie goes to the lowest state index, as tf.argmax's.  workspace:
+ *   ddsp_b200_crepe_viterbi_workspace_bytes(B, T) bytes of back pointers (E_WORKSPACE if
+ *   smaller; 0 for T = 1, when it may be null), 4-byte aligned.  B >= 0, T >= 1, both
+ *   otherwise unbounded; B = 0 returns after the checks without a launch.
+ * ddsp_b200_crepe_decode: activations_to_f0_and_confidence of activations [M,360]:
+ *   confidence [M] = the row max, f0 [M] = 10 2^(c / 1200) Hz with c the weighted mean of
+ *   the float32 cents linspace(0, 7180, 360) + 1997.3794084376191 over bins
+ *   centre - 4 .. centre + 5, each clamped into 0 .. 359.  The centre is the row's first
+ *   argmax, or centers[m] (int32, any value) when centers is not null.  Weights summing
+ *   to 0 give NaN (0 / 0), as in the reference.  M >= 0; M = 0 launches nothing. */
+enum { DDSP_B200_CREPE_BINS = 360, DDSP_B200_CREPE_FRAME = 1024 };
+int ddsp_b200_crepe_frames(const float* audio, float* frames, int B, int N, int n_frames,
+                           int hop, int padding, void* stream);
+size_t ddsp_b200_crepe_viterbi_workspace_bytes(int B, int T);
+int ddsp_b200_crepe_viterbi(const float* activations, int* centers, void* workspace,
+                            size_t workspace_bytes, int B, int T, void* stream);
+int ddsp_b200_crepe_decode(const float* activations, const int* centers, float* f0,
+                           float* confidence, int64_t M, void* stream);
 
 /* output stage of ddsp_b200_mel_forward / _backward */
 enum { DDSP_B200_MEL = 0, DDSP_B200_LOGMEL = 1, DDSP_B200_MFCC = 2 };
