@@ -177,8 +177,30 @@ def on_operands_device(fn):
   return wrapper
 
 
-def _check_out(out, shape, like, name='out'):
-  """`out=` of the synthesizers is written by a kernel: B*N contiguous floats."""
+def _byte_range(t):
+  """[first, last + 1) byte of the contiguous tensor t in its device memory."""
+  return t.data_ptr(), t.data_ptr() + t.numel() * t.element_size()
+
+
+def _overlaps(a, b):
+  """Whether the contiguous tensors a and b share a byte of memory."""
+  if a.numel() == 0 or b.numel() == 0 or a.device != b.device:
+    return False
+  a0, a1 = _byte_range(a)
+  b0, b1 = _byte_range(b)
+  return a0 < b1 and b0 < a1
+
+
+def _check_out(out, shape, like, inputs=(), exact_alias_ok=False, name='out'):
+  """`out=` of the synthesizers is written by a kernel: B*N contiguous floats.
+
+  Returns `inputs` (tensors or None) with every one that overlaps `out` cloned, so
+  that no kernel reads memory it is writing: `out=` never changes the result.  With
+  exact_alias_ok the kernel is elementwise, and an input that IS `out` (same first
+  byte and extent) is passed as it is.  Inputs the kernel reads only in launches
+  before the one that writes `out` need not be passed.  Un-aliased calls copy
+  nothing.  Under grad mode an `out` that requires grad is refused, as torch's own
+  out= ops refuse it; call _wrote(out) after the write."""
   if (not isinstance(out, torch.Tensor) or not out.is_cuda or
       out.dtype != torch.float32 or not out.is_contiguous() or
       tuple(out.shape) != tuple(shape) or out.device != like.device):
@@ -186,6 +208,21 @@ def _check_out(out, shape, like, name='out'):
         f'{name} must be a contiguous float32 CUDA tensor of shape {tuple(shape)} '
         f'on {like.device}; got {type(out).__name__}'
         + (f' {tuple(out.shape)} {out.dtype} {out.device}' if isinstance(out, torch.Tensor) else ''))
+  if torch.is_grad_enabled() and out.requires_grad:
+    raise RuntimeError(
+        f'ddsp_b200: functions with {name}= arguments do not support automatic '
+        f'differentiation, but {name} requires grad.  Call without {name}= to get a '
+        'differentiable result, or pass an output that does not require grad.')
+  return [x.clone() if x is not None and _overlaps(x, out) and not (
+      exact_alias_ok and _byte_range(x) == _byte_range(out)) else x for x in inputs]
+
+
+def _wrote(out):
+  """Records a kernel's write to `out` in its autograd version counter, so that a
+  backward pass that saved `out` before the write raises instead of using the new
+  values.  Returns out."""
+  torch.autograd.graph.increment_version(out)
+  return out
 
 
 def _no_grad_path(name, *tensors):
@@ -829,11 +866,11 @@ def sinusoidal_synthesis(frequencies, amplitudes, n_samples: int = 64000,
     out = torch.empty((b, n_samples), dtype=torch.float32, device=freqs.device)
     accumulate = False
   else:
-    _check_out(out, (b, n_samples), freqs)
+    freqs, amps = _check_out(out, (b, n_samples), freqs, (freqs, amps))
   _launch('ddsp_b200_sinusoidal_forward', freqs, amps, out, b, f, k, n_samples,
           float(sample_rate), AMP_METHODS[amp_resample_method], int(bool(accumulate)),
           *_workspace('ddsp_b200_sinusoidal_workspace', freqs.device, b, f, k))
-  return out
+  return _wrote(out)
 
 
 @on_operands_device
@@ -932,7 +969,9 @@ def harmonic_synthesis(frequencies,
   if harmonic_shifts is not None:
     harmonic_shifts = torch_float32(harmonic_shifts)
   if out is not None:
-    _check_out(out, (b, n_samples), frequencies)
+    frequencies, amplitudes, harmonic_distribution, harmonic_shifts = _check_out(
+        out, (b, n_samples), frequencies,
+        (frequencies, amplitudes, harmonic_distribution, harmonic_shifts))
   else:
     accumulate = False
 
@@ -954,7 +993,7 @@ def harmonic_synthesis(frequencies,
     _launch('ddsp_b200_harmonic_forward', frequencies, amplitudes, harmonic_distribution,
             out, b, f, k, n_samples, float(sample_rate), AMP_METHODS[amp_resample_method],
             mode, int(bool(accumulate)))
-    return out
+    return _wrote(out)
 
   # frame-rate harmonic frequencies / amplitudes, float32 op for op as the
   # reference (core.py:1091-1099): (f0 * k) * (1 + shifts), amplitudes * hd
@@ -1286,13 +1325,16 @@ def fft_convolve_lti(audio, impulse_response, start, out_len, out=None,
   if out is None:
     out = torch.empty((b, out_len), dtype=torch.float32, device=audio.device)
     accumulate = False
+  else:
+    # the kernel reads both operands into its workspace before it writes out
+    _check_out(out, (b, out_len), audio)
   flags = ((_lib.LTI_REVERSE_AUDIO if reverse_audio else 0) |
            (_lib.LTI_REVERSE_IR if reverse_ir else 0))
   _launch('ddsp_b200_fft_convolve_lti', audio, impulse_response, out, b, n, s_len, ir_batch,
           int(start), int(out_len), int(bool(accumulate)), flags,
           *_workspace('ddsp_b200_fft_convolve_lti_workspace', audio.device, b, n, s_len,
                       ir_batch))
-  return out
+  return _wrote(out)
 
 
 def _fft_convolve_geometry(sa, si, padding, delay_compensation):
@@ -1360,28 +1402,30 @@ def fft_convolve(audio, impulse_response, padding: Text = 'same',
       # trainable reverb (effects.py:70-79): forward and backward are the same
       # kernels (the backward on time-reversed operands)
       from ddsp_b200 import autograd as _ag
+      if out is not None:
+        # the backward reads the operands it saved: not the ones out= overwrites
+        audio, ir2 = _check_out(out, (batch_size, crop_size), audio, (audio, ir2))
       wet = _ag.FftConvolveLtiFn.apply(audio, ir2, int(start), int(crop_size))
       if out is None:
         return wet
-      _check_out(out, (batch_size, crop_size), audio)
       if accumulate:
         out += wet
       else:
         out.copy_(wet)
       return out
-    if out is not None:
-      _check_out(out, (batch_size, crop_size), audio)
     return fft_convolve_lti(audio, ir2, int(start), int(crop_size), out=out,
                             accumulate=accumulate)
   if ir_size >= FFT_CONVOLVE_MIN_IR:
     # time-varying filter with long impulse responses (several IR frames of >= 2048
     # taps): no reference configuration does this; the reference's own framed
     # algorithm on cuFFT
+    if out is not None:
+      # the result is a fresh tensor: out is written only after every read
+      _check_out(out, (batch_size, crop_size), audio)
     wet = _fft_convolve_cufft(audio, impulse_response, n_ir_frames, frame_size,
                               fft_size, int(start), int(crop_size))
     if out is None:
       return wet
-    _check_out(out, tuple(wet.shape), audio)
     if accumulate:
       out += wet
     else:
@@ -1391,7 +1435,9 @@ def fft_convolve(audio, impulse_response, padding: Text = 'same',
     # time-varying FIR under training (FIRFilter, short reverbs): CUDA backward
     # kernels for both operands (csrc/fir_backward.cuh)
     if out is not None:
-      _check_out(out, (batch_size, crop_size), audio)
+      # the backward reads the operands it saved: not the ones out= overwrites
+      audio, impulse_response = _check_out(out, (batch_size, crop_size), audio,
+                                           (audio, impulse_response))
     from ddsp_b200 import autograd as _ag
     wet = _ag.FirTimeVaryingFn.apply(audio, impulse_response, padding, int(start))
     if out is None:
@@ -1406,12 +1452,13 @@ def fft_convolve(audio, impulse_response, padding: Text = 'same',
                       device=audio.device)
     accumulate = False
   else:
-    _check_out(out, (batch_size, crop_size), audio)
+    audio, impulse_response = _check_out(out, (batch_size, crop_size), audio,
+                                         (audio, impulse_response))
   impulse_response = impulse_response.contiguous()
   _launch('ddsp_b200_fir_time_varying', audio, impulse_response, out, batch_size,
           audio_size, n_ir_frames, ir_size, ir_batch, _lib.PADDING[padding], int(start),
           int(bool(accumulate)))
-  return out
+  return _wrote(out)
 
 
 @on_operands_device
@@ -1862,12 +1909,12 @@ def filtered_noise(magnitudes, n_samples, window_size=257, noise=None, seed=0,
                       device=magnitudes.device)
     accumulate = False
   else:
-    _check_out(out, (b, n_samples), magnitudes)
+    magnitudes, noise = _check_out(out, (b, n_samples), magnitudes, (magnitudes, noise))
   _launch('ddsp_b200_filtered_noise_forward', magnitudes, noise, int(seed), int(offset),
           out, b, f, nb, n_samples, int(window_size), int(bool(accumulate)),
           *_workspace('ddsp_b200_filtered_noise_workspace', magnitudes.device, b, f, nb,
                       n_samples, int(window_size)))
-  return out
+  return _wrote(out)
 
 
 @on_operands_device
@@ -1942,5 +1989,7 @@ def add_forward(a, b, out=None):
     a, b = a.contiguous(), b.contiguous()
   if out is None:
     out = torch.empty_like(a)
+  else:
+    a, b = _check_out(out, tuple(a.shape), a, (a, b), exact_alias_ok=True)
   _launch('ddsp_b200_add', a, b, out, a.numel())
-  return out
+  return _wrote(out)

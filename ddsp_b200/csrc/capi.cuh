@@ -32,6 +32,19 @@ static int ir_frame(int N, int F) {
   return frame;
 }
 
+// Whether the byte ranges [a, a + a_bytes) and [b, b + b_bytes) share a byte (a null
+// pointer or an empty range shares none).
+inline bool overlaps(const void* a, size_t a_bytes, const void* b, size_t b_bytes) {
+  return a && b && a_bytes && b_bytes && (uintptr_t)a < (uintptr_t)b + b_bytes &&
+         (uintptr_t)b < (uintptr_t)a + a_bytes;
+}
+
+// Elements of an extent given as a product of shape arguments; a negative factor
+// (an invalid shape, refused by the entry point's own checks) counts as empty.
+inline size_t extent(int64_t a, int64_t b = 1, int64_t c = 1) {
+  return (a <= 0 || b <= 0 || c <= 0) ? 0 : (size_t)a * (size_t)b * (size_t)c;
+}
+
 // Workspaces are carved from the first 256-byte boundary at or after `p`.
 template <typename T>
 static T* align256(const void* p) {
@@ -40,7 +53,25 @@ static T* align256(const void* p) {
 
 }  // namespace ddsp
 
-#define DDSP_CUDA_TRY(expr, what)                                         \
+// E_INVALID, before any launch, when the float output `out` of `out_n` elements
+// overlaps the float input `in` of `in_n` elements: a kernel whose threads read
+// inputs that other threads write would race.
+#define DDSP_REQUIRE_DISJOINT(fn, out, out_n, in, in_n)                          \
+  DDSP_REQUIRE(!::ddsp::overlaps((out), sizeof(float) * (out_n), (in),            \
+                                 sizeof(float) * (in_n)),                         \
+               DDSP_B200_E_INVALID, "%s: %s must not overlap %s", (fn), #out, #in)
+
+// The same for an output that may BE the input `in` (an elementwise kernel in place):
+// only the exact alias, same first element and extent, passes besides disjoint ranges.
+#define DDSP_REQUIRE_SAME_OR_DISJOINT(fn, out, out_n, in, in_n)                  \
+  DDSP_REQUIRE(((const void*)(out) == (const void*)(in) &&                        \
+                (size_t)(out_n) == (size_t)(in_n)) ||                             \
+                   !::ddsp::overlaps((out), sizeof(float) * (out_n), (in),        \
+                                     sizeof(float) * (in_n)),                     \
+               DDSP_B200_E_INVALID, "%s: %s must be %s or not overlap it", (fn), #out, \
+               #in)
+
+#define DDSP_CUDA_TRY(expr, what)                                       \
   do {                                                                    \
     cudaError_t e__ = (expr);                                             \
     if (e__ != cudaSuccess) {                                             \

@@ -20,6 +20,7 @@ int ddsp_b200_sinc_impulse_response(const float* cutoff, float* ir, int64_t BF, 
                "%s: bad shape BF=%lld S=%d (S must be odd)", name, (long long)BF, S);
   DDSP_REQUIRE(BF < (1ll << 31), DDSP_B200_E_INVALID, "%s: too many frames", name);
   if (BF == 0) return 0;
+  DDSP_REQUIRE_DISJOINT(name, ir, extent(BF, S), cutoff, extent(BF));
   sinc_ir_kernel<<<(unsigned)BF, kSincThreads, 0, (cudaStream_t)stream>>>(cutoff, ir, S, scale,
                                                                           high_pass);
   DDSP_CHECK_LAUNCH(name);
@@ -81,6 +82,8 @@ int ddsp_b200_sinc_filter(const float* audio, const float* cutoff, float* out, i
   int rc = sinc_filter_check(name, B, N, F, S, cutoff_batch, padding, &frame, &start,
                              &out_len);
   if (rc || B == 0) return rc;
+  DDSP_REQUIRE_DISJOINT(name, out, extent(B, out_len), audio, extent(B, N));
+  DDSP_REQUIRE_DISJOINT(name, out, extent(B, out_len), cutoff, extent(cutoff_batch, F));
   const size_t smem = sinc_filter_smem(S);
   rc = set_smem(sinc_filter_kernel, smem, name);
   if (rc) return rc;
@@ -247,6 +250,7 @@ int ddsp_b200_resample(const float* in, float* out, int B, int F, int C, int N,
                  "frames:%d, add_endpoint=%s).", add_endpoint ? "" : " - 1", N,
                  n_frames, add_endpoint ? "True" : "False");
   }
+  DDSP_REQUIRE_DISJOINT("resample", out, extent(B, N, C), in, extent(B, F, C));
   if (B == 0) return 0;
   const int64_t total = (int64_t)B * N * C;
   resample_kernel<<<grid_for(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(
@@ -260,6 +264,8 @@ int ddsp_b200_add(const float* a, const float* b, float* out, int64_t n,
   DDSP_REQUIRE(a && b && out, DDSP_B200_E_INVALID, "add: null pointer");
   DDSP_REQUIRE(n >= 0, DDSP_B200_E_INVALID, "add: n < 0");
   if (n == 0) return 0;
+  DDSP_REQUIRE_SAME_OR_DISJOINT("add", out, extent(n), a, extent(n));
+  DDSP_REQUIRE_SAME_OR_DISJOINT("add", out, extent(n), b, extent(n));
   add_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(a, b, out, n);
   DDSP_CHECK_LAUNCH("add");
   return 0;
@@ -309,6 +315,9 @@ int ddsp_b200_mix_forward(const float* signal_one, const float* signal_two,
                "mix_forward: null pointer");
   DDSP_REQUIRE(B >= 0 && N >= 1 && C >= 1, DDSP_B200_E_INVALID,
                "mix_forward: bad shape B=%d N=%d C=%d", B, N, C);
+  DDSP_REQUIRE_SAME_OR_DISJOINT("mix_forward", out, extent(B, N, C), signal_one, extent(B, N, C));
+  DDSP_REQUIRE_SAME_OR_DISJOINT("mix_forward", out, extent(B, N, C), signal_two, extent(B, N, C));
+  DDSP_REQUIRE_SAME_OR_DISJOINT("mix_forward", out, extent(B, N, C), mix_level, extent(B, N));
   if (B == 0) return 0;
   const int64_t total = (int64_t)B * N * C;
   rt_::mix_kernel<<<grid_for(total, rt_::kThreads), rt_::kThreads, 0, (cudaStream_t)stream>>>(
@@ -341,6 +350,9 @@ int ddsp_b200_exp_decay_ir(const float* gain, const float* decay, const float* n
   DDSP_REQUIRE(gain && decay && ir, DDSP_B200_E_INVALID, "exp_decay_ir: null pointer");
   DDSP_REQUIRE(rows >= 0 && L >= 1, DDSP_B200_E_INVALID,
                "exp_decay_ir: bad shape rows=%d L=%d", rows, L);
+  DDSP_REQUIRE_DISJOINT("exp_decay_ir", ir, extent(rows, L), gain, extent(rows));
+  DDSP_REQUIRE_DISJOINT("exp_decay_ir", ir, extent(rows, L), decay, extent(rows));
+  DDSP_REQUIRE_DISJOINT("exp_decay_ir", ir, extent(rows, L), noise, extent(L));
   if (rows == 0) return 0;
   const int64_t total = (int64_t)rows * ((L + 3) / 4);
   rt_::exp_decay_ir_kernel<<<grid_for(total, rt_::kThreads), rt_::kThreads, 0,
@@ -373,6 +385,9 @@ int ddsp_b200_mod_delay_forward(const float* audio, const float* phase, const fl
   DDSP_REQUIRE(B >= 0 && B <= 65535 && N >= 1 && max_length >= 1 && max_length < (1 << 29),
                DDSP_B200_E_INVALID, "mod_delay_forward: bad shape B=%d N=%d max_length=%d",
                B, N, max_length);
+  DDSP_REQUIRE_DISJOINT("mod_delay_forward", out, extent(B, N), audio, extent(B, N));
+  DDSP_REQUIRE_SAME_OR_DISJOINT("mod_delay_forward", out, extent(B, N), phase, extent(B, N));
+  DDSP_REQUIRE_SAME_OR_DISJOINT("mod_delay_forward", out, extent(B, N), gain, extent(B, N));
   if (B == 0) return 0;
   dim3 grid((unsigned)((N + md_::kThreads - 1) / md_::kThreads), B);
   md_::mod_delay_forward_kernel<<<grid, md_::kThreads, 0, (cudaStream_t)stream>>>(

@@ -22,6 +22,8 @@ int ddsp_b200_frame_window(const float* audio, const float* window, float* frame
                N, n_frames, frame_size, frame_step);
   DDSP_REQUIRE((((uintptr_t)window | (uintptr_t)frames) & 15) == 0, DDSP_B200_E_INVALID,
                "frame_window: window / frames must be 16-byte aligned");
+  DDSP_REQUIRE_DISJOINT("frame_window", frames, extent(B, n_frames, frame_size), audio, extent(B, N));
+  DDSP_REQUIRE_DISJOINT("frame_window", frames, extent(B, n_frames, frame_size), window, extent(frame_size));
   if (B == 0) return 0;
   const long long quads = ((long long)n_frames * frame_size) / 4;
   dim3 grid((unsigned)((quads + 255) / 256), B);
@@ -41,6 +43,10 @@ int ddsp_b200_frame_window_adjoint(const float* grad_frames, const float* window
   DDSP_REQUIRE(B >= 0 && N >= 1 && n_frames >= 1 && frame_size >= 1 && frame_step >= 1 &&
                    B <= 65535,
                DDSP_B200_E_INVALID, "frame_window_adjoint: bad shape");
+  DDSP_REQUIRE_DISJOINT("frame_window_adjoint", grad_audio, extent(B, N), grad_frames,
+                        extent(B, n_frames, frame_size));
+  DDSP_REQUIRE_DISJOINT("frame_window_adjoint", grad_audio, extent(B, N), window, extent(frame_size));
+  DDSP_REQUIRE_DISJOINT("frame_window_adjoint", grad_audio, extent(B, N), scale_device, extent(1));
   if (B == 0) return 0;
   dim3 grid((N + 255) / 256, B);
   frame_window_adjoint_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
@@ -62,6 +68,8 @@ int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
                (long long)n_bins_total, n_bins, irfft_size);
   DDSP_REQUIRE((((uintptr_t)stft_target | (uintptr_t)stft_value | (uintptr_t)grad_value) & 15) == 0,
                DDSP_B200_E_INVALID, "spectral_l1: tensors must be 16-byte aligned");
+  DDSP_REQUIRE_DISJOINT("spectral_l1", grad_value, extent(n_bins_total, 2), stft_target, extent(n_bins_total, 2));
+  DDSP_REQUIRE_SAME_OR_DISJOINT("spectral_l1", grad_value, extent(n_bins_total, 2), stft_value, extent(n_bins_total, 2));
   const long long blocks = std::min<long long>((n_bins_total / 2 + 255) / 256 + 1, 8ll * num_sms());
   spectral_l1_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
       reinterpret_cast<const float2*>(stft_target), reinterpret_cast<const float2*>(stft_value),
@@ -88,12 +96,15 @@ int ddsp_b200_spectral_terms(const float* stft_target, const float* stft_value,
                DDSP_B200_E_INVALID, "spectral_terms: STFTs must be 8-byte aligned");
   const size_t bytes = sizeof(float2) * (size_t)B * T * F;
   DDSP_REQUIRE(!(terms & DDSP_B200_TERM_DELTA_TIME) ||
-                   !(st_::overlaps(grad_value, stft_target, bytes) ||
-                     st_::overlaps(grad_value, stft_value, bytes)),
+                   !(overlaps(grad_value, bytes, stft_target, bytes) ||
+                     overlaps(grad_value, bytes, stft_value, bytes)),
                DDSP_B200_E_INVALID,
                "spectral_terms: with delta_time, grad_value must not overlap either STFT");
   DDSP_REQUIRE(F <= st_::kMaxBins, DDSP_B200_E_UNSUPPORTED,
                "spectral_terms: F=%d bins exceed the %d per frame supported", F, st_::kMaxBins);
+  DDSP_REQUIRE_SAME_OR_DISJOINT("spectral_terms", grad_value, extent(B, T, 2 * F), stft_target,
+                                extent(B, T, 2 * F));
+  DDSP_REQUIRE_SAME_OR_DISJOINT("spectral_terms", grad_value, extent(B, T, 2 * F), stft_value, extent(B, T, 2 * F));
   if (B == 0) return 0;
   // per-term weight / element count; delta_time has none when T = 1
   const double counts[5] = {(double)B * T * F, (double)B * (T - 1) * F,
@@ -193,6 +204,8 @@ int ddsp_b200_loudness_forward(const float* audio, const float* weights, float* 
   ld_::LoudParams p;
   int rc = loud_check("loudness_forward", B, N, n_frames, n_fft, hop, padding, &p);
   if (rc || B == 0 || n_frames == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("loudness_forward", loudness, extent(B, n_frames), audio, extent(B, N));
+  DDSP_REQUIRE_DISJOINT("loudness_forward", loudness, extent(B, n_frames), weights, extent(n_fft / 2 + 1));
   p.audio = audio; p.weights = weights;
   db_params(&p, range_db, ref_db);
   const int warps = ld_warps(n_fft);
@@ -241,6 +254,7 @@ int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n
   int pad_left = 0;
   int rc = framing_check("rms_power", B, N, n_frames, frame_size, hop, padding, &pad_left);
   if (rc || B == 0 || n_frames == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("rms_power", power_db, extent(B, n_frames), audio, extent(B, N));
   ld_::LoudParams d;
   db_params(&d, range_db, ref_db);
   const int64_t total = (int64_t)B * n_frames;
@@ -264,6 +278,7 @@ int ddsp_b200_crepe_frames(const float* audio, float* frames, int B, int N, int 
   int rc = framing_check("crepe_frames", B > 0, N, n_frames, crepe_::kFrame, hop, padding,
                          &pad_left);
   if (rc || B == 0 || n_frames == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("crepe_frames", frames, extent(B, n_frames, crepe_::kFrame), audio, extent(B, N));
   const int64_t total = (int64_t)B * n_frames;
   const int threads = 32 * crepe_::kFrameWarps;
   crepe_::crepe_frames_kernel<<<grid_for(total * 32, threads, 16), threads, 0,
@@ -302,6 +317,8 @@ int ddsp_b200_crepe_decode(const float* activations, const int* centers, float* 
   DDSP_REQUIRE(M == 0 || (activations && f0 && confidence), DDSP_B200_E_INVALID,
                "crepe_decode: null pointer");
   if (M == 0) return 0;
+  DDSP_REQUIRE_DISJOINT("crepe_decode", f0, extent(M), activations, extent(M, DDSP_B200_CREPE_BINS));
+  DDSP_REQUIRE_DISJOINT("crepe_decode", confidence, extent(M), activations, extent(M, DDSP_B200_CREPE_BINS));
   const int threads = 32 * crepe_::kDecodeWarps;
   crepe_::crepe_decode_kernel<<<grid_for(M * 32, threads, 16), threads, 0,
                                 (cudaStream_t)stream>>>(activations, centers, f0,
@@ -392,6 +409,8 @@ int ddsp_b200_mel_forward(const float* audio, const float* window, const void* m
   int rc = mel_check("mel_forward", B, N, n_frames, fft_size, fft_length, hop, pad_end, bins,
                      n_out, mode, &p);
   if (rc || B == 0 || n_frames == 0 || n_out == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("mel_forward", out, extent(B, n_frames, n_out), audio, extent(B, N));
+  DDSP_REQUIRE_DISJOINT("mel_forward", out, extent(B, n_frames, n_out), window, extent(fft_size));
   mel_tables(&p, audio, window, mel_table, fft_length, bins);
   const int warps = mel_warps(p.M, bins, mode);
   const size_t fixed = mel_fixed_smem(p.M, warps, bins, mode);

@@ -37,6 +37,12 @@ int ddsp_b200_harmonic_controls(const float* amps_in, const float* hd_in,
   if (rows == 0) return 0;
   DDSP_REQUIRE(rows < (1ll << 31) / 32, DDSP_B200_E_INVALID,
                "harmonic_controls: B*F too large");
+  DDSP_REQUIRE_DISJOINT("harmonic_controls", amps_out, extent(B, F), hd_in, extent(B, F, K));
+  DDSP_REQUIRE_DISJOINT("harmonic_controls", amps_out, extent(B, F), f0_hz, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("harmonic_controls", hd_out, extent(B, F, K), amps_in, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("harmonic_controls", hd_out, extent(B, F, K), f0_hz, extent(B, F));
+  DDSP_REQUIRE_SAME_OR_DISJOINT("harmonic_controls", amps_out, extent(B, F), amps_in, extent(B, F));
+  DDSP_REQUIRE_SAME_OR_DISJOINT("harmonic_controls", hd_out, extent(B, F, K), hd_in, extent(B, F, K));
   const int threads = 256;
   const int blocks = (int)((rows * 32 + threads - 1) / threads);
   harmonic_controls_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(
@@ -73,6 +79,9 @@ int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
   DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
                "harmonic_forward: B=%d exceeds the 65535 grid limit", B);
 
+  DDSP_REQUIRE_DISJOINT("harmonic_forward", audio, extent(B, N), f0_hz, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("harmonic_forward", audio, extent(B, N), amps, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("harmonic_forward", audio, extent(B, N), hd, extent(B, F, K));
   HarmonicParams p = harm_params(f0_hz, amps, hd, audio, B, F, K, N, sample_rate,
                                  amp_method);
   p.accumulate = accumulate;
@@ -124,6 +133,14 @@ int ddsp_b200_streaming_harmonic_forward(const float* f0_hz, const float* amps,
   p.FT = fit_tile("streaming_harmonic_forward", std::max(1, std::min(F, 2048 / p.hop)),
                   K, p.Kp, harm_smem_bytes);
   if (!p.FT) return DDSP_B200_E_UNSUPPORTED;
+  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", audio, extent(B, N), f0_hz, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", audio, extent(B, N), amps, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", audio, extent(B, N), hd, extent(B, F, K));
+  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", audio, extent(B, N), initial_phase, extent(B));
+  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", final_phase, extent(B), f0_hz, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", final_phase, extent(B), amps, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", final_phase, extent(B), hd, extent(B, F, K));
+  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", final_phase, extent(B), initial_phase, extent(B));
   const size_t smem = harm_smem_bytes(p.FT, p.Kp);
   rc = set_smem(harmonic_generic_kernel<0>, smem, "streaming_harmonic_forward");
   if (rc) return rc;
@@ -139,6 +156,7 @@ int ddsp_b200_noise_controls(const float* mag_in, float* mag_out, int64_t n,
                "noise_controls: null pointer");
   DDSP_REQUIRE(n >= 0, DDSP_B200_E_INVALID, "noise_controls: n < 0");
   if (n == 0) return 0;
+  DDSP_REQUIRE_SAME_OR_DISJOINT("noise_controls", mag_out, extent(n), mag_in, extent(n));
   noise_controls_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(
       mag_in, mag_out, n, initial_bias, apply_scale);
   DDSP_CHECK_LAUNCH("noise_controls");

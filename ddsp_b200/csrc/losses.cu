@@ -46,6 +46,9 @@ int ddsp_b200_mixture_nll_forward(const float* x, const float* mu, const float* 
   int64_t rows = 0;
   int rc = mix_check("mixture_nll_forward", B, T, Q, J, scale, &p, &rows);
   if (rc || rows == 0 || Q == 0 || J == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("mixture_nll_forward", nll, extent(rows, Q), x, extent(rows, Q));
+  DDSP_REQUIRE_DISJOINT("mixture_nll_forward", nll, extent(rows, Q), mu, extent(rows, J));
+  DDSP_REQUIRE_DISJOINT("mixture_nll_forward", nll, extent(rows, Q), lw, extent(rows, J));
   p.x = x; p.mu = mu; p.lw = lw;
   const size_t smem = sizeof(float) * 2 * (size_t)J;
   rc = set_smem(cons_::mixture_nll_kernel, smem, "mixture_nll_forward");
@@ -122,6 +125,9 @@ int ddsp_b200_comb_nll_forward(const float* f0, const float* f, const float* a, 
   int64_t rows = 0;
   int rc = comb_check("comb_nll_forward", B, T, C, P, G, scale, &p, &rows);
   if (rc || rows == 0 || C == 0 || P == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("comb_nll_forward", out, extent(rows, C), f0, extent(rows, C));
+  DDSP_REQUIRE_DISJOINT("comb_nll_forward", out, extent(rows, C), f, extent(rows, P));
+  DDSP_REQUIRE_DISJOINT("comb_nll_forward", out, extent(rows, C), a, extent(rows, P));
   p.f0 = f0; p.f = f; p.a = a;
   const size_t smem = sizeof(float) * (2 * (size_t)P + C + 1);
   rc = set_smem(cons_::comb_nll_kernel, smem, "comb_nll_forward");
@@ -187,6 +193,12 @@ int ddsp_b200_sinusoidal_to_harmonic(const float* sin_amps, const float* sin_fre
   int rc = s2h_check("sinusoidal_to_harmonic", B, T, S, K, width, sample_rate, normalize, &p,
                      &rows);
   if (rc || rows == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_amp, extent(rows), sin_amps, extent(rows, S));
+  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_amp, extent(rows), sin_freqs, extent(rows, S));
+  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_amp, extent(rows), f0_hz, extent(rows));
+  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_dist, extent(rows, K), sin_amps, extent(rows, S));
+  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_dist, extent(rows, K), sin_freqs, extent(rows, S));
+  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_dist, extent(rows, K), f0_hz, extent(rows));
   p.a = sin_amps; p.f = sin_freqs; p.f0 = f0_hz;
   const size_t smem = sizeof(float) * (2 * (size_t)S + cons_::kThreads + 1);
   rc = set_smem(cons_::sin_to_harm_kernel, smem, "sinusoidal_to_harmonic");
@@ -260,6 +272,9 @@ int ddsp_b200_hmm_log_prob(const float* obs, const float* loc, const float* scal
   hmm_::Params p;
   int rc = hmm_check("hmm_log_prob", obs, loc, scale, B, T, K, hold, other, &p);
   if (rc || B == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("hmm_log_prob", log_prob, extent(B), obs, extent(B, T, 2));
+  DDSP_REQUIRE_DISJOINT("hmm_log_prob", log_prob, extent(B), loc, extent(K, 2));
+  DDSP_REQUIRE_DISJOINT("hmm_log_prob", log_prob, extent(B), scale, extent(K, 2));
   hmm_::hmm_log_prob_kernel<<<(unsigned)B, hmm_threads(K), 0, (cudaStream_t)stream>>>(
       p, log_prob);
   DDSP_CHECK_LAUNCH("hmm_log_prob");
@@ -345,6 +360,10 @@ int ddsp_b200_wasserstein_forward(const float* u, const float* v, const float* w
   ws_::Params wp;
   int rc = ws_check("wasserstein_forward", R, Nu, Nv, p, &wp);
   if (rc || empty) return rc;
+  DDSP_REQUIRE_DISJOINT("wasserstein_forward", out, extent(R), u, extent(R, Nu));
+  DDSP_REQUIRE_DISJOINT("wasserstein_forward", out, extent(R), v, extent(R, Nv));
+  DDSP_REQUIRE_DISJOINT("wasserstein_forward", out, extent(R), wu, extent(R, Nu));
+  DDSP_REQUIRE_DISJOINT("wasserstein_forward", out, extent(R), wv, extent(R, Nv));
   wp.u = u; wp.v = v; wp.wu = wu; wp.wv = wv;
   const int m = ws_::padded(Nu + Nv);
   const size_t smem = ws_::smem_bytes(m);
@@ -399,6 +418,8 @@ int ddsp_b200_note_mask(const float* q, const float* onset, float* mask, void* w
                "note_mask: workspace of %zu B is smaller than the %zu B needed",
                workspace_bytes, need);
   if (empty) return 0;
+  DDSP_REQUIRE_DISJOINT("note_mask", mask, extent(B, onset || T > 1 ? T : 2, R), q, extent(B, T));
+  DDSP_REQUIRE_DISJOINT("note_mask", mask, extent(B, onset || T > 1 ? T : 2, R), onset, extent(B, T));
   notes_::MaskParams p;
   p.q = q;
   p.onset = onset;
@@ -457,6 +478,16 @@ int ddsp_b200_note_moments(const float* x, const float* mask, float* mean, float
   rc = notes_grid("note_moments", B, T, &pt, &grid_t);
   if (rc) return rc;
   if (B == 0 || D == 0) return 0;
+  DDSP_REQUIRE_DISJOINT("note_moments", mean, extent(B, N, D), x, extent(B, T, D));
+  DDSP_REQUIRE_DISJOINT("note_moments", mean, extent(B, N, D), mask, extent(B, T, N));
+  DDSP_REQUIRE(!overlaps(stdev, sizeof(float) * extent(B, N, D), x, sizeof(float) * extent(B, T, D)),
+               DDSP_B200_E_INVALID, "note_moments: std must not overlap x");
+  DDSP_REQUIRE(!overlaps(stdev, sizeof(float) * extent(B, N, D), mask, sizeof(float) * extent(B, T, N)),
+               DDSP_B200_E_INVALID, "note_moments: std must not overlap mask");
+  DDSP_REQUIRE_DISJOINT("note_moments", pooled_mean, extent(B, T, D), x, extent(B, T, D));
+  DDSP_REQUIRE_DISJOINT("note_moments", pooled_mean, extent(B, T, D), mask, extent(B, T, N));
+  DDSP_REQUIRE_DISJOINT("note_moments", pooled_std, extent(B, T, D), x, extent(B, T, D));
+  DDSP_REQUIRE_DISJOINT("note_moments", pooled_std, extent(B, T, D), mask, extent(B, T, N));
   if (N == 0) {   // nothing to pool: the pooled sums are zero
     const size_t bytes = sizeof(float) * (size_t)B * T * D;
     if (pooled_mean)

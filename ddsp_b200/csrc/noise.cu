@@ -32,6 +32,7 @@ int ddsp_b200_frequency_impulse_response(const float* mags, float* ir,
   const size_t smem = sizeof(float) * ((size_t)g.S0 + (size_t)kIrFrames * nb);
   DDSP_REQUIRE(smem <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
                "frequency_impulse_response: n_frequencies=%d too large", nb);
+  DDSP_REQUIRE_DISJOINT("frequency_impulse_response", ir, extent(BF, g.S), mags, extent(BF, nb));
   int rc = set_smem(ir_kernel, smem, "frequency_impulse_response");
   if (rc) return rc;
   const int64_t blocks = (BF + kIrFrames - 1) / kIrFrames;
@@ -74,6 +75,8 @@ int ddsp_b200_fir_time_varying(const float* audio, const float* ir, float* out,
   DDSP_REQUIRE(smem <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
                "fir_time_varying: impulse response of %d taps is beyond the "
                "shared-memory FIR (long-IR convolution is not built yet)", S);
+  DDSP_REQUIRE_DISJOINT("fir_time_varying", out, extent(B, out_len), audio, extent(B, N));
+  DDSP_REQUIRE_DISJOINT("fir_time_varying", out, extent(B, out_len), ir, extent(ir_batch, F, S));
   int rc = set_smem(fir_kernel, smem, "fir_time_varying");
   if (rc) return rc;
   dim3 grid((out_len + kFirThreads - 1) / kFirThreads, B);
@@ -121,6 +124,8 @@ int ddsp_b200_filtered_noise_forward(const float* mags, const float* noise,
   if (B == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (noise_fused_supported(F, nb, N, window_size)) {
+    DDSP_REQUIRE_DISJOINT("filtered_noise_forward", audio, extent(B, N), mags, extent(B, F, nb));
+    DDSP_REQUIRE_DISJOINT("filtered_noise_forward", audio, extent(B, N), noise, extent(B, N));
     return launch_noise_best(mags, noise, seed, offset, audio, B, F, nb, N,
                              window_size, accumulate, st);
   }
@@ -129,6 +134,8 @@ int ddsp_b200_filtered_noise_forward(const float* mags, const float* noise,
                DDSP_B200_E_WORKSPACE,
                "filtered_noise_forward: workspace of %zu B needed, %zu given",
                need, workspace_bytes);
+  DDSP_REQUIRE_DISJOINT("filtered_noise_forward", audio, extent(B, N), mags, extent(B, F, nb));
+  DDSP_REQUIRE_DISJOINT("filtered_noise_forward", audio, extent(B, N), noise, extent(B, N));
   IrGeom g = make_ir_geom(nb, window_size);
   float* ir = align256<float>(workspace);
   float* nz = ir + (size_t)B * F * g.S;
@@ -173,6 +180,11 @@ static int decoder_forward_impl(const float* amps_raw, const float* hd_raw,
                DDSP_B200_E_UNSUPPORTED,
                "decoder_forward: shape outside the fused decoder path "
                "(needs hop %% 64 == 0, n_frequencies <= %d)", kNfMaxNb);
+  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), amps_raw, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), hd_raw, extent(B, F, K));
+  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), f0_hz, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), mags_raw, extent(B, F, nb));
+  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), noise, extent(B, N));
   cudaStream_t st = (cudaStream_t)stream;
   rc = launch_harmonic_v4(p, st);
   if (rc == 1) {

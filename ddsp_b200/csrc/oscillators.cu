@@ -36,6 +36,10 @@ int ddsp_b200_oscillator_bank(const float* frequency_envelopes,
   DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
                "oscillator_bank: workspace of %zu B needed, %zu given", need,
                workspace_bytes);
+  DDSP_REQUIRE_DISJOINT("oscillator_bank", out, extent(B, N, sum_sinusoids ? 1 : K), frequency_envelopes,
+                        extent(B, N, K));
+  DDSP_REQUIRE_DISJOINT("oscillator_bank", out, extent(B, N, sum_sinusoids ? 1 : K), amplitude_envelopes,
+                        extent(B, N, K));
   unsigned long long* sums = align256<unsigned long long>(workspace);
   const int n_chunks = (N + kObChunk - 1) / kObChunk;
   const double inv_sr = 1.0 / (double)sample_rate;
@@ -101,6 +105,7 @@ int ddsp_b200_angular_cumsum(const float* angular_frequency, float* phase, int B
   if (B == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (mode != 0) {
+    DDSP_REQUIRE_DISJOINT("angular_cumsum", phase, extent(B, N, C), angular_frequency, extent(B, N, C));
     const int64_t BC = (int64_t)B * C;
     tf_sequential_cumsum<<<(int)((BC + 127) / 128), 128, 0, st>>>(
         angular_frequency, nullptr, phase, B, N, C, mode, chunk_size, 0, 1.0f);
@@ -113,6 +118,7 @@ int ddsp_b200_angular_cumsum(const float* angular_frequency, float* phase, int B
   DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
                "angular_cumsum: workspace of %zu B needed, %zu given", need,
                workspace_bytes);
+  DDSP_REQUIRE_DISJOINT("angular_cumsum", phase, extent(B, N, C), angular_frequency, extent(B, N, C));
   unsigned long long* sums = align256<unsigned long long>(workspace);
   const int n_chunks = (N + kObChunk - 1) / kObChunk;
   const double inv_two_pi = 0.15915494309189535;
@@ -156,6 +162,10 @@ int ddsp_b200_oscillator_bank_tf_sequential(const float* frequency_envelopes,
                "oscillator_bank_tf_sequential: null pointer");
   DDSP_REQUIRE(B >= 0 && N >= 1 && K >= 1 && chunk_size >= 1 && sample_rate > 0.f,
                DDSP_B200_E_INVALID, "oscillator_bank_tf_sequential: bad arguments");
+  DDSP_REQUIRE_DISJOINT("oscillator_bank_tf_sequential", out, extent(B, N, K), frequency_envelopes,
+                        extent(B, N, K));
+  DDSP_REQUIRE_DISJOINT("oscillator_bank_tf_sequential", out, extent(B, N, K), amplitude_envelopes,
+                        extent(B, N, K));
   if (B == 0) return 0;
   const int64_t BK = (int64_t)B * K;
   tf_sequential_cumsum<<<(int)((BK + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
@@ -231,6 +241,8 @@ int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitud
   int rc = sinus_check("sinusoidal_forward", B, F, K, N, sample_rate, amp_method, workspace,
                        workspace_bytes, ddsp_b200_sinusoidal_workspace(B, F, K));
   if (rc || B == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("sinusoidal_forward", audio, extent(B, N), frequencies, extent(B, F, K));
+  DDSP_REQUIRE_DISJOINT("sinusoidal_forward", audio, extent(B, N), amplitudes, extent(B, F, K));
   const int FT = sinus_tile_frames(F, K);
   const SfSmem L = sf_smem(FT, K);
   unsigned long long* sums = align256<unsigned long long>(workspace);
@@ -377,6 +389,9 @@ int ddsp_b200_wavetable_forward(const float* f0_hz, const float* amplitudes,
   int rc = wt_check("wavetable_forward", B, F, N, Fw, W, sample_rate, amp_method, workspace,
                     workspace_bytes, ddsp_b200_wavetable_workspace(B, F));
   if (rc || B == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("wavetable_forward", audio, extent(B, N), f0_hz, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("wavetable_forward", audio, extent(B, N), amplitudes, extent(B, F));
+  DDSP_REQUIRE_DISJOINT("wavetable_forward", audio, extent(B, N), wavetables, extent(B, Fw, W));
   cudaStream_t st = (cudaStream_t)stream;
   const int hop = N / F;
   const WtPhase w = wt_phase_layout(workspace, B, F);
@@ -472,6 +487,12 @@ int ddsp_b200_harmonic_oscillator_bank(const float* frequency,
   if (rc || B == 0) return rc;
   DDSP_REQUIRE(frequency && amplitude_envelopes && audio, DDSP_B200_E_INVALID,
                "harmonic_oscillator_bank: null pointer");
+  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", audio, extent(B, N), frequency, extent(B, N));
+  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", audio, extent(B, N), amplitude_envelopes, extent(B, N, K));
+  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", audio, extent(B, N), initial_phase, extent(B));
+  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", final_phase, extent(B), frequency, extent(B, N));
+  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", final_phase, extent(B), amplitude_envelopes, extent(B, N, K));
+  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", final_phase, extent(B), initial_phase, extent(B));
   hob_::hob_forward<<<dim3(B, hob_::n_spans(N)), hob_::kThreads, 0, (cudaStream_t)stream>>>(
       frequency, amplitude_envelopes, initial_phase, audio, final_phase, N, K,
       1.0 / (double)sample_rate, use_angular_cumsum ? 0 : 1);
@@ -520,6 +541,8 @@ int ddsp_b200_linear_lookup_forward(const float* phase, const float* wavetables,
                "linear_lookup_forward: null pointer");
   int rc = ll_check("linear_lookup_forward", B, N, W, per_sample);
   if (rc || B == 0) return rc;
+  DDSP_REQUIRE_DISJOINT("linear_lookup_forward", out, extent(B, N), phase, extent(B, N));
+  DDSP_REQUIRE_DISJOINT("linear_lookup_forward", out, extent(B, N), wavetables, extent(B, per_sample ? N : 1, W));
   auto kern = per_sample ? ll_::ll_samples<true, false> : ll_::ll_samples<false, false>;
   const int64_t rows = (int64_t)B * N;
   kern<<<(unsigned)((rows + ll_::kThreads - 1) / ll_::kThreads), ll_::kThreads, 0,

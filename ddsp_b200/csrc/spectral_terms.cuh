@@ -234,10 +234,6 @@ Kernel pick(int terms, bool l2) {
   return nullptr;
 }
 
-inline bool overlaps(const void* a, const void* b, size_t bytes) {
-  return (uintptr_t)a < (uintptr_t)b + bytes && (uintptr_t)b < (uintptr_t)a + bytes;
-}
-
 // Frames per CTA for F bins, and the shared memory it stages.
 inline int tile_rows(int T, int F) { return std::max(1, std::min(T, kTileBins / F)); }
 inline size_t tile_smem(int rows, int F, int terms) {

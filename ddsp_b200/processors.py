@@ -155,6 +155,10 @@ class ProcessorGroup(dags.DAGLayer):
       except NotImplementedError:
         pass   # outside the fused regime: per-processor path below
     audio = harm.get_signal(**harm.get_controls(*h_in, **kwargs))
+    # the noise is added into the harmonic buffer through out=, which autograd does
+    # not differentiate: a harmonic signal that carries a graph is refused here, with
+    # the way to train, rather than by the out= check below
+    core._no_grad_path('ProcessorGroup', audio)
     return noise.get_signal(out=audio, accumulate=True, offset=offset,
                             **noise.get_controls(*n_in, **kwargs))
 

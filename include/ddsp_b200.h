@@ -19,6 +19,10 @@
  *     thread-local).
  *   - Return value: 0 = ok, negative = DDSP_B200_E_* below.  Shape/argument
  *     errors are detected BEFORE any launch.
+ *   - Aliasing: each forward entry point says which outputs may BE which inputs (the
+ *     same pointer and extent) or may overlap them at all; every other overlap of a
+ *     float output with a float input, partial ones included, is E_INVALID, after the
+ *     other argument checks and before any launch.
  *   - The *_workspace, *_workspace_bytes, *_takes and ddsp_b200_ir_size queries
  *     are pure host functions: they launch nothing and set no error.
  *
@@ -80,7 +84,8 @@ uint64_t ddsp_b200_launch_count(void);
 /* Harmonic.get_controls (synths.py:94-121): exp_sigmoid (core.py:386-404) on
  * amplitudes and harmonic_distribution, Nyquist mask + row normalisation
  * (core.normalize_harmonics, core.py:894-907; safe_divide core.py:207-210).
- * amps_in/out [B,F,1]; hd_in/out [B,F,K]; f0_hz [B,F,1]. In-place is allowed. */
+ * amps_in/out [B,F,1]; hd_in/out [B,F,K]; f0_hz [B,F,1].  amps_out may be amps_in
+ * and hd_out may be hd_in (in place); neither may overlap another input. */
 int ddsp_b200_harmonic_controls(const float* amps_in, const float* hd_in,
                                 const float* f0_hz, float* amps_out,
                                 float* hd_out, int B, int F, int K,
@@ -91,7 +96,8 @@ int ddsp_b200_harmonic_controls(const float* amps_in, const float* hd_in,
  * of f0*k (573-642), resample amp*hd by amp_method (645-714), oscillator_bank
  * (911-962) incl. audio-rate remove_above_nyquist (869-891).
  * f0_hz [B,F,1], amps [B,F,1], hd [B,F,K] or NULL (K must be 1), audio [B,N].
- * N must be a multiple of F.  accumulate!=0: audio += result (fused Add).    */
+ * N must be a multiple of F.  accumulate!=0: audio += result (fused Add).
+ * audio must not overlap f0_hz, amps or hd. */
 int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
                                const float* hd, float* audio, int B, int F,
                                int K, int N, float sample_rate, int amp_method,
@@ -104,20 +110,22 @@ int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
  * sample is returned (wrapped cumsum in [0, 2 pi) + initial_phase, as
  * angular_cumsum gives).  hd must already be normalize_harmonics'ed
  * (ddsp_b200_harmonic_controls with DDSP_B200_CTL_NYQUIST only).
- * initial_phase [B] radians or NULL; final_phase [B] or NULL. */
+ * initial_phase [B] radians or NULL; final_phase [B] or NULL.  Neither audio nor
+ * final_phase may overlap an input. */
 int ddsp_b200_streaming_harmonic_forward(const float* f0_hz, const float* amps,
                                          const float* hd, const float* initial_phase,
                                          float* audio, float* final_phase, int B,
                                          int F, int K, int N, float sample_rate,
                                          int amp_method, void* stream);
 
-/* FilteredNoise.get_controls (synths.py:165-179): exp_sigmoid(x + bias). */
+/* FilteredNoise.get_controls (synths.py:165-179): exp_sigmoid(x + bias).  mag_out
+ * may be mag_in (in place). */
 int ddsp_b200_noise_controls(const float* mag_in, float* mag_out, int64_t n,
                              float initial_bias, int apply_scale, void* stream);
 
 /* core.frequency_impulse_response + apply_window_to_impulse_response
  * (core.py:1534-1565, 1477-1531).  mags [BF, nb] -> ir [BF, S] with
- * S = ddsp_b200_ir_size(nb, window_size). */
+ * S = ddsp_b200_ir_size(nb, window_size).  ir must not overlap mags. */
 int ddsp_b200_ir_size(int nb, int window_size);
 int ddsp_b200_frequency_impulse_response(const float* mags, float* ir,
                                          int64_t BF, int nb, int window_size,
@@ -128,7 +136,7 @@ int ddsp_b200_frequency_impulse_response(const float* mags, float* ir,
  * crop_and_compensate_delay folded into index math).  audio [B,N]; ir
  * [ir_batch(1 or B), F, S]; out [B, N] ('same') or [B, N+S-1] ('valid').
  * delay_compensation < 0 -> (S-1)/2 - 1 as in the reference.
- * accumulate!=0: out += result. */
+ * accumulate!=0: out += result.  out must not overlap audio or ir. */
 int ddsp_b200_fir_time_varying(const float* audio, const float* ir, float* out,
                                int B, int N, int F, int S, int ir_batch,
                                int padding, int delay_compensation,
@@ -144,7 +152,8 @@ int ddsp_b200_uniform_noise(float* out, int B, int N, uint64_t seed,
  * mags [B,F,nb]; noise [B,N] or NULL (NULL: in-kernel Philox(seed, offset));
  * audio [B,N].  accumulate!=0: audio += result (the fused processors.Add,
  * processors.py:174-176).  workspace: ddsp_b200_filtered_noise_workspace()
- * bytes (0 for the fused path; may be NULL then). */
+ * bytes (0 for the fused path; may be NULL then).  audio must not overlap mags or
+ * noise. */
 size_t ddsp_b200_filtered_noise_workspace(int B, int F, int nb, int N,
                                           int window_size);
 int ddsp_b200_filtered_noise_forward(const float* mags, const float* noise,
@@ -162,7 +171,8 @@ int ddsp_b200_filtered_noise_forward(const float* mags, const float* noise,
  * into the harmonic audio (processors.py:174-176).  harmonic_flags:
  * DDSP_B200_CTL_SCALE | DDSP_B200_CTL_NYQUIST as in harmonic_controls.
  * Returns DDSP_B200_E_UNSUPPORTED outside the decoder regime (hop % 64 == 0,
- * n_frequencies <= 80); callers then use the per-processor entry points. */
+ * n_frequencies <= 80); callers then use the per-processor entry points.
+ * audio must not overlap an input. */
 int ddsp_b200_decoder_forward(const float* amps_raw, const float* hd_raw,
                               const float* f0_hz, const float* mags_raw,
                               const float* noise, uint64_t seed, uint64_t offset,
@@ -313,7 +323,8 @@ int ddsp_b200_frequency_filter_backward(const float* audio, const float* ir,
 
 /* core.sinc_impulse_response (core.py:1576-1625): cutoff [BF] -> ir [BF, S] for
  * S = 2 (window_size / 2) + 1 taps (odd).  The cutoff is multiplied by `scale` in
- * float32 first (1, or float32(2 / sample_rate)); high_pass != 0 gives delta - h. */
+ * float32 first (1, or float32(2 / sample_rate)); high_pass != 0 gives delta - h.
+ * ir must not overlap cutoff. */
 int ddsp_b200_sinc_impulse_response(const float* cutoff, float* ir, int64_t BF, int S,
                                     float scale, int high_pass, void* stream);
 /* Its backward: d_ir [BF, S] -> d_cutoff [BF] (the gradient of the unscaled cutoff). */
@@ -326,7 +337,7 @@ int ddsp_b200_sinc_impulse_response_backward(const float* cutoff, const float* d
  * delay compensation, taps built in shared memory and never stored.  out [B, N] for
  * 'same', [B, N+S-1] for 'valid'; accumulate != 0: out += result.  The reference's
  * errors for batch, frames and padding; E_UNSUPPORTED for S < 3 (an empty crop) and
- * S >= 2048. */
+ * S >= 2048.  out must not overlap audio or cutoff. */
 int ddsp_b200_sinc_filter(const float* audio, const float* cutoff, float* out, int B, int N,
                           int F, int S, int cutoff_batch, float scale, int high_pass,
                           int padding, int accumulate, void* stream);
@@ -346,7 +357,8 @@ int ddsp_b200_sinc_filter_backward(const float* audio, const float* cutoff, cons
 /* core.oscillator_bank (core.py:911-962) on audio-rate envelopes [B,N,K]:
  * Nyquist mask, exact wrapped phase accumulation (three-pass chunked scan in
  * 64-bit fixed point), amp * sin(phase), summed over k when sum_sinusoids != 0
- * (out [B,N]) or not (out [B,N,K]).  workspace: *_workspace(B,N,K) bytes. */
+ * (out [B,N]) or not (out [B,N,K]).  workspace: *_workspace(B,N,K) bytes.
+ * out must not overlap either envelope. */
 size_t ddsp_b200_oscillator_bank_workspace(int B, int N, int K);
 int ddsp_b200_oscillator_bank(const float* frequency_envelopes,
                               const float* amplitude_envelopes, float* out, int B,
@@ -381,7 +393,9 @@ int ddsp_b200_oscillator_bank_backward(const float* frequency_envelopes,
  * ddsp_b200_fft_convolve_lti_workspace(B, N, S, ir_batch) bytes.
  * flags: DDSP_B200_LTI_REVERSE_AUDIO / _IR read that operand back to front - the
  * backward pass is the same convolution on time-reversed signals:
- *   d audio = (g * reverse(ir)) [S-1-start, +N),  d ir = (g * reverse(audio)) [N-1-start, +S). */
+ *   d audio = (g * reverse(ir)) [S-1-start, +N),  d ir = (g * reverse(audio)) [N-1-start, +S).
+ * out may overlap audio or impulse_response in any way: both are transformed into the
+ * workspace by launches that end before out is written. */
 enum { DDSP_B200_LTI_REVERSE_AUDIO = 1, DDSP_B200_LTI_REVERSE_IR = 2 };
 size_t ddsp_b200_fft_convolve_lti_workspace(int B, int N, int S, int ir_batch);
 int ddsp_b200_fft_convolve_lti(const float* audio, const float* impulse_response,
@@ -398,9 +412,11 @@ int ddsp_b200_fft_convolve_lti(const float* audio, const float* impulse_response
  *   2  tf_sequential, angular_cumsum: float32, chunked by chunk_size with the
  *      reference's mod-2pi stitching (debug mode: reproduces TensorFlow's own
  *      float32 error, one thread per (b, c) - small shapes).
+ * phase must not overlap angular_frequency.
  * ddsp_b200_oscillator_bank_tf_sequential is core.oscillator_bank evaluated that
  * way end to end (omega = f * 2pi / sr in float32, modes 1 / 2, Nyquist mask,
- * amp * sin(phase)); out is [B,N,K], the sum over k is left to the caller. */
+ * amp * sin(phase)); out is [B,N,K], the sum over k is left to the caller.  Its out
+ * must not overlap either envelope. */
 int ddsp_b200_angular_cumsum(const float* angular_frequency, float* phase, int B,
                              int N, int C, int chunk_size, int mode,
                              void* workspace, size_t workspace_bytes, void* stream);
@@ -424,7 +440,7 @@ int ddsp_b200_oscillator_bank_tf_sequential(const float* frequency_envelopes,
  * NULL) is phi after the last sample: with use_angular_cumsum != 0 the wrapped sum in
  * [0, 2 pi) plus initial_phase, else the unwrapped sum (accumulated exactly, rounded once)
  * plus initial_phase.  The audio does not depend on use_angular_cumsum.  B = 0 is a no-op.
- * No workspace. */
+ * No workspace.  Neither audio nor final_phase may overlap an input. */
 int ddsp_b200_harmonic_oscillator_bank(const float* frequency,
                                        const float* amplitude_envelopes,
                                        const float* initial_phase, float* audio,
@@ -456,7 +472,8 @@ int ddsp_b200_harmonic_oscillator_bank_backward(
  * core.harmonic_synthesis with harmonic_shifts (core.py:1084-1111; the caller
  * forms f0 * k * (1 + shifts) and amp * hd at frame rate, as the reference does).
  * frequencies, amplitudes [B,F,K] -> audio [B,N] (summed over k), N % F == 0.
- * workspace: ddsp_b200_sinusoidal_workspace(B,F,K) bytes. */
+ * workspace: ddsp_b200_sinusoidal_workspace(B,F,K) bytes.  audio must not overlap
+ * frequencies or amplitudes. */
 size_t ddsp_b200_sinusoidal_workspace(int B, int F, int K);
 int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitudes,
                                  float* audio, int B, int F, int K, int N,
@@ -483,7 +500,8 @@ int ddsp_b200_sinusoidal_backward(const float* frequencies, const float* amplitu
  * in [B,F,C] -> out [B,N,C].  method: 0 'window', 1 'linear', 2 'nearest',
  * 3 'cubic' (tf.compat.v1 bicubic, Keys A = -0.75).  add_endpoint as in the
  * reference.  4-D inputs [B,F,n_freq,C] are the 3-D case with n_freq*C channels
- * (the reference resizes the n_freq axis to itself, core.py:616-621). */
+ * (the reference resizes the n_freq axis to itself, core.py:616-621).  out must not
+ * overlap in. */
 int ddsp_b200_resample(const float* in, float* out, int B, int F, int C, int N,
                        int method, int add_endpoint, void* stream);
 
@@ -502,7 +520,9 @@ int ddsp_b200_resample(const float* in, float* out, int B, int F, int C, int N,
  * irfft_size = 2 (n_bins - 1): it is pre-scaled so that irfft(grad_value,
  * irfft_size) is the gradient w.r.t. the real frames (the transpose of rfft);
  * irfft_size = -1: the same for an UNNORMALISED inverse transform (no 1/n pass).
- * sums must be zeroed by the caller. */
+ * sums must be zeroed by the caller.  frames must not overlap audio or window;
+ * grad_audio must not overlap grad_frames, window or *scale_device; spectral_l1's
+ * grad_value may be stft_value (in place) and must not overlap stft_target. */
 int ddsp_b200_frame_window(const float* audio, const float* window, float* frames,
                            int B, int N, int n_frames, int frame_size, int frame_step,
                            void* stream);
@@ -525,7 +545,8 @@ int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
  * an unnormalised inverse transform (spectral_l1's irfft_size = -1).  The terms of
  * m = |X|: mag m, delta_time core.diff(m, axis=1), delta_freq core.diff(m, axis=2),
  * cumsum_freq cumsum(m, axis=2), logmag safe_log(m).  grad_value may be
- * stft_value unless delta_time is active, when it must overlap neither STFT.
+ * stft_value or stft_target (in place) unless delta_time is active, when it must
+ * overlap neither STFT.
  * F > DDSP_B200_SPECTRAL_TERMS_MAX_BINS (fft_size 8192) is E_UNSUPPORTED. */
 enum {
   DDSP_B200_TERM_MAG = 1,
@@ -542,7 +563,7 @@ int ddsp_b200_spectral_terms(const float* stft_target, const float* stft_value,
                              float delta_freq_weight, float cumsum_freq_weight,
                              float logmag_weight, void* stream);
 
-/* processors.Add.get_signal (processors.py:174-176). out may alias a or b. */
+/* processors.Add.get_signal (processors.py:174-176).  out may be a or b (in place). */
 int ddsp_b200_add(const float* a, const float* b, float* out, int64_t n,
                   void* stream);
 
@@ -556,7 +577,7 @@ int ddsp_b200_add(const float* a, const float* b, float* out, int64_t n,
  *   v_j = 0 for j < 0 or j > max_length.
  * audio, phase, out: [B, N]; gain: [B, N] or NULL (= 1).  core.variable_length_delay
  * is scale = 1, offset = 0, gain = NULL, add_dry = 0.  1 <= max_length < 2^29.
- * out must not alias audio.
+ * out must not overlap audio; it may be phase or gain.
  *
  * backward: for the upstream gradient grad_out [B, N], writes any of
  *   grad_audio [B, N]  (d out / d audio, dry path included),
@@ -586,7 +607,8 @@ int ddsp_b200_resample_backward(const float* grad_out, float* grad_in, int B, in
  * backward: writes any of grad_signal_one, grad_signal_two [B,N,C] and
  * grad_mix_level [B,N,1] (summed over C in channel order); NULL outputs are not
  * computed.  grad_mix_level is NaN where m is exactly 0 or 1, as the reference's
- * autodiff gives it (0 * inf). */
+ * autodiff gives it (0 * inf).  The forward's out may be signal_one, signal_two or,
+ * with C = 1, mix_level (in place); with C > 1 it must not overlap mix_level. */
 int ddsp_b200_mix_forward(const float* signal_one, const float* signal_two,
                           const float* mix_level, float* out, int B, int N, int C,
                           void* stream);
@@ -604,7 +626,7 @@ int ddsp_b200_mix_backward(const float* signal_one, const float* signal_two,
  *   grad_gain[r]  = sum_t grad_ir e n,
  *   grad_decay[r] = -exp(decay[r]) gain[r] sum_t grad_ir time e n
  * (NULL outputs are not computed); the noise is regenerated, the sums are in double
- * in a fixed order. */
+ * in a fixed order.  The forward's ir must not overlap gain, decay or noise. */
 int ddsp_b200_exp_decay_ir(const float* gain, const float* decay, const float* noise,
                            uint64_t seed, uint64_t offset, float* ir, int rows, int L,
                            void* stream);
@@ -626,7 +648,8 @@ int ddsp_b200_exp_decay_ir_backward(const float* gain, const float* decay,
  * d_wavetables [B,Fw,W]; a NULL output is not computed.  d_f0 follows TensorFlow's
  * subgradients: 0 where pos is an integer.  Table entries no sample reads are 0.
  * No atomics: the gradients are bit-reproducible.
- * workspace: ddsp_b200_wavetable_backward_workspace(B,F,N,Fw,W) bytes. */
+ * workspace: ddsp_b200_wavetable_backward_workspace(B,F,N,Fw,W) bytes.
+ * The forward's audio must not overlap f0_hz, amplitudes or wavetables. */
 size_t ddsp_b200_wavetable_workspace(int B, int F);
 int ddsp_b200_wavetable_forward(const float* f0_hz, const float* amplitudes,
                                 const float* wavetables, float* audio, int B, int F,
@@ -647,7 +670,8 @@ int ddsp_b200_wavetable_backward(const float* f0_hz, const float* amplitudes,
  * wrapped.  W <= DDSP_B200_LOOKUP_MAX_W (more is E_UNSUPPORTED).
  * The backward writes d_phase [B,N] (TensorFlow's subgradients: 0 on a grid point of a
  * power-of-two W) and d_wavetables (the table's shape); a NULL output is not computed.
- * No atomics and no workspace: bit-reproducible. */
+ * No atomics and no workspace: bit-reproducible.  The forward's out must not overlap
+ * phase or wavetables. */
 enum { DDSP_B200_LOOKUP_MAX_W = 4194304 /* the four candidate columns stay exact */ };
 int ddsp_b200_linear_lookup_forward(const float* phase, const float* wavetables, float* out,
                                     int B, int N, int W, int per_sample, void* stream);
@@ -664,7 +688,8 @@ int ddsp_b200_linear_lookup_backward(const float* phase, const float* wavetables
  * ceil(N/hop) for SAME).  n_fft is a power of two, hop <= n_fft unless VALID;
  * n_fft > 16384 is E_UNSUPPORTED.  B <= 65535.
  * backward: grad_audio [B,N] for grad_loudness [B,T], with tf.maximum's tie rule (no
- * gradient through an active clamp).  No atomics: bit-reproducible. */
+ * gradient through an active clamp).  No atomics: bit-reproducible.  The forward's
+ * loudness must not overlap audio or weights. */
 int ddsp_b200_loudness_forward(const float* audio, const float* weights, float* loudness,
                                int B, int N, int n_frames, int n_fft, int hop, int padding,
                                float range_db, float ref_db, void* stream);
@@ -675,7 +700,8 @@ int ddsp_b200_loudness_backward(const float* audio, const float* weights,
 /* spectral_ops.compute_power (spectral_ops.py:223-249): power_db[b,t] =
  * power_to_db(mean(frame^2)) with frames of any frame_size every hop, padded as above
  * (CENTER pads frame_size/2 zeros on both sides).  in_db == 0 writes
- * compute_rms_energy's mean(frame^2)^0.5 instead.  Forward only. */
+ * compute_rms_energy's mean(frame^2)^0.5 instead.  Forward only.
+ * power_db must not overlap audio. */
 int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n_frames,
                         int frame_size, int hop, int padding, int in_db, float range_db,
                         float ref_db, void* stream);
@@ -702,7 +728,9 @@ int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n
  *   the float32 cents linspace(0, 7180, 360) + 1997.3794084376191 over bins
  *   centre - 4 .. centre + 5, each clamped into 0 .. 359.  The centre is the row's first
  *   argmax, or centers[m] (int32, any value) when centers is not null.  Weights summing
- *   to 0 give NaN (0 / 0), as in the reference.  M >= 0; M = 0 launches nothing. */
+ *   to 0 give NaN (0 / 0), as in the reference.  M >= 0; M = 0 launches nothing.
+ * crepe_frames' frames must not overlap audio; crepe_decode's f0 and confidence must
+ * not overlap activations. */
 enum { DDSP_B200_CREPE_BINS = 360, DDSP_B200_CREPE_FRAME = 1024 };
 int ddsp_b200_crepe_frames(const float* audio, float* frames, int B, int N, int n_frames,
                            int hop, int padding, void* stream);
@@ -730,7 +758,8 @@ enum { DDSP_B200_MEL = 0, DDSP_B200_LOGMEL = 1, DDSP_B200_MFCC = 2 };
  * outside 2..16384 and bins > 1024 are E_UNSUPPORTED.  B <= 65535.  B = 0, n_frames = 0
  * and n_out = 0 return before any launch (backward: grad_audio is then not written).
  * backward: grad_audio [B,N] for grad_out [B,T,C], TensorFlow's gradient (no gradient
- * through mel <= 0 in the log, none through |X_k| = 0).  No atomics: bit-reproducible. */
+ * through mel <= 0 in the log, none through |X_k| = 0).  No atomics: bit-reproducible.
+ * The forward's out must not overlap audio or window. */
 int ddsp_b200_mel_forward(const float* audio, const float* window, const void* mel_table,
                           float* out, int B, int N, int n_frames, int fft_size, int fft_length,
                           int hop, int pad_end, int bins, int n_out, int mode, void* stream);
@@ -756,7 +785,8 @@ enum { DDSP_B200_MAX_ROWS = 2147483647, DDSP_B200_CONSISTENCY_MAX_STAGED = 4096 
  * backward: for g [B,T,Q], with responsibilities r_qj and z_qj = (x_q - mu_j) / scale,
  *   dx = g_q / scale sum_j r_qj z_qj, dmu = -1/scale sum_q g_q r_qj z_qj,
  *   dlw = -sum_q g_q r_qj;
- * every sum in a fixed order, no atomics: bit-reproducible. */
+ * every sum in a fixed order, no atomics: bit-reproducible.  The forward's nll must not
+ * overlap x, mu or lw. */
 int ddsp_b200_mixture_nll_forward(const float* x, const float* mu, const float* lw,
                                   float* nll, int B, int T, int Q, int J, float scale,
                                   void* stream);
@@ -776,7 +806,7 @@ int ddsp_b200_mixture_nll_backward(const float* x, const float* mu, const float*
  * return before any launch and write nothing; the pointers may then be null.
  * backward: d_f0 [B,T,C], d_f and d_a [B,T,P] for g [B,T,C]; no gradient through a
  * safe_divide denominator that was 0 (d_f0 = 0 at f0 = 0).  Fixed-order sums, no
- * atomics: bit-reproducible. */
+ * atomics: bit-reproducible.  The forward's out must not overlap f0, f or a. */
 int ddsp_b200_comb_nll_forward(const float* f0, const float* f, const float* a, float* out,
                                int B, int T, int C, int P, int G, float scale, void* stream);
 int ddsp_b200_comb_nll_backward(const float* f0, const float* f, const float* a,
@@ -802,7 +832,8 @@ int ddsp_b200_comb_nll_backward(const float* f0, const float* f, const float* a,
  * S = 0).  TensorFlow's gradient: none through a safe_divide denominator that took its
  * 1e-7 (f0 = 0, harm_amp = 0), sign(0) = 0 in |q|, none to the branch of normalize's
  * where that was not taken, none through harmonics at or above Nyquist.  Every sum in a
- * fixed order, no atomics: bit-reproducible. */
+ * fixed order, no atomics: bit-reproducible.  The forward's harm_amp and harm_dist must
+ * not overlap an input. */
 int ddsp_b200_sinusoidal_to_harmonic(const float* sin_amps, const float* sin_freqs,
                                      const float* f0_hz, float* harm_amp, float* harm_dist,
                                      int B, int T, int S, int K, float width,
@@ -830,7 +861,8 @@ int ddsp_b200_sinusoidal_to_harmonic_backward(
  *     1 for T >= 1 steps of K >= 1 states within that bound, else 0.
  * All three take B >= 0, T >= 1, 2 <= K <= DDSP_B200_HMM_MAX_STATES (more is
  * E_UNSUPPORTED), hold and other finite, non-negative and not both 0.  B = 0 returns
- * after the checks without a launch (the pointers may then be null). */
+ * after the checks without a launch (the pointers may then be null).  hmm_log_prob's
+ * log_prob must not overlap obs, loc or scale. */
 enum {
   DDSP_B200_HMM_MAX_STATES = 1024,      /* one CTA runs the states, a thread each      */
   DDSP_B200_HMM_SEGMENT_FLOATS = 49152, /* the backward's segment buffer (192 KiB)     */
@@ -865,7 +897,7 @@ int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale
  *   dwu_k = sum_{i: s_i >= u_k} g_i,  dwv_k = -sum_{i: s_i >= v_k} g_i.
  * An exact U_i = V_i at p < 1, or S = 0 at p > 1, gives NaN (0 * inf) as autograd does;
  * at p = 1 everything finite stays finite.  Fixed-order scans and sums, no atomics:
- * bit-reproducible. */
+ * bit-reproducible.  The forward's out must not overlap u, v, wu or wv. */
 enum { DDSP_B200_WASSERSTEIN_MAX_SIDE = 4096 /* values per side one CTA sorts */ };
 int ddsp_b200_wasserstein_forward(const float* u, const float* v, const float* wu,
                                   const float* wv, float* out, int64_t R, int Nu, int Nv,
@@ -907,7 +939,7 @@ int ddsp_b200_wasserstein_backward(const float* u, const float* v, const float* 
  * Both moment entry points take B >= 0, T >= 1, N, D >= 0 and at most 2^31 - 1 CTAs (B
  * times the tiles of 32 notes or frames by 64 dims); B = 0 or D = 0 returns after the
  * checks without a launch.  All three: no atomics, fixed summation orders,
- * bit-reproducible. */
+ * bit-reproducible.  No output of note_mask or note_moments may overlap an input. */
 int ddsp_b200_note_mask(const float* q, const float* onset, float* mask, void* workspace,
                         size_t workspace_bytes, int B, int T, int R, int note_on_only,
                         void* stream);
