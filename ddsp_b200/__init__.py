@@ -8,6 +8,7 @@ from ddsp_b200 import _lib
 from ddsp_b200 import core
 from ddsp_b200 import dags
 from ddsp_b200 import effects
+from ddsp_b200 import heuristics
 from ddsp_b200 import host
 from ddsp_b200 import nn
 from ddsp_b200 import preprocessing

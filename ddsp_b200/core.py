@@ -5,6 +5,7 @@ cited per function); the arithmetic happens in libddsp_b200.so (hand-written
 sm_90a kernels) through the ctypes C ABI in `_lib.py`.  torch is plumbing:
 device memory and streams.  There is no CPU fallback.
 """
+import ctypes
 import functools
 import math
 from collections import abc
@@ -522,6 +523,42 @@ def note_mask(q, onset, max_regions, note_on_only):
   _launch('ddsp_b200_note_mask', q, onset, mask, *_workspace(nbytes, q.device),
           b, t, max_regions, flag)
   return mask
+
+
+def note_heuristic(x, f0, on, status, stages, log_values, shift, pool_width, pool_pad,
+                   positive, num_devs, widths, strided_pad, min_samples, glue_back):
+  """The launch behind the binarizers of ddsp_b200.heuristics: (mask [B, T] bool, status
+  [B] int32) of the contiguous [B, T] CUDA operands x (float32 amplitudes or power), f0
+  (float32 Hz) and on (uint8), any of them None where the stages do not read it.  status
+  may be a preallocated int32 [B]; nothing is synchronised."""
+  like = next(v for v in (x, f0, on) if v is not None)
+  b, t = like.shape
+  mask = torch.empty((b, t), dtype=torch.bool, device=like.device)
+  if status is None:
+    status = torch.empty((b,), dtype=torch.int32, device=like.device)
+  host_widths = (ctypes.c_int * max(1, len(widths)))(*widths)   # read before the launch
+  _launch('ddsp_b200_note_heuristic', x, f0, on, mask, status,
+          *_workspace('ddsp_b200_note_heuristic_workspace_bytes', like.device, b, t),
+          b, t, stages, log_values, shift, pool_width, pool_pad, positive, num_devs,
+          ctypes.addressof(host_widths), len(widths), strided_pad, min_samples, glue_back)
+  return mask, status
+
+
+def note_table_buffer(b, t, device):
+  """One int32 buffer and its views (buffer, status [B], count [B], note records
+  [B, (T+1)//2, 4]), so that a whole batch comes to the host in one copy; the records
+  start 16-byte aligned."""
+  cap = (t + 1) // 2
+  head = (2 * b + 3) // 4 * 4
+  buf = torch.empty((head + b * cap * 4,), dtype=torch.int32, device=device)
+  return buf, buf[:b], buf[b:2 * b], buf[head:].view(b, cap, 4)
+
+
+def note_segments(mask, f0, notes, count, median):
+  """The launch behind heuristics.note_table: the records {start, stop, pitch, f0 bits}
+  of the runs of nonzero bytes of mask [B, T] into notes [B, (T+1)//2, 4] and count [B]."""
+  b, t = f0.shape
+  _launch('ddsp_b200_note_segments', mask, f0, notes, count, b, t, int(bool(median)))
 
 
 def safe_divide(numerator, denominator, eps=1e-7):

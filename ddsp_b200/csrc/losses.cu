@@ -1,8 +1,9 @@
 // C ABI of the loss family: the consistency mixture and comb NLLs,
 // sinusoidal_to_harmonic, the HMM, the Wasserstein distance and the note functions of
-// the MIDI autoencoder, forward and backward.
+// the MIDI autoencoder, forward and backward, and its controls-to-notes heuristics.
 #include "capi.cuh"
 #include "consistency.cuh"
+#include "heuristics.cuh"
 #include "hmm.cuh"
 #include "notes.cuh"
 #include "wasserstein.cuh"
@@ -576,6 +577,149 @@ int ddsp_b200_note_moments_backward(const float* x, const float* mask, const flo
     notes_::note_over_n_kernel<notes_::kDxMean><<<grid_t, notes_::kThreads, 0,
                                                   (cudaStream_t)stream>>>(pt, o, dx, nullptr);
   DDSP_CHECK_LAUNCH("note_moments_backward");
+  return 0;
+}
+
+// ---- heuristics: binarizers and the note table ------------------------------------------
+// The workspace of note_heuristic: per item, the pooled values and MIDI pitches (floats),
+// T + 1 counts and T transition bytes, each region 256-byte aligned.
+static size_t heur_region(int B, int64_t per_item, size_t elem) {
+  return ((size_t)B * (size_t)per_item * elem + 255) & ~(size_t)255;
+}
+
+size_t ddsp_b200_note_heuristic_workspace_bytes(int B, int T) {
+  if (B <= 0 || T <= 0) return 0;
+  return 256 + 2 * heur_region(B, T, sizeof(float)) + heur_region(B, (int64_t)T + 1, sizeof(int)) +
+         heur_region(B, T, 1);
+}
+
+int ddsp_b200_note_heuristic_takes(int T) {
+  return T >= 1 && T <= DDSP_B200_NOTE_HEURISTIC_MAX_T;
+}
+
+static int heur_pad(const char* what, int pad) {
+  DDSP_REQUIRE(pad == DDSP_B200_HEURISTIC_PAD_FRONT || pad == DDSP_B200_HEURISTIC_PAD_CENTER ||
+                   pad == DDSP_B200_HEURISTIC_PAD_END,
+               DDSP_B200_E_INVALID, "note_heuristic: unrecognized %s pad mode %d", what, pad);
+  return 0;
+}
+
+int ddsp_b200_note_heuristic(const float* x, const float* f0, const unsigned char* on,
+                             unsigned char* mask, int* status, void* workspace,
+                             size_t workspace_bytes, int B, int T, int stages, int log_values,
+                             float shift, int pool_width, int pool_pad, int pool_positive,
+                             double num_devs, const int* widths, int n_widths,
+                             int strided_pad, int min_samples, int glue_back, void* stream) {
+  DDSP_REQUIRE(B >= 0 && T >= 1, DDSP_B200_E_INVALID, "note_heuristic: bad shape B=%d T=%d",
+               B, T);
+  DDSP_REQUIRE(ddsp_b200_note_heuristic_takes(T), DDSP_B200_E_UNSUPPORTED,
+               "note_heuristic: T=%d frames exceed the %d supported", T,
+               DDSP_B200_NOTE_HEURISTIC_MAX_T);
+  DDSP_REQUIRE(stages >= 0 && stages <= 15, DDSP_B200_E_INVALID,
+               "note_heuristic: bad stage mask %d", stages);
+  const bool pool = stages & heur_::kPool, strided = stages & heur_::kStrided;
+  const bool uses_f0 = stages & (heur_::kStrided | heur_::kF0Pos);
+  DDSP_REQUIRE(B == 0 || ((!pool || x) && (!uses_f0 || f0) && (pool || strided || on) &&
+                          mask && status),
+               DDSP_B200_E_INVALID, "note_heuristic: null pointer");
+  if (pool) {
+    DDSP_REQUIRE(pool_width >= 1, DDSP_B200_E_INVALID,
+                 "note_heuristic: frame_width must be at least 1, got %d", pool_width);
+    DDSP_REQUIRE(num_devs == num_devs, DDSP_B200_E_INVALID, "note_heuristic: num_devs is NaN");
+    int rc = heur_pad("pooled", pool_pad);
+    if (rc) return rc;
+  }
+  if (strided) {
+    DDSP_REQUIRE(n_widths >= 0 && n_widths <= DDSP_B200_HEURISTIC_MAX_WIDTHS &&
+                     (n_widths == 0 || widths),
+                 DDSP_B200_E_INVALID, "note_heuristic: %d frame widths, at most %d", n_widths,
+                 DDSP_B200_HEURISTIC_MAX_WIDTHS);
+    for (int i = 0; i < n_widths; ++i)
+      DDSP_REQUIRE(widths[i] >= 1, DDSP_B200_E_INVALID,
+                   "note_heuristic: frame widths must be at least 1, got %d", widths[i]);
+    int rc = heur_pad("strided", strided_pad);
+    if (rc) return rc;
+  }
+  const size_t need = ddsp_b200_note_heuristic_workspace_bytes(B, T);
+  DDSP_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), DDSP_B200_E_WORKSPACE,
+               "note_heuristic: workspace of %zu B is smaller than the %zu B needed",
+               workspace_bytes, need);
+  if (B == 0) return 0;
+  const size_t mb = (size_t)B * T;
+  DDSP_REQUIRE(!overlaps(mask, mb, x, pool ? mb * 4 : 0) &&
+                   !overlaps(mask, mb, f0, uses_f0 ? mb * 4 : 0) &&
+                   !overlaps(status, 4 * (size_t)B, x, pool ? mb * 4 : 0) &&
+                   !overlaps(status, 4 * (size_t)B, f0, uses_f0 ? mb * 4 : 0) &&
+                   !overlaps(status, 4 * (size_t)B, on, pool || strided ? 0 : mb) &&
+                   !overlaps(status, 4 * (size_t)B, mask, mb),
+               DDSP_B200_E_INVALID, "note_heuristic: mask and status must not overlap the "
+               "inputs or each other");
+  DDSP_REQUIRE((const void*)mask == (const void*)on || !overlaps(mask, mb, on, pool || strided ? 0 : mb),
+               DDSP_B200_E_INVALID, "note_heuristic: mask must be on or not overlap it");
+  heur_::Params p;
+  p.x = x;
+  p.f0 = f0;
+  p.on = on;
+  p.mask = mask;
+  p.status = status;
+  char* ws = align256<char>(workspace);
+  p.val = reinterpret_cast<float*>(ws);
+  ws += heur_region(B, T, sizeof(float));
+  p.midi = reinterpret_cast<float*>(ws);
+  ws += heur_region(B, T, sizeof(float));
+  p.cnt = reinterpret_cast<int*>(ws);
+  ws += heur_region(B, (int64_t)T + 1, sizeof(int));
+  p.tr = reinterpret_cast<uint8_t*>(ws);
+  p.T = T;
+  p.stages = stages;
+  p.log_values = log_values != 0;
+  p.shift = shift;
+  p.pool_width = pool_width;
+  p.pool_pad = pool_pad;
+  p.pool_positive = pool_positive != 0;
+  p.num_devs = num_devs;
+  p.n_widths = strided ? n_widths : 0;
+  for (int i = 0; i < heur_::kMaxWidths; ++i) p.widths[i] = i < p.n_widths ? widths[i] : 1;
+  p.strided_pad = strided_pad;
+  p.min_samples = min_samples;
+  p.glue_back = glue_back != 0;
+  heur_::note_heuristic_kernel<<<(unsigned)B, heur_::kMaskThreads, 0, (cudaStream_t)stream>>>(p);
+  DDSP_CHECK_LAUNCH("note_heuristic");
+  return 0;
+}
+
+int ddsp_b200_note_segments(const unsigned char* mask, const float* f0, ddsp_b200_note* notes,
+                            int* count, int B, int T, int median, void* stream) {
+  DDSP_REQUIRE(B >= 0 && T >= 1, DDSP_B200_E_INVALID, "note_segments: bad shape B=%d T=%d",
+               B, T);
+  DDSP_REQUIRE(ddsp_b200_note_heuristic_takes(T), DDSP_B200_E_UNSUPPORTED,
+               "note_segments: T=%d frames exceed the %d supported", T,
+               DDSP_B200_NOTE_HEURISTIC_MAX_T);
+  DDSP_REQUIRE(median == 0 || median == 1, DDSP_B200_E_INVALID,
+               "note_segments: median must be 0 or 1, got %d", median);
+  DDSP_REQUIRE(B == 0 || (mask && f0 && notes && count), DDSP_B200_E_INVALID,
+               "note_segments: null pointer");
+  DDSP_REQUIRE((uintptr_t)notes % 16 == 0, DDSP_B200_E_INVALID,
+               "note_segments: notes must be 16-byte aligned");
+  if (B == 0) return 0;
+  const int cap = (T + 1) / 2;
+  const size_t mb = (size_t)B * T, nb = (size_t)B * cap * sizeof(ddsp_b200_note);
+  DDSP_REQUIRE(!overlaps(notes, nb, mask, mb) && !overlaps(notes, nb, f0, 4 * mb) &&
+                   !overlaps(count, 4 * (size_t)B, mask, mb) &&
+                   !overlaps(count, 4 * (size_t)B, f0, 4 * mb) &&
+                   !overlaps(count, 4 * (size_t)B, notes, nb),
+               DDSP_B200_E_INVALID, "note_segments: notes and count must not overlap the "
+               "inputs or each other");
+  heur_::SegParams p;
+  p.mask = mask;
+  p.f0 = f0;
+  p.notes = reinterpret_cast<int4*>(notes);
+  p.count = count;
+  p.T = T;
+  p.cap = cap;
+  p.median = median;
+  heur_::note_segments_kernel<<<(unsigned)B, heur_::kMaskThreads, 0, (cudaStream_t)stream>>>(p);
+  DDSP_CHECK_LAUNCH("note_segments");
   return 0;
 }
 

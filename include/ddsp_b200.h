@@ -953,6 +953,69 @@ int ddsp_b200_note_moments_backward(const float* x, const float* mask, const flo
                                     size_t workspace_bytes, int B, int T, int N, int D,
                                     void* stream);
 
+/* training/heuristics.py, DDSP controls to notes.
+ * ddsp_b200_note_heuristic: the binary mask [B,T] (one byte per frame, 0 or 1) of one or
+ *   more of heuristics.py's binarizers, one CTA per item.  stages is a bit mask:
+ *   DDSP_B200_HEURISTIC_POOL: pooled outliers of v = log(x) (log_values, amplitudes) or
+ *     v = x + shift in float32 (power): frame t is on iff mean(w) - num_devs std(w) < v_t
+ *     for its window w of pool_width padded values (population std), decided in double
+ *     on deviations from v_t; a window with a non-finite value is off; with
+ *     pool_positive also v_t > 0.
+ *   DDSP_B200_HEURISTIC_STRIDED: strided_freq_change's transitions for the n_widths
+ *     widths in `widths` (HOST memory, read before the launch), in order, on the float32
+ *     hz_to_midi(f0); a frame is turned off where the padded window of the transitions
+ *     before this width is all on and |midi(first) - midi(last)| > 0.75.
+ *   DDSP_B200_HEURISTIC_F0_POSITIVE: and f0 > 0.
+ *   With neither POOL nor STRIDED the mask starts from `on` [B,T] (nonzero bytes are on;
+ *   mask may be on), else from the AND of the two.
+ *   DDSP_B200_HEURISTIC_REMOVE_SHORT: then remove_short(min_samples, glue_back): a run of
+ *     on frames that an off frame ends is cleared when shorter than min_samples; with
+ *     glue_back an off frame is set on instead when the run before the next off frame is
+ *     shorter than min_samples.
+ *   Pads (DDSP_B200_HEURISTIC_PAD_*) repeat the edge values truncated toward zero; front
+ *   pads width - 1 frames before, center width / 2 before and the rest after, end
+ *   width - 1 after.  status [B]: 0, or DDSP_B200_HEURISTIC_POOL_EDGE /
+ *   DDSP_B200_HEURISTIC_PITCH_EDGE where a padded vector has a non-finite first or last
+ *   value (the reference raises); that item's mask row is all 0.  workspace:
+ *   ddsp_b200_note_heuristic_workspace_bytes(B, T) bytes (E_WORKSPACE if smaller).
+ * ddsp_b200_note_segments: the note table of the runs of nonzero bytes of mask [B,T]:
+ *   notes [B, (T+1)/2] records (16-byte aligned), the first count[b] of them the notes in
+ *   order and the rest zero.  f0 is the run's mean of f0 (summed in double, rounded once
+ *   to float) or, with median, np.median's (the middle value, or the float32 mean of the
+ *   two middle values; NaN when the run holds a NaN).  pitch is round-half-even of the
+ *   float32 hz_to_midi(f0), -2^31 for a non-finite value.
+ * Both take B >= 0 and 1 <= T <= DDSP_B200_NOTE_HEURISTIC_MAX_T
+ * (ddsp_b200_note_heuristic_takes(T); more is E_UNSUPPORTED); B = 0 returns after the
+ * checks.  No output may overlap an input (except mask on), no atomics, bit-reproducible. */
+enum {
+  DDSP_B200_HEURISTIC_POOL = 1,
+  DDSP_B200_HEURISTIC_STRIDED = 2,
+  DDSP_B200_HEURISTIC_F0_POSITIVE = 4,
+  DDSP_B200_HEURISTIC_REMOVE_SHORT = 8,
+  DDSP_B200_HEURISTIC_PAD_FRONT = 0,
+  DDSP_B200_HEURISTIC_PAD_CENTER = 1,
+  DDSP_B200_HEURISTIC_PAD_END = 2,
+  DDSP_B200_HEURISTIC_POOL_EDGE = 1,
+  DDSP_B200_HEURISTIC_PITCH_EDGE = 2,
+  DDSP_B200_HEURISTIC_MAX_WIDTHS = 8,
+  DDSP_B200_NOTE_HEURISTIC_MAX_T = 268435456 /* 2^28 frames: int counts and positions */
+};
+typedef struct {
+  int start, stop; /* frames [start, stop) */
+  int pitch;
+  float f0;
+} ddsp_b200_note;
+size_t ddsp_b200_note_heuristic_workspace_bytes(int B, int T);
+int ddsp_b200_note_heuristic_takes(int T);
+int ddsp_b200_note_heuristic(const float* x, const float* f0, const unsigned char* on,
+                             unsigned char* mask, int* status, void* workspace,
+                             size_t workspace_bytes, int B, int T, int stages, int log_values,
+                             float shift, int pool_width, int pool_pad, int pool_positive,
+                             double num_devs, const int* widths, int n_widths,
+                             int strided_pad, int min_samples, int glue_back, void* stream);
+int ddsp_b200_note_segments(const unsigned char* mask, const float* f0, ddsp_b200_note* notes,
+                            int* count, int B, int T, int median, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
