@@ -5,12 +5,14 @@ Drop-in for the signal-generation layer of magenta/ddsp: `Processor`,
 backed by hand-written CUDA kernels behind a ctypes C ABI (include/ddsp_b200.h).
 """
 from ddsp_b200 import _lib
+from ddsp_b200 import colab_utils
 from ddsp_b200 import core
 from ddsp_b200 import dags
 from ddsp_b200 import effects
 from ddsp_b200 import heuristics
 from ddsp_b200 import host
 from ddsp_b200 import nn
+from ddsp_b200 import postprocessing
 from ddsp_b200 import preprocessing
 from ddsp_b200 import processors
 from ddsp_b200 import synths

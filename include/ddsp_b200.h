@@ -1016,6 +1016,70 @@ int ddsp_b200_note_heuristic(const float* x, const float* f0, const unsigned cha
 int ddsp_b200_note_segments(const unsigned char* mask, const float* f0, ddsp_b200_note* notes,
                             int* count, int B, int T, int median, void* stream);
 
+/* training/postprocessing.py and colab_utils.get_tuning_factor / auto_tune: adjusting
+ * controls for tone transfer.  Every input is float64 (float32 values widened exactly);
+ * flags make the kernels round the reference's float32 steps to float32, so that the
+ * caller's cast of a result back to float32 is exact.  Forward only, no atomics,
+ * bit-reproducible.  No output may overlap an input or another output.
+ * ddsp_b200_detect_notes: [B,T] (n = B T) in two launches.  smooth's box filter of
+ *   conf ** exponent (numpy's fast paths for 2, 0.5, 1, -1, 0; in float32 with
+ *   DETECT_CONF_F32), converted to float32, over `smoothing` taps of float32(1 / k) with
+ *   TF 'SAME' zero padding ((k-1)/2 taps left), summed in float32 tap by tap.  ratio =
+ *   smoothed (loudness - min_db) / ((mean - min_db) weight), the mean over all n frames
+ *   summed in double over a partition fixed by n; in float32 with DETECT_LOUD_F32.
+ *   mask = ratio >= note_threshold.  DETECT_SMOOTH_ONLY writes the smoothed input into
+ *   ratio (loudness and mask may be NULL).  workspace:
+ *   ddsp_b200_detect_notes_workspace_bytes(n) bytes (E_WORKSPACE if smaller).
+ * ddsp_b200_quantile_fit: np.nanpercentile(col, 100 q) then np.maximum.accumulate, for
+ *   each of F columns of `sorted` [F, n_rows] (ascending, NaN last; counts[f] non-NaN
+ *   values, 0 gives NaN), into quantiles [nq, F]: numpy 2.3's linear method, b - a in
+ *   float32 with QUANTILE_F32.
+ * ddsp_b200_quantile_transform: QuantileTransformer._transform_col of every column of
+ *   x [n, F] into out [n, F], forward or inverse, QUANTILE_UNIFORM or QUANTILE_NORMAL,
+ *   with np.interp's rules on the column's quantiles [nq, F] and references [nq]
+ *   (1 <= nq <= DDSP_B200_QUANTILE_MAX_N).  The 'normal' forward output is clipped to
+ *   [ppf(1e-7 - eps), ppf(1 - (1e-7 - eps))], computed on the device.  QUANTILE_F32: x is a float32 column (the forward result is
+ *   rounded to float32 before the bounds, and scipy's float32 ppf).
+ * ddsp_b200_tuning_factor: get_tuning_factor on the N masked frames f0 [N] and conf [N]
+ *   for n_factors <= DDSP_B200_TUNING_MAX_FACTORS factors: costs [2, n_factors] (the
+ *   mean weighted distance, the mean weighted note change) and index [1], np.argmin of
+ *   their normalised sum, in two launches.
+ * ddsp_b200_auto_tune: out [T] = f0 - amount midi_diff.  chromatic: midi_diff =
+ *   (f0 - tuning_factor) % 1, less 1 above 0.5 (in float32 with AUTO_TUNE_F32); else
+ *   the major scale s with the least mean distance of the N masked frames f0_on to its
+ *   nearest note (scale_cost [12], scale_index [1]), and each frame's difference to its
+ *   nearest note of scale s. */
+enum {
+  DDSP_B200_DETECT_SMOOTH_ONLY = 1,
+  DDSP_B200_DETECT_CONF_F32 = 2,
+  DDSP_B200_DETECT_LOUD_F32 = 4,
+  DDSP_B200_QUANTILE_F32 = 1,
+  DDSP_B200_QUANTILE_UNIFORM = 0,
+  DDSP_B200_QUANTILE_NORMAL = 1,
+  DDSP_B200_QUANTILE_MAX_N = 8192,  /* quantiles and references of a column in shared memory */
+  DDSP_B200_TUNING_MAX_FACTORS = 128,
+  DDSP_B200_SCALE_NOTES = 70,
+  DDSP_B200_AUTO_TUNE_F32 = 1
+};
+size_t ddsp_b200_detect_notes_workspace_bytes(int64_t n);
+int ddsp_b200_detect_notes(const double* loudness, const double* conf, double* ratio,
+                           unsigned char* mask, void* workspace, size_t workspace_bytes, int B,
+                           int T, int smoothing, double exponent, double weight, double min_db,
+                           double note_threshold, int flags, void* stream);
+int ddsp_b200_quantile_fit(const double* sorted, const int64_t* counts, const double* q,
+                           double* quantiles, int64_t n_rows, int F, int nq, int flags,
+                           void* stream);
+int ddsp_b200_quantile_transform(const double* x, const double* quantiles,
+                                 const double* references, double* out, int64_t n, int F,
+                                 int nq, int inverse, int distribution, int flags,
+                                 void* stream);
+int ddsp_b200_tuning_factor(const double* f0, const double* conf, const double* factors,
+                            double* costs, int* index, int64_t N, int n_factors, void* stream);
+int ddsp_b200_auto_tune(const double* f0, const double* f0_on, double* scale_cost,
+                        int* scale_index, double* out, int64_t T, int64_t N,
+                        double tuning_factor, double amount, int chromatic, int flags,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif
