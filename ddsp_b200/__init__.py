@@ -15,6 +15,7 @@ from ddsp_b200 import nn
 from ddsp_b200 import postprocessing
 from ddsp_b200 import preprocessing
 from ddsp_b200 import processors
+from ddsp_b200 import synthetic_data
 from ddsp_b200 import synths
 from ddsp_b200.effects import (ExpDecayReverb, FIRFilter, FilteredNoiseReverb,
                                ModDelay, Reverb)

@@ -1080,6 +1080,35 @@ int ddsp_b200_auto_tune(const double* f0, const double* f0_on, double* scale_cos
                         double tuning_factor, double amount, int chromatic, int flags,
                         void* stream);
 
+/* training/data_preparation/synthetic_data.py generate_notes_v2: InverseSynthesis's
+ * synthetic notes, drawn from numpy's legacy RandomState (MT19937) in the reference's
+ * order, as the reference's float64 arrays before its TF steps: harm_amp [B, T],
+ * harm_dist [B, T, K], f0_midi [B, T], mags [B, T, M], and (get_controls) the harm_amp
+ * divisor [B], drawn once per stream after all of its items.
+ *   Seeds mode (seeds [B] non-NULL, each in [0, 2^32)): item b is
+ *   np.random.seed(seeds[b]); generate_notes_v2(n_batch=1), one CTA per item, whatever B
+ *   and b; key, pos and gauss are ignored.
+ *   State mode (seeds NULL): generate_notes_v2(n_batch=B) continuing numpy's state, key
+ *   [624] words, pos [2] = (pos, has_gauss) and gauss [1] the cached Gaussian, all
+ *   device memory read before and written after the call; one CTA walks the items in
+ *   order and every item gets the one divisor.
+ * Elementary float64 steps round as numpy's do; cos, sin, pow and log are CUDA's (ulps),
+ * and every integer decision is the reference's.  B >= 0; 1 <= min_note_length <=
+ * max_note_length; T, K, M >= 1 and within ddsp_b200_synthetic_notes_takes(T, K, M)
+ * (T <= DDSP_B200_SYNTHETIC_MAX_T, K and M <= DDSP_B200_SYNTHETIC_MAX_BANDS; more is
+ * E_UNSUPPORTED).  No output may overlap an input or another output.  No atomics,
+ * bit-reproducible. */
+enum {
+  DDSP_B200_SYNTHETIC_MAX_T = 8192,     /* a note's blend in shared memory */
+  DDSP_B200_SYNTHETIC_MAX_BANDS = 4096  /* a note's two distributions in shared memory */
+};
+int ddsp_b200_synthetic_notes_takes(int T, int K, int M);
+int ddsp_b200_synthetic_notes(const int64_t* seeds, unsigned int* key, int* pos, double* gauss,
+                              double* harm_amp, double* harm_dist, double* f0_midi,
+                              double* mags, double* divisor, int B, int T, int K, int M,
+                              int min_note_length, int max_note_length, double p_silent,
+                              double p_vibrato, int get_controls, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
