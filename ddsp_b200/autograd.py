@@ -55,6 +55,8 @@ kernels, exposed as `torch.autograd.Function`s:
   * `HmmLogProbFn` - the HMM log-likelihood of `losses.HmmTranscriber`, with
     gradients to the observations (pitch and amplitude); routed to by
     `core.hmm_log_prob` under grad;
+  * `CrepeLossFramesFn` - the framing and per-frame normalisation of
+    `losses.PretrainedCREPE`, d audio, which the embedding losses train through;
   * `DecoderFn` / `decoder_train` - the whole `ae.gin` decoder from RAW network
     outputs: forward is the fused two-kernel pipeline (`get_controls` in shared
     memory), backward is the two synthesizer backward kernels plus the
@@ -932,6 +934,38 @@ class NoteMomentsFn(torch.autograd.Function):
     core._launch('ddsp_b200_note_moments_backward', x, mask, mean, std, gm, gs, gpm, gps, dx,
                  *core._workspace(nbytes, x.device), b, t, n, d)
     return dx, None, None, None
+
+
+class CrepeLossFramesFn(torch.autograd.Function):
+  """losses.PretrainedCREPE.frame_audio on audio [B, N] (a contiguous float32 CUDA
+  tensor): the frames [B, n_frames, 1024] of 1024 samples every `hop`, after 512 zeros
+  on both sides when `center`, each normalised to (x - mean) / (sqrt(var) + 1e-5)
+  (csrc/crepe.cuh).  Differentiable in the audio by one call of
+  `ddsp_b200_crepe_frames_backward`, which recomputes each frame's statistics: only
+  the audio is saved, not the frames.  A frame of variance 0 gives NaN gradients on the
+  samples it covers, as TensorFlow does."""
+
+  @staticmethod
+  def forward(ctx, audio, hop, center):
+    b, n = audio.shape
+    padding = (_lib.PAD_CENTER if center else _lib.PAD_VALID) | _lib.CREPE_LOSS_FRAMES
+    padded = n + (2 * (_lib.CREPE_FRAME // 2) if center else 0)
+    n_frames = 1 + (padded - _lib.CREPE_FRAME) // hop if padded >= _lib.CREPE_FRAME else 0
+    frames = torch.empty((b, n_frames, _lib.CREPE_FRAME), dtype=torch.float32,
+                         device=audio.device)
+    core._launch('ddsp_b200_crepe_frames', audio, frames, b, n, n_frames, hop, padding)
+    ctx.save_for_backward(audio)
+    ctx.cfg = (n_frames, hop, padding)
+    return frames
+
+  @staticmethod
+  def backward(ctx, grad_frames):
+    audio, = ctx.saved_tensors
+    b, n = audio.shape
+    d_audio = torch.empty_like(audio)
+    core._launch('ddsp_b200_crepe_frames_backward', audio,
+                 grad_frames.contiguous().to(torch.float32), d_audio, b, n, *ctx.cfg)
+    return d_audio, None, None
 
 
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):

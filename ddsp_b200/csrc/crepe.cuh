@@ -1,12 +1,32 @@
 // spectral_ops.PretrainedCREPE (spectral_ops.py:432-566) around its network: the frames
 // the network reads, the Viterbi path of create_hmm's 360-state HMM, and the
 // local-average f0 of activations_to_f0_and_confidence.  All three are forward only.
+// The frames of losses.PretrainedCREPE (losses.py:418-486), which the embedding losses
+// train through, also have a backward pass.
 //
 // Frames (crepe_frames_kernel).  One warp per frame of 1024 samples, 32 per lane, read
 // once into registers: samples outside the audio are pad's zeros.  Mean and population
 // variance about the mean (tf.nn.moments) are two passes in double, each lane summing
 // its samples in order and the lanes combined by an xor butterfly, so every lane holds
-// the same bits.  std = sqrt(var), or 1e-8 where var = 0; out = (x - mean) / std.
+// the same bits.  spectral_ops: std = sqrt(var), or 1e-8 where var = 0;
+// out = (x - mean) / std.  losses (kEps): out = (x - mean) / (sqrt(var) + 1e-5).
+//
+// Frames backward (losses' normalisation only).  Per frame, with mu, s = sqrt(var),
+// d = s + 1e-5, gbar = mean(g) and c = sum_j g_j (x_j - mu):
+//   dx_k = (g_k - gbar) / d - c (x_k - mu) / (d^2 1024 s),
+// the statistics in double as in the forward (tf.nn.moments stops the gradient of the
+// mean inside the variance; the term it would add sums to zero).  A frame of variance
+// 0 has c = 0 and s = 0: the second term is 0 / 0 = NaN on every sample the frame
+// covers, as TensorFlow's infinite derivative of var**0.5 at 0 times 0 gives.  Samples
+// no frame covers get 0.  No atomics: bit-reproducible.
+//   hop >= 1024 (crepe_frames_bwd_disjoint_kernel): no sample is in two frames.  One
+//     warp per frame computes its statistics and writes its samples, and zeroes the gap
+//     up to the next frame (the audio's end after the last).
+//   hop < 1024 (crepe_frames_bwd_overlap_kernel): a CTA owns kBwdOwn samples.  Its
+//     warps compute the statistics of every frame that covers one of them into shared
+//     memory, then each thread sums its sample's terms over those frames in increasing
+//     frame order, in double.  A frame on a span boundary has its statistics computed
+//     by both CTAs, with the same code and so the same bits.
 //
 // Viterbi (crepe_viterbi_kernel).  tfp's posterior_mode on create_hmm's model: uniform
 // initial distribution, transition w(i, j) / rs_i with w = max(12 - |i - j|, 1e-5) and
@@ -55,6 +75,10 @@ constexpr int kFromG = 2 * kBand + 1;            // the pointer code for "came f
 constexpr int kRecordWords = kWarps * kPlanes + 1;
 constexpr int kChunk = 64;                       // records staged per backtrack pass
 constexpr int kDecodeWarps = 8;
+constexpr double kLossEps = 1e-5;                // losses.PretrainedCREPE: std + 1e-5
+constexpr int kBwdOwn = 1024;                    // samples a CTA owns (hop < kFrame)
+constexpr int kBwdThreads = 256;
+constexpr int kDisjointWarps = 4;                // 12 warps per SM at its registers
 
 static_assert(kFrame % 32 == 0, "a lane reads kFrame / 32 samples");
 static_assert(kFromG < (1 << kPlanes), "pointer codes fit kPlanes bits");
@@ -67,7 +91,9 @@ __device__ __forceinline__ double warp_sum(double v) {
 }
 
 // frames [B * F, kFrame]: frame r = b F + f reads padded samples f hop .. f hop + 1023,
-// i.e. audio[b, f hop - pad_left + k] (zero outside 0 .. N - 1).
+// i.e. audio[b, f hop - pad_left + k] (zero outside 0 .. N - 1).  kEps: losses'
+// normalisation, by sqrt(var) + 1e-5.
+template <bool kEps>
 __global__ void __launch_bounds__(32 * kFrameWarps)
 crepe_frames_kernel(const float* __restrict__ audio, float* __restrict__ frames, int N,
                     int F, int64_t total, int hop, int pad_left) {
@@ -94,11 +120,127 @@ crepe_frames_kernel(const float* __restrict__ audio, float* __restrict__ frames,
       q = fma(d, d, q);
     }
     const double var = warp_sum(q) * (1.0 / kFrame);
-    const double inv = var > 0.0 ? 1.0 / sqrt(var) : 1e8;
+    const double inv = kEps ? 1.0 / (sqrt(var) + kLossEps) : var > 0.0 ? 1.0 / sqrt(var) : 1e8;
     float* out = frames + r * kFrame + lane;
 #pragma unroll
     for (int k = 0; k < kPerLane; ++k) out[32 * k] = (float)(((double)v[k] - mean) * inv);
   }
+}
+
+// ---- frames backward (losses' normalisation) ------------------------------------------
+__device__ __forceinline__ int64_t i64min(int64_t a, int64_t b) { return a < b ? a : b; }
+__device__ __forceinline__ int64_t i64max(int64_t a, int64_t b) { return a > b ? a : b; }
+
+// What a sample's gradient needs of one frame: dx = (g - gbar) inv - coef (x - mu).
+struct FrameGrad { double mu, inv, coef, gbar; };
+
+// The statistics of the frame of padded samples start .. start + 1023 of x [N] (zero
+// outside 0 .. N - 1), with upstream gradient g [1024]; every lane returns the same bits.
+// v and w receive the lane's samples and gradients (sample start + lane + 32 k).
+__device__ __forceinline__ FrameGrad frame_grad(const float* __restrict__ x,
+                                                const float* __restrict__ g, int N,
+                                                int64_t start, int lane, float (&v)[kPerLane],
+                                                float (&w)[kPerLane]) {
+  double s = 0.0, sg = 0.0;
+#pragma unroll
+  for (int k = 0; k < kPerLane; ++k) {
+    const int64_t i = start + lane + 32 * k;
+    v[k] = (i >= 0 && i < N) ? x[i] : 0.f;
+    w[k] = g[lane + 32 * k];
+    s += (double)v[k];
+    sg += (double)w[k];
+  }
+  const double mu = warp_sum(s) * (1.0 / kFrame);
+  double q = 0.0, c = 0.0;
+#pragma unroll
+  for (int k = 0; k < kPerLane; ++k) {
+    const double d = (double)v[k] - mu;
+    q = fma(d, d, q);
+    c = fma((double)w[k], d, c);
+  }
+  const double sd = sqrt(warp_sum(q) * (1.0 / kFrame));
+  c = warp_sum(c);
+  const double inv = 1.0 / (sd + kLossEps);
+  // c = 0 and sd = 0 on a frame of variance 0: NaN, as TensorFlow's gradient
+  return FrameGrad{mu, inv, c * inv * inv / ((double)kFrame * sd), warp_sum(sg) * (1.0 / kFrame)};
+}
+
+__device__ __forceinline__ double frame_term(const FrameGrad& s, float g, float x) {
+  return ((double)g - s.gbar) * s.inv - s.coef * ((double)x - s.mu);
+}
+
+// hop >= kFrame: warp r = b F + f writes frame f's samples of grad_audio [B, N], and
+// zeroes the samples after it up to frame f + 1's first (or N).
+__global__ void __launch_bounds__(32 * kDisjointWarps)
+crepe_frames_bwd_disjoint_kernel(const float* __restrict__ audio,
+                                 const float* __restrict__ grad_frames,
+                                 float* __restrict__ grad_audio, int N, int F, int64_t total,
+                                 int hop, int pad_left) {
+  const int lane = threadIdx.x & 31;
+  const int64_t stride = (int64_t)gridDim.x * kDisjointWarps;
+  for (int64_t r = (int64_t)blockIdx.x * kDisjointWarps + (threadIdx.x >> 5); r < total;
+       r += stride) {
+    const int64_t b = r / F, f = r - b * F;
+    const float* x = audio + b * N;
+    const float* g = grad_frames + r * kFrame;
+    float* dx = grad_audio + b * N;
+    const int64_t start = f * hop - pad_left;
+    float v[kPerLane], w[kPerLane];
+    const FrameGrad st = frame_grad(x, g, N, start, lane, v, w);
+#pragma unroll
+    for (int k = 0; k < kPerLane; ++k) {
+      const int64_t i = start + lane + 32 * k;
+      if (i >= 0 && i < N) dx[i] = (float)(0.0 + frame_term(st, w[k], v[k]));
+    }
+    // frame 0 starts at or before sample 0, so only gaps after a frame remain
+    const int64_t end = f + 1 < F ? i64min(start + hop, N) : (int64_t)N;
+    for (int64_t i = i64max(start + kFrame, 0) + lane; i < end; i += 32) dx[i] = 0.f;
+  }
+}
+
+// hop < kFrame: CTA t = b spans + s owns samples s kBwdOwn .. + kBwdOwn - 1 of item b.
+// fg: the FrameGrad of every frame covering one of them, in dynamic shared memory.
+__global__ void __launch_bounds__(kBwdThreads)
+crepe_frames_bwd_overlap_kernel(const float* __restrict__ audio,
+                                const float* __restrict__ grad_frames,
+                                float* __restrict__ grad_audio, int N, int F, int spans,
+                                int64_t total, int hop, int pad_left) {
+  extern __shared__ FrameGrad fg[];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int64_t t = blockIdx.x; t < total; t += gridDim.x) {
+    const int64_t b = t / spans;
+    const int64_t k0 = (t - b * spans) * (int64_t)kBwdOwn;
+    const int64_t k1 = i64min(k0 + kBwdOwn, N);
+    const float* x = audio + b * N;
+    const float* g = grad_frames + b * F * (int64_t)kFrame;
+    // frames f with f hop - pad_left <= k1 - 1 and f hop - pad_left + 1023 >= k0
+    const int64_t lo_num = k0 + pad_left - (kFrame - 1);
+    const int64_t f_lo = lo_num <= 0 ? 0 : (lo_num + hop - 1) / hop;
+    const int64_t f_hi = i64min((k1 - 1 + pad_left) / hop, (int64_t)F - 1);
+    __syncthreads();   // the previous span has finished reading fg
+    for (int64_t f = f_lo + warp; f <= f_hi; f += kBwdThreads / 32) {
+      float v[kPerLane], w[kPerLane];
+      const FrameGrad st = frame_grad(x, g + f * kFrame, N, f * hop - pad_left, lane, v, w);
+      if (lane == 0) fg[f - f_lo] = st;
+    }
+    __syncthreads();
+    for (int64_t i = k0 + threadIdx.x; i < k1; i += kBwdThreads) {
+      const float xi = x[i];
+      const int64_t num = i + pad_left - (kFrame - 1);
+      const int64_t a = i64max(f_lo, num <= 0 ? 0 : (num + hop - 1) / hop);
+      const int64_t e = i64min(f_hi, (i + pad_left) / hop);
+      double acc = 0.0;
+      for (int64_t f = a; f <= e; ++f)
+        acc += frame_term(fg[f - f_lo], g[f * kFrame + (i + pad_left - f * hop)], xi);
+      grad_audio[b * N + i] = (float)acc;
+    }
+  }
+}
+
+// Frames whose statistics one CTA of the overlap kernel keeps: those covering a span
+// of kBwdOwn samples.
+__host__ __device__ constexpr int bwd_frames_per_span(int hop) {
+  return (kBwdOwn - 1 + kFrame - 1) / hop + 2;
 }
 
 // ---- argmax helpers -------------------------------------------------------------------

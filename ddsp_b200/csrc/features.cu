@@ -267,8 +267,45 @@ int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n
 }
 
 // ---- CREPE: frames, Viterbi path, f0 and confidence ------------------------------
+// The framing of losses.PretrainedCREPE.frame_audio (CENTER pads 512 zeros on both
+// sides, VALID nothing; any hop, N >= 0); sets *pad_left.
+static int crepe_loss_check(const char* name, int B, int N, int n_frames, int hop,
+                            int padding, int* pad_left) {
+  DDSP_REQUIRE(B >= 0 && N >= 0 && n_frames >= 0 && hop >= 1, DDSP_B200_E_INVALID,
+               "%s: bad shape B=%d N=%d T=%d hop=%d", name, B, N, n_frames, hop);
+  DDSP_REQUIRE(padding == DDSP_B200_PAD_VALID || padding == DDSP_B200_PAD_CENTER,
+               DDSP_B200_E_INVALID, "%s: bad padding %d (CENTER or VALID)", name, padding);
+  *pad_left = padding == DDSP_B200_PAD_CENTER ? crepe_::kFrame / 2 : 0;
+  const long long padded = (long long)N + 2ll * *pad_left;
+  const long long want = padded >= crepe_::kFrame ? 1 + (padded - crepe_::kFrame) / hop : 0;
+  DDSP_REQUIRE(n_frames == want, DDSP_B200_E_INVALID, "%s: n_frames=%d, the padding gives %lld",
+               name, n_frames, want);
+  return 0;
+}
+
+static int crepe_loss_frames(const float* audio, float* frames, int B, int N, int n_frames,
+                             int hop, int padding, void* stream) {
+  int pad_left = 0;
+  int rc = crepe_loss_check("crepe_frames", B, N, n_frames, hop, padding, &pad_left);
+  if (rc) return rc;
+  DDSP_REQUIRE((audio || N == 0 || B == 0) && (frames || n_frames == 0 || B == 0),
+               DDSP_B200_E_INVALID, "crepe_frames: null pointer");
+  if (B == 0 || n_frames == 0) return 0;
+  DDSP_REQUIRE_DISJOINT("crepe_frames", frames, extent(B, n_frames, crepe_::kFrame), audio, extent(B, N));
+  const int64_t total = (int64_t)B * n_frames;
+  const int threads = 32 * crepe_::kFrameWarps;
+  crepe_::crepe_frames_kernel<true><<<grid_for(total * 32, threads, 16), threads, 0,
+                                      (cudaStream_t)stream>>>(audio, frames, N, n_frames,
+                                                              total, hop, pad_left);
+  DDSP_CHECK_LAUNCH("crepe_frames");
+  return 0;
+}
+
 int ddsp_b200_crepe_frames(const float* audio, float* frames, int B, int N, int n_frames,
                            int hop, int padding, void* stream) {
+  if (padding & DDSP_B200_CREPE_LOSS_FRAMES)
+    return crepe_loss_frames(audio, frames, B, N, n_frames, hop,
+                             padding & ~DDSP_B200_CREPE_LOSS_FRAMES, stream);
   DDSP_REQUIRE(audio && (frames || n_frames == 0 || B == 0), DDSP_B200_E_INVALID,
                "crepe_frames: null pointer");
   int pad_left = 0;
@@ -281,10 +318,44 @@ int ddsp_b200_crepe_frames(const float* audio, float* frames, int B, int N, int 
   DDSP_REQUIRE_DISJOINT("crepe_frames", frames, extent(B, n_frames, crepe_::kFrame), audio, extent(B, N));
   const int64_t total = (int64_t)B * n_frames;
   const int threads = 32 * crepe_::kFrameWarps;
-  crepe_::crepe_frames_kernel<<<grid_for(total * 32, threads, 16), threads, 0,
-                                (cudaStream_t)stream>>>(audio, frames, N, n_frames, total,
-                                                        hop, pad_left);
+  crepe_::crepe_frames_kernel<false><<<grid_for(total * 32, threads, 16), threads, 0,
+                                       (cudaStream_t)stream>>>(audio, frames, N, n_frames,
+                                                               total, hop, pad_left);
   DDSP_CHECK_LAUNCH("crepe_frames");
+  return 0;
+}
+
+int ddsp_b200_crepe_frames_backward(const float* audio, const float* grad_frames,
+                                    float* grad_audio, int B, int N, int n_frames, int hop,
+                                    int padding, void* stream) {
+  int pad_left = 0;
+  int rc = crepe_loss_check("crepe_frames_backward", B, N, n_frames, hop,
+                            padding & ~DDSP_B200_CREPE_LOSS_FRAMES, &pad_left);
+  if (rc) return rc;
+  DDSP_REQUIRE(B == 0 || N == 0 || (audio && grad_audio && (grad_frames || n_frames == 0)),
+               DDSP_B200_E_INVALID, "crepe_frames_backward: null pointer");
+  if (B == 0 || N == 0) return 0;
+  DDSP_REQUIRE_DISJOINT("crepe_frames_backward", grad_audio, extent(B, N), audio, extent(B, N));
+  DDSP_REQUIRE_DISJOINT("crepe_frames_backward", grad_audio, extent(B, N), grad_frames,
+                        extent(B, n_frames, crepe_::kFrame));
+  cudaStream_t s = (cudaStream_t)stream;
+  if (hop >= crepe_::kFrame && n_frames > 0) {
+    const int64_t total = (int64_t)B * n_frames;
+    const int threads = 32 * crepe_::kDisjointWarps;
+    crepe_::crepe_frames_bwd_disjoint_kernel<<<grid_for(total * 32, threads, 16), threads, 0,
+                                               s>>>(audio, grad_frames, grad_audio, N,
+                                                    n_frames, total, hop, pad_left);
+  } else {
+    const int spans = (N + crepe_::kBwdOwn - 1) / crepe_::kBwdOwn;
+    const int64_t total = (int64_t)B * spans;
+    const size_t smem = sizeof(crepe_::FrameGrad) * crepe_::bwd_frames_per_span(hop);
+    rc = set_smem(crepe_::crepe_frames_bwd_overlap_kernel, smem, "crepe_frames_backward");
+    if (rc) return rc;
+    const int blocks = (int)std::min<int64_t>(total, 16ll * num_sms());
+    crepe_::crepe_frames_bwd_overlap_kernel<<<blocks, crepe_::kBwdThreads, smem, s>>>(
+        audio, grad_frames, grad_audio, N, n_frames, spans, total, hop, pad_left);
+  }
+  DDSP_CHECK_LAUNCH("crepe_frames_backward");
   return 0;
 }
 

@@ -6,6 +6,9 @@ the CUDA kernels of `csrc/consistency.cuh` (`autograd.MixtureNLLFn`, `CombNLLFn`
 the [B, T, K]-sized elementwise work around them is torch autograd.  The HMM of
 `HmmTranscriber` (`losses.py:247-345`) runs on the kernels of `csrc/hmm.cuh`, and
 `wasserstein_distance` (`losses.py:641-686`) on those of `csrc/wasserstein.cuh`.
+The perceptual losses (`EmbeddingLoss`, `PretrainedCREPEEmbeddingLoss` and
+`PretrainedCREPE`, `losses.py:353-486`) frame and normalise the audio on the kernels
+of `csrc/crepe.cuh`, with their backward, around a CREPE network the caller supplies.
 `LossGroup` (`losses.py:50-98`) runs a DAG of losses."""
 import functools
 import math
@@ -189,6 +192,181 @@ class SpectralLoss:
             spectral_ops.safe_log(target_mag), spectral_ops.safe_log(value_mag),
             self.loss_type, weights=weights)
     return loss
+
+
+# ------------------------------------------------------------------------------
+# Perceptual losses (losses.py:353-486)
+# ------------------------------------------------------------------------------
+class EmbeddingLoss(Loss):
+  """losses.EmbeddingLoss (losses.py:356-388): weight * mean_difference of the
+  embeddings `pretrained_model` gives the target audio and the audio, so that the
+  synthesizer learns to match what a pretrained network hears.  pretrained_model is
+  any callable on float32 audio tensors: a `PretrainedCREPE`, or a TorchScript module
+  or plain function.  With weight <= 0 it returns the Python float 0.0 and does not
+  call the model."""
+
+  def __init__(self, weight=1.0, loss_type='L1', pretrained_model=None,
+               name='embedding_loss'):
+    super().__init__(name)
+    self.weight = weight
+    self.loss_type = loss_type
+    self.pretrained_model = pretrained_model
+
+  def call(self, target_audio, audio):
+    loss = 0.0
+    if self.weight > 0.0:
+      audio = core.torch_float32(audio)
+      target_audio = core.torch_float32(target_audio, audio.device)
+      target_emb = self.pretrained_model(target_audio)
+      synth_emb = self.pretrained_model(audio)
+      loss = self.weight * mean_difference(target_emb, synth_emb, self.loss_type)
+    return loss
+
+
+# Scales that bring each layer's embedding loss to comparable sizes (losses.py:400-414).
+CREPE_LAYER_SCALE = {
+    'conv1-BN': 1.3,
+    'conv1-maxpool': 1.0,
+    'conv2-BN': 1.4,
+    'conv2-maxpool': 1.1,
+    'conv3-BN': 1.9,
+    'conv3-maxpool': 1.6,
+    'conv4-BN': 1.5,
+    'conv4-maxpool': 1.4,
+    'conv5-BN': 1.9,
+    'conv5-maxpool': 1.7,
+    'conv6-BN': 30,
+    'conv6-maxpool': 25,
+    'classifier': 130,
+}
+
+
+class PretrainedCREPEEmbeddingLoss(EmbeddingLoss):
+  """losses.PretrainedCREPEEmbeddingLoss (losses.py:391-421): an EmbeddingLoss on the
+  activations of `activation_layer` of a CREPE network (`PretrainedCREPE`), weighted by
+  20 * CREPE_LAYER_SCALE[activation_layer] * weight.  model_capacity is the network, a
+  torch.nn.Module (see PretrainedCREPE).  An unknown activation_layer raises KeyError
+  before the network is looked at."""
+
+  def __init__(self, weight=1.0, loss_type='L1', model_capacity='tiny',
+               activation_layer='classifier', name='pretrained_crepe_embedding_loss'):
+    scale = CREPE_LAYER_SCALE[activation_layer]
+    super().__init__(
+        weight=20.0 * scale * weight,
+        loss_type=loss_type,
+        name=name,
+        pretrained_model=PretrainedCREPE(model_capacity=model_capacity,
+                                         activation_layer=activation_layer))
+
+
+class _Captured(Exception):
+  """Stops a network's forward once the activation layer has run."""
+
+
+class PretrainedCREPE:
+  """losses.PretrainedCREPE (losses.py:424-486): the activations of one layer of a CREPE
+  network on normalised frames of the audio, [batch, n_frames, -1].
+
+  model_capacity is the network, a torch.nn.Module mapping frames [M, 1024] to its
+  output; activation_layer names one of its submodules (`named_modules()`), whose
+  output is taken by a forward hook, removed after each call, and the forward stops
+  there.  The crepe package's size names ('tiny', 'small', 'medium', 'large', 'full')
+  name weights that are not shipped here and raise NotImplementedError; anything but a
+  torch.nn.Module raises TypeError, and so do TorchScript modules, which cannot take
+  submodule hooks (pass such a network, or any callable on audio, to
+  EmbeddingLoss(pretrained_model=...) instead).  An unknown activation_layer raises
+  ValueError.
+
+  The frames come from `autograd.CrepeLossFramesFn`, so gradients flow from the
+  activations back to the audio.  With trainable=False the network runs on detached
+  copies of its parameters (torch.func.functional_call): no gradient reaches them and
+  their .grad stays None, while the caller's requires_grad flags and the module's
+  train/eval mode are left as they are.  With trainable=True the module is called
+  directly.
+
+  The activation [M, ...] is reshaped to [batch, n_frames, -1] in the network's own
+  memory order: a torch conv net's [M, C, T, 1] flattens channel-major where Keras's
+  [M, T, 1, C] flattens time-major.  The L1, L2 and COSINE embedding losses compare the
+  two embeddings element by element (COSINE along the last axis, where both share the
+  order), so they do not depend on it."""
+
+  def __init__(self, model_capacity='tiny', activation_layer='conv5-maxpool',
+               name='pretrained_crepe', trainable=False):
+    if isinstance(model_capacity, str) and model_capacity in _CREPE_CAPACITIES:
+      raise NotImplementedError(
+          f"losses.PretrainedCREPE: the '{model_capacity}' weights come with the crepe "
+          'package and are not available here; pass the network as a torch.nn.Module.')
+    if isinstance(model_capacity, torch.jit.ScriptModule):
+      raise TypeError('losses.PretrainedCREPE: TorchScript modules cannot take the '
+                      'forward hook that reads activation_layer; pass a callable on '
+                      'audio to EmbeddingLoss(pretrained_model=...) instead.')
+    if not isinstance(model_capacity, torch.nn.Module):
+      raise TypeError('losses.PretrainedCREPE: model_capacity must be a torch.nn.Module, '
+                      f'got {type(model_capacity).__name__}')
+    self.layer_names = [n for n, _ in model_capacity.named_modules() if n]
+    if activation_layer not in self.layer_names:
+      raise ValueError('activation layer {} not found, valid names are {}'.format(
+          activation_layer, self.layer_names))
+    self.name = name
+    self.trainable = trainable
+    self._model_capacity = model_capacity
+    self._activation_layer = activation_layer
+    self._model = model_capacity
+    self.frame_length = spectral_ops.CREPE_FRAME_SIZE
+
+  def frame_audio(self, audio, hop_length=1024, center=True):
+    """Frames [batch, n_frames, 1024] of audio [batch, length]: 512 zeros on both sides
+    when `center`, frames of 1024 every hop_length (1 + (padded - 1024) // hop_length of
+    them, or none when the padded audio is shorter than a frame), each normalised to
+    (x - mean) / (sqrt(var) + 1e-5) with tf.nn.moments' mean and population variance.
+    Differentiable in the audio."""
+    shape = core._shape(audio)
+    if len(shape) != 2:
+      raise ValueError(f'audio must be [batch, length], got shape {tuple(shape)}')
+    if int(hop_length) != hop_length or hop_length < 1:
+      raise ValueError(f'hop_length must be a positive integer, got {hop_length}')
+    return autograd.CrepeLossFramesFn.apply(core.torch_float32(audio), int(hop_length),
+                                            bool(center))
+
+  @core.on_operands_device
+  def __call__(self, audio):
+    return self.call(audio)
+
+  def call(self, audio):
+    """The activations of activation_layer, [batch, n_frames, -1], for audio
+    [batch, length] framed every 1024 samples with centring."""
+    frames = self.frame_audio(audio)
+    batch_size, n_frames = frames.shape[:2]
+    outputs = self._activations(frames.reshape(-1, self.frame_length))
+    return outputs.reshape(batch_size, n_frames, -1)
+
+  def _activations(self, frames):
+    captured = []
+
+    def hook(module, inputs, output):
+      captured.append(output)
+      raise _Captured
+
+    layer = self._model.get_submodule(self._activation_layer)
+    handle = layer.register_forward_hook(hook)
+    try:
+      if self.trainable:
+        self._model(frames)
+      else:
+        state = {k: v.detach() for k, v in self._model.named_parameters()}
+        state.update(self._model.named_buffers())
+        torch.func.functional_call(self._model, state, (frames,))
+    except _Captured:
+      pass
+    finally:
+      handle.remove()
+    if not captured:
+      raise RuntimeError(f'losses.PretrainedCREPE: the network did not run '
+                         f'{self._activation_layer!r}')
+    return captured[0]
+
+
+_CREPE_CAPACITIES = ('tiny', 'small', 'medium', 'large', 'full')
 
 
 # ------------------------------------------------------------------------------

@@ -730,10 +730,34 @@ int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n
  *   argmax, or centers[m] (int32, any value) when centers is not null.  Weights summing
  *   to 0 give NaN (0 / 0), as in the reference.  M >= 0; M = 0 launches nothing.
  * crepe_frames' frames must not overlap audio; crepe_decode's f0 and confidence must
- * not overlap activations. */
+ * not overlap activations.
+ *
+ * losses.PretrainedCREPE.frame_audio (losses.py:455-468), the frames the embedding losses
+ * train through: padding DDSP_B200_PAD_CENTER or _VALID OR'ed with
+ * DDSP_B200_CREPE_LOSS_FRAMES makes ddsp_b200_crepe_frames normalise each frame to
+ * (x - mean) / (sqrt(var) + 1e-5) instead (a frame of variance 0 becomes zeros).  In
+ * that mode any hop >= 1 is taken with either padding, N may be 0 (CENTER then gives one
+ * frame of zeros, and audio may be null), and n_frames must be
+ * 1 + (N + 2 pad - 1024) / hop (pad = 512 for CENTER, 0 for VALID), or 0 when that
+ * padded length is below 1024.  SAME is E_INVALID.
+ * ddsp_b200_crepe_frames_backward: grad_audio [B,N] of that normalisation for
+ *   grad_frames [B * n_frames, 1024], the same B, N, n_frames, hop and padding (with or
+ *   without the flag).  Every element of grad_audio is written, 0 where no frame reads
+ *   the sample.  Per frame with mu, s = sqrt(var), gbar = mean(g) and
+ *   c = sum_j g_j (x_j - mu):
+ *     dx_k = (g_k - gbar) / (s + 1e-5) - c (x_k - mu) / ((s + 1e-5)^2 1024 s),
+ *   statistics in double; overlapping frames (hop < 1024) add in increasing frame order.
+ *   A frame of variance 0 makes every sample it covers NaN, as TensorFlow's gradient of
+ *   var**0.5 at 0 does.  No atomics and no workspace: bit-reproducible.  grad_audio must
+ *   not overlap audio or grad_frames.  B = 0 or N = 0 returns after the checks without a
+ *   launch; B and N are otherwise unbounded. */
 enum { DDSP_B200_CREPE_BINS = 360, DDSP_B200_CREPE_FRAME = 1024 };
+enum { DDSP_B200_CREPE_LOSS_FRAMES = 256 /* OR'ed into crepe_frames' padding */ };
 int ddsp_b200_crepe_frames(const float* audio, float* frames, int B, int N, int n_frames,
                            int hop, int padding, void* stream);
+int ddsp_b200_crepe_frames_backward(const float* audio, const float* grad_frames,
+                                    float* grad_audio, int B, int N, int n_frames, int hop,
+                                    int padding, void* stream);
 size_t ddsp_b200_crepe_viterbi_workspace_bytes(int B, int T);
 int ddsp_b200_crepe_viterbi(const float* activations, int* centers, void* workspace,
                             size_t workspace_bytes, int B, int T, void* stream);
