@@ -6,6 +6,8 @@
 #include <algorithm>
 #include <cfloat>
 #include <cmath>
+#include <cstring>
+#include <initializer_list>
 #include <vector>
 
 #include "common.cuh"
@@ -51,25 +53,53 @@ static T* align256(const void* p) {
   return reinterpret_cast<T*>(((uintptr_t)p + 255) & ~(uintptr_t)255);
 }
 
+// A float operand of an entry point: its C parameter name, first element and extent in
+// elements.  An output's `may_be` lists, comma-separated, the inputs it may BE.
+struct Operand {
+  const char* name;
+  const void* p;
+  size_t n;
+  const char* may_be;
+};
+
+// Whether the comma-separated list `names` holds `name`.
+inline bool lists(const char* names, const char* name) {
+  const size_t len = strlen(name);
+  for (const char* s = names + strspn(names, ", "); *s; s += strspn(s, ", ")) {
+    const size_t n = strcspn(s, ", ");
+    if (n == len && !strncmp(s, name, n)) return true;
+    s += n;
+  }
+  return false;
+}
+
+// E_INVALID, before any launch, when a float output of entry point `fn` overlaps one
+// of its float inputs: a kernel whose threads read inputs that other threads write
+// would race.  An output may be an input its `may_be` lists (an elementwise kernel in
+// place), but only exactly: same first element and extent.  Walks outputs x inputs in
+// order and reports the first pair that overlaps.
+inline int check_overlap(const char* fn, std::initializer_list<Operand> outs,
+                         std::initializer_list<Operand> ins) {
+  for (const Operand& o : outs)
+    for (const Operand& i : ins) {
+      const bool may_be = lists(o.may_be, i.name);
+      if (may_be && o.p == i.p && o.n == i.n) continue;
+      if (!overlaps(o.p, sizeof(float) * o.n, i.p, sizeof(float) * i.n)) continue;
+      if (may_be)
+        set_error("%s: %s must be %s or not overlap it", fn, o.name, i.name);
+      else
+        set_error("%s: %s must not overlap %s", fn, o.name, i.name);
+      return DDSP_B200_E_INVALID;
+    }
+  return 0;
+}
+
 }  // namespace ddsp
 
-// E_INVALID, before any launch, when the float output `out` of `out_n` elements
-// overlaps the float input `in` of `in_n` elements: a kernel whose threads read
-// inputs that other threads write would race.
-#define DDSP_REQUIRE_DISJOINT(fn, out, out_n, in, in_n)                          \
-  DDSP_REQUIRE(!::ddsp::overlaps((out), sizeof(float) * (out_n), (in),            \
-                                 sizeof(float) * (in_n)),                         \
-               DDSP_B200_E_INVALID, "%s: %s must not overlap %s", (fn), #out, #in)
-
-// The same for an output that may BE the input `in` (an elementwise kernel in place):
-// only the exact alias, same first element and extent, passes besides disjoint ranges.
-#define DDSP_REQUIRE_SAME_OR_DISJOINT(fn, out, out_n, in, in_n)                  \
-  DDSP_REQUIRE(((const void*)(out) == (const void*)(in) &&                        \
-                (size_t)(out_n) == (size_t)(in_n)) ||                             \
-                   !::ddsp::overlaps((out), sizeof(float) * (out_n), (in),        \
-                                     sizeof(float) * (in_n)),                     \
-               DDSP_B200_E_INVALID, "%s: %s must be %s or not overlap it", (fn), #out, \
-               #in)
+// Operands of check_overlap, named after their C parameter.  DDSP_OUT's trailing
+// arguments name the inputs the output may be.
+#define DDSP_IN(x, n) (::ddsp::Operand{#x, (x), (size_t)(n), ""})
+#define DDSP_OUT(x, n, ...) (::ddsp::Operand{#x, (x), (size_t)(n), #__VA_ARGS__})
 
 #define DDSP_CUDA_TRY(expr, what)                                       \
   do {                                                                    \

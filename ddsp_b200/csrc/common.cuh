@@ -52,6 +52,19 @@ int set_smem(K kernel, size_t bytes, const char* name) {
   return 0;
 }
 
+// Reserves `smem`, launches `kern` and checks the launch: how every kernel of the
+// library starts (noise_ring.cuh's programmatic dependent launch aside).  Returns 0, or
+// E_CUDA with `name` in front of the message.
+template <typename... KArgs, typename... Args>
+int launch(const char* name, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
+           cudaStream_t st, Args&&... args) {
+  int rc = set_smem(kern, smem, name);
+  if (rc) return rc;
+  kern<<<grid, block, smem, st>>>(static_cast<Args&&>(args)...);
+  DDSP_CHECK_LAUNCH(name);
+  return 0;
+}
+
 // Upper bound on the SM count, for per-SM debug arrays (H100 SXM has 132).
 constexpr int kMaxSMs = 256;
 

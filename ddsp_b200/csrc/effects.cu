@@ -20,11 +20,11 @@ int ddsp_b200_sinc_impulse_response(const float* cutoff, float* ir, int64_t BF, 
                "%s: bad shape BF=%lld S=%d (S must be odd)", name, (long long)BF, S);
   DDSP_REQUIRE(BF < (1ll << 31), DDSP_B200_E_INVALID, "%s: too many frames", name);
   if (BF == 0) return 0;
-  DDSP_REQUIRE_DISJOINT(name, ir, extent(BF, S), cutoff, extent(BF));
-  sinc_ir_kernel<<<(unsigned)BF, kSincThreads, 0, (cudaStream_t)stream>>>(cutoff, ir, S, scale,
-                                                                          high_pass);
-  DDSP_CHECK_LAUNCH(name);
-  return 0;
+  int rc = check_overlap(name, {DDSP_OUT(ir, extent(BF, S))},
+                         {DDSP_IN(cutoff, extent(BF))});
+  if (rc) return rc;
+  return launch(name, sinc_ir_kernel, (unsigned)BF, kSincThreads, 0, (cudaStream_t)stream,
+                cutoff, ir, S, scale, high_pass);
 }
 
 int ddsp_b200_sinc_impulse_response_backward(const float* cutoff, const float* d_ir,
@@ -36,10 +36,8 @@ int ddsp_b200_sinc_impulse_response_backward(const float* cutoff, const float* d
                "%s: bad shape BF=%lld S=%d (S must be odd)", name, (long long)BF, S);
   DDSP_REQUIRE(BF < (1ll << 31), DDSP_B200_E_INVALID, "%s: too many frames", name);
   if (BF == 0) return 0;
-  sinc_ir_backward_kernel<<<(unsigned)BF, kSincThreads, 0, (cudaStream_t)stream>>>(
-      cutoff, d_ir, d_cutoff, S, scale, high_pass);
-  DDSP_CHECK_LAUNCH(name);
-  return 0;
+  return launch(name, sinc_ir_backward_kernel, (unsigned)BF, kSincThreads, 0,
+                (cudaStream_t)stream, cutoff, d_ir, d_cutoff, S, scale, high_pass);
 }
 
 // The checks both sinc_filter entry points make after the null-pointer check; sets
@@ -82,20 +80,19 @@ int ddsp_b200_sinc_filter(const float* audio, const float* cutoff, float* out, i
   int rc = sinc_filter_check(name, B, N, F, S, cutoff_batch, padding, &frame, &start,
                              &out_len);
   if (rc || B == 0) return rc;
-  DDSP_REQUIRE_DISJOINT(name, out, extent(B, out_len), audio, extent(B, N));
-  DDSP_REQUIRE_DISJOINT(name, out, extent(B, out_len), cutoff, extent(cutoff_batch, F));
-  const size_t smem = sinc_filter_smem(S);
-  rc = set_smem(sinc_filter_kernel, smem, name);
+  rc = check_overlap(name, {DDSP_OUT(out, extent(B, out_len))},
+                     {DDSP_IN(audio, extent(B, N)),
+                      DDSP_IN(cutoff, extent(cutoff_batch, F))});
   if (rc) return rc;
+  const size_t smem = sinc_filter_smem(S);
   SincFilterParams p;
   p.x = audio; p.cutoff = cutoff; p.out = out;
   p.N = N; p.F = F; p.frame = frame; p.S = S; p.cutoff_stride = cutoff_batch == 1 ? 0 : F;
   p.scale = scale; p.high_pass = high_pass ? 1 : 0; p.start = start; p.out_len = out_len;
   p.accumulate = accumulate ? 1 : 0;
   dim3 grid((out_len + kSincTile - 1) / kSincTile, B);
-  sinc_filter_kernel<<<grid, kSincThreads, smem, (cudaStream_t)stream>>>(p);
-  DDSP_CHECK_LAUNCH(name);
-  return 0;
+  return launch(name, sinc_filter_kernel, grid, kSincThreads, smem, (cudaStream_t)stream,
+                p);
 }
 
 // Partial d cutoff sums the backward needs: none when every frame is one tile and every
@@ -142,22 +139,14 @@ int ddsp_b200_sinc_filter_backward(const float* audio, const float* cutoff, cons
   p.scale = scale; p.high_pass = high_pass ? 1 : 0; p.start = start; p.out_len = out_len;
   sinc_bwd_tiles(N, F, frame, &p.fpt, &p.n_seg, &p.seg, &p.tiles);
   const size_t smem = sinc_bwd_smem(S);
-  dim3 grid((unsigned)p.tiles, B);
-  if (d_cutoff) {
-    rc = set_smem(sinc_filter_backward_kernel<true>, smem, name);
-    if (rc) return rc;
-    sinc_filter_backward_kernel<true><<<grid, kSincThreads, smem, st>>>(p);
-  } else {
-    rc = set_smem(sinc_filter_backward_kernel<false>, smem, name);
-    if (rc) return rc;
-    sinc_filter_backward_kernel<false><<<grid, kSincThreads, smem, st>>>(p);
-  }
-  DDSP_CHECK_LAUNCH(name);
+  auto kern = d_cutoff ? sinc_filter_backward_kernel<true> : sinc_filter_backward_kernel<false>;
+  rc = launch(name, kern, dim3((unsigned)p.tiles, B), kSincThreads, smem, st, p);
+  if (rc) return rc;
   if (part) {
     const long long n_out = (long long)cutoff_batch * F;
-    sinc_dc_reduce<<<grid_for(n_out, 256), 256, 0, st>>>(part, d_cutoff, B, F, p.n_seg,
-                                                         cutoff_batch == 1 && B > 1, n_out);
-    DDSP_CHECK_LAUNCH(name);
+    rc = launch(name, sinc_dc_reduce, grid_for(n_out, 256), 256, 0, st, part, d_cutoff, B,
+                F, p.n_seg, cutoff_batch == 1 && B > 1, n_out);
+    if (rc) return rc;
   }
   return 0;
 }
@@ -201,12 +190,14 @@ int ddsp_b200_fft_convolve_lti(const float* audio, const float* impulse_response
   cudaStream_t st = (cudaStream_t)stream;
   DDSP_REQUIRE((flags & ~3) == 0, DDSP_B200_E_INVALID,
                "fft_convolve_lti: bad flags %d", flags);
-  lc::lc_fft_blocks<<<dim3(g.P, ir_batch), lc::THREADS, 0, st>>>(
-      impulse_response, H, S, 0, g.P, 1, (flags & DDSP_B200_LTI_REVERSE_IR) ? 1 : 0);
-  DDSP_CHECK_LAUNCH("fft_convolve_lti(ir spectra)");
-  lc::lc_fft_blocks<<<dim3(g.n_in, B), lc::THREADS, 0, st>>>(
-      audio, Z, N, g.n2, g.n_in, 0, (flags & DDSP_B200_LTI_REVERSE_AUDIO) ? 1 : 0);
-  DDSP_CHECK_LAUNCH("fft_convolve_lti(audio spectra)");
+  int rc = launch("fft_convolve_lti(ir spectra)", lc::lc_fft_blocks, dim3(g.P, ir_batch),
+                  lc::THREADS, 0, st, impulse_response, H, S, 0, g.P, 1,
+                  (flags & DDSP_B200_LTI_REVERSE_IR) ? 1 : 0);
+  if (rc) return rc;
+  rc = launch("fft_convolve_lti(audio spectra)", lc::lc_fft_blocks, dim3(g.n_in, B),
+              lc::THREADS, 0, st, audio, Z, N, g.n2, g.n_in, 0,
+              (flags & DDSP_B200_LTI_REVERSE_AUDIO) ? 1 : 0);
+  if (rc) return rc;
   // w blocks the crop reads: positions [start, start + out_len) through the real
   // half and [start - n2, start + out_len - n2) through the imaginary half
   const int lo_pos = std::max(0, start - g.n2);
@@ -214,20 +205,15 @@ int ddsp_b200_fft_convolve_lti(const float* audio, const float* impulse_response
   const int j_first = lo_pos / lc::L;
   const int j_last = std::min(g.n_out - 1, (hi_pos - 1) / lc::L);
   const int n_blocks = j_last - j_first + 1;
-  {
-    int rc = set_smem(lc::lc_mac_ifft, lc::kMacSmem, "fft_convolve_lti");
-    if (rc) return rc;
-  }
-  lc::lc_mac_ifft<<<dim3((n_blocks + lc::JT - 1) / lc::JT, B), lc::THREADS, lc::kMacSmem,
-                    st>>>(
-      Z, H, W, g.n_in, g.P, g.n_out, ir_batch == 1 ? 0 : g.P * lc::M, j_first, n_blocks);
-  DDSP_CHECK_LAUNCH("fft_convolve_lti(multiply-accumulate + inverse)");
+  rc = launch("fft_convolve_lti(multiply-accumulate + inverse)", lc::lc_mac_ifft,
+              dim3((n_blocks + lc::JT - 1) / lc::JT, B), lc::THREADS, lc::kMacSmem, st, Z,
+              H, W, g.n_in, g.P, g.n_out, ir_batch == 1 ? 0 : g.P * lc::M, j_first,
+              n_blocks);
+  if (rc) return rc;
   const int cgrid = std::min((out_len + 255) / 256, 8 * num_sms());
-  lc::lc_combine<<<dim3(cgrid, B), 256, 0, st>>>(W, out, g.n2, g.w_len, start, out_len,
-                                               N + S - 1, accumulate, j_first * lc::L,
-                                               (j_last + 1) * lc::L);
-  DDSP_CHECK_LAUNCH("fft_convolve_lti(combine)");
-  return 0;
+  return launch("fft_convolve_lti(combine)", lc::lc_combine, dim3(cgrid, B), 256, 0, st, W,
+                out, g.n2, g.w_len, start, out_len, N + S - 1, accumulate, j_first * lc::L,
+                (j_last + 1) * lc::L);
 }
 
 int ddsp_b200_resample(const float* in, float* out, int B, int F, int C, int N,
@@ -250,13 +236,13 @@ int ddsp_b200_resample(const float* in, float* out, int B, int F, int C, int N,
                  "frames:%d, add_endpoint=%s).", add_endpoint ? "" : " - 1", N,
                  n_frames, add_endpoint ? "True" : "False");
   }
-  DDSP_REQUIRE_DISJOINT("resample", out, extent(B, N, C), in, extent(B, F, C));
+  int rc = check_overlap("resample", {DDSP_OUT(out, extent(B, N, C))},
+                         {DDSP_IN(in, extent(B, F, C))});
+  if (rc) return rc;
   if (B == 0) return 0;
   const int64_t total = (int64_t)B * N * C;
-  resample_kernel<<<grid_for(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(
-      in, out, B, F, C, N, method, add_endpoint);
-  DDSP_CHECK_LAUNCH("resample");
-  return 0;
+  return launch("resample", resample_kernel, grid_for(total, 256, 16), 256, 0,
+                (cudaStream_t)stream, in, out, B, F, C, N, method, add_endpoint);
 }
 
 int ddsp_b200_add(const float* a, const float* b, float* out, int64_t n,
@@ -264,11 +250,11 @@ int ddsp_b200_add(const float* a, const float* b, float* out, int64_t n,
   DDSP_REQUIRE(a && b && out, DDSP_B200_E_INVALID, "add: null pointer");
   DDSP_REQUIRE(n >= 0, DDSP_B200_E_INVALID, "add: n < 0");
   if (n == 0) return 0;
-  DDSP_REQUIRE_SAME_OR_DISJOINT("add", out, extent(n), a, extent(n));
-  DDSP_REQUIRE_SAME_OR_DISJOINT("add", out, extent(n), b, extent(n));
-  add_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(a, b, out, n);
-  DDSP_CHECK_LAUNCH("add");
-  return 0;
+  int rc = check_overlap("add", {DDSP_OUT(out, extent(n), a, b)},
+                         {DDSP_IN(a, extent(n)), DDSP_IN(b, extent(n))});
+  if (rc) return rc;
+  return launch("add", add_kernel, grid_for(n, 256), 256, 0, (cudaStream_t)stream, a, b,
+                out, n);
 }
 
 // ---- routing: resample backward, Mix, ExpDecayReverb impulse response -----------
@@ -295,17 +281,10 @@ int ddsp_b200_resample_backward(const float* grad_out, float* grad_in, int B, in
   if (B == 0) return 0;
   const rt_::ResampleGeom g = rt_::resample_geom(F, N, method, add_endpoint);
   const int64_t total = (int64_t)B * F * C;
-  if (N >= 8 * F) {   // long frames: a warp per frame
-    rt_::resample_backward_kernel<32>
-        <<<grid_for(total * 32, rt_::kThreads, 16), rt_::kThreads, 0, (cudaStream_t)stream>>>(
-            grad_out, grad_in, B, C, g);
-  } else {
-    rt_::resample_backward_kernel<1>
-        <<<grid_for(total, rt_::kThreads, 16), rt_::kThreads, 0, (cudaStream_t)stream>>>(
-            grad_out, grad_in, B, C, g);
-  }
-  DDSP_CHECK_LAUNCH("resample_backward");
-  return 0;
+  const int lanes = N >= 8 * F ? 32 : 1;   // long frames: a warp per frame
+  auto kern = lanes == 32 ? rt_::resample_backward_kernel<32> : rt_::resample_backward_kernel<1>;
+  return launch("resample_backward", kern, grid_for(total * lanes, rt_::kThreads, 16),
+                rt_::kThreads, 0, (cudaStream_t)stream, grad_out, grad_in, B, C, g);
 }
 
 int ddsp_b200_mix_forward(const float* signal_one, const float* signal_two,
@@ -315,15 +294,17 @@ int ddsp_b200_mix_forward(const float* signal_one, const float* signal_two,
                "mix_forward: null pointer");
   DDSP_REQUIRE(B >= 0 && N >= 1 && C >= 1, DDSP_B200_E_INVALID,
                "mix_forward: bad shape B=%d N=%d C=%d", B, N, C);
-  DDSP_REQUIRE_SAME_OR_DISJOINT("mix_forward", out, extent(B, N, C), signal_one, extent(B, N, C));
-  DDSP_REQUIRE_SAME_OR_DISJOINT("mix_forward", out, extent(B, N, C), signal_two, extent(B, N, C));
-  DDSP_REQUIRE_SAME_OR_DISJOINT("mix_forward", out, extent(B, N, C), mix_level, extent(B, N));
+  int rc = check_overlap("mix_forward",
+                         {DDSP_OUT(out, extent(B, N, C), signal_one, signal_two, mix_level)},
+                         {DDSP_IN(signal_one, extent(B, N, C)),
+                          DDSP_IN(signal_two, extent(B, N, C)),
+                          DDSP_IN(mix_level, extent(B, N))});
+  if (rc) return rc;
   if (B == 0) return 0;
   const int64_t total = (int64_t)B * N * C;
-  rt_::mix_kernel<<<grid_for(total, rt_::kThreads), rt_::kThreads, 0, (cudaStream_t)stream>>>(
-      signal_one, signal_two, mix_level, out, (int64_t)B * N, C);
-  DDSP_CHECK_LAUNCH("mix_forward");
-  return 0;
+  return launch("mix_forward", rt_::mix_kernel, grid_for(total, rt_::kThreads),
+                rt_::kThreads, 0, (cudaStream_t)stream, signal_one, signal_two, mix_level,
+                out, (int64_t)B * N, C);
 }
 
 int ddsp_b200_mix_backward(const float* signal_one, const float* signal_two,
@@ -336,12 +317,9 @@ int ddsp_b200_mix_backward(const float* signal_one, const float* signal_two,
                "mix_backward: bad shape B=%d N=%d C=%d", B, N, C);
   if (B == 0 || (!grad_signal_one && !grad_signal_two && !grad_mix_level)) return 0;
   const int64_t rows = (int64_t)B * N;
-  rt_::mix_backward_kernel<<<grid_for(rows, rt_::kThreads), rt_::kThreads, 0,
-                             (cudaStream_t)stream>>>(
-      signal_one, signal_two, mix_level, grad_out, grad_signal_one, grad_signal_two,
-      grad_mix_level, rows, C);
-  DDSP_CHECK_LAUNCH("mix_backward");
-  return 0;
+  return launch("mix_backward", rt_::mix_backward_kernel, grid_for(rows, rt_::kThreads),
+                rt_::kThreads, 0, (cudaStream_t)stream, signal_one, signal_two, mix_level,
+                grad_out, grad_signal_one, grad_signal_two, grad_mix_level, rows, C);
 }
 
 int ddsp_b200_exp_decay_ir(const float* gain, const float* decay, const float* noise,
@@ -350,16 +328,15 @@ int ddsp_b200_exp_decay_ir(const float* gain, const float* decay, const float* n
   DDSP_REQUIRE(gain && decay && ir, DDSP_B200_E_INVALID, "exp_decay_ir: null pointer");
   DDSP_REQUIRE(rows >= 0 && L >= 1, DDSP_B200_E_INVALID,
                "exp_decay_ir: bad shape rows=%d L=%d", rows, L);
-  DDSP_REQUIRE_DISJOINT("exp_decay_ir", ir, extent(rows, L), gain, extent(rows));
-  DDSP_REQUIRE_DISJOINT("exp_decay_ir", ir, extent(rows, L), decay, extent(rows));
-  DDSP_REQUIRE_DISJOINT("exp_decay_ir", ir, extent(rows, L), noise, extent(L));
+  int rc = check_overlap("exp_decay_ir", {DDSP_OUT(ir, extent(rows, L))},
+                         {DDSP_IN(gain, extent(rows)), DDSP_IN(decay, extent(rows)),
+                          DDSP_IN(noise, extent(L))});
+  if (rc) return rc;
   if (rows == 0) return 0;
   const int64_t total = (int64_t)rows * ((L + 3) / 4);
-  rt_::exp_decay_ir_kernel<<<grid_for(total, rt_::kThreads), rt_::kThreads, 0,
-                             (cudaStream_t)stream>>>(gain, decay, noise, seed, offset, ir,
-                                                     rows, L);
-  DDSP_CHECK_LAUNCH("exp_decay_ir");
-  return 0;
+  return launch("exp_decay_ir", rt_::exp_decay_ir_kernel, grid_for(total, rt_::kThreads),
+                rt_::kThreads, 0, (cudaStream_t)stream, gain, decay, noise, seed, offset,
+                ir, rows, L);
 }
 
 int ddsp_b200_exp_decay_ir_backward(const float* gain, const float* decay,
@@ -371,10 +348,9 @@ int ddsp_b200_exp_decay_ir_backward(const float* gain, const float* decay,
   DDSP_REQUIRE(rows >= 0 && L >= 1, DDSP_B200_E_INVALID,
                "exp_decay_ir_backward: bad shape rows=%d L=%d", rows, L);
   if (rows == 0 || (!grad_gain && !grad_decay)) return 0;
-  rt_::exp_decay_ir_backward_kernel<<<rows, rt_::kIrBwdThreads, 0, (cudaStream_t)stream>>>(
-      gain, decay, noise, seed, offset, grad_ir, grad_gain, grad_decay, L);
-  DDSP_CHECK_LAUNCH("exp_decay_ir_backward");
-  return 0;
+  return launch("exp_decay_ir_backward", rt_::exp_decay_ir_backward_kernel, rows,
+                rt_::kIrBwdThreads, 0, (cudaStream_t)stream, gain, decay, noise, seed,
+                offset, grad_ir, grad_gain, grad_decay, L);
 }
 
 // ---- modulated delay ----------------------------------------------------------
@@ -385,15 +361,15 @@ int ddsp_b200_mod_delay_forward(const float* audio, const float* phase, const fl
   DDSP_REQUIRE(B >= 0 && B <= 65535 && N >= 1 && max_length >= 1 && max_length < (1 << 29),
                DDSP_B200_E_INVALID, "mod_delay_forward: bad shape B=%d N=%d max_length=%d",
                B, N, max_length);
-  DDSP_REQUIRE_DISJOINT("mod_delay_forward", out, extent(B, N), audio, extent(B, N));
-  DDSP_REQUIRE_SAME_OR_DISJOINT("mod_delay_forward", out, extent(B, N), phase, extent(B, N));
-  DDSP_REQUIRE_SAME_OR_DISJOINT("mod_delay_forward", out, extent(B, N), gain, extent(B, N));
+  int rc = check_overlap("mod_delay_forward", {DDSP_OUT(out, extent(B, N), phase, gain)},
+                         {DDSP_IN(audio, extent(B, N)), DDSP_IN(phase, extent(B, N)),
+                          DDSP_IN(gain, extent(B, N))});
+  if (rc) return rc;
   if (B == 0) return 0;
   dim3 grid((unsigned)((N + md_::kThreads - 1) / md_::kThreads), B);
-  md_::mod_delay_forward_kernel<<<grid, md_::kThreads, 0, (cudaStream_t)stream>>>(
-      audio, phase, gain, out, N, max_length, scale, offset, add_dry);
-  DDSP_CHECK_LAUNCH("mod_delay_forward");
-  return 0;
+  return launch("mod_delay_forward", md_::mod_delay_forward_kernel, grid, md_::kThreads, 0,
+                (cudaStream_t)stream, audio, phase, gain, out, N, max_length, scale, offset,
+                add_dry);
 }
 
 int ddsp_b200_mod_delay_backward(const float* audio, const float* phase, const float* gain,
@@ -409,15 +385,10 @@ int ddsp_b200_mod_delay_backward(const float* audio, const float* phase, const f
                B, N, max_length);
   if (B == 0 || (!grad_audio && !grad_gain && !grad_phase)) return 0;
   const size_t smem = grad_audio ? md_::backward_smem_bytes() : 0;
-  int rc = set_smem(md_::mod_delay_backward_kernel, md_::backward_smem_bytes(),
-                    "mod_delay_backward");
-  if (rc) return rc;
   dim3 grid((unsigned)((N + md_::kTile - 1) / md_::kTile), B);
-  md_::mod_delay_backward_kernel<<<grid, md_::kThreads, smem, (cudaStream_t)stream>>>(
-      audio, phase, gain, grad_out, grad_audio, grad_gain, grad_phase, N, max_length, scale,
-      offset, add_dry);
-  DDSP_CHECK_LAUNCH("mod_delay_backward");
-  return 0;
+  return launch("mod_delay_backward", md_::mod_delay_backward_kernel, grid, md_::kThreads,
+                smem, (cudaStream_t)stream, audio, phase, gain, grad_out, grad_audio,
+                grad_gain, grad_phase, N, max_length, scale, offset, add_dry);
 }
 
 }  // extern "C"

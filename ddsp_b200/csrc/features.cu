@@ -22,15 +22,16 @@ int ddsp_b200_frame_window(const float* audio, const float* window, float* frame
                N, n_frames, frame_size, frame_step);
   DDSP_REQUIRE((((uintptr_t)window | (uintptr_t)frames) & 15) == 0, DDSP_B200_E_INVALID,
                "frame_window: window / frames must be 16-byte aligned");
-  DDSP_REQUIRE_DISJOINT("frame_window", frames, extent(B, n_frames, frame_size), audio, extent(B, N));
-  DDSP_REQUIRE_DISJOINT("frame_window", frames, extent(B, n_frames, frame_size), window, extent(frame_size));
+  int rc = check_overlap("frame_window",
+                         {DDSP_OUT(frames, extent(B, n_frames, frame_size))},
+                         {DDSP_IN(audio, extent(B, N)),
+                          DDSP_IN(window, extent(frame_size))});
+  if (rc) return rc;
   if (B == 0) return 0;
   const long long quads = ((long long)n_frames * frame_size) / 4;
   dim3 grid((unsigned)((quads + 255) / 256), B);
-  frame_window_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(audio, window, frames, N, n_frames,
-                                                            frame_size, frame_step);
-  DDSP_CHECK_LAUNCH("frame_window");
-  return 0;
+  return launch("frame_window", frame_window_kernel, grid, 256, 0, (cudaStream_t)stream,
+                audio, window, frames, N, n_frames, frame_size, frame_step);
 }
 
 int ddsp_b200_frame_window_adjoint(const float* grad_frames, const float* window,
@@ -43,17 +44,16 @@ int ddsp_b200_frame_window_adjoint(const float* grad_frames, const float* window
   DDSP_REQUIRE(B >= 0 && N >= 1 && n_frames >= 1 && frame_size >= 1 && frame_step >= 1 &&
                    B <= 65535,
                DDSP_B200_E_INVALID, "frame_window_adjoint: bad shape");
-  DDSP_REQUIRE_DISJOINT("frame_window_adjoint", grad_audio, extent(B, N), grad_frames,
-                        extent(B, n_frames, frame_size));
-  DDSP_REQUIRE_DISJOINT("frame_window_adjoint", grad_audio, extent(B, N), window, extent(frame_size));
-  DDSP_REQUIRE_DISJOINT("frame_window_adjoint", grad_audio, extent(B, N), scale_device, extent(1));
+  int rc = check_overlap("frame_window_adjoint", {DDSP_OUT(grad_audio, extent(B, N))},
+                         {DDSP_IN(grad_frames, extent(B, n_frames, frame_size)),
+                          DDSP_IN(window, extent(frame_size)),
+                          DDSP_IN(scale_device, extent(1))});
+  if (rc) return rc;
   if (B == 0) return 0;
   dim3 grid((N + 255) / 256, B);
-  frame_window_adjoint_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
-      grad_frames, window, grad_audio, N, n_frames, frame_size, frame_step,
-      scale_device, accumulate);
-  DDSP_CHECK_LAUNCH("frame_window_adjoint");
-  return 0;
+  return launch("frame_window_adjoint", frame_window_adjoint_kernel, grid, 256, 0,
+                (cudaStream_t)stream, grad_frames, window, grad_audio, N, n_frames,
+                frame_size, frame_step, scale_device, accumulate);
 }
 
 int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
@@ -68,15 +68,17 @@ int ddsp_b200_spectral_l1(const float* stft_target, const float* stft_value,
                (long long)n_bins_total, n_bins, irfft_size);
   DDSP_REQUIRE((((uintptr_t)stft_target | (uintptr_t)stft_value | (uintptr_t)grad_value) & 15) == 0,
                DDSP_B200_E_INVALID, "spectral_l1: tensors must be 16-byte aligned");
-  DDSP_REQUIRE_DISJOINT("spectral_l1", grad_value, extent(n_bins_total, 2), stft_target, extent(n_bins_total, 2));
-  DDSP_REQUIRE_SAME_OR_DISJOINT("spectral_l1", grad_value, extent(n_bins_total, 2), stft_value, extent(n_bins_total, 2));
+  int rc = check_overlap("spectral_l1",
+                         {DDSP_OUT(grad_value, extent(n_bins_total, 2), stft_value)},
+                         {DDSP_IN(stft_target, extent(n_bins_total, 2)),
+                          DDSP_IN(stft_value, extent(n_bins_total, 2))});
+  if (rc) return rc;
   const long long blocks = std::min<long long>((n_bins_total / 2 + 255) / 256 + 1, 8ll * num_sms());
-  spectral_l1_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
-      reinterpret_cast<const float2*>(stft_target), reinterpret_cast<const float2*>(stft_value),
-      reinterpret_cast<float2*>(grad_value), sums, n_bins_total, mag_weight, logmag_weight,
-      1.0f / (float)n_bins_total, 1e-5f, n_bins, irfft_size);
-  DDSP_CHECK_LAUNCH("spectral_l1");
-  return 0;
+  return launch("spectral_l1", spectral_l1_kernel, (unsigned)blocks, 256, 0,
+                (cudaStream_t)stream, reinterpret_cast<const float2*>(stft_target),
+                reinterpret_cast<const float2*>(stft_value),
+                reinterpret_cast<float2*>(grad_value), sums, n_bins_total, mag_weight,
+                logmag_weight, 1.0f / (float)n_bins_total, 1e-5f, n_bins, irfft_size);
 }
 
 int ddsp_b200_spectral_terms(const float* stft_target, const float* stft_value,
@@ -102,9 +104,11 @@ int ddsp_b200_spectral_terms(const float* stft_target, const float* stft_value,
                "spectral_terms: with delta_time, grad_value must not overlap either STFT");
   DDSP_REQUIRE(F <= st_::kMaxBins, DDSP_B200_E_UNSUPPORTED,
                "spectral_terms: F=%d bins exceed the %d per frame supported", F, st_::kMaxBins);
-  DDSP_REQUIRE_SAME_OR_DISJOINT("spectral_terms", grad_value, extent(B, T, 2 * F), stft_target,
-                                extent(B, T, 2 * F));
-  DDSP_REQUIRE_SAME_OR_DISJOINT("spectral_terms", grad_value, extent(B, T, 2 * F), stft_value, extent(B, T, 2 * F));
+  int rc = check_overlap("spectral_terms",
+                         {DDSP_OUT(grad_value, extent(B, T, 2 * F), stft_target, stft_value)},
+                         {DDSP_IN(stft_target, extent(B, T, 2 * F)),
+                          DDSP_IN(stft_value, extent(B, T, 2 * F))});
+  if (rc) return rc;
   if (B == 0) return 0;
   // per-term weight / element count; delta_time has none when T = 1
   const double counts[5] = {(double)B * T * F, (double)B * (T - 1) * F,
@@ -116,14 +120,11 @@ int ddsp_b200_spectral_terms(const float* stft_target, const float* stft_value,
   const int rows = st_::tile_rows(T, F);
   const size_t smem = st_::tile_smem(rows, F, terms);
   st_::Kernel kern = st_::pick<1>(terms, loss_type == DDSP_B200_LOSS_L2);
-  int rc = set_smem(kern, smem, "spectral_terms");
-  if (rc) return rc;
   dim3 grid((unsigned)((T + rows - 1) / rows), B);
-  kern<<<grid, st_::kThreads, smem, (cudaStream_t)stream>>>(
-      reinterpret_cast<const float2*>(stft_target), reinterpret_cast<const float2*>(stft_value),
-      reinterpret_cast<float2*>(grad_value), sums, T, F, rows, k);
-  DDSP_CHECK_LAUNCH("spectral_terms");
-  return 0;
+  return launch("spectral_terms", kern, grid, st_::kThreads, smem, (cudaStream_t)stream,
+                reinterpret_cast<const float2*>(stft_target),
+                reinterpret_cast<const float2*>(stft_value),
+                reinterpret_cast<float2*>(grad_value), sums, T, F, rows, k);
 }
 
 // ---- loudness and RMS power ----------------------------------------------------
@@ -204,8 +205,10 @@ int ddsp_b200_loudness_forward(const float* audio, const float* weights, float* 
   ld_::LoudParams p;
   int rc = loud_check("loudness_forward", B, N, n_frames, n_fft, hop, padding, &p);
   if (rc || B == 0 || n_frames == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("loudness_forward", loudness, extent(B, n_frames), audio, extent(B, N));
-  DDSP_REQUIRE_DISJOINT("loudness_forward", loudness, extent(B, n_frames), weights, extent(n_fft / 2 + 1));
+  rc = check_overlap("loudness_forward", {DDSP_OUT(loudness, extent(B, n_frames))},
+                     {DDSP_IN(audio, extent(B, N)),
+                      DDSP_IN(weights, extent(n_fft / 2 + 1))});
+  if (rc) return rc;
   p.audio = audio; p.weights = weights;
   db_params(&p, range_db, ref_db);
   const int warps = ld_warps(n_fft);
@@ -215,13 +218,9 @@ int ddsp_b200_loudness_forward(const float* audio, const float* weights, float* 
     per_cta /= 2;
   const int span = (int)((int64_t)(per_cta - 1) * hop + n_fft);
   const size_t smem = ld_fwd_smem(p.M, warps, span);
-  rc = set_smem(ld_::loudness_kernel, smem, "loudness_forward");
-  if (rc) return rc;
   dim3 grid((unsigned)((n_frames + per_cta - 1) / per_cta), B);
-  ld_::loudness_kernel<<<grid, 32 * warps, smem, (cudaStream_t)stream>>>(p, loudness, per_cta,
-                                                                         span);
-  DDSP_CHECK_LAUNCH("loudness_forward");
-  return 0;
+  return launch("loudness_forward", ld_::loudness_kernel, grid, 32 * warps, smem,
+                (cudaStream_t)stream, p, loudness, per_cta, span);
 }
 
 int ddsp_b200_loudness_backward(const float* audio, const float* weights,
@@ -237,13 +236,9 @@ int ddsp_b200_loudness_backward(const float* audio, const float* weights,
   db_params(&p, range_db, ref_db);
   const int warps = ld_warps(n_fft), own = ld_own(n_fft);
   const size_t smem = ld_bwd_smem(p.M, warps, own);
-  rc = set_smem(ld_::loudness_backward_kernel, smem, "loudness_backward");
-  if (rc) return rc;
   dim3 grid((unsigned)((N + own - 1) / own), B);
-  ld_::loudness_backward_kernel<<<grid, 32 * warps, smem, (cudaStream_t)stream>>>(
-      p, grad_loudness, grad_audio, own);
-  DDSP_CHECK_LAUNCH("loudness_backward");
-  return 0;
+  return launch("loudness_backward", ld_::loudness_backward_kernel, grid, 32 * warps, smem,
+                (cudaStream_t)stream, p, grad_loudness, grad_audio, own);
 }
 
 int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n_frames,
@@ -254,16 +249,15 @@ int ddsp_b200_rms_power(const float* audio, float* power_db, int B, int N, int n
   int pad_left = 0;
   int rc = framing_check("rms_power", B, N, n_frames, frame_size, hop, padding, &pad_left);
   if (rc || B == 0 || n_frames == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("rms_power", power_db, extent(B, n_frames), audio, extent(B, N));
+  rc = check_overlap("rms_power", {DDSP_OUT(power_db, extent(B, n_frames))},
+                     {DDSP_IN(audio, extent(B, N))});
+  if (rc) return rc;
   ld_::LoudParams d;
   db_params(&d, range_db, ref_db);
   const int64_t total = (int64_t)B * n_frames;
-  ld_::rms_power_kernel<<<grid_for(total * 32, ld_::kRmsThreads), ld_::kRmsThreads, 0,
-                          (cudaStream_t)stream>>>(audio, power_db, N, n_frames, total,
-                                                  frame_size, hop, pad_left, in_db, d.pmin,
-                                                  d.range_db, d.ref_db);
-  DDSP_CHECK_LAUNCH("rms_power");
-  return 0;
+  return launch("rms_power", ld_::rms_power_kernel, grid_for(total * 32, ld_::kRmsThreads),
+                ld_::kRmsThreads, 0, (cudaStream_t)stream, audio, power_db, N, n_frames,
+                total, frame_size, hop, pad_left, in_db, d.pmin, d.range_db, d.ref_db);
 }
 
 // ---- CREPE: frames, Viterbi path, f0 and confidence ------------------------------
@@ -291,14 +285,15 @@ static int crepe_loss_frames(const float* audio, float* frames, int B, int N, in
   DDSP_REQUIRE((audio || N == 0 || B == 0) && (frames || n_frames == 0 || B == 0),
                DDSP_B200_E_INVALID, "crepe_frames: null pointer");
   if (B == 0 || n_frames == 0) return 0;
-  DDSP_REQUIRE_DISJOINT("crepe_frames", frames, extent(B, n_frames, crepe_::kFrame), audio, extent(B, N));
+  rc = check_overlap("crepe_frames",
+                     {DDSP_OUT(frames, extent(B, n_frames, crepe_::kFrame))},
+                     {DDSP_IN(audio, extent(B, N))});
+  if (rc) return rc;
   const int64_t total = (int64_t)B * n_frames;
   const int threads = 32 * crepe_::kFrameWarps;
-  crepe_::crepe_frames_kernel<true><<<grid_for(total * 32, threads, 16), threads, 0,
-                                      (cudaStream_t)stream>>>(audio, frames, N, n_frames,
-                                                              total, hop, pad_left);
-  DDSP_CHECK_LAUNCH("crepe_frames");
-  return 0;
+  return launch("crepe_frames", crepe_::crepe_frames_kernel<true>,
+                grid_for(total * 32, threads, 16), threads, 0, (cudaStream_t)stream, audio,
+                frames, N, n_frames, total, hop, pad_left);
 }
 
 int ddsp_b200_crepe_frames(const float* audio, float* frames, int B, int N, int n_frames,
@@ -315,14 +310,15 @@ int ddsp_b200_crepe_frames(const float* audio, float* frames, int B, int N, int 
   int rc = framing_check("crepe_frames", B > 0, N, n_frames, crepe_::kFrame, hop, padding,
                          &pad_left);
   if (rc || B == 0 || n_frames == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("crepe_frames", frames, extent(B, n_frames, crepe_::kFrame), audio, extent(B, N));
+  rc = check_overlap("crepe_frames",
+                     {DDSP_OUT(frames, extent(B, n_frames, crepe_::kFrame))},
+                     {DDSP_IN(audio, extent(B, N))});
+  if (rc) return rc;
   const int64_t total = (int64_t)B * n_frames;
   const int threads = 32 * crepe_::kFrameWarps;
-  crepe_::crepe_frames_kernel<false><<<grid_for(total * 32, threads, 16), threads, 0,
-                                       (cudaStream_t)stream>>>(audio, frames, N, n_frames,
-                                                               total, hop, pad_left);
-  DDSP_CHECK_LAUNCH("crepe_frames");
-  return 0;
+  return launch("crepe_frames", crepe_::crepe_frames_kernel<false>,
+                grid_for(total * 32, threads, 16), threads, 0, (cudaStream_t)stream, audio,
+                frames, N, n_frames, total, hop, pad_left);
 }
 
 int ddsp_b200_crepe_frames_backward(const float* audio, const float* grad_frames,
@@ -335,28 +331,25 @@ int ddsp_b200_crepe_frames_backward(const float* audio, const float* grad_frames
   DDSP_REQUIRE(B == 0 || N == 0 || (audio && grad_audio && (grad_frames || n_frames == 0)),
                DDSP_B200_E_INVALID, "crepe_frames_backward: null pointer");
   if (B == 0 || N == 0) return 0;
-  DDSP_REQUIRE_DISJOINT("crepe_frames_backward", grad_audio, extent(B, N), audio, extent(B, N));
-  DDSP_REQUIRE_DISJOINT("crepe_frames_backward", grad_audio, extent(B, N), grad_frames,
-                        extent(B, n_frames, crepe_::kFrame));
+  rc = check_overlap("crepe_frames_backward", {DDSP_OUT(grad_audio, extent(B, N))},
+                     {DDSP_IN(audio, extent(B, N)),
+                      DDSP_IN(grad_frames, extent(B, n_frames, crepe_::kFrame))});
+  if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   if (hop >= crepe_::kFrame && n_frames > 0) {
     const int64_t total = (int64_t)B * n_frames;
     const int threads = 32 * crepe_::kDisjointWarps;
-    crepe_::crepe_frames_bwd_disjoint_kernel<<<grid_for(total * 32, threads, 16), threads, 0,
-                                               s>>>(audio, grad_frames, grad_audio, N,
-                                                    n_frames, total, hop, pad_left);
-  } else {
-    const int spans = (N + crepe_::kBwdOwn - 1) / crepe_::kBwdOwn;
-    const int64_t total = (int64_t)B * spans;
-    const size_t smem = sizeof(crepe_::FrameGrad) * crepe_::bwd_frames_per_span(hop);
-    rc = set_smem(crepe_::crepe_frames_bwd_overlap_kernel, smem, "crepe_frames_backward");
-    if (rc) return rc;
-    const int blocks = (int)std::min<int64_t>(total, 16ll * num_sms());
-    crepe_::crepe_frames_bwd_overlap_kernel<<<blocks, crepe_::kBwdThreads, smem, s>>>(
-        audio, grad_frames, grad_audio, N, n_frames, spans, total, hop, pad_left);
+    return launch("crepe_frames_backward", crepe_::crepe_frames_bwd_disjoint_kernel,
+                  grid_for(total * 32, threads, 16), threads, 0, s, audio, grad_frames,
+                  grad_audio, N, n_frames, total, hop, pad_left);
   }
-  DDSP_CHECK_LAUNCH("crepe_frames_backward");
-  return 0;
+  const int spans = (N + crepe_::kBwdOwn - 1) / crepe_::kBwdOwn;
+  const int64_t total = (int64_t)B * spans;
+  const size_t smem = sizeof(crepe_::FrameGrad) * crepe_::bwd_frames_per_span(hop);
+  const int blocks = (int)std::min<int64_t>(total, 16ll * num_sms());
+  return launch("crepe_frames_backward", crepe_::crepe_frames_bwd_overlap_kernel, blocks,
+                crepe_::kBwdThreads, smem, s, audio, grad_frames, grad_audio, N, n_frames,
+                spans, total, hop, pad_left);
 }
 
 size_t ddsp_b200_crepe_viterbi_workspace_bytes(int B, int T) {
@@ -376,10 +369,9 @@ int ddsp_b200_crepe_viterbi(const float* activations, int* centers, void* worksp
   DDSP_REQUIRE(((uintptr_t)workspace & 3) == 0, DDSP_B200_E_INVALID,
                "crepe_viterbi: workspace must be 4-byte aligned");
   if (B == 0) return 0;
-  crepe_::crepe_viterbi_kernel<<<B, crepe_::kThreads, 0, (cudaStream_t)stream>>>(
-      activations, centers, T, static_cast<uint32_t*>(workspace));
-  DDSP_CHECK_LAUNCH("crepe_viterbi");
-  return 0;
+  return launch("crepe_viterbi", crepe_::crepe_viterbi_kernel, B, crepe_::kThreads, 0,
+                (cudaStream_t)stream, activations, centers, T,
+                static_cast<uint32_t*>(workspace));
 }
 
 int ddsp_b200_crepe_decode(const float* activations, const int* centers, float* f0,
@@ -388,14 +380,13 @@ int ddsp_b200_crepe_decode(const float* activations, const int* centers, float* 
   DDSP_REQUIRE(M == 0 || (activations && f0 && confidence), DDSP_B200_E_INVALID,
                "crepe_decode: null pointer");
   if (M == 0) return 0;
-  DDSP_REQUIRE_DISJOINT("crepe_decode", f0, extent(M), activations, extent(M, DDSP_B200_CREPE_BINS));
-  DDSP_REQUIRE_DISJOINT("crepe_decode", confidence, extent(M), activations, extent(M, DDSP_B200_CREPE_BINS));
+  int rc = check_overlap("crepe_decode", {DDSP_OUT(f0, extent(M)),
+                                          DDSP_OUT(confidence, extent(M))},
+                         {DDSP_IN(activations, extent(M, DDSP_B200_CREPE_BINS))});
+  if (rc) return rc;
   const int threads = 32 * crepe_::kDecodeWarps;
-  crepe_::crepe_decode_kernel<<<grid_for(M * 32, threads, 16), threads, 0,
-                                (cudaStream_t)stream>>>(activations, centers, f0,
-                                                        confidence, M);
-  DDSP_CHECK_LAUNCH("crepe_decode");
-  return 0;
+  return launch("crepe_decode", crepe_::crepe_decode_kernel, grid_for(M * 32, threads, 16),
+                threads, 0, (cudaStream_t)stream, activations, centers, f0, confidence, M);
 }
 
 // ---- mel, log-mel and MFCC -------------------------------------------------------
@@ -480,8 +471,9 @@ int ddsp_b200_mel_forward(const float* audio, const float* window, const void* m
   int rc = mel_check("mel_forward", B, N, n_frames, fft_size, fft_length, hop, pad_end, bins,
                      n_out, mode, &p);
   if (rc || B == 0 || n_frames == 0 || n_out == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("mel_forward", out, extent(B, n_frames, n_out), audio, extent(B, N));
-  DDSP_REQUIRE_DISJOINT("mel_forward", out, extent(B, n_frames, n_out), window, extent(fft_size));
+  rc = check_overlap("mel_forward", {DDSP_OUT(out, extent(B, n_frames, n_out))},
+                     {DDSP_IN(audio, extent(B, N)), DDSP_IN(window, extent(fft_size))});
+  if (rc) return rc;
   mel_tables(&p, audio, window, mel_table, fft_length, bins);
   const int warps = mel_warps(p.M, bins, mode);
   const size_t fixed = mel_fixed_smem(p.M, warps, bins, mode);
@@ -500,12 +492,9 @@ int ddsp_b200_mel_forward(const float* audio, const float* window, const void* m
   auto kern = mode == DDSP_B200_MEL      ? mel_::mel_kernel<mel_::kMel>
               : mode == DDSP_B200_LOGMEL ? mel_::mel_kernel<mel_::kLogMel>
                                          : mel_::mel_kernel<mel_::kMfcc>;
-  rc = set_smem(kern, smem, "mel_forward");
-  if (rc) return rc;
   dim3 grid((unsigned)((n_frames + per_cta - 1) / per_cta), B);
-  kern<<<grid, 32 * warps, smem, (cudaStream_t)stream>>>(p, out, per_cta, span);
-  DDSP_CHECK_LAUNCH("mel_forward");
-  return 0;
+  return launch("mel_forward", kern, grid, 32 * warps, smem, (cudaStream_t)stream, p, out,
+                per_cta, span);
 }
 
 int ddsp_b200_mel_backward(const float* audio, const float* window, const void* mel_table,
@@ -526,12 +515,9 @@ int ddsp_b200_mel_backward(const float* audio, const float* window, const void* 
   auto kern = mode == DDSP_B200_MEL      ? mel_::mel_backward_kernel<mel_::kMel>
               : mode == DDSP_B200_LOGMEL ? mel_::mel_backward_kernel<mel_::kLogMel>
                                          : mel_::mel_backward_kernel<mel_::kMfcc>;
-  rc = set_smem(kern, smem, "mel_backward");
-  if (rc) return rc;
   dim3 grid((unsigned)((N + own - 1) / own), B);
-  kern<<<grid, 32 * warps, smem, (cudaStream_t)stream>>>(p, grad_out, grad_audio, own);
-  DDSP_CHECK_LAUNCH("mel_backward");
-  return 0;
+  return launch("mel_backward", kern, grid, 32 * warps, smem, (cudaStream_t)stream, p,
+                grad_out, grad_audio, own);
 }
 
 }  // extern "C"

@@ -37,19 +37,16 @@ int ddsp_b200_harmonic_controls(const float* amps_in, const float* hd_in,
   if (rows == 0) return 0;
   DDSP_REQUIRE(rows < (1ll << 31) / 32, DDSP_B200_E_INVALID,
                "harmonic_controls: B*F too large");
-  DDSP_REQUIRE_DISJOINT("harmonic_controls", amps_out, extent(B, F), hd_in, extent(B, F, K));
-  DDSP_REQUIRE_DISJOINT("harmonic_controls", amps_out, extent(B, F), f0_hz, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("harmonic_controls", hd_out, extent(B, F, K), amps_in, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("harmonic_controls", hd_out, extent(B, F, K), f0_hz, extent(B, F));
-  DDSP_REQUIRE_SAME_OR_DISJOINT("harmonic_controls", amps_out, extent(B, F), amps_in, extent(B, F));
-  DDSP_REQUIRE_SAME_OR_DISJOINT("harmonic_controls", hd_out, extent(B, F, K), hd_in, extent(B, F, K));
+  int rc = check_overlap("harmonic_controls", {DDSP_OUT(amps_out, extent(B, F), amps_in),
+                                               DDSP_OUT(hd_out, extent(B, F, K), hd_in)},
+                         {DDSP_IN(amps_in, extent(B, F)), DDSP_IN(hd_in, extent(B, F, K)),
+                          DDSP_IN(f0_hz, extent(B, F))});
+  if (rc) return rc;
   const int threads = 256;
   const int blocks = (int)((rows * 32 + threads - 1) / threads);
-  harmonic_controls_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(
-      amps_in, hd_in, f0_hz, amps_out, hd_out, (int)rows, K,
-      sample_rate * 0.5f, flags);
-  DDSP_CHECK_LAUNCH("harmonic_controls");
-  return 0;
+  return launch("harmonic_controls", harmonic_controls_kernel, blocks, threads, 0,
+                (cudaStream_t)stream, amps_in, hd_in, f0_hz, amps_out, hd_out, (int)rows, K,
+                sample_rate * 0.5f, flags);
 }
 
 int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
@@ -79,9 +76,10 @@ int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
   DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
                "harmonic_forward: B=%d exceeds the 65535 grid limit", B);
 
-  DDSP_REQUIRE_DISJOINT("harmonic_forward", audio, extent(B, N), f0_hz, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("harmonic_forward", audio, extent(B, N), amps, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("harmonic_forward", audio, extent(B, N), hd, extent(B, F, K));
+  rc = check_overlap("harmonic_forward", {DDSP_OUT(audio, extent(B, N))},
+                     {DDSP_IN(f0_hz, extent(B, F)), DDSP_IN(amps, extent(B, F)),
+                      DDSP_IN(hd, extent(B, F, K))});
+  if (rc) return rc;
   HarmonicParams p = harm_params(f0_hz, amps, hd, audio, B, F, K, N, sample_rate,
                                  amp_method);
   p.accumulate = accumulate;
@@ -103,11 +101,8 @@ int ddsp_b200_harmonic_forward(const float* f0_hz, const float* amps,
   const size_t smem = harm_smem_bytes(p.FT, p.Kp);
   auto kern = phase_mode == DDSP_B200_PHASE_DIRECT ? harmonic_generic_kernel<1>
                                                    : harmonic_generic_kernel<0>;
-  rc = set_smem(kern, smem, "harmonic_forward");
-  if (rc) return rc;
-  kern<<<dim3((F + p.FT - 1) / p.FT, B), kHarmThreads, smem, st>>>(p);
-  DDSP_CHECK_LAUNCH("harmonic_forward");
-  return 0;
+  return launch("harmonic_forward", kern, dim3((F + p.FT - 1) / p.FT, B), kHarmThreads,
+                smem, st, p);
 }
 
 int ddsp_b200_streaming_harmonic_forward(const float* f0_hz, const float* amps,
@@ -133,21 +128,15 @@ int ddsp_b200_streaming_harmonic_forward(const float* f0_hz, const float* amps,
   p.FT = fit_tile("streaming_harmonic_forward", std::max(1, std::min(F, 2048 / p.hop)),
                   K, p.Kp, harm_smem_bytes);
   if (!p.FT) return DDSP_B200_E_UNSUPPORTED;
-  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", audio, extent(B, N), f0_hz, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", audio, extent(B, N), amps, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", audio, extent(B, N), hd, extent(B, F, K));
-  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", audio, extent(B, N), initial_phase, extent(B));
-  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", final_phase, extent(B), f0_hz, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", final_phase, extent(B), amps, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", final_phase, extent(B), hd, extent(B, F, K));
-  DDSP_REQUIRE_DISJOINT("streaming_harmonic_forward", final_phase, extent(B), initial_phase, extent(B));
-  const size_t smem = harm_smem_bytes(p.FT, p.Kp);
-  rc = set_smem(harmonic_generic_kernel<0>, smem, "streaming_harmonic_forward");
+  rc = check_overlap("streaming_harmonic_forward", {DDSP_OUT(audio, extent(B, N)),
+                                                    DDSP_OUT(final_phase, extent(B))},
+                     {DDSP_IN(f0_hz, extent(B, F)), DDSP_IN(amps, extent(B, F)),
+                      DDSP_IN(hd, extent(B, F, K)), DDSP_IN(initial_phase, extent(B))});
   if (rc) return rc;
+  const size_t smem = harm_smem_bytes(p.FT, p.Kp);
   dim3 grid((F + p.FT - 1) / p.FT, B);
-  harmonic_generic_kernel<0><<<grid, kHarmThreads, smem, (cudaStream_t)stream>>>(p);
-  DDSP_CHECK_LAUNCH("streaming_harmonic_forward");
-  return 0;
+  return launch("streaming_harmonic_forward", harmonic_generic_kernel<0>, grid,
+                kHarmThreads, smem, (cudaStream_t)stream, p);
 }
 
 int ddsp_b200_noise_controls(const float* mag_in, float* mag_out, int64_t n,
@@ -156,11 +145,11 @@ int ddsp_b200_noise_controls(const float* mag_in, float* mag_out, int64_t n,
                "noise_controls: null pointer");
   DDSP_REQUIRE(n >= 0, DDSP_B200_E_INVALID, "noise_controls: n < 0");
   if (n == 0) return 0;
-  DDSP_REQUIRE_SAME_OR_DISJOINT("noise_controls", mag_out, extent(n), mag_in, extent(n));
-  noise_controls_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(
-      mag_in, mag_out, n, initial_bias, apply_scale);
-  DDSP_CHECK_LAUNCH("noise_controls");
-  return 0;
+  int rc = check_overlap("noise_controls", {DDSP_OUT(mag_out, extent(n), mag_in)},
+                         {DDSP_IN(mag_in, extent(n))});
+  if (rc) return rc;
+  return launch("noise_controls", noise_controls_kernel, grid_for(n, 256), 256, 0,
+                (cudaStream_t)stream, mag_in, mag_out, n, initial_bias, apply_scale);
 }
 
 int ddsp_b200_harmonic_backward_takes(int B, int F, int N) {
@@ -194,11 +183,8 @@ int ddsp_b200_harmonic_backward(const float* f0_hz, const float* grad_audio,
   const size_t smem = harmonic_backward_smem(p.FT, p.hop);
   auto kern = amp_method == DDSP_B200_AMP_WINDOW ? harmonic_backward_kernel<true>
                                                  : harmonic_backward_kernel<false>;
-  rc = set_smem(kern, smem, "harmonic_backward");
-  if (rc) return rc;
-  kern<<<dim3((F + p.FT - 1) / p.FT, B), kHbThreads, smem, st>>>(p, grad_audio, g0, g1);
-  DDSP_CHECK_LAUNCH("harmonic_backward");
-  return 0;
+  return launch("harmonic_backward", kern, dim3((F + p.FT - 1) / p.FT, B), kHbThreads, smem,
+                st, p, grad_audio, g0, g1);
 }
 
 int ddsp_b200_harmonic_backward_f0(const float* f0_hz, const float* amps,
@@ -232,14 +218,11 @@ int ddsp_b200_harmonic_backward_f0(const float* f0_hz, const float* amps,
   float* sq = reinterpret_cast<float*>(workspace);
   auto kern = amp_method == DDSP_B200_AMP_WINDOW ? harmonic_df0_kernel<true>
                                                  : harmonic_df0_kernel<false>;
-  rc = set_smem(kern, smem, "harmonic_backward_f0");
+  rc = launch("harmonic_backward_f0", kern, dim3((F + p.FT - 1) / p.FT, B), kDf0Threads,
+              smem, st, p, grad_audio, sq);
   if (rc) return rc;
-  kern<<<dim3((F + p.FT - 1) / p.FT, B), kDf0Threads, smem, st>>>(p, grad_audio, sq);
-  DDSP_CHECK_LAUNCH("harmonic_backward_f0");
-  harmonic_df0_finalize<<<(B + 127) / 128, 128, 0, st>>>(sq, d_f0, B, F, p.hop,
-                                                       (float)p.inv_sr);
-  DDSP_CHECK_LAUNCH("harmonic_backward_f0(finalize)");
-  return 0;
+  return launch("harmonic_backward_f0(finalize)", harmonic_df0_finalize, (B + 127) / 128,
+                128, 0, st, sq, d_f0, B, F, p.hop, (float)p.inv_sr);
 }
 
 int ddsp_b200_harmonic_controls_backward(const float* amps_raw, const float* hd_raw,
@@ -257,11 +240,9 @@ int ddsp_b200_harmonic_controls_backward(const float* amps_raw, const float* hd_
                "harmonic_controls_backward: B*F too large");
   const int threads = 256;
   const int blocks = (int)((rows * 32 + threads - 1) / threads);
-  harmonic_controls_backward_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(
-      amps_raw, hd_raw, f0_hz, g0, g1, d_amps_raw, d_hd_raw, (int)rows, F, K,
-      sample_rate * 0.5f, flags);
-  DDSP_CHECK_LAUNCH("harmonic_controls_backward");
-  return 0;
+  return launch("harmonic_controls_backward", harmonic_controls_backward_kernel, blocks,
+                threads, 0, (cudaStream_t)stream, amps_raw, hd_raw, f0_hz, g0, g1,
+                d_amps_raw, d_hd_raw, (int)rows, F, K, sample_rate * 0.5f, flags);
 }
 
 int ddsp_b200_harmonic_controls_vjp(const float* amps_raw, const float* hd_raw,
@@ -279,11 +260,9 @@ int ddsp_b200_harmonic_controls_vjp(const float* amps_raw, const float* hd_raw,
                "harmonic_controls_vjp: B*F too large");
   const int threads = 256;
   const int blocks = (int)((rows * 32 + threads - 1) / threads);
-  harmonic_controls_vjp_kernel<<<blocks, threads, 0, (cudaStream_t)stream>>>(
-      amps_raw, hd_raw, f0_hz, d_amplitudes, d_hd, d_amps_raw, d_hd_raw, (int)rows, K,
-      sample_rate * 0.5f, flags);
-  DDSP_CHECK_LAUNCH("harmonic_controls_vjp");
-  return 0;
+  return launch("harmonic_controls_vjp", harmonic_controls_vjp_kernel, blocks, threads, 0,
+                (cudaStream_t)stream, amps_raw, hd_raw, f0_hz, d_amplitudes, d_hd,
+                d_amps_raw, d_hd_raw, (int)rows, K, sample_rate * 0.5f, flags);
 }
 
 int ddsp_b200_noise_controls_backward(const float* mags_raw, const float* d_mags,
@@ -293,10 +272,8 @@ int ddsp_b200_noise_controls_backward(const float* mags_raw, const float* d_mags
                "noise_controls_backward: null pointer");
   DDSP_REQUIRE(n >= 0, DDSP_B200_E_INVALID, "noise_controls_backward: n < 0");
   if (n == 0) return 0;
-  noise_controls_backward_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(
-      mags_raw, d_mags, d_raw, n, initial_bias);
-  DDSP_CHECK_LAUNCH("noise_controls_backward");
-  return 0;
+  return launch("noise_controls_backward", noise_controls_backward_kernel, grid_for(n, 256),
+                256, 0, (cudaStream_t)stream, mags_raw, d_mags, d_raw, n, initial_bias);
 }
 
 #ifdef DDSP_HV4_TIMING

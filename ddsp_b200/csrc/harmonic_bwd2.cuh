@@ -264,9 +264,7 @@ inline int launch_harmonic_backward2(HarmonicParams p, const float* grad, float*
   dim3 grid((p.F + FW * NW - 1) / (FW * NW), p.B);
   auto kern = p.amp_method == DDSP_B200_AMP_WINDOW ? harmonic_backward2_kernel<true>
                                                    : harmonic_backward2_kernel<false>;
-  kern<<<grid, NT, smem, st>>>(p, grad, g0, g1, FW);
-  DDSP_CHECK_LAUNCH("harmonic_backward(v2)");
-  return 0;
+  return launch("harmonic_backward(v2)", kern, grid, NT, smem, st, p, grad, g0, g1, FW);
 }
 
 }  // namespace ddsp

@@ -772,11 +772,7 @@ int launch_harmonic_v4(HarmonicParams p, cudaStream_t st) {
   const bool win = p.amp_method == DDSP_B200_AMP_WINDOW;
   auto kern = p.hop == 64 ? (win ? harmonic_v4_kernel<true, 64> : harmonic_v4_kernel<false, 64>)
                           : (win ? harmonic_v4_kernel<true, 0> : harmonic_v4_kernel<false, 0>);
-  int rc = set_smem(kern, smem, "harmonic_forward(v4)");
-  if (rc) return rc;
-  kern<<<grid, NT, smem, st>>>(p, use_tma, FW);
-  DDSP_CHECK_LAUNCH("harmonic_forward(v4)");
-  return 0;
+  return launch("harmonic_forward(v4)", kern, grid, NT, smem, st, p, use_tma, FW);
 }
 
 }  // namespace ddsp

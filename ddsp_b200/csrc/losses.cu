@@ -47,17 +47,14 @@ int ddsp_b200_mixture_nll_forward(const float* x, const float* mu, const float* 
   int64_t rows = 0;
   int rc = mix_check("mixture_nll_forward", B, T, Q, J, scale, &p, &rows);
   if (rc || rows == 0 || Q == 0 || J == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("mixture_nll_forward", nll, extent(rows, Q), x, extent(rows, Q));
-  DDSP_REQUIRE_DISJOINT("mixture_nll_forward", nll, extent(rows, Q), mu, extent(rows, J));
-  DDSP_REQUIRE_DISJOINT("mixture_nll_forward", nll, extent(rows, Q), lw, extent(rows, J));
+  rc = check_overlap("mixture_nll_forward", {DDSP_OUT(nll, extent(rows, Q))},
+                     {DDSP_IN(x, extent(rows, Q)), DDSP_IN(mu, extent(rows, J)),
+                      DDSP_IN(lw, extent(rows, J))});
+  if (rc) return rc;
   p.x = x; p.mu = mu; p.lw = lw;
   const size_t smem = sizeof(float) * 2 * (size_t)J;
-  rc = set_smem(cons_::mixture_nll_kernel, smem, "mixture_nll_forward");
-  if (rc) return rc;
-  cons_::mixture_nll_kernel<<<(unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream>>>(
-      p, nll);
-  DDSP_CHECK_LAUNCH("mixture_nll_forward");
-  return 0;
+  return launch("mixture_nll_forward", cons_::mixture_nll_kernel, (unsigned)rows,
+                cons_::kThreads, smem, (cudaStream_t)stream, p, nll);
 }
 
 int ddsp_b200_mixture_nll_backward(const float* x, const float* mu, const float* lw,
@@ -72,12 +69,8 @@ int ddsp_b200_mixture_nll_backward(const float* x, const float* mu, const float*
   if (rc || rows == 0 || Q == 0 || J == 0) return rc;
   p.x = x; p.mu = mu; p.lw = lw;
   const size_t smem = sizeof(float) * (4 * (size_t)J + 5 * cons_::kChunk);
-  rc = set_smem(cons_::mixture_nll_backward_kernel, smem, "mixture_nll_backward");
-  if (rc) return rc;
-  cons_::mixture_nll_backward_kernel<<<(unsigned)rows, cons_::kThreads, smem,
-                                       (cudaStream_t)stream>>>(p, grad, dx, dmu, dlw);
-  DDSP_CHECK_LAUNCH("mixture_nll_backward");
-  return 0;
+  return launch("mixture_nll_backward", cons_::mixture_nll_backward_kernel, (unsigned)rows,
+                cons_::kThreads, smem, (cudaStream_t)stream, p, grad, dx, dmu, dlw);
 }
 
 // Half-width W of the comb window: the smallest W for which the terms |k - k0| > W
@@ -126,17 +119,14 @@ int ddsp_b200_comb_nll_forward(const float* f0, const float* f, const float* a, 
   int64_t rows = 0;
   int rc = comb_check("comb_nll_forward", B, T, C, P, G, scale, &p, &rows);
   if (rc || rows == 0 || C == 0 || P == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("comb_nll_forward", out, extent(rows, C), f0, extent(rows, C));
-  DDSP_REQUIRE_DISJOINT("comb_nll_forward", out, extent(rows, C), f, extent(rows, P));
-  DDSP_REQUIRE_DISJOINT("comb_nll_forward", out, extent(rows, C), a, extent(rows, P));
+  rc = check_overlap("comb_nll_forward", {DDSP_OUT(out, extent(rows, C))},
+                     {DDSP_IN(f0, extent(rows, C)), DDSP_IN(f, extent(rows, P)),
+                      DDSP_IN(a, extent(rows, P))});
+  if (rc) return rc;
   p.f0 = f0; p.f = f; p.a = a;
   const size_t smem = sizeof(float) * (2 * (size_t)P + C + 1);
-  rc = set_smem(cons_::comb_nll_kernel, smem, "comb_nll_forward");
-  if (rc) return rc;
-  cons_::comb_nll_kernel<<<(unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream>>>(
-      p, out);
-  DDSP_CHECK_LAUNCH("comb_nll_forward");
-  return 0;
+  return launch("comb_nll_forward", cons_::comb_nll_kernel, (unsigned)rows, cons_::kThreads,
+                smem, (cudaStream_t)stream, p, out);
 }
 
 int ddsp_b200_comb_nll_backward(const float* f0, const float* f, const float* a,
@@ -152,12 +142,8 @@ int ddsp_b200_comb_nll_backward(const float* f0, const float* f, const float* a,
   if (rc || rows == 0 || C == 0 || P == 0) return rc;
   p.f0 = f0; p.f = f; p.a = a;
   const size_t smem = sizeof(float) * (2 * (size_t)P + 3 * (size_t)C + 1);
-  rc = set_smem(cons_::comb_nll_backward_kernel, smem, "comb_nll_backward");
-  if (rc) return rc;
-  cons_::comb_nll_backward_kernel<<<(unsigned)rows, cons_::kThreads, smem,
-                                    (cudaStream_t)stream>>>(p, grad, d_f0, d_f, d_a);
-  DDSP_CHECK_LAUNCH("comb_nll_backward");
-  return 0;
+  return launch("comb_nll_backward", cons_::comb_nll_backward_kernel, (unsigned)rows,
+                cons_::kThreads, smem, (cudaStream_t)stream, p, grad, d_f0, d_f, d_a);
 }
 
 // ---- core.sinusoidal_to_harmonic ---------------------------------------------------
@@ -194,20 +180,15 @@ int ddsp_b200_sinusoidal_to_harmonic(const float* sin_amps, const float* sin_fre
   int rc = s2h_check("sinusoidal_to_harmonic", B, T, S, K, width, sample_rate, normalize, &p,
                      &rows);
   if (rc || rows == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_amp, extent(rows), sin_amps, extent(rows, S));
-  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_amp, extent(rows), sin_freqs, extent(rows, S));
-  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_amp, extent(rows), f0_hz, extent(rows));
-  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_dist, extent(rows, K), sin_amps, extent(rows, S));
-  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_dist, extent(rows, K), sin_freqs, extent(rows, S));
-  DDSP_REQUIRE_DISJOINT("sinusoidal_to_harmonic", harm_dist, extent(rows, K), f0_hz, extent(rows));
+  rc = check_overlap("sinusoidal_to_harmonic", {DDSP_OUT(harm_amp, extent(rows)),
+                                                DDSP_OUT(harm_dist, extent(rows, K))},
+                     {DDSP_IN(sin_amps, extent(rows, S)),
+                      DDSP_IN(sin_freqs, extent(rows, S)), DDSP_IN(f0_hz, extent(rows))});
+  if (rc) return rc;
   p.a = sin_amps; p.f = sin_freqs; p.f0 = f0_hz;
   const size_t smem = sizeof(float) * (2 * (size_t)S + cons_::kThreads + 1);
-  rc = set_smem(cons_::sin_to_harm_kernel, smem, "sinusoidal_to_harmonic");
-  if (rc) return rc;
-  cons_::sin_to_harm_kernel<<<(unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream>>>(
-      p, harm_amp, harm_dist);
-  DDSP_CHECK_LAUNCH("sinusoidal_to_harmonic");
-  return 0;
+  return launch("sinusoidal_to_harmonic", cons_::sin_to_harm_kernel, (unsigned)rows,
+                cons_::kThreads, smem, (cudaStream_t)stream, p, harm_amp, harm_dist);
 }
 
 int ddsp_b200_sinusoidal_to_harmonic_backward(
@@ -227,13 +208,9 @@ int ddsp_b200_sinusoidal_to_harmonic_backward(
   p.a = sin_amps; p.f = sin_freqs; p.f0 = f0_hz;
   const size_t smem =
       sizeof(float) * (4 * (size_t)S + 4 * cons_::kHarmChunk + cons_::kThreads + 1);
-  rc = set_smem(cons_::sin_to_harm_backward_kernel, smem, "sinusoidal_to_harmonic_backward");
-  if (rc) return rc;
-  cons_::sin_to_harm_backward_kernel<<<(unsigned)rows, cons_::kThreads, smem,
-                                       (cudaStream_t)stream>>>(
-      p, grad_amp, grad_dist, d_sin_amps, d_sin_freqs, d_f0_hz);
-  DDSP_CHECK_LAUNCH("sinusoidal_to_harmonic_backward");
-  return 0;
+  return launch("sinusoidal_to_harmonic_backward", cons_::sin_to_harm_backward_kernel,
+                (unsigned)rows, cons_::kThreads, smem, (cudaStream_t)stream, p, grad_amp,
+                grad_dist, d_sin_amps, d_sin_freqs, d_f0_hz);
 }
 
 // ---- losses.HmmTranscriber -----------------------------------------------------------
@@ -273,13 +250,12 @@ int ddsp_b200_hmm_log_prob(const float* obs, const float* loc, const float* scal
   hmm_::Params p;
   int rc = hmm_check("hmm_log_prob", obs, loc, scale, B, T, K, hold, other, &p);
   if (rc || B == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("hmm_log_prob", log_prob, extent(B), obs, extent(B, T, 2));
-  DDSP_REQUIRE_DISJOINT("hmm_log_prob", log_prob, extent(B), loc, extent(K, 2));
-  DDSP_REQUIRE_DISJOINT("hmm_log_prob", log_prob, extent(B), scale, extent(K, 2));
-  hmm_::hmm_log_prob_kernel<<<(unsigned)B, hmm_threads(K), 0, (cudaStream_t)stream>>>(
-      p, log_prob);
-  DDSP_CHECK_LAUNCH("hmm_log_prob");
-  return 0;
+  rc = check_overlap("hmm_log_prob", {DDSP_OUT(log_prob, extent(B))},
+                     {DDSP_IN(obs, extent(B, T, 2)), DDSP_IN(loc, extent(K, 2)),
+                      DDSP_IN(scale, extent(K, 2))});
+  if (rc) return rc;
+  return launch("hmm_log_prob", hmm_::hmm_log_prob_kernel, (unsigned)B, hmm_threads(K), 0,
+                (cudaStream_t)stream, p, log_prob);
 }
 
 int ddsp_b200_hmm_log_prob_backward(const float* obs, const float* loc, const float* scale,
@@ -296,12 +272,9 @@ int ddsp_b200_hmm_log_prob_backward(const float* obs, const float* loc, const fl
                seg, hmm_::kSegFloats);
   if (B == 0) return 0;
   const size_t smem = sizeof(float) * (size_t)seg * K;
-  rc = set_smem(hmm_::hmm_backward_kernel, smem, "hmm_log_prob_backward");
-  if (rc) return rc;
-  hmm_::hmm_backward_kernel<<<(unsigned)B, hmm_threads(K), smem, (cudaStream_t)stream>>>(
-      p, seg, grad, reinterpret_cast<float2*>(d_obs), checkpoints);
-  DDSP_CHECK_LAUNCH("hmm_log_prob_backward");
-  return 0;
+  return launch("hmm_log_prob_backward", hmm_::hmm_backward_kernel, (unsigned)B,
+                hmm_threads(K), smem, (cudaStream_t)stream, p, seg, grad,
+                reinterpret_cast<float2*>(d_obs), checkpoints);
 }
 
 // Shared bytes of the Viterbi back pointers of T steps of K states.
@@ -326,12 +299,8 @@ int ddsp_b200_hmm_viterbi(const float* obs, const float* loc, const float* scale
                "hmm_viterbi: T=%d steps of K=%d states need %zu B of back pointers, more "
                "than the %zu supported", T, K, smem, hmm_::kViterbiBytes);
   if (B == 0) return 0;
-  rc = set_smem(hmm_::hmm_viterbi_kernel, smem, "hmm_viterbi");
-  if (rc) return rc;
-  hmm_::hmm_viterbi_kernel<<<(unsigned)B, hmm_threads(K), smem, (cudaStream_t)stream>>>(
-      p, path);
-  DDSP_CHECK_LAUNCH("hmm_viterbi");
-  return 0;
+  return launch("hmm_viterbi", hmm_::hmm_viterbi_kernel, (unsigned)B, hmm_threads(K), smem,
+                (cudaStream_t)stream, p, path);
 }
 
 // ---- losses.wasserstein_distance ------------------------------------------------------
@@ -361,19 +330,15 @@ int ddsp_b200_wasserstein_forward(const float* u, const float* v, const float* w
   ws_::Params wp;
   int rc = ws_check("wasserstein_forward", R, Nu, Nv, p, &wp);
   if (rc || empty) return rc;
-  DDSP_REQUIRE_DISJOINT("wasserstein_forward", out, extent(R), u, extent(R, Nu));
-  DDSP_REQUIRE_DISJOINT("wasserstein_forward", out, extent(R), v, extent(R, Nv));
-  DDSP_REQUIRE_DISJOINT("wasserstein_forward", out, extent(R), wu, extent(R, Nu));
-  DDSP_REQUIRE_DISJOINT("wasserstein_forward", out, extent(R), wv, extent(R, Nv));
+  rc = check_overlap("wasserstein_forward", {DDSP_OUT(out, extent(R))},
+                     {DDSP_IN(u, extent(R, Nu)), DDSP_IN(v, extent(R, Nv)),
+                      DDSP_IN(wu, extent(R, Nu)), DDSP_IN(wv, extent(R, Nv))});
+  if (rc) return rc;
   wp.u = u; wp.v = v; wp.wu = wu; wp.wv = wv;
   const int m = ws_::padded(Nu + Nv);
   const size_t smem = ws_::smem_bytes(m);
-  rc = set_smem(ws_::wasserstein_kernel, smem, "wasserstein_forward");
-  if (rc) return rc;
-  ws_::wasserstein_kernel<<<(unsigned)R, ws_::threads_for(m), smem, (cudaStream_t)stream>>>(
-      wp, out);
-  DDSP_CHECK_LAUNCH("wasserstein_forward");
-  return 0;
+  return launch("wasserstein_forward", ws_::wasserstein_kernel, (unsigned)R,
+                ws_::threads_for(m), smem, (cudaStream_t)stream, wp, out);
 }
 
 int ddsp_b200_wasserstein_backward(const float* u, const float* v, const float* wu,
@@ -389,12 +354,9 @@ int ddsp_b200_wasserstein_backward(const float* u, const float* v, const float* 
   wp.u = u; wp.v = v; wp.wu = wu; wp.wv = wv;
   const int m = ws_::padded(Nu + Nv);
   const size_t smem = ws_::smem_bytes(m);
-  rc = set_smem(ws_::wasserstein_backward_kernel, smem, "wasserstein_backward");
-  if (rc) return rc;
-  ws_::wasserstein_backward_kernel<<<(unsigned)R, ws_::threads_for(m), smem,
-                                     (cudaStream_t)stream>>>(wp, grad, du, dv, dwu, dwv);
-  DDSP_CHECK_LAUNCH("wasserstein_backward");
-  return 0;
+  return launch("wasserstein_backward", ws_::wasserstein_backward_kernel, (unsigned)R,
+                ws_::threads_for(m), smem, (cudaStream_t)stream, wp, grad, du, dv, dwu,
+                dwv);
 }
 
 // ---- nn.get_note_mask, get_note_moments, pool_over_notes ---------------------------------
@@ -419,8 +381,10 @@ int ddsp_b200_note_mask(const float* q, const float* onset, float* mask, void* w
                "note_mask: workspace of %zu B is smaller than the %zu B needed",
                workspace_bytes, need);
   if (empty) return 0;
-  DDSP_REQUIRE_DISJOINT("note_mask", mask, extent(B, onset || T > 1 ? T : 2, R), q, extent(B, T));
-  DDSP_REQUIRE_DISJOINT("note_mask", mask, extent(B, onset || T > 1 ? T : 2, R), onset, extent(B, T));
+  int rc = check_overlap("note_mask",
+                         {DDSP_OUT(mask, extent(B, onset || T > 1 ? T : 2, R))},
+                         {DDSP_IN(q, extent(B, T)), DDSP_IN(onset, extent(B, T))});
+  if (rc) return rc;
   notes_::MaskParams p;
   p.q = q;
   p.onset = onset;
@@ -430,14 +394,9 @@ int ddsp_b200_note_mask(const float* q, const float* onset, float* mask, void* w
   p.R = R;
   p.Rf = R < T ? R : T;
   p.note_on_only = note_on_only;
-  if (onset)
-    notes_::note_mask_kernel<true><<<(unsigned)B, notes_::kMaskThreads, 0,
-                                     (cudaStream_t)stream>>>(p, mask);
-  else
-    notes_::note_mask_kernel<false><<<(unsigned)B, notes_::kMaskThreads, 0,
-                                      (cudaStream_t)stream>>>(p, mask);
-  DDSP_CHECK_LAUNCH("note_mask");
-  return 0;
+  auto kern = onset ? notes_::note_mask_kernel<true> : notes_::note_mask_kernel<false>;
+  return launch("note_mask", kern, (unsigned)B, notes_::kMaskThreads, 0, (cudaStream_t)stream,
+                p, mask);
 }
 
 // The shape checks of the moments entry points, and the CTA count of a grid of tiles of
@@ -479,16 +438,14 @@ int ddsp_b200_note_moments(const float* x, const float* mask, float* mean, float
   rc = notes_grid("note_moments", B, T, &pt, &grid_t);
   if (rc) return rc;
   if (B == 0 || D == 0) return 0;
-  DDSP_REQUIRE_DISJOINT("note_moments", mean, extent(B, N, D), x, extent(B, T, D));
-  DDSP_REQUIRE_DISJOINT("note_moments", mean, extent(B, N, D), mask, extent(B, T, N));
-  DDSP_REQUIRE(!overlaps(stdev, sizeof(float) * extent(B, N, D), x, sizeof(float) * extent(B, T, D)),
-               DDSP_B200_E_INVALID, "note_moments: std must not overlap x");
-  DDSP_REQUIRE(!overlaps(stdev, sizeof(float) * extent(B, N, D), mask, sizeof(float) * extent(B, T, N)),
-               DDSP_B200_E_INVALID, "note_moments: std must not overlap mask");
-  DDSP_REQUIRE_DISJOINT("note_moments", pooled_mean, extent(B, T, D), x, extent(B, T, D));
-  DDSP_REQUIRE_DISJOINT("note_moments", pooled_mean, extent(B, T, D), mask, extent(B, T, N));
-  DDSP_REQUIRE_DISJOINT("note_moments", pooled_std, extent(B, T, D), x, extent(B, T, D));
-  DDSP_REQUIRE_DISJOINT("note_moments", pooled_std, extent(B, T, D), mask, extent(B, T, N));
+  // `stdev` is the header's `std`, a name the std namespace takes here
+  rc = check_overlap("note_moments",
+                     {DDSP_OUT(mean, extent(B, N, D)),
+                      Operand{"std", stdev, extent(B, N, D), ""},
+                      DDSP_OUT(pooled_mean, extent(B, T, D)),
+                      DDSP_OUT(pooled_std, extent(B, T, D))},
+                     {DDSP_IN(x, extent(B, T, D)), DDSP_IN(mask, extent(B, T, N))});
+  if (rc) return rc;
   if (N == 0) {   // nothing to pool: the pooled sums are zero
     const size_t bytes = sizeof(float) * (size_t)B * T * D;
     if (pooled_mean)
@@ -499,25 +456,16 @@ int ddsp_b200_note_moments(const float* x, const float* mask, float* mean, float
   }
   p.x = pt.x = x;
   p.m = pt.m = mask;
-  if (stdev)
-    notes_::note_moments_kernel<true><<<grid_n, notes_::kThreads, 0, (cudaStream_t)stream>>>(
-        p, mean, stdev);
-  else
-    notes_::note_moments_kernel<false><<<grid_n, notes_::kThreads, 0, (cudaStream_t)stream>>>(
-        p, mean, nullptr);
-  DDSP_CHECK_LAUNCH("note_moments");
+  auto moments = stdev ? notes_::note_moments_kernel<true> : notes_::note_moments_kernel<false>;
+  rc = launch("note_moments", moments, grid_n, notes_::kThreads, 0, (cudaStream_t)stream, p,
+              mean, stdev);
+  if (rc) return rc;
   if (!pooled_mean) return 0;
   const notes_::OverN o{mean, stdev, nullptr};
-  if (pooled_std)
-    notes_::note_over_n_kernel<notes_::kPoolBoth><<<grid_t, notes_::kThreads, 0,
-                                                    (cudaStream_t)stream>>>(
-        pt, o, pooled_mean, pooled_std);
-  else
-    notes_::note_over_n_kernel<notes_::kPoolMean><<<grid_t, notes_::kThreads, 0,
-                                                    (cudaStream_t)stream>>>(
-        pt, o, pooled_mean, nullptr);
-  DDSP_CHECK_LAUNCH("note_pool");
-  return 0;
+  auto pool = pooled_std ? notes_::note_over_n_kernel<notes_::kPoolBoth>
+                         : notes_::note_over_n_kernel<notes_::kPoolMean>;
+  return launch("note_pool", pool, grid_t, notes_::kThreads, 0, (cudaStream_t)stream, pt, o,
+                pooled_mean, pooled_std);
 }
 
 // The backward's A and C, [B,N,D] floats each, from a 256-byte boundary.
@@ -562,22 +510,16 @@ int ddsp_b200_note_moments_backward(const float* x, const float* mask, const flo
   float* A = align256<float>(workspace);
   float* C = A + (size_t)B * N * D;
   const notes_::Grads g{mean, stdev, grad_mean, grad_std, grad_pooled_mean, grad_pooled_std};
-  if (with_std)
-    notes_::note_moments_backward_kernel<true><<<grid_n, notes_::kThreads, 0,
-                                                 (cudaStream_t)stream>>>(p, g, A, C);
-  else
-    notes_::note_moments_backward_kernel<false><<<grid_n, notes_::kThreads, 0,
-                                                  (cudaStream_t)stream>>>(p, g, A, nullptr);
-  DDSP_CHECK_LAUNCH("note_moments_backward");
+  auto moments = with_std ? notes_::note_moments_backward_kernel<true>
+                          : notes_::note_moments_backward_kernel<false>;
+  rc = launch("note_moments_backward", moments, grid_n, notes_::kThreads, 0,
+              (cudaStream_t)stream, p, g, A, with_std ? C : nullptr);
+  if (rc) return rc;
   const notes_::OverN o{A, C, mean};
-  if (with_std)
-    notes_::note_over_n_kernel<notes_::kDxBoth><<<grid_t, notes_::kThreads, 0,
-                                                  (cudaStream_t)stream>>>(pt, o, dx, nullptr);
-  else
-    notes_::note_over_n_kernel<notes_::kDxMean><<<grid_t, notes_::kThreads, 0,
-                                                  (cudaStream_t)stream>>>(pt, o, dx, nullptr);
-  DDSP_CHECK_LAUNCH("note_moments_backward");
-  return 0;
+  auto over_n = with_std ? notes_::note_over_n_kernel<notes_::kDxBoth>
+                         : notes_::note_over_n_kernel<notes_::kDxMean>;
+  return launch("note_moments_backward", over_n, grid_t, notes_::kThreads, 0,
+                (cudaStream_t)stream, pt, o, dx, nullptr);
 }
 
 // ---- heuristics: binarizers and the note table ------------------------------------------
@@ -683,9 +625,8 @@ int ddsp_b200_note_heuristic(const float* x, const float* f0, const unsigned cha
   p.strided_pad = strided_pad;
   p.min_samples = min_samples;
   p.glue_back = glue_back != 0;
-  heur_::note_heuristic_kernel<<<(unsigned)B, heur_::kMaskThreads, 0, (cudaStream_t)stream>>>(p);
-  DDSP_CHECK_LAUNCH("note_heuristic");
-  return 0;
+  return launch("note_heuristic", heur_::note_heuristic_kernel, (unsigned)B,
+                heur_::kMaskThreads, 0, (cudaStream_t)stream, p);
 }
 
 int ddsp_b200_note_segments(const unsigned char* mask, const float* f0, ddsp_b200_note* notes,
@@ -718,9 +659,8 @@ int ddsp_b200_note_segments(const unsigned char* mask, const float* f0, ddsp_b20
   p.T = T;
   p.cap = cap;
   p.median = median;
-  heur_::note_segments_kernel<<<(unsigned)B, heur_::kMaskThreads, 0, (cudaStream_t)stream>>>(p);
-  DDSP_CHECK_LAUNCH("note_segments");
-  return 0;
+  return launch("note_segments", heur_::note_segments_kernel, (unsigned)B,
+                heur_::kMaskThreads, 0, (cudaStream_t)stream, p);
 }
 
 }  // extern "C"

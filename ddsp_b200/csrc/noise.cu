@@ -32,16 +32,14 @@ int ddsp_b200_frequency_impulse_response(const float* mags, float* ir,
   const size_t smem = sizeof(float) * ((size_t)g.S0 + (size_t)kIrFrames * nb);
   DDSP_REQUIRE(smem <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
                "frequency_impulse_response: n_frequencies=%d too large", nb);
-  DDSP_REQUIRE_DISJOINT("frequency_impulse_response", ir, extent(BF, g.S), mags, extent(BF, nb));
-  int rc = set_smem(ir_kernel, smem, "frequency_impulse_response");
+  int rc = check_overlap("frequency_impulse_response", {DDSP_OUT(ir, extent(BF, g.S))},
+                         {DDSP_IN(mags, extent(BF, nb))});
   if (rc) return rc;
   const int64_t blocks = (BF + kIrFrames - 1) / kIrFrames;
   DDSP_REQUIRE(blocks < (1ll << 31), DDSP_B200_E_INVALID,
                "frequency_impulse_response: too many frames");
-  ir_kernel<<<(int)blocks, kIrThreads, smem, (cudaStream_t)stream>>>(mags, ir,
-                                                                     BF, g);
-  DDSP_CHECK_LAUNCH("frequency_impulse_response");
-  return 0;
+  return launch("frequency_impulse_response", ir_kernel, (int)blocks, kIrThreads, smem,
+                (cudaStream_t)stream, mags, ir, BF, g);
 }
 
 int ddsp_b200_fir_time_varying(const float* audio, const float* ir, float* out,
@@ -75,16 +73,14 @@ int ddsp_b200_fir_time_varying(const float* audio, const float* ir, float* out,
   DDSP_REQUIRE(smem <= kMaxDynSmem, DDSP_B200_E_UNSUPPORTED,
                "fir_time_varying: impulse response of %d taps is beyond the "
                "shared-memory FIR (long-IR convolution is not built yet)", S);
-  DDSP_REQUIRE_DISJOINT("fir_time_varying", out, extent(B, out_len), audio, extent(B, N));
-  DDSP_REQUIRE_DISJOINT("fir_time_varying", out, extent(B, out_len), ir, extent(ir_batch, F, S));
-  int rc = set_smem(fir_kernel, smem, "fir_time_varying");
+  int rc = check_overlap("fir_time_varying", {DDSP_OUT(out, extent(B, out_len))},
+                         {DDSP_IN(audio, extent(B, N)),
+                          DDSP_IN(ir, extent(ir_batch, F, S))});
   if (rc) return rc;
   dim3 grid((out_len + kFirThreads - 1) / kFirThreads, B);
-  fir_kernel<<<grid, kFirThreads, smem, (cudaStream_t)stream>>>(
-      audio, ir, out, N, F, S, frame, ir_batch == 1 ? 0 : F * S, start, out_len,
-      accumulate);
-  DDSP_CHECK_LAUNCH("fir_time_varying");
-  return 0;
+  return launch("fir_time_varying", fir_kernel, grid, kFirThreads, smem,
+                (cudaStream_t)stream, audio, ir, out, N, F, S, frame,
+                ir_batch == 1 ? 0 : F * S, start, out_len, accumulate);
 }
 
 int ddsp_b200_uniform_noise(float* out, int B, int N, uint64_t seed,
@@ -93,10 +89,8 @@ int ddsp_b200_uniform_noise(float* out, int B, int N, uint64_t seed,
   DDSP_REQUIRE(B >= 0 && N >= 0, DDSP_B200_E_INVALID, "uniform_noise: bad shape");
   if (B == 0 || N == 0) return 0;
   const int64_t n = (int64_t)B * ((N + 3) / 4);
-  uniform_noise_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(
-      out, B, N, seed, offset);
-  DDSP_CHECK_LAUNCH("uniform_noise");
-  return 0;
+  return launch("uniform_noise", uniform_noise_kernel, grid_for(n, 256), 256, 0,
+                (cudaStream_t)stream, out, B, N, seed, offset);
 }
 
 size_t ddsp_b200_filtered_noise_workspace(int B, int F, int nb, int N,
@@ -124,8 +118,9 @@ int ddsp_b200_filtered_noise_forward(const float* mags, const float* noise,
   if (B == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (noise_fused_supported(F, nb, N, window_size)) {
-    DDSP_REQUIRE_DISJOINT("filtered_noise_forward", audio, extent(B, N), mags, extent(B, F, nb));
-    DDSP_REQUIRE_DISJOINT("filtered_noise_forward", audio, extent(B, N), noise, extent(B, N));
+    int rc = check_overlap("filtered_noise_forward", {DDSP_OUT(audio, extent(B, N))},
+                           {DDSP_IN(mags, extent(B, F, nb)), DDSP_IN(noise, extent(B, N))});
+    if (rc) return rc;
     return launch_noise_best(mags, noise, seed, offset, audio, B, F, nb, N,
                              window_size, accumulate, st);
   }
@@ -134,13 +129,14 @@ int ddsp_b200_filtered_noise_forward(const float* mags, const float* noise,
                DDSP_B200_E_WORKSPACE,
                "filtered_noise_forward: workspace of %zu B needed, %zu given",
                need, workspace_bytes);
-  DDSP_REQUIRE_DISJOINT("filtered_noise_forward", audio, extent(B, N), mags, extent(B, F, nb));
-  DDSP_REQUIRE_DISJOINT("filtered_noise_forward", audio, extent(B, N), noise, extent(B, N));
+  int rc = check_overlap("filtered_noise_forward", {DDSP_OUT(audio, extent(B, N))},
+                         {DDSP_IN(mags, extent(B, F, nb)), DDSP_IN(noise, extent(B, N))});
+  if (rc) return rc;
   IrGeom g = make_ir_geom(nb, window_size);
   float* ir = align256<float>(workspace);
   float* nz = ir + (size_t)B * F * g.S;
-  int rc = ddsp_b200_frequency_impulse_response(mags, ir, (int64_t)B * F, nb,
-                                                window_size, stream);
+  rc = ddsp_b200_frequency_impulse_response(mags, ir, (int64_t)B * F, nb, window_size,
+                                            stream);
   if (rc) return rc;
   const float* x = noise;
   if (x == nullptr) {
@@ -180,11 +176,11 @@ static int decoder_forward_impl(const float* amps_raw, const float* hd_raw,
                DDSP_B200_E_UNSUPPORTED,
                "decoder_forward: shape outside the fused decoder path "
                "(needs hop %% 64 == 0, n_frequencies <= %d)", kNfMaxNb);
-  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), amps_raw, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), hd_raw, extent(B, F, K));
-  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), f0_hz, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), mags_raw, extent(B, F, nb));
-  DDSP_REQUIRE_DISJOINT("decoder_forward", audio, extent(B, N), noise, extent(B, N));
+  rc = check_overlap("decoder_forward", {DDSP_OUT(audio, extent(B, N))},
+                     {DDSP_IN(amps_raw, extent(B, F)), DDSP_IN(hd_raw, extent(B, F, K)),
+                      DDSP_IN(f0_hz, extent(B, F)), DDSP_IN(mags_raw, extent(B, F, nb)),
+                      DDSP_IN(noise, extent(B, N))});
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   rc = launch_harmonic_v4(p, st);
   if (rc == 1) {
@@ -392,13 +388,9 @@ static NoiseBwdParams noise_bwd_params(const float* grad, const float* noise, ui
 // Launches noise_backward_kernel on checked parameters.
 static int noise_bwd_launch(const NoiseBwdParams& p, size_t smem, cudaStream_t st,
                             const char* name) {
-  int rc = set_smem(noise_backward_kernel, smem, name);
-  if (rc) return rc;
   const int per_sm = smem <= 100 * 1024 ? 2 : 1;
   const int grid = (int)std::min<long long>(p.n_tiles, (long long)num_sms() * per_sm);
-  noise_backward_kernel<<<grid, kNbThreads, smem, st>>>(p);
-  DDSP_CHECK_LAUNCH(name);
-  return 0;
+  return launch(name, noise_backward_kernel, grid, kNbThreads, smem, st, p);
 }
 
 int ddsp_b200_filtered_noise_backward_takes(int F, int nb, int N, int window_size) {
@@ -507,33 +499,29 @@ static int fir_bwd_launch(const float* audio, const float* ir, const float* grad
                           float* d_audio, float* d_ir, int B, int N, int F, int S,
                           int ir_batch, int frame, int start, int out_len, float* part,
                           cudaStream_t st, const char* name) {
+  int rc = 0;
   if (d_audio) {
     const size_t smem = sizeof(float) * ((size_t)kFadjThreads + S - 1);
-    int rc = set_smem(fir_adjoint_kernel, smem, name);
-    if (rc) return rc;
     dim3 grid((N + kFadjThreads - 1) / kFadjThreads, B);
-    fir_adjoint_kernel<<<grid, kFadjThreads, smem, st>>>(
-        grad, ir, d_audio, N, S, frame, ir_batch == 1 ? 0 : F * S, start, out_len);
-    DDSP_CHECK_LAUNCH(name);
+    rc = launch(name, fir_adjoint_kernel, grid, kFadjThreads, smem, st, grad, ir, d_audio, N,
+                S, frame, ir_batch == 1 ? 0 : F * S, start, out_len);
+    if (rc) return rc;
   }
   if (d_ir) {
     FirDirParams p = fir_dir_params(audio, grad, B, N, F, S, frame, start, out_len);
     p.out = part ? part : d_ir;
     const size_t smem = fir_dir_smem(p);
-    int rc = set_smem(fir_dir_kernel, smem, name);
-    if (rc) return rc;
     dim3 grid((unsigned)((p.n_rows + kDirRows - 1) / kDirRows),
               (unsigned)((S + kDirTaps - 1) / kDirTaps));
-    fir_dir_kernel<<<grid, kDirThreads, smem, st>>>(p);
-    DDSP_CHECK_LAUNCH(name);
+    rc = launch(name, fir_dir_kernel, grid, kDirThreads, smem, st, p);
+    if (rc) return rc;
     if (part) {
       const long long n_out = (long long)ir_batch * F * S;
-      fir_dir_reduce<<<grid_for(n_out, 256), 256, 0, st>>>(
-          part, d_ir, B, F, S, p.n_chunk, ir_batch == 1 && B > 1, n_out);
-      DDSP_CHECK_LAUNCH(name);
+      rc = launch(name, fir_dir_reduce, grid_for(n_out, 256), 256, 0, st, part, d_ir, B, F, S,
+                  p.n_chunk, ir_batch == 1 && B > 1, n_out);
     }
   }
-  return 0;
+  return rc;
 }
 
 // The route of frequency_filter's d magnitudes: the fused noise_backward_kernel reads
@@ -598,12 +586,8 @@ int ddsp_b200_frequency_impulse_response_backward(const float* d_ir, float* d_ma
   const int64_t blocks = (BF + kIrFrames - 1) / kIrFrames;
   DDSP_REQUIRE(blocks < (1ll << 31), DDSP_B200_E_INVALID,
                "frequency_impulse_response_backward: too many frames");
-  int rc = set_smem(ir_backward_kernel, smem, "frequency_impulse_response_backward");
-  if (rc) return rc;
-  ir_backward_kernel<<<(int)blocks, kIrThreads, smem, (cudaStream_t)stream>>>(d_ir, d_mags,
-                                                                              BF, g);
-  DDSP_CHECK_LAUNCH("frequency_impulse_response_backward");
-  return 0;
+  return launch("frequency_impulse_response_backward", ir_backward_kernel, (int)blocks,
+                kIrThreads, smem, (cudaStream_t)stream, d_ir, d_mags, BF, g);
 }
 
 size_t ddsp_b200_frequency_filter_backward_workspace(int B, int F, int nb, int N,

@@ -494,13 +494,10 @@ inline int launch_noise_fused(const float* mags, const float* noise,
   }
   p.n_tiles = (int)n_tiles;
   const size_t smem = nf_smem_layout(p).total;
-  int rc = set_smem(noise_fused_kernel, smem, "filtered_noise_forward");
-  if (rc) return rc;
   const int ctas_per_sm = smem <= 110 * 1024 ? 2 : 1;
   const int grid = (int)std::min<long long>(n_tiles, (long long)num_sms() * ctas_per_sm);
-  noise_fused_kernel<<<grid, kNfThreads, smem, st>>>(p);
-  DDSP_CHECK_LAUNCH("filtered_noise_forward(fused)");
-  return 0;
+  return launch("filtered_noise_forward(fused)", noise_fused_kernel, grid, kNfThreads, smem,
+                st, p);
 }
 
 }  // namespace ddsp

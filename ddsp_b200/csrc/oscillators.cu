@@ -36,27 +36,28 @@ int ddsp_b200_oscillator_bank(const float* frequency_envelopes,
   DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
                "oscillator_bank: workspace of %zu B needed, %zu given", need,
                workspace_bytes);
-  DDSP_REQUIRE_DISJOINT("oscillator_bank", out, extent(B, N, sum_sinusoids ? 1 : K), frequency_envelopes,
-                        extent(B, N, K));
-  DDSP_REQUIRE_DISJOINT("oscillator_bank", out, extent(B, N, sum_sinusoids ? 1 : K), amplitude_envelopes,
-                        extent(B, N, K));
+  int rc = check_overlap("oscillator_bank",
+                         {DDSP_OUT(out, extent(B, N, sum_sinusoids ? 1 : K))},
+                         {DDSP_IN(frequency_envelopes, extent(B, N, K)),
+                          DDSP_IN(amplitude_envelopes, extent(B, N, K))});
+  if (rc) return rc;
   unsigned long long* sums = align256<unsigned long long>(workspace);
   const int n_chunks = (N + kObChunk - 1) / kObChunk;
   const double inv_sr = 1.0 / (double)sample_rate;
   cudaStream_t st = (cudaStream_t)stream;
   dim3 grid(n_chunks, B);
-  oscbank_chunk_sums<<<grid, kObThreads, 0, st>>>(frequency_envelopes, sums, N, K,
-                                                 n_chunks, inv_sr);
-  DDSP_CHECK_LAUNCH("oscillator_bank(chunk sums)");
+  rc = launch("oscillator_bank(chunk sums)", oscbank_chunk_sums, grid, kObThreads, 0, st,
+              frequency_envelopes, sums, N, K, n_chunks, inv_sr);
+  if (rc) return rc;
   const int64_t BK = (int64_t)B * K;
-  oscbank_scan_chunks<<<(int)((BK + kObThreads - 1) / kObThreads), kObThreads, 0, st>>>(
-      sums, K, n_chunks, BK);
-  DDSP_CHECK_LAUNCH("oscillator_bank(scan)");
+  rc = launch("oscillator_bank(scan)", oscbank_scan_chunks,
+              (int)((BK + kObThreads - 1) / kObThreads), kObThreads, 0, st, sums, K,
+              n_chunks, BK);
+  if (rc) return rc;
   auto apply = sum_sinusoids ? oscbank_apply<true> : oscbank_apply<false>;
-  apply<<<grid, kObThreads, 0, st>>>(frequency_envelopes, amplitude_envelopes, sums, out,
-                                     N, K, n_chunks, inv_sr, sample_rate * 0.5f);
-  DDSP_CHECK_LAUNCH("oscillator_bank(apply)");
-  return 0;
+  return launch("oscillator_bank(apply)", apply, grid, kObThreads, 0, st,
+                frequency_envelopes, amplitude_envelopes, sums, out, N, K, n_chunks, inv_sr,
+                sample_rate * 0.5f);
 }
 
 // One cluster per (b, tile of kObbLanes oscillators) along x, batch along y.
@@ -83,12 +84,11 @@ int ddsp_b200_oscillator_bank_backward(const float* frequency_envelopes,
   DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
                "oscillator_bank_backward: B=%d exceeds the 65535 grid limit", B);
   auto kernel = sum_sinusoids ? oscbank_backward<kObbSum> : oscbank_backward<kObbFull>;
-  kernel<<<oscbank_backward_grid(B, K), kObbLanes * kObbWarps, 0, (cudaStream_t)stream>>>(
-      frequency_envelopes, amplitude_envelopes, grad, d_frequency_envelopes,
-      d_amplitude_envelopes, N, K, 1.0 / (double)sample_rate, sample_rate * 0.5f,
-      6.283185307179586 / (double)sample_rate);
-  DDSP_CHECK_LAUNCH("oscillator_bank_backward");
-  return 0;
+  return launch("oscillator_bank_backward", kernel, oscbank_backward_grid(B, K),
+                kObbLanes * kObbWarps, 0, (cudaStream_t)stream, frequency_envelopes,
+                amplitude_envelopes, grad, d_frequency_envelopes, d_amplitude_envelopes, N,
+                K, 1.0 / (double)sample_rate, sample_rate * 0.5f,
+                6.283185307179586 / (double)sample_rate);
 }
 
 int ddsp_b200_angular_cumsum(const float* angular_frequency, float* phase, int B,
@@ -105,12 +105,13 @@ int ddsp_b200_angular_cumsum(const float* angular_frequency, float* phase, int B
   if (B == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   if (mode != 0) {
-    DDSP_REQUIRE_DISJOINT("angular_cumsum", phase, extent(B, N, C), angular_frequency, extent(B, N, C));
+    int rc = check_overlap("angular_cumsum", {DDSP_OUT(phase, extent(B, N, C))},
+                           {DDSP_IN(angular_frequency, extent(B, N, C))});
+    if (rc) return rc;
     const int64_t BC = (int64_t)B * C;
-    tf_sequential_cumsum<<<(int)((BC + 127) / 128), 128, 0, st>>>(
-        angular_frequency, nullptr, phase, B, N, C, mode, chunk_size, 0, 1.0f);
-    DDSP_CHECK_LAUNCH("angular_cumsum(tf_sequential)");
-    return 0;
+    return launch("angular_cumsum(tf_sequential)", tf_sequential_cumsum,
+                  (int)((BC + 127) / 128), 128, 0, st, angular_frequency, nullptr, phase, B,
+                  N, C, mode, chunk_size, 0, 1.0f);
   }
   DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
                "angular_cumsum: B=%d exceeds the 65535 grid limit", B);
@@ -118,22 +119,23 @@ int ddsp_b200_angular_cumsum(const float* angular_frequency, float* phase, int B
   DDSP_REQUIRE(workspace != nullptr && workspace_bytes >= need, DDSP_B200_E_WORKSPACE,
                "angular_cumsum: workspace of %zu B needed, %zu given", need,
                workspace_bytes);
-  DDSP_REQUIRE_DISJOINT("angular_cumsum", phase, extent(B, N, C), angular_frequency, extent(B, N, C));
+  int rc = check_overlap("angular_cumsum", {DDSP_OUT(phase, extent(B, N, C))},
+                         {DDSP_IN(angular_frequency, extent(B, N, C))});
+  if (rc) return rc;
   unsigned long long* sums = align256<unsigned long long>(workspace);
   const int n_chunks = (N + kObChunk - 1) / kObChunk;
   const double inv_two_pi = 0.15915494309189535;
   dim3 grid(n_chunks, B);
-  oscbank_chunk_sums<<<grid, kObThreads, 0, st>>>(angular_frequency, sums, N, C,
-                                                 n_chunks, inv_two_pi);
-  DDSP_CHECK_LAUNCH("angular_cumsum(chunk sums)");
+  rc = launch("angular_cumsum(chunk sums)", oscbank_chunk_sums, grid, kObThreads, 0, st,
+              angular_frequency, sums, N, C, n_chunks, inv_two_pi);
+  if (rc) return rc;
   const int64_t BK = (int64_t)B * C;
-  oscbank_scan_chunks<<<(int)((BK + kObThreads - 1) / kObThreads), kObThreads, 0, st>>>(
-      sums, C, n_chunks, BK);
-  DDSP_CHECK_LAUNCH("angular_cumsum(scan)");
-  oscbank_phase_out<<<grid, kObThreads, 0, st>>>(angular_frequency, sums, phase, N, C,
-                                                n_chunks, inv_two_pi);
-  DDSP_CHECK_LAUNCH("angular_cumsum(apply)");
-  return 0;
+  rc = launch("angular_cumsum(scan)", oscbank_scan_chunks,
+              (int)((BK + kObThreads - 1) / kObThreads), kObThreads, 0, st, sums, C,
+              n_chunks, BK);
+  if (rc) return rc;
+  return launch("angular_cumsum(apply)", oscbank_phase_out, grid, kObThreads, 0, st,
+                angular_frequency, sums, phase, N, C, n_chunks, inv_two_pi);
 }
 
 int ddsp_b200_angular_cumsum_backward(const float* grad, float* d_angular_frequency, int B,
@@ -146,11 +148,9 @@ int ddsp_b200_angular_cumsum_backward(const float* grad, float* d_angular_freque
   if (empty) return 0;
   DDSP_REQUIRE(B <= 65535, DDSP_B200_E_INVALID,
                "angular_cumsum_backward: B=%d exceeds the 65535 grid limit", B);
-  oscbank_backward<kObbCumsum>
-      <<<oscbank_backward_grid(B, C), kObbLanes * kObbWarps, 0, (cudaStream_t)stream>>>(
-          nullptr, nullptr, grad, d_angular_frequency, nullptr, N, C, 0.0, 0.f, 1.0);
-  DDSP_CHECK_LAUNCH("angular_cumsum_backward");
-  return 0;
+  return launch("angular_cumsum_backward", oscbank_backward<kObbCumsum>,
+                oscbank_backward_grid(B, C), kObbLanes * kObbWarps, 0, (cudaStream_t)stream,
+                nullptr, nullptr, grad, d_angular_frequency, nullptr, N, C, 0.0, 0.f, 1.0);
 }
 
 int ddsp_b200_oscillator_bank_tf_sequential(const float* frequency_envelopes,
@@ -162,17 +162,16 @@ int ddsp_b200_oscillator_bank_tf_sequential(const float* frequency_envelopes,
                "oscillator_bank_tf_sequential: null pointer");
   DDSP_REQUIRE(B >= 0 && N >= 1 && K >= 1 && chunk_size >= 1 && sample_rate > 0.f,
                DDSP_B200_E_INVALID, "oscillator_bank_tf_sequential: bad arguments");
-  DDSP_REQUIRE_DISJOINT("oscillator_bank_tf_sequential", out, extent(B, N, K), frequency_envelopes,
-                        extent(B, N, K));
-  DDSP_REQUIRE_DISJOINT("oscillator_bank_tf_sequential", out, extent(B, N, K), amplitude_envelopes,
-                        extent(B, N, K));
+  int rc = check_overlap("oscillator_bank_tf_sequential", {DDSP_OUT(out, extent(B, N, K))},
+                         {DDSP_IN(frequency_envelopes, extent(B, N, K)),
+                          DDSP_IN(amplitude_envelopes, extent(B, N, K))});
+  if (rc) return rc;
   if (B == 0) return 0;
   const int64_t BK = (int64_t)B * K;
-  tf_sequential_cumsum<<<(int)((BK + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
-      frequency_envelopes, amplitude_envelopes, out, B, N, K,
-      use_angular_cumsum ? 2 : 1, chunk_size, 1, sample_rate);
-  DDSP_CHECK_LAUNCH("oscillator_bank_tf_sequential");
-  return 0;
+  return launch("oscillator_bank_tf_sequential", tf_sequential_cumsum,
+                (int)((BK + 127) / 128), 128, 0, (cudaStream_t)stream, frequency_envelopes,
+                amplitude_envelopes, out, B, N, K, use_angular_cumsum ? 2 : 1, chunk_size,
+                1, sample_rate);
 }
 
 static int sinus_tile_frames(int F, int K) {
@@ -221,14 +220,12 @@ static int sinus_tile_offsets(const float* frequencies, unsigned long long* sums
                               int F, int K, int hop, int FT, double inv_sr,
                               cudaStream_t st, const char* name) {
   const int n_tiles = (F + FT - 1) / FT;
-  sinus_tile_sums<<<dim3(n_tiles, B), kSfThreads, 0, st>>>(frequencies, sums, F, K, hop,
-                                                           FT, n_tiles, inv_sr);
-  DDSP_CHECK_LAUNCH(name);
+  int rc = launch(name, sinus_tile_sums, dim3(n_tiles, B), kSfThreads, 0, st, frequencies,
+                  sums, F, K, hop, FT, n_tiles, inv_sr);
+  if (rc) return rc;
   const int64_t BK = (int64_t)B * K;
-  oscbank_scan_chunks<<<(int)((BK + kObThreads - 1) / kObThreads), kObThreads, 0, st>>>(
-      sums, K, n_tiles, BK);
-  DDSP_CHECK_LAUNCH(name);
-  return 0;
+  return launch(name, oscbank_scan_chunks, (int)((BK + kObThreads - 1) / kObThreads),
+                kObThreads, 0, st, sums, K, n_tiles, BK);
 }
 
 int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitudes,
@@ -241,8 +238,10 @@ int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitud
   int rc = sinus_check("sinusoidal_forward", B, F, K, N, sample_rate, amp_method, workspace,
                        workspace_bytes, ddsp_b200_sinusoidal_workspace(B, F, K));
   if (rc || B == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("sinusoidal_forward", audio, extent(B, N), frequencies, extent(B, F, K));
-  DDSP_REQUIRE_DISJOINT("sinusoidal_forward", audio, extent(B, N), amplitudes, extent(B, F, K));
+  rc = check_overlap("sinusoidal_forward", {DDSP_OUT(audio, extent(B, N))},
+                     {DDSP_IN(frequencies, extent(B, F, K)),
+                      DDSP_IN(amplitudes, extent(B, F, K))});
+  if (rc) return rc;
   const int FT = sinus_tile_frames(F, K);
   const SfSmem L = sf_smem(FT, K);
   unsigned long long* sums = align256<unsigned long long>(workspace);
@@ -254,13 +253,9 @@ int ddsp_b200_sinusoidal_forward(const float* frequencies, const float* amplitud
                           "sinusoidal_forward(tile offsets)");
   if (rc) return rc;
   auto kern = amp_method == DDSP_B200_AMP_WINDOW ? sinus_apply<true> : sinus_apply<false>;
-  rc = set_smem(kern, L.total, "sinusoidal_forward");
-  if (rc) return rc;
-  kern<<<dim3(n_tiles, B), kSfThreads, L.total, st>>>(
-      frequencies, amplitudes, sums, audio, F, K, N, hop, FT, n_tiles, inv_sr,
-      sample_rate * 0.5f, accumulate);
-  DDSP_CHECK_LAUNCH("sinusoidal_forward(apply)");
-  return 0;
+  return launch("sinusoidal_forward(apply)", kern, dim3(n_tiles, B), kSfThreads, L.total,
+                st, frequencies, amplitudes, sums, audio, F, K, N, hop, FT, n_tiles, inv_sr,
+                sample_rate * 0.5f, accumulate);
 }
 
 size_t ddsp_b200_sinusoidal_backward_workspace(int B, int F, int K) {
@@ -296,14 +291,13 @@ int ddsp_b200_sinusoidal_backward(const float* frequencies, const float* amplitu
   auto kern = amp_method == DDSP_B200_AMP_WINDOW
                   ? (phase ? sinus_bwd_frames<true, true> : sinus_bwd_frames<true, false>)
                   : (phase ? sinus_bwd_frames<false, true> : sinus_bwd_frames<false, false>);
-  kern<<<n_blocks, kSbThreads, 0, st>>>(frequencies, amplitudes, grad_audio, sums, part, F,
-                                        K, N, hop, FT, n_tiles, BFK, inv_sr,
-                                        sample_rate * 0.5f);
-  DDSP_CHECK_LAUNCH("sinusoidal_backward(frames)");
-  sinus_bwd_finalize<<<dim3((K + 31) / 32, B), 32 * kSfinWarps, 0, st>>>(
-      part, d_amplitudes, d_frequencies, F, K, hop, BFK, inv_sr);
-  DDSP_CHECK_LAUNCH("sinusoidal_backward(finalize)");
-  return 0;
+  rc = launch("sinusoidal_backward(frames)", kern, n_blocks, kSbThreads, 0, st, frequencies,
+              amplitudes, grad_audio, sums, part, F, K, N, hop, FT, n_tiles, BFK, inv_sr,
+              sample_rate * 0.5f);
+  if (rc) return rc;
+  return launch("sinusoidal_backward(finalize)", sinus_bwd_finalize, dim3((K + 31) / 32, B),
+                32 * kSfinWarps, 0, st, part, d_amplitudes, d_frequencies, F, K, hop, BFK,
+                inv_sr);
 }
 
 size_t ddsp_b200_wavetable_workspace(int B, int F) {
@@ -369,15 +363,14 @@ static int wt_frame_phases(const WtPhase& w, const float* f0, int B, int F, int 
                            float sample_rate, cudaStream_t st, const char* name) {
   const int n_tiles = (F + wt_::kFT - 1) / wt_::kFT;
   const double sr = (double)sample_rate;
-  wt_::wt_tile_sums<<<dim3(n_tiles, B), wt_::kFT, 0, st>>>(f0, w.sums, F, hop, n_tiles, sr);
-  DDSP_CHECK_LAUNCH(name);
-  oscbank_scan_chunks<<<(B + kObThreads - 1) / kObThreads, kObThreads, 0, st>>>(
-      w.sums, 1, n_tiles, (int64_t)B);
-  DDSP_CHECK_LAUNCH(name);
-  wt_::wt_frame_phase<<<dim3(n_tiles, B), wt_::kFT, 0, st>>>(f0, w.sums, w.P, w.A, w.D, F,
-                                                             hop, n_tiles, sr);
-  DDSP_CHECK_LAUNCH(name);
-  return 0;
+  int rc = launch(name, wt_::wt_tile_sums, dim3(n_tiles, B), wt_::kFT, 0, st, f0, w.sums, F,
+                  hop, n_tiles, sr);
+  if (rc) return rc;
+  rc = launch(name, oscbank_scan_chunks, (B + kObThreads - 1) / kObThreads, kObThreads, 0,
+              st, w.sums, 1, n_tiles, (int64_t)B);
+  if (rc) return rc;
+  return launch(name, wt_::wt_frame_phase, dim3(n_tiles, B), wt_::kFT, 0, st, f0, w.sums,
+                w.P, w.A, w.D, F, hop, n_tiles, sr);
 }
 
 int ddsp_b200_wavetable_forward(const float* f0_hz, const float* amplitudes,
@@ -389,9 +382,10 @@ int ddsp_b200_wavetable_forward(const float* f0_hz, const float* amplitudes,
   int rc = wt_check("wavetable_forward", B, F, N, Fw, W, sample_rate, amp_method, workspace,
                     workspace_bytes, ddsp_b200_wavetable_workspace(B, F));
   if (rc || B == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("wavetable_forward", audio, extent(B, N), f0_hz, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("wavetable_forward", audio, extent(B, N), amplitudes, extent(B, F));
-  DDSP_REQUIRE_DISJOINT("wavetable_forward", audio, extent(B, N), wavetables, extent(B, Fw, W));
+  rc = check_overlap("wavetable_forward", {DDSP_OUT(audio, extent(B, N))},
+                     {DDSP_IN(f0_hz, extent(B, F)), DDSP_IN(amplitudes, extent(B, F)),
+                      DDSP_IN(wavetables, extent(B, Fw, W))});
+  if (rc) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int hop = N / F;
   const WtPhase w = wt_phase_layout(workspace, B, F);
@@ -399,10 +393,9 @@ int ddsp_b200_wavetable_forward(const float* f0_hz, const float* amplitudes,
   if (rc) return rc;
   auto kern = amp_method == DDSP_B200_AMP_WINDOW ? wt_::wt_forward<true>
                                                  : wt_::wt_forward<false>;
-  kern<<<dim3((unsigned)((N + wt_::kThreads - 1) / wt_::kThreads), B), wt_::kThreads, 0, st>>>(
-      amplitudes, wavetables, w.P, w.A, w.D, audio, F, N, hop, Fw, W);
-  DDSP_CHECK_LAUNCH("wavetable_forward");
-  return 0;
+  return launch("wavetable_forward", kern,
+                dim3((unsigned)((N + wt_::kThreads - 1) / wt_::kThreads), B), wt_::kThreads,
+                0, st, amplitudes, wavetables, w.P, w.A, w.D, audio, F, N, hop, Fw, W);
 }
 
 int ddsp_b200_wavetable_backward(const float* f0_hz, const float* amplitudes,
@@ -433,32 +426,31 @@ int ddsp_b200_wavetable_backward(const float* f0_hz, const float* amplitudes,
                                 : wt_::wt_bwd_frames<true, false>)
                        : (phase ? wt_::wt_bwd_frames<false, true>
                                 : wt_::wt_bwd_frames<false, false>);
-    kern<<<(unsigned)((BF + 31) / 32), kSbThreads, 0, st>>>(
-        amplitudes, wavetables, grad_audio, w.P, w.A, w.D, part, F, N, hop, Fw, W, BF);
-    DDSP_CHECK_LAUNCH("wavetable_backward(frames)");
+    rc = launch("wavetable_backward(frames)", kern, (unsigned)((BF + 31) / 32), kSbThreads,
+                0, st, amplitudes, wavetables, grad_audio, w.P, w.A, w.D, part, F, N, hop,
+                Fw, W, BF);
+    if (rc) return rc;
     // K = 1; sinus_bwd_finalize always writes d amplitudes
-    sinus_bwd_finalize<<<dim3(1, B), 32 * kSfinWarps, 0, st>>>(
-        part, d_amplitudes ? d_amplitudes : d_amp_scratch, d_f0, F, 1, hop, BF,
-        1.0 / (double)sample_rate);
-    DDSP_CHECK_LAUNCH("wavetable_backward(finalize)");
+    rc = launch("wavetable_backward(finalize)", sinus_bwd_finalize, dim3(1, B),
+                32 * kSfinWarps, 0, st, part, d_amplitudes ? d_amplitudes : d_amp_scratch,
+                d_f0, F, 1, hop, BF, 1.0 / (double)sample_rate);
+    if (rc) return rc;
   }
 
   if (d_wavetables) {
     const int n_seg = wt_::table_segments(N, Fw);
     const size_t smem = wt_::table_smem_bytes(W);
     auto kern = window ? wt_::wt_bwd_table<true> : wt_::wt_bwd_table<false>;
-    rc = set_smem(kern, smem, "wavetable_backward");
-    if (rc) return rc;
     const unsigned gx = (unsigned)((int64_t)Fw * n_seg * wt_::table_col_tiles(W));
-    kern<<<dim3(gx, B), wt_::kTabWarps * 32, smem, st>>>(
-        amplitudes, grad_audio, w.P, w.A, w.D, n_seg > 1 ? tab_part : d_wavetables, F, N,
-        hop, Fw, W, n_seg);
-    DDSP_CHECK_LAUNCH("wavetable_backward(wavetables)");
+    rc = launch("wavetable_backward(wavetables)", kern, dim3(gx, B), wt_::kTabWarps * 32,
+                smem, st, amplitudes, grad_audio, w.P, w.A, w.D,
+                n_seg > 1 ? tab_part : d_wavetables, F, N, hop, Fw, W, n_seg);
+    if (rc) return rc;
     if (n_seg > 1) {
       const int64_t RW = (int64_t)B * Fw * W;
-      wt_::wt_table_reduce<<<grid_for(RW, 256), 256, 0, st>>>(tab_part, d_wavetables, RW, W,
-                                                            n_seg);
-      DDSP_CHECK_LAUNCH("wavetable_backward(reduce)");
+      rc = launch("wavetable_backward(reduce)", wt_::wt_table_reduce, grid_for(RW, 256),
+                  256, 0, st, tab_part, d_wavetables, RW, W, n_seg);
+      if (rc) return rc;
     }
   }
   return 0;
@@ -487,17 +479,16 @@ int ddsp_b200_harmonic_oscillator_bank(const float* frequency,
   if (rc || B == 0) return rc;
   DDSP_REQUIRE(frequency && amplitude_envelopes && audio, DDSP_B200_E_INVALID,
                "harmonic_oscillator_bank: null pointer");
-  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", audio, extent(B, N), frequency, extent(B, N));
-  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", audio, extent(B, N), amplitude_envelopes, extent(B, N, K));
-  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", audio, extent(B, N), initial_phase, extent(B));
-  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", final_phase, extent(B), frequency, extent(B, N));
-  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", final_phase, extent(B), amplitude_envelopes, extent(B, N, K));
-  DDSP_REQUIRE_DISJOINT("harmonic_oscillator_bank", final_phase, extent(B), initial_phase, extent(B));
-  hob_::hob_forward<<<dim3(B, hob_::n_spans(N)), hob_::kThreads, 0, (cudaStream_t)stream>>>(
-      frequency, amplitude_envelopes, initial_phase, audio, final_phase, N, K,
-      1.0 / (double)sample_rate, use_angular_cumsum ? 0 : 1);
-  DDSP_CHECK_LAUNCH("harmonic_oscillator_bank");
-  return 0;
+  rc = check_overlap("harmonic_oscillator_bank", {DDSP_OUT(audio, extent(B, N)),
+                                                  DDSP_OUT(final_phase, extent(B))},
+                     {DDSP_IN(frequency, extent(B, N)),
+                      DDSP_IN(amplitude_envelopes, extent(B, N, K)),
+                      DDSP_IN(initial_phase, extent(B))});
+  if (rc) return rc;
+  return launch("harmonic_oscillator_bank", hob_::hob_forward, dim3(B, hob_::n_spans(N)),
+                hob_::kThreads, 0, (cudaStream_t)stream, frequency, amplitude_envelopes,
+                initial_phase, audio, final_phase, N, K, 1.0 / (double)sample_rate,
+                use_angular_cumsum ? 0 : 1);
 }
 
 int ddsp_b200_harmonic_oscillator_bank_backward(
@@ -514,12 +505,11 @@ int ddsp_b200_harmonic_oscillator_bank_backward(
   DDSP_REQUIRE(frequency && amplitude_envelopes && grad_audio, DDSP_B200_E_INVALID,
                "harmonic_oscillator_bank_backward: null pointer");
   if (!d_frequency && !d_amplitude_envelopes && !d_initial_phase) return 0;
-  hob_::hob_backward<<<dim3(hob_::kCl, B), hob_::kBwWarps * 32, 0, (cudaStream_t)stream>>>(
-      frequency, amplitude_envelopes, initial_phase, grad_audio, grad_final_phase,
-      d_frequency, d_amplitude_envelopes, d_initial_phase, N, K, 1.0 / (double)sample_rate,
-      6.283185307179586 / (double)sample_rate);
-  DDSP_CHECK_LAUNCH("harmonic_oscillator_bank_backward");
-  return 0;
+  return launch("harmonic_oscillator_bank_backward", hob_::hob_backward, dim3(hob_::kCl, B),
+                hob_::kBwWarps * 32, 0, (cudaStream_t)stream, frequency,
+                amplitude_envelopes, initial_phase, grad_audio, grad_final_phase,
+                d_frequency, d_amplitude_envelopes, d_initial_phase, N, K,
+                1.0 / (double)sample_rate, 6.283185307179586 / (double)sample_rate);
 }
 
 // ---- core.linear_lookup (lookup.cuh) -------------------------------------------------
@@ -541,14 +531,15 @@ int ddsp_b200_linear_lookup_forward(const float* phase, const float* wavetables,
                "linear_lookup_forward: null pointer");
   int rc = ll_check("linear_lookup_forward", B, N, W, per_sample);
   if (rc || B == 0) return rc;
-  DDSP_REQUIRE_DISJOINT("linear_lookup_forward", out, extent(B, N), phase, extent(B, N));
-  DDSP_REQUIRE_DISJOINT("linear_lookup_forward", out, extent(B, N), wavetables, extent(B, per_sample ? N : 1, W));
+  rc = check_overlap("linear_lookup_forward", {DDSP_OUT(out, extent(B, N))},
+                     {DDSP_IN(phase, extent(B, N)),
+                      DDSP_IN(wavetables, extent(B, per_sample ? N : 1, W))});
+  if (rc) return rc;
   auto kern = per_sample ? ll_::ll_samples<true, false> : ll_::ll_samples<false, false>;
   const int64_t rows = (int64_t)B * N;
-  kern<<<(unsigned)((rows + ll_::kThreads - 1) / ll_::kThreads), ll_::kThreads, 0,
-         (cudaStream_t)stream>>>(phase, wavetables, nullptr, out, rows, N, W);
-  DDSP_CHECK_LAUNCH("linear_lookup_forward");
-  return 0;
+  return launch("linear_lookup_forward", kern,
+                (unsigned)((rows + ll_::kThreads - 1) / ll_::kThreads), ll_::kThreads, 0,
+                (cudaStream_t)stream, phase, wavetables, nullptr, out, rows, N, W);
 }
 
 int ddsp_b200_linear_lookup_backward(const float* phase, const float* wavetables,
@@ -562,24 +553,21 @@ int ddsp_b200_linear_lookup_backward(const float* phase, const float* wavetables
   const int64_t rows = (int64_t)B * N;
   if (d_phase) {
     auto kern = per_sample ? ll_::ll_samples<true, true> : ll_::ll_samples<false, true>;
-    kern<<<(unsigned)((rows + ll_::kThreads - 1) / ll_::kThreads), ll_::kThreads, 0, st>>>(
-        phase, wavetables, grad, d_phase, rows, N, W);
-    DDSP_CHECK_LAUNCH("linear_lookup_backward(phase)");
+    rc = launch("linear_lookup_backward(phase)", kern,
+                (unsigned)((rows + ll_::kThreads - 1) / ll_::kThreads), ll_::kThreads, 0,
+                st, phase, wavetables, grad, d_phase, rows, N, W);
+    if (rc) return rc;
   }
   if (!d_wavetables) return 0;
   if (per_sample) {
-    ll_::ll_dtab_rows<<<grid_for(rows * 32, ll_::kThreads), ll_::kThreads, 0, st>>>(
-        phase, grad, d_wavetables, rows, W);
-    DDSP_CHECK_LAUNCH("linear_lookup_backward(wavetables)");
-    return 0;
+    return launch("linear_lookup_backward(wavetables)", ll_::ll_dtab_rows,
+                  grid_for(rows * 32, ll_::kThreads), ll_::kThreads, 0, st, phase, grad,
+                  d_wavetables, rows, W);
   }
   const size_t smem = wt_::table_smem_bytes(W);
-  rc = set_smem(ll_::ll_dtab_items, smem, "linear_lookup_backward");
-  if (rc) return rc;
-  ll_::ll_dtab_items<<<dim3((unsigned)(ll_::kCl * wt_::table_col_tiles(W)), std::min(B, 65535)),
-                       wt_::kTabWarps * 32, smem, st>>>(phase, grad, d_wavetables, B, N, W);
-  DDSP_CHECK_LAUNCH("linear_lookup_backward(wavetables)");
-  return 0;
+  return launch("linear_lookup_backward(wavetables)", ll_::ll_dtab_items,
+                dim3((unsigned)(ll_::kCl * wt_::table_col_tiles(W)), std::min(B, 65535)),
+                wt_::kTabWarps * 32, smem, st, phase, grad, d_wavetables, B, N, W);
 }
 
 }  // extern "C"

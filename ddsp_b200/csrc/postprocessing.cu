@@ -79,11 +79,11 @@ int ddsp_b200_detect_notes(const double* loudness, const double* conf, double* r
   p.min_db = min_db;
   p.note_threshold = note_threshold;
   cudaStream_t s = (cudaStream_t)stream;
-  post_::detect_prepare_kernel<<<(unsigned)p.n_partials, post_::kThreads, 0, s>>>(p);
-  DDSP_CHECK_LAUNCH("detect_notes (prepare)");
-  post_::detect_notes_kernel<<<grid_for(n, post_::kThreads), post_::kThreads, 0, s>>>(p);
-  DDSP_CHECK_LAUNCH("detect_notes");
-  return 0;
+  int rc = launch("detect_notes (prepare)", post_::detect_prepare_kernel,
+                  (unsigned)p.n_partials, post_::kThreads, 0, s, p);
+  if (rc) return rc;
+  return launch("detect_notes", post_::detect_notes_kernel, grid_for(n, post_::kThreads),
+                post_::kThreads, 0, s, p);
 }
 
 // ---- QuantileTransformer ---------------------------------------------------------------
@@ -112,9 +112,8 @@ int ddsp_b200_quantile_fit(const double* sorted, const int64_t* counts, const do
   p.F = F;
   p.nq = nq;
   p.f32 = flags & DDSP_B200_QUANTILE_F32;
-  post_::quantile_fit_kernel<<<(unsigned)F, post_::kThreads, 0, (cudaStream_t)stream>>>(p);
-  DDSP_CHECK_LAUNCH(fn);
-  return 0;
+  return launch(fn, post_::quantile_fit_kernel, (unsigned)F, post_::kThreads, 0,
+                (cudaStream_t)stream, p);
 }
 
 int ddsp_b200_quantile_transform(const double* x, const double* quantiles,
@@ -153,14 +152,11 @@ int ddsp_b200_quantile_transform(const double* x, const double* quantiles,
   p.normal = distribution == DDSP_B200_QUANTILE_NORMAL;
   p.f32 = flags & DDSP_B200_QUANTILE_F32;
   const size_t smem = 2 * (size_t)nq * sizeof(double);
-  int rc = set_smem(post_::quantile_transform_kernel, smem, fn);
-  if (rc) return rc;
   const int64_t row_blocks = (n + post_::kThreads - 1) / post_::kThreads;
   const int64_t cap = std::max<int64_t>(1, (int64_t)num_sms() * 8 / F);
   const dim3 grid((unsigned)std::min(row_blocks, cap), (unsigned)F);
-  post_::quantile_transform_kernel<<<grid, post_::kThreads, smem, (cudaStream_t)stream>>>(p);
-  DDSP_CHECK_LAUNCH(fn);
-  return 0;
+  return launch(fn, post_::quantile_transform_kernel, grid, post_::kThreads, smem,
+                (cudaStream_t)stream, p);
 }
 
 // ---- get_tuning_factor / auto_tune -----------------------------------------------------
@@ -189,11 +185,10 @@ int ddsp_b200_tuning_factor(const double* f0, const double* conf, const double* 
   p.N = N;
   p.n_factors = n_factors;
   cudaStream_t s = (cudaStream_t)stream;
-  post_::tuning_costs_kernel<<<(unsigned)n_factors, post_::kThreads, 0, s>>>(p);
-  DDSP_CHECK_LAUNCH("tuning_factor (costs)");
-  post_::tuning_argmin_kernel<<<1, 32, 0, s>>>(p);
-  DDSP_CHECK_LAUNCH(fn);
-  return 0;
+  int rc = launch("tuning_factor (costs)", post_::tuning_costs_kernel, (unsigned)n_factors,
+                  post_::kThreads, 0, s, p);
+  if (rc) return rc;
+  return launch(fn, post_::tuning_argmin_kernel, 1, 32, 0, s, p);
 }
 
 int ddsp_b200_auto_tune(const double* f0, const double* f0_on, double* scale_cost,
@@ -234,16 +229,15 @@ int ddsp_b200_auto_tune(const double* f0, const double* f0_on, double* scale_cos
   p.chromatic = chromatic;
   p.f32 = flags & DDSP_B200_AUTO_TUNE_F32;
   cudaStream_t s = (cudaStream_t)stream;
+  int rc = 0;
   if (!chromatic) {
-    post_::scale_costs_kernel<<<12, post_::kThreads, 0, s>>>(p);
-    DDSP_CHECK_LAUNCH("auto_tune (scales)");
+    rc = launch("auto_tune (scales)", post_::scale_costs_kernel, 12, post_::kThreads, 0, s, p);
+    if (rc) return rc;
   }
-  if (T > 0 || !chromatic) {
-    post_::auto_tune_kernel<<<grid_for(std::max<int64_t>(T, 1), post_::kThreads),
-                              post_::kThreads, 0, s>>>(p);
-    DDSP_CHECK_LAUNCH(fn);
-  }
-  return 0;
+  if (T > 0 || !chromatic)
+    rc = launch(fn, post_::auto_tune_kernel, grid_for(std::max<int64_t>(T, 1), post_::kThreads),
+                post_::kThreads, 0, s, p);
+  return rc;
 }
 
 }  // extern "C"

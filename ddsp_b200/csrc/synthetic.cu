@@ -75,12 +75,9 @@ int ddsp_b200_synthetic_notes(const int64_t* seeds, unsigned int* key, int* pos,
   p.p_silent = p_silent;
   p.p_vibrato = p_vibrato;
   const size_t smem = synth_::smem_bytes(T, K, M);
-  int rc = set_smem(synth_::synthetic_notes_kernel, smem, fn);
-  if (rc) return rc;
   const unsigned grid = state ? 1u : (unsigned)B;
-  synth_::synthetic_notes_kernel<<<grid, synth_::kThreads, smem, (cudaStream_t)stream>>>(p);
-  DDSP_CHECK_LAUNCH(fn);
-  return 0;
+  return launch(fn, synth_::synthetic_notes_kernel, grid, synth_::kThreads, smem,
+                (cudaStream_t)stream, p);
 }
 
 }  // extern "C"
