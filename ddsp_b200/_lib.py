@@ -89,6 +89,16 @@ _lib = None
 _lock = threading.Lock()
 
 
+def bind(path):
+  """Opens the library at `path` and gives each C entry point its header signature."""
+  lib = ctypes.CDLL(path)
+  for name, (restype, argtypes) in SIGNATURES.items():
+    fn = getattr(lib, name)  # AttributeError if the .so lacks a symbol
+    fn.restype = restype
+    fn.argtypes = argtypes
+  return lib
+
+
 def load():
   """Loads the library once; raises RuntimeError loudly if it is absent."""
   global _lib
@@ -102,12 +112,7 @@ def load():
           'ddsp_b200: %s is missing. The CUDA extension is the product - '
           'there is no CPU fallback. Build it with `python -m ddsp_b200.build` '
           '(or __graft_entry__.build()).' % LIB_PATH)
-    lib = ctypes.CDLL(LIB_PATH)
-    for name, (restype, argtypes) in SIGNATURES.items():
-      fn = getattr(lib, name)  # AttributeError if the .so lacks a symbol
-      fn.restype = restype
-      fn.argtypes = argtypes
-    _lib = lib
+    _lib = bind(LIB_PATH)
   return _lib
 
 

@@ -25,7 +25,6 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -33,41 +32,10 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import losses  # noqa: E402
+from tools import measure  # noqa: E402
 
 DEV = 'cuda'
 HALF_LOG_2PI = 0.5 * math.log(2 * math.pi)
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
-
-
-def _time(fn, iters, warmup=3):
-  for _ in range(warmup):
-    fn()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  torch.cuda.synchronize()
-  start.record()
-  for _ in range(iters):
-    fn()
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters * 1e-3
-
-
-def _peak(fn):
-  torch.cuda.synchronize()
-  base = torch.cuda.memory_allocated()
-  torch.cuda.reset_peak_memory_stats()
-  fn()
-  torch.cuda.synchronize()
-  return torch.cuda.max_memory_allocated() - base
 
 
 # ---- the reference formulation, float32 torch ------------------------------------
@@ -180,21 +148,16 @@ def main():
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('consistency_time.py needs a CUDA device')
+  measure.require_cuda('consistency_time.py')
   torch.backends.cuda.matmul.allow_tf32 = False
-  card = _card()
+  card = measure.card()
   rows = []
   for name, ours, theirs, evals in configs():
-    t_ours, t_ref = [], []
-    for _ in range(args.rounds):
-      t_ours.append(_time(ours, args.iters))
-      t_ref.append(_time(theirs, max(2, args.iters // 4)))
+    t = measure.alternate({'ms': ours, 'torch_ms': theirs}, args.rounds,
+                          {'ms': args.iters, 'torch_ms': max(2, args.iters // 4)}, 3)
     torch.cuda.empty_cache()
-    row = {'config': name, 'ms': sorted(t_ours)[len(t_ours) // 2] * 1e3,
-           'torch_ms': sorted(t_ref)[len(t_ref) // 2] * 1e3,
-           'peak_mb': _peak(ours) / 2**20, 'torch_peak_mb': _peak(theirs) / 2**20,
-           'component_evals': evals}
+    row = {'config': name, **t, 'peak_mb': measure.peak_bytes(ours) / 2**20,
+           'torch_peak_mb': measure.peak_bytes(theirs) / 2**20, 'component_evals': evals}
     row['evals_per_s'] = evals / (row['ms'] * 1e-3)
     row['torch_evals_per_s'] = evals / (row['torch_ms'] * 1e-3)
     row.update(card)
@@ -202,8 +165,7 @@ def main():
     print(json.dumps(row), flush=True)
     torch.cuda.empty_cache()
   if args.out:
-    with open(args.out, 'w') as f:
-      json.dump(rows, f, indent=1)
+    measure.append_rows(args.out, rows)
 
 
 if __name__ == '__main__':

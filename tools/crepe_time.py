@@ -17,7 +17,6 @@ the card name and power limit read in the same run."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -25,21 +24,12 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import spectral_ops  # noqa: E402
+from tools import measure  # noqa: E402
 
 DEV = 'cuda'
 B, SECONDS, SR, HOP = 64, 4, 16000, 64
 N = SECONDS * SR
 T = 1 + N // HOP
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
 
 
 # ---- torch compositions of the reference's ops ----------------------------------------
@@ -86,28 +76,15 @@ def torch_decode(acts):
   return 10 * 2 ** (f0_cent / 1200.0), confidence
 
 
-def _time(fn, iters):
-  fn()
-  torch.cuda.synchronize()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  start.record()
-  for _ in range(iters):
-    fn()
-  stop.record()
-  stop.synchronize()
-  return start.elapsed_time(stop) / iters
-
-
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--iters', type=int, default=20)
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('crepe_time.py needs a CUDA device')
+  measure.require_cuda('crepe_time.py')
   torch.manual_seed(0)
-  card = _card()
+  card = measure.card()
   print(card)
   audio = torch.randn(B, N, device=DEV) * 0.1
   centre = torch.clamp(180 + torch.cumsum(torch.randn(B, T, device=DEV) * 3, -1), 0, 359)
@@ -138,20 +115,13 @@ def main():
   lines = []
   with torch.no_grad():
     for what, (cuda_fn, torch_fn, iters) in cases.items():
-      cuda_ms, torch_ms = [], []
-      for _ in range(args.rounds):
-        cuda_ms.append(_time(cuda_fn, iters))
-        torch_ms.append(_time(torch_fn, iters))
-      line = dict(card, config=f'B={B} T={T} hop={HOP} center', what=what,
-                  cuda_ms=float(np.median(cuda_ms)), torch_ms=float(np.median(torch_ms)),
+      t = measure.alternate({'cuda_ms': cuda_fn, 'torch_ms': torch_fn}, args.rounds, iters, 1)
+      line = dict(card, config=f'B={B} T={T} hop={HOP} center', what=what, **t,
                   agreement=checks[what](), iters=iters, rounds=args.rounds)
       print(json.dumps(line))
       lines.append(line)
   if args.out:
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, 'a') as f:
-      for line in lines:
-        f.write(json.dumps(line) + '\n')
+    measure.append_rows(args.out, lines)
 
 
 if __name__ == '__main__':

@@ -15,27 +15,16 @@ the card name and power limit read in the same run."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
-import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import autograd  # noqa: E402
+from tools import measure  # noqa: E402
 
 DEV = 'cuda'
 B, N = 64, 64000
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
 
 
 def torch_frames(audio, hop):
@@ -52,28 +41,15 @@ def _step(frames_fn, audio, grad, hop):
   return x.grad
 
 
-def _time(fn, iters):
-  fn()
-  torch.cuda.synchronize()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  start.record()
-  for _ in range(iters):
-    fn()
-  stop.record()
-  stop.synchronize()
-  return start.elapsed_time(stop) / iters
-
-
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--iters', type=int, default=20)
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('embedding_loss_time.py needs a CUDA device')
+  measure.require_cuda('embedding_loss_time.py')
   torch.manual_seed(0)
-  card = _card()
+  card = measure.card()
   print(card)
   audio = torch.randn(B, N, device=DEV) * 0.1
   cuda_frames = lambda x, hop: autograd.CrepeLossFramesFn.apply(x, hop, True)
@@ -83,10 +59,8 @@ def main():
     grad = torch.randn(B, f, 1024, device=DEV)
     cuda_fn = lambda: _step(cuda_frames, audio, grad, hop)
     torch_fn = lambda: _step(torch_frames, audio, grad, hop)
-    cuda_ms, torch_ms = [], []
-    for _ in range(args.rounds):
-      cuda_ms.append(_time(cuda_fn, args.iters))
-      torch_ms.append(_time(torch_fn, args.iters))
+    t = measure.alternate({'cuda_ms': cuda_fn, 'torch_ms': torch_fn}, args.rounds,
+                          args.iters, 1)
     got, want = cuda_fn(), torch_fn()
     with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
       cuda_fn()
@@ -94,18 +68,14 @@ def main():
     kernels = {e.key: round(e.device_time_total / 1e3, 4) for e in prof.key_averages()
                if 'crepe' in e.key}
     line = dict(card, config=f'B={B} N={N} hop={hop} center frames={f}',
-                what='frames forward + backward', cuda_ms=float(np.median(cuda_ms)),
-                torch_ms=float(np.median(torch_ms)),
+                what='frames forward + backward', **t,
                 grad_rel_diff=float((got - want).abs().max() / want.abs().max()),
                 kernel_ms=kernels,
                 iters=args.iters, rounds=args.rounds)
     print(json.dumps(line))
     lines.append(line)
   if args.out:
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, 'a') as f:
-      for line in lines:
-        f.write(json.dumps(line) + '\n')
+    measure.append_rows(args.out, lines)
 
 
 if __name__ == '__main__':

@@ -13,46 +13,18 @@ power limit read in the same run.
 
   python tools/fir_backward_time.py [--iters 50]"""
 import argparse
+import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import _lib, core  # noqa: E402
+from tools import measure  # noqa: E402
 
-L2_BYTES = 50 << 20
 SAME = _lib.PAD_SAME
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return '%s (%s)' % (torch.cuda.get_device_name(), q)
-
-
-def _ms(fn, iters, warmup=3):
-  """Mean ms of fn(i) over `iters` launches, i the launch number."""
-  for i in range(warmup):
-    fn(i)
-  torch.cuda.synchronize()
-  e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  e0.record()
-  for i in range(iters):
-    fn(i)
-  e1.record()
-  torch.cuda.synchronize()
-  return e0.elapsed_time(e1) / iters
-
-
-def _copies(nbytes):
-  return max(2, math.ceil(2 * L2_BYTES / max(nbytes, 1)))
 
 
 def _torch_filter32(x, mags, ws):
@@ -97,7 +69,7 @@ def _filter_shape(label, B, F, nb, ws, iters):
   st = torch.cuda.current_stream().cuda_stream
   S = core._ir_size(nb, ws)
   per_set = 4 * (2 * B * N + B * F * nb + B * F * S)
-  R = _copies(per_set)
+  R = measure.ring_len(per_set)
   xs = [torch.randn(B, N, device='cuda') for _ in range(R)]
   ms = [torch.rand(B, F, nb, device='cuda') + 0.05 for _ in range(R)]
   gs = [torch.randn(B, N, device='cuda') for _ in range(R)]
@@ -108,22 +80,24 @@ def _filter_shape(label, B, F, nb, ws, iters):
   print('%s: B=%d N=%d F=%d nb=%d window %d (S=%d), %d input copies' %
         (label, B, N, F, nb, ws, S, R), flush=True)
 
+  ring, warmup = range(R), max(3, R)     # warm-up touches every input set
+
   def fwd(i):
     with torch.no_grad():
-      return core.frequency_filter(xs[i % R], ms[i % R], window_size=ws)
-  t_fwd = _ms(fwd, iters)
+      return core.frequency_filter(xs[i], ms[i], window_size=ws)
+  t_fwd = measure.event_ms(fwd, iters, warmup, ring)
   print('  forward (IR + FIR)                     %8.3f ms' % t_fwd, flush=True)
 
   def k_audio(i):
     _lib.check(lib.ddsp_b200_fir_time_varying_backward(
-        xs[i % R].data_ptr(), irs[i % R].data_ptr(), gs[i % R].data_ptr(), d_audio.data_ptr(),
+        xs[i].data_ptr(), irs[i].data_ptr(), gs[i].data_ptr(), d_audio.data_ptr(),
         None, B, N, F, S, B, SAME, -1, None, 0, st))
   nbytes = lib.ddsp_b200_fir_time_varying_backward_workspace(B, N, F, S, B)
   wsb = torch.empty(max(nbytes, 1), dtype=torch.uint8, device='cuda')
 
   def k_ir(i):
     _lib.check(lib.ddsp_b200_fir_time_varying_backward(
-        xs[i % R].data_ptr(), irs[i % R].data_ptr(), gs[i % R].data_ptr(), None,
+        xs[i].data_ptr(), irs[i].data_ptr(), gs[i].data_ptr(), None,
         d_ir.data_ptr(), B, N, F, S, B, SAME, -1, wsb.data_ptr(), nbytes, st))
 
   def k_irb(i):
@@ -134,10 +108,11 @@ def _filter_shape(label, B, F, nb, ws, iters):
 
   def k_mags(i):        # the entry point's own d magnitudes route
     _lib.check(lib.ddsp_b200_frequency_filter_backward(
-        xs[i % R].data_ptr(), irs[i % R].data_ptr(), gs[i % R].data_ptr(), None,
+        xs[i].data_ptr(), irs[i].data_ptr(), gs[i].data_ptr(), None,
         d_mags.data_ptr(), B, F, nb, N, B, ws, SAME, fwsb.data_ptr(), fnbytes, st))
   route = 'fused noise_backward_kernel' if fnbytes == 0 else 'd IR + IR adjoint'
-  t_a, t_ir, t_irb, t_m = (_ms(k, iters) for k in (k_audio, k_ir, k_irb, k_mags))
+  t_a, t_ir, t_irb, t_m = (measure.event_ms(k, iters, warmup, ring)
+                           for k in (k_audio, k_ir, k_irb, k_mags))
   fma = B * N * S
   print('  d audio   fir_adjoint_kernel           %8.3f ms  (%.1f TFMA/s)' %
         (t_a, fma / t_a / 1e9))
@@ -151,19 +126,20 @@ def _filter_shape(label, B, F, nb, ws, iters):
   m1s = [m.clone().requires_grad_(True) for m in ms]
 
   def fwd_bwd(i):
-    x1, m1 = x1s[i % R], m1s[i % R]
+    x1, m1 = x1s[i], m1s[i]
     x1.grad = m1.grad = None
-    core.frequency_filter(x1, m1, window_size=ws).backward(gs[i % R])
-  t_fb = _ms(fwd_bwd, iters)
+    core.frequency_filter(x1, m1, window_size=ws).backward(gs[i])
+  t_fb = measure.event_ms(fwd_bwd, iters, warmup, ring)
   print('  forward + .backward()                  %8.3f ms   backward %.3f ms' %
         (t_fb, t_fb - t_fwd), flush=True)
   del x1s, m1s
 
-  def torch_fb(i):
+  def torch_fb():
     x1 = xs[0].clone().requires_grad_(True)
     m1 = ms[0].clone().requires_grad_(True)
     _torch_filter32(x1, m1, ws).backward(gs[0])
-  print('  float32 torch autograd                 %8.3f ms' % _ms(torch_fb, 5, 1), flush=True)
+  print('  float32 torch autograd                 %8.3f ms' % measure.event_ms(torch_fb, 5, 1),
+        flush=True)
   torch.cuda.empty_cache()
 
 
@@ -171,7 +147,8 @@ def _reverb_shape(B, S, iters):
   N = 64000
   lib = _lib.load()
   st = torch.cuda.current_stream().cuda_stream
-  R = _copies(4 * (2 * B * N + B * S))
+  R = measure.ring_len(4 * (2 * B * N + B * S))
+  ring, warmup = range(R), max(3, R)     # warm-up touches every input set
   xs = [torch.randn(B, N, device='cuda') for _ in range(R)]
   hs = [torch.randn(B, S, device='cuda') / 45.0 for _ in range(R)]
   gs = [torch.randn(B, N, device='cuda') for _ in range(R)]
@@ -184,19 +161,19 @@ def _reverb_shape(B, S, iters):
 
   def fwd(i):
     with torch.no_grad():
-      return core.fft_convolve(xs[i % R], hs[i % R], delay_compensation=0)
+      return core.fft_convolve(xs[i], hs[i], delay_compensation=0)
 
   def k_audio(i):
     _lib.check(lib.ddsp_b200_fir_time_varying_backward(
-        xs[i % R].data_ptr(), hs[i % R].data_ptr(), gs[i % R].data_ptr(), d_audio.data_ptr(),
+        xs[i].data_ptr(), hs[i].data_ptr(), gs[i].data_ptr(), d_audio.data_ptr(),
         None, B, N, 1, S, B, SAME, 0, None, 0, st))
 
   def k_ir(i):
     _lib.check(lib.ddsp_b200_fir_time_varying_backward(
-        xs[i % R].data_ptr(), hs[i % R].data_ptr(), gs[i % R].data_ptr(), None,
+        xs[i].data_ptr(), hs[i].data_ptr(), gs[i].data_ptr(), None,
         d_ir.data_ptr(), B, N, 1, S, B, SAME, 0, wsb.data_ptr(), nbytes, st))
   fma = B * N * S
-  t_f, t_a, t_ir = (_ms(k, iters) for k in (fwd, k_audio, k_ir))
+  t_f, t_a, t_ir = (measure.event_ms(k, iters, warmup, ring) for k in (fwd, k_audio, k_ir))
   print('  forward (fir_kernel)                   %8.3f ms  (%.1f TFMA/s)' % (t_f, fma / t_f / 1e9))
   print('  d audio   fir_adjoint_kernel           %8.3f ms  (%.1f TFMA/s)' % (t_a, fma / t_a / 1e9))
   print('  d IR      fir_dir_kernel + reduce      %8.3f ms  (%.1f TFMA/s)' % (t_ir, fma / t_ir / 1e9))
@@ -204,19 +181,20 @@ def _reverb_shape(B, S, iters):
   h1s = [h.clone().requires_grad_(True) for h in hs]
 
   def fwd_bwd(i):
-    x1, h1 = x1s[i % R], h1s[i % R]
+    x1, h1 = x1s[i], h1s[i]
     x1.grad = h1.grad = None
-    core.fft_convolve(x1, h1, delay_compensation=0).backward(gs[i % R])
-  t_fb = _ms(fwd_bwd, iters)
+    core.fft_convolve(x1, h1, delay_compensation=0).backward(gs[i])
+  t_fb = measure.event_ms(fwd_bwd, iters, warmup, ring)
   print('  forward + .backward()                  %8.3f ms   backward %.3f ms' %
         (t_fb, t_fb - t_f), flush=True)
   del x1s, h1s
 
-  def torch_fb(i):
+  def torch_fb():
     x1 = xs[0].clone().requires_grad_(True)
     h1 = hs[0].clone().requires_grad_(True)
     _torch_convolve32(x1, h1[:, None, :], 0).backward(gs[0])
-  print('  float32 torch autograd                 %8.3f ms' % _ms(torch_fb, 5, 1), flush=True)
+  print('  float32 torch autograd                 %8.3f ms' % measure.event_ms(torch_fb, 5, 1),
+        flush=True)
   torch.cuda.empty_cache()
 
 
@@ -224,7 +202,8 @@ def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--iters', type=int, default=50)
   args = ap.parse_args()
-  print(_card(), flush=True)
+  measure.require_cuda('fir_backward_time.py')
+  print(json.dumps(measure.card()), flush=True)
   torch.manual_seed(0)
   _filter_shape('(a) FIRFilter', 32, 1000, 65, 257, args.iters)
   _filter_shape('(a) FIRFilter', 256, 1000, 65, 257, args.iters)

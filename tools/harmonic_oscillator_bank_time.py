@@ -25,7 +25,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import core  # noqa: E402
-from tools.oscillator_bank_time import HBM_BYTES_PER_S, _card, _ms, _ring  # noqa: E402
+from tools import measure  # noqa: E402
 
 
 def _torch_reference(f, a, init, sr):
@@ -36,7 +36,7 @@ def _torch_reference(f, a, init, sr):
 
 def _shape(B, N, K, iters, with_torch, sr=16000.0):
   gen = torch.Generator(device='cuda').manual_seed(B * K)
-  n = _ring(4 * (2 * B * N * K + 3 * B * N))
+  n = measure.ring_len(4 * (2 * B * N * K + 3 * B * N))
   fs = [torch.rand(B, N, 1, device='cuda', generator=gen) * 600 + 60 for _ in range(n)]
   as_ = [torch.rand(B, N, K, device='cuda', generator=gen) * 0.05 for _ in range(n)]
   ps = [torch.rand(B, 1, 1, device='cuda', generator=gen) * 6 for _ in range(n)]
@@ -59,16 +59,17 @@ def _shape(B, N, K, iters, with_torch, sr=16000.0):
     out, fin = _torch_reference(f, a, p, sr)
     ((out * gs[i]).sum() + fin.sum()).backward()
 
+  ring, few = range(n), max(3, iters // 4)
   res = {'shape': [B, N, K]}
-  res['forward_ms'] = _ms(fwd, n, iters)
-  res['backward_ms'] = _ms(bwd, n, iters)
-  res['backward_da_only_ms'] = _ms(lambda i: bwd(i, False), n, iters)
+  res['forward_ms'] = measure.event_ms(fwd, iters, 2 * n, ring)
+  res['backward_ms'] = measure.event_ms(bwd, iters, 2 * n, ring)
+  res['backward_da_only_ms'] = measure.event_ms(lambda i: bwd(i, False), iters, 2 * n, ring)
   if with_torch:
-    res['torch_forward_ms'] = _ms(lambda i: _torch_reference(fs[i], as_[i], ps[i], sr), n,
-                                  max(3, iters // 4))
-    res['torch_forward_backward_ms'] = _ms(torch_train, n, max(3, iters // 4))
-  res['forward_floor_ms'] = 4 * (B * N * K + 2 * B * N) / HBM_BYTES_PER_S * 1e3
-  res['backward_floor_ms'] = 4 * (2 * B * N * K + 3 * B * N) / HBM_BYTES_PER_S * 1e3
+    res['torch_forward_ms'] = measure.event_ms(
+        lambda i: _torch_reference(fs[i], as_[i], ps[i], sr), few, 2 * n, ring)
+    res['torch_forward_backward_ms'] = measure.event_ms(torch_train, few, 2 * n, ring)
+  res['forward_floor_ms'] = 4 * (B * N * K + 2 * B * N) / measure.HBM_BYTES_PER_S * 1e3
+  res['backward_floor_ms'] = 4 * (2 * B * N * K + 3 * B * N) / measure.HBM_BYTES_PER_S * 1e3
   return res
 
 
@@ -77,15 +78,14 @@ def main():
   ap.add_argument('--iters', type=int, default=20)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  res = {'card': _card(),
+  measure.require_cuda('harmonic_oscillator_bank_time.py')
+  res = {'card': measure.card(),
          'shapes': [_shape(32, 64000, 64, args.iters, True),
                     _shape(1, 1000000, 1, args.iters, False),
                     _shape(1, 64000, 64, args.iters, False)]}
-  line = json.dumps(res)
-  print(line)
+  print(json.dumps(res))
   if args.out:
-    with open(args.out, 'a') as fh:
-      fh.write(line + '\n')
+    measure.append_rows(args.out, [res])
 
 
 if __name__ == '__main__':

@@ -16,7 +16,6 @@ reference sources) and labels the line as CPU."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -24,6 +23,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from tests.golden import make_heuristics_golden as mk  # noqa: E402
+from tools import measure  # noqa: E402
 
 SIZES = ((32, 1001), (8, 15001))
 
@@ -31,16 +31,6 @@ SIZES = ((32, 1001), (8, 15001))
 def _inputs(b, t):
   f0, amps = zip(*(mk.track(t, 100 + i) for i in range(b)))
   return np.stack(f0), np.stack(amps)
-
-
-def _card(torch):
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
 
 
 # ---- the composition in float32 torch ------------------------------------------------------
@@ -92,20 +82,9 @@ def torch_note_table(torch, mask, f0):
   return sb, ss, se, pitch
 
 
-def _events(torch, fn, iters):
-  fn()
-  torch.cuda.synchronize()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  start.record()
-  for _ in range(iters):
-    fn()
-  stop.record()
-  stop.synchronize()
-  return start.elapsed_time(stop) / iters
-
-
 def gpu(args):
   import torch
+  measure.require_cuda('heuristics_time.py')
   from ddsp_b200 import heuristics as h
   rows = []
   for b, t in SIZES:
@@ -122,16 +101,13 @@ def gpu(args):
       m = torch_midi_heuristic(torch, f2, a2)
       return m, torch_note_table(torch, m, f2)
 
-    cuda_ms, torch_ms = [], []
-    for _ in range(args.rounds):
-      cuda_ms.append(_events(torch, ours, args.iters))
-      torch_ms.append(_events(torch, theirs, args.iters))
+    times = measure.alternate({'cuda_ms': ours, 'torch_ms': theirs}, args.rounds,
+                              args.iters, 1)
     mine = h.midi_heuristic(c)
     table = h.note_table(mine, f0)
     m, (_, _, _, pitch) = theirs()
-    row = dict(_card(torch), config=f'B={b} T={t}',
-               what='midi_heuristic + note_table (mean)',
-               cuda_ms=float(np.median(cuda_ms)), torch_ms=float(np.median(torch_ms)),
+    row = dict(measure.card(), config=f'B={b} T={t}',
+               what='midi_heuristic + note_table (mean)', **times,
                mask_frames_differ=int((mine != m).sum()),
                notes=int(table.count.sum()), torch_notes=int(pitch.numel()),
                iters=args.iters, rounds=args.rounds)
@@ -167,10 +143,7 @@ def main():
   args = ap.parse_args()
   rows = reference(args) if args.reference else gpu(args)
   if args.out:
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, 'a') as f:
-      for r in rows:
-        f.write(json.dumps(r) + '\n')
+    measure.append_rows(args.out, rows)
 
 
 if __name__ == '__main__':

@@ -22,7 +22,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import core, losses  # noqa: E402
-from tools.consistency_time import _card, _peak, _time  # noqa: E402
+from tools import measure  # noqa: E402
 
 DEV = 'cuda'
 T, K = 1000, 128
@@ -72,11 +72,11 @@ def main():
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  assert torch.cuda.is_available(), 'hmm_time.py measures on a CUDA device'
+  measure.require_cuda('hmm_time.py')
   hmm = losses.HmmTranscriber(n_timesteps=T, n_pitches=K)
   loc, scale = (torch.as_tensor(v, device=DEV) for v in (hmm.loc, hmm.scale))
   dense = dense_params(hmm)
-  result = {'card': _card(), 'T': T, 'K': K, 'rows': []}
+  result = {'card': measure.card(), 'T': T, 'K': K, 'rows': []}
   for b in (16, 256):
     rng = np.random.default_rng(b)
     x = torch.as_tensor(np.stack([rng.integers(1, K, (b, T)) + 0.2 * rng.normal(size=(b, T)),
@@ -109,13 +109,11 @@ def main():
     pairs = {'log_prob': (cuda_fwd, torch_fwd), 'log_prob+backward': (cuda_bwd, torch_bwd),
              'viterbi': (cuda_vit, torch_vit)}
     for name, (c, r) in pairs.items():
-      tc, tr = [], []
-      for _ in range(args.rounds):
-        tc.append(_time(c, args.iters))
-        tr.append(_time(r, max(1, args.iters // 5), warmup=1))
-      row = {'B': b, 'op': name, 'cuda_ms': 1e3 * float(np.median(tc)),
-             'torch_ms': 1e3 * float(np.median(tr)),
-             'cuda_peak_MB': _peak(c) / 2**20, 'torch_peak_MB': _peak(r) / 2**20}
+      t = measure.alternate({'cuda_ms': c, 'torch_ms': r}, args.rounds,
+                            {'cuda_ms': args.iters, 'torch_ms': max(1, args.iters // 5)},
+                            {'cuda_ms': 3, 'torch_ms': 1})
+      row = {'B': b, 'op': name, **t, 'cuda_peak_MB': measure.peak_bytes(c) / 2**20,
+             'torch_peak_MB': measure.peak_bytes(r) / 2**20}
       row['speedup'] = row['torch_ms'] / row['cuda_ms']
       result['rows'].append(row)
       print(json.dumps(row), flush=True)
@@ -124,9 +122,7 @@ def main():
   result['log_prob_max_rel_vs_float64'] = float(((lp.double() - ref) / ref).abs().max())
   print(json.dumps({k: v for k, v in result.items() if k != 'rows'}))
   if args.out:
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, 'w') as f:
-      json.dump(result, f, indent=1)
+    measure.append_rows(args.out, [result])
 
 
 if __name__ == '__main__':

@@ -23,7 +23,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import core  # noqa: E402
-from tools.oscillator_bank_time import HBM_BYTES_PER_S, _card, _ms, _ring  # noqa: E402
+from tools import measure  # noqa: E402
 
 
 def _torch_reference(phase, tab):
@@ -39,7 +39,7 @@ def _torch_reference(phase, tab):
 def _case(B, N, W, per_sample, iters):
   gen = torch.Generator(device='cuda').manual_seed(W)
   tshape = (B, N, W) if per_sample else (B, W)
-  n = _ring(4 * (3 * B * N + 2 * B * (N if per_sample else 1) * W))
+  n = measure.ring_len(4 * (3 * B * N + 2 * B * (N if per_sample else 1) * W))
   ph = [torch.rand(B, N, device='cuda', generator=gen) for _ in range(n)]
   tabs = [torch.randn(tshape, device='cuda', generator=gen) for _ in range(n)]
   gs = [torch.randn(B, N, device='cuda', generator=gen) for _ in range(n)]
@@ -64,17 +64,18 @@ def _case(B, N, W, per_sample, iters):
     (_torch_reference(p, t) * gs[i][:, :nt]).sum().backward()
 
   tab_bytes = 4 * B * (N if per_sample else 1) * W
+  ring, few = range(n), max(3, iters // 4)
   res = {'tables': list(tshape)}
-  res['forward_ms'] = _ms(fwd, n, iters)
-  res['backward_ms'] = _ms(bwd, n, iters)
-  few = max(3, iters // 4)
-  res['torch_forward_ms'] = scale * _ms(lambda i: _torch_reference(ph[i][:, :nt], torch_tab(i)),
-                                        n, few)
-  res['torch_forward_backward_ms'] = scale * _ms(torch_train, n, few)
+  res['forward_ms'] = measure.event_ms(fwd, iters, 2 * n, ring)
+  res['backward_ms'] = measure.event_ms(bwd, iters, 2 * n, ring)
+  res['torch_forward_ms'] = scale * measure.event_ms(
+      lambda i: _torch_reference(ph[i][:, :nt], torch_tab(i)), few, 2 * n, ring)
+  res['torch_forward_backward_ms'] = scale * measure.event_ms(torch_train, few, 2 * n, ring)
   if scale != 1:
     res['torch_note'] = 'torch run on %d samples per item, times scaled by %g' % (nt, scale)
-  res['forward_floor_ms'] = (8 * B * N + (32 * B * N if per_sample else 0)) / HBM_BYTES_PER_S * 1e3
-  res['backward_floor_ms'] = (12 * B * N + tab_bytes) / HBM_BYTES_PER_S * 1e3
+  res['forward_floor_ms'] = ((8 * B * N + (32 * B * N if per_sample else 0)) /
+                             measure.HBM_BYTES_PER_S * 1e3)
+  res['backward_floor_ms'] = (12 * B * N + tab_bytes) / measure.HBM_BYTES_PER_S * 1e3
   return res
 
 
@@ -83,13 +84,12 @@ def main():
   ap.add_argument('--iters', type=int, default=20)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  res = {'card': _card(), 'per_item': _case(32, 64000, 2048, False, args.iters),
+  measure.require_cuda('linear_lookup_time.py')
+  res = {'card': measure.card(), 'per_item': _case(32, 64000, 2048, False, args.iters),
          'per_sample': _case(4, 16000, 512, True, args.iters)}
-  line = json.dumps(res)
-  print(line)
+  print(json.dumps(res))
   if args.out:
-    with open(args.out, 'a') as fh:
-      fh.write(line + '\n')
+    measure.append_rows(args.out, [res])
 
 
 if __name__ == '__main__':

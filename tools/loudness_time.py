@@ -24,45 +24,16 @@ import argparse
 import json
 import math
 import os
-import subprocess
+import statistics
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import losses, spectral_ops  # noqa: E402
+from tools import measure  # noqa: E402
 
-HBM_PEAK = 3.35e12
-FP32_PEAK = 67e12
 DEV = 'cuda'
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
-
-
-def _time(fn, iters, warmup=3):
-  for _ in range(warmup):
-    fn()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  torch.cuda.synchronize()
-  start.record()
-  for _ in range(iters):
-    fn()
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters * 1e-3
-
-
-def _median(xs):
-  xs = sorted(xs)
-  return xs[len(xs) // 2]
 
 
 def torch_loudness(audio, n_fft, hop=64, sample_rate=16000):
@@ -93,8 +64,9 @@ def main():
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
+  measure.require_cuda('loudness_time.py')
   torch.backends.cuda.matmul.allow_tf32 = False
-  res = {'card': _card(), 'rows': []}
+  res = {'card': measure.card(), 'rows': []}
   gen = torch.Generator(DEV).manual_seed(0)
   B, N = 128, 64000
   audio = torch.rand((B, N), device=DEV, generator=gen) * 2 - 1
@@ -119,25 +91,27 @@ def main():
       a.grad = None
       torch_loudness(a, n_fft).backward(g)
 
-    times = {k: [] for k in ('ours_fwd', 'ours_fwd_bwd', 'torch_fwd', 'torch_fwd_bwd')}
-    for _ in range(args.rounds):
-      times['ours_fwd'].append(_time(ours_fwd, args.iters))
-      times['torch_fwd'].append(_time(torch_fwd, max(2, args.iters // 4)))
-      times['ours_fwd_bwd'].append(_time(ours_fb, args.iters))
-      times['torch_fwd_bwd'].append(_time(torch_fb, max(2, args.iters // 4)))
-    t = {k: _median(v) for k, v in times.items()}
+    few = max(2, args.iters // 4)
+    runs = (('ours_fwd', ours_fwd, args.iters), ('torch_fwd', torch_fwd, few),
+            ('ours_fwd_bwd', ours_fb, args.iters), ('torch_fwd_bwd', torch_fb, few))
+    times = {k: [] for k, _, _ in runs}
+    for _ in range(args.rounds):     # alternated rounds, each kept for the spread
+      for k, fn, n in runs:
+        times[k].append(measure.event_ms(fn, n, 3))
+    t = {k: statistics.median(v) * 1e-3 for k, v in times.items()}
     t_bwd = t['ours_fwd_bwd'] - t['ours_fwd']
     f_fwd, f_bwd = _flops(B * T, n_fft, False), _flops(B * T, n_fft, True)
     bytes_fwd, bytes_bwd = 4.0 * (B * N + B * T), 4.0 * (2 * B * N + B * T)
+    fp32, hbm = measure.FP32_FLOPS_PER_S, measure.HBM_BYTES_PER_S
     row = {'what': 'loudness', 'B': B, 'N': N, 'n_fft': n_fft, 'frames': B * T,
            'fwd_ms': t['ours_fwd'] * 1e3, 'bwd_ms': t_bwd * 1e3,
            'fwd_bwd_ms': t['ours_fwd_bwd'] * 1e3,
            'torch_fwd_ms': t['torch_fwd'] * 1e3, 'torch_fwd_bwd_ms': t['torch_fwd_bwd'] * 1e3,
            'fwd_tflops': f_fwd / t['ours_fwd'] / 1e12, 'bwd_tflops': f_bwd / t_bwd / 1e12,
-           'fwd_share_of_peak': max(f_fwd / FP32_PEAK, bytes_fwd / HBM_PEAK) / t['ours_fwd'],
-           'bwd_share_of_peak': max(f_bwd / FP32_PEAK, bytes_bwd / HBM_PEAK) / t_bwd,
-           'bound': 'FP32' if f_fwd / FP32_PEAK > bytes_fwd / HBM_PEAK else 'HBM',
-           'spread_fwd_ms': [round(x * 1e3, 4) for x in times['ours_fwd']]}
+           'fwd_share_of_peak': max(f_fwd / fp32, bytes_fwd / hbm) / t['ours_fwd'],
+           'bwd_share_of_peak': max(f_bwd / fp32, bytes_bwd / hbm) / t_bwd,
+           'bound': 'FP32' if f_fwd / fp32 > bytes_fwd / hbm else 'HBM',
+           'spread_fwd_ms': [round(x, 4) for x in times['ours_fwd']]}
     res['rows'].append(row)
     print(json.dumps(row), flush=True)
     del a, g
@@ -151,9 +125,9 @@ def main():
     def step():
       a.grad = None
       loss_obj(target, a).backward()
-    ts = [_time(step, max(2, args.iters // 2)) for _ in range(args.rounds)]
+    ts = [measure.event_ms(step, max(2, args.iters // 2), 3) for _ in range(args.rounds)]
     row = {'what': 'spectral_loss_fwd_bwd', 'B': B, 'N': N, 'loudness_weight': lw,
-           'ms': _median(ts) * 1e3, 'spread_ms': [round(x * 1e3, 4) for x in ts]}
+           'ms': statistics.median(ts), 'spread_ms': [round(x, 4) for x in ts]}
     res['rows'].append(row)
     print(json.dumps(row), flush=True)
   del a, target
@@ -162,20 +136,19 @@ def main():
   B2 = 256
   audio2 = torch.rand((B2, N), device=DEV, generator=gen) * 2 - 1
   for frame in (64, 1024):
-    ts = [_time(lambda: spectral_ops.compute_power(audio2, frame_size=frame), args.iters)
-          for _ in range(args.rounds)]
+    ts = [measure.event_ms(lambda: spectral_ops.compute_power(audio2, frame_size=frame),
+                           args.iters, 3) for _ in range(args.rounds)]
     T = spectral_ops.get_framed_lengths(N, frame, 64, 'center')[0]
-    t = _median(ts)
+    t = statistics.median(ts) * 1e-3
     nbytes = 4.0 * (B2 * N + B2 * T)
     row = {'what': 'rms_power', 'B': B2, 'N': N, 'frame_size': frame, 'ms': t * 1e3,
-           'hbm_share': nbytes / HBM_PEAK / t, 'flops': 2.0 * B2 * T * frame,
-           'fp32_share': 2.0 * B2 * T * frame / FP32_PEAK / t}
+           'hbm_share': nbytes / measure.HBM_BYTES_PER_S / t, 'flops': 2.0 * B2 * T * frame,
+           'fp32_share': 2.0 * B2 * T * frame / measure.FP32_FLOPS_PER_S / t}
     res['rows'].append(row)
     print(json.dumps(row), flush=True)
   print(json.dumps(res['card']))
   if args.out:
-    with open(args.out, 'w') as f:
-      json.dump(res, f, indent=1)
+    measure.append_rows(args.out, [res])
 
 
 if __name__ == '__main__':

@@ -23,15 +23,14 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import spectral_ops  # noqa: E402
+from tools import measure  # noqa: E402
 
-FP32_PEAK = 67e12
 DEV = 'cuda'
 CONFIGS = [
     ('mfcc', 'compute_mfcc', dict(lo_hz=20.0, hi_hz=8000.0, fft_size=1024, mel_bins=128,
@@ -40,34 +39,6 @@ CONFIGS = [
                                       overlap=0.75)),
     ('mel', 'compute_mel', dict()),
 ]
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
-
-
-def _time(fn, iters, warmup=3):
-  for _ in range(warmup):
-    fn()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  torch.cuda.synchronize()
-  start.record()
-  for _ in range(iters):
-    fn()
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters * 1e-3
-
-
-def _median(xs):
-  xs = sorted(xs)
-  return xs[len(xs) // 2]
 
 
 def _params(fn, kw):
@@ -133,8 +104,9 @@ def main():
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
+  measure.require_cuda('mel_time.py')
   torch.backends.cuda.matmul.allow_tf32 = False
-  res = {'card': _card(), 'B': 128, 'N': 64000, 'rows': []}
+  res = {'card': measure.card(), 'B': 128, 'N': 64000, 'rows': []}
   gen = torch.Generator(DEV).manual_seed(0)
   B, N = 128, 64000
   audio = torch.rand((B, N), device=DEV, generator=gen) * 2 - 1
@@ -163,27 +135,22 @@ def main():
       a.grad = None
       torch_features(a, fn, p).backward(g)
 
-    times = {k: [] for k in ('ours_fwd', 'ours_fb', 'torch_fwd', 'torch_fb')}
-    for _ in range(args.rounds):
-      for k, f in (('ours_fwd', ours_fwd), ('torch_fwd', torch_fwd), ('ours_fb', ours_fb),
-                   ('torch_fb', torch_fb)):
-        times[k].append(_time(f, args.iters))
-    t = {k: _median(v) for k, v in times.items()}
+    t = measure.alternate({'ours_fwd': ours_fwd, 'torch_fwd': torch_fwd, 'ours_fb': ours_fb,
+                           'torch_fb': torch_fb}, args.rounds, args.iters, 3)
     T = out.shape[1]
     ffw, ffb = _flops(p, B * T, False), _flops(p, B * T, True)
     row = {'config': name, 'fn': fn, 'kwargs': kw, 'frames': T,
-           'ours_fwd_ms': t['ours_fwd'] * 1e3, 'ours_fwd_bwd_ms': t['ours_fb'] * 1e3,
-           'torch_fwd_ms': t['torch_fwd'] * 1e3, 'torch_fwd_bwd_ms': t['torch_fb'] * 1e3,
+           'ours_fwd_ms': t['ours_fwd'], 'ours_fwd_bwd_ms': t['ours_fb'],
+           'torch_fwd_ms': t['torch_fwd'], 'torch_fwd_bwd_ms': t['torch_fb'],
            'fwd_gflop': ffw / 1e9, 'fwd_bwd_gflop': ffb / 1e9,
-           'fwd_fp32_share': ffw / t['ours_fwd'] / FP32_PEAK,
-           'fwd_bwd_fp32_share': ffb / t['ours_fb'] / FP32_PEAK,
+           'fwd_fp32_share': ffw / (t['ours_fwd'] * 1e-3) / measure.FP32_FLOPS_PER_S,
+           'fwd_bwd_fp32_share': ffb / (t['ours_fb'] * 1e-3) / measure.FP32_FLOPS_PER_S,
            'max_abs_vs_torch': float((out - ref).abs().max())}
     res['rows'].append(row)
     print(json.dumps(row), flush=True)
   print(json.dumps({'card': res['card']}))
   if args.out:
-    with open(args.out, 'w') as f:
-      json.dump(res, f, indent=1)
+    measure.append_rows(args.out, [res])
 
 
 if __name__ == '__main__':

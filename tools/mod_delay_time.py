@@ -13,7 +13,6 @@ Prints the card name and power limit read in the same run."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -21,32 +20,9 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import _lib  # noqa: E402
 from ddsp_b200 import core  # noqa: E402
+from tools import measure  # noqa: E402
 
-HBM_PEAK = 3.35e12
 BWD_TILE = 1024      # md_::kTile
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
-
-
-def _time(fn, sets, iters, warmup):
-  for i in range(warmup):
-    fn(sets[i % len(sets)])
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  torch.cuda.synchronize()
-  start.record()
-  for i in range(iters):
-    fn(sets[i % len(sets)])
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters * 1e-3
 
 
 def main():
@@ -57,14 +33,12 @@ def main():
   ap.add_argument('--iters', type=int, default=50)
   ap.add_argument('--warmup', type=int, default=10)
   args = ap.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('mod_delay_time: needs a CUDA device')
+  measure.require_cuda('mod_delay_time.py')
   B, N, L = args.batch, args.n, args.max_length
   lib = _lib.load()
   st = torch.cuda.current_stream().cuda_stream
-  l2 = torch.cuda.get_device_properties(0).L2_cache_size
   set_bytes = 4 * 4 * B * N                      # audio, phase, gain, gradient
-  n_sets = max(2, -(-2 * l2 // set_bytes) + 1)
+  n_sets = measure.ring_len(set_bytes)
   gen = torch.Generator(device='cuda').manual_seed(0)
   t = torch.arange(N, device='cuda') / 16000.0
   sets = []
@@ -94,18 +68,18 @@ def main():
   with torch.no_grad():
     core.mod_delay(sets[0][0], sets[0][2], sets[0][1], L, 0.4, 0.6, True)
   samples = B * N
-  res = {'card': _card(), 'B': B, 'N': N, 'L': L, 'input_sets': n_sets,
-         'ring_bytes': n_sets * set_bytes, 'l2_bytes': l2}
+  res = {'card': measure.card(), 'B': B, 'N': N, 'L': L, 'input_sets': n_sets,
+         'ring_bytes': n_sets * set_bytes, 'l2_bytes': measure.l2_bytes()}
   for name, fn, per_sample, halo in (('forward', fwd, 16, 0.0),
                                      ('backward', bwd, 28, 12.0 * (L - 1) / BWD_TILE)):
-    sec = _time(fn, sets, args.iters, args.warmup)
+    sec = measure.event_ms(fn, args.iters, args.warmup, sets) * 1e-3
     res[name] = {
         'us': sec * 1e6,
         'algorithmic_bytes': per_sample * samples,
         'halo_bytes': halo * samples,
         'achieved_TBps': per_sample * samples / sec / 1e12,
-        'fraction_of_hbm_peak': per_sample * samples / sec / HBM_PEAK,
-        'fraction_with_halo': (per_sample + halo) * samples / sec / HBM_PEAK,
+        'fraction_of_hbm_peak': per_sample * samples / sec / measure.HBM_BYTES_PER_S,
+        'fraction_with_halo': (per_sample + halo) * samples / sec / measure.HBM_BYTES_PER_S,
     }
   print(json.dumps(res))
 

@@ -17,7 +17,6 @@ the card name and power limit read in the same run."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -25,19 +24,10 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import nn  # noqa: E402
+from tools import measure  # noqa: E402
 
 DEV = 'cuda'
 B, T, R, D = 32, 1000, 100, 128
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
 
 
 # ---- the reference's formulas (training/nn.py:375-547) in float32 torch ----------------
@@ -89,34 +79,14 @@ def _run(mask_fn, pool_fn, q, z, w, backward):
   return mean
 
 
-def _time(fn, iters):
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  start.record()
-  for _ in range(iters):
-    fn()
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters
-
-
-def _peak(fn):
-  torch.cuda.synchronize()
-  base = torch.cuda.memory_allocated()
-  torch.cuda.reset_peak_memory_stats()
-  fn()
-  torch.cuda.synchronize()
-  return torch.cuda.max_memory_allocated() - base
-
-
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--iters', type=int, default=20)
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   a = ap.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('notes_time.py needs a CUDA device')
-  card = _card()
+  measure.require_cuda('notes_time.py')
+  card = measure.card()
   q, z = _inputs()
   w = torch.randn((B, T, D), device=DEV)
   ours = (lambda x: nn.get_note_mask(x, R), nn.pool_over_notes)
@@ -126,23 +96,17 @@ def main():
     fns = {name: (lambda f=f: _run(*f, q, z, w, backward)) for name, f in
            (('cuda', ours), ('torch', ref))}
     diff = float((fns['cuda']().detach() - fns['torch']().detach()).abs().max())
-    times = {k: [] for k in fns}
-    for _ in range(a.rounds):
-      for k, f in fns.items():
-        f()
-        times[k].append(_time(f, a.iters))
+    t = measure.alternate(fns, a.rounds, a.iters, 1)
     row = dict(card, config=f'B={B} T={T} R={R} D={D}',
                what='forward+backward' if backward else 'forward',
-               cuda_ms=float(np.median(times['cuda'])), torch_ms=float(np.median(times['torch'])),
-               cuda_peak_bytes=_peak(fns['cuda']), torch_peak_bytes=_peak(fns['torch']),
+               cuda_ms=t['cuda'], torch_ms=t['torch'],
+               cuda_peak_bytes=measure.peak_bytes(fns['cuda']),
+               torch_peak_bytes=measure.peak_bytes(fns['torch']),
                max_abs_diff_pooled_mean=diff, iters=a.iters, rounds=a.rounds)
     rows.append(row)
     print(json.dumps(row), flush=True)
   if a.out:
-    os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-    with open(a.out, 'w') as f:
-      for row in rows:
-        f.write(json.dumps(row) + '\n')
+    measure.append_rows(a.out, rows)
 
 
 if __name__ == '__main__':

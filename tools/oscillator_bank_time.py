@@ -16,44 +16,13 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import core  # noqa: E402
-
-HBM_BYTES_PER_S = 3.35e12     # H100 SXM data sheet
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return '%s (%s)' % (torch.cuda.get_device_name(), q)
-
-
-def _ms(fn, n_ring, iters, warmup=2):
-  """Mean time of fn(i) over `iters` calls, i walking the ring."""
-  for i in range(warmup * n_ring):
-    fn(i % n_ring)
-  torch.cuda.synchronize()
-  e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  e0.record()
-  for i in range(iters):
-    fn(i % n_ring)
-  e1.record()
-  torch.cuda.synchronize()
-  return e0.elapsed_time(e1) / iters
-
-
-def _ring(set_bytes):
-  l2 = torch.cuda.get_device_properties(torch.cuda.current_device()).L2_cache_size
-  return max(1, math.ceil(2 * l2 / set_bytes) + 1)
+from tools import measure  # noqa: E402
 
 
 def _torch_reference(f, a, sr, sum_sinusoids):
@@ -66,7 +35,7 @@ def _bank(B, N, K, sum_sinusoids, iters, sr=16000.0):
   gen = torch.Generator(device='cuda').manual_seed(B * K + sum_sinusoids)
   g_shape = (B, N) if sum_sinusoids else (B, N, K)
   set_bytes = 4 * (2 * B * N * K + math.prod(g_shape))
-  n = _ring(set_bytes)
+  n = measure.ring_len(set_bytes)
   fs = [torch.rand(B, N, K, device='cuda', generator=gen) * 7900 + 20 for _ in range(n)]
   as_ = [torch.rand(B, N, K, device='cuda', generator=gen) * 0.05 for _ in range(n)]
   gs = [torch.randn(g_shape, device='cuda', generator=gen) for _ in range(n)]
@@ -82,17 +51,19 @@ def _bank(B, N, K, sum_sinusoids, iters, sr=16000.0):
   leaves = [(f.clone().requires_grad_(True), a.clone().requires_grad_(True))
             for f, a in zip(fs[:1], as_[:1])]
 
-  def torch_fwd_bwd(i):
+  def torch_fwd_bwd():
     f, a = leaves[0]
     f.grad = a.grad = None
-    _torch_reference(f, a, sr, sum_sinusoids).backward(gs[i])
+    _torch_reference(f, a, sr, sum_sinusoids).backward(gs[0])
 
-  t_f = _ms(fwd, n, iters)
-  t_b = _ms(bwd, n, iters)
-  t_ba = _ms(lambda i: bwd(i, False), n, iters)
-  t_torch_f = _ms(lambda i: _torch_reference(fs[i], as_[i], sr, sum_sinusoids), n, 3, 1)
-  t_torch = _ms(torch_fwd_bwd, 1, 3, 1)
-  floor = 4 * 4 * B * N * K / HBM_BYTES_PER_S * 1e3
+  ring = range(n)
+  t_f = measure.event_ms(fwd, iters, 2 * n, ring)
+  t_b = measure.event_ms(bwd, iters, 2 * n, ring)
+  t_ba = measure.event_ms(lambda i: bwd(i, False), iters, 2 * n, ring)
+  t_torch_f = measure.event_ms(lambda i: _torch_reference(fs[i], as_[i], sr, sum_sinusoids),
+                               3, n, ring)
+  t_torch = measure.event_ms(torch_fwd_bwd, 3, 1)
+  floor = 4 * 4 * B * N * K / measure.HBM_BYTES_PER_S * 1e3
   row = dict(B=B, N=N, K=K, sum_sinusoids=sum_sinusoids, ring=n, forward_ms=t_f,
              backward_ms=t_b, backward_da_only_ms=t_ba, torch_forward_ms=t_torch_f,
              torch_fwd_bwd_ms=t_torch, byte_floor_ms=floor)
@@ -111,21 +82,22 @@ def _bank(B, N, K, sum_sinusoids, iters, sr=16000.0):
 
 def _cumsum(B, N, C, iters):
   gen = torch.Generator(device='cuda').manual_seed(5)
-  n = _ring(4 * 2 * B * N * C)
+  n = measure.ring_len(4 * 2 * B * N * C)
   xs = [torch.rand(B, N, C, device='cuda', generator=gen) * 0.5 for _ in range(n)]
   gs = [torch.randn(B, N, C, device='cuda', generator=gen) for _ in range(n)]
   d = torch.empty_like(xs[0])
   x_leaf = xs[0].clone().requires_grad_(True)
 
-  def torch_fwd_bwd(i):
+  def torch_fwd_bwd():
     x_leaf.grad = None
-    torch.remainder(torch.cumsum(x_leaf, 1), 2 * math.pi).backward(gs[i])
+    torch.remainder(torch.cumsum(x_leaf, 1), 2 * math.pi).backward(gs[0])
 
-  t_f = _ms(lambda i: core.angular_cumsum(xs[i]), n, iters)
-  t_b = _ms(lambda i: core._launch('ddsp_b200_angular_cumsum_backward', gs[i], d, B, N, C),
-            n, iters)
-  t_torch = _ms(torch_fwd_bwd, 1, 3, 1)
-  floor = 2 * 4 * B * N * C / HBM_BYTES_PER_S * 1e3
+  t_f = measure.event_ms(lambda i: core.angular_cumsum(xs[i]), iters, 2 * n, range(n))
+  t_b = measure.event_ms(
+      lambda i: core._launch('ddsp_b200_angular_cumsum_backward', gs[i], d, B, N, C),
+      iters, 2 * n, range(n))
+  t_torch = measure.event_ms(torch_fwd_bwd, 3, 1)
+  floor = 2 * 4 * B * N * C / measure.HBM_BYTES_PER_S * 1e3
   print('angular_cumsum [%d, %d, %d] (ring of %d)' % (B, N, C, n))
   print('  forward %8.3f ms   backward %8.3f ms = %.2fx the %.3f ms byte floor   float32 '
         'torch autograd forward+backward %8.3f ms' % (t_f, t_b, t_b / floor, floor, t_torch),
@@ -139,16 +111,16 @@ def _cumsum(B, N, C, iters):
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--iters', type=int, default=20)
-  ap.add_argument('--out', default=None, help='also write the rows as JSON')
+  ap.add_argument('--out', default=None, help='also append the rows as one JSON line')
   args = ap.parse_args()
-  card = _card()
-  print(card, flush=True)
+  measure.require_cuda('oscillator_bank_time.py')
+  card = measure.card()
+  print(json.dumps(card), flush=True)
   rows = [_bank(32, 64000, 100, True, args.iters), _bank(32, 64000, 100, False, args.iters),
           _bank(4, 64000, 16, True, args.iters), _bank(4, 64000, 16, False, args.iters),
           _cumsum(32, 64000, 100, args.iters)]
   if args.out:
-    with open(args.out, 'w') as fh:
-      json.dump(dict(card=card, rows=rows), fh, indent=1)
+    measure.append_rows(args.out, [dict(card=card, rows=rows)])
 
 
 if __name__ == '__main__':

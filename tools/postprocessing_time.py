@@ -18,7 +18,6 @@ import contextlib
 import io
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -27,18 +26,9 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from tests.golden import make_postprocessing_golden as mk  # noqa: E402
+from tools import measure  # noqa: E402
 
 T = 15000
-
-
-def _card(torch):
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
 
 
 def _clip():
@@ -90,18 +80,6 @@ def _gpu_adjust(post, cu, loud, f0_midi, conf, inv):
     return cu.auto_tune(f0_midi, tf, mask, amount=0.5)
 
 
-def _time_gpu(torch, fn, iters):
-  fn()
-  torch.cuda.synchronize()
-  a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  a.record()
-  for _ in range(iters):
-    fn()
-  b.record()
-  torch.cuda.synchronize()
-  return a.elapsed_time(b) / iters
-
-
 def _time_cpu(fn, iters):
   t0 = time.perf_counter()
   for _ in range(iters):
@@ -111,6 +89,7 @@ def _time_cpu(fn, iters):
 
 def run_gpu(args):
   import torch
+  measure.require_cuda('postprocessing_time.py')
   from ddsp_b200 import colab_utils as cu
   from ddsp_b200 import postprocessing as post
   loud, f0_midi, conf = _clip()
@@ -128,11 +107,11 @@ def run_gpu(args):
   for name, (gpu_fn, cpu_fn) in cases.items():
     g, c = [], []
     for _ in range(args.rounds):
-      g.append(_time_gpu(torch, gpu_fn, args.iters))
+      g.append(measure.event_ms(gpu_fn, args.iters, 1))
       c.append(_time_cpu(cpu_fn, max(1, args.iters // 5)))
     rows.append({'case': name, 'cuda_ms': float(np.median(g)),
                  'cpu_numpy_ms': float(np.median(c)), 'label_cpu': 'CPU (numpy)',
-                 **_card(torch)})
+                 **measure.card()})
   return rows
 
 
@@ -167,11 +146,9 @@ def main():
                                                'postprocessing_h100.jsonl'))
   args = p.parse_args()
   rows = run_reference(args) if args.reference else run_gpu(args)
-  os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-  with open(args.out, 'a') as f:
-    for r in rows:
-      print(json.dumps(r))
-      f.write(json.dumps(r) + '\n')
+  for r in rows:
+    print(json.dumps(r))
+  measure.append_rows(args.out, rows)
 
 
 if __name__ == '__main__':

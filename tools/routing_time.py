@@ -19,7 +19,6 @@ tap (read).  Prints the card name and power limit read in the same run."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -28,31 +27,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import _lib  # noqa: E402
 from ddsp_b200 import core  # noqa: E402
 from ddsp_b200 import effects  # noqa: E402
-
-HBM_PEAK = 3.35e12
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
-
-
-def _time(fn, sets, iters, warmup):
-  for i in range(warmup):
-    fn(sets[i % len(sets)])
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  torch.cuda.synchronize()
-  start.record()
-  for i in range(iters):
-    fn(sets[i % len(sets)])
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters * 1e-3
+from tools import measure  # noqa: E402
 
 
 def _linear_taps(F, N, device):
@@ -65,18 +40,17 @@ def _linear_taps(F, N, device):
   return lo.to(device), hi.to(device), (src - fl).to(device)
 
 
-def _entry(sec, nbytes, torch_sec):
-  return {'us': sec * 1e6, 'bytes': nbytes, 'achieved_TBps': nbytes / sec / 1e12,
-          'fraction_of_hbm_peak': nbytes / sec / HBM_PEAK, 'torch_us': torch_sec * 1e6,
-          'speedup_vs_torch': torch_sec / sec}
+def _entry(ms, nbytes, torch_ms):
+  sec = ms * 1e-3
+  return {'us': ms * 1e3, 'bytes': nbytes, 'achieved_TBps': nbytes / sec / 1e12,
+          'fraction_of_hbm_peak': nbytes / sec / measure.HBM_BYTES_PER_S,
+          'torch_us': torch_ms * 1e3, 'speedup_vs_torch': torch_ms / ms}
 
 
 def run(B, N, F, L, iters, warmup):
   lib = _lib.load()
   st = torch.cuda.current_stream().cuda_stream
-  l2 = torch.cuda.get_device_properties(0).L2_cache_size
-  set_bytes = 4 * 4 * B * N
-  n_sets = max(2, -(-2 * l2 // set_bytes) + 1)
+  n_sets = measure.ring_len(4 * 4 * B * N)
   gen = torch.Generator(device='cuda').manual_seed(B)
   sets = []
   for _ in range(n_sets):
@@ -86,6 +60,9 @@ def run(B, N, F, L, iters, warmup):
   out = torch.empty((B, N, 1), device='cuda')
   d = [torch.empty((B, N, 1), device='cuda') for _ in range(3)]
   res = {'B': B, 'N': N, 'input_sets': n_sets}
+
+  def ms(fn, inputs):
+    return measure.event_ms(fn, iters, warmup, inputs)
 
   def mix_f(s):
     _lib.check(lib.ddsp_b200_mix_forward(s[0].data_ptr(), s[1].data_ptr(), s[2].data_ptr(),
@@ -108,10 +85,8 @@ def run(B, N, F, L, iters, warmup):
     torch.autograd.grad(torch_mix(s), s[:3], s[3])
 
   samples = B * N
-  res['mix_forward'] = _entry(_time(mix_f, sets, iters, warmup), 16 * samples,
-                              _time(torch_mix_f, sets, iters, warmup))
-  res['mix_backward'] = _entry(_time(mix_b, sets, iters, warmup), 28 * samples,
-                               _time(torch_mix_b, tsets, iters, warmup))
+  res['mix_forward'] = _entry(ms(mix_f, sets), 16 * samples, ms(torch_mix_f, sets))
+  res['mix_backward'] = _entry(ms(mix_b, sets), 28 * samples, ms(torch_mix_b, tsets))
 
   # resample backward of a [B, F, 1] mix level
   lo, hi, frac = _linear_taps(F, N, 'cuda')
@@ -130,8 +105,8 @@ def run(B, N, F, L, iters, warmup):
     y = top + (bot - top) * frac[None, :, None]
     torch.autograd.grad(y, x, s[1])
 
-  res['resample_backward'] = _entry(_time(rs_b, rsets, iters, warmup), 4 * (samples + B * F),
-                                    _time(torch_rs_b, rsets, iters, warmup))
+  res['resample_backward'] = _entry(ms(rs_b, rsets), 4 * (samples + B * F),
+                                    ms(torch_rs_b, rsets))
 
   # ExpDecayReverb impulse response, one row per item
   gains = [torch.rand((B,), device='cuda', generator=gen) for _ in range(n_sets)]
@@ -165,10 +140,8 @@ def run(B, N, F, L, iters, warmup):
   def torch_ir_b(s):
     torch.autograd.grad(torch_ir(s[0], s[1]), s[:2], s[2])
 
-  res['ir_forward'] = _entry(_time(ir_f, isets, iters, warmup), 4 * B * L,
-                             _time(torch_ir_f, isets, iters, warmup))
-  res['ir_backward'] = _entry(_time(ir_b, isets, iters, warmup), 4 * B * L,
-                              _time(torch_ir_b, tisets, iters, warmup))
+  res['ir_forward'] = _entry(ms(ir_f, isets), 4 * B * L, ms(torch_ir_f, isets))
+  res['ir_backward'] = _entry(ms(ir_b, isets), 4 * B * L, ms(torch_ir_b, tisets))
 
   # the whole ExpDecayReverb, forward + backward
   audio = [s[0][:, :, 0].clone().requires_grad_(True) for s in sets]
@@ -189,9 +162,9 @@ def run(B, N, F, L, iters, warmup):
     wet = torch.fft.irfft(torch.fft.rfft(s[0], m) * torch.fft.rfft(ir_, m), m)[:, :N]
     torch.autograd.grad(wet + s[0], s[:3], s[3])
 
-  t_ours = _time(reverb, gsets, max(iters // 5, 3), 3)
-  t_torch = _time(torch_reverb, gsets, max(iters // 5, 3), 3)
-  res['exp_decay_reverb_fwd_bwd'] = {'ms': t_ours * 1e3, 'torch_ms': t_torch * 1e3,
+  t_ours = measure.event_ms(reverb, max(iters // 5, 3), 3, gsets)
+  t_torch = measure.event_ms(torch_reverb, max(iters // 5, 3), 3, gsets)
+  res['exp_decay_reverb_fwd_bwd'] = {'ms': t_ours, 'torch_ms': t_torch,
                                      'speedup_vs_torch': t_torch / t_ours}
   return res
 
@@ -204,9 +177,8 @@ def main():
   ap.add_argument('--iters', type=int, default=50)
   ap.add_argument('--warmup', type=int, default=10)
   args = ap.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('routing_time: needs a CUDA device')
-  out = {'card': _card(), 'runs': []}
+  measure.require_cuda('routing_time.py')
+  out = {'card': measure.card(), 'runs': []}
   for B in (32, 256):
     out['runs'].append(run(B, args.n, args.frames, args.reverb_length, args.iters,
                            args.warmup))

@@ -18,7 +18,6 @@ power limit read in the same run.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -26,8 +25,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import core  # noqa: E402
+from tools import measure  # noqa: E402
 
-FMA_PEAK = 33.5e12     # H100 SXM data sheet: 67 TFLOP/s FP32 = 33.5e12 FMA/s at 700 W
+FMA_PEAK = measure.FP32_FLOPS_PER_S / 2     # an FMA is two FLOPs
 
 SHAPES = {
     'a': (32, 64000, (32, 1000, 1), 512),
@@ -35,29 +35,6 @@ SHAPES = {
     'c': (32, 64000, (1, 1, 1), 1024),
     'd': (8, 64000, (8, 64000, 1), 512),
 }
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
-
-
-def _time(fn, iters, warmup):
-  for _ in range(warmup):
-    fn()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  torch.cuda.synchronize()
-  start.record()
-  for _ in range(iters):
-    fn()
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters * 1e-3
 
 
 def _torch_reference(audio, cutoff, s):
@@ -82,10 +59,13 @@ def main():
   ap.add_argument('--warmup', type=int, default=5)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  if not torch.cuda.is_available():
-    sys.exit('sinc_filter_time.py needs a CUDA device')
-  res = {'card': _card(), 'shapes': {}}
+  measure.require_cuda('sinc_filter_time.py')
+  res = {'card': measure.card(), 'shapes': {}}
   rng = np.random.default_rng(0)
+
+  def seconds(fn):
+    return measure.event_ms(fn, args.iters, args.warmup) * 1e-3
+
   for key, (b, n, cshape, ws) in SHAPES.items():
     s = 2 * (ws // 2) + 1
     audio = torch.from_numpy(rng.standard_normal((b, n)).astype(np.float32)).cuda()
@@ -93,16 +73,14 @@ def main():
     g = torch.randn(b, n, device='cuda')
     row = {'B': b, 'N': n, 'cutoff': list(cshape), 'taps': s, 'fma': b * n * s}
     with torch.no_grad():
-      row['fused_fwd_s'] = _time(lambda: core.sinc_filter(audio, cutoff, window_size=ws),
-                                 args.iters, args.warmup)
-      row['composition_fwd_s'] = _time(
-          lambda: core.fft_convolve(audio, core.sinc_impulse_response(cutoff, window_size=ws)),
-          args.iters, args.warmup)
+      row['fused_fwd_s'] = seconds(lambda: core.sinc_filter(audio, cutoff, window_size=ws))
+      row['composition_fwd_s'] = seconds(
+          lambda: core.fft_convolve(audio, core.sinc_impulse_response(cutoff, window_size=ws)))
     xa = audio.clone().requires_grad_(True)
     ct = cutoff.clone().requires_grad_(True)
     y = core.sinc_filter(xa, ct, window_size=ws)
-    row['fused_bwd_s'] = _time(
-        lambda: torch.autograd.grad(y, (xa, ct), g, retain_graph=True), args.iters, args.warmup)
+    row['fused_bwd_s'] = seconds(
+        lambda: torch.autograd.grad(y, (xa, ct), g, retain_graph=True))
     row['fused_fwd_fma_per_s'] = row['fma'] / row['fused_fwd_s']
     row['fused_fwd_share_of_fp32_peak'] = row['fused_fwd_fma_per_s'] / FMA_PEAK
     row['fused_bwd_share_of_fp32_peak'] = 2 * row['fma'] / row['fused_bwd_s'] / FMA_PEAK
@@ -115,7 +93,7 @@ def main():
         cr = cutoff.clone().requires_grad_(True)
         yr = _torch_reference(xr, cr, s)
         torch.autograd.grad(yr, (xr, cr), g)
-      row['torch_fwd_bwd_s'] = _time(ref_step, max(3, args.iters // 4), 2)
+      row['torch_fwd_bwd_s'] = measure.event_ms(ref_step, max(3, args.iters // 4), 2) * 1e-3
     else:
       row['torch_fwd_bwd_s'] = None
     del y, xa, ct
@@ -124,8 +102,7 @@ def main():
     print(key, json.dumps(row), flush=True)
   print(json.dumps(res['card']))
   if args.out:
-    with open(args.out, 'w') as f:
-      json.dump(res, f, indent=1)
+    measure.append_rows(args.out, [res])
 
 
 if __name__ == '__main__':

@@ -8,9 +8,9 @@ prints the card name and power limit read in the same run.
 
   python tools/sinusoidal_time.py [--iters 20] [--profile]"""
 import argparse
+import json
 import math
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -18,29 +18,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import core  # noqa: E402
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return '%s (%s)' % (torch.cuda.get_device_name(), q)
-
-
-def _ms(fn, iters, warmup=3):
-  for _ in range(warmup):
-    fn()
-  torch.cuda.synchronize()
-  e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  e0.record()
-  for _ in range(iters):
-    fn()
-  e1.record()
-  torch.cuda.synchronize()
-  return e0.elapsed_time(e1) / iters
+from tools import measure  # noqa: E402
 
 
 def _torch_decomposition(f, a, n, sr=16000.0):
@@ -65,7 +43,8 @@ def main():
   ap.add_argument('--profile', action='store_true',
                   help='also list the per-kernel device times (torch.profiler)')
   args = ap.parse_args()
-  print(_card(), flush=True)
+  measure.require_cuda('sinusoidal_time.py')
+  print(json.dumps(measure.card()), flush=True)
   rng = np.random.default_rng(0)
 
   # inference: fused against the reference's decomposition on our kernels
@@ -82,7 +61,8 @@ def main():
                                   core.resample(amps, N, method='window'))
     for name, fn in (('fused frame-rate bank', fused),
                      ('resample + resample + oscillator_bank', materialised)):
-      print('B=%d K=%d %-40s %.3f ms' % (B, K, name, _ms(fn, 5, 2)), flush=True)
+      print('B=%d K=%d %-40s %.3f ms' % (B, K, name, measure.event_ms(fn, 5, 2)),
+            flush=True)
     print('  max |fused - materialised| = %.2e' % (fused() - materialised()).abs().max().item())
     del freqs, amps
 
@@ -105,10 +85,10 @@ def main():
     def torch_fwd_bwd():
       f1.grad = a1.grad = None
       _torch_decomposition(f1, a1, N).backward(g)
-    t_f = _ms(fwd, args.iters)
-    t_fb = _ms(fwd_bwd, args.iters)
-    t_fa = _ms(lambda: fwd_bwd(False), args.iters)
-    t_torch = _ms(torch_fwd_bwd, 3, 1)
+    t_f = measure.event_ms(fwd, args.iters, 3)
+    t_fb = measure.event_ms(fwd_bwd, args.iters, 3)
+    t_fa = measure.event_ms(lambda: fwd_bwd(False), args.iters, 3)
+    t_torch = measure.event_ms(torch_fwd_bwd, 3, 1)
     print('B=%d F=%d K=%d N=%d hop=%d' % (B, F, K, N, N // F))
     print('  forward                              %8.3f ms' % t_f)
     print('  forward + backward (d amp, d freq)   %8.3f ms   backward %.3f ms = %.2fx forward'

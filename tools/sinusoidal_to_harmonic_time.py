@@ -23,7 +23,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import core  # noqa: E402
-from tools.consistency_time import _card, _peak, _time  # noqa: E402
+from tools import measure  # noqa: E402
 
 DEV = 'cuda'
 B, T, S, K = 32, 1000, 100, 100
@@ -94,29 +94,23 @@ def main():
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('sinusoidal_to_harmonic_time.py needs a CUDA device')
-  card = _card()
+  measure.require_cuda('sinusoidal_to_harmonic_time.py')
+  card = measure.card()
   rows = []
   for name, ours, theirs, pairs in configs():
-    t_ours, t_ref = [], []
-    for _ in range(args.rounds):
-      t_ours.append(_time(ours, args.iters))
-      t_ref.append(_time(theirs, max(2, args.iters // 4)))
+    t = measure.alternate({'ms': ours, 'torch_ms': theirs}, args.rounds,
+                          {'ms': args.iters, 'torch_ms': max(2, args.iters // 4)}, 3)
     torch.cuda.empty_cache()
-    row = {'config': name, 'B': B, 'T': T, 'S': S, 'K': K,
-           'ms': sorted(t_ours)[len(t_ours) // 2] * 1e3,
-           'torch_ms': sorted(t_ref)[len(t_ref) // 2] * 1e3,
-           'peak_mb': _peak(ours) / 2**20, 'torch_peak_mb': _peak(theirs) / 2**20,
-           'pairs': pairs}
+    row = {'config': name, 'B': B, 'T': T, 'S': S, 'K': K, **t,
+           'peak_mb': measure.peak_bytes(ours) / 2**20,
+           'torch_peak_mb': measure.peak_bytes(theirs) / 2**20, 'pairs': pairs}
     row['pairs_per_s'] = pairs / (row['ms'] * 1e-3)
     row.update(card)
     rows.append(row)
     print(json.dumps(row), flush=True)
     torch.cuda.empty_cache()
   if args.out:
-    with open(args.out, 'w') as f:
-      json.dump(rows, f, indent=1)
+    measure.append_rows(args.out, rows)
 
 
 if __name__ == '__main__':

@@ -14,14 +14,13 @@ power limit read in the same run.
 import argparse
 import json
 import os
-import statistics
 import sys
 
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import losses, spectral_ops  # noqa: E402
-from tools.oscillator_bank_time import _card  # noqa: E402
+from tools import measure  # noqa: E402
 
 B, N = 128, 64000
 SIZES = (2048, 1024, 512, 256, 128, 64)
@@ -41,36 +40,18 @@ def _fused(loss, target, audio):
       loss.delta_freq_weight, loss.cumsum_freq_weight, loss.loss_type)
 
 
-def _time(fn, iters):
-  e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  e0.record()
-  for _ in range(iters):
-    fn()
-  e1.record()
-  torch.cuda.synchronize()
-  return e0.elapsed_time(e1) / iters
-
-
-def _peak(fn):
-  torch.cuda.synchronize()
-  torch.cuda.reset_peak_memory_stats()
-  base = torch.cuda.memory_allocated()
-  fn()
-  torch.cuda.synchronize()
-  return (torch.cuda.max_memory_allocated() - base) / 2**20
-
-
 def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--iters', type=int, default=5)
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
+  measure.require_cuda('spectral_loss_time.py')
   gen = torch.Generator(device='cuda').manual_seed(0)
   target = 0.1 * torch.randn(B, N, device='cuda', generator=gen)
   audio = (0.7 * target + 0.05 * torch.randn(B, N, device='cuda', generator=gen))
   a = audio.clone().requires_grad_(True)
-  res = {'card': _card(), 'shape': [B, N], 'fft_sizes': list(SIZES), 'configs': {}}
+  res = {'card': measure.card(), 'shape': [B, N], 'fft_sizes': list(SIZES), 'configs': {}}
   for name, kw in CONFIGS.items():
     loss = losses.SpectralLoss(fft_sizes=SIZES, **kw)
     paths = {
@@ -81,24 +62,20 @@ def main():
     for p, f in paths.items():          # warm-up: cuFFT plans, caches
       values[p] = float(f().detach())
       f().backward()
-    times = {p + k: [] for p in paths for k in ('_forward_ms', '_forward_backward_ms')}
-    for _ in range(args.rounds):
-      for p, f in paths.items():
-        with torch.no_grad():
-          times[p + '_forward_ms'].append(_time(f, args.iters))
-        times[p + '_forward_backward_ms'].append(_time(lambda: f().backward(), args.iters))
-    r = {k: statistics.median(v) for k, v in times.items()}
+    timed = {}
     for p, f in paths.items():
-      r[p + '_peak_mib'] = _peak(lambda: f().backward())
+      timed[p + '_forward_ms'] = torch.no_grad()(f)
+      timed[p + '_forward_backward_ms'] = lambda f=f: f().backward()
+    r = measure.alternate(timed, args.rounds, args.iters, 0)
+    for p, f in paths.items():
+      r[p + '_peak_mib'] = measure.peak_bytes(lambda: f().backward()) / 2**20
     r['loss_rel_diff'] = abs(values['fused'] - values['torch']) / abs(values['torch'])
     r['fused_routed'] = loss._fusable(target, a, None)
     res['configs'][name] = r
     a.grad = None
-  line = json.dumps(res)
-  print(line)
+  print(json.dumps(res))
   if args.out:
-    with open(args.out, 'a') as fh:
-      fh.write(line + '\n')
+    measure.append_rows(args.out, [res])
 
 
 if __name__ == '__main__':

@@ -8,50 +8,28 @@ measurement, the card name and power limit in every line.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 import warnings
 
 import numpy as np
-import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from ddsp_b200 import synthetic_data as sd   # noqa: E402
 from tests import synthetic_data_ref as ref  # noqa: E402
+from tools import measure  # noqa: E402
 
 T, K, M = 125, 100, 65
 # bytes written per example: the kernel's float64 rows and the float32 controls
 # (harm_amp, harm_dist, f0_hz, sin_amps, sin_freqs, noise_magnitudes)
 F64_BYTES = 8 * (T + T * K + T + T * M + 1)
 F32_BYTES = 4 * (T + 3 * T * K + T + T * M)
-HBM_GBPS = 3350.0   # H100 SXM data sheet
-
-
-def card():
-  name = torch.cuda.get_device_name()
-  try:
-    power = subprocess.run(['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader',
-                            '-i', str(torch.cuda.current_device())],
-                           capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    power = 'unknown'
-  return name, power
 
 
 def gpu_ms(fn, reps):
-  for _ in range(3):
-    fn()
-  torch.cuda.synchronize()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  times = []
-  for _ in range(reps):
-    start.record()
-    fn()
-    stop.record()
-    stop.synchronize()
-    times.append(start.elapsed_time(stop))
+  """Median and least ms of `reps` calls, each timed on its own after 3 warm-up calls."""
+  times = [measure.event_ms(fn, 1, 3 if r == 0 else 0) for r in range(reps)]
   return float(np.median(times)), float(np.min(times))
 
 
@@ -59,11 +37,12 @@ def main():
   ap = argparse.ArgumentParser()
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  name, power = card()
+  measure.require_cuda('synthetic_data_time.py')
+  card = measure.card()
   rows = []
 
   def emit(**kw):
-    kw.update(card=name, power_limit=power)
+    kw.update(card=card)
     rows.append(kw)
     print(json.dumps(kw), flush=True)
 
@@ -75,7 +54,7 @@ def main():
          examples_per_s=b / med * 1e3,
          bytes_per_example=F64_BYTES + F32_BYTES,
          write_gbps=b * (F64_BYTES + F32_BYTES) / med * 1e-6,
-         hbm_fraction=b * (F64_BYTES + F32_BYTES) / med * 1e-6 / HBM_GBPS)
+         hbm_fraction=b * (F64_BYTES + F32_BYTES) / med * 1e3 / measure.HBM_BYTES_PER_S)
   np.random.seed(0)
   med, best = gpu_ms(lambda: sd.generate_notes_v2(n_batch=64), 5)
   emit(what='v2 state mode', batch=64, ms_median=med, ms_min=best,
@@ -102,9 +81,7 @@ def main():
   except Exception as e:  # the reference sources are not everywhere
     print('reference on the shim not timed: %s' % e, file=sys.stderr)
   if args.out:
-    with open(args.out, 'a') as f:
-      for r in rows:
-        f.write(json.dumps(r) + '\n')
+    measure.append_rows(args.out, rows)
 
 
 if __name__ == '__main__':

@@ -18,7 +18,6 @@ the card name and power limit read in the same run."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -26,40 +25,9 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import losses  # noqa: E402
+from tools import measure  # noqa: E402
 
 DEV = 'cuda'
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
-
-
-def _time(fn, iters, warmup=3):
-  for _ in range(warmup):
-    fn()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  torch.cuda.synchronize()
-  start.record()
-  for _ in range(iters):
-    fn()
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters * 1e-3
-
-
-def _peak(fn):
-  torch.cuda.synchronize()
-  base = torch.cuda.memory_allocated()
-  torch.cuda.reset_peak_memory_stats()
-  fn()
-  torch.cuda.synchronize()
-  return torch.cuda.max_memory_allocated() - base
 
 
 # ---- the reference formula, float32 torch ----------------------------------------
@@ -113,23 +81,18 @@ def main():
   ap.add_argument('--rounds', type=int, default=3)
   ap.add_argument('--out', default=None)
   args = ap.parse_args()
-  if not torch.cuda.is_available():
-    raise SystemExit('wasserstein_time.py needs a CUDA device')
-  card = _card()
+  measure.require_cuda('wasserstein_time.py')
+  card = measure.card()
   rows = []
   for name, ours, theirs, plain in configs():
     with torch.no_grad():
       a, b = losses.wasserstein_distance(*plain), ref_distance(*plain)
       diff = float(torch.max(torch.abs(a - b)))
       scale = float(torch.max(torch.abs(b)))
-    t_ours, t_ref = [], []
-    for _ in range(args.rounds):
-      t_ours.append(_time(ours, args.iters))
-      t_ref.append(_time(theirs, args.iters))
+    t = measure.alternate({'ms': ours, 'torch_ms': theirs}, args.rounds, args.iters, 3)
     torch.cuda.empty_cache()
-    row = {'config': name, 'ms': sorted(t_ours)[len(t_ours) // 2] * 1e3,
-           'torch_ms': sorted(t_ref)[len(t_ref) // 2] * 1e3,
-           'peak_mb': _peak(ours) / 2**20, 'torch_peak_mb': _peak(theirs) / 2**20,
+    row = {'config': name, **t, 'peak_mb': measure.peak_bytes(ours) / 2**20,
+           'torch_peak_mb': measure.peak_bytes(theirs) / 2**20,
            'max_abs_diff': diff, 'max_abs_value': scale, 'rows': int(plain[0][..., 0].numel())}
     row['speedup'] = row['torch_ms'] / row['ms']
     row.update(card)
@@ -137,8 +100,7 @@ def main():
     print(json.dumps(row), flush=True)
     torch.cuda.empty_cache()
   if args.out:
-    with open(args.out, 'w') as f:
-      json.dump(rows, f, indent=1)
+    measure.append_rows(args.out, rows)
 
 
 if __name__ == '__main__':

@@ -18,7 +18,6 @@ Prints the card name and power limit read in the same run."""
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -26,37 +25,11 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from ddsp_b200 import _lib  # noqa: E402
 from ddsp_b200 import core  # noqa: E402
-
-HBM_PEAK = 3.35e12
-L2_BYTES = 50 * 2**20
-
-
-def _card():
-  try:
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader',
-                        '-i', str(torch.cuda.current_device())],
-                       capture_output=True, text=True, timeout=30).stdout.strip()
-  except (OSError, subprocess.SubprocessError):
-    q = ''
-  return {'device': torch.cuda.get_device_name(), 'nvidia_smi': q}
-
-
-def _time(fn, sets, iters, warmup):
-  for i in range(warmup):
-    fn(sets[i % len(sets)])
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  torch.cuda.synchronize()
-  start.record()
-  for i in range(iters):
-    fn(sets[i % len(sets)])
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters * 1e-3
+from tools import measure  # noqa: E402
 
 
 def _sets(B, F, Fw, W, N, dev):
-  per = 4 * (B * Fw * W + 3 * B * F + B * N)
-  n = max(2, -(-2 * L2_BYTES // per) + 1)
+  n = measure.ring_len(4 * (B * Fw * W + 3 * B * F + B * N))
   g = torch.Generator(dev).manual_seed(0)
   out = []
   for _ in range(n):
@@ -86,10 +59,13 @@ def _shape(B, F, Fw, W, N, iters, warmup, dev):
   ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
   outs = (torch.empty((B, F), device=dev), torch.empty((B, F), device=dev),
           torch.empty((B, Fw, W), device=dev))
-  fwd = _time(lambda s: core.wavetable_forward(s[0], s[1], s[2], N, 16000.0, 'window'),
-              sets, iters, warmup)
+
+  def ms(fn):
+    return measure.event_ms(fn, iters, warmup, sets)
+
+  fwd = ms(lambda s: core.wavetable_forward(s[0], s[1], s[2], N, 16000.0, 'window'))
   bwd, bwd_nof0, bwd_frames, bwd_table = (
-      _time(lambda s, w=w: _backward_call(s, N, w, ws, nbytes, outs), sets, iters, warmup)
+      ms(lambda s, w=w: _backward_call(s, N, w, ws, nbytes, outs))
       for w in ('fat', 'at', 'fa', 't'))
 
   def step(s):
@@ -99,14 +75,14 @@ def _shape(B, F, Fw, W, N, iters, warmup, dev):
     for t in x:
       t.grad = None
       t.requires_grad_(False)
-  both = _time(step, sets, iters, warmup)
+  both = ms(step)
   fb, bb = 4.0 * (B * Fw * W + B * N), 4.0 * (2 * B * Fw * W + B * N)
   return {'B': B, 'F': F, 'Fw': Fw, 'W': W, 'N': N,
-          'forward_ms': fwd * 1e3, 'backward_ms': bwd * 1e3,
-          'backward_no_f0_ms': bwd_nof0 * 1e3,
-          'backward_f0_amplitudes_ms': bwd_frames * 1e3,
-          'backward_wavetables_ms': bwd_table * 1e3, 'forward_backward_ms': both * 1e3,
-          'forward_hbm_share': fb / fwd / HBM_PEAK, 'backward_hbm_share': bb / bwd / HBM_PEAK,
+          'forward_ms': fwd, 'backward_ms': bwd, 'backward_no_f0_ms': bwd_nof0,
+          'backward_f0_amplitudes_ms': bwd_frames, 'backward_wavetables_ms': bwd_table,
+          'forward_backward_ms': both,
+          'forward_hbm_share': fb / (fwd * 1e-3) / measure.HBM_BYTES_PER_S,
+          'backward_hbm_share': bb / (bwd * 1e-3) / measure.HBM_BYTES_PER_S,
           'ring_sets': len(sets)}
 
 
@@ -130,15 +106,7 @@ def _torch_reference(B, F, W, N, iters, dev):
     lin = torch.linspace(0.0, 1.0, W + 1, device=dev)
     w = torch.relu(1.0 - torch.abs(ph - lin) * W)
     ((w * t).sum(-1) * amp).backward(up)
-  step()
-  torch.cuda.synchronize()
-  start, stop = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-  start.record()
-  for _ in range(iters):
-    step()
-  stop.record()
-  torch.cuda.synchronize()
-  return start.elapsed_time(stop) / iters
+  return measure.event_ms(step, iters, 1)
 
 
 def main():
@@ -147,8 +115,9 @@ def main():
   ap.add_argument('--warmup', type=int, default=5)
   ap.add_argument('--out', default=None)
   a = ap.parse_args()
+  measure.require_cuda('wavetable_time.py')
   dev = torch.device('cuda', 0)
-  res = {'card': _card(), 'shapes': []}
+  res = {'card': measure.card(), 'shapes': []}
   for B in (32, 256):
     for Fw, W in ((1000, 1024), (1000, 2048), (1, 2048)):
       r = _shape(B, 1000, Fw, W, 64000, a.iters, a.warmup, dev)
@@ -168,8 +137,7 @@ def main():
     print(json.dumps(res['torch_reference'][-1]), flush=True)
   print(json.dumps(res['card']))
   if a.out:
-    with open(a.out, 'w') as f:
-      json.dump(res, f, indent=1)
+    measure.append_rows(a.out, [res])
 
 
 if __name__ == '__main__':
