@@ -15,6 +15,11 @@ TEST INFRASTRUCTURE.
     amp(t) = A_i w0(r) + A_{i+1} w1(r),         audio = sum_k m amp sin(2 pi phase)
   with w1 = 0.5 - 0.5 cos(pi r / hop) ('window', the Hann overlap-add) or r / hop
   ('linear') and w0 = 1 - w1.
+* `regime`: the frequency regimes the kernel tests sweep.
+* `float64_grads`: audio and gradients of float64 autograd through
+  `torch_sinusoidal`, with the forward kernel's float32 mask.
+* `harmonic_sinusoidal64`: core.harmonic_synthesis on its sinusoidal route
+  ((f0 k)(1 + shifts), amplitudes * distribution) restated on `torch_sinusoidal`.
 """
 import math
 
@@ -69,3 +74,52 @@ def torch_sinusoidal(frequencies, amplitudes, n_samples, sample_rate=16000,
   # the oracle's order: omega = f * 2 pi / sr, then the running sum in radians
   phase = torch.cumsum(fe * (2.0 * math.pi) / sample_rate, dim=1)
   return (amp * torch.sin(phase)).sum(-1)
+
+
+def regime(name, B, F, K, sr, seed):
+  """Frequencies [B, F, K] in Hz, float32."""
+  rng = np.random.default_rng(seed)
+  nyq = sr / 2.0
+  f = rng.uniform(20.0, 7900.0, (B, F, K))
+  if name == 'zero':              # silent sinusoids and silent frames
+    f[..., ::2] = 0.0
+    f[:, ::3, :] = 0.0
+  elif name == 'glide':           # every other frame across Nyquist, both ways
+    up = np.where(np.arange(F) % 2 == 0, 0.9, 1.1)[None, :, None]
+    f[..., ::2] = nyq * up * rng.uniform(0.95, 1.05, (B, F, 1))
+  elif name == 'above':           # sinusoid 0 above Nyquist in every frame
+    f[..., 0] = rng.uniform(1.01 * nyq, 1.9 * nyq, (B, F))
+  return f.astype(np.float32)
+
+
+def float64_grads(f32, a32, g, n_samples, sample_rate, method):
+  """(audio, d frequencies, d amplitudes) of float64 autograd through
+  `torch_sinusoidal` on the device of f32, with the forward kernel's float32 mask."""
+  mask = torch.from_numpy(nyquist_mask(f32.cpu().numpy(), n_samples,
+                                       sample_rate)).to(f32.device)
+  f64 = f32.detach().double().requires_grad_(True)
+  a64 = a32.detach().double().requires_grad_(True)
+  out = torch_sinusoidal(f64, a64, n_samples, sample_rate, method, mask=mask)
+  out.backward(g.double())
+  return out.detach(), f64.grad, a64.grad
+
+
+def harmonic_sinusoidal64(f0, amps, hd, shifts, n_samples, sample_rate, method):
+  """core.harmonic_synthesis through its frame-rate oscillator bank in float64.
+  The harmonic frequencies take the values of the float32 products the kernel is
+  given, (f0 k)(1 + shifts), with their float64 derivatives: a float64 product
+  differs by up to half a float32 ulp, which over thousands of cycles of a harmonic
+  near Nyquist drifts the phase by 1e-3 rad.  The audio-rate mask is decided on the
+  same float32 frequencies."""
+  k = hd.shape[-1]
+  ratios32 = torch.linspace(1.0, float(k), k, device=f0.device)
+  hf32 = f0.detach().float() * ratios32
+  if shifts is not None:
+    hf32 = hf32 * (1.0 + shifts.detach().float())
+  mask = torch.from_numpy(nyquist_mask(hf32.cpu().numpy(), n_samples,
+                                       sample_rate)).to(f0.device)
+  hf = f0 * ratios32.double()
+  if shifts is not None:
+    hf = hf * (1.0 + shifts)
+  hf = hf + (hf32.double() - hf).detach()
+  return torch_sinusoidal(hf, amps * hd, n_samples, sample_rate, method, mask=mask)

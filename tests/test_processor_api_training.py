@@ -671,21 +671,6 @@ def test_vst_layout_trains():
     assert torch.isfinite(v.grad).all() and float(v.grad.abs().max()) > 0, k
 
 
-def _sinusoidal64(f0, amps, hd, shifts, N, method):
-  """core.harmonic_synthesis through its frame-rate oscillator bank in float64, the
-  audio-rate mask decided on the float32 frequencies the kernel sees."""
-  k = hd.shape[-1]
-  ratios32 = torch.linspace(1.0, float(k), k, device=f0.device)
-  hf32 = f0.detach().float() * ratios32
-  if shifts is not None:
-    hf32 = hf32 * (1.0 + shifts.detach().float())
-  mask = torch.from_numpy(sinusoidal_ref.nyquist_mask(hf32.cpu().numpy(), N, SR)).to(f0.device)
-  hf = f0 * ratios32.double()
-  if shifts is not None:
-    hf = hf * (1.0 + shifts)
-  return sinusoidal_ref.torch_sinusoidal(hf, amps * hd, N, SR, method, mask=mask)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('hop,method,with_shifts', [(64, 'window', True), (100, 'window', False),
                                                     (100, 'linear', True)])
@@ -708,7 +693,7 @@ def test_harmonic_shifts_and_other_hops_against_float64(hop, method, with_shifts
   out.backward(up)
   l64 = [t.double().requires_grad_(True) for t in (f0, amps, hd)]
   s64 = shifts.double().requires_grad_(True) if with_shifts else None
-  want = _sinusoidal64(l64[0], l64[1], l64[2], s64, N, method)
+  want = sinusoidal_ref.harmonic_sinusoidal64(l64[0], l64[1], l64[2], s64, N, SR, method)
   want.backward(up.double())
   _check('audio', out, want, 1e-4, 1e-4)
   for name, got, ref in zip(('f0', 'amps', 'hd'), leaves, l64):

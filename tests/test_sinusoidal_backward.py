@@ -18,22 +18,6 @@ from tests import sinusoidal_ref as ref
 from tests.util import linearity, rel_err
 
 
-def _regime(regime, B, F, K, sr, seed):
-  """Frequencies [B, F, K] in Hz, float32."""
-  rng = np.random.default_rng(seed)
-  nyq = sr / 2.0
-  f = rng.uniform(20.0, 7900.0, (B, F, K))
-  if regime == 'zero':            # silent sinusoids and silent frames
-    f[..., ::2] = 0.0
-    f[:, ::3, :] = 0.0
-  elif regime == 'glide':         # every other frame across Nyquist, both ways
-    up = np.where(np.arange(F) % 2 == 0, 0.9, 1.1)[None, :, None]
-    f[..., ::2] = nyq * up * rng.uniform(0.95, 1.05, (B, F, 1))
-  elif regime == 'above':         # sinusoid 0 above Nyquist in every frame
-    f[..., 0] = rng.uniform(1.01 * nyq, 1.9 * nyq, (B, F))
-  return f.astype(np.float32)
-
-
 # ---- CPU ---------------------------------------------------------------------
 @pytest.mark.parametrize('method', ['window', 'linear'])
 @pytest.mark.parametrize('F,hop,sr', [(1, 400, 16000), (7, 64, 16000), (16, 441, 44100),
@@ -68,7 +52,7 @@ def test_float32_mask_follows_the_forward_rule():
   frequency exactly at Nyquist, and can differ from float64 only within float32
   rounding of it."""
   B, F, K, hop, sr = 2, 9, 6, 160, 16000
-  f = _regime('glide', B, F, K, sr, seed=3)
+  f = ref.regime('glide', B, F, K, sr, seed=3)
   f[0, 4, 1] = f[0, 5, 1] = 8000.0
   f[1, 2, 2], f[1, 3, 2] = 7999.0, 8001.0
   m32 = ref.nyquist_mask(f, F * hop, sr)
@@ -153,22 +137,11 @@ def _check(name, got, want, tol_max, tol_l2):
   assert emax < tol_max and el2 < tol_l2, (name, emax, el2)
 
 
-def _float64_grads(f32, a32, g, N, sr, method):
-  """Audio and gradients of float64 autograd through the restatement, on the GPU,
-  with the forward kernel's float32 mask."""
-  mask = torch.from_numpy(ref.nyquist_mask(f32.cpu().numpy(), N, sr)).to(f32.device)
-  f64 = f32.detach().double().requires_grad_(True)
-  a64 = a32.detach().double().requires_grad_(True)
-  out = ref.torch_sinusoidal(f64, a64, N, sr, method, mask=mask)
-  out.backward(g.double())
-  return out.detach(), f64.grad, a64.grad
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize('B,F,K,hop,sr,method,regime', CASES)
 def test_backward_against_float64_autograd(B, F, K, hop, sr, method, regime):
   N = F * hop
-  f = torch.from_numpy(_regime(regime, B, F, K, sr, seed=F * K + hop)).to(DEV)
+  f = torch.from_numpy(ref.regime(regime, B, F, K, sr, seed=F * K + hop)).to(DEV)
   gen = torch.Generator(device='cpu').manual_seed(hop)
   a = (torch.rand((B, F, K), generator=gen) + 0.1).to(DEV)
   g = torch.randn((B, N), generator=gen).to(DEV)
@@ -177,7 +150,7 @@ def test_backward_against_float64_autograd(B, F, K, hop, sr, method, regime):
   out = core.sinusoidal_synthesis(f1, a1, n_samples=N, sample_rate=sr,
                                   amp_resample_method=method)
   out.backward(g)
-  want, d_f, d_a = _float64_grads(f, a, g, N, sr, method)
+  want, d_f, d_a = ref.float64_grads(f, a, g, N, sr, method)
   _check('audio', out, want, 1e-4, 1e-4)
   _check('d amplitudes', a1.grad, d_a, 2e-4, 1e-4)
   _check('d frequencies', f1.grad, d_f, 5e-4, 2e-4)
@@ -192,7 +165,7 @@ def test_d_amplitudes_inner_product_identity(method, hop, sr):
   float64 oracle evaluates it with no restatement involved."""
   B, F, K = 2, 12, 9
   N = F * hop
-  f32 = _regime('random', B, F, K, sr, seed=hop)
+  f32 = ref.regime('random', B, F, K, sr, seed=hop)
   f32 = np.minimum(f32, 0.45 * sr).astype(np.float32)
   gen = torch.Generator(device='cpu').manual_seed(7)
   g = torch.randn((B, N), generator=gen).to(DEV)
@@ -209,7 +182,7 @@ def test_amplitudes_only_is_bit_identical(method):
   """With only the amplitudes requiring grad the phase path is skipped, and d
   amplitudes is bit for bit what the call with both inputs gives."""
   B, F, K, N = 3, 50, 33, 16000
-  f = torch.from_numpy(_regime('glide', B, F, K, 16000, seed=2)).to(DEV)
+  f = torch.from_numpy(ref.regime('glide', B, F, K, 16000, seed=2)).to(DEV)
   gen = torch.Generator(device='cpu').manual_seed(2)
   a = torch.rand((B, F, K), generator=gen).to(DEV)
   g = torch.randn((B, N), generator=gen).to(DEV)
@@ -274,7 +247,7 @@ def test_full_size_inverse_synthesis_shape():
   from ddsp_b200 import autograd as ag
   from ddsp_b200 import losses
   B, F, K, N, sr = 32, 125, 100, 64000, 16000
-  f = torch.from_numpy(_regime('random', B, F, K, sr, seed=0)).to(DEV)
+  f = torch.from_numpy(ref.regime('random', B, F, K, sr, seed=0)).to(DEV)
   gen = torch.Generator(device=DEV).manual_seed(0)
   a = torch.rand((B, F, K), device=DEV, generator=gen) * 0.05
   g = torch.randn((B, N), device=DEV, generator=gen)
@@ -290,7 +263,7 @@ def test_full_size_inverse_synthesis_shape():
     assert torch.equal(first, second)
   for b in (0, B - 1):
     rows = slice(b, b + 1)
-    want, d_f, d_a = _float64_grads(f[rows], a[rows], g[rows], N, sr, 'window')
+    want, d_f, d_a = ref.float64_grads(f[rows], a[rows], g[rows], N, sr, 'window')
     _check('audio', runs[0][0][rows], want, 1e-4, 1e-4)
     _check('d amplitudes', runs[0][2][rows], d_a, 2e-4, 1e-4)
     _check('d frequencies', runs[0][1][rows], d_f, 5e-4, 2e-4)
