@@ -17,6 +17,7 @@ import torch
 from ddsp_b200 import _lib
 
 AMP_METHODS = {'window': _lib.AMP_WINDOW, 'linear': _lib.AMP_LINEAR}
+DB_RANGE = 80.0  # dB (core.py:27)
 
 
 # ----------------------------------------------------------------------------
@@ -90,6 +91,41 @@ def nested_lookup(nested_key: Text, nested_dict: Dict[Text, Any],
                      'not found during nested dictionary lookup, out of '
                      f'available keys: {nested_keys(nested_dict)}')
   return value
+
+
+def copy_if_tf_function(x):
+  """core.copy_if_tf_function (core.py:64-75): returns x unchanged.  The reference
+  copies x only inside a tf.function, so that a later change to a traced input cannot
+  reach the function; torch always runs eagerly, where the reference returns x too."""
+  return x
+
+
+def leaf_key(nested_key: Text, delimiter: Text = '/'):
+  """core.leaf_key (core.py:132-144): the last key of "key/key/key..."."""
+  return nested_key.split(delimiter)[-1]
+
+
+def map_shape(x):
+  """core.map_shape (core.py:147-149): the shape of every tensor or array of a nested
+  dict / list / tuple as a list of ints, in the same structure."""
+  if isinstance(x, dict):
+    return {k: map_shape(v) for k, v in x.items()}
+  if isinstance(x, (list, tuple)):
+    return type(x)(map_shape(v) for v in x)
+  return [int(d) for d in _shape(x)]
+
+
+def pad_axis(x, padding=(0, 0), axis=0, **pad_kwargs):
+  """core.pad_axis (core.py:152-168): pads only `axis` of x by (before, after) with
+  torch.nn.functional.pad.  tf.pad's keywords map to torch's: `mode` in any case
+  ('CONSTANT' -> 'constant') and `constant_values` -> `value`."""
+  x = x if torch.is_tensor(x) else _as_f32(x)
+  if 'constant_values' in pad_kwargs:
+    pad_kwargs['value'] = pad_kwargs.pop('constant_values')
+  if 'mode' in pad_kwargs:
+    pad_kwargs['mode'] = pad_kwargs['mode'].lower()
+  n_end_dims = x.dim() - axis % x.dim() - 1
+  return torch.nn.functional.pad(x, (0, 0) * n_end_dims + tuple(padding), **pad_kwargs)
 
 
 def _shape(x):
@@ -260,6 +296,13 @@ def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):
   return max_value * torch.sigmoid(x)**float(np.log(exponent)) + threshold
 
 
+def sym_exp_sigmoid(x, width=8.0):
+  """core.sym_exp_sigmoid (core.py:407-411): exp_sigmoid(width * (|x| / 2 - 1)),
+  symmetric about x = 0.  exp_sigmoid's CUDA kernel runs it outside grad."""
+  x = torch_float32(x)
+  return exp_sigmoid(width * (torch.abs(x) / 2.0 - 1.0))
+
+
 # ----------------------------------------------------------------------------
 # Frequency scaling of network outputs (core.py:207-348, 414-508) - frame-rate
 # torch ops (a few thousand elements per item), device-agnostic.
@@ -297,6 +340,65 @@ def logb(x, base=2.0, eps=1e-5):
 def log10(x, eps=1e-5):
   """core.log10 (core.py:224-226)."""
   return logb(x, base=10, eps=eps)
+
+
+# The math helpers and scalers below take a tensor as it is (float64 stays float64) and
+# anything else as a float32 CPU tensor.
+def nan_to_num(x, value=0.0):
+  """core.nan_to_num (core.py:202-204): NaN -> value.  +-inf stay, unlike the
+  defaults of torch.nan_to_num."""
+  x = x if torch.is_tensor(x) else _as_f32(x)
+  return torch.where(torch.isnan(x), torch.full_like(x, value), x)
+
+
+def log_scale(x, min_x, max_x):
+  """core.log_scale (core.py:229-233): [-1, 1] to [min_x, max_x], logarithmically."""
+  x = x if torch.is_tensor(x) else _as_f32(x)
+  x = (x + 1.0) / 2.0
+  log_min, log_max = (torch.log(torch.as_tensor(v, dtype=x.dtype, device=x.device))
+                      for v in (min_x, max_x))
+  return torch.exp((1.0 - x) * log_min + x * log_max)
+
+
+def soft_limit(x, x_min=0.0, x_max=1.0):
+  """core.soft_limit (core.py:236-238): softly limits x to [x_min, x_max]."""
+  x = x if torch.is_tensor(x) else _as_f32(x)
+  softplus = torch.nn.functional.softplus
+  return softplus(x) + x_min - softplus(x - (x_max - x_min))
+
+
+def gradient_reversal(x):
+  """core.gradient_reversal (core.py:241-243): the identity forward, -grad backward,
+  as the reference writes it: stop_gradient(2 x) - x."""
+  x = x if torch.is_tensor(x) else _as_f32(x)
+  return (2.0 * x).detach() - x
+
+
+def amplitude_to_db(amplitude, ref_db=0.0, range_db=DB_RANGE, use_tf=True):
+  """core.amplitude_to_db (core.py:247-250): power_to_db(amplitude**2)."""
+  return power_to_db(amplitude**2.0, ref_db=ref_db, range_db=range_db, use_tf=use_tf)
+
+
+def power_to_db(power, ref_db=0.0, range_db=DB_RANGE, use_tf=True):
+  """core.power_to_db (core.py:253-268): 10 log10(max(10^(-range_db / 10), power))
+  - ref_db, floored at -range_db.  use_tf=True is torch with core.log10 (safe_log,
+  float32) on the input's device; use_tf=False is NumPy with np.log10."""
+  pmin = 10**-(range_db / 10.0)
+  if not use_tf:
+    db = 10.0 * np.log10(np.maximum(pmin, power))
+    return np.maximum(db - ref_db, -range_db)
+  db = 10.0 * log10(torch.clamp(_as_f32(power), min=pmin))
+  return torch.clamp(db - ref_db, min=-range_db)
+
+
+def db_to_amplitude(db):
+  """core.db_to_amplitude (core.py:271-273)."""
+  return db_to_power(db / 2.0)
+
+
+def db_to_power(db):
+  """core.db_to_power (core.py:276-278)."""
+  return 10.0**(db / 10.0)
 
 
 def midi_to_hz(notes, midi_zero_silence: bool = False):
@@ -339,6 +441,39 @@ def hz_to_unit(hz, hz_min, hz_max, clip: bool = False):
   """core.hz_to_unit (core.py:339-348)."""
   return midi_to_unit(hz_to_midi(hz), midi_min=hz_to_midi(hz_min),
                       midi_max=hz_to_midi(hz_max), clip=clip)
+
+
+# Perceptual scales (core.py:351-383): NumPy stays NumPy, as frequencies_critical_bands
+# needs for its float64 band centres, and tensors stay tensors.
+def hz_to_bark(hz):
+  """core.hz_to_bark (core.py:351-353): Traunmüller (1990)."""
+  return 26.81 / (1.0 + (1960.0 / hz)) - 0.53
+
+
+def bark_to_hz(bark):
+  """core.bark_to_hz (core.py:356-358): Traunmüller (1990)."""
+  return 1960.0 / (26.81 / (bark + 0.53) - 1.0)
+
+
+def hz_to_mel(hz):
+  """core.hz_to_mel (core.py:361-363): HTK's 2595 log10(1 + hz / 700) with core.logb's
+  safe log.  A tensor gives float32 through core.logb; NumPy and numbers give float64
+  NumPy."""
+  if torch.is_tensor(hz):
+    return 2595.0 * logb(1.0 + hz / 700.0, 10.0)
+  x = 1.0 + np.asarray(hz, np.float64) / 700.0
+  return 2595.0 * (np.log(np.where(x <= 0.0, 1e-5, x)) / np.log(10.0))
+
+
+def mel_to_hz(mel):
+  """core.mel_to_hz (core.py:366-368): HTK."""
+  return 700.0 * (10.0**(mel / 2595.0) - 1.0)
+
+
+def hz_to_erb(hz):
+  """core.hz_to_erb (core.py:371-383): the equivalent rectangular bandwidth in Hz,
+  Moore & Glasberg (1996)."""
+  return 0.108 * hz + 24.7
 
 
 def _add_depth_axis(freqs, depth: int = 1):
@@ -386,6 +521,31 @@ def frequencies_sigmoid(freqs, depth: int = 1, hz_min: float = 0.0,
       remainder -= hz_max
     hz_scales.append(unit_to_hz(f_probs[..., i], hz_min=hz_min, hz_max=hz_max))
   return torch.sum(torch.stack(hz_scales, dim=-1), dim=-1)
+
+
+def frequencies_critical_bands(freqs, depth=1, depth_scale=10.0, bandwidth_scale=1.0,
+                               hz_min=20.0, hz_max=8000.0, scale='bark'):
+  """core.frequencies_critical_bands (core.py:511-569): sinusoid k sits at the k-th of
+  centres spaced evenly on the bark scale (any other `scale`: mel) over [hz_min, hz_max]
+  and moves by up to bandwidth_scale ERBs of its centre: soft_limit(centre +
+  bandwidth_scale * erb * sum_d tanh(freqs_d) depth_scale^-d, hz_min, hz_max).
+  freqs [B, T, N * depth] or [B, T, N, depth] -> Hz [B, T, N].  The centres are float64
+  NumPy, as in the reference, used as float32 on the input's device."""
+  freqs = freqs if torch.is_tensor(freqs) else _as_f32(freqs)
+  if freqs.dim() == 3:
+    freqs = _add_depth_axis(freqs, depth)
+  else:
+    depth = int(freqs.shape[-1])
+  n_sinusoids = freqs.shape[-2]
+  if scale == 'bark':
+    f_center = bark_to_hz(np.linspace(hz_to_bark(hz_min), hz_to_bark(hz_max), n_sinusoids))
+  else:
+    f_center = mel_to_hz(np.linspace(hz_to_mel(hz_min), hz_to_mel(hz_max), n_sinusoids))
+  bw = torch.as_tensor(hz_to_erb(f_center), dtype=torch.float32, device=freqs.device)
+  f_center = torch.as_tensor(f_center, dtype=torch.float32, device=freqs.device)
+  depth_modifier = depth_scale**-torch.arange(depth, dtype=torch.float32, device=freqs.device)
+  modifier = torch.sum(torch.tanh(freqs) * depth_modifier, dim=-1)
+  return soft_limit(f_center + bandwidth_scale * bw * modifier, hz_min, hz_max)
 
 
 # ----------------------------------------------------------------------------
@@ -473,6 +633,13 @@ def resample(inputs, n_timesteps: int, method: Text = 'linear',
   elif len(shape) == 4:
     out = out.reshape(shape[0], int(n_timesteps), shape[2], shape[3])
   return out
+
+
+def center_crop(audio, frame_size):
+  """core.center_crop (core.py:717-730): removes the frame_size // 2 samples that
+  centred framing pads at each end of axis 1."""
+  pad_amount = int(frame_size // 2)
+  return audio[:, pad_amount:-pad_amount]
 
 
 # ----------------------------------------------------------------------------

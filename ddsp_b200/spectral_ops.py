@@ -53,6 +53,28 @@ def compute_mag(audio, size=2048, overlap=0.75, pad_end=True):
   return torch.abs(stft(audio, frame_size=size, overlap=overlap, pad_end=pad_end))
 
 
+def stft_np(audio, frame_size=2048, overlap=0.75, pad_end=True):
+  """spectral_ops.stft_np (spectral_ops.py:50-64): the non-differentiable NumPy STFT of
+  audio [N] or [batch, N] -> [n_frames, frame_size // 2 + 1] or [batch, n_frames, ...],
+  complex64 for float32 audio.  The reference calls librosa.stft(y, n_fft=frame_size,
+  hop_length=hop, center=False).T on each example; this restates those semantics
+  without librosa: frames of frame_size samples every hop = frame_size * (1 - overlap)
+  samples from the first, not centred, times librosa's default window (a periodic Hann
+  of length frame_size, in float64), then an rfft of frame_size points.  pad_end pads
+  the end with pad(..., 'same') first."""
+  assert frame_size * overlap % 2.0 == 0.0
+  frame_size = int(frame_size)
+  hop_size = int(frame_size * (1.0 - overlap))
+  is_2d = (len(audio.shape) == 2)
+  if pad_end:
+    audio = pad(audio, frame_size, hop_size, 'same', axis=int(is_2d)).cpu().numpy()
+  audio = np.asarray(audio)
+  window = 0.5 - 0.5 * np.cos(2.0 * np.pi * np.arange(frame_size) / frame_size)
+  frames = np.lib.stride_tricks.sliding_window_view(audio, frame_size, axis=-1)
+  s = np.fft.rfft(frames[..., ::hop_size, :] * window, axis=-1)
+  return s.astype(np.result_type(audio.dtype, np.complex64))
+
+
 # ---- CUDA pieces of the spectrogram loss (include/ddsp_b200.h) ---------------
 _WINDOWS = {}
 
@@ -264,7 +286,7 @@ def stft_cuda(audio, frame_size, overlap=0.75):
 
 # ---- loudness and RMS power (spectral_ops.py:136-324, csrc/loudness.cuh) ------
 F0_RANGE = 127.0  # MIDI
-DB_RANGE = 80.0
+DB_RANGE = core.DB_RANGE  # dB (80.0)
 _A_WEIGHTS = {}
 
 
@@ -764,3 +786,26 @@ class PretrainedCREPE:
     core._launch('ddsp_b200_crepe_viterbi', x, centers,
                  *core._workspace('ddsp_b200_crepe_viterbi_workspace_bytes', x.device, b, t), b, t)
     return centers.to(torch.int64)
+
+
+def pad_or_trim_to_expected_length(vector, expected_len, pad_value=0, len_tolerance=20,
+                                   use_tf=False):
+  """spectral_ops.pad_or_trim_to_expected_length (spectral_ops.py:367-425): pads the
+  end of the last axis of a 1-D or 2-D vector with pad_value, or trims it, to
+  expected_len; ValueError if the lengths differ by more than len_tolerance.
+  use_tf=True works on torch tensors and keeps the gradient; use_tf=False returns
+  NumPy."""
+  expected_len = int(expected_len)
+  vector_len = int(vector.shape[-1])
+  if abs(vector_len - expected_len) > len_tolerance:
+    raise ValueError('Vector length: {} differs from expected length: {} '
+                     'beyond tolerance of : {}'.format(vector_len, expected_len,
+                                                       len_tolerance))
+  vector = torch.as_tensor(vector) if use_tf else np.asarray(vector)
+  if vector_len < expected_len:
+    n_padding = expected_len - vector_len
+    if use_tf:
+      return torch.nn.functional.pad(vector, (0, n_padding), value=pad_value)
+    return np.pad(vector, [(0, 0)] * (vector.ndim - 1) + [(0, n_padding)],
+                  mode='constant', constant_values=pad_value)
+  return vector[..., :expected_len]
