@@ -8,6 +8,7 @@ from ddsp_b200 import _lib
 from ddsp_b200 import colab_utils
 from ddsp_b200 import core
 from ddsp_b200 import dags
+from ddsp_b200 import decoders
 from ddsp_b200 import effects
 from ddsp_b200 import heuristics
 from ddsp_b200 import host
@@ -17,6 +18,7 @@ from ddsp_b200 import preprocessing
 from ddsp_b200 import processors
 from ddsp_b200 import synthetic_data
 from ddsp_b200 import synths
+from ddsp_b200.decoders import RnnFcDecoder
 from ddsp_b200.effects import (ExpDecayReverb, FIRFilter, FilteredNoiseReverb,
                                ModDelay, Reverb)
 from ddsp_b200.host import HostDecoder

@@ -35,7 +35,7 @@ def _ctype(spelling, is_return=False):
   t = re.sub(r'\bconst\b|\s', '', spelling)
   if is_return and t == 'char*':
     return ctypes.c_char_p
-  if t == 'ddsp_b200_host_pipeline**':
+  if t in ('ddsp_b200_host_pipeline**', 'ddsp_b200_gru**'):
     return ctypes.POINTER(ctypes.c_void_p)
   if t.endswith('*') and not t.endswith('**'):
     return ctypes.c_void_p

@@ -55,6 +55,9 @@ kernels, exposed as `torch.autograd.Function`s:
   * `HmmLogProbFn` - the HMM log-likelihood of `losses.HmmTranscriber`, with
     gradients to the observations (pitch and amplitude); routed to by
     `core.hmm_log_prob` under grad;
+  * `GruFn` - the Keras GRU of `nn.Rnn` / `decoders.RnnFcDecoder`: the recurrence and
+    its backpropagation through time are one launch each (`csrc/gru.cuh`), the GEMMs
+    around them cuBLAS;
   * `CrepeLossFramesFn` - the framing and per-frame normalisation of
     `losses.PretrainedCREPE`, d audio, which the embedding losses train through;
   * `DecoderFn` / `decoder_train` - the whole `ae.gin` decoder from RAW network
@@ -65,6 +68,7 @@ kernels, exposed as `torch.autograd.Function`s:
 `harmonic_controls` / `exp_sigmoid` below are the same `get_controls` arithmetic as
 differentiable torch ops, kept for callers that compose their own graphs.
 """
+import ctypes
 import math
 
 import torch
@@ -966,6 +970,92 @@ class CrepeLossFramesFn(torch.autograd.Function):
     core._launch('ddsp_b200_crepe_frames_backward', audio,
                  grad_frames.contiguous().to(torch.float32), d_audio, b, n, *ctx.cfg)
     return d_audio, None, None
+
+
+class GruHandle:
+  """A `ddsp_b200_gru` handle: the recurrent weights of one GRU layer packed for the
+  recurrence kernels on one device.  Freed with the object.  Copying or pickling it
+  raises TypeError: two objects would free one handle."""
+
+  def __init__(self, units, device):
+    self.units, self.device = int(units), torch.device(device)
+    self.ptr = None
+    self.loaded = None   # (data_ptr, version) of the weights the last load packed
+    lib = _lib.load()
+    out = ctypes.c_void_p()
+    with torch.cuda.device(self.device):
+      _lib.check(lib.ddsp_b200_gru_create(ctypes.byref(out), self.units))
+    self.ptr = out.value
+
+  def load(self, recurrent_kernel, recurrent_bias):
+    core._launch('ddsp_b200_gru_load', self.ptr, recurrent_kernel, recurrent_bias)
+    self.loaded = _weights_key(recurrent_kernel, recurrent_bias)
+
+  def __del__(self):
+    if self.ptr is not None:
+      _lib.load().ddsp_b200_gru_destroy(self.ptr)
+      self.ptr = None
+
+  def _refuse_copy(self, *args):
+    raise TypeError('GruHandle owns device memory and cannot be copied or pickled; '
+                    'create a new handle (nn.Gru does so on its next call)')
+
+  __copy__ = __deepcopy__ = __reduce_ex__ = _refuse_copy
+
+
+def _weights_key(recurrent_kernel, recurrent_bias):
+  return tuple((t.data_ptr(), t._version) for t in (recurrent_kernel, recurrent_bias))
+
+
+class GruFn(torch.autograd.Function):
+  """The Keras GRU (reset_after=True, gate columns z | r | h, h0 = 0) over x [B, T, in]
+  with kernel [in, 3H], recurrent_kernel [H, 3H] and bias [2, 3H]: every state
+  [B, T, H].  The input projection and the gradients' GEMMs run on cuBLAS; the
+  recurrence is one `ddsp_b200_gru_forward` launch after one `ddsp_b200_gru_load`, and
+  its backward one `ddsp_b200_gru_backward` launch.  The gate buffer [B, T, 4H] takes
+  x W + b and then what the backward reads, so nothing else is stored.  `save` is
+  whether to keep it for a backward (grad mode with an input that requires grad)."""
+
+  @staticmethod
+  def forward(ctx, x, kernel, recurrent_kernel, bias, handle, save):
+    b, t, _ = x.shape
+    h = handle.units
+    gates = torch.empty((b, t, 4 * h), dtype=torch.float32, device=x.device)
+    states = torch.empty((b, t + 1, h), dtype=torch.float32, device=x.device)
+    states[:, 0].zero_()
+    if b and t:
+      torch.addmm(bias[0], x.reshape(b * t, -1), kernel,
+                  out=gates.view(b * t, 4 * h)[:, :3 * h])
+      handle.load(recurrent_kernel, bias[1])
+      core._launch('ddsp_b200_gru_forward', handle.ptr, gates, states, b, t)
+    if save:
+      ctx.save_for_backward(x, kernel, recurrent_kernel, bias, gates, states)
+      ctx.handle = handle
+      ctx.key = _weights_key(recurrent_kernel, bias[1])
+    return states[:, 1:]
+
+  @staticmethod
+  def backward(ctx, grad_out):
+    x, kernel, recurrent_kernel, bias, gates, states = ctx.saved_tensors
+    b, t, n_in = x.shape
+    h = ctx.handle.units
+    d_pre = torch.empty((b, t, 3 * h), dtype=torch.float32, device=x.device)
+    # row t + 1 of each item is zero: d_rec and states then pair up row by row
+    d_rec = torch.empty((b, t + 1, 3 * h), dtype=torch.float32, device=x.device)
+    if b and t:
+      if ctx.handle.loaded != ctx.key:   # another call of the layer packed other weights
+        ctx.handle.load(recurrent_kernel, bias[1])
+      core._launch('ddsp_b200_gru_backward', ctx.handle.ptr, gates, states,
+                   grad_out.contiguous().to(torch.float32), d_pre, d_rec, b, t)
+    else:
+      d_pre.zero_()
+      d_rec.zero_()
+    d_pre2, d_rec2 = d_pre.view(b * t, 3 * h), d_rec.view(b * (t + 1), 3 * h)
+    dx = (d_pre2 @ kernel.t()).view(b, t, n_in)
+    d_kernel = x.reshape(b * t, n_in).t() @ d_pre2
+    d_recurrent = states.view(b * (t + 1), h).t() @ d_rec2
+    d_bias = torch.stack([d_pre2.sum(0), d_rec2.sum(0)])
+    return dx, d_kernel, d_recurrent, d_bias, None, None
 
 
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):

@@ -1,0 +1,253 @@
+// C ABI of the network layers' recurrences (gru.cuh): the GRU handle, which owns the
+// packed recurrent weights of one layer on one device, and its pack, forward and
+// backward-through-time launches.
+#include "capi.cuh"
+#include "gru.cuh"
+
+using namespace ddsp;
+
+struct ddsp_b200_gru {
+  int device = -1;
+  int H = 0;
+  float* pack = nullptr;   // forward blocks, backward blocks, c: 6 H^2 + 3 H floats
+  bool loaded = false;
+  // clusters of each launch that fit on the device at once (0: it does not fit)
+  int fwd_clusters[kGruMaxSlice] = {};
+  int bwd_clusters[kGruMaxSlice] = {};
+};
+
+namespace {
+
+template <int BS>
+void* gru_kernel(int H, bool backward) {
+  if (gru_chunks(H) == 4)
+    return backward ? (void*)gru_backward_kernel<kGruRegRowsBwd, BS>
+                    : (void*)gru_forward_kernel<kGruRegRowsFwd, BS>;
+  return backward ? (void*)gru_backward_kernel<0, BS> : (void*)gru_forward_kernel<0, BS>;
+}
+
+void* gru_kernel(int H, int BS, bool backward) {
+  switch (BS) {
+    case 1: return gru_kernel<1>(H, backward);
+    case 2: return gru_kernel<2>(H, backward);
+    case 3: return gru_kernel<3>(H, backward);
+    default: return gru_kernel<4>(H, backward);
+  }
+}
+
+// How many clusters of the launch (H, BS, direction) the device runs at once, asked of
+// the occupancy calculator; 0 when its shared memory does not fit.
+int gru_max_clusters(int H, int BS, bool backward) {
+  const size_t smem = gru_smem_bytes(H, BS, backward);
+  if (smem > kGruMaxSmem) return 0;
+  const void* kern = gru_kernel(H, BS, backward);
+  // The calculator needs the reservation the launch will make, so this is the one place
+  // outside launch() that sets it (launch() sets it again before every launch).
+  if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) !=
+      cudaSuccess) {
+    (void)cudaGetLastError();
+    return 0;
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(kGruCluster);
+  cfg.blockDim = dim3(gru_chunks(H) * (H / kGruCluster));
+  cfg.dynamicSmemBytes = smem;
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return 0;
+  }
+  return n;
+}
+
+// Items per cluster for B items: the smallest slice whose clusters all run at once, or
+// else the largest that fits (the clusters then run in waves).  0: nothing fits.
+int gru_slice(const int* clusters, int B) {
+  int best = 0;
+  for (int bs = 1; bs <= kGruMaxSlice; ++bs) {
+    if (clusters[bs - 1] <= 0) continue;
+    best = bs;
+    if ((B + bs - 1) / bs <= clusters[bs - 1]) return bs;
+  }
+  return best;
+}
+
+// The handle's own checks: not null, loaded, and on the current device.
+int gru_check(const ddsp_b200_gru* gru, const char* fn) {
+  DDSP_REQUIRE(gru != nullptr, DDSP_B200_E_INVALID, "%s: null handle", fn);
+  int dev = 0;
+  DDSP_CUDA_TRY(cudaGetDevice(&dev), fn);
+  DDSP_REQUIRE(dev == gru->device, DDSP_B200_E_INVALID,
+               "%s: the handle belongs to device %d, the current device is %d", fn,
+               gru->device, dev);
+  return 0;
+}
+
+template <int RR, int BS>
+int launch_gru_forward(const ddsp_b200_gru* g, float* gates, float* states, int B, int T,
+                       cudaStream_t st) {
+  const int H = g->H;
+  return launch("gru_forward", gru_forward_kernel<RR, BS>,
+                dim3(kGruCluster * ((B + BS - 1) / BS)), dim3(gru_chunks(H) * (H / kGruCluster)),
+                gru_smem_bytes(H, BS, false), st, (const float*)g->pack, gates, states, B, T, H);
+}
+
+template <int RR, int BS>
+int launch_gru_backward(const ddsp_b200_gru* g, const float* gates, const float* states,
+                        const float* grad_out, float* d_pre, float* d_rec, int B, int T,
+                        cudaStream_t st) {
+  const int H = g->H;
+  return launch("gru_backward", gru_backward_kernel<RR, BS>,
+                dim3(kGruCluster * ((B + BS - 1) / BS)), dim3(gru_chunks(H) * (H / kGruCluster)),
+                gru_smem_bytes(H, BS, true), st, (const float*)g->pack, gates, states,
+                grad_out, d_pre, d_rec, B, T, H);
+}
+
+template <int BS>
+int gru_forward_bs(const ddsp_b200_gru* g, float* gates, float* states, int B, int T,
+                   cudaStream_t st) {
+  return gru_chunks(g->H) == 4
+             ? launch_gru_forward<kGruRegRowsFwd, BS>(g, gates, states, B, T, st)
+             : launch_gru_forward<0, BS>(g, gates, states, B, T, st);
+}
+
+template <int BS>
+int gru_backward_bs(const ddsp_b200_gru* g, const float* gates, const float* states,
+                    const float* grad_out, float* d_pre, float* d_rec, int B, int T,
+                    cudaStream_t st) {
+  return gru_chunks(g->H) == 4
+             ? launch_gru_backward<kGruRegRowsBwd, BS>(g, gates, states, grad_out, d_pre,
+                                                       d_rec, B, T, st)
+             : launch_gru_backward<0, BS>(g, gates, states, grad_out, d_pre, d_rec, B, T, st);
+}
+
+}  // namespace
+
+extern "C" {
+
+int ddsp_b200_gru_takes(int units) { return units >= 32 && units <= 512 && units % 32 == 0; }
+
+int ddsp_b200_gru_create(ddsp_b200_gru** out, int units) {
+  const char* fn = "gru_create";
+  DDSP_REQUIRE(out != nullptr, DDSP_B200_E_INVALID, "%s: null out", fn);
+  *out = nullptr;
+  DDSP_REQUIRE(ddsp_b200_gru_takes(units), DDSP_B200_E_UNSUPPORTED,
+               "%s: units=%d; the GRU takes multiples of 32 from 32 to 512", fn, units);
+  int dev = 0;
+  DDSP_CUDA_TRY(cudaGetDevice(&dev), "gru_create: cudaGetDevice");
+  ddsp_b200_gru* g = new ddsp_b200_gru();
+  g->device = dev;
+  g->H = units;
+  const size_t n = 6 * (size_t)units * units + 3 * (size_t)units;
+  cudaError_t e = cudaMalloc(&g->pack, n * sizeof(float));
+  if (e != cudaSuccess) {
+    (void)cudaGetLastError();
+    delete g;
+    set_error("%s: cudaMalloc(%zu B): %s", fn, n * sizeof(float), cudaGetErrorString(e));
+    return DDSP_B200_E_CUDA;
+  }
+  for (int bs = 1; bs <= kGruMaxSlice; ++bs) {
+    g->fwd_clusters[bs - 1] = gru_max_clusters(units, bs, false);
+    g->bwd_clusters[bs - 1] = gru_max_clusters(units, bs, true);
+  }
+  *out = g;
+  return 0;
+}
+
+int ddsp_b200_gru_destroy(ddsp_b200_gru* gru) {
+  if (!gru) return 0;
+  int cur = 0;
+  cudaGetDevice(&cur);
+  cudaSetDevice(gru->device);
+  cudaFree(gru->pack);   // waits for the handle's queued launches to finish
+  cudaSetDevice(cur);
+  delete gru;
+  return 0;
+}
+
+int ddsp_b200_gru_clusters(const ddsp_b200_gru* gru, int B, int backward) {
+  if (!gru || B < 1) return 0;
+  const int* c = backward ? gru->bwd_clusters : gru->fwd_clusters;
+  const int bs = gru_slice(c, B);
+  return bs ? c[bs - 1] : 0;
+}
+
+int ddsp_b200_gru_load(ddsp_b200_gru* gru, const float* recurrent_kernel,
+                       const float* recurrent_bias, void* stream) {
+  const char* fn = "gru_load";
+  DDSP_REQUIRE(gru != nullptr, DDSP_B200_E_INVALID, "%s: null handle", fn);
+  DDSP_REQUIRE(recurrent_kernel && recurrent_bias, DDSP_B200_E_INVALID, "%s: null pointer", fn);
+  if (int rc = gru_check(gru, fn)) return rc;
+  const int H = gru->H;
+  if (int rc = check_overlap(fn, {DDSP_OUT(gru->pack, 6 * (size_t)H * H + 3 * H)},
+                             {DDSP_IN(recurrent_kernel, 3 * (size_t)H * H),
+                              DDSP_IN(recurrent_bias, 3 * H)}))
+    return rc;
+  const int64_t n = 6LL * H * H + 3 * H;
+  int rc = launch("gru_pack", gru_pack_kernel, dim3(grid_for(n, 256)), dim3(256), 0,
+                  (cudaStream_t)stream, recurrent_kernel, recurrent_bias, gru->pack, H);
+  if (rc) return rc;
+  gru->loaded = true;
+  return 0;
+}
+
+int ddsp_b200_gru_forward(ddsp_b200_gru* gru, float* gates, float* states, int B, int T,
+                          void* stream) {
+  const char* fn = "gru_forward";
+  DDSP_REQUIRE(gru != nullptr, DDSP_B200_E_INVALID, "%s: null handle", fn);
+  DDSP_REQUIRE(B >= 0 && T >= 0, DDSP_B200_E_INVALID, "%s: bad shape B=%d T=%d", fn, B, T);
+  if (B == 0 || T == 0) return 0;
+  DDSP_REQUIRE(gates && states, DDSP_B200_E_INVALID, "%s: null pointer", fn);
+  if (int rc = gru_check(gru, fn)) return rc;
+  DDSP_REQUIRE(gru->loaded, DDSP_B200_E_INVALID,
+               "%s: no recurrent weights: call ddsp_b200_gru_load first", fn);
+  const int H = gru->H;
+  if (int rc = check_overlap(fn, {DDSP_OUT(gates, extent(B, T, 4 * H))},
+                             {DDSP_IN(states, extent(B, T + 1, H))}))
+    return rc;
+  const int bs = gru_slice(gru->fwd_clusters, B);
+  DDSP_REQUIRE(bs > 0, DDSP_B200_E_UNSUPPORTED,
+               "%s: no cluster of the H=%d recurrence fits on this device", fn, H);
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (bs) {
+    case 1: return gru_forward_bs<1>(gru, gates, states, B, T, st);
+    case 2: return gru_forward_bs<2>(gru, gates, states, B, T, st);
+    case 3: return gru_forward_bs<3>(gru, gates, states, B, T, st);
+    default: return gru_forward_bs<4>(gru, gates, states, B, T, st);
+  }
+}
+
+int ddsp_b200_gru_backward(ddsp_b200_gru* gru, const float* gates, const float* states,
+                           const float* grad_out, float* d_pre, float* d_rec, int B, int T,
+                           void* stream) {
+  const char* fn = "gru_backward";
+  DDSP_REQUIRE(gru != nullptr, DDSP_B200_E_INVALID, "%s: null handle", fn);
+  DDSP_REQUIRE(B >= 0 && T >= 0, DDSP_B200_E_INVALID, "%s: bad shape B=%d T=%d", fn, B, T);
+  if (B == 0 || T == 0) return 0;
+  DDSP_REQUIRE(gates && states && grad_out && d_pre && d_rec, DDSP_B200_E_INVALID,
+               "%s: null pointer", fn);
+  if (int rc = gru_check(gru, fn)) return rc;
+  DDSP_REQUIRE(gru->loaded, DDSP_B200_E_INVALID,
+               "%s: no recurrent weights: call ddsp_b200_gru_load first", fn);
+  const int H = gru->H;
+  const size_t n_pre = extent(B, T, 3 * H), n_rec = extent(B, T + 1, 3 * H);
+  DDSP_REQUIRE(!overlaps(d_pre, n_pre * sizeof(float), d_rec, n_rec * sizeof(float)),
+               DDSP_B200_E_INVALID, "%s: d_pre must not overlap d_rec", fn);
+  if (int rc = check_overlap(fn, {DDSP_OUT(d_pre, n_pre), DDSP_OUT(d_rec, n_rec)},
+                             {DDSP_IN(gates, extent(B, T, 4 * H)),
+                              DDSP_IN(states, extent(B, T + 1, H)),
+                              DDSP_IN(grad_out, extent(B, T, H))}))
+    return rc;
+  const int bs = gru_slice(gru->bwd_clusters, B);
+  DDSP_REQUIRE(bs > 0, DDSP_B200_E_UNSUPPORTED,
+               "%s: no cluster of the H=%d recurrence fits on this device", fn, H);
+  cudaStream_t st = (cudaStream_t)stream;
+  switch (bs) {
+    case 1: return gru_backward_bs<1>(gru, gates, states, grad_out, d_pre, d_rec, B, T, st);
+    case 2: return gru_backward_bs<2>(gru, gates, states, grad_out, d_pre, d_rec, B, T, st);
+    case 3: return gru_backward_bs<3>(gru, gates, states, grad_out, d_pre, d_rec, B, T, st);
+    default: return gru_backward_bs<4>(gru, gates, states, grad_out, d_pre, d_rec, B, T, st);
+  }
+}
+
+}  // extern "C"

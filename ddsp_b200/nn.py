@@ -1,7 +1,17 @@
-"""The masking functions of `ddsp/training/nn.py:359-557`: note segmentation, per-note
-moments and pooling over notes, as the MIDI autoencoder uses them
+"""The layers of `ddsp/training/nn.py` that decoders.RnnFcDecoder builds from (Fc,
+FcStack, Rnn, split_to_dict), and its masking functions (nn.py:359-557): note
+segmentation, per-note moments and pooling over notes, as the MIDI autoencoder uses them
 (`models/midi_autoencoder.py`: `add_slowness_loss` and `ZMidiAutoencoder.z_note_encode`).
-Same names, arguments and defaults as the reference; no network layers.
+Same names, arguments and defaults as the reference.
+
+The layers are torch modules with Keras semantics: parameters keep the Keras names,
+layouts and initialisers (Dense `kernel` [in, out] glorot-uniform and `bias` zeros,
+LayerNormalization `gamma` ones and `beta` zeros, GRU `kernel` [in, 3H] glorot-uniform,
+`recurrent_kernel` [H, 3H] orthogonal and `bias` [2, 3H] zeros), so a reference
+checkpoint's arrays assign one to one.  As Keras builds a layer at its first call, the
+input width is fixed then and the parameters are created on the input's device.
+Dense and LayerNormalization are torch ops (cuBLAS); the GRU's recurrence runs on the
+CUDA kernels of `csrc/gru.cuh` (DESIGN.md section 3.32).
 
 get_note_mask, get_note_mask_from_onset, get_note_moments and pool_over_notes run on the
 CUDA kernels of `csrc/notes.cuh` (DESIGN.md section 3.25), which never build the
@@ -9,8 +19,11 @@ reference's [batch, time, notes, dims] products.  get_note_lengths,
 get_short_note_loss_mask and straight_through_int_quantization are small torch
 reductions and elementwise ops.
 """
+import math
+
 import torch
 
+from ddsp_b200 import _lib
 from ddsp_b200 import autograd
 from ddsp_b200 import core
 
@@ -144,3 +157,177 @@ def get_short_note_loss_mask(note_mask, note_lengths, note_pitches, min_length=4
   short = ((core._as_f32(note_lengths).to(note_mask.device) < min_length) &
            (core._as_f32(note_pitches).to(note_mask.device) > 0.0))
   return torch.sum(note_mask * short.to(torch.float32)[:, None, :], dim=-1)
+
+
+# ------------------ Utilities ---------------------------------------------------
+def split_to_dict(tensor, tensor_splits):
+  """nn.split_to_dict (nn.py:324-329): the last axis of tensor cut into
+  {label: [..., size]} for the (label, size) pairs of tensor_splits, in order.  The sizes
+  must add up to the axis (ValueError otherwise, as tf.split raises)."""
+  labels = [v[0] for v in tensor_splits]
+  sizes = [int(v[1]) for v in tensor_splits]
+  if sum(sizes) != tensor.shape[-1]:
+    raise ValueError(f'split_to_dict: sizes {sizes} add up to {sum(sizes)}, but the last '
+                     f'axis of the tensor has {tensor.shape[-1]}')
+  return dict(zip(labels, torch.split(tensor, sizes, dim=-1)))
+
+
+def _leaky_relu(x):
+  """get_nonlinearity('leaky_relu') (nn.py:332-339): tf.nn.leaky_relu, slope 0.2."""
+  return torch.nn.functional.leaky_relu(x, 0.2)
+
+
+def _glorot_uniform(shape, device):
+  """tf.keras.initializers.GlorotUniform for a [fan_in, fan_out] kernel."""
+  limit = math.sqrt(6.0 / (shape[0] + shape[1]))
+  return torch.nn.init.uniform_(torch.zeros(shape, device=device), -limit, limit)
+
+
+def _width(x, name):
+  if not torch.is_tensor(x):
+    raise TypeError(f'{name}: expected a torch tensor, got {type(x).__name__}')
+  if x.dim() < 2:
+    raise ValueError(f'{name}: expected [..., features], got shape {tuple(x.shape)}')
+  return int(x.shape[-1])
+
+
+class _Lazy(torch.nn.Module):
+  """A layer whose parameters are created at its first call (Keras build): the input
+  width is fixed then, and a later call with another width raises ValueError."""
+
+  def __init__(self, name):
+    super().__init__()
+    self._name = name
+    self.input_width = None
+
+  def _built(self, x):
+    width = _width(x, self._name)
+    if self.input_width is None:
+      self.input_width = width
+      self.build(width, x.device)
+    elif width != self.input_width:
+      raise ValueError(f'{self._name}: built for inputs of width {self.input_width}, '
+                       f'called with width {width}')
+
+
+class Dense(_Lazy):
+  """tf.keras.layers.Dense(units) without activation: x kernel + bias."""
+
+  def __init__(self, units):
+    super().__init__('Dense')
+    self.units = int(units)
+
+  def build(self, width, device):
+    self.kernel = torch.nn.Parameter(_glorot_uniform((width, self.units), device))
+    self.bias = torch.nn.Parameter(torch.zeros(self.units, device=device))
+
+  def forward(self, x):
+    self._built(x)
+    return torch.matmul(x, self.kernel) + self.bias
+
+
+class LayerNormalization(_Lazy):
+  """tf.keras.layers.LayerNormalization() over the last axis: epsilon 1e-3, gamma ones,
+  beta zeros."""
+
+  def __init__(self, epsilon=1e-3):
+    super().__init__('LayerNormalization')
+    self.epsilon = float(epsilon)
+
+  def build(self, width, device):
+    self.gamma = torch.nn.Parameter(torch.ones(width, device=device))
+    self.beta = torch.nn.Parameter(torch.zeros(width, device=device))
+
+  def forward(self, x):
+    self._built(x)
+    return torch.nn.functional.layer_norm(x, (self.input_width,), self.gamma, self.beta,
+                                          self.epsilon)
+
+
+class Fc(torch.nn.Sequential):
+  """nn.Fc (nn.py:843-852): Dense(ch) -> LayerNormalization -> leaky ReLU."""
+
+  def __init__(self, ch=128, nonlinearity='leaky_relu'):
+    if nonlinearity != 'leaky_relu':
+      raise NotImplementedError(f'Fc: nonlinearity {nonlinearity!r}; only '
+                                "'leaky_relu' is supported")
+    super().__init__(Dense(ch), LayerNormalization())
+
+  def forward(self, x):
+    return _leaky_relu(super().forward(x))
+
+
+class FcStack(torch.nn.Sequential):
+  """nn.FcStack (nn.py:855-862): `layers` Fc(ch) layers."""
+
+  def __init__(self, ch=256, layers=2, nonlinearity='leaky_relu'):
+    super().__init__(*[Fc(ch, nonlinearity) for _ in range(layers)])
+
+
+class Gru(_Lazy):
+  """tf.keras.layers.GRU(units, return_sequences) with TF2's defaults: reset_after=True,
+  gate columns z | r | h, h0 = 0.  x [B, T, in] (float32 CUDA) -> [B, T, units], or the
+  last state [B, units] without return_sequences.  units must be a multiple of 32 from 32
+  to 512 (NotImplementedError at construction otherwise).  One handle per device
+  holds the packed recurrent weights; it is created at the first call on that device
+  and freed with the layer.  copy.deepcopy and pickling (torch.save) leave the handles
+  behind, so a copy never shares or frees the original's."""
+
+  def __init__(self, units, return_sequences=True):
+    super().__init__('GRU')
+    self.units = int(units)
+    if not _lib.load().ddsp_b200_gru_takes(self.units):
+      raise NotImplementedError(f'GRU: units={units}; the CUDA recurrence takes '
+                                'multiples of 32 from 32 to 512')
+    self.return_sequences = bool(return_sequences)
+    self._handles = {}
+
+  def __getstate__(self):
+    """Copies and pickles leave the handles behind: they own device memory, and the copy
+    creates its own at its first call on each device."""
+    state = dict(super().__getstate__())
+    state['_handles'] = {}
+    return state
+
+  def build(self, width, device):
+    self.kernel = torch.nn.Parameter(_glorot_uniform((width, 3 * self.units), device))
+    self.recurrent_kernel = torch.nn.Parameter(torch.nn.init.orthogonal_(
+        torch.zeros((self.units, 3 * self.units), device=device)))
+    self.bias = torch.nn.Parameter(torch.zeros((2, 3 * self.units), device=device))
+
+  def forward(self, x):
+    if not torch.is_tensor(x) or x.dim() != 3:
+      raise ValueError('GRU: expected x [batch, time, features], got '
+                       f'{tuple(x.shape) if torch.is_tensor(x) else type(x).__name__}')
+    if not x.is_cuda:
+      raise ValueError(f'GRU: x is on {x.device}; the recurrence runs on CUDA devices only')
+    self._built(x)
+    params = (self.kernel, self.recurrent_kernel, self.bias)
+    if any(p.device != x.device for p in params):
+      raise ValueError(f'GRU: x is on {x.device}, the parameters on {self.kernel.device}')
+    handle = self._handles.get(x.device)
+    if handle is None:
+      handle = self._handles[x.device] = autograd.GruHandle(self.units, x.device)
+    save = torch.is_grad_enabled() and any(t.requires_grad for t in (x,) + params)
+    with torch.cuda.device(x.device):
+      out = autograd.GruFn.apply(x.to(torch.float32).contiguous(),
+                                 *[p.contiguous() for p in params], handle, save)
+    return out if self.return_sequences else out[:, -1]
+
+
+class Rnn(torch.nn.Module):
+  """nn.Rnn (nn.py:866-879): one RNN layer, `dims` units.  rnn_type 'gru' only;
+  'lstm' and bidir=True raise NotImplementedError."""
+
+  def __init__(self, dims, rnn_type, return_sequences=True, bidir=False):
+    super().__init__()
+    if rnn_type not in ('gru', 'lstm'):
+      raise KeyError(rnn_type)
+    if rnn_type != 'gru' or bidir:
+      raise NotImplementedError(
+          f'Rnn: rnn_type={rnn_type!r}, bidir={bidir}; only the unidirectional '
+          "rnn_type='gru' is supported")
+    self.rnn = Gru(dims, return_sequences=return_sequences)
+
+  def forward(self, x):
+    return self.rnn(x)

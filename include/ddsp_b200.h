@@ -13,7 +13,7 @@
  *     current CUDA device.  Controls are [B, F, C]; audio is [B, N].
  *   - The caller allocates every input, output and workspace.  The library never
  *     allocates, frees or retains a pointer past the call (one exception, with
- *     explicit create/destroy: ddsp_b200_host_pipeline, below).
+ *     explicit create/destroy: ddsp_b200_host_pipeline and ddsp_b200_gru, below).
  *   - `stream` is a cudaStream_t passed as void*.  Calls are asynchronous and
  *     re-entrant; there is no global mutable state (the last-error string is
  *     thread-local).
@@ -192,7 +192,7 @@ int ddsp_b200_decoder_forward(const float* amps_raw, const float* hd_raw,
  * batch (the Philox item index of a chunk's rows is offset accordingly).
  *
  * The pipeline handle owns one device staging allocation for max_B items of
- * shape (F, K, nb, N), two copy streams and the events - the only objects this
+ * shape (F, K, nb, N), two copy streams and the events - with ddsp_b200_gru, the only objects this
  * library ever allocates; *_destroy releases them.  A handle belongs to the
  * device that was current at creation and serialises its own calls.
  * amps_raw/f0_hz [B,F,1], hd_raw [B,F,K], mags_raw [B,F,nb], audio [B,N]: HOST
@@ -1132,6 +1132,47 @@ int ddsp_b200_synthetic_notes(const int64_t* seeds, unsigned int* key, int* pos,
                               double* mags, double* divisor, int B, int T, int K, int M,
                               int min_note_length, int max_note_length, double p_silent,
                               double p_vibrato, int get_controls, void* stream);
+
+/* The recurrence of tf.keras.layers.GRU (TF2 defaults: reset_after=True, gate columns
+ * z | r | h), as decoders.RnnFcDecoder runs it (nn.Rnn, nn.py:866-879):
+ *   z = sigmoid(x W_z + b_z + h U_z + c_z),  r = sigmoid(x W_r + b_r + h U_r + c_r),
+ *   h~ = tanh(x W_h + b_h + r * (h U_h + c_h)),  h' = z * h + (1 - z) * h~.
+ * Only the sequential part is here; the caller computes x W + b before the forward and
+ * the weight, bias and input gradients from d_pre and d_rec after the backward.
+ *
+ * A handle belongs to one layer on the device that was current at creation and owns
+ * the recurrent weights packed for the kernels (6 H^2 + 3 H floats of device memory,
+ * freed by _destroy).  units = H must be a multiple of 32 from 32 to 512
+ * (ddsp_b200_gru_takes(H); any other H is E_UNSUPPORTED).  Launches of one handle
+ * must be ordered on one stream: _load rewrites what later launches read.
+ *
+ * _load packs recurrent_kernel U [H, 3H] and recurrent_bias c [3H] (one launch).
+ * _forward (one launch): gates [B, T, 4H] holds x W + b in its first 3H columns and
+ *   receives what the backward reads, z | r | h~ | h U_h + c_h; states [B, T + 1, H]
+ *   holds h_0 in row 0 and receives h_1 .. h_T.  gates must not overlap states.
+ * _backward (one launch): grad_out [B, T, H] = dL/dh_1 .. h_T -> d_pre [B, T, 3H], the
+ *   gradient of x W + b, and d_rec [B, T + 1, 3H], the gradient of h U + c in rows
+ *   0 .. T-1 and zeros in row T, from the forward's gates and states and the weights of
+ *   the last _load.  Row b (T + 1) + t of d_rec pairs with the same row of states (h_t),
+ *   so dU = states^T d_rec is one GEMM over both flat buffers.  d_pre and d_rec overlap
+ *   no operand.
+ * B = 0 or T = 0 launches nothing.  FP32 in a fixed order: bit-reproducible, and item
+ * b's results depend on item b alone.
+ * _clusters: how many thread-block clusters of the B-item forward (backward != 0:
+ * backward) launch the device runs at once, as its occupancy calculator answered at
+ * creation (a pure host query; 0 for a null handle or B < 1). */
+typedef struct ddsp_b200_gru ddsp_b200_gru;
+int ddsp_b200_gru_takes(int units);
+int ddsp_b200_gru_create(ddsp_b200_gru** out, int units);
+int ddsp_b200_gru_destroy(ddsp_b200_gru* gru);
+int ddsp_b200_gru_clusters(const ddsp_b200_gru* gru, int B, int backward);
+int ddsp_b200_gru_load(ddsp_b200_gru* gru, const float* recurrent_kernel,
+                       const float* recurrent_bias, void* stream);
+int ddsp_b200_gru_forward(ddsp_b200_gru* gru, float* gates, float* states, int B, int T,
+                          void* stream);
+int ddsp_b200_gru_backward(ddsp_b200_gru* gru, const float* gates, const float* states,
+                           const float* grad_out, float* d_pre, float* d_rec, int B, int T,
+                           void* stream);
 
 #ifdef __cplusplus
 }
