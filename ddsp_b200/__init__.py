@@ -10,8 +10,10 @@ from ddsp_b200 import core
 from ddsp_b200 import dags
 from ddsp_b200 import decoders
 from ddsp_b200 import effects
+from ddsp_b200 import encoders
 from ddsp_b200 import heuristics
 from ddsp_b200 import host
+from ddsp_b200 import models
 from ddsp_b200 import nn
 from ddsp_b200 import postprocessing
 from ddsp_b200 import preprocessing

@@ -28,6 +28,16 @@ class Reverb(processors.Processor):
     self._add_dry = add_dry
     self._ir = None
 
+  # build()'s variables: the reference's weight name -> the attribute that holds it
+  _VARIABLES = {'ir': '_ir'}
+
+  def named_variables(self):
+    """[(name, torch.nn.Parameter)] of the variables build() created, with the
+    reference's weight names: empty before the first call, or when not trainable.
+    models.Autoencoder registers them as its parameters."""
+    return [(name, getattr(self, attr)) for name, attr in self._VARIABLES.items()
+            if getattr(self, attr) is not None]
+
   def _mask_dry_ir(self, ir):
     """effects.py:50-59: zero the first tap (the dry path)."""
     if ir.dim() == 1:
@@ -46,8 +56,8 @@ class Reverb(processors.Processor):
   def build(self, device=None):
     """effects.py:70-79: the single learned impulse response, N(0, 1e-6)."""
     if self.trainable and self._ir is None:
-      self._ir = (1e-6 * torch.randn(self._reverb_length, dtype=torch.float32,
-                                     device=device)).requires_grad_(True)
+      self._ir = torch.nn.Parameter(1e-6 * torch.randn(
+          self._reverb_length, dtype=torch.float32, device=device))
 
   def get_controls(self, audio, ir=None):
     """effects.py:81-101."""
@@ -88,6 +98,8 @@ class ExpDecayReverb(Reverb):
     # Test hook: a [1, reverb_length] tensor used instead of the Philox stream.
     self.injected_noise = None
 
+  _VARIABLES = {'gain': '_gain', 'decay': '_decay'}
+
   def next_offset(self):
     """Per-call Philox counter offset, so successive calls draw fresh noise."""
     return next(self._calls)
@@ -95,10 +107,10 @@ class ExpDecayReverb(Reverb):
   def build(self, device=None):
     """effects.py:153-166: the learned gain 2.0 and decay 4.0, shape [1]."""
     if self.trainable and self._gain is None:
-      self._gain = torch.full((1,), 2.0, dtype=torch.float32,
-                              device=device).requires_grad_(True)
-      self._decay = torch.full((1,), 4.0, dtype=torch.float32,
-                               device=device).requires_grad_(True)
+      self._gain = torch.nn.Parameter(torch.full((1,), 2.0, dtype=torch.float32,
+                                                 device=device))
+      self._decay = torch.nn.Parameter(torch.full((1,), 4.0, dtype=torch.float32,
+                                                  device=device))
 
   def _get_ir(self, gain, decay):
     """effects.py:144-151."""
@@ -143,12 +155,13 @@ class FilteredNoiseReverb(Reverb):
                                        initial_bias=initial_bias)
     self._magnitudes = None
 
+  _VARIABLES = {'magnitudes': '_magnitudes'}
+
   def build(self, device=None):
     """effects.py:240-249: the learned magnitudes, N(0, 1e-2)."""
     if self.trainable and self._magnitudes is None:
-      self._magnitudes = (1e-2 * torch.randn(
-          self._n_frames, self._n_filter_banks, dtype=torch.float32,
-          device=device)).requires_grad_(True)
+      self._magnitudes = torch.nn.Parameter(1e-2 * torch.randn(
+          self._n_frames, self._n_filter_banks, dtype=torch.float32, device=device))
 
   def _synth_ir(self, magnitudes):
     """`self._synth(magnitudes)` (effects.py:272); with gradients to the magnitudes

@@ -172,6 +172,52 @@ def split_to_dict(tensor, tensor_splits):
   return dict(zip(labels, torch.split(tensor, sizes, dim=-1)))
 
 
+# ------------------ Shapes ------------------------------------------------------
+def ensure_4d(x):
+  """nn.ensure_4d (nn.py:302-309): [B, C] -> [B, 1, 1, C] and [B, T, C] -> [B, T, 1, C];
+  any other rank is returned as it is."""
+  if x.dim() == 2:
+    return x[:, None, None, :]
+  if x.dim() == 3:
+    return x[:, :, None, :]
+  return x
+
+
+def inv_ensure_4d(x, n_dims):
+  """nn.inv_ensure_4d (nn.py:312-319): the inverse of ensure_4d for an input of rank
+  n_dims."""
+  if n_dims == 2:
+    return x[:, 0, 0, :]
+  if n_dims == 3:
+    return x[:, :, 0, :]
+  return x
+
+
+# ------------------ Normalization -----------------------------------------------
+def normalize_op(x, norm_type='layer', eps=1e-5):
+  """nn.normalize_op (nn.py:561-575): group, instance or layer normalization of x
+  [B, H, W, C], or x itself for norm_type None.  The C channels form
+  {'instance': C, 'layer': 1, 'group': 32}[norm_type] groups (KeyError for any other
+  name); each item's group is normalized over H, W and its channels by its mean and
+  population variance, (x - mean) / sqrt(var + eps).  'group' needs C to be a multiple
+  of 32 (ValueError otherwise, where TensorFlow fails in its reshape).  Torch ops,
+  differentiable, on any device."""
+  if norm_type is None:
+    return x
+  if x.dim() != 4:
+    raise ValueError(f'normalize_op: expected x [batch, height, width, channels], got '
+                     f'shape {tuple(x.shape)}')
+  shape = x.shape
+  channels = int(shape[-1])
+  n_groups = {'instance': channels, 'layer': 1, 'group': 32}[norm_type]
+  if channels % n_groups:
+    raise ValueError(f'normalize_op: norm_type={norm_type!r} splits the channels into '
+                     f'{n_groups} groups; {channels} channels do not divide evenly')
+  x = x.reshape(*shape[:-1], n_groups, channels // n_groups)
+  var, mean = torch.var_mean(x, dim=(1, 2, 4), correction=0, keepdim=True)
+  return ((x - mean) / torch.sqrt(var + eps)).reshape(shape)
+
+
 def _leaky_relu(x):
   """get_nonlinearity('leaky_relu') (nn.py:332-339): tf.nn.leaky_relu, slope 0.2."""
   return torch.nn.functional.leaky_relu(x, 0.2)
@@ -242,6 +288,30 @@ class LayerNormalization(_Lazy):
     self._built(x)
     return torch.nn.functional.layer_norm(x, (self.input_width,), self.gamma, self.beta,
                                           self.epsilon)
+
+
+class Normalize(_Lazy):
+  """nn.Normalize (nn.py:578-603): normalize_op(x, norm_type) with epsilon 1e-5, then a
+  learned per-channel `scale` (ones) and `shift` (zeros), both [1, 1, 1, C].  x is
+  [B, C], [B, T, C] or [B, H, W, C] (made 4-D by ensure_4d) and the result has x's
+  rank."""
+
+  def __init__(self, norm_type='layer'):
+    super().__init__('Normalize')
+    self.norm_type = norm_type
+
+  def build(self, width, device):
+    self.scale = torch.nn.Parameter(torch.ones((1, 1, 1, width), device=device))
+    self.shift = torch.nn.Parameter(torch.zeros((1, 1, 1, width), device=device))
+
+  def forward(self, x):
+    if not torch.is_tensor(x) or x.dim() not in (2, 3, 4):
+      raise ValueError('Normalize: expected x of rank 2, 3 or 4, got '
+                       f'{tuple(x.shape) if torch.is_tensor(x) else type(x).__name__}')
+    n_dims = x.dim()
+    x = normalize_op(ensure_4d(x), self.norm_type)
+    self._built(x)
+    return inv_ensure_4d(x * self.scale + self.shift, n_dims)
 
 
 class Fc(torch.nn.Sequential):

@@ -1,5 +1,5 @@
-"""How the timing scripts measure on the GPU: the card record, CUDA-event timing, input
-rings larger than the L2 cache, alternated rounds with their median, peak memory,
+"""How the timing scripts measure on the GPU: the card record, CUDA-event timing of calls
+and of the stages of a step, input rings larger than the L2 cache, alternated rounds with their median, peak memory,
 data-sheet peaks and JSON-line results.  Importing this module does not initialise
 CUDA, so a script's CPU-only paths still run without a GPU."""
 import json
@@ -51,6 +51,36 @@ def event_ms(fn, iters, warmup, inputs=None):
   stop.record()
   torch.cuda.synchronize()
   return start.elapsed_time(stop) / iters
+
+
+class StageEvents:
+  """Device time of the named stages of a step: begin(name) and end(name) record CUDA
+  events around a stage (a stage may recur within a step), and mean_ms(steps) gives
+  {name: ms per step} over every stage recorded since the last clear()."""
+
+  def __init__(self):
+    self._open, self._log = {}, []
+
+  def _record(self):
+    event = torch.cuda.Event(enable_timing=True)
+    event.record()
+    return event
+
+  def begin(self, name):
+    self._open[name] = self._record()
+
+  def end(self, name):
+    self._log.append((name, self._open.pop(name), self._record()))
+
+  def clear(self):
+    self._open, self._log = {}, []
+
+  def mean_ms(self, steps):
+    torch.cuda.synchronize()
+    totals = {}
+    for name, start, stop in self._log:
+      totals[name] = totals.get(name, 0.0) + start.elapsed_time(stop) / steps
+    return totals
 
 
 def l2_bytes():
