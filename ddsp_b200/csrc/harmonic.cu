@@ -5,7 +5,6 @@
 #include "harmonic.cuh"
 #include "harmonic_v4.cuh"
 #include "harmonic_backward.cuh"
-#include "harmonic_bwd2.cuh"
 #include "controls_bwd.cuh"
 
 namespace ddsp {
@@ -171,20 +170,11 @@ int ddsp_b200_harmonic_backward(const float* f0_hz, const float* grad_audio,
   HarmonicParams p = harm_params(f0_hz, nullptr, nullptr, nullptr, B, F, K, N,
                                  sample_rate, amp_method);
   p.Kp = K;
+  DDSP_REQUIRE(B <= 65535, DDSP_B200_E_UNSUPPORTED,
+               "harmonic_backward: B=%d exceeds the 65535 grid limit", B);
   DDSP_REQUIRE(ddsp_b200_harmonic_backward_takes(B, F, N), DDSP_B200_E_UNSUPPORTED,
                "harmonic_backward: needs hop %% 64 == 0 (hop = %d)", p.hop);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (harmonic_backward2_supported(p))
-    return launch_harmonic_backward2(p, grad_audio, g0, g1, st);
-  const size_t gbytes = sizeof(float) * (size_t)B * F * K;
-  DDSP_CUDA_TRY(cudaMemsetAsync(g0, 0, gbytes, st), "harmonic_backward: memset g0");
-  DDSP_CUDA_TRY(cudaMemsetAsync(g1, 0, gbytes, st), "harmonic_backward: memset g1");
-  p.FT = std::max(1, std::min(F, 2048 / p.hop));
-  const size_t smem = harmonic_backward_smem(p.FT, p.hop);
-  auto kern = amp_method == DDSP_B200_AMP_WINDOW ? harmonic_backward_kernel<true>
-                                                 : harmonic_backward_kernel<false>;
-  return launch("harmonic_backward", kern, dim3((F + p.FT - 1) / p.FT, B), kHbThreads, smem,
-                st, p, grad_audio, g0, g1);
+  return launch_harmonic_backward(p, grad_audio, g0, g1, (cudaStream_t)stream);
 }
 
 int ddsp_b200_harmonic_backward_f0(const float* f0_hz, const float* amps,

@@ -100,7 +100,7 @@ static HarmonicParams harm_params(const float* f0, const float* amps, const floa
 // Fixed-point phase (2^64 = one turn) of a frame where a = f / sr goes linearly
 // from a0 to a1: its total and its slope D = (a1 - a0) / hop.  harmonic_v4_kernel
 // alone forms D as (a1 - a0) * (1.0 / hop), equal for power-of-two hops; at hop
-// 192 the v4 forward's D and the v1 backward's may differ in the last bit.
+// 192 the v4 forward's D and the backward's may differ in the last bit.
 __device__ __forceinline__ unsigned long long frame_total_fix64(double a0, double a1, int hop) {
   return turns_to_fix64((double)hop * a0 + (a1 - a0) * (0.5 * (hop - 1)));
 }
@@ -112,9 +112,9 @@ __device__ __forceinline__ unsigned long long frame_slope_fix64(double a0, doubl
 // one double evaluation (2^-38 turn resolution).  base_sum sums their f0;
 // a_first and a_tile, f / sr of frame 0 and of the tile's first frame, are
 // formed by each caller in its own order.  v4 sums base_sum in float4 groups
-// ((x + y) + (z + w)), the two backward kernels strided over their threads: the
-// sums can differ in the last bit, and the forward and backward phases then by
-// about 2^-37 turns.
+// ((x + y) + (z + w)), the backward kernel strided over its threads: the sums can
+// differ in the last bit, and the forward and backward phases then by about 2^-37
+// turns.
 __device__ __forceinline__ unsigned long long tile_phase_base(
     double base_sum, double a_first, double a_tile, int hop, double inv_sr) {
   return turns_to_fix64((double)hop * (base_sum * inv_sr) +

@@ -244,9 +244,12 @@ def spectral_loss(target, value, fft_sizes=(2048, 1024, 512, 256, 128, 64),
 
 
 # Harmonic backward cases: (B, F, K, hop, sample_rate, amp method, f0 regime).  Every
-# hop (64: harmonic_backward2_kernel; 128 / 192 / 256: harmonic_backward_kernel), K,
-# F, method, rate and regime at least once; K = 7 / 9 / 100 / 260 reach the uniform
-# loop of the hop-64 kernel with K % 8 != 0.
+# K, F, method, rate and regime at least once, at hops of 1 to 128 64-sample blocks
+# (harmonic_backward_kernel stores block 0's totals and adds the later blocks');
+# K = 7 / 9 / 13 / 100 / 260 reach the harmonic-group loop with K % 8 != 0.  From hop
+# 512 on a CTA takes 4 frames, so F = 3, 5, 7 and 9 leave it a partial tile; there
+# 'cross1hz' and 'jump' reach the exact f0 < 1 Hz path, and 'glide' and 'nyquist' the
+# per-sample live counts, in blocks after the first.
 HARMONIC_CASES = [
     (2, 33, 100, 64, 16000, 'window', 'jump'),
     (2, 33, 100, 64, 16000, 'linear', 'glide'),
@@ -259,6 +262,12 @@ HARMONIC_CASES = [
     (2, 33, 7, 192, 16000, 'window', 'unvoiced'),
     (2, 33, 260, 256, 16000, 'window', 'nyquist'),
     (1, 33, 100, 256, 16000, 'linear', 'jump'),
+    (1, 33, 100, 512, 16000, 'window', 'cross1hz'),
+    (2, 9, 13, 512, 44100, 'linear', 'nyquist'),
+    (1, 7, 100, 1024, 16000, 'linear', 'jump'),
+    (2, 5, 60, 1024, 16000, 'window', 'glide'),
+    (1, 5, 100, 8192, 16000, 'window', 'nyquist'),
+    (1, 3, 9, 8192, 44100, 'linear', 'cross1hz'),
 ]
 
 # Filtered-noise backward cases: (B, F, nb, window_size, frame, ragged).  `ragged`

@@ -52,10 +52,11 @@ def _harmonic_inputs(B, F, K, sr, regime, seed):
 @pytest.mark.parametrize('B,F,K,hop,sr,method,regime', grad_ref.HARMONIC_CASES)
 def test_harmonic_backward_every_hop_and_f0_regime(B, F, K, hop, sr, method, regime):
   """HarmonicSynthesisFn with amplitudes, harmonic_distribution and f0 requiring
-  grad: hop 64 runs harmonic_backward2_kernel, other hops harmonic_backward_kernel;
+  grad: harmonic_backward_kernel at hops of one to 128 64-sample blocks per frame;
   the f0 regimes reach the exact f0 < 1 Hz branch (with harmonics actually masked
   in the 'jump' frames), the per-sample masks of frames whose live count changes,
-  and frames with no live harmonic."""
+  and frames with no live harmonic, in the first block of a frame and the later
+  ones."""
   N = F * hop
   f0, amp, hd = _harmonic_inputs(B, F, K, sr, regime, seed=K + hop)
   g = torch.randn(B, N, device=DEV, generator=torch.Generator(device=DEV).manual_seed(F))

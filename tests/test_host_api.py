@@ -134,7 +134,7 @@ _ABI_CASES = [
     ('harmonic_backward-B0', 'harmonic_backward', (P, P, P, P, 0, 10, 4, 640, SR, 0, None), 0, None),
     ('harmonic_backward-hop65', 'harmonic_backward', (P, P, P, P, 1, 10, 4, 650, SR, 0, None), E_UNSUPPORTED, b'harmonic_backward: needs hop % 64 == 0 (hop = 65)'),
     ('harmonic_backward-hop8256', 'harmonic_backward', (P, P, P, P, 1, 1, 4, 8256, SR, 0, None), E_UNSUPPORTED, b'harmonic_backward: needs hop % 64 == 0 (hop = 8256)'),
-    ('harmonic_backward-grid', 'harmonic_backward', (P, P, P, P, 65536, 10, 4, 640, SR, 0, None), E_UNSUPPORTED, b'harmonic_backward: needs hop % 64 == 0 (hop = 64)'),
+    ('harmonic_backward-grid-limit', 'harmonic_backward', (P, P, P, P, 65536, 10, 4, 640, SR, 0, None), E_UNSUPPORTED, b'harmonic_backward: B=65536 exceeds the 65535 grid limit'),
     ('harmonic_backward_f0-null', 'harmonic_backward_f0', (P, P, P, P, None, 1, 10, 4, 640, SR, 0, P, 120, None), E_INVALID, b'harmonic_backward_f0: null pointer'),
     ('harmonic_backward_f0-B', 'harmonic_backward_f0', (P, P, P, P, P, -1, 10, 4, 640, SR, 0, P, 120, None), E_INVALID, b'harmonic_backward_f0: bad shape B=-1 F=10 K=4 N=640'),
     ('harmonic_backward_f0-N', 'harmonic_backward_f0', (P, P, P, P, P, 1, 10, 4, 0, SR, 0, P, 120, None), E_INVALID, b'harmonic_backward_f0: bad shape B=1 F=10 K=4 N=0'),

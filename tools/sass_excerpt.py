@@ -14,7 +14,7 @@ LIB = os.path.join(ROOT, 'ddsp_b200', 'libddsp_b200.so')
 KERNELS = {
     'harmonic_v4': 'harmonic_v4_kernelILb1ELi64',
     'noise_ring': 'noise_ring_kernel',
-    'harmonic_backward2': 'harmonic_backward2_kernelILb1',
+    'harmonic_backward': 'harmonic_backward_kernelILb1',
     'lc_mac_ifft': 'lc_mac_ifft',
 }
 
