@@ -58,6 +58,9 @@ kernels, exposed as `torch.autograd.Function`s:
   * `GruFn` - the Keras GRU of `nn.Rnn` / `decoders.RnnFcDecoder`: the recurrence and
     its backpropagation through time are one launch each (`csrc/gru.cuh`), the GEMMs
     around them cuBLAS;
+  * `NormReluFn` - nn.Normalize followed by a ReLU at every site of `nn.ResNet`: one
+    fused launch forward (`csrc/norm.cuh`), and one backward launch plus a fixed-order
+    reduction of dscale and dshift; only the per-(item, group) mean and rstd are saved;
   * `CrepeLossFramesFn` - the framing and per-frame normalisation of
     `losses.PretrainedCREPE`, d audio, which the embedding losses train through;
   * `DecoderFn` / `decoder_train` - the whole `ae.gin` decoder from RAW network
@@ -1056,6 +1059,44 @@ class GruFn(torch.autograd.Function):
     d_recurrent = states.view(b * (t + 1), h).t() @ d_rec2
     d_bias = torch.stack([d_pre2.sum(0), d_rec2.sum(0)])
     return dx, d_kernel, d_recurrent, d_bias, None, None
+
+
+class NormReluFn(torch.autograd.Function):
+  """relu(normalize(x) * scale + shift) on x [B, H, W, C] (a contiguous, 16-byte aligned
+  float32 CUDA tensor) with scale and shift [C] and the channels in `groups` groups
+  (csrc/norm.cuh): one `ddsp_b200_norm_relu_forward` launch, which also writes each
+  (item, group)'s mean and rstd [B, groups]; those and x are all the backward keeps.
+  The backward is one `ddsp_b200_norm_relu_backward` call (two launches) that gives dx,
+  dscale and dshift."""
+
+  @staticmethod
+  def forward(ctx, x, scale, shift, groups):
+    b, h, w, c = x.shape
+    y = torch.empty_like(x)
+    mean = torch.empty((b, groups), dtype=torch.float32, device=x.device)
+    rstd = torch.empty_like(mean)
+    if y.numel():
+      core._launch('ddsp_b200_norm_relu_forward', x, scale, shift, y, mean, rstd, b, h * w,
+                   c, groups, 1e-5)
+    ctx.save_for_backward(x, scale, shift, mean, rstd)
+    ctx.groups = groups
+    return y
+
+  @staticmethod
+  def backward(ctx, grad_y):
+    x, scale, shift, mean, rstd = ctx.saved_tensors
+    b, h, w, c = x.shape
+    if not x.numel():
+      return torch.zeros_like(x), torch.zeros_like(scale), torch.zeros_like(shift), None
+    dy = grad_y.to(torch.float32).contiguous()
+    if dy.data_ptr() % 16:
+      dy = dy.clone()
+    dx = torch.empty_like(x)
+    dscale, dshift = torch.empty_like(scale), torch.empty_like(shift)
+    nbytes = 4 * 2 * _lib.NORM_CLUSTER * b * c   # partial [B, cluster, 2, C]
+    core._launch('ddsp_b200_norm_relu_backward', x, scale, shift, mean, rstd, dy, dx, dscale,
+                 dshift, *core._workspace(nbytes, x.device), b, h * w, c, ctx.groups)
+    return dx, dscale, dshift, None
 
 
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):

@@ -1,8 +1,9 @@
-// C ABI of the network layers' recurrences (gru.cuh): the GRU handle, which owns the
-// packed recurrent weights of one layer on one device, and its pack, forward and
-// backward-through-time launches.
+// C ABI of the network layers' kernels: the GRU handle (gru.cuh), which owns the packed
+// recurrent weights of one layer on one device, and its pack, forward and
+// backward-through-time launches; and the ResNet's fused normalize + ReLU (norm.cuh).
 #include "capi.cuh"
 #include "gru.cuh"
+#include "norm.cuh"
 
 using namespace ddsp;
 
@@ -248,6 +249,97 @@ int ddsp_b200_gru_backward(ddsp_b200_gru* gru, const float* gates, const float* 
     case 3: return gru_backward_bs<3>(gru, gates, states, grad_out, d_pre, d_rec, B, T, st);
     default: return gru_backward_bs<4>(gru, gates, states, grad_out, d_pre, d_rec, B, T, st);
   }
+}
+
+int ddsp_b200_norm_relu_takes(int C, int G) {
+  return C >= 4 && C <= kNormMaxChannels && C % 4 == 0 && G >= 1 && C % G == 0;
+}
+
+}  // extern "C"
+
+namespace {
+
+// The checks both directions share: shape, takes-query and the float4 alignment of the
+// [B, HW, C] operands.  Returns 0, or the status with the error set.
+int norm_relu_check(const char* fn, int B, int HW, int C, int G,
+                    std::initializer_list<const void*> rows) {
+  DDSP_REQUIRE(B >= 0 && HW >= 0, DDSP_B200_E_INVALID, "%s: bad shape B=%d HW=%d", fn, B, HW);
+  DDSP_REQUIRE(ddsp_b200_norm_relu_takes(C, G), DDSP_B200_E_UNSUPPORTED,
+               "%s: C=%d channels in G=%d groups; the kernel takes C a multiple of 4 from 4 "
+               "to %d, in groups that divide it", fn, C, G, kNormMaxChannels);
+  for (const void* p : rows)
+    DDSP_REQUIRE(((uintptr_t)p & 15) == 0, DDSP_B200_E_INVALID,
+                 "%s: the [B, HW, C] operands must be 16-byte aligned", fn);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int ddsp_b200_norm_relu_forward(const float* x, const float* scale, const float* shift,
+                                void* y_out, void* mean_out, void* rstd_out, int B, int HW,
+                                int C, int G, float eps, void* stream) {
+  const char* fn = "norm_relu_forward";
+  float* y = static_cast<float*>(y_out);
+  float* mean = static_cast<float*>(mean_out);
+  float* rstd = static_cast<float*>(rstd_out);
+  if (int rc = norm_relu_check(fn, B, HW, C, G, {x, y})) return rc;
+  if (B == 0 || HW == 0) return 0;
+  DDSP_REQUIRE(x && scale && shift && y && mean && rstd, DDSP_B200_E_INVALID,
+               "%s: null pointer", fn);
+  const size_t n = extent(B, HW, C);
+  if (int rc = check_overlap(fn, {DDSP_OUT(y, n), DDSP_OUT(mean, extent(B, G)),
+                                  DDSP_OUT(rstd, extent(B, G))},
+                             {DDSP_IN(x, n), DDSP_IN(scale, C), DDSP_IN(shift, C)}))
+    return rc;
+  DDSP_REQUIRE(!overlaps(y, n * sizeof(float), mean, extent(B, G) * sizeof(float)) &&
+                   !overlaps(y, n * sizeof(float), rstd, extent(B, G) * sizeof(float)) &&
+                   !overlaps(mean, extent(B, G) * sizeof(float), rstd,
+                             extent(B, G) * sizeof(float)),
+               DDSP_B200_E_INVALID, "%s: y, mean and rstd must not overlap", fn);
+  return launch("norm_relu_forward", norm_relu_forward_kernel, dim3(kNormCluster * B),
+                dim3(kNormThreads), norm_smem_bytes(C, G, false), (cudaStream_t)stream, x,
+                scale, shift, y, mean, rstd, HW, C, G, eps);
+}
+
+int ddsp_b200_norm_relu_backward(const float* x, const float* scale, const float* shift,
+                                 const float* mean, const float* rstd, const float* dy,
+                                 float* dx, float* dscale, float* dshift, void* workspace,
+                                 size_t workspace_bytes, int B, int HW, int C, int G,
+                                 void* stream) {
+  const char* fn = "norm_relu_backward";
+  if (int rc = norm_relu_check(fn, B, HW, C, G, {x, dy, dx})) return rc;
+  if (B == 0 || HW == 0) return 0;
+  DDSP_REQUIRE(x && scale && shift && mean && rstd && dy && dx && dscale && dshift &&
+                   workspace, DDSP_B200_E_INVALID, "%s: null pointer", fn);
+  const size_t n = extent(B, HW, C), np = extent(B, kNormCluster, 2 * C);
+  DDSP_REQUIRE(workspace_bytes >= np * sizeof(float), DDSP_B200_E_INVALID,
+               "%s: the workspace has %zu B, it needs %zu", fn, workspace_bytes,
+               np * sizeof(float));
+  float* partial = static_cast<float*>(workspace);
+  if (int rc = check_overlap(fn, {DDSP_OUT(dx, n), DDSP_OUT(dscale, C), DDSP_OUT(dshift, C),
+                                  DDSP_OUT(partial, np)},
+                             {DDSP_IN(x, n), DDSP_IN(scale, C), DDSP_IN(shift, C),
+                              DDSP_IN(mean, extent(B, G)), DDSP_IN(rstd, extent(B, G)),
+                              DDSP_IN(dy, n)}))
+    return rc;
+  DDSP_REQUIRE(!overlaps(dx, n * sizeof(float), dscale, C * sizeof(float)) &&
+                   !overlaps(dx, n * sizeof(float), dshift, C * sizeof(float)) &&
+                   !overlaps(dscale, C * sizeof(float), dshift, C * sizeof(float)) &&
+                   !overlaps(partial, np * sizeof(float), dx, n * sizeof(float)) &&
+                   !overlaps(partial, np * sizeof(float), dscale, C * sizeof(float)) &&
+                   !overlaps(partial, np * sizeof(float), dshift, C * sizeof(float)),
+               DDSP_B200_E_INVALID, "%s: dx, dscale, dshift and the workspace must not "
+               "overlap", fn);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (int rc = launch("norm_relu_backward", norm_relu_backward_kernel, dim3(kNormCluster * B),
+                      dim3(kNormThreads), norm_smem_bytes(C, G, true), st, x, scale, shift,
+                      mean, rstd, dy, dx, partial, HW, C, G))
+    return rc;
+  return launch("norm_relu_param_grad", norm_relu_param_grad_kernel,
+                dim3((2 * C + 255) / 256), dim3(256), 0, st, (const float*)partial, dscale,
+                dshift, kNormCluster * B, C);
 }
 
 }  // extern "C"

@@ -3,7 +3,14 @@
 z_midiae.gin: MFCCs of the audio, instance-normalized, through a GRU and a Dense layer
 to a latent z, resampled to the frame rate of the other conditioning.  The MFCCs
 (`csrc/mel.cuh`), the GRU's recurrence (`csrc/gru.cuh`) and the resample run on the
-library's CUDA kernels; the normalization and the Dense layer are torch ops."""
+library's CUDA kernels; the normalization and the Dense layer are torch ops.
+
+encoders.ResnetSinusoidalEncoder and encoders.SinusoidalToHarmonicEncoder
+(encoders.py:129-251) are the two networks of models.InverseSynthesis: audio -> log-mel
+-> ResNet -> sinusoid controls, and sinusoids -> harmonic controls.  The log-mel
+(`csrc/mel.cuh`), the ResNet's normalize-ReLU sites (`csrc/norm.cuh`) and the GRU of
+nn.RnnSandwich run on the library's CUDA kernels; convolutions, Dense layers and the
+output scalings are torch ops."""
 import inspect
 
 import torch
@@ -87,3 +94,78 @@ class MfccTimeDistributedRnnEncoder(ZEncoder):
     z = self.z_norm(mfccs[:, :, None, :])[:, :, 0, :]
     z = self.rnn(z)
     return self.dense_out(z)
+
+
+def _audio(features, name):
+  if isinstance(features, dict):
+    if 'audio' not in features:
+      raise KeyError(f'{name}: the features lack [\'audio\']')
+    return features['audio']
+  return features
+
+
+class ResnetSinusoidalEncoder(torch.nn.Module):
+  """Audio [B, n_samples] (or a features dict's 'audio') straight to synthesizer
+  controls: spectral_fn (log-mel) -> nn.ResNet(size) -> the frequency and channel axes
+  flattened -> one Dense per (key, width) of output_splits.  Returns {key: [B, T, width]}.
+
+  The defaults are the reference's, including size='tiny', which nn.ResNet does not
+  have (KeyError at construction, as in the reference): pretrain_model.gin sets 'small'
+  and a log-mel of 229 bins (fft_size 2048, overlap 0.75), for which 64000 samples give
+  a ResNet output [B, 125, 8, 1024] and Dense inputs of 8192."""
+
+  def __init__(self, output_splits=(('frequencies', 100 * 64), ('amplitudes', 100),
+                                    ('noise_magnitudes', 60)),
+               spectral_fn=spectral_ops.compute_logmel, size='tiny'):
+    super().__init__()
+    self.output_splits = tuple((k, int(v)) for k, v in output_splits)
+    self.output_keys = [k for k, _ in self.output_splits]
+    self.spectral_fn = spectral_fn
+    self.resnet = nn.ResNet(size=size)
+    self.dense_outs = torch.nn.ModuleList([nn.Dense(v) for _, v in self.output_splits])
+
+  def forward(self, features, training=True):
+    mag = self.spectral_fn(_audio(features, 'ResnetSinusoidalEncoder'))
+    x = self.resnet(mag[:, :, :, None])
+    x = x.reshape(int(x.shape[0]), int(x.shape[1]), -1)
+    return {key: layer(x) for layer, key in zip(self.dense_outs, self.output_keys)}
+
+
+def _f0_softmax(x):
+  return core.frequencies_softmax(x, depth=64, hz_min=20.0, hz_max=1200.0)
+
+
+class SinusoidalToHarmonicEncoder(torch.nn.Module):
+  """Harmonic controls from sinusoidal ones: sin_freqs (Hz) mapped by hz_to_unit over
+  [0, Nyquist] and concatenated with sin_amps, through `net` (e.g. nn.RnnSandwich; a
+  dict output's 'out' is taken), then three Dense heads: harm_amp [.., 1] and harm_dist
+  [.., n_harmonics] through amp_scale_fn (exp_sigmoid), f0_hz [.., 1] through
+  freq_scale_fn (frequencies_softmax, depth 64, 20-1200 Hz).  Harmonics at or above
+  Nyquist are zeroed and the distribution renormalized with safe_divide.  Returns
+  {'harm_amp', 'harm_dist', 'f0_hz'}."""
+
+  def __init__(self, net=None, n_harmonics=100, f0_depth=64, amp_scale_fn=core.exp_sigmoid,
+               freq_scale_fn=_f0_softmax, sample_rate=16000):
+    super().__init__()
+    self.n_harmonics = int(n_harmonics)
+    self.amp_scale_fn = amp_scale_fn
+    self.freq_scale_fn = freq_scale_fn
+    self.sample_rate = sample_rate
+    self.net = net
+    self.amp_out = nn.Dense(1)
+    self.hd_out = nn.Dense(n_harmonics)
+    self.f0_out = nn.Dense(f0_depth)
+
+  def forward(self, sin_freqs, sin_amps):
+    nyquist = self.sample_rate / 2.0
+    sin_freqs_unit = core.hz_to_unit(sin_freqs, hz_min=0.0, hz_max=nyquist)
+    x = torch.cat([sin_freqs_unit, sin_amps], dim=-1)
+    x = self.net(x)
+    x = x['out'] if isinstance(x, dict) else x
+    harm_amp = self.amp_scale_fn(self.amp_out(x))
+    harm_dist = self.amp_scale_fn(self.hd_out(x))
+    f0_hz = self.freq_scale_fn(self.f0_out(x))
+    harm_freqs = core.get_harmonic_frequencies(f0_hz, self.n_harmonics)
+    harm_dist = core.remove_above_nyquist(harm_freqs, harm_dist, self.sample_rate)
+    harm_dist = core.safe_divide(harm_dist, torch.sum(harm_dist, dim=-1, keepdim=True))
+    return {'harm_amp': harm_amp, 'harm_dist': harm_dist, 'f0_hz': f0_hz}

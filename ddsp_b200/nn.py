@@ -1,5 +1,7 @@
 """The layers of `ddsp/training/nn.py` that decoders.RnnFcDecoder builds from (Fc,
-FcStack, Rnn, split_to_dict), and its masking functions (nn.py:359-557): note
+FcStack, Rnn, split_to_dict), the ResNet and RnnSandwich of the inverse-synthesis
+encoders (Conv2D, MaxPool2D, NormReluConv, ResidualLayer, ResidualStack, ResNet), and
+its masking functions (nn.py:359-557): note
 segmentation, per-note moments and pooling over notes, as the MIDI autoencoder uses them
 (`models/midi_autoencoder.py`: `add_slowness_loss` and `ZMidiAutoencoder.z_note_encode`).
 Same names, arguments and defaults as the reference.
@@ -11,7 +13,10 @@ LayerNormalization `gamma` ones and `beta` zeros, GRU `kernel` [in, 3H] glorot-u
 checkpoint's arrays assign one to one.  As Keras builds a layer at its first call, the
 input width is fixed then and the parameters are created on the input's device.
 Dense and LayerNormalization are torch ops (cuBLAS); the GRU's recurrence runs on the
-CUDA kernels of `csrc/gru.cuh` (DESIGN.md section 3.32).
+CUDA kernels of `csrc/gru.cuh` (DESIGN.md section 3.32).  The ResNet's convolutions are
+torch ops (cuDNN) on channels-last views, with TensorFlow's 'same' padding; every one of
+its Normalize -> ReLU pairs runs on the fused kernel of `csrc/norm.cuh` (normalize_relu,
+DESIGN.md section 3.34).
 
 get_note_mask, get_note_mask_from_onset, get_note_moments and pool_over_notes run on the
 CUDA kernels of `csrc/notes.cuh` (DESIGN.md section 3.25), which never build the
@@ -314,6 +319,255 @@ class Normalize(_Lazy):
     return inv_ensure_4d(x * self.scale + self.shift, n_dims)
 
 
+_N_GROUPS = {'layer': lambda channels: 1, 'group': lambda channels: 32,
+             'instance': lambda channels: channels}
+
+
+def normalize_relu(x, scale, shift, norm_type='layer'):
+  """relu(normalize_op(x, norm_type) * scale + shift) for x [B, H, W, C] (a CUDA tensor)
+  and scale, shift of C elements ([1, 1, 1, C] as Normalize holds them), on the fused
+  kernel of csrc/norm.cuh: one launch forward, two backward, with gradients to x, scale
+  and shift.  Only each (item, group)'s mean and rstd are saved besides x.
+
+  The numerics are normalize_op's (eps 1e-5, population variance); the gradient at a
+  ReLU input of exactly 0 is 0.  An unknown norm_type raises KeyError and a channel
+  count that the groups do not divide ValueError, as normalize_op does; channel counts
+  the kernel does not take (ddsp_b200_norm_relu_takes: C a multiple of 4 up to 2048)
+  raise NotImplementedError.  A CPU tensor raises ValueError: there is no CPU path."""
+  if not torch.is_tensor(x) or x.dim() != 4:
+    raise ValueError('normalize_relu: expected x [batch, height, width, channels], got '
+                     f'{tuple(x.shape) if torch.is_tensor(x) else type(x).__name__}')
+  if not x.is_cuda:
+    raise ValueError(f'normalize_relu: x is on {x.device}; the kernel runs on CUDA '
+                     'devices only')
+  b, h, w, c = (int(v) for v in x.shape)
+  groups = _N_GROUPS[norm_type](c)
+  if c % groups:
+    raise ValueError(f'normalize_relu: norm_type={norm_type!r} splits the channels into '
+                     f'{groups} groups; {c} channels do not divide evenly')
+  if not _lib.load().ddsp_b200_norm_relu_takes(c, groups):
+    raise NotImplementedError(f'normalize_relu: {c} channels in {groups} groups; the '
+                              'kernel takes multiples of 4 from 4 to 2048')
+  if scale.numel() != c or shift.numel() != c:
+    raise ValueError(f'normalize_relu: scale and shift need {c} elements, got '
+                     f'{scale.numel()} and {shift.numel()}')
+  if scale.device != x.device or shift.device != x.device:
+    raise ValueError(f'normalize_relu: x is on {x.device}, scale on {scale.device} and '
+                     f'shift on {shift.device}')
+  x = x.to(torch.float32).contiguous()
+  if x.data_ptr() % 16:   # the kernel reads rows of four channels
+    x = x.clone()
+  return autograd.NormReluFn.apply(x, scale.to(torch.float32).reshape(c).contiguous(),
+                                   shift.to(torch.float32).reshape(c).contiguous(), groups)
+
+
+class NormRelu(Normalize):
+  """A Normalize layer (`scale` and `shift`, [1, 1, 1, C]) whose output goes through a
+  ReLU, both on the fused normalize_relu: the Normalize -> ReLU pair of every ResNet
+  site, with the parameters the reference's Normalize holds there."""
+
+  def __init__(self, norm_type='layer'):
+    super().__init__(norm_type)
+    self._name = 'NormRelu'
+
+  def forward(self, x):
+    if not torch.is_tensor(x) or x.dim() not in (2, 3, 4):
+      raise ValueError('NormRelu: expected x of rank 2, 3 or 4, got '
+                       f'{tuple(x.shape) if torch.is_tensor(x) else type(x).__name__}')
+    n_dims = x.dim()
+    x = ensure_4d(x)
+    self._built(x)
+    return inv_ensure_4d(normalize_relu(x, self.scale, self.shift, self.norm_type), n_dims)
+
+
+# ------------------ Convolutions -------------------------------------------------
+def same_padding(size, kernel, stride):
+  """TensorFlow's 'same' padding of one axis of `size` for a window of `kernel` at
+  `stride`: (before, after).  The output has ceil(size / stride) elements; the padding
+  is max((out - 1) stride + kernel - size, 0), with the odd element after."""
+  out = -(-int(size) // int(stride))
+  total = max((out - 1) * int(stride) + int(kernel) - int(size), 0)
+  return total // 2, total - total // 2
+
+
+def _pair(v):
+  return (int(v), int(v)) if isinstance(v, int) else tuple(int(u) for u in v)
+
+
+def _check_nhwc(x, name):
+  if not torch.is_tensor(x) or x.dim() != 4:
+    raise ValueError(f'{name}: expected x [batch, height, width, channels], got '
+                     f'{tuple(x.shape) if torch.is_tensor(x) else type(x).__name__}')
+
+
+class Conv2D(_Lazy):
+  """tf.keras.layers.Conv2D(filters, kernel_size, strides, padding='same') on NHWC x:
+  `kernel` [kh, kw, in, filters] glorot-uniform (fans kh kw in and kh kw filters) and
+  `bias` [filters] zeros.  Runs as torch's conv2d (cuDNN) on x's channels-last NCHW view
+  with the kernel viewed as OIHW, so neither is copied to another layout; the output is
+  contiguous NHWC.  The symmetric part of the 'same' padding goes to the convolution and
+  the odd element after (stride 2) is padded explicitly."""
+
+  def __init__(self, filters, kernel_size, strides=(1, 1), padding='same'):
+    super().__init__('Conv2D')
+    if padding != 'same':
+      raise NotImplementedError(f"Conv2D: padding={padding!r}; only 'same' is supported")
+    self.filters = int(filters)
+    self.kernel_size = _pair(kernel_size)
+    self.strides = _pair(strides)
+
+  def build(self, width, device):
+    kh, kw = self.kernel_size
+    limit = math.sqrt(6.0 / (kh * kw * width + kh * kw * self.filters))
+    self.kernel = torch.nn.Parameter(torch.nn.init.uniform_(
+        torch.zeros((kh, kw, width, self.filters), device=device), -limit, limit))
+    self.bias = torch.nn.Parameter(torch.zeros(self.filters, device=device))
+
+  def forward(self, x):
+    _check_nhwc(x, 'Conv2D')
+    self._built(x)
+    (kh, kw), (sh, sw) = self.kernel_size, self.strides
+    top, bottom = same_padding(x.shape[1], kh, sh)
+    left, right = same_padding(x.shape[2], kw, sw)
+    ph, pw = min(top, bottom), min(left, right)
+    if (top, bottom, left, right) != (ph, ph, pw, pw):
+      x = torch.nn.functional.pad(x, (0, 0, left - pw, right - pw, top - ph, bottom - ph))
+    y = torch.nn.functional.conv2d(x.permute(0, 3, 1, 2), self.kernel.permute(3, 2, 0, 1),
+                                   self.bias, self.strides, (ph, pw))
+    return y.permute(0, 2, 3, 1).contiguous()
+
+
+class MaxPool2D(torch.nn.Module):
+  """tf.keras.layers.MaxPool2D(pool_size, strides, padding='same') on NHWC x: the
+  'same' padding is -inf, so padded positions never win."""
+
+  def __init__(self, pool_size=(2, 2), strides=None, padding='same'):
+    super().__init__()
+    if padding != 'same':
+      raise NotImplementedError(f"MaxPool2D: padding={padding!r}; only 'same' is "
+                                'supported')
+    self.pool_size = _pair(pool_size)
+    self.strides = _pair(strides if strides is not None else pool_size)
+
+  def forward(self, x):
+    _check_nhwc(x, 'MaxPool2D')
+    (kh, kw), (sh, sw) = self.pool_size, self.strides
+    top, bottom = same_padding(x.shape[1], kh, sh)
+    left, right = same_padding(x.shape[2], kw, sw)
+    if top or bottom or left or right:
+      x = torch.nn.functional.pad(x, (0, 0, left, right, top, bottom), value=-math.inf)
+    y = torch.nn.functional.max_pool2d(x.permute(0, 3, 1, 2), self.pool_size, self.strides)
+    return y.permute(0, 2, 3, 1).contiguous()
+
+
+# ------------------ ResNet ------------------------------------------------------
+def _unconditional(name, conditional):
+  if conditional:
+    raise NotImplementedError(f'{name}: conditional=True needs ConditionalNorm, which '
+                              'this library does not have')
+
+
+class NormReluConv(torch.nn.Module):
+  """nn.NormReluConv (nn.py:699-709): Normalize -> ReLU (fused, `norm`) -> Conv2D(ch,
+  (k, k), (1, s)) (`conv`)."""
+
+  def __init__(self, ch, k, s, norm_type):
+    super().__init__()
+    self.norm = NormRelu(norm_type)
+    self.conv = Conv2D(ch, (k, k), (1, s))
+
+  def forward(self, x):
+    return self.conv(self.norm(x))
+
+
+class ResidualLayer(torch.nn.Module):
+  """nn.ResidualLayer (nn.py:712-756): a bottleneck layer with 4 ch output channels,
+  downsampling the frequency axis by `stride`.  norm_input -> ReLU (fused), then
+  `bottleneck` (Conv2D(ch, 1x1), NormReluConv(ch, 3, stride), NormReluConv(4 ch, 1, 1))
+  plus the shortcut: `conv_proj` (Conv2D(4 ch, 1x1, (1, stride))) of the normalized
+  input when `shortcut`, else the input itself.  conditional=True raises
+  NotImplementedError."""
+
+  def __init__(self, ch, stride, shortcut, norm_type, conditional=False, shift_only=False):
+    super().__init__()
+    _unconditional('ResidualLayer', conditional)
+    self.shortcut = bool(shortcut)
+    self.conditional = False
+    self.norm_input = NormRelu(norm_type)
+    if self.shortcut:
+      self.conv_proj = Conv2D(4 * ch, (1, 1), (1, stride))
+    self.bottleneck = torch.nn.Sequential(
+        Conv2D(ch, (1, 1), (1, 1)),
+        NormReluConv(ch, 3, stride, norm_type),
+        NormReluConv(4 * ch, 1, 1, norm_type))
+
+  def forward(self, x):
+    r = x
+    x = self.norm_input(ensure_4d(x))
+    r = self.conv_proj(x) if self.shortcut else r
+    return self.bottleneck(x) + r
+
+
+class ResidualStack(torch.nn.Module):
+  """nn.ResidualStack (nn.py:759-802): for each (ch, n_layers, stride), a
+  ResidualLayer with the shortcut and the stride, then n_layers - 1 without; then
+  Normalize -> ReLU (fused, the last of `layers`).  nonlinearity 'relu' only (another
+  raises NotImplementedError, as does conditional=True)."""
+
+  def __init__(self, filters, block_sizes, strides, norm_type, conditional=False,
+               shift_only=False, nonlinearity='relu'):
+    super().__init__()
+    _unconditional('ResidualStack', conditional)
+    if nonlinearity != 'relu':
+      raise NotImplementedError(f'ResidualStack: nonlinearity {nonlinearity!r}; only '
+                                "'relu' is supported")
+    self.conditional = False
+    layers = []
+    for ch, n_layers, stride in zip(filters, block_sizes, strides):
+      layers.append(ResidualLayer(ch, stride, True, norm_type))
+      for _ in range(1, n_layers):
+        layers.append(ResidualLayer(ch, 1, False, norm_type))
+    layers.append(NormRelu(norm_type))
+    self.layers = torch.nn.ModuleList(layers)
+
+  def forward(self, x):
+    for layer in self.layers:
+      x = layer(x)
+    return x
+
+
+class ResNet(torch.nn.Module):
+  """nn.ResNet (nn.py:805-839) on x [B, T, F, channels]: Conv2D(64, 7x7, (1, 2)),
+  MaxPool2D((1, 3), (1, 2)), ResidualStack([ch, 2 ch, 4 ch], blocks, [1, 2, 2]) and
+  ResidualStack([8 ch], [3], [2]), with (ch, blocks) = (32, [2, 3, 4]) 'small',
+  (32, [3, 4, 6]) 'medium' and (64, [3, 4, 6]) 'large' (another size raises KeyError,
+  as the reference's lookup does).  The frequency axis shrinks by 16 and the output has
+  32 ch channels: log-mel [B, 125, 229, 1] -> [B, 125, 8, 1024] at 'small'.
+  conditional=True raises NotImplementedError."""
+
+  def __init__(self, size='large', norm_type='layer', conditional=False, shift_only=False):
+    super().__init__()
+    _unconditional('ResNet', conditional)
+    self.conditional = False
+    size_dict = {
+        'small': (32, [2, 3, 4]),
+        'medium': (32, [3, 4, 6]),
+        'large': (64, [3, 4, 6]),
+    }
+    ch, blocks = size_dict[size]
+    self.layers = torch.nn.ModuleList([
+        Conv2D(64, (7, 7), (1, 2)),
+        MaxPool2D((1, 3), (1, 2)),
+        ResidualStack([ch, 2 * ch, 4 * ch], blocks, [1, 2, 2], norm_type),
+        ResidualStack([8 * ch], [3], [2], norm_type),
+    ])
+
+  def forward(self, x):
+    for layer in self.layers:
+      x = layer(x)
+    return x
+
+
 class Fc(torch.nn.Sequential):
   """nn.Fc (nn.py:843-852): Dense(ch) -> LayerNormalization -> leaky ReLU."""
 
@@ -401,3 +655,12 @@ class Rnn(torch.nn.Module):
 
   def forward(self, x):
     return self.rnn(x)
+
+
+class RnnSandwich(torch.nn.Sequential):
+  """nn.RnnSandwich (nn.py:919-934): FcStack(fc_stack_ch, fc_stack_layers) ->
+  Rnn(rnn_ch, rnn_type) -> FcStack(fc_stack_ch, fc_stack_layers)."""
+
+  def __init__(self, fc_stack_ch=256, fc_stack_layers=2, rnn_ch=512, rnn_type='gru'):
+    super().__init__(FcStack(fc_stack_ch, fc_stack_layers), Rnn(rnn_ch, rnn_type),
+                     FcStack(fc_stack_ch, fc_stack_layers))

@@ -1174,6 +1174,35 @@ int ddsp_b200_gru_backward(ddsp_b200_gru* gru, const float* gates, const float* 
                            const float* grad_out, float* d_pre, float* d_rec, int B, int T,
                            void* stream);
 
+/* nn.Normalize followed by a ReLU, as every site of nn.ResNet runs them (nn.py:699-839),
+ * on x [B, HW, C] channels-last (NHWC with H and W flattened) with the C channels in G
+ * groups (G = 1 'layer', 32 'group', C 'instance'; normalize_op, nn.py:561-575):
+ *   y = max(0, (x - mean) rstd scale[c] + shift[c]),  rstd = 1 / sqrt(var + eps),
+ * mean and population variance of each (item, group) over HW and its C / G channels.
+ * C must be a multiple of 4 from 4 to 2048 and G must divide it
+ * (ddsp_b200_norm_relu_takes(C, G); anything else is E_UNSUPPORTED).  x, y, dy and dx
+ * are 16-byte aligned (E_INVALID otherwise).
+ * _forward (one launch) writes y [B, HW, C] and the per-(item, group) mean and rstd
+ *   [B, G], float32 buffers that autograd.NormReluFn allocates, which are all the
+ *   backward needs besides x.
+ * _backward (two launches): dy -> dx [B, HW, C] and dscale, dshift [C] summed over
+ *   B and HW.  The ReLU mask is recomputed from x with the forward's arithmetic; its
+ *   gradient at an input of exactly 0 is 0.  The workspace holds
+ *   DDSP_B200_NORM_CLUSTER B 2 C floats (each CTA's per-channel partial sums).
+ * No output overlaps an input or another output.  B = 0 or HW = 0 launches nothing
+ * and writes nothing.  FP32 with every sum in a fixed order and no atomics:
+ * bit-reproducible, and item b's y and dx depend on item b alone. */
+#define DDSP_B200_NORM_CLUSTER 8   /* CTAs per item */
+int ddsp_b200_norm_relu_takes(int C, int G);
+int ddsp_b200_norm_relu_forward(const float* x, const float* scale, const float* shift,
+                                void* y, void* mean, void* rstd, int B, int HW, int C, int G,
+                                float eps, void* stream);
+int ddsp_b200_norm_relu_backward(const float* x, const float* scale, const float* shift,
+                                 const float* mean, const float* rstd, const float* dy,
+                                 float* dx, float* dscale, float* dshift, void* workspace,
+                                 size_t workspace_bytes, int B, int HW, int C, int G,
+                                 void* stream);
+
 #ifdef __cplusplus
 }
 #endif
