@@ -20,12 +20,13 @@ from ddsp_b200 import preprocessing
 from ddsp_b200 import processors
 from ddsp_b200 import synthetic_data
 from ddsp_b200 import synths
-from ddsp_b200.decoders import RnnFcDecoder
+from ddsp_b200.decoders import DilatedConvDecoder, MidiToHarmonicDecoder, RnnFcDecoder
 from ddsp_b200.effects import (ExpDecayReverb, FIRFilter, FilteredNoiseReverb,
                                ModDelay, Reverb)
-from ddsp_b200.encoders import ResnetSinusoidalEncoder, SinusoidalToHarmonicEncoder
+from ddsp_b200.encoders import (ExpressionEncoder, HarmonicToMidiEncoder, OneHotEncoder,
+                                ResnetSinusoidalEncoder, SinusoidalToHarmonicEncoder)
 from ddsp_b200.host import HostDecoder
-from ddsp_b200.models import InverseSynthesis
+from ddsp_b200.models import InverseSynthesis, MidiAutoencoder, ZMidiAutoencoder
 from ddsp_b200.processors import Add, Crop, Mix, Processor, ProcessorGroup
 from ddsp_b200.synths import (FilteredNoise, Harmonic, Sinusoidal, TensorToAudio,
                               Wavetable)

@@ -61,6 +61,9 @@ kernels, exposed as `torch.autograd.Function`s:
   * `NormReluFn` - nn.Normalize followed by a ReLU at every site of `nn.ResNet`: one
     fused launch forward (`csrc/norm.cuh`), and one backward launch plus a fixed-order
     reduction of dscale and dshift; only the per-(item, group) mean and rstd are saved;
+  * `NormResidualFn` - the residual site of `nn.DilatedConvStack`, x + normalize(y) s + h
+    and its ReLU, with s and h per channel or read in place from a FiLM Dense output
+    (`csrc/norm.cuh`): one launch forward, one or two backward;
   * `CrepeLossFramesFn` - the framing and per-frame normalisation of
     `losses.PretrainedCREPE`, d audio, which the embedding losses train through;
   * `DecoderFn` / `decoder_train` - the whole `ae.gin` decoder from RAW network
@@ -1097,6 +1100,77 @@ class NormReluFn(torch.autograd.Function):
     core._launch('ddsp_b200_norm_relu_backward', x, scale, shift, mean, rstd, dy, dx, dscale,
                  dshift, *core._workspace(nbytes, x.device), b, h * w, c, ctx.groups)
     return dx, dscale, dshift, None
+
+
+class NormResidualFn(torch.autograd.Function):
+  """The residual site of nn.DilatedConvStack (csrc/norm.cuh): x_next = x +
+  normalize(y) s + h and r = relu(x_next) over y, x [B, T, C] (contiguous, 16-byte
+  aligned float32 CUDA tensors), with the channels in `groups` groups (0: no
+  normalization).  s and h are scale and shift [C] (film None), or read in place from
+  film [B, T, ld], the FiLM Dense output: scale in columns [0, C) and shift in [C, 2C),
+  or the shift alone in [0, C) with shift_only.  Returns (x_next, r), or x_next alone
+  without want_r.  One `ddsp_b200_norm_residual_forward` launch; x_next, y and the
+  per-(item, group) mean and rstd are all the backward keeps.  The backward is one
+  `ddsp_b200_norm_residual_backward` call: gradients to y, x and scale and shift (two
+  launches) or film (one launch, written in film's layout)."""
+
+  @staticmethod
+  def forward(ctx, y, x, scale, shift, film, groups, shift_only, want_r):
+    b, t, c = y.shape
+    x_next = torch.empty_like(y)
+    r = torch.empty_like(y) if want_r else None
+    mean = torch.empty((b, groups), dtype=torch.float32, device=y.device) if groups else None
+    rstd = torch.empty_like(mean) if groups else None
+    ld, s, h = _norm_residual_affine(film, scale, shift, c, shift_only)
+    if y.numel():
+      core._launch('ddsp_b200_norm_residual_forward', y, x, s, h, ld, x_next, r, mean, rstd,
+                   b, t, c, groups, 1e-5)
+    ctx.save_for_backward(y, x_next, scale, film, mean, rstd)
+    ctx.cfg = (groups, bool(shift_only))
+    ctx.set_materialize_grads(False)
+    return (x_next, r) if want_r else x_next
+
+  @staticmethod
+  def backward(ctx, gx, gr=None):
+    y, x_next, scale, film, mean, rstd = ctx.saved_tensors
+    groups, shift_only = ctx.cfg
+    b, t, c = y.shape
+    per_row = film is not None
+    if gx is None and gr is None or not y.numel():
+      zero = torch.zeros_like(y)
+      return (zero, zero, None if per_row else torch.zeros_like(scale),
+              None if per_row else torch.zeros_like(scale),
+              torch.zeros_like(film) if per_row else None, None, None, None)
+
+    def rows(g):
+      g = g.to(torch.float32).contiguous()
+      return g.clone() if g.data_ptr() % 16 else g
+
+    gx = rows(gx) if gx is not None else torch.zeros_like(y)
+    gr = rows(gr) if gr is not None else None
+    dy, dx = torch.empty_like(y), torch.empty_like(y)
+    if per_row:
+      dfilm = torch.empty_like(film)   # film is [B, T, 2C], or [B, T, C] with shift_only
+      ld, s, _ = _norm_residual_affine(film, None, None, c, shift_only)
+      ds, dh = (None, dfilm) if shift_only else (dfilm.data_ptr(), dfilm.data_ptr() + 4 * c)
+      core._launch('ddsp_b200_norm_residual_backward', y, s, ld, x_next, mean, rstd, gx, gr,
+                   dy, dx, ds, dh, None, 0, b, t, c, groups)
+      return dy, dx, None, None, dfilm, None, None, None
+    dscale, dshift = torch.empty_like(scale), torch.empty_like(scale)
+    nbytes = 4 * 2 * _lib.NORM_CLUSTER * b * c   # partial [B, cluster, 2, C]
+    core._launch('ddsp_b200_norm_residual_backward', y, scale, 0, x_next, mean, rstd, gx, gr,
+                 dy, dx, dscale, dshift, *core._workspace(nbytes, y.device), b, t, c, groups)
+    return dy, dx, dscale, dshift, None, None, None, None
+
+
+def _norm_residual_affine(film, scale, shift, c, shift_only):
+  """(ld, scale, shift) arguments of the residual site's entry points: the per-channel
+  tensors with ld 0, or film's row stride and the addresses of its scale and shift
+  columns (scale None with shift_only)."""
+  if film is None:
+    return 0, scale, shift
+  p, ld = film.data_ptr(), int(film.shape[-1])
+  return (ld, None, film) if shift_only else (ld, p, p + 4 * c)
 
 
 def exp_sigmoid(x, exponent=10.0, max_value=2.0, threshold=1e-7):

@@ -1,6 +1,7 @@
 // C ABI of the network layers' kernels: the GRU handle (gru.cuh), which owns the packed
 // recurrent weights of one layer on one device, and its pack, forward and
-// backward-through-time launches; and the ResNet's fused normalize + ReLU (norm.cuh).
+// backward-through-time launches; the ResNet's fused normalize + ReLU and the dilated
+// convolution stack's residual site (norm.cuh).
 #include "capi.cuh"
 #include "gru.cuh"
 #include "norm.cuh"
@@ -337,6 +338,164 @@ int ddsp_b200_norm_relu_backward(const float* x, const float* scale, const float
                       dim3(kNormThreads), norm_smem_bytes(C, G, true), st, x, scale, shift,
                       mean, rstd, dy, dx, partial, HW, C, G))
     return rc;
+  return launch("norm_relu_param_grad", norm_relu_param_grad_kernel,
+                dim3((2 * C + 255) / 256), dim3(256), 0, st, (const float*)partial, dscale,
+                dshift, kNormCluster * B, C);
+}
+
+int ddsp_b200_norm_residual_takes(int C, int G) {
+  return C >= 4 && C <= kNormMaxChannels && C % 4 == 0 && G >= 0 && (G == 0 || C % G == 0);
+}
+
+}  // extern "C"
+
+namespace {
+
+// Elements from the first to the last of B T rows of C at stride ld (ld = 0: C alone).
+size_t row_extent(int B, int T, int C, int ld) {
+  const size_t rows = extent(B, T);
+  return ld == 0 ? (size_t)C : rows ? (rows - 1) * (size_t)ld + C : 0;
+}
+
+// Whether no two of the float ranges (first element, extent) share a byte.
+bool pairwise_disjoint(std::initializer_list<std::pair<const void*, size_t>> ranges) {
+  for (auto a = ranges.begin(); a != ranges.end(); ++a)
+    for (auto b = a + 1; b != ranges.end(); ++b)
+      if (overlaps(a->first, a->second * sizeof(float), b->first, b->second * sizeof(float)))
+        return false;
+  return true;
+}
+
+// The checks both directions of the residual site share: shape, takes-query, the row
+// stride and the float4 alignment of every row operand.  Returns 0, or the status with
+// the error set.
+int norm_residual_check(const char* fn, int B, int T, int C, int G, int ld,
+                        std::initializer_list<const void*> rows) {
+  DDSP_REQUIRE(B >= 0 && T >= 0, DDSP_B200_E_INVALID, "%s: bad shape B=%d T=%d", fn, B, T);
+  DDSP_REQUIRE(ddsp_b200_norm_residual_takes(C, G), DDSP_B200_E_UNSUPPORTED,
+               "%s: C=%d channels in G=%d groups; the kernel takes C a multiple of 4 from 4 "
+               "to %d, in groups that divide it, or G = 0 (no normalization)", fn, C, G,
+               kNormMaxChannels);
+  DDSP_REQUIRE(ld == 0 || (ld >= C && ld % 4 == 0), DDSP_B200_E_INVALID,
+               "%s: row stride ld=%d; it is 0 (per-channel scale and shift) or a multiple of "
+               "4 of at least C=%d", fn, ld, C);
+  for (const void* p : rows)
+    DDSP_REQUIRE(((uintptr_t)p & 15) == 0, DDSP_B200_E_INVALID,
+                 "%s: the row operands must be 16-byte aligned", fn);
+  return 0;
+}
+
+template <bool kNorm, bool kRow>
+int launch_norm_residual_forward(const float* y, const float* x, const float* scale,
+                                 const float* shift, int ld, float* x_next, float* r,
+                                 float* mean, float* rstd, int B, int T, int C, int G,
+                                 float eps, cudaStream_t st) {
+  return launch("norm_residual_forward", norm_residual_forward_kernel<kNorm, kRow>,
+                dim3(kNormCluster * B), dim3(kNormThreads),
+                kNorm ? norm_smem_bytes(C, G, false) : 0, st, y, x, scale, shift, ld, x_next,
+                r, mean, rstd, T, C, G, eps);
+}
+
+template <bool kNorm, bool kRow>
+int launch_norm_residual_backward(const float* y, const float* scale, int ld,
+                                  const float* x_next, const float* mean, const float* rstd,
+                                  const float* gx, const float* gr, float* dy, float* dx,
+                                  float* dscale, float* dshift, float* partial, int B, int T,
+                                  int C, int G, cudaStream_t st) {
+  const bool smem = kNorm || !kRow;
+  return launch("norm_residual_backward", norm_residual_backward_kernel<kNorm, kRow>,
+                dim3(kNormCluster * B), dim3(kNormThreads),
+                smem ? norm_smem_bytes(C, kNorm ? G : 0, true) : 0, st, y, scale, ld, x_next,
+                mean, rstd, gx, gr, dy, dx, dscale, dshift, partial, T, C, G);
+}
+
+}  // namespace
+
+extern "C" {
+
+int ddsp_b200_norm_residual_forward(const float* y, const float* x, const float* scale,
+                                    const float* shift, int ld, void* x_next_out, void* r_out,
+                                    void* mean_out, void* rstd_out, int B, int T, int C, int G,
+                                    float eps, void* stream) {
+  const char* fn = "norm_residual_forward";
+  float* x_next = static_cast<float*>(x_next_out);
+  float* r = static_cast<float*>(r_out);
+  float* mean = static_cast<float*>(mean_out);
+  float* rstd = static_cast<float*>(rstd_out);
+  const bool row = ld > 0;
+  if (int rc = norm_residual_check(fn, B, T, C, G, ld,
+                                   {y, x, x_next, r, row ? scale : nullptr,
+                                    row ? shift : nullptr}))
+    return rc;
+  if (B == 0 || T == 0) return 0;
+  DDSP_REQUIRE(y && x && shift && x_next && (scale || row) && (G == 0 || (mean && rstd)),
+               DDSP_B200_E_INVALID, "%s: null pointer", fn);
+  const size_t n = extent(B, T, C), ns = row_extent(B, T, C, ld), nm = G ? extent(B, G) : 0;
+  if (int rc = check_overlap(fn, {DDSP_OUT(x_next, n), DDSP_OUT(r, r ? n : 0),
+                                  DDSP_OUT(mean, nm), DDSP_OUT(rstd, nm)},
+                             {DDSP_IN(y, n), DDSP_IN(x, n), DDSP_IN(scale, scale ? ns : 0),
+                              DDSP_IN(shift, ns)}))
+    return rc;
+  DDSP_REQUIRE(pairwise_disjoint({{x_next, n}, {r, r ? n : 0}, {mean, nm}, {rstd, nm}}),
+               DDSP_B200_E_INVALID, "%s: x_next, r, mean and rstd must not overlap", fn);
+  cudaStream_t st = (cudaStream_t)stream;
+#define DDSP_NR_FWD(N, ROW) \
+  launch_norm_residual_forward<N, ROW>(y, x, scale, shift, ld, x_next, r, mean, rstd, B, T, C, \
+                                     G, eps, st)
+  if (G > 0) return row ? DDSP_NR_FWD(true, true) : DDSP_NR_FWD(true, false);
+  return row ? DDSP_NR_FWD(false, true) : DDSP_NR_FWD(false, false);
+#undef DDSP_NR_FWD
+}
+
+int ddsp_b200_norm_residual_backward(const float* y, const float* scale, int ld,
+                                     const float* x_next, const float* mean, const float* rstd,
+                                     const float* gx, const float* gr, float* dy, float* dx,
+                                     float* dscale, float* dshift, void* workspace,
+                                     size_t workspace_bytes, int B, int T, int C, int G,
+                                     void* stream) {
+  const char* fn = "norm_residual_backward";
+  const bool row = ld > 0;
+  if (int rc = norm_residual_check(fn, B, T, C, G, ld,
+                                   {y, x_next, gx, gr, dy, dx, row ? scale : nullptr,
+                                    row ? dscale : nullptr, row ? dshift : nullptr}))
+    return rc;
+  if (B == 0 || T == 0) return 0;
+  DDSP_REQUIRE(y && gx && dy && dx && dshift && (!gr || x_next) && (G == 0 || (mean && rstd)) &&
+                   (row ? !scale == !dscale : scale && dscale && workspace),
+               DDSP_B200_E_INVALID, "%s: null pointer", fn);
+  if (row && dscale) {
+    const ptrdiff_t gap = dshift > dscale ? dshift - dscale : dscale - dshift;
+    DDSP_REQUIRE(gap >= C && gap <= ld - C, DDSP_B200_E_INVALID,
+                 "%s: dscale and dshift must be disjoint column blocks of one row", fn);
+  }
+  const size_t n = extent(B, T, C), ns = row_extent(B, T, C, ld), nm = G ? extent(B, G) : 0;
+  const size_t np = row ? 0 : extent(B, kNormCluster, 2 * C);
+  DDSP_REQUIRE(workspace_bytes >= np * sizeof(float), DDSP_B200_E_INVALID,
+               "%s: the workspace has %zu B, it needs %zu", fn, workspace_bytes,
+               np * sizeof(float));
+  float* partial = row ? nullptr : static_cast<float*>(workspace);
+  if (int rc = check_overlap(fn, {DDSP_OUT(dy, n), DDSP_OUT(dx, n),
+                                  DDSP_OUT(dscale, dscale ? ns : 0), DDSP_OUT(dshift, ns),
+                                  DDSP_OUT(partial, np)},
+                             {DDSP_IN(y, n), DDSP_IN(scale, scale ? ns : 0),
+                              DDSP_IN(x_next, gr ? n : 0), DDSP_IN(mean, nm),
+                              DDSP_IN(rstd, nm), DDSP_IN(gx, n), DDSP_IN(gr, gr ? n : 0)}))
+    return rc;
+  // Per row, dscale and dshift are column blocks of one buffer, checked above.
+  const bool disjoint =
+      row ? pairwise_disjoint({{dy, n}, {dx, n}, {dscale, dscale ? ns : 0}}) &&
+                pairwise_disjoint({{dy, n}, {dx, n}, {dshift, ns}})
+          : pairwise_disjoint({{dy, n}, {dx, n}, {dscale, ns}, {dshift, ns}, {partial, np}});
+  DDSP_REQUIRE(disjoint, DDSP_B200_E_INVALID,
+               "%s: dy, dx, dscale, dshift and the workspace must not overlap", fn);
+  cudaStream_t st = (cudaStream_t)stream;
+#define DDSP_NR_BWD(N, ROW)                                                                   \
+  launch_norm_residual_backward<N, ROW>(y, scale, ld, x_next, mean, rstd, gx, gr, dy, dx,     \
+                                      dscale, dshift, partial, B, T, C, G, st)
+  const int rc = G > 0 ? (row ? DDSP_NR_BWD(true, true) : DDSP_NR_BWD(true, false))
+                       : (row ? DDSP_NR_BWD(false, true) : DDSP_NR_BWD(false, false));
+#undef DDSP_NR_BWD
+  if (rc || row) return rc;
   return launch("norm_relu_param_grad", norm_relu_param_grad_kernel,
                 dim3((2 * C + 255) / 256), dim3(256), 0, st, (const float*)partial, dscale,
                 dshift, kNormCluster * B, C);

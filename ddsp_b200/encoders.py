@@ -10,7 +10,11 @@ encoders.ResnetSinusoidalEncoder and encoders.SinusoidalToHarmonicEncoder
 -> ResNet -> sinusoid controls, and sinusoids -> harmonic controls.  The log-mel
 (`csrc/mel.cuh`), the ResNet's normalize-ReLU sites (`csrc/norm.cuh`) and the GRU of
 nn.RnnSandwich run on the library's CUDA kernels; convolutions, Dense layers and the
-output scalings are torch ops."""
+output scalings are torch ops.
+
+encoders.OneHotEncoder, encoders.HarmonicToMidiEncoder and encoders.ExpressionEncoder
+(encoders.py:254-284, 419-517) are the MIDI autoencoders' encoders; the last two run a
+network such as nn.DilatedConvStack, whose residual sites run on `csrc/norm.cuh`."""
 import inspect
 
 import torch
@@ -169,3 +173,77 @@ class SinusoidalToHarmonicEncoder(torch.nn.Module):
     harm_dist = core.remove_above_nyquist(harm_freqs, harm_dist, self.sample_rate)
     harm_dist = core.safe_divide(harm_dist, torch.sum(harm_dist, dim=-1, keepdim=True))
     return {'harm_amp': harm_amp, 'harm_dist': harm_dist, 'f0_hz': f0_hz}
+
+
+class OneHotEncoder(ZEncoder):
+  """An embedding (nn.get_embedding: `embedding`) of an integer id such as an instrument,
+  read from one_hot_key ([B] or [B, 1]): z [B, n_dims] or [B, 1, n_dims].  Unless
+  skip_expand, z is given a time axis and repeated over the frames of 'f0_scaled', as
+  ZEncoder.expand_z does; with skip_expand it is returned as it is, for broadcasting."""
+
+  def __init__(self, one_hot_key='instrument', vocab_size=1024, n_dims=256,
+               skip_expand=True):
+    super().__init__(input_keys=[one_hot_key])
+    self.one_hot_key = one_hot_key
+    self.vocab_size = vocab_size
+    self.n_dims = n_dims
+    self.skip_expand = skip_expand
+    self.embedding = nn.get_embedding(vocab_size=vocab_size, n_dims=n_dims)
+
+  def compute_z(self, one_hot):
+    return self.embedding(one_hot)
+
+  def expand_z(self, z, time_steps):
+    return z if self.skip_expand else super().expand_z(z, time_steps)
+
+
+class HarmonicToMidiEncoder(torch.nn.Module):
+  """Harmonic synthesizer controls to a MIDI-like encoding: f0_midi, amps, hd and noise
+  ([B, T, .] each) concatenated, through `net`, Normalize('layer') (`norm`) and
+  Dense(2) (`dense_out`).  Returns {'z_pitch', 'z_vel'} ([B, T, 1] each), with f0_midi
+  added to z_pitch when f0_residual."""
+
+  def __init__(self, net=None, f0_residual=True):
+    super().__init__()
+    self.net = net
+    self.f0_residual = f0_residual
+    self.dense_out = nn.Dense(2)
+    self.norm = nn.Normalize('layer')
+
+  def forward(self, f0_midi, amps, hd, noise):
+    x = torch.cat([f0_midi, amps, hd, noise], dim=-1)
+    x = self.dense_out(self.norm(self.net(x)))
+    z_pitch = x[..., 0:1]
+    z_vel = x[..., 1:2]
+    if self.f0_residual:
+      z_pitch = z_pitch + f0_midi
+    return {'z_pitch': z_pitch, 'z_vel': z_vel}
+
+
+class ExpressionEncoder(ZEncoder):
+  """A latent from frame-rate features: the input_keys ([B, T, .] each) concatenated,
+  through `net`, Normalize('layer') (`norm`) and Dense(z_dims) (`dense_out`), averaged
+  over time when pool_time, then expanded to the frames of 'f0_scaled'.  The reference's
+  'audio' input (MFCCs) cannot run there (it pops from a tuple), so 'audio' in
+  input_keys raises NotImplementedError."""
+
+  def __init__(self, net=None, z_dims=128, input_keys=('f0_scaled', 'ld_scaled'),
+               mfcc_bins=60, fft_size=1024, mel_bins=128, pool_time=True):
+    if 'audio' in input_keys:
+      raise NotImplementedError("ExpressionEncoder: 'audio' in input_keys (MFCC inputs) "
+                                'is not supported')
+    super().__init__(list(input_keys))
+    self.compute_mfccs = False
+    self.mfcc_bins = mfcc_bins
+    self.fft_size = fft_size
+    self.mel_bins = mel_bins
+    self.pool_time = pool_time
+    self.net = net
+    self.norm = nn.Normalize('layer')
+    self.dense_out = nn.Dense(z_dims)
+
+  def compute_z(self, *inputs):
+    z = self.dense_out(self.norm(self.net(torch.cat(inputs, dim=-1))))
+    if self.pool_time:
+      z = torch.mean(z, dim=1, keepdim=True)
+    return z

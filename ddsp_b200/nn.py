@@ -1,6 +1,7 @@
 """The layers of `ddsp/training/nn.py` that decoders.RnnFcDecoder builds from (Fc,
 FcStack, Rnn, split_to_dict), the ResNet and RnnSandwich of the inverse-synthesis
-encoders (Conv2D, MaxPool2D, NormReluConv, ResidualLayer, ResidualStack, ResNet), and
+encoders (Conv2D, MaxPool2D, NormReluConv, ResidualLayer, ResidualStack, ResNet), the
+MIDI autoencoders' DilatedConvStack with ConditionalNorm, FcStackOut and get_embedding, and
 its masking functions (nn.py:359-557): note
 segmentation, per-note moments and pooling over notes, as the MIDI autoencoder uses them
 (`models/midi_autoencoder.py`: `add_slowness_loss` and `ZMidiAutoencoder.z_note_encode`).
@@ -16,7 +17,8 @@ Dense and LayerNormalization are torch ops (cuBLAS); the GRU's recurrence runs o
 CUDA kernels of `csrc/gru.cuh` (DESIGN.md section 3.32).  The ResNet's convolutions are
 torch ops (cuDNN) on channels-last views, with TensorFlow's 'same' padding; every one of
 its Normalize -> ReLU pairs runs on the fused kernel of `csrc/norm.cuh` (normalize_relu,
-DESIGN.md section 3.34).
+DESIGN.md section 3.34), and every residual site of DilatedConvStack on the same header's
+norm_residual kernel (DESIGN.md section 3.35).
 
 get_note_mask, get_note_mask_from_onset, get_note_moments and pool_over_notes run on the
 CUDA kernels of `csrc/notes.cuh` (DESIGN.md section 3.25), which never build the
@@ -380,6 +382,64 @@ class NormRelu(Normalize):
     return inv_ensure_4d(normalize_relu(x, self.scale, self.shift, self.norm_type), n_dims)
 
 
+def norm_residual(y, x, norm_type=None, scale=None, shift=None, film=None,
+                  shift_only=False, relu=True):
+  """One residual site of DilatedConvStack on the fused kernel of csrc/norm.cuh:
+  x_next = x + normalize_op(y, norm_type) s + h, and r = relu(x_next), the next layer's
+  convolution input.  Returns (x_next, r), or x_next alone with relu=False (the stack's
+  last layer).  y and x are [B, T, C] CUDA tensors.
+
+  s and h are Normalize's scale and shift (C elements each), or, with film, read in place
+  from the FiLM Dense output film [B, T, ld] of ConditionalNorm: scale in columns
+  [0, C) and shift in [C, 2C), or the shift alone in [0, C) with shift_only (s = 1).
+  One launch forward; the backward gives y, x and the parameters or film their
+  gradients (ReLU gradient 0 at exactly 0).  The numerics are normalize_op's (eps 1e-5,
+  population variance); norm_type None normalizes nothing.  An unknown norm_type raises
+  KeyError and channels the groups do not divide ValueError, as normalize_op does;
+  channel counts the kernel does not take (multiples of 4 up to 2048) raise
+  NotImplementedError.  A CPU tensor raises ValueError: there is no CPU path."""
+  for name, t in (('y', y), ('x', x)):
+    if not torch.is_tensor(t) or t.dim() != 3:
+      raise ValueError(f'norm_residual: expected {name} [batch, time, channels], got '
+                       f'{tuple(t.shape) if torch.is_tensor(t) else type(t).__name__}')
+  if y.shape != x.shape:
+    raise ValueError(f'norm_residual: y {tuple(y.shape)} and x {tuple(x.shape)} differ')
+  if not y.is_cuda:
+    raise ValueError(f'norm_residual: y is on {y.device}; the kernel runs on CUDA devices '
+                     'only')
+  b, t, c = (int(v) for v in y.shape)
+  groups = 0 if norm_type is None else _N_GROUPS[norm_type](c)
+  if groups and c % groups:
+    raise ValueError(f'norm_residual: norm_type={norm_type!r} splits the channels into '
+                     f'{groups} groups; {c} channels do not divide evenly')
+  if not _lib.load().ddsp_b200_norm_residual_takes(c, groups):
+    raise NotImplementedError(f'norm_residual: {c} channels in {groups} groups; the '
+                              'kernel takes multiples of 4 from 4 to 2048')
+  params = [film] if film is not None else [scale, shift]
+  if any(p is None for p in params) or (film is not None and (scale, shift) != (None, None)):
+    raise ValueError('norm_residual: give scale and shift, or film alone')
+  if any(p.device != y.device for p in params + [x]):
+    raise ValueError(f'norm_residual: y is on {y.device}, and x or the parameters are not')
+
+  def rows(v):
+    v = v.to(torch.float32).contiguous()
+    return v.clone() if v.data_ptr() % 16 else v   # the kernel reads rows of four channels
+
+  if film is not None:
+    width = c if shift_only else 2 * c
+    if film.dim() != 3 or tuple(film.shape[:2]) != (b, t) or film.shape[-1] != width:
+      raise ValueError(f'norm_residual: film must be [{b}, {t}, {width}], got '
+                       f'{tuple(film.shape)}')
+    return autograd.NormResidualFn.apply(rows(y), rows(x), None, None, rows(film), groups,
+                                         bool(shift_only), bool(relu))
+  if scale.numel() != c or shift.numel() != c:
+    raise ValueError(f'norm_residual: scale and shift need {c} elements, got '
+                     f'{scale.numel()} and {shift.numel()}')
+  return autograd.NormResidualFn.apply(
+      rows(y), rows(x), scale.to(torch.float32).reshape(c).contiguous(),
+      shift.to(torch.float32).reshape(c).contiguous(), None, groups, False, bool(relu))
+
+
 # ------------------ Convolutions -------------------------------------------------
 def same_padding(size, kernel, stride):
   """TensorFlow's 'same' padding of one axis of `size` for a window of `kernel` at
@@ -401,39 +461,57 @@ def _check_nhwc(x, name):
 
 
 class Conv2D(_Lazy):
-  """tf.keras.layers.Conv2D(filters, kernel_size, strides, padding='same') on NHWC x:
-  `kernel` [kh, kw, in, filters] glorot-uniform (fans kh kw in and kh kw filters) and
-  `bias` [filters] zeros.  Runs as torch's conv2d (cuDNN) on x's channels-last NCHW view
-  with the kernel viewed as OIHW, so neither is copied to another layout; the output is
-  contiguous NHWC.  The symmetric part of the 'same' padding goes to the convolution and
-  the odd element after (stride 2) is padded explicitly."""
+  """tf.keras.layers.Conv2D(filters, kernel_size, strides, padding='same', dilation_rate,
+  kernel_initializer) on NHWC x: `kernel` [kh, kw, in, filters], glorot-uniform (fans
+  kh kw in and kh kw filters) or 'orthogonal' (Keras's: the kernel as a
+  [kh kw in, filters] matrix with orthonormal columns or rows, gain 1), and `bias`
+  [filters] zeros.  Runs as torch's conv2d (cuDNN) on x's channels-last NCHW view with
+  the kernel viewed as OIHW, so neither is copied to another layout; the output is
+  contiguous NHWC.  'same' padding is TensorFlow's for the dilated extent (k - 1) d + 1;
+  its symmetric part goes to the convolution and the odd element after (stride 2, or an
+  even dilated extent) is padded explicitly.  Keras refuses strides and dilations both
+  above 1, and so does this layer (ValueError)."""
 
-  def __init__(self, filters, kernel_size, strides=(1, 1), padding='same'):
+  def __init__(self, filters, kernel_size, strides=(1, 1), padding='same',
+               dilation_rate=(1, 1), kernel_initializer='glorot_uniform'):
     super().__init__('Conv2D')
     if padding != 'same':
       raise NotImplementedError(f"Conv2D: padding={padding!r}; only 'same' is supported")
+    if kernel_initializer not in ('glorot_uniform', 'orthogonal'):
+      raise NotImplementedError(f'Conv2D: kernel_initializer={kernel_initializer!r}; only '
+                                "'glorot_uniform' and 'orthogonal' are supported")
     self.filters = int(filters)
     self.kernel_size = _pair(kernel_size)
     self.strides = _pair(strides)
+    self.dilation_rate = _pair(dilation_rate)
+    self.kernel_initializer = kernel_initializer
+    if max(self.strides) > 1 and max(self.dilation_rate) > 1:
+      raise ValueError(f'Conv2D: strides {self.strides} and dilation_rate '
+                       f'{self.dilation_rate} cannot both exceed 1')
 
   def build(self, width, device):
     kh, kw = self.kernel_size
-    limit = math.sqrt(6.0 / (kh * kw * width + kh * kw * self.filters))
-    self.kernel = torch.nn.Parameter(torch.nn.init.uniform_(
-        torch.zeros((kh, kw, width, self.filters), device=device), -limit, limit))
+    kernel = torch.zeros((kh, kw, width, self.filters), device=device)
+    if self.kernel_initializer == 'orthogonal':
+      kernel = torch.nn.init.orthogonal_(kernel.view(kh * kw * width, self.filters)).view(
+          kernel.shape)
+    else:
+      limit = math.sqrt(6.0 / (kh * kw * width + kh * kw * self.filters))
+      torch.nn.init.uniform_(kernel, -limit, limit)
+    self.kernel = torch.nn.Parameter(kernel)
     self.bias = torch.nn.Parameter(torch.zeros(self.filters, device=device))
 
   def forward(self, x):
     _check_nhwc(x, 'Conv2D')
     self._built(x)
-    (kh, kw), (sh, sw) = self.kernel_size, self.strides
-    top, bottom = same_padding(x.shape[1], kh, sh)
-    left, right = same_padding(x.shape[2], kw, sw)
+    (kh, kw), (sh, sw), (dh, dw) = self.kernel_size, self.strides, self.dilation_rate
+    top, bottom = same_padding(x.shape[1], (kh - 1) * dh + 1, sh)
+    left, right = same_padding(x.shape[2], (kw - 1) * dw + 1, sw)
     ph, pw = min(top, bottom), min(left, right)
     if (top, bottom, left, right) != (ph, ph, pw, pw):
       x = torch.nn.functional.pad(x, (0, 0, left - pw, right - pw, top - ph, bottom - ph))
     y = torch.nn.functional.conv2d(x.permute(0, 3, 1, 2), self.kernel.permute(3, 2, 0, 1),
-                                   self.bias, self.strides, (ph, pw))
+                                   self.bias, self.strides, (ph, pw), self.dilation_rate)
     return y.permute(0, 2, 3, 1).contiguous()
 
 
@@ -664,3 +742,189 @@ class RnnSandwich(torch.nn.Sequential):
   def __init__(self, fc_stack_ch=256, fc_stack_layers=2, rnn_ch=512, rnn_type='gru'):
     super().__init__(FcStack(fc_stack_ch, fc_stack_layers), Rnn(rnn_ch, rnn_type),
                      FcStack(fc_stack_ch, fc_stack_layers))
+
+
+# ------------------ Embeddings --------------------------------------------------
+class Embedding(torch.nn.Module):
+  """tf.keras.layers.Embedding(input_dim, output_dim): `embeddings` [input_dim,
+  output_dim], uniform(-0.05, 0.05), created on the ids' device at the first call.  Ids
+  of any shape (float ids are truncated to integers, as Keras casts them) give
+  [*ids.shape, output_dim]; an id outside [0, input_dim) raises IndexError."""
+
+  def __init__(self, input_dim, output_dim):
+    super().__init__()
+    self.input_dim = int(input_dim)
+    self.output_dim = int(output_dim)
+    self.embeddings = None
+
+  def forward(self, ids):
+    if not torch.is_tensor(ids):
+      raise TypeError(f'Embedding: expected a torch tensor, got {type(ids).__name__}')
+    if self.embeddings is None:
+      self.embeddings = torch.nn.Parameter(torch.nn.init.uniform_(
+          torch.zeros((self.input_dim, self.output_dim), device=ids.device), -0.05, 0.05))
+    return torch.nn.functional.embedding(ids.to(torch.int64), self.embeddings)
+
+
+def get_embedding(vocab_size=1024, n_dims=256):
+  """nn.get_embedding (nn.py:1066-1071): a real-valued embedding of integer ids."""
+  return Embedding(vocab_size, n_dims)
+
+
+# ------------------ Conditional normalization -------------------------------------
+class ConditionalScaleAndShift(torch.nn.Module):
+  """nn.ConditionalScaleAndShift (nn.py:1075-1099): x * scale + shift with (scale,
+  shift) = `dense`(z) split at x's channel count C, or x + `dense`(z) with shift_only.
+  The Dense (2 C units, or C) is created at the first call, when C is known.  Torch ops;
+  x and z broadcast as TensorFlow's would."""
+
+  def __init__(self, shift_only=False):
+    super().__init__()
+    self.shift_only = bool(shift_only)
+    self.x_ch = None
+    self.dense = None
+
+  def film(self, x_ch, z):
+    """The Dense output for x of x_ch channels: [..., 2 x_ch], or [..., x_ch] with
+    shift_only.  DilatedConvStack's fused sites read it in place."""
+    if self.dense is None:
+      self.x_ch = int(x_ch)
+      self.dense = Dense(self.x_ch if self.shift_only else 2 * self.x_ch)
+    elif int(x_ch) != self.x_ch:
+      raise ValueError(f'ConditionalScaleAndShift: built for {self.x_ch} channels, called '
+                       f'with {x_ch}')
+    return self.dense(z)
+
+  def forward(self, inputs):
+    x, z = inputs
+    out = self.film(int(x.shape[-1]), z)
+    if self.shift_only:
+      return x + out
+    return x * out[..., :self.x_ch] + out[..., self.x_ch:]
+
+
+class ConditionalNorm(torch.nn.Module):
+  """nn.ConditionalNorm (nn.py:1102-1136): normalize_op(x, norm_type) then
+  ConditionalScaleAndShift(shift_only) with z (`conditional_scale_and_shift`).  x is
+  [B, H, W, C].  Torch ops; inside DilatedConvStack the Dense feeds the fused site
+  instead."""
+
+  def __init__(self, norm_type='instance', shift_only=False):
+    super().__init__()
+    self.norm_type = norm_type
+    self.conditional_scale_and_shift = ConditionalScaleAndShift(shift_only=shift_only)
+
+  def forward(self, inputs):
+    x, z = inputs
+    return self.conditional_scale_and_shift([normalize_op(x, self.norm_type), z])
+
+
+# ------------------ Stacks ------------------------------------------------------
+class DilatedConvStack(torch.nn.Module):
+  """nn.DilatedConvStack (nn.py:1152-1323): `conv_in` (Conv2D(ch, (kernel_size, 1))),
+  then stacks x layers_per_stack residual layers
+    x <- x + norm(conv_i(relu(x)))
+  with conv_i (`layers`) a Conv2D(ch, (kernel_size, 1)) of dilation dilation^j at depth j
+  of its stack (or (-dilation)^(layers_per_stack - 1 - j) for a negative dilation) and
+  norm (`norms`) Normalize(norm_type), or ConditionalNorm(norm_type, shift_only) on the
+  conditioning z when conditional.  Kernels are orthogonal with ortho_init, else
+  glorot-uniform.
+
+  Takes x [B, T, C_in], or [x, z] when conditional, with z [B, T, C_z] or of one frame
+  ([B, C_z] or [B, 1, C_z]), broadcast over time as TensorFlow broadcasts it.  Returns
+  [B, T, ch].  The convolutions run on cuDNN (Conv2D) and every residual site on the fused
+  kernel of csrc/norm.cuh (norm_residual), which also writes the ReLU the next
+  convolution reads; a conditional site reads its ConditionalNorm's Dense output in
+  place.  The first ReLU, of conv_in's output, is a torch op.  CUDA tensors only
+  (ValueError otherwise).  The kernel takes ch a multiple of 4 from 4 to 2048, which
+  the reference does not require: another ch raises NotImplementedError at construction
+  ('group' norm also needs ch a multiple of 32, ValueError).  Resampling (resample_type
+  other than None, or a resample_stride other than 1) and spectral_norm=True raise
+  NotImplementedError."""
+
+  def __init__(self, ch=256, layers_per_stack=5, stacks=2, kernel_size=3, dilation=2,
+               norm_type=None, resample_type=None, resample_stride=1,
+               stacks_per_resample=1, resample_after_convolve=True, spectral_norm=False,
+               ortho_init=False, shift_only=False, conditional=False):
+    super().__init__()
+    if resample_type is not None or resample_stride != 1:
+      raise NotImplementedError(f'DilatedConvStack: resample_type={resample_type!r}, '
+                                f'resample_stride={resample_stride}; resampling inside the '
+                                'stack is not supported')
+    if spectral_norm:
+      raise NotImplementedError('DilatedConvStack: spectral_norm=True '
+                                '(SpectralNormalization) is not supported')
+    groups = 0 if norm_type is None else _N_GROUPS[norm_type](ch)   # KeyError if unknown
+    if groups and ch % groups:
+      raise ValueError(f'DilatedConvStack: norm_type={norm_type!r} splits the channels into '
+                       f'{groups} groups; ch={ch} does not divide evenly')
+    if not _lib.load().ddsp_b200_norm_residual_takes(ch, groups):
+      raise NotImplementedError(f'DilatedConvStack: ch={ch}; the residual-site kernel takes '
+                                'multiples of 4 from 4 to 2048')
+    self.conditional = bool(conditional)
+    self.norm_type = norm_type
+    self.shift_only = bool(shift_only)
+    self.resample_after_convolve = resample_after_convolve
+    init = 'orthogonal' if ortho_init else 'glorot_uniform'
+
+    def conv(dilation_rate=1):
+      return Conv2D(ch, (kernel_size, 1), (1, 1), dilation_rate=(dilation_rate, 1),
+                    kernel_initializer=init)
+
+    def rate(i):
+      if dilation > 0:
+        return int(dilation**i)
+      return int((-dilation)**(layers_per_stack - i - 1))
+
+    self.conv_in = conv()
+    self.layers = torch.nn.ModuleList(
+        [conv(rate(j)) for _ in range(stacks) for j in range(layers_per_stack)])
+    self.norms = torch.nn.ModuleList([
+        ConditionalNorm(norm_type, shift_only) if self.conditional else Normalize(norm_type)
+        for _ in range(stacks * layers_per_stack)])
+
+  def forward(self, inputs):
+    if self.conditional:
+      x, z = inputs
+    else:
+      x, z = inputs, None
+    if not torch.is_tensor(x) or x.dim() != 3:
+      raise ValueError('DilatedConvStack: expected x [batch, time, channels], got '
+                       f'{tuple(x.shape) if torch.is_tensor(x) else type(x).__name__}')
+    x = self.conv_in(ensure_4d(x))[:, :, 0, :]
+    b, t, ch = (int(v) for v in x.shape)
+    r = torch.relu(x)
+    if z is not None:
+      if z.dim() == 2:
+        z = z[:, None, :]
+      if z.dim() != 3 or int(z.shape[0]) != b or int(z.shape[1]) not in (1, t):
+        raise ValueError(f'DilatedConvStack: z {tuple(z.shape)} does not broadcast to '
+                         f'[{b}, {t}, channels]')
+    n = len(self.layers)
+    for i, (layer, norm) in enumerate(zip(self.layers, self.norms)):
+      y = layer(r[:, :, None, :])[:, :, 0, :]
+      relu = i < n - 1
+      if self.conditional:
+        film = norm.conditional_scale_and_shift.film(ch, z)
+        if int(film.shape[1]) != t:
+          film = film.expand(b, t, int(film.shape[-1]))
+        out = norm_residual(y, x, self.norm_type, film=film, shift_only=self.shift_only,
+                            relu=relu)
+      else:
+        norm._built(y)
+        out = norm_residual(y, x, self.norm_type, norm.scale, norm.shift, relu=relu)
+      x, r = out if relu else (out, None)
+    return x
+
+
+class FcStackOut(torch.nn.Module):
+  """nn.FcStackOut (nn.py:1326-1337): FcStack(ch, layers) (`stack`) then Dense(n_out)
+  (`dense_out`)."""
+
+  def __init__(self, ch, layers, n_out):
+    super().__init__()
+    self.stack = FcStack(ch, layers)
+    self.dense_out = Dense(n_out)
+
+  def forward(self, x):
+    return self.dense_out(self.stack(x))

@@ -1203,6 +1203,44 @@ int ddsp_b200_norm_relu_backward(const float* x, const float* scale, const float
                                  size_t workspace_bytes, int B, int HW, int C, int G,
                                  void* stream);
 
+/* The residual site of nn.DilatedConvStack (nn.py:1153-1324) on the same cluster
+ * geometry and statistics pass, over y (the convolution's output) and x (the residual
+ * stream), both [B, T, C]:
+ *   x_next = x + xh s + h,  r = relu(x_next),
+ * with xh = (y - mean) rstd of y's (item, group) statistics as above for G >= 1, or
+ * xh = y for G = 0 (norm_type None).  ddsp_b200_norm_residual_takes(C, G): C a multiple
+ * of 4 from 4 to 2048, and G = 0 or a divisor of C (anything else is E_UNSUPPORTED).
+ * s and h are per channel when ld = 0: scale and shift [C] (nn.Normalize).  When ld > 0
+ * (a multiple of 4, at least C) they are per row: item b's row t reads C values from
+ * scale + (b T + t) ld and from shift + (b T + t) ld, so a FiLM Dense output [B, T, ld]
+ * is read in place (nn.ConditionalNorm: scale = out, shift = out + C).  A null scale with
+ * ld > 0 is s = 1 (shift_only).  Row operands (y, x, x_next, r, dy, dx, gx, gr, and the
+ * per-row scale, shift, dscale and dshift) are 16-byte aligned (E_INVALID otherwise).
+ * _forward (one launch) writes x_next, r unless it is null, and for G >= 1 the
+ *   per-(item, group) mean and rstd [B, G] (null for G = 0).
+ * _backward: g = gx + gr 1[x_next > 0] (gr may be null, and then x_next too; the
+ *   gradient at x_next = 0 is 0) is dx [B, T, C], and dy is the normalization's
+ *   backward of g s, with xh recomputed from y with the forward's arithmetic.  ld = 0:
+ *   two launches, dscale = sum g xh and dshift = sum g [C] over B and T, through a
+ *   workspace of DDSP_B200_NORM_CLUSTER B 2 C floats.  ld > 0: one launch, which writes
+ *   g xh per row to dscale (null when scale is) and g to dshift at the forward's offsets
+ *   and stride (other columns of the rows are not written; dscale and dshift are
+ *   disjoint column blocks); no workspace.
+ * No output overlaps an input or another output.  B = 0 or T = 0 launches nothing and
+ * writes nothing.  FP32 with every sum in a fixed order and no atomics: bit-reproducible,
+ * and item b's outputs depend on item b alone. */
+int ddsp_b200_norm_residual_takes(int C, int G);
+int ddsp_b200_norm_residual_forward(const float* y, const float* x, const float* scale,
+                                    const float* shift, int ld, void* x_next, void* r,
+                                    void* mean, void* rstd, int B, int T, int C, int G,
+                                    float eps, void* stream);
+int ddsp_b200_norm_residual_backward(const float* y, const float* scale, int ld,
+                                     const float* x_next, const float* mean, const float* rstd,
+                                     const float* gx, const float* gr, float* dy, float* dx,
+                                     float* dscale, float* dshift, void* workspace,
+                                     size_t workspace_bytes, int B, int T, int C, int G,
+                                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif
